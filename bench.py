@@ -4,6 +4,7 @@
     python bench.py --gpus 1 --steps 20 --warmup 5            # this repo's CUDA engine
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 2   # CPU reference path (oracle port)
     python bench.py --workload resnet18_iao_w8a8_bnfuse       # another BASELINE.json config as the measured workload
+    python bench.py --steps 20 --dump-outputs out/            # also write what the last timed step computed (.npy)
 
 Workload (BASELINE.json configs[1]): NIN-GC, wbwtab W-ternary / A-binary, batch 256 per GPU,
 3x32x32 inputs, CrossEntropy + Adam(lr 0.01) - the reference's training step
@@ -15,10 +16,16 @@ One JSON line on stdout (rank 0).  `value` is timed with inputs resident in HBM;
 same step fed from pinned HOST buffers (H2D of the batch + D2H of the loss / logits inside the timed
 region); `roofline` is for the dominant engine kernel, timed live with CUDA events on the
 launching stream; `cpu_baseline` is the oracle port of the reference timed on the host cores;
-`extra_workloads` (N = 1 only) are short runs of the other BASELINE.json configs in the same process."""
+`extra_workloads` (N = 1 only) are short runs of the other BASELINE.json configs in the same process.
+
+--dump-outputs DIR writes, right after the timed steps, what the timed path computed in its last step as float32 .npy
+files: the loss (QAT) or the logits (inference) and every parameter of the model after that step (a fixed, seeded sample
+of each tensor when the whole set would exceed 48 MB).  Inputs and initial weights are seeded, so two builds run with the
+same arguments can be compared file by file."""
 import argparse
 import json
 import os
+import re
 import subprocess
 import sys
 import threading
@@ -59,11 +66,11 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], d["bf16_tflops"], "measured"
-    return 6650.0, 1590.0, "fallback"
+    return 3350.0, 989.0, "datasheet (H100 SXM: HBM3, dense BF16)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -137,7 +144,7 @@ def config_dict(workload, n_gpus, cpu_arm=False):
             "global_batch": b * n_gpus, "per_gpu_batch": b,
             "optimizer": "none (inference)" if w.get("inference") else "Adam lr=0.01",
             "parallelism": f"{n_gpus} independent replicas" if w.get("inference") else f"dp{n_gpus}",
-            "l2": "per-step activation working set >> 126 MB L2, 4 rotating input batches (no flush needed)"}
+            "l2": "per-step activation working set >> 50 MB L2, 4 rotating input batches (no flush needed)"}
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -198,7 +205,28 @@ def main_reference(args):
 # ----------------------------------------------------------------------------------------------------------
 # engine arm
 # ----------------------------------------------------------------------------------------------------------
-def run_engine(workload, steps, warmup, dev, rank, world, detail):
+DUMP_BYTES = 48 << 20   # parameters written by --dump-outputs (plus the loss / logits): well inside 64 MB
+
+
+def dump_outputs(out_dir, result, model, inference):
+    """float32 .npy files of the last timed step: its result (loss or logits) and the model parameters after it"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "logits.npy" if inference else "loss.npy"),
+            result.detach().float().cpu().numpy().reshape(result.shape))
+    params = [(n, p.detach()) for n, p in model.named_parameters()]
+    total = sum(p.numel() for _, p in params) * 4
+    frac = min(1.0, DUMP_BYTES / max(1, total))
+    g = torch.Generator().manual_seed(1234)
+    for n, p in params:
+        flat = p.float().flatten().cpu()
+        if frac < 1.0:   # fixed, seeded sample of every tensor (sorted flat indices)
+            k = max(1, int(flat.numel() * frac))
+            flat = flat[torch.randperm(flat.numel(), generator=g)[:k].sort().values]
+        np.save(os.path.join(out_dir, "param." + re.sub(r"[^A-Za-z0-9_.]", "_", n) + ".npy"), flat.numpy())
+
+
+def run_engine(workload, steps, warmup, dev, rank, world, detail, dump_dir=None):
     """time `steps` steps of one workload; returns the measurement dict (rank-local, max over ranks for times)"""
     from micronet_b200 import _lib as L, functional as F_
     w = H.WORKLOADS[workload]
@@ -233,9 +261,13 @@ def run_engine(workload, steps, warmup, dev, rank, world, detail):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return ms.item()
 
+    last = {}
+
     def step_resident(i):
         x, t = devb[i % nbuf]
-        stepper.step(x, t)
+        # detached: a loss that keeps its autograd graph alive would keep that step's AccumulateGrad nodes (and their
+        # stream) alive into the CUDA-graph capture of a later step and break it
+        last["out"] = stepper.step(x, t).detach()
 
     out_host = torch.empty((B, 10) if inference else (), dtype=torch.float32).pin_memory()
 
@@ -256,6 +288,8 @@ def run_engine(workload, steps, warmup, dev, rank, world, detail):
     ms_total = timed(step_resident, steps)
     torch.cuda.synchronize()
     L.tc_check()   # a bounded pipeline wait that gave up would have produced garbage: fail loudly instead
+    if dump_dir:
+        dump_outputs(dump_dir, last["out"], model, inference)
     clocks = sampler.stop() if sampler else None
     for i in range(2):
         step_e2e(i)
@@ -323,7 +357,11 @@ def main():
     ap.add_argument("--kernels-json", default=None, help="dump the per-kernel CUDA-event timings of the timed region")
     ap.add_argument("--workload", default=WORKLOAD, choices=sorted(H.WORKLOADS),
                     help="default: the headline configuration (BASELINE.json configs[1])")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss / logits and the model parameters as float32 .npy files")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return main_reference(args)
     args.warmup = max(args.warmup, 3)
@@ -342,7 +380,8 @@ def main():
     torch.backends.cuda.matmul.allow_tf32 = False
 
     wl = args.workload
-    main_res = run_engine(wl, args.steps, args.warmup, dev, rank, world, detail=True)
+    main_res = run_engine(wl, args.steps, args.warmup, dev, rank, world, detail=True,
+                          dump_dir=args.dump_outputs if rank == 0 else None)
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -368,16 +407,9 @@ def main():
         else:
             roof = {"bound": "tensor", "achieved": flops / avg_s / 1e12, "peak": tfl, "unit": "TFLOP/s"}
         roof["frac"] = roof["achieved"] / roof["peak"]
-        traffic = tsrc = None
-        tpath = os.path.join(ROOT, "profiles", "kernel_traffic.json")
-        if os.path.exists(tpath):  # measured dram__bytes_{read,write}.sum per launch from the committed ncu capture
-            tj = json.load(open(tpath))
-            rec = tj["kernels"].get(f"{dk}:{list(dshape)}")
-            traffic = rec["dram_bytes"] if rec else None
-            tsrc = tj.get("source")
         t_roof_sum = sum(max(conv_algorithmic(sh, k)[1] / (hbm * 1e9), conv_algorithmic(sh, k)[0] / (tfl * 1e12)) * n
                          for (k, sh), (_, n) in agg.items())
-        roof.update({"traffic": traffic, "traffic_source": tsrc, "algorithmic_bytes": nbytes, "algorithmic_flops": flops,
+        roof.update({"algorithmic_bytes": nbytes, "algorithmic_flops": flops,
                      "peak_source": peak_src,
                      "kernel": f"conv2d_{dk} shape(B,C,H,W,K,R,S,sh,sw,ph,pw,dh,dw,G)={list(dshape)}",
                      "avg_launch_us": avg_s * 1e6, "launches_timed": dn, "share_of_step": dtot / dsteps / step_ms,

@@ -1,4 +1,4 @@
-"""Micro-benchmark (GPU box): cycles per tcgen05.mma M128 x N x K16 (bf16, smem operands)."""
+"""Micro-benchmark (GPU): cycles per wgmma M64 x N x K16 (bf16, smem operands) from one warpgroup."""
 import os, sys
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

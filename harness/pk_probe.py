@@ -53,7 +53,7 @@ def main():
     args = ap.parse_args()
     from micronet_b200 import _lib as L, pk as PK
     dev = torch.device("cuda:0")
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}
+    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
     hbm, tfl = peaks["hbm_gbs"], peaks["bf16_tflops"]
     rows = []
     B = args.batch
@@ -110,7 +110,7 @@ def main():
             rec["wgrad_3x3"] = timeit(lambda i=0: L.check(PK.wgrad(sh, dyp[i % nb], 3, xr[i % nb], 3, dw), "w"))
         plan = (C.c_int32 * 16)()
         L.load().mnb_pk_conv_plan(C.byref(sh), 0, 1, 1, plan)
-        rec["plan_fwd"] = dict(zip("Nt ntiles MT CC chunks nstage smem tmem TH TB BW n_mtiles n_items ny".split(), list(plan)[2:]))
+        rec["plan_fwd"] = dict(zip("Nt ntiles MT CC chunks nstage smem acc TH TB BW n_mtiles n_items ny".split(), list(plan)[2:]))
         L.tc_check()
         rows.append(rec)
         print(json.dumps(rec))

@@ -1,9 +1,9 @@
-"""Debug: where do the roles of the tensor-core conv kernel wait?  (run on the GPU box)
+"""Debug: where do the roles of the tensor-core conv kernel wait?  (needs a GPU)
 
     python harness/tc_role_profile.py
 
 Prints, per layer shape of NIN-GC at batch 256 and per kernel (fwd / dgrad), the fraction of the
-kernel's cycles each warp role (TMA producer, MMA issuer, epilogue, converters) spent inside
+kernel's cycles each warp role (TMA producer, the two MMA warpgroups, converters) spent inside
 pipeline waits.  The role that barely waits is the bottleneck."""
 import os
 import sys
@@ -15,7 +15,7 @@ from micronet_b200 import _lib as L, functional as F_  # noqa: E402
 
 SHAPES = [(256, 256, 32, 32, 256, 1, 2), (256, 256, 16, 16, 512, 3, 16), (256, 512, 16, 16, 512, 1, 4),
           (256, 512, 8, 8, 1024, 3, 32), (256, 1024, 8, 8, 1024, 1, 8)]
-NAMES = ["tma", "mma", "epilogue", "converter"]
+NAMES = ("tma", "mma0", "mma1", "conv")
 
 
 def main():
@@ -50,7 +50,7 @@ def main():
             for i, n in enumerate(NAMES):
                 tot = max(p[i, 3].item(), 1.0)
                 line += f" | {n}: wait {100 * p[i, 0] / tot:4.0f}% +{100 * p[i, 1] / tot:4.0f}% +{100 * p[i, 2] / tot:3.0f}%"
-            print(line + f" | cycles/CTA {p[1, 3].item() / 148:.0f}")
+            print(line + f" | cycles/CTA {p[1, 3].item() / 132:.0f}")
 
 
 if __name__ == "__main__":

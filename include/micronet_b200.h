@@ -1,5 +1,5 @@
 /*
- * micronet_b200 — C-ABI of the B200 (sm_100a) fake-quant conv/linear engine.
+ * micronet_b200 — C-ABI of the H100 (sm_90a) fake-quant conv/linear engine.
  *
  * The reference (666DZY666/micronet) has no FFI: its hot path is Python
  * nn.Module code that composes ATen ops.  This header is the boundary a
@@ -187,7 +187,7 @@ int mnb_channel_stats_bwd(const float* x, const float* mean, const float* dmean,
                           int32_t batch, int32_t channels, int32_t hw, float* dx, mnb_stream_t stream);
 
 /* ------------------------------------------------------------------------
- * Fused tensor-core forward (tcgen05 + TMA): fake-quantize the fp32 NCHW input on the fly while
+ * Fused tensor-core forward (wgmma + TMA): fake-quantize the fp32 NCHW input on the fly while
  * it is staged for the MMA, convolve exact integer levels, scale + bias in the epilogue.
  *   qp == NULL : x is used as it is (wbwtab: +-1 or plain fp32 activations, exact 3-term bf16 split)
  *   qp != NULL : DoReFa / IAO quantizer; `codes` (u8, same shape as x) and `pass_bits`
@@ -295,7 +295,7 @@ int mnb_fconv2d_wgrad_tc(const mnb_conv_shape* s, const float* dy, const float* 
                          int32_t* err_flag, mnb_stream_t stream);
 
 /* ------------------------------------------------------------------------
- * Packed-operand ("pk") tensor-core family (mnb_pk.cu): every conv geometry of the QAT models on tcgen05 - weights
+ * Packed-operand ("pk") tensor-core family (mnb_pk.cu): every conv geometry of the QAT models on wgmma - weights
  * streamed per K-chunk, N / W tiling, stride 1 and 2 (space-to-depth), any filter with <= 64 taps.  Same math as
  * F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen convolution_backward.
  *
@@ -382,8 +382,7 @@ int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, c
  * Bit-packed XNOR-popcount forward for wbwtab layers (mnb_xnor.cu): binary activations (WB:11-36, sign with 0 -> +1)
  * times binary / ternary weights (WB:40-75, 98-146) as sum = popc(N) - 2 popc(N & (A ^ S)) on 1-bit planes; the integer
  * sum is exact, y = fmaf(sum, alpha[k], bias[k]) equals mnb_pk_conv's result bit for bit.  Forward only (the gradients
- * of a QAT step multiply real-valued dy).  functional.py picks it per layer from the measured table of
- * profiles/r2_xnor_vs_tc.md (north_star: "picked when ncu shows it beating the tensor-core path").
+ * of a QAT step multiply real-valued dy).  functional.py picks it per layer (functional.xnor_preferred).
  *   a_bits : u32 [B][G][ceil(C/g / 32)][H][W], bit j of word n = [x[b][g*C/g + 32 n + j][h][w] is not < 0]
  *   w_img  : mnb_xnor_wimage_bytes() bytes, built from the i16 levels {-1, 0, +1} [K][C/g][R][S] of mnb_wb_weight_fwd
  * Cover: square filter 1/3/5, equal strides / pads, dilation 1, C/g <= 128 (3x3), <= 64 (5x5), <= 256 (1x1); else
@@ -407,10 +406,10 @@ int mnb_adam_step(float* params, const float* grads, float* exp_avg, float* exp_
 void mnb_set_tc_profile_buffer(void* dev_int64x16);
 
 /* ------------------------------------------------------------------------
- * Hardware self-tests of the sm_100a building blocks (run by tests/test_gpu_tc_selftest.py).
+ * Hardware self-tests of the sm_90a building blocks (run by tests/test_gpu_tc_selftest.py).
  * Bounded waits: a wrong descriptor sets *err_flag (device int) instead of hanging the GPU.
  * ---------------------------------------------------------------------- */
-/* D[128 x N] = A[128 x K] * B[N x K]^T through tcgen05.mma (kind::f16 on bf16, or kind::i8) with
+/* D[128 x N] = A[128 x K] * B[N x K]^T through wgmma (bf16 -> f32, or s8 -> s32), two 64-row halves, with
  * thread-written no-swizzle operands; A/B/D are fp32 row-major device arrays.
  * int8: 0 = bf16 K-major operands, 1 = int8 K-major, 2 = bf16 MN-major (the wgrad kernel's form).    */
 int mnb_selftest_umma(const float* A, const float* B, float* D, int32_t N, int32_t K, int32_t int8,
@@ -420,8 +419,9 @@ int mnb_selftest_umma(const float* A, const float* B, float* D, int32_t N, int32
 int mnb_selftest_tma3d(const float* src, const int64_t* dims3_host, const int32_t* box3_host,
                        const int32_t* coord3_host, float* out, int32_t* err_flag, mnb_stream_t stream);
 
-/* micro-benchmark: `iters` back-to-back M128 x N x K16 bf16 MMAs from one thread over n_acc accumulators;
- * out2[0] = cycles until all have retired, out2[1] = cycles spent issuing.                         */
+/* micro-benchmark: `iters` back-to-back M64 x N x K16 bf16 wgmma (N = 32, 64 or 128) from one warpgroup into one
+ * register accumulator (n_acc >= 1 is accepted and ignored); out2[0] = cycles until all have retired, out2[1] = cycles
+ * spent issuing.                                                                                   */
 int mnb_selftest_mma_rate(int32_t N, int32_t n_acc, int32_t a_shift16, int32_t iters, int32_t mn_major,
                           int64_t* out2, int32_t* err_flag, mnb_stream_t stream);
 

@@ -1,4 +1,4 @@
-"""micronet_b200 — a B200 (sm_100a) engine for the fake-quant conv/linear hot path of
+"""micronet_b200 — an H100 (sm_90a) engine for the fake-quant conv/linear hot path of
 666DZY666/micronet, behind the reference's own module surface:
 
     from micronet_b200 import wbwtab, dorefa, iao     # <-> micronet.compression.quantization.{...}.quantize

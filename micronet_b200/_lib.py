@@ -150,7 +150,7 @@ def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "micronet_b200: the fake-quant engine runs on CUDA (sm_100a) tensors only; "
+                "micronet_b200: the fake-quant engine runs on CUDA (sm_90a) tensors only; "
                 "got a CPU tensor - there is deliberately no CPU fallback")
 
 
@@ -187,9 +187,8 @@ def tc_check(device=None):
 E_UNSUPPORTED = -2
 KEEP_DEBUG = False   # tests only: modules keep the fake-quantized weight of their last call
 USE_TC = os.environ.get("MNB_DISABLE_TC", "0") != "1"
-# packed bf16 operands from the BN+binarizer producer to the next conv's forward.  Measured (r2h): the convs gain 0.1 ms per
-# step (fwd 158 -> 120 us on the 256-channel 1x1) but the producer's extra 2 B / element plane and its scalar form cost 0.7 ms,
-# so it stays opt-in (MNB_PACKED_OPERANDS=1) until the producer is vectorised and stops writing the fp32 plane as well
+# packed bf16 operands from the BN+binarizer producer to the next conv's forward (experimental, opt-in with
+# MNB_PACKED_OPERANDS=1): the producer's extra 2 B / element plane costs more than the conv gains
 USE_PACKED = os.environ.get("MNB_PACKED_OPERANDS", "0") == "1"
 # packed-operand tensor-core family (mnb_pk.cu): "auto" = wherever the fused kernels have no cover and for every fused-quantizer
 # layer; "all" = every conv it supports; "off" = never
@@ -207,7 +206,7 @@ PK_TERMS_BWD = int(os.environ.get("MNB_PK_TERMS_BWD", "2"))
 # (mnb_bn_sign_bwd_pack); 3x3 layers take it in any case.  MNB_PK_WBWTAB=0 keeps every wbwtab layer on the fused kernels.
 PK_WBWTAB = os.environ.get("MNB_PK_WBWTAB", "1") == "1"
 
-# bit-packed XNOR-popcount forward for wbwtab inference (mnb_xnor.cu): "auto" = the layers where it was measured to beat the
+# bit-packed XNOR-popcount forward for wbwtab inference (mnb_xnor.cu): "auto" = the layers where it is expected to beat the
 # tensor-core forward (functional.xnor_preferred), "all" = wherever it has cover, "off" = never
 XNOR_MODE = os.environ.get("MNB_XNOR", "auto")
 

@@ -1,8 +1,8 @@
-"""Build the sm_100a shared library in-tree with nvcc (no torch involvement).
+"""Build the sm_90a (H100) shared library in-tree with nvcc (no torch involvement).
 
     python -m micronet_b200.build            # builds micronet_b200/lib/libmicronet_b200.so
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot."""
+The .so and its objects are build products (git-ignored): a checkout builds them with this module."""
 import os
 import subprocess
 import sys
@@ -13,8 +13,9 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmicronet_b200.so")
 SOURCES = ["mnb_quant.cu", "mnb_fused.cu", "mnb_conv_generic.cu", "mnb_conv_tc.cu", "mnb_conv_tc_fwd.cu", "mnb_conv_tc_wgrad.cu", "mnb_conv_fp32_tc.cu", "mnb_conv_packed.cu", "mnb_pk.cu", "mnb_xnor.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+ARCH = "arch=compute_90a,code=sm_90a"   # wgmma / TMA / mbarrier: Hopper only
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", ARCH, "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-cudart", "static", "--expt-relaxed-constexpr",
 ]
 
@@ -40,7 +41,7 @@ def build(force=False, verbose=False):
         cmd = [NVCC, *FLAGS, "-c", path, "-o", obj] + (["-Xptxas", "-v"] if verbose else [])
         subprocess.run(cmd, check=True)
         objs.append(obj)
-    subprocess.run([NVCC, "-shared", "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.run([NVCC, "-shared", "-cudart", "static", "-gencode", ARCH,
                     "-o", LIB_PATH, *objs], check=True)
     return LIB_PATH
 

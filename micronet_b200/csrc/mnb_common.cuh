@@ -1,4 +1,4 @@
-// Shared helpers for the micronet_b200 sm_100a kernels.
+// Shared helpers for the micronet_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <float.h>
@@ -24,7 +24,7 @@ void mnb_count_launches(int n);
   } while (0)
 
 static inline int mnb_ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-constexpr int MNB_NUM_SMS = 148;  // B200: 2 dies x 74 SMs
+constexpr int MNB_NUM_SMS = 132;  // H100 SXM
 
 // ---- exact-rounding primitives (never contracted into FMA, never fast-math) ----
 
@@ -194,9 +194,8 @@ __device__ __forceinline__ float mnb_act_level_certified(const MnbActQ& q, float
 // Branch-free first half of mnb_act_level_certified: the provisional level / pass flag from the reciprocal product, and
 // `exact` = this element sits within `delta` of a decision boundary and must be redone with the IEEE division
 // (mnb_act_level_certified does that).  Callers evaluate a whole vector of elements with this straight-line code and
-// take ONE rarely-taken branch for the flagged ones: with the fallback branch inside every element (first version) a
-// lone epilogue warp could not overlap the elements' dependent chains - 360 cycles per element in pk_conv's fused
-// consumer epilogue, ncu r2q/r2r.
+// take ONE rarely-taken branch for the flagged ones: with the fallback branch inside every element the epilogue cannot
+// overlap the elements' dependent chains.
 __device__ __forceinline__ float mnb_act_level_fast(const MnbActQ& q, float x, bool& pass, bool& exact) {
   if (q.mode == MNB_ACT_DOREFA) {
     const float t = __fmul_rn(x, 0.1f);

@@ -1,5 +1,5 @@
 // fp32 convolution with few input channels (the un-quantized FIRST layer of every QAT model: 3 -> 192/256,
-// 5x5 or 3x3; nin_gc.py:82, nin.py, resnet.py) on tcgen05 tensor cores: forward and weight gradient.
+// 5x5 or 3x3; nin_gc.py:82, nin.py, resnet.py) on Hopper tensor cores (wgmma): forward and weight gradient.
 //
 // C*R*S (75 for 3x5x5) is far too small a reduction for the per-tap implicit GEMM of mnb_conv_tc_fwd.cu
 // (one MMA K-step would carry 3 real channels out of 16), so this layer uses a real im2col operand, built in
@@ -35,8 +35,8 @@ struct Params {
   int NP;             // forward: Cout padded to 16 (MMA N); wgrad: Cout padded to 128 (MMA M halves)
   int TH, PH, PW;     // tile = TH full rows (TH * W = 128); patch = C x PH x PW floats (zero padded)
   int tiles_per_img, n_tiles;
-  int nbuf_a, acc_cols, tmem_cols;
-  int off_b, off_a, off_patch, off_tab, off_sum, sum_bytes, a_term_bytes, a_buf_bytes, b_term_bytes, patch_bytes;
+  int nbuf_a;
+  int off_b, off_a, off_patch, off_tab, off_sum, off_stg, sum_bytes, a_term_bytes, a_buf_bytes, b_term_bytes, patch_bytes;
   const float* x; const float* w; const float* bias; float* y;
   const float* dy; float* partial;
   int* err;
@@ -44,8 +44,7 @@ struct Params {
 };
 
 struct alignas(16) Shared {
-  uint64_t a_full[2], a_empty[2], acc_full[2], acc_empty[2], done;
-  uint32_t tmem_slot;
+  uint64_t a_full[2], a_empty[2];
   uint32_t abort;
 };
 
@@ -72,10 +71,13 @@ __device__ __forceinline__ void store_split8(const float (&v)[8], uint8_t* dst, 
 __device__ __forceinline__ void conv_bar_sync(int nthreads) {  // named barrier 1: converter warps only
   asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void mma_bar_sync() {  // named barrier 2: the MMA warpgroup (warps 4..7)
+  asm volatile("bar.sync 2, 128;" ::: "memory");
+}
 
-// The six (A piece, B piece) products kept, SMALLEST FIRST.  The tensor core truncates the running fp32 accumulator
-// after every MMA (about half an ulp of |D|, always toward zero), so the 2^-16 and 2^-8 products are added while
-// |D| is still tiny and only the hi x hi MMAs run at full magnitude.
+// The six (A piece, B piece) products kept, SMALLEST FIRST: the 2^-16 and 2^-8 products are added while the running
+// fp32 accumulator is still tiny, so whatever rounding the tensor core applies to it acts on the small terms at their
+// own magnitude and only the hi x hi MMAs run at full magnitude.
 __device__ __constant__ int kProdA[6] = {1, 2, 0, 1, 0, 0};
 __device__ __constant__ int kProdB[6] = {1, 0, 2, 0, 1, 0};
 
@@ -111,7 +113,7 @@ __device__ __forceinline__ void patch_commit(const Params& p, float* patch, int 
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-// warps: 0 = MMA issue, 4..7 = epilogue (TMEM lane quarters), the other 11 = im2col converters
+// warps: 4..7 = MMA warpgroup (wgmma + epilogue), the other 11 except warp 0 = im2col converters
 constexpr int FWD_NCONV = NTHREADS - 32 - 128;
 
 __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
@@ -126,16 +128,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
 
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&sh.a_full[i], FWD_NCONV / 32); tc::mbar_init(&sh.a_empty[i], 1);
-      tc::mbar_init(&sh.acc_full[i], 1); tc::mbar_init(&sh.acc_empty[i], 4);
+      tc::mbar_init(&sh.a_full[i], FWD_NCONV / 32); tc::mbar_init(&sh.a_empty[i], 4);
     }
     sh.abort = 0;
     tc::fence_barrier_init();
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&sh.tmem_slot)),
-                 "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   for (int n = tid; n < 256; n += NTHREADS) epi_bias[n] = (p.bias && n < p.K) ? __ldg(p.bias + n) : 0.f;
   // resident B operand: w[n][kk] as K-major core matrices [piece][kk / 8][n][8], zero beyond Cout / KR
@@ -159,15 +155,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
     tab[kk] = off;
   }
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = sh.tmem_slot;
 
-  if (warp == 0) {
-    // ================================================================= MMA issuer (warp-converged, lane 0 issues)
-    const uint32_t lead = lane == 0;
-    const uint32_t idesc = tc::make_idesc(1, 1, 1, 128, (uint32_t)p.NP);
+  if (warp >= 4 && warp < 8) {
+    // ================================================================= MMA warpgroup: wgmma -> + bias -> y (NCHW)
+    // 32 output channels at a time: both 64-row halves of the tile in registers (m64n32), through a 128 x 32 staging tile
+    // so that thread m stores position m of every channel (coalesced NCHW rows)
+    const int m = (warp - 4) * 32 + lane;
+    float* stage = reinterpret_cast<float*>(smem + p.off_stg);
+    const int64_t plane = (int64_t)p.H * p.W;
     const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(aop), 128u * 16u, 128u);
     const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(bop), (uint32_t)p.NP * 16u, 128u);
     const uint32_t a_term16 = (uint32_t)p.a_term_bytes >> 4, b_term16 = (uint32_t)p.b_term_bytes >> 4;
@@ -176,64 +172,52 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
     uint32_t t = 0;
     for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x, ++t) {
       const uint32_t ab = p.nbuf_a == 2 ? (t & 1u) : 0u, aph = p.nbuf_a == 2 ? ((t >> 1) & 1u) : (t & 1u);
-      const uint32_t acc = t & 1u, cph = (t >> 1) & 1u;
-      tc::mbar_wait_soft(&sh.acc_empty[acc], cph ^ 1u, p.err, 501, &sh.abort);
       tc::mbar_wait_soft(&sh.a_full[ab], aph, p.err, 502, &sh.abort);
-      tc::tc_fence_after();
-      const uint32_t d_tmem = tmem + acc * (uint32_t)p.acc_cols;
-      for (int q = (p.dbg & 2) ? 6 : 0; q < 6; ++q) {
-        const uint64_t aq = a_desc0 + (uint64_t)(ab * a_buf16 + (uint32_t)kProdA[q] * a_term16);
-        const uint64_t bq = b_desc0 + (uint64_t)((uint32_t)kProdB[q] * b_term16);
-        for (int ks = 0; ks < p.KP / 16; ++ks)
-          tc::mma_f16_guarded(d_tmem, aq + (uint64_t)((uint32_t)ks * a_step16), bq + (uint64_t)((uint32_t)ks * b_step16), idesc,
-                              (uint32_t)(ks | q) != 0u, lead);
-      }
-      if (lead) { tc::mma_commit(&sh.a_empty[ab]); tc::mma_commit(&sh.acc_full[acc]); }
-      __syncwarp();
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ================================================================= epilogue: TMEM -> + bias -> y (NCHW)
-    const int q = warp - 4, m = q * 32 + lane;
-    const int64_t plane = (int64_t)p.H * p.W;
-    uint32_t t = 0;
-    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x, ++t) {
       const int b = tile / p.tiles_per_img, h0 = (tile - b * p.tiles_per_img) * p.TH;
-      const uint32_t acc = t & 1u, cph = (t >> 1) & 1u;
-      if (!tc::mbar_wait(&sh.acc_full[acc], cph, p.err, 503)) break;
-      tc::tc_fence_after();
       float* dst = p.y + (int64_t)b * p.K * plane + (int64_t)h0 * p.W + m;
-      const uint32_t t_row = tmem + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)p.acc_cols;
-      for (int n0 = 0; n0 < p.NP; n0 += 64) {
-        // two 32-column chunks per TMEM round trip; bias as vector loads from shared memory up front so that the
-        // store loop is a pure FADD + STG stream (a per-element bias load serialises against the stores)
-        uint32_t r0[32], r1[32];
-        const bool two = n0 + 32 < p.NP;
-        tc::tmem_ld_32x32(t_row + (uint32_t)n0, r0);
-        if (two) tc::tmem_ld_32x32(t_row + (uint32_t)n0 + 32u, r1);
-        tc::tmem_ld_wait();
-        if (p.dbg & 4) continue;
-#pragma unroll
-        for (int hc = 0; hc < 2; ++hc) {
-          if (hc == 1 && !two) break;
-          const int nb = n0 + 32 * hc;
-          float bs[32];
-#pragma unroll
-          for (int v = 0; v < 8; ++v) {
-            const float4 c4 = *reinterpret_cast<const float4*>(&epi_bias[nb + 4 * v]);
-            bs[4 * v] = c4.x; bs[4 * v + 1] = c4.y; bs[4 * v + 2] = c4.z; bs[4 * v + 3] = c4.w;
+      for (int n0 = 0; n0 < p.NP; n0 += 32) {
+        float acc0[16], acc1[16];
+        tc::zero_acc(acc0); tc::zero_acc(acc1);
+        tc::wg_fence();
+        tc::fence_acc(acc0); tc::fence_acc(acc1);
+        for (int q = (p.dbg & 2) ? 6 : 0; q < 6; ++q) {
+          const uint64_t aq = a_desc0 + (uint64_t)(ab * a_buf16 + (uint32_t)kProdA[q] * a_term16);
+          const uint64_t bq = b_desc0 + (uint64_t)((uint32_t)kProdB[q] * b_term16 + (uint32_t)n0);
+          for (int ks = 0; ks < p.KP / 16; ++ks) {
+            const uint64_t ad = aq + (uint64_t)((uint32_t)ks * a_step16), bd = bq + (uint64_t)((uint32_t)ks * b_step16);
+            tc::Mma<32>::bf16<0, 0>(acc0, ad, bd, 1);
+            tc::Mma<32>::bf16<0, 0>(acc1, ad + 64u, bd, 1);   // rows 64..127: 64 core-matrix rows further
           }
-          float* op = dst + (int64_t)nb * plane;
-#pragma unroll
-          for (int j = 0; j < 32; ++j, op += plane)
-            if (nb + j < p.K) *op = __uint_as_float(hc ? r1[j] : r0[j]) + bs[j];
         }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::fence_acc(acc0); tc::fence_acc(acc1);
+        if (n0 + 32 >= p.NP) {   // the tile's last MMAs retired: its operand buffer is free
+          __syncwarp();
+          if (lane == 0) tc::mbar_arrive(&sh.a_empty[ab]);
+        }
+        mma_bar_sync();          // every thread is done reading the previous staging tile
+        tc::frag_to_smem(acc0, stage, tc::kStageLd, 0);
+        tc::frag_to_smem(acc1, stage, tc::kStageLd, 64);
+        mma_bar_sync();
+        if (p.dbg & 4) continue;
+        // bias as vector loads from shared memory up front so that the store loop is a pure FADD + STG stream (a
+        // per-element bias load serialises against the stores)
+        float bs[32];
+#pragma unroll
+        for (int v = 0; v < 8; ++v) {
+          const float4 c4 = *reinterpret_cast<const float4*>(&epi_bias[n0 + 4 * v]);
+          bs[4 * v] = c4.x; bs[4 * v + 1] = c4.y; bs[4 * v + 2] = c4.z; bs[4 * v + 3] = c4.w;
+        }
+        float* op = dst + (int64_t)n0 * plane;
+#pragma unroll
+        for (int j = 0; j < 32; ++j, op += plane)
+          if (n0 + j < p.K) *op = stage[j * tc::kStageLd + m] + bs[j];
       }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&sh.acc_empty[acc]);
     }
   } else {
     // ================================================================= converters: patch -> im2col A operand
+    if (warp == 0) goto done;
     const int ct = warp < 4 ? tid - 32 : tid - 32 - 128;   // 0 .. FWD_NCONV-1
     float* patch0 = reinterpret_cast<float*>(smem + p.off_patch);
     const int items = 128 * kchunks;
@@ -269,22 +253,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
       if (next < p.n_tiles) patch_commit(p, patch0 + (size_t)((t + 1) & 1u) * patch_floats, next, ct, FWD_NCONV, pre);
     }
   }
-  tc::tc_fence_before();
+done:
   __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols));
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ weight gradient
-// warps: 0 = MMA issue, 4..7 = accumulator drain, the other 11 = converters (dy split + im2col of x).
-// A TMEM accumulator only ever holds FLUSH tiles (48 MMAs per column set and tile): the drain warps add it into an
-// fp32 running sum in shared memory with round-to-nearest adds.  The accumulator truncation (see kProdA) is a bias
-// proportional to chain length x |D|, so short chains matter: measured 8e-6 relative error for one chain over the
-// whole batch, 3e-6 with FLUSH = 4, ~1e-6 with FLUSH = 1.
+// warps: 4..7 = MMA warpgroup, the other 11 except warp 0 = converters (dy split + im2col of x).
+// A register accumulator only ever holds ONE step (12 MMAs per column set): the MMA warpgroup adds it into an fp32
+// running sum in shared memory with round-to-nearest adds.  Short accumulation chains keep the tensor core's
+// accumulator rounding (see kProdA) at the size of one step's terms.
 constexpr int WG_NCONV = NTHREADS - 32 - 128;
-constexpr int FLUSH = 1;
 
 __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -295,20 +273,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
   int* tab = reinterpret_cast<int*>(smem + p.off_tab);
   const int halves = p.NP / 128;
   const int nsub = 128 / SUB;
-  const int my_tiles = (p.n_tiles > (int)blockIdx.x) ? (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
 
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&sh.a_full[i], WG_NCONV / 32); tc::mbar_init(&sh.a_empty[i], 1);
-      tc::mbar_init(&sh.acc_full[i], 1); tc::mbar_init(&sh.acc_empty[i], 4);
+      tc::mbar_init(&sh.a_full[i], WG_NCONV / 32); tc::mbar_init(&sh.a_empty[i], 4);
     }
     sh.abort = 0;
     tc::fence_barrier_init();
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&sh.tmem_slot)),
-                 "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   // operand buffers start as zeros (channel rows >= Cout and im2col rows >= KR are never written), and so does the
   // running sum that follows them
@@ -324,51 +295,71 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
     tab[kk] = off;
   }
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = sh.tmem_slot;
   const int b_buf_bytes = 3 * p.b_term_bytes;
 
-  if (warp == 0) {
-    // ================================================================= MMA issuer
-    const uint32_t lead = lane == 0;
-    const uint32_t idesc = tc::make_idesc(1, 1, 1, 128, (uint32_t)p.KP);
+  if (warp >= 4 && warp < 8) {
+    // ================================================================= MMA warpgroup: wgmma -> fp32 running sum -> partial dw
+    // per step and 128-channel half: 32 im2col columns at a time, both 64-row halves in registers (m64n32), added into
+    // the running sum straight from the fragment (every (channel, column) element belongs to exactly one thread)
+    const int m = (warp - 4) * 32 + lane, wq = warp - 4;
+    float* sum = reinterpret_cast<float*>(smem + p.off_sum);   // [half][kk][128 channels]
     const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(aop), (uint32_t)p.NP * 16u, 128u);
     const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(bop), (uint32_t)p.KP * 16u, 128u);
     const uint32_t a_term16 = (uint32_t)p.a_term_bytes >> 4, b_term16 = (uint32_t)p.b_term_bytes >> 4;
     const uint32_t a_buf16 = (uint32_t)p.a_buf_bytes >> 4, b_buf16 = (uint32_t)b_buf_bytes >> 4;
     const uint32_t a_step16 = 2u * (uint32_t)p.NP, b_step16 = 2u * (uint32_t)p.KP;
-    uint32_t it = 0, t = 0;
-    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t grp = t / FLUSH, in_grp = t % FLUSH;
-      const uint32_t acc = grp & 1u, cph = (grp >> 1) & 1u;
-      if (in_grp == 0) tc::mbar_wait_soft(&sh.acc_empty[acc], cph ^ 1u, p.err, 514, &sh.abort);
-      const uint32_t d_base = tmem + acc * 256u;
+    const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);   // fragment row / column of this thread
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
       for (int sub = 0; sub < nsub; ++sub, ++it) {
         const uint32_t ob = it & 1u, oph = (it >> 1) & 1u;
         tc::mbar_wait_soft(&sh.a_full[ob], oph, p.err, 511, &sh.abort);
-        tc::tc_fence_after();
         for (int hf = (p.dbg & 2) ? halves : 0; hf < halves; ++hf) {
-          for (int q = 0; q < 6; ++q) {
-            const uint64_t aq = a_desc0 + (uint64_t)(ob * a_buf16 + (uint32_t)kProdA[q] * a_term16 + (uint32_t)hf * 128u);
-            const uint64_t bq = b_desc0 + (uint64_t)(ob * b_buf16 + (uint32_t)kProdB[q] * b_term16);
+          for (int k0 = 0; k0 < p.KP; k0 += 32) {
+            float acc0[16], acc1[16];
+            tc::zero_acc(acc0); tc::zero_acc(acc1);
+            tc::wg_fence();
+            tc::fence_acc(acc0); tc::fence_acc(acc1);
+            for (int q = 0; q < 6; ++q) {
+              const uint64_t aq = a_desc0 + (uint64_t)(ob * a_buf16 + (uint32_t)kProdA[q] * a_term16 + (uint32_t)hf * 128u);
+              const uint64_t bq = b_desc0 + (uint64_t)(ob * b_buf16 + (uint32_t)kProdB[q] * b_term16 + (uint32_t)k0);
 #pragma unroll
-            for (int ks = 0; ks < SUB / 16; ++ks)
-              tc::mma_f16_guarded(d_base + (uint32_t)hf * 128u, aq + (uint64_t)((uint32_t)ks * a_step16),
-                                  bq + (uint64_t)((uint32_t)ks * b_step16), idesc,
-                                  (in_grp | (uint32_t)sub | (uint32_t)ks | (uint32_t)q) != 0u, lead);
+              for (int ks = 0; ks < SUB / 16; ++ks) {
+                const uint64_t ad = aq + (uint64_t)((uint32_t)ks * a_step16), bd = bq + (uint64_t)((uint32_t)ks * b_step16);
+                tc::Mma<32>::bf16<0, 0>(acc0, ad, bd, 1);
+                tc::Mma<32>::bf16<0, 0>(acc1, ad + 64u, bd, 1);
+              }
+            }
+            tc::wg_commit();
+            tc::wg_wait<0>();
+            tc::fence_acc(acc0); tc::fence_acc(acc1);
+            if (p.dbg & 4) continue;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const int col = k0 + 8 * j + fc + (e & 1), row = fr + 8 * (e >> 1);
+                if (col < p.KP) {
+                  float* s0 = sum + ((hf * p.KP) + col) * 128 + row;
+                  s0[0] = __fadd_rn(s0[0], acc0[4 * j + e]);
+                  s0[64] = __fadd_rn(s0[64], acc1[4 * j + e]);
+                }
+              }
           }
         }
-        if (lead) tc::mma_commit(&sh.a_empty[ob]);
         __syncwarp();
-      }
-      if (in_grp == FLUSH - 1 || tile + (int)gridDim.x >= p.n_tiles) {
-        if (lead) tc::mma_commit(&sh.acc_full[acc]);
-        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&sh.a_empty[ob]);
       }
     }
-  } else if (warp < 4 || warp >= 8) {
+    mma_bar_sync();   // running sums complete (written by other threads of the warpgroup)
+    float* mine = p.partial + (int64_t)blockIdx.x * p.K * p.KR;
+    for (int hf = 0; hf < halves; ++hf) {
+      const int n = hf * 128 + m;
+      if (n < p.K)
+        for (int kk = 0; kk < p.KR; ++kk) mine[(int64_t)n * p.KR + kk] = sum[((hf * p.KP) + kk) * 128 + m];
+    }
+  } else if (warp != 0) {
     // ================================================================= converters
     const int ct = warp < 4 ? tid - 32 : tid - 32 - 128;
     float* patch0 = reinterpret_cast<float*>(smem + p.off_patch);
@@ -443,43 +434,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
       }
       if (next < p.n_tiles) patch_commit(p, patch0 + (size_t)((t + 1) & 1u) * patch_floats, next, ct, WG_NCONV, pre);
     }
-  } else {
-    // ================================================================= drain: TMEM accumulators -> fp32 running sum -> partial dw
-    const int q = warp - 4, m = q * 32 + lane;
-    float* sum = reinterpret_cast<float*>(smem + p.off_sum);   // [half][kk][128 channels]
-    const int groups = (my_tiles + FLUSH - 1) / FLUSH;
-    for (int grp = 0; grp < groups; ++grp) {
-      const uint32_t acc = grp & 1u, cph = (grp >> 1) & 1u;
-      if (!tc::mbar_wait(&sh.acc_full[acc], cph, p.err, 513)) goto done;
-      tc::tc_fence_after();
-      for (int hf = 0; hf < halves; ++hf) {
-        for (int k0 = 0; k0 < p.KP; k0 += 32) {
-          uint32_t r[32];
-          tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + acc * 256u + (uint32_t)(hf * 128 + k0), r);
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (k0 + j < p.KP && !(p.dbg & 4)) sum[((hf * p.KP) + k0 + j) * 128 + m] += __uint_as_float(r[j]);
-        }
-      }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&sh.acc_empty[acc]);
-    }
-    float* mine = p.partial + (int64_t)blockIdx.x * p.K * p.KR;
-    for (int hf = 0; hf < halves; ++hf) {
-      const int n = hf * 128 + m;
-      if (n < p.K)
-        for (int kk = 0; kk < p.KR; ++kk) mine[(int64_t)n * p.KR + kk] = sum[((hf * p.KP) + kk) * 128 + m];
-    }
   }
 done:
-  tc::tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols));
-  }
 }
 
 __global__ void __launch_bounds__(256) reduce_partials_kernel(const float* __restrict__ partial, int n, int ranks,
@@ -520,12 +477,11 @@ static int plan(const mnb_conv_shape* s, bool wgrad, Params& p, int& smem_bytes)
     p.a_buf_bytes = 3 * p.a_term_bytes;
     p.off_b = 0;
     p.off_a = 3 * p.b_term_bytes;
-    p.acc_cols = p.NP <= 32 ? 32 : p.NP <= 64 ? 64 : p.NP <= 128 ? 128 : 256;
-    p.tmem_cols = 2 * p.acc_cols;
     for (p.nbuf_a = 2; p.nbuf_a >= 1; --p.nbuf_a) {
       p.off_patch = p.off_a + p.nbuf_a * p.a_buf_bytes;
       p.off_tab = p.off_patch + 2 * p.patch_bytes;
-      smem_bytes = p.off_tab + p.KP * 4;
+      p.off_stg = (p.off_tab + p.KP * 4 + 15) / 16 * 16;
+      smem_bytes = p.off_stg + 32 * tc::kStageLd * 4;   // 128 x 32 staging tile of the epilogue
       if (smem_bytes <= kMaxDynSmem) break;
     }
     if (p.nbuf_a < 1) return unsupported("shared memory budget");
@@ -543,8 +499,6 @@ static int plan(const mnb_conv_shape* s, bool wgrad, Params& p, int& smem_bytes)
     p.off_tab = p.off_patch + 2 * p.patch_bytes;
     smem_bytes = p.off_tab + p.KP * 4;
     p.nbuf_a = 2;
-    p.acc_cols = 128;
-    p.tmem_cols = 512;   // two accumulator sets of (2 halves x 128 columns)
     if (smem_bytes > kMaxDynSmem) return unsupported("shared memory budget");
   }
   return 0;

@@ -3,7 +3,7 @@
 // This is the shape-agnostic path of the engine: forward (exact s32 accumulation when both
 // operands are integer levels, fp32 otherwise), dgrad fused with the activation STE mask, and
 // split-K wgrad with a deterministic two-stage reduction.  Hot, regular shapes are taken by the
-// tcgen05 tensor-core kernels in mnb_conv_tc.cu; everything else (C_in = 3 stems, 10-way heads,
+// wgmma tensor-core kernels (mnb_conv_tc_fwd.cu, mnb_conv_tc_wgrad.cu, mnb_pk.cu); everything else (C_in = 3 stems, 10-way heads,
 // odd strides, asymmetric weights) lands here.
 //
 // GEMM views (per group g; Cg = in_c/groups, Ng = out_c/groups, RS = kh*kw):

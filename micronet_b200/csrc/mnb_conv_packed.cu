@@ -36,9 +36,8 @@ __device__ __forceinline__ void store_vec(float* p, const float (&v)[VEC]) {
 
 // ---------------------------------------------------------------------------------------------- producer
 // One warp = 32 * VEC consecutive positions of one OUTPUT channel octet of one image; a lane owns VEC consecutive positions
-// (16-byte loads of x for VEC = 4, VEC consecutive 16-byte pixels of the plane = 64 contiguous bytes per lane).  The first
-// version (one position per lane, 4-byte accesses, always writing the fp32 plane too) ran at 1.95 TB/s of the 10 B per
-// element it moved (r2z launch list: 1.2 ms of the 6.6 ms headline step); y is optional now - a consuming conv of the
+// (16-byte loads of x for VEC = 4, VEC consecutive 16-byte pixels of the plane = 64 contiguous bytes per lane: one position
+// per lane with 4-byte accesses leaves this stream far below HBM bandwidth).  y is optional - a consuming conv of the
 // packed-operand family reads only the plane.
 template <int VEC>
 __global__ void __launch_bounds__(256) bn_sign_packed_fwd_kernel(const float* __restrict__ x, int batch, int channels, int hw,

@@ -1,13 +1,14 @@
-// tcgen05 / TMA tensor-core path of the fake-quant convolution (sm_100a only).
+// wgmma / TMA tensor-core plumbing of the fake-quant convolution (sm_90a only).
 //
-// Part 1 of this file: two hardware self-tests exported through the C-ABI.  They pin the two
-// things that cannot be checked on a CPU-only build box - the UMMA shared-memory / instruction
-// descriptor encodings and the TMA box geometry with out-of-bounds zero fill - on tiny problems
-// with known answers, under bounded waits (a wrong descriptor must fail a test, not hang a GPU).
+// Host-side tensor-map encoding, and two hardware self-tests exported through the C-ABI.  They pin the two
+// things that cannot be checked on a CPU-only build box - the wgmma shared-memory descriptor encodings (K-major
+// and MN-major operands) and the TMA box geometry with out-of-bounds zero fill - on tiny problems with known
+// answers, under bounded waits (a wrong descriptor must fail a test, not hang a GPU).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #include <mutex>
+#include <type_traits>
 
 #include "mnb_common.cuh"
 #include "mnb_tc.cuh"
@@ -85,126 +86,98 @@ int mnb_make_tmap_strided(CUtensorMap* out, const void* base, int elem_bytes, in
   return 0;
 }
 
-// ------------------------------------------------------------------ self-test 1: UMMA descriptors
+// ------------------------------------------------------------------ self-test 1: wgmma descriptors
 // D[128 x N] = A[128 x K] * B[N x K]^T, operands converted by threads into the K-major no-swizzle
-// canonical layout  buf[k_chunk][row][16 bytes]  (SBO = 128 B, LBO = rows * 16 B).
+// canonical layout  buf[k_chunk][row][16 bytes]  (SBO = 128 B, LBO = rows * 16 B).  One warpgroup computes the two
+// 64-row halves with N = 128 instructions (columns >= N are discarded).
 template <bool INT8>
-__global__ void __launch_bounds__(160) selftest_umma_kernel(const float* __restrict__ A, const float* __restrict__ B,
+__global__ void __launch_bounds__(128) selftest_umma_kernel(const float* __restrict__ A, const float* __restrict__ B,
                                                             float* __restrict__ D, int N, int K, int* err) {
   constexpr int EPC = INT8 ? 16 : 8;  // elements per 16-byte chunk
   __shared__ __align__(128) uint8_t a_s[128 * 64 * 2];
   __shared__ __align__(128) uint8_t b_s[128 * 64 * 2];
-  __shared__ __align__(8) uint64_t done_bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int nchunk = K / EPC;
-
-  if (tid < 128) {
-    for (int kc = 0; kc < nchunk; ++kc) {
-      uint8_t* dst = a_s + ((size_t)kc * 128 + tid) * 16;
+  for (int i = tid; i < (int)sizeof(b_s) / 16; i += 128) reinterpret_cast<uint4*>(b_s)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  for (int kc = 0; kc < nchunk; ++kc) {
+    uint8_t* dst = a_s + ((size_t)kc * 128 + tid) * 16;
+    for (int e = 0; e < EPC; ++e) {
+      float v = A[(size_t)tid * K + kc * EPC + e];
+      if (INT8) reinterpret_cast<int8_t*>(dst)[e] = (int8_t)v;
+      else reinterpret_cast<__nv_bfloat16*>(dst)[e] = __float2bfloat16_rn(v);
+    }
+    if (tid < N) {
+      uint8_t* db = b_s + ((size_t)kc * N + tid) * 16;
       for (int e = 0; e < EPC; ++e) {
-        float v = A[(size_t)tid * K + kc * EPC + e];
-        if (INT8) reinterpret_cast<int8_t*>(dst)[e] = (int8_t)v;
-        else reinterpret_cast<__nv_bfloat16*>(dst)[e] = __float2bfloat16_rn(v);
-      }
-      if (tid < N) {
-        uint8_t* db = b_s + ((size_t)kc * N + tid) * 16;
-        for (int e = 0; e < EPC; ++e) {
-          float v = B[(size_t)tid * K + kc * EPC + e];
-          if (INT8) reinterpret_cast<int8_t*>(db)[e] = (int8_t)v;
-          else reinterpret_cast<__nv_bfloat16*>(db)[e] = __float2bfloat16_rn(v);
-        }
+        float v = B[(size_t)tid * K + kc * EPC + e];
+        if (INT8) reinterpret_cast<int8_t*>(db)[e] = (int8_t)v;
+        else reinterpret_cast<__nv_bfloat16*>(db)[e] = __float2bfloat16_rn(v);
       }
     }
-    tc::fence_proxy_async_smem();
   }
-  if (warp == 4) {
-    tc::tmem_alloc<128>(&tmem_slot);
-    if (lane == 0) { tc::mbar_init(&done_bar, 1); tc::fence_barrier_init(); }
-  }
-  tc::tc_fence_before();
+  tc::fence_proxy_async_smem();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-
-  if (warp == 4 && lane == 0) {
-    const uint32_t idesc = INT8 ? tc::make_idesc(2, 1, 1, 128, N) : tc::make_idesc(1, 1, 1, 128, N);
-    const int ksteps = nchunk / 2;
+  const int ksteps = nchunk / 2;   // one MMA K-step = two 16-byte chunks (16 bf16 / 32 int8)
+  for (int h = 0; h < 2; ++h) {
+    typename std::conditional<INT8, int32_t, float>::type acc[64];
+    tc::zero_acc(acc);
+    tc::wg_fence();
+    tc::fence_acc(acc);
     for (int ks = 0; ks < ksteps; ++ks) {
-      uint64_t ad = tc::smem_desc_kmajor_noswz(tc::smem_u32(a_s) + ks * 2 * 128 * 16, 128 * 16, 128);
-      uint64_t bd = tc::smem_desc_kmajor_noswz(tc::smem_u32(b_s) + ks * 2 * N * 16, N * 16, 128);
-      if (INT8) tc::mma_i8(tmem, ad, bd, idesc, ks > 0);
-      else tc::mma_f16(tmem, ad, bd, idesc, ks > 0);
+      const uint64_t ad = tc::smem_desc_kmajor_noswz(tc::smem_u32(a_s) + ks * 2 * 128 * 16 + h * 64 * 16, 128 * 16, 128);
+      const uint64_t bd = tc::smem_desc_kmajor_noswz(tc::smem_u32(b_s) + ks * 2 * N * 16, N * 16, 128);
+      if constexpr (INT8) tc::mma_s8_n128(acc, ad, bd, 1);
+      else tc::Mma<128>::bf16<0, 0>(acc, ad, bd, 1);
     }
-    tc::mma_commit(&done_bar);
-  }
-  if (warp < 4) {
-    bool ok = tc::mbar_wait(&done_bar, 0, err, 101);
-    tc::tc_fence_after();
-    if (ok) {
-      for (int n0 = 0; n0 < N; n0 += 32) {
-        uint32_t r[32];
-        tc::tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + n0, r);
-        tc::tmem_ld_wait();
-        for (int j = 0; j < 32 && n0 + j < N; ++j)
-          D[(size_t)(warp * 32 + lane) * N + n0 + j] = INT8 ? (float)(int)r[j] : __uint_as_float(r[j]);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::fence_acc(acc);
+    const int r = h * 64 + 16 * w + (lane >> 2), c = 2 * (lane & 3);
+    for (int j = 0; j < 16; ++j)
+      for (int e = 0; e < 4; ++e) {
+        const int row = r + 8 * (e >> 1), col = 8 * j + c + (e & 1);
+        if (col < N) D[(size_t)row * N + col] = (float)acc[4 * j + e];
       }
-    }
-    tc::tc_fence_before();
   }
-  __syncthreads();
-  if (warp == 4) tc::tmem_dealloc<128>(tmem);
 }
 
-// MN-major variant (the wgrad kernel's operand form): operands stored as buf[m/8][k][8 elements],
+// MN-major variant (the weight-gradient kernels' operand form): operands stored as buf[m/8][k][8 elements],
 // i.e. D[128 x N] = sum_k At[k][m] * Bt[k][n] with both operands "transposed" in shared memory.
-__global__ void __launch_bounds__(160) selftest_umma_mn_kernel(const float* __restrict__ A, const float* __restrict__ B,
+__global__ void __launch_bounds__(128) selftest_umma_mn_kernel(const float* __restrict__ A, const float* __restrict__ B,
                                                                float* __restrict__ D, int N, int K, int* err) {
   __shared__ __align__(128) uint8_t a_s[128 * 64 * 2];
   __shared__ __align__(128) uint8_t b_s[128 * 64 * 2];
-  __shared__ __align__(8) uint64_t done_bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid < 128) {
-    for (int k = 0; k < K; ++k) {
-      reinterpret_cast<__nv_bfloat16*>(a_s)[((size_t)(tid >> 3) * K + k) * 8 + (tid & 7)] = __float2bfloat16_rn(A[(size_t)tid * K + k]);
-      if (tid < N)
-        reinterpret_cast<__nv_bfloat16*>(b_s)[((size_t)(tid >> 3) * K + k) * 8 + (tid & 7)] = __float2bfloat16_rn(B[(size_t)tid * K + k]);
-    }
-    tc::fence_proxy_async_smem();
-  }
-  if (warp == 4) {
-    tc::tmem_alloc<128>(&tmem_slot);
-    if (lane == 0) { tc::mbar_init(&done_bar, 1); tc::fence_barrier_init(); }
-  }
-  tc::tc_fence_before();
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  for (int i = tid; i < (int)sizeof(b_s) / 16; i += 128) reinterpret_cast<uint4*>(b_s)[i] = make_uint4(0, 0, 0, 0);
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  if (warp == 4 && lane == 0) {
-    const uint32_t idesc = tc::make_idesc_major(1, 1, 1, 128, N, 1, 1);
+  for (int k = 0; k < K; ++k) {
+    reinterpret_cast<__nv_bfloat16*>(a_s)[((size_t)(tid >> 3) * K + k) * 8 + (tid & 7)] = __float2bfloat16_rn(A[(size_t)tid * K + k]);
+    if (tid < N)
+      reinterpret_cast<__nv_bfloat16*>(b_s)[((size_t)(tid >> 3) * K + k) * 8 + (tid & 7)] = __float2bfloat16_rn(B[(size_t)tid * K + k]);
+  }
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+  for (int h = 0; h < 2; ++h) {
+    float acc[64];
+    tc::zero_acc(acc);
+    tc::wg_fence();
+    tc::fence_acc(acc);
     for (int ks = 0; ks < K / 16; ++ks) {
-      uint64_t ad = tc::smem_desc_mnmajor_noswz(tc::smem_u32(a_s) + ks * 256, 128, K * 16);
-      uint64_t bd = tc::smem_desc_mnmajor_noswz(tc::smem_u32(b_s) + ks * 256, 128, K * 16);
-      tc::mma_f16(tmem, ad, bd, idesc, ks > 0);
+      const uint64_t ad = tc::smem_desc_mnmajor_noswz(tc::smem_u32(a_s) + ks * 256 + h * 8 * K * 16, 128, K * 16);
+      const uint64_t bd = tc::smem_desc_mnmajor_noswz(tc::smem_u32(b_s) + ks * 256, 128, K * 16);
+      tc::Mma<128>::bf16<1, 1>(acc, ad, bd, 1);
     }
-    tc::mma_commit(&done_bar);
-  }
-  if (warp < 4) {
-    bool ok = tc::mbar_wait(&done_bar, 0, err, 102);
-    tc::tc_fence_after();
-    if (ok) {
-      for (int n0 = 0; n0 < N; n0 += 32) {
-        uint32_t r[32];
-        tc::tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + n0, r);
-        tc::tmem_ld_wait();
-        for (int j = 0; j < 32 && n0 + j < N; ++j) D[(size_t)(warp * 32 + lane) * N + n0 + j] = __uint_as_float(r[j]);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::fence_acc(acc);
+    const int r = h * 64 + 16 * w + (lane >> 2), c = 2 * (lane & 3);
+    for (int j = 0; j < 16; ++j)
+      for (int e = 0; e < 4; ++e) {
+        const int row = r + 8 * (e >> 1), col = 8 * j + c + (e & 1);
+        if (col < N) D[(size_t)row * N + col] = acc[4 * j + e];
       }
-    }
-    tc::tc_fence_before();
   }
-  __syncthreads();
-  if (warp == 4) tc::tmem_dealloc<128>(tmem);
 }
 
 extern "C" int mnb_selftest_umma(const float* A, const float* B, float* D, int32_t N, int32_t K, int32_t int8,
@@ -214,9 +187,9 @@ extern "C" int mnb_selftest_umma(const float* A, const float* B, float* D, int32
   MNB_REQUIRE(K >= 32 && K <= (int8 == 1 ? 128 : 64) && K % 32 == 0, "self-test K out of range");
   if (int8 == 2) {
     MNB_REQUIRE(K <= 64, "MN-major self-test K <= 64");
-    selftest_umma_mn_kernel<<<1, 160, 0, (cudaStream_t)stream>>>(A, B, D, N, K, err_flag);
-  } else if (int8) selftest_umma_kernel<true><<<1, 160, 0, (cudaStream_t)stream>>>(A, B, D, N, K, err_flag);
-  else selftest_umma_kernel<false><<<1, 160, 0, (cudaStream_t)stream>>>(A, B, D, N, K, err_flag);
+    selftest_umma_mn_kernel<<<1, 128, 0, (cudaStream_t)stream>>>(A, B, D, N, K, err_flag);
+  } else if (int8) selftest_umma_kernel<true><<<1, 128, 0, (cudaStream_t)stream>>>(A, B, D, N, K, err_flag);
+  else selftest_umma_kernel<false><<<1, 128, 0, (cudaStream_t)stream>>>(A, B, D, N, K, err_flag);
   MNB_LAUNCHED(1);
   return 0;
 }
@@ -258,53 +231,45 @@ extern "C" int mnb_selftest_tma3d(const float* src, const int64_t* dims3, const 
 
 
 // ------------------------------------------------------------------ micro-benchmark: MMA issue / execution rate
-// `iters` back-to-back tcgen05.mma (M=128, N, K=16, bf16, K-major no-swizzle operands of zeros) from one
-// thread, cycling over `n_acc` accumulators; A start address shifted by `a_shift16` 16-byte units.
-// out[0] = SM cycles from first issue until the final commit arrives.
-__global__ void __launch_bounds__(64) mma_rate_kernel(int N, int n_acc, int a_shift16, int iters, int mn_major,
-                                                      long long* out, int* err) {
+// `iters` back-to-back wgmma (M=64, N, K=16, bf16, no-swizzle operands of zeros) from one warpgroup into one register
+// accumulator; A start address shifted by `a_shift16` 16-byte units.
+// out[0] = SM cycles from first issue until the last MMA retired, out[1] = cycles spent issuing.
+template <int N>
+__global__ void __launch_bounds__(128) mma_rate_kernel(int a_shift16, int iters, int mn_major, long long* out) {
   __shared__ __align__(1024) uint8_t ab[48 * 1024 - 1024];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int i = tid; i < (int)sizeof(ab) / 16; i += 64) reinterpret_cast<uint4*>(ab)[i] = make_uint4(0, 0, 0, 0);
+  const int tid = threadIdx.x;
+  for (int i = tid; i < (int)sizeof(ab) / 16; i += 128) reinterpret_cast<uint4*>(ab)[i] = make_uint4(0, 0, 0, 0);
   tc::fence_proxy_async_smem();
-  if (warp == 1) {
-    tc::tmem_alloc<512>(&tmem_slot);
-    if (lane == 0) { tc::mbar_init(&bar, 1); tc::fence_barrier_init(); }
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  if (warp == 0) {
-    const uint32_t idesc = mn_major ? tc::make_idesc_major(1, 1, 1, 128, N, 1, 1) : tc::make_idesc(1, 1, 1, 128, N);
-    const uint32_t a_addr = tc::smem_u32(ab) + (uint32_t)a_shift16 * 16u, b_addr = tc::smem_u32(ab) + 24 * 1024;
-    const uint64_t ad = mn_major ? tc::smem_desc_mnmajor_noswz(a_addr, 128, 136 * 16) : tc::smem_desc_kmajor_noswz(a_addr, 136 * 16, 128);
-    const uint64_t bd = mn_major ? tc::smem_desc_mnmajor_noswz(b_addr, 128, 136 * 16) : tc::smem_desc_kmajor_noswz(b_addr, (uint32_t)N * 16, 128);
-    const uint32_t guard = lane == 0;
-    const uint32_t mask = (uint32_t)n_acc - 1;  // n_acc is a power of two
-    const long long t0 = clock64();
-    if (a_shift16 >= 100) {
-      if (lane == 0) for (int i = 0; i < iters; ++i) tc::mma_f16(tmem + (uint32_t)((i & mask) * N), ad + (i & 3), bd, idesc, 1);
-    } else {
-      for (int i = 0; i < iters; ++i) tc::mma_f16_guarded(tmem + (uint32_t)((i & mask) * N), ad + (i & 3), bd, idesc, 1, guard);
-    }
-    const long long t1 = clock64();
-    if (lane == 0) tc::mma_commit(&bar);
-    bool ok = tc::mbar_wait(&bar, 0, err, 501);
-    const long long t2 = clock64();
-    if (lane == 0) { out[0] = ok ? (t2 - t0) : -1; out[1] = t1 - t0; }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc<512>(tmem);
+  const uint32_t a_addr = tc::smem_u32(ab) + (uint32_t)(a_shift16 % 100) * 16u, b_addr = tc::smem_u32(ab) + 24 * 1024;
+  const uint64_t ad = mn_major ? tc::smem_desc_mnmajor_noswz(a_addr, 128, 136 * 16) : tc::smem_desc_kmajor_noswz(a_addr, 136 * 16, 128);
+  const uint64_t bd = mn_major ? tc::smem_desc_mnmajor_noswz(b_addr, 128, 136 * 16) : tc::smem_desc_kmajor_noswz(b_addr, (uint32_t)N * 16, 128);
+  float acc[N / 2];
+  tc::zero_acc(acc);
+  tc::wg_fence();
+  tc::fence_acc(acc);
+  const long long t0 = clock64();
+  if (mn_major) for (int i = 0; i < iters; ++i) tc::Mma<N>::template bf16<1, 1>(acc, ad + (i & 3), bd, 1);
+  else for (int i = 0; i < iters; ++i) tc::Mma<N>::template bf16<0, 0>(acc, ad + (i & 3), bd, 1);
+  const long long t1 = clock64();
+  tc::wg_commit();
+  tc::wg_wait<0>();
+  tc::fence_acc(acc);
+  const long long t2 = clock64();
+  if (tid == 0) { out[0] = acc[0] == 0.f ? (t2 - t0) : -1; out[1] = t1 - t0; }
 }
 
 extern "C" int mnb_selftest_mma_rate(int32_t N, int32_t n_acc, int32_t a_shift16, int32_t iters, int32_t mn_major,
                                      int64_t* out2, int32_t* err_flag, mnb_stream_t stream) {
-  MNB_REQUIRE(out2 && err_flag && N >= 16 && N <= 256 && N % 16 == 0 && n_acc >= 1 && n_acc * N <= 512, "bad mma_rate arguments");
-  mma_rate_kernel<<<1, 64, 0, (cudaStream_t)stream>>>(N, n_acc, a_shift16, iters, mn_major, reinterpret_cast<long long*>(out2), err_flag);
+  MNB_REQUIRE(out2 && err_flag && n_acc >= 1 && iters >= 0, "bad mma_rate arguments");
+  long long* o = reinterpret_cast<long long*>(out2);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (N) {
+    case 32: mma_rate_kernel<32><<<1, 128, 0, st>>>(a_shift16, iters, mn_major, o); break;
+    case 64: mma_rate_kernel<64><<<1, 128, 0, st>>>(a_shift16, iters, mn_major, o); break;
+    case 128: mma_rate_kernel<128><<<1, 128, 0, st>>>(a_shift16, iters, mn_major, o); break;
+    default: return mnb_fail(MNB_E_UNSUPPORTED, "mma_rate: N must be 32, 64 or 128");
+  }
   MNB_LAUNCHED(1);
   return 0;
 }

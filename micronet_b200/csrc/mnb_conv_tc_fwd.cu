@@ -1,4 +1,4 @@
-// Fused fake-quant convolution on tcgen05 tensor cores: forward and data-gradient.
+// Fused fake-quant convolution on Hopper tensor cores (wgmma): forward and data-gradient.
 //
 // Both are "same"-padded stride-1 correlations of an fp32 NCHW tensor with small-integer weights:
 //
@@ -10,18 +10,17 @@
 //
 //   TMA warp    : cp.async.bulk.tensor.4d box (W, TH+2p, CC, TB) of the fp32 input -> staging ring;
 //                 rows above / below the image are zero-filled by the TMA unit
-//   8 converter : staging fp32 -> integer level (DoReFa / IAO fake-quant) or exact 3-way bf16 split
+//   7 converter : staging fp32 -> integer level (DoReFa / IAO fake-quant) or exact 3-way bf16 split
 //     warps       of a raw / pre-scaled fp32 value -> "position-major" bf16 operand
 //                 op[c/8][position][8 ch], position = row*(W+2p) + col of the zero-padded tile.
-//                 This IS the UMMA K-major no-swizzle canonical layout with positions as GEMM rows,
+//                 This IS the wgmma K-major no-swizzle canonical layout with positions as GEMM rows,
 //                 so filter tap (r, s) is the same buffer with the descriptor start address moved by
 //                 (r*BW + s)*16 bytes: implicit GEMM without any im2col copy.  Side outputs of the
 //                 fused quantizer: u8 level codes + STE pass bits for the backward pass.
-//   MMA warp    : one thread issues tcgen05.mma kind::f16 (bf16 x bf16 -> fp32 accumulators in TMEM);
-//                 every operand is an exact small integer or an exact bf16 piece of an fp32 value,
-//                 M = 128 positions, N = output channels of the group, K = 16 channels per MMA
-//   4 epilogue  : tcgen05.ld accumulator rows -> scale + bias (fwd) or STE mask (dgrad) -> coalesced
-//     warps       fp32 NCHW stores
+//   2 MMA       : wgmma bf16 x bf16 -> fp32 accumulators in registers, one warpgroup per 64 positions;
+//     warpgroups  every operand is an exact small integer or an exact bf16 piece of an fp32 value,
+//                 M = 128 positions, N = output channels of the group, K = 16 channels per MMA; then the
+//                 epilogue: scale + bias (fwd) or STE mask (dgrad) -> coalesced fp32 NCHW stores
 #include <cuda.h>
 #include <cstdlib>
 #include <cuda_bf16.h>
@@ -32,12 +31,14 @@
 namespace tcconv {
 
 constexpr int NTHREADS = 512;
-constexpr int NCONV = 320;  // converter threads (warps 2, 3 and 8..15)
+constexpr int NCONV = 224;  // converter threads (warps 1..3 and 12..15); warps 4..11 are the two MMA warpgroups
 constexpr int NCW = NCONV / 32;
-constexpr int NEPI = 128;   // epilogue threads (warps 4..7)
-constexpr int MAXST = 8, BASEST = 4, MAXOP = 4, NACC = 2;  // staging ring / operand ring: as deep as shared memory allows (plan())
+constexpr int MAXST = 8, BASEST = 4, MAXOP = 4;  // staging ring / operand ring: as deep as shared memory allows (plan())
+constexpr int kMaxNG = 160;  // output channels per group: the accumulator row of one thread is NG / 2 registers
 constexpr int KMAX = 6;     // operand entries per converter thread and chunk
 constexpr int kMaxDynSmem = 227 * 1024 - 6144;  // 227 KB per CTA minus the static block below (5 KB)
+constexpr int kStgBytes = 2 * 32 * 68 * 4;        // two 64 x 32 epilogue staging tiles (tc::kStageLd64)
+constexpr int kPlanSmem = kMaxDynSmem - kStgBytes;
 
 struct Params {
   // tensors: input [B, Cin, H, W], output [B, Cout, H, W]
@@ -47,8 +48,8 @@ struct Params {
   int quant_mode;   // 0: raw fp32 input (exact 3-term split); else MNB_ACT_DOREFA / MNB_ACT_IAO
   int dgrad;        // 1: weights transposed + flipped, per-input-channel pre-scale, STE epilogue
   int dbg;          // MNB_TC_DEBUG (timing experiments only): 1 no converter fence, 2 no converter work, 4 no epilogue stores, 8 no MMAs
-  int a_offset, tmem_cols;
-  int stage_bytes, op_term_bytes, op_buf_bytes, b_group_bytes, off_stage, off_op, off_b;
+  int a_offset;
+  int stage_bytes, op_term_bytes, op_buf_bytes, b_group_bytes, off_stage, off_op, off_b, off_stg;
   float a_scale_const;
   mnb_act_qparams qp;
   const int16_t* w_int;     // [K, Cg, R, S] integer weights (K = fwd output channels)
@@ -62,14 +63,12 @@ struct Params {
   int* err;
   long long* prof;  // optional debug counters (cycles): see mnb_set_tc_profile_buffer
   // per (tap, k-step): start-address offsets (16-byte units) of the A and B operands.  Kept in the kernel parameters
-  // (constant bank), NOT in shared memory: the MMA warp's descriptor arithmetic then stays in uniform registers; a
-  // table read with LDS forces an ELECT + five R2UR.BROADCAST in front of every tcgen05.mma.
+  // (constant bank), NOT in shared memory: the MMA warps' descriptor arithmetic then stays in uniform registers.
   uint2 mma_off[64];
 };
 
 struct alignas(16) Shared {
-  uint64_t stage_full[MAXST], stage_empty[MAXST], op_full[MAXOP], op_empty[MAXOP], acc_full[NACC], acc_empty[NACC], b_full;
-  uint32_t tmem_slot;
+  uint64_t stage_full[MAXST], stage_empty[MAXST], op_full[MAXOP], op_empty[MAXOP], b_full;
   uint32_t abort;
   uint32_t op_flags[MAXOP][NCW];
   alignas(16) float epi_scale[288];   // per output channel of the slab (fixed for the whole kernel)
@@ -106,6 +105,11 @@ __device__ __forceinline__ void split3_pair(float a, float b, uint32_t& hp, uint
     if (p.prof) prof_acc[slot] += clock64() - t0__;             \
   } while (0)
 
+__device__ __forceinline__ void wg_bar_sync(int wg) {  // named barriers 2, 3: one MMA warpgroup
+  asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+}
+
+template <int NG>   // output channels per group (GEMM N)
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -114,7 +118,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
   uint8_t* stage_base = smem + p.off_stage;
   uint8_t* op_base = smem + p.off_op;
   uint8_t* b_base = smem + p.off_b;
-  const int RS = p.R * p.S, c8_per_group = p.cin_g / 8;
   long long prof_acc[3] = {0, 0, 0};
   const long long prof_t0 = p.prof ? clock64() : 0;
 
@@ -128,19 +131,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
   // ---- one-time setup
   if (tid == 0) {
     for (int i = 0; i < p.nst; ++i) { tc::mbar_init(&sh.stage_full[i], 1); tc::mbar_init(&sh.stage_empty[i], NCONV / 32); }
-    for (int i = 0; i < MAXOP; ++i) { tc::mbar_init(&sh.op_full[i], NCONV / 32); tc::mbar_init(&sh.op_empty[i], 1); }
-    for (int i = 0; i < NACC; ++i) { tc::mbar_init(&sh.acc_full[i], 1); tc::mbar_init(&sh.acc_empty[i], NEPI); }
+    for (int i = 0; i < MAXOP; ++i) { tc::mbar_init(&sh.op_full[i], NCONV / 32); tc::mbar_init(&sh.op_empty[i], 8); }
     tc::mbar_init(&sh.b_full, 1);
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tmap_in);
   }
   if (tid < MAXOP * NCW) sh.op_flags[tid / NCW][tid % NCW] = 0;
   if (tid == 0) sh.abort = 0;
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&sh.tmem_slot)),
-                 "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   // zero the operand buffers once: the mid / lo planes are only rewritten when a chunk needs them
   for (int i = tid; i < p.nop * p.op_buf_bytes / 16; i += NTHREADS)
     reinterpret_cast<uint4*>(op_base)[i] = make_uint4(0, 0, 0, 0);
@@ -158,10 +155,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
     }
   }
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = sh.tmem_slot;
 
   if (warp == 0) {
     // ================================================================= TMA producer
@@ -195,156 +189,132 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================================================= MMA issuer
-    // The whole warp runs the (warp-uniform) loops and address arithmetic; only lane 0's guard lets the
-    // tcgen05.mma through.  Terms that a chunk does not need are predicated off instead of shortening
-    // the loop, so every trip count stays uniform.
-    {
-      const uint32_t lead = lane == 0;
-      const uint32_t idesc = tc::make_idesc(1, 1, 1, 128, (uint32_t)p.cout_g);
-      const uint32_t a_lbo = (uint32_t)p.npos_in * 16u, b_lbo = (uint32_t)p.cout_g * 16u;
-      // descriptors differ only in the 14-bit start-address field: build once, then add (bytes >> 4)
-      const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(op_base), a_lbo, 128);
-      const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(b_base), b_lbo, 128);
-      const uint32_t a_kstep = (2u * a_lbo) >> 4, a_term = (uint32_t)p.op_term_bytes >> 4, a_buf = (uint32_t)p.op_buf_bytes >> 4;
-      const uint32_t b_kstep = (2u * b_lbo) >> 4, b_tap = (uint32_t)(c8_per_group * p.cout_g * 16) >> 4;
-      const uint32_t b_chunk = (uint32_t)((p.CC / 8) * p.cout_g * 16) >> 4, b_group = (uint32_t)p.b_group_bytes >> 4;
-      const int ksteps = p.CC / 16, slab_cols = g_count * p.cout_g;
-      const int max_terms = p.quant_mode == 0 ? 3 : 1;
-      PROF_SOFT(0, tc::mbar_wait_soft(&sh.b_full, 0, p.err, 307, &sh.abort));
-      uint32_t item = 0;
-      int ob = -1;
-      uint32_t oph = 1;
-      for (int tile = rank_in_slab; tile < p.n_tiles; tile += ctas_in_slab, ++item) {
-        const int acc = item % NACC;
-        const uint32_t aph = (item / NACC) & 1;
-        PROF_SOFT(0, tc::mbar_wait_soft(&sh.acc_empty[acc], aph ^ 1, p.err, 302, &sh.abort));
-        tc::tc_fence_after();
-        for (int gi = 0; gi < g_count; ++gi) {
-          const uint32_t d_tmem = tmem + (uint32_t)(acc * slab_cols + gi * p.cout_g);
-          uint32_t accumulate = 0;
-          for (int ch = 0; ch < p.nchunk; ++ch) {
-            if (++ob == p.nop) ob = 0;
-            oph ^= (ob == 0);
-            PROF_SOFT(1, tc::mbar_wait_soft(&sh.op_full[ob], oph, p.err, 303, &sh.abort));
-            tc::tc_fence_after();
-            bool need_low = false;  // mid / lo planes needed for this chunk?
-            if (p.quant_mode == 0) {
-              uint32_t any = 0;
-#pragma unroll
-              for (int w8 = 0; w8 < NCW; ++w8) any |= sh.op_flags[ob][w8];
-              need_low = __any_sync(0xffffffffu, any != 0);   // a vote result is provably warp-uniform (uniform datapath below)
-            }
-            const uint64_t a_chunk = a_desc0 + (uint64_t)((uint32_t)ob * a_buf);
-            const uint64_t b_chunk_d = b_desc0 + (uint64_t)((uint32_t)gi * b_group + (uint32_t)ch * b_chunk);
-            const long long tmma0 = p.prof ? clock64() : 0;
-            // one flat loop over (tap, k-step): the offsets come from a small shared-memory table so the
-            // single issuing thread spends a handful of instructions per MMA
-            const int n_off = (p.dbg & 8) ? 0 : RS * ksteps;
-            if (max_terms == 3 && need_low) {
-              for (int e = 0; e < n_off; ++e) {
-                const uint2 off = p.mma_off[e];
-                const uint64_t ad = a_chunk + (uint64_t)off.x, bd = b_chunk_d + (uint64_t)off.y;
-                tc::mma_f16_guarded(d_tmem, ad, bd, idesc, accumulate, lead);
-                tc::mma_f16_guarded(d_tmem, ad + a_term, bd, idesc, 1, lead);
-                tc::mma_f16_guarded(d_tmem, ad + 2 * a_term, bd, idesc, 1, lead);
-                accumulate = 1;
-              }
-            } else {
-              for (int e = 0; e < n_off; ++e) {
-                const uint2 off = p.mma_off[e];
-                tc::mma_f16_guarded(d_tmem, a_chunk + (uint64_t)off.x, b_chunk_d + (uint64_t)off.y, idesc, accumulate, lead);
-                accumulate = 1;
-              }
-            }
-            if (p.prof) prof_acc[2] += clock64() - tmma0;
-            if (lead) tc::mma_commit(&sh.op_empty[ob]);  // operand buffer is free once these MMAs retire
-            __syncwarp();
-          }
-        }
-        if (lead) tc::mma_commit(&sh.acc_full[acc]);
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ================================================================= epilogue
-    const int q = warp - 4;            // TMEM lane quarter of this warp (warp % 4)
-    const int pos = q * 32 + lane;     // GEMM row = padded-tile position
+  } else if (warp >= 4 && warp < 12) {
+    // ================================================================= MMA warpgroups + epilogue
+    // Warpgroup wg (warps 4..7 / 8..11) owns GEMM rows (= padded-tile positions) 64*wg .. 64*wg+63 of every group's
+    // accumulator (m64 x NG in registers).  Epilogue: 32 columns at a time through a 64 x 32 staging tile; thread lt of
+    // the warpgroup then owns position 64*wg + lt%64 and 16 of the 32 columns (lt / 64), stored as coalesced NCHW rows.
+    const int wg = (warp - 4) >> 2, lt = tid - 128 * (wg + 1);
+    float* stage = reinterpret_cast<float*>(smem + p.off_stg) + wg * 32 * tc::kStageLd64;
+    const int pos = 64 * wg + (lt & 63), ehalf = lt >> 6;
     const int tb = pos / (p.THH * p.BW);
     const int rem = pos - tb * (p.THH * p.BW);
     const int th = rem / p.BW, wc = rem - th * p.BW;
     MnbActQ ste;
     if (p.dgrad && p.ste_bits) ste = mnb_load_actq(p.qp);
     const int64_t plane = (int64_t)p.H * p.W;
-    const int slab_cols = g_count * p.cout_g, ch_first = g_first * p.cout_g;
-    uint32_t item = 0;
-    for (int tile = rank_in_slab; tile < p.n_tiles; tile += ctas_in_slab, ++item) {
+    const int ch_first = g_first * p.cout_g;
+    const uint32_t a_lbo = (uint32_t)p.npos_in * 16u, b_lbo = (uint32_t)p.cout_g * 16u;
+    // descriptors differ only in the 14-bit start-address field: build once, then add (bytes >> 4)
+    const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(op_base), a_lbo, 128) + (uint64_t)(64 * wg);
+    const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(b_base), b_lbo, 128);
+    const uint32_t a_term = (uint32_t)p.op_term_bytes >> 4, a_buf = (uint32_t)p.op_buf_bytes >> 4;
+    const uint32_t b_chunk = (uint32_t)((p.CC / 8) * p.cout_g * 16) >> 4, b_group = (uint32_t)p.b_group_bytes >> 4;
+    const int ksteps = p.CC / 16;
+    const int max_terms = p.quant_mode == 0 ? 3 : 1;
+    PROF_SOFT(0, tc::mbar_wait_soft(&sh.b_full, 0, p.err, 307, &sh.abort));
+    int ob = -1;
+    uint32_t oph = 1;
+    for (int tile = rank_in_slab; tile < p.n_tiles; tile += ctas_in_slab) {
       const int bt = tile / p.row_tiles, rt = tile - bt * p.row_tiles;
       const int b = bt * p.TB + tb, h = rt * p.TH + th;
       const bool valid = tb < p.TB && th < p.TH && wc < p.W && b < p.B && h < p.H;
-      const int acc = item % NACC;
-      const uint32_t aph = (item / NACC) & 1;
-      PROF_WAIT(0, tc::mbar_wait(&sh.acc_full[acc], aph, p.err, 304));
-      tc::tc_fence_after();
       float* orow = p.out + (((int64_t)b * p.Cout + ch_first) * p.H + h) * p.W + wc;
       const int64_t obase = (((int64_t)b * p.Cout + ch_first) * p.H + h) * p.W + wc;
-      for (int n0 = 0; n0 < slab_cols; n0 += 32) {
-        uint32_t r[32];
-        tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * slab_cols + n0), r);
-        tc::tmem_ld_wait();
-        if (valid && !(p.dbg & 4)) {
-          if (!p.dgrad) {
-            // scale / bias of the 32 columns as 16 vector loads up front (the per-element LDS latency
-            // chain was the kernel's bottleneck), then a pure FFMA + STG stream
-            float sc[32], bs[32];
+      for (int gi = 0; gi < g_count; ++gi) {
+        float acc[NG / 2];
+        tc::zero_acc(acc);
+        for (int ch = 0; ch < p.nchunk; ++ch) {
+          if (++ob == p.nop) ob = 0;
+          oph ^= (ob == 0);
+          PROF_SOFT(1, tc::mbar_wait_soft(&sh.op_full[ob], oph, p.err, 303, &sh.abort));
+          bool need_low = false;  // mid / lo planes needed for this chunk?
+          if (p.quant_mode == 0) {
+            uint32_t any = 0;
 #pragma unroll
-            for (int v = 0; v < 8; ++v) {
-              const float4 a = *reinterpret_cast<const float4*>(&sh.epi_scale[n0 + 4 * v]);
-              const float4 c = *reinterpret_cast<const float4*>(&sh.epi_bias[n0 + 4 * v]);
+            for (int w8 = 0; w8 < NCW; ++w8) any |= sh.op_flags[ob][w8];
+            need_low = __any_sync(0xffffffffu, any != 0);
+          }
+          const uint64_t a_chunk = a_desc0 + (uint64_t)((uint32_t)ob * a_buf);
+          const uint64_t b_chunk_d = b_desc0 + (uint64_t)((uint32_t)gi * b_group + (uint32_t)ch * b_chunk);
+          const long long tmma0 = p.prof ? clock64() : 0;
+          const int n_off = (p.dbg & 8) ? 0 : p.R * p.S * ksteps;
+          tc::wg_fence();
+          tc::fence_acc(acc);
+          if (max_terms == 3 && need_low) {
+            for (int e = 0; e < n_off; ++e) {
+              const uint2 off = p.mma_off[e];
+              const uint64_t ad = a_chunk + (uint64_t)off.x, bd = b_chunk_d + (uint64_t)off.y;
+              tc::Mma<NG>::template bf16<0, 0>(acc, ad, bd, 1);
+              tc::Mma<NG>::template bf16<0, 0>(acc, ad + a_term, bd, 1);
+              tc::Mma<NG>::template bf16<0, 0>(acc, ad + 2 * a_term, bd, 1);
+            }
+          } else {
+            for (int e = 0; e < n_off; ++e) {
+              const uint2 off = p.mma_off[e];
+              tc::Mma<NG>::template bf16<0, 0>(acc, a_chunk + (uint64_t)off.x, b_chunk_d + (uint64_t)off.y, 1);
+            }
+          }
+          tc::wg_commit();
+          tc::wg_wait<0>();
+          tc::fence_acc(acc);
+          if (p.prof) prof_acc[2] += clock64() - tmma0;
+          __syncwarp();
+          if (lane == 0) tc::mbar_arrive(&sh.op_empty[ob]);  // this warp's share of the operand buffer is read
+        }
+        const int gcol = gi * p.cout_g;
+#pragma unroll
+        for (int c0 = 0; c0 < NG; c0 += 32) {
+          wg_bar_sync(wg);   // the previous staging tile has been read
+          tc::frag_cols_to_smem(acc, stage, tc::kStageLd64, 0, c0, 32);
+          wg_bar_sync(wg);
+          const int nb = gcol + c0 + 16 * ehalf;   // first slab column of this thread
+          if (c0 + 16 * ehalf >= NG || !valid || (p.dbg & 4)) continue;
+          float r[16];
+#pragma unroll
+          for (int j = 0; j < 16; ++j) r[j] = stage[(16 * ehalf + j) * tc::kStageLd64 + (lt & 63)];
+          if (!p.dgrad) {
+            // scale / bias of the 16 columns as vector loads up front, then a pure FFMA + STG stream
+            float sc[16], bs[16];
+#pragma unroll
+            for (int v = 0; v < 4; ++v) {
+              const float4 a = *reinterpret_cast<const float4*>(&sh.epi_scale[nb + 4 * v]);
+              const float4 c = *reinterpret_cast<const float4*>(&sh.epi_bias[nb + 4 * v]);
               sc[4 * v] = a.x; sc[4 * v + 1] = a.y; sc[4 * v + 2] = a.z; sc[4 * v + 3] = a.w;
               bs[4 * v] = c.x; bs[4 * v + 1] = c.y; bs[4 * v + 2] = c.z; bs[4 * v + 3] = c.w;
             }
-            float* op = orow + (int64_t)n0 * plane;
+            float* op = orow + (int64_t)nb * plane;
 #pragma unroll
-            for (int j = 0; j < 32; ++j, op += plane)
-              if (n0 + j < slab_cols) *op = fmaf(__uint_as_float(r[j]), sc[j], bs[j]);
+            for (int j = 0; j < 16; ++j, op += plane) *op = fmaf(r[j], sc[j], bs[j]);
           } else if (p.ste_bits) {
-            // the 32 channel planes' mask words first (independent loads), then select + store.  The
-            // reference's STE computes ((g*s)*pass)/s (IAO) or (((g*s)/s)*pass)*0.1 (DoReFa); (g*s)/s is
-            // g to within one ulp, so the epilogue passes g itself (well inside the 1e-5 contract).
-            const int64_t fi0 = obase + (int64_t)n0 * plane;
+            // the 16 channel planes' mask words first (independent loads), then select + store.  The reference's STE
+            // computes ((g*s)*pass)/s (IAO) or (((g*s)/s)*pass)*0.1 (DoReFa); (g*s)/s is g to within one ulp, so the
+            // epilogue passes g itself (well inside the 1e-5 contract).
+            const int64_t fi0 = obase + (int64_t)nb * plane;
             const uint32_t shift = (uint32_t)(fi0 & 31);
             const bool same_bit = (plane & 31) == 0;
-            uint32_t wbits[32];
+            uint32_t wbits[16];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int64_t fi = fi0 + (int64_t)j * plane;
-              wbits[j] = (n0 + j < slab_cols) ? __ldg(p.ste_bits + (fi >> 5)) : 0u;
-            }
+            for (int j = 0; j < 16; ++j) wbits[j] = __ldg(p.ste_bits + ((fi0 + (int64_t)j * plane) >> 5));
             const float gain = ste.mode == MNB_ACT_DOREFA ? 0.1f : 1.f;
-            float* op = orow + (int64_t)n0 * plane;
+            float* op = orow + (int64_t)nb * plane;
 #pragma unroll
-            for (int j = 0; j < 32; ++j, op += plane)
-              if (n0 + j < slab_cols) {
-                const uint32_t sh_j = same_bit ? shift : (uint32_t)((fi0 + (int64_t)j * plane) & 31);
-                const bool pass = (wbits[j] >> sh_j) & 1u;
-                *op = pass ? __uint_as_float(r[j]) * gain : 0.f;
-              }
+            for (int j = 0; j < 16; ++j, op += plane) {
+              const uint32_t sh_j = same_bit ? shift : (uint32_t)((fi0 + (int64_t)j * plane) & 31);
+              const bool pass = (wbits[j] >> sh_j) & 1u;
+              *op = pass ? r[j] * gain : 0.f;
+            }
           } else {
-            float* op = orow + (int64_t)n0 * plane;
+            float* op = orow + (int64_t)nb * plane;
 #pragma unroll
-            for (int j = 0; j < 32; ++j, op += plane)
-              if (n0 + j < slab_cols) *op = __uint_as_float(r[j]);
+            for (int j = 0; j < 16; ++j, op += plane) *op = r[j];
           }
         }
       }
-      tc::tc_fence_before();
-      tc::mbar_arrive(&sh.acc_empty[acc]);
     }
-  } else if (warp >= 8 || warp == 2 || warp == 3) {
-    // ================================================================= converters
-    const int ct = warp >= 8 ? tid - 256 + 64 : tid - 64;
+  } else {
+    // ================================================================= converters (warps 1..3, 12..15)
+    const int ct = warp >= 12 ? tid - 384 + 96 : tid - 32;
     const int cw = ct >> 5;
     MnbActQ q;
     if (p.quant_mode != 0) q = mnb_load_actq(p.qp);
@@ -501,20 +471,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
     }
   }
 done:
-  if (p.prof && lane == 0 && (warp == 0 || warp == 1 || warp == 4 || warp == 8)) {
-    // slots: [role 0..3 = tma, mma, epilogue, converter][wait a, wait b, wait c, total]
-    const int role = warp == 0 ? 0 : (warp == 1 ? 1 : (warp == 4 ? 2 : 3));
+  if (p.prof && lane == 0 && (warp == 0 || warp == 4 || warp == 8 || warp == 12)) {
+    // slots: [role 0..3 = tma, mma warpgroup 0, mma warpgroup 1, converter][wait a, wait b, wait c, total]
+    const int role = warp == 0 ? 0 : (warp == 4 ? 1 : (warp == 8 ? 2 : 3));
     atomicAdd(reinterpret_cast<unsigned long long*>(p.prof + role * 4 + 0), (unsigned long long)prof_acc[0]);
     atomicAdd(reinterpret_cast<unsigned long long*>(p.prof + role * 4 + 1), (unsigned long long)prof_acc[1]);
     atomicAdd(reinterpret_cast<unsigned long long*>(p.prof + role * 4 + 2), (unsigned long long)prof_acc[2]);
     atomicAdd(reinterpret_cast<unsigned long long*>(p.prof + role * 4 + 3), (unsigned long long)(clock64() - prof_t0));
   }
-  tc::tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc::tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols));
-  }
 }
 
 static long long* g_prof_buffer = nullptr;
@@ -555,7 +520,7 @@ static int plan(const mnb_conv_shape* s, bool dgrad, int quant_mode, Params& p, 
   p.dgrad = dgrad ? 1 : 0;
   p.Cin = dgrad ? K : C; p.Cout = dgrad ? C : K;
   p.cin_g = p.Cin / G; p.cout_g = p.Cout / G;
-  if (p.cin_g % 16 || p.cout_g % 16 || p.cout_g > 256) return unsupported("channels per group");
+  if (p.cin_g % 16 || p.cout_g % 16 || p.cout_g > kMaxNG) return unsupported("channels per group");
   if ((p.W * 4) % 16 || p.W > 64 || p.H > 255) return unsupported("image size");
   p.BW = p.W + 2 * p.pad;
   p.TH = std::min(p.H, 128 / p.BW);
@@ -589,12 +554,12 @@ static int plan(const mnb_conv_shape* s, bool dgrad, int quant_mode, Params& p, 
   int fixed = 0, budget = 0;
   for (;; --p.nst) {
     fixed = (p.nst * p.stage_bytes + 1023) / 1024 * 1024 + (p.nop * p.op_buf_bytes + 1023) / 1024 * 1024;
-    budget = kMaxDynSmem - fixed;
+    budget = kPlanSmem - fixed;
     if (budget >= p.b_group_bytes || p.nst == 2) break;
   }
   if (budget < p.b_group_bytes) return unsupported("weights of one group do not fit in shared memory");
   int max_groups = std::max(1, std::min(p.G, std::min(budget / p.b_group_bytes, std::max(1, 64 * 1024 / p.b_group_bytes))));
-  max_groups = std::max(1, std::min(max_groups, 256 / p.cout_g));  // one accumulator row block per tile: <= 256 columns
+  max_groups = std::max(1, std::min(max_groups, 256 / p.cout_g));  // per-channel constants of a slab: <= 256 columns
   if (dgrad) {  // per-input-channel scales of the slab are staged in a 288-float shared array
     if (p.cin_g > 288) return unsupported("more than 288 gradient channels per group");
     max_groups = std::max(1, std::min(max_groups, 288 / p.cin_g));
@@ -602,25 +567,22 @@ static int plan(const mnb_conv_shape* s, bool dgrad, int quant_mode, Params& p, 
   while (p.G % max_groups) --max_groups;  // equal slabs: every CTA does the same work per tile
   p.slab_groups = max_groups;
   p.n_slabs = p.G / p.slab_groups;
-  // The pipeline floor is TMA latency x bytes in flight (measured: 4 slots of 16 KB sustain ~22 B/ns per SM, half of
-  // what the HBM share of an SM needs), so every kilobyte the weights and operands leave free becomes staging slots.
+  // The pipeline floor is TMA latency x bytes in flight, so every kilobyte the weights and operands leave free becomes
+  // staging slots.
   auto fits = [&](int nst, int nop) {
     return (nst * p.stage_bytes + 1023) / 1024 * 1024 + (nop * p.op_buf_bytes + 1023) / 1024 * 1024 +
-               p.slab_groups * p.b_group_bytes <= kMaxDynSmem;
+               p.slab_groups * p.b_group_bytes <= kPlanSmem;
   };
-  // Spare shared memory goes to the OPERAND ring first: the converter -> MMA -> commit -> converter round trip costs
-  // ~1300 cycles even with no work in it (measured with the kernel's parts switched off), so with two operand buffers
-  // a chunk cannot take less than ~650 cycles; extra staging slots were measured to change nothing.
+  // Spare shared memory goes to the OPERAND ring first: the converter -> MMA -> release -> converter round trip has a
+  // fixed latency even with no work in it, and more operand buffers hide it.
   while (p.nop < MAXOP && fits(p.nst, p.nop + 1)) ++p.nop;
   while (p.nst < MAXST && fits(p.nst + 1, p.nop)) ++p.nst;
   p.off_stage = 0;
   p.off_op = (p.nst * p.stage_bytes + 1023) / 1024 * 1024;
   p.off_b = p.off_op + (p.nop * p.op_buf_bytes + 1023) / 1024 * 1024;
-  smem_bytes = p.off_b + p.slab_groups * p.b_group_bytes;
+  p.off_stg = (p.off_b + p.slab_groups * p.b_group_bytes + 15) / 16 * 16;
+  smem_bytes = p.off_stg + kStgBytes;
   if (smem_bytes > kMaxDynSmem) return unsupported("shared memory budget");
-  int cols = 32;
-  while (cols < NACC * p.slab_groups * p.cout_g) cols <<= 1;
-  p.tmem_cols = cols;
   return 0;
 }
 
@@ -632,7 +594,7 @@ static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t 
   }
   CUtensorMap tmap;
   if (p.pad == 0) {
-    // The TMA unit's cost is per box row (measured ~12 cycles per row per SM, whatever its length): a 1x1 filter
+    // The TMA unit's cost is per box row, whatever its length: a 1x1 filter
     // needs no halo, so H and W collapse into one dimension and a tile is TH*W contiguous floats per channel
     // (4 x fewer rows than W-wide ones at 32x32).  Same shared-memory image as the 4-D box.
     uint64_t dims[3] = {(uint64_t)p.H * p.W, (uint64_t)p.Cin, (uint64_t)p.B};
@@ -643,11 +605,16 @@ static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t 
     uint32_t box[4] = {(uint32_t)p.W, (uint32_t)p.THH, (uint32_t)p.CC, (uint32_t)p.TB};
     if (int e = mnb_make_tmap(&tmap, in, 4, 4, dims, box)) return e;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t ce = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  using KernelFn = void (*)(const CUtensorMap, const Params);
+  static const KernelFn kernels[kMaxNG / 16] = {conv_tc_kernel<16>,  conv_tc_kernel<32>,  conv_tc_kernel<48>,  conv_tc_kernel<64>,
+                                                conv_tc_kernel<80>,  conv_tc_kernel<96>,  conv_tc_kernel<112>, conv_tc_kernel<128>,
+                                                conv_tc_kernel<144>, conv_tc_kernel<160>};
+  static bool attr_set[kMaxNG / 16] = {};
+  const int ki = p.cout_g / 16 - 1;
+  if (!attr_set[ki]) {
+    cudaError_t ce = cudaFuncSetAttribute(kernels[ki], cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
     if (ce != cudaSuccess) return mnb_fail((int)ce, "cudaFuncSetAttribute: %s", cudaGetErrorString(ce));
-    attr_set = true;
+    attr_set[ki] = true;
   }
   const int64_t items = (int64_t)p.n_tiles * p.n_slabs;
   int grid = (int)std::min<int64_t>(items, MNB_NUM_SMS);
@@ -667,7 +634,7 @@ static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t 
                                  (uint32_t)tap * (uint32_t)(c8_per_group * p.cout_g) + (uint32_t)j * (uint32_t)(2 * p.cout_g));
     }
   }
-  conv_tc_kernel<<<grid, NTHREADS, smem_bytes, st>>>(tmap, pp);
+  kernels[ki]<<<grid, NTHREADS, smem_bytes, st>>>(tmap, pp);
   MNB_LAUNCHED(2);
   return 0;
 }

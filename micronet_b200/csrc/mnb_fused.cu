@@ -244,7 +244,7 @@ static bool planes_vectorizable(int64_t n, int hw, const void* a, const void* b,
          (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15) == 0;
 }
 // (channels x splits) blocks: about two waves of 8 resident 256-thread blocks per SM, so that every block streams
-// >= ~100 KB (blocks of 32 KB spend as long being scheduled as loading: 2.4 TB/s instead of 4.5+)
+// >= ~100 KB (small blocks spend as long being scheduled as loading)
 static int plane_splits(int batch, int64_t per, int channels) {
   const int64_t want = (2 * 8 * MNB_NUM_SMS + channels - 1) / channels;
   return (int)std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(std::min<int64_t>(FUSED_SPLITS, batch), per / 2048), want));

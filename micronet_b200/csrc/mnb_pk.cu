@@ -1,4 +1,4 @@
-// Packed-operand ("pk") tensor-core convolution family: any conv geometry of the QAT models on tcgen05.
+// Packed-operand ("pk") tensor-core convolution family: any conv geometry of the QAT models on Hopper wgmma.
 //
 // Why a second family next to mnb_conv_tc_fwd.cu / mnb_conv_tc_wgrad.cu: those kernels keep the whole weight
 // slab of a group resident in shared memory and convert fp32 activations inside the kernel, which limits them
@@ -12,9 +12,9 @@
 //   weights                 : bf16 image [n-tile][group][stage][term][tap][c/8][n][8] (K-major, rows = n), written
 //                             once per optimizer step by pk_pack_weight_kernel;
 //
-// so the convolution itself is the canonical Blackwell pipeline TMA -> tcgen05.mma -> TMEM -> epilogue with no
+// so the convolution itself is the canonical Hopper pipeline TMA -> wgmma (register accumulators) -> epilogue with no
 // converter warps.  A 5-D tensor map (8, W, H, B, C/8) with the channel-octet dimension declared LAST makes one
-// box land in shared memory as op[c/8][position][8]: the UMMA K-major no-swizzle canonical layout with the
+// box land in shared memory as op[c/8][position][8]: the wgmma K-major no-swizzle canonical layout with the
 // positions of the zero-padded tile as GEMM rows (halo rows AND columns zero-filled by the TMA unit), so filter tap
 // (r, s) is the same buffer with the descriptor start address moved by (r*BW + s)*16 bytes: implicit GEMM without
 // im2col.  The same buffers read as MN-major operands give the weight gradient (positions = reduction dimension).
@@ -23,7 +23,7 @@
 // channel octets, every filter tap then is a stride-1 tap of ONE phase plane with a shift in {-1, 0} (data gradient:
 // four output phases, each a stride-1 conv of dy with a subset of the taps).
 //
-// Exactness: integer levels (|e| <= 256) are exact in bf16, products exact, fp32 accumulation in TMEM.  fp32 operands
+// Exactness: integer levels (|e| <= 256) are exact in bf16, products exact, fp32 accumulation in registers.  fp32 operands
 // are split into T exact bf16 pieces; the products p_i * q_j with i + j < max(Ta, Tb) are accumulated, smallest first.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -37,10 +37,10 @@
 
 namespace pk {
 
-constexpr int NTHREADS = 256;      // warp 0 TMA, warp 1 MMA issue, warp 2 TMEM alloc, warps 4..7 epilogue
 constexpr int MAXST = 8;           // operand ring (power of two: ring index = counter & mask)
 constexpr int MAXTAP = 64, MAXTMPL = 16, MAXY = 4, MAXPAIR = 6, MAXPROG = 512;
 constexpr int kSmemBudget = 227 * 1024 - 3072;   // dynamic shared memory the kernels may ask for
+constexpr int kNtSizes[] = {16, 32, 48, 64, 96, 128};   // N tiles the convolution kernel is instantiated for
 
 // ---------------------------------------------------------------------------------------------------------
 // plan: everything about a (shape, mode) pair that the weight packer and the convolution must agree on
@@ -64,7 +64,7 @@ struct Plan {
   short tap_r[MAXY][MAXTAP], tap_s[MAXY][MAXTAP];
   int img_bytes[MAXY], y_off[MAXY];      // bytes of one (n-tile, group) weight image of output phase y; prefix offsets
   int64_t wimg_bytes;
-  int a_box_bytes, a_bytes, b_off, stage_bytes, nstage, st_log2, smem_bytes, tmem_cols;
+  int a_box_bytes, a_bytes, b_off, stage_bytes, nstage, st_log2, smem_bytes, off_stg;
   int segmented, seg_len;   // stages per accumulation segment (segmented mode)
 };
 
@@ -159,9 +159,8 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   {
     const int ct_min = ceil_div(p.OWr, 128 - halo_w);
     double best = 1e30;
-    // (measured, r2w / r2x: the single-product kernels gain from narrower tiles - 64 -> 64 3x3 @32: 62 -> 53 us - while the
-    // segmented split-fp32 kernels lose 10 - 15 % unless the widest tiling re-reads its halo rows more than ~2.2 x, as on
-    // 112- and 224-wide planes)
+    // (the single-product kernels gain from narrower tiles, while the segmented split-fp32 kernels keep the widest tiling
+    // unless it re-reads its halo rows more than ~2.2 x, as on 112- and 224-wide planes)
     int ct_max = std::min(p.OWr, ct_min + 14);
     if (p.npairs > 1) {
       const int wt0 = ceil_div(p.OWr, ct_min), bw0 = wt0 + halo_w;
@@ -198,14 +197,11 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   p.n_mtiles = p.img_tiles * p.row_tiles * p.col_tiles;
   // ---- N tile
   const int ng16 = round_up(p.ng, 16);
-  // Split fp32 operands (more than one piece product per K-step) run in SEGMENTED mode: tcgen05.mma truncates the running
-  // fp32 accumulator after every instruction (a bias of ~2e-8 of |D| per MMA, measured: 3e-5 after 1700 chained MMAs),
-  // so the K loop is cut into segments of <= ~64 MMAs, each into a fresh TMEM accumulator, and the epilogue warps add
-  // the segments in registers with round-to-nearest adds.  That needs the whole N tile in registers: Nt <= 128, MT = 1.
-  // A K loop that is short anyway needs no segments: the whole chain of one accumulator (taps x piece pairs x K-steps) is
-  // then no longer than a segment would be, and the kernel keeps the rolled epilogue, MT > 1 and N tiles up to 256 (the
-  // data gradients of NIN-GC's grouped layers: 16 / 36 MMAs per accumulator; r2z: the segmented form of the 256-channel 1x1
-  // data gradient took 226 us against 95 us for the forward of the same tile shape).
+  // Split fp32 operands (more than one piece product per K-step) run in SEGMENTED mode: the tensor core does not round the
+  // running fp32 accumulator to nearest after every instruction, so the K loop is cut into segments of <= ~64 MMAs, each
+  // into zeroed accumulators, and the segments are added into running sums with round-to-nearest fp32 adds.  A K loop that
+  // is short anyway needs no segments: the whole chain of one accumulator (taps x piece pairs x K-steps) is then no longer
+  // than a segment would be.
   {
     int seg_target = 64;
     if (const char* e = getenv("MNB_PK_SEG_MMAS")) seg_target = std::max(1, atoi(e));
@@ -213,17 +209,18 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
     for (int y = 0; y < p.ny; ++y) chain = std::max(chain, p.ntap[y] * p.npairs * ceil_div(p.kg, 16));
     p.segmented = p.npairs > 1 && chain > seg_target;
   }
-  if (ng16 <= 128) p.Nt = ng16;
-  else if (ng16 % 128 == 0) p.Nt = 128;
-  else if (ng16 <= 256 && !p.segmented) p.Nt = ng16;
-  else if (ng16 <= 256) p.Nt = round_up(ceil_div(p.ng, 2), 16);
-  else p.Nt = 128;
+  // N tile: the accumulators of a thread are MT x Nt / 2 registers (two warpgroups, 64 rows each), so Nt <= 128, and Nt is
+  // one of the widths the kernel is instantiated for (kNtSizes); the weight image zero-pads the columns beyond ng
+  {
+    const int ntiles = ceil_div(ng16, 128);
+    const int want = round_up(ceil_div(ng16, ntiles), 16);
+    p.Nt = 128;
+    for (int v : kNtSizes) if (v >= want) { p.Nt = v; break; }
+  }
   p.n_ntiles = ceil_div(p.ng, p.Nt);
-  // M tiles per work item: every item streams the WHOLE weight block of its (N tile, group) from L2 - measured floor of the
-  // 64 -> 64 3x3 layer with the MMAs switched off (MNB_PK_DEBUG=2): 190 us for the split-fp32 forward at MT = 1, i.e. L2 ->
-  // shared-memory bandwidth on the re-fetched weights.  MT M tiles share one weight fetch (TMEM: 2 x MT x Nt <= 512 columns;
-  // segmented mode keeps MT x Nt <= 128 running sums per thread in registers).  The items are dealt to 148 persistent
-  // CTAs, so a larger MT is taken only while it costs no wave efficiency.
+  // M tiles per work item: every item streams the WHOLE weight block of its (N tile, group) from L2, so at MT = 1 the
+  // L2 -> shared-memory bandwidth on the re-fetched weights bounds the kernel.  MT M tiles share one weight fetch (registers: MT x Nt <= 128).
+  // The items are dealt to MNB_NUM_SMS persistent CTAs, so a larger MT is taken only while it costs no wave efficiency.
   p.MT = 1;
   {
     auto wave_eff = [&](int mt) {
@@ -231,7 +228,7 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
       const int64_t ctas = std::max<int64_t>(1, MNB_NUM_SMS / p.ny);
       return (double)items / (double)(ceil_div((int)std::min<int64_t>(items, 1 << 30), (int)ctas) * ctas);
     };
-    const int cap = p.segmented ? std::max(1, 128 / p.Nt) : std::max(1, 256 / p.Nt);
+    const int cap = std::max(1, 128 / p.Nt);
     for (int mt = 2; mt <= std::min(4, cap); mt *= 2) {
       if (p.n_mtiles < mt) break;
       if ((int64_t)ceil_div(p.n_mtiles, mt) * p.n_ntiles * G * p.ny < 120) break;
@@ -240,7 +237,7 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   }
   if (const char* e = getenv("MNB_PK_MT")) {
     const int v = atoi(e);
-    if ((v == 1 || v == 2 || v == 4) && v * p.Nt <= (p.segmented ? 128 : 256)) p.MT = v;
+    if ((v == 1 || v == 2 || v == 4) && v * p.Nt <= 128) p.MT = v;
   }
   p.n_mgroups = ceil_div(p.n_mtiles, p.MT);
   p.n_items = p.n_mgroups * p.n_ntiles * G;
@@ -304,16 +301,15 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   p.stage_bytes = round_up(p.b_off + max_blk, 1024);
   // slack behind the last stage: MMAs of invalid halo rows read up to 128 + max tap offset rows past a plane start
   const int slack = round_up((128 + (hlo + hhi) * p.BW + halo_w + 8) * 16, 1024);
-  int nst = (kSmemBudget - slack) / p.stage_bytes;
+  const int stg = 32 * tc::kStageLd * 4;   // 128 x 32 epilogue staging tile behind the slack
+  int nst = (kSmemBudget - slack - stg) / p.stage_bytes;
   if (nst < 2) return unsupported("fewer than two pipeline stages fit");
   p.nstage = nst >= 8 ? 8 : (nst >= 4 ? 4 : 2);
   if (const char* e = getenv("MNB_PK_STAGES")) { const int v = atoi(e); if ((v == 2 || v == 4 || v == 8) && v <= nst) p.nstage = v; }
   p.st_log2 = p.nstage == 8 ? 3 : (p.nstage == 4 ? 2 : 1);
-  p.smem_bytes = p.nstage * p.stage_bytes + slack;
-  int cols = 32;
-  while (cols < 2 * p.MT * p.Nt) cols <<= 1;
-  if (cols > 512) return unsupported("accumulators exceed tensor memory");
-  p.tmem_cols = cols;
+  p.off_stg = p.nstage * p.stage_bytes + slack;
+  p.smem_bytes = p.off_stg + stg;
+  if (p.MT * p.Nt > 128) return unsupported("accumulators exceed the register budget");
   return 0;
 }
 
@@ -341,8 +337,7 @@ __global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__
     q = mnb_load_actq(qp);
     if (qp.mode == MNB_ACT_IAO && qp.zero_point) zp = __ldg(qp.zero_point);
   }
-  // grid = (chunks of the H*W plane, B * C8 planes): 32-bit index arithmetic only (the first version decoded a flat
-  // 64-bit index with five divisions per pixel and ran at 0.9 TB/s)
+  // grid = (chunks of the H*W plane, B * C8 planes): 32-bit index arithmetic only (no per-pixel divisions)
   const uint32_t HW = (uint32_t)H * (uint32_t)W;
   // block = (positions, planes): small images put several planes into one 256-thread block
   const uint32_t plane = blockIdx.y * blockDim.y + threadIdx.y;                 // b * C8 + c8
@@ -506,8 +501,7 @@ template <> struct PkVec<4> { typedef float4 type; };
 //   dx = gamma * invstd * (g * pass - dbeta / N - xhat * dgamma / N)            (training-mode BatchNorm, saturate STE)
 // One warp = 32 * VEC consecutive pixels of one channel octet (the conv's own channel order; g is read in the shuffled
 // order); a lane owns VEC consecutive pixels: 16-byte loads of g and x (VEC = 4), one word of pass bits per channel, VEC
-// consecutive 16-byte pixels per piece plane.  (First version: one pixel per thread, 4-byte loads with the g load predicated
-// on the bits load - 2.0 TB/s of its 12 B per element, 1.0 ms of the 6.6 ms headline step in the r2z launch list.)
+// consecutive 16-byte pixels per piece plane (one pixel per thread with 4-byte loads is far below HBM bandwidth).
 template <int VEC>
 __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __restrict__ g, const uint32_t* __restrict__ bits,
                                                                const float* __restrict__ x, int batch, int channels, int hw,
@@ -706,15 +700,13 @@ __global__ void __launch_bounds__(256) pack_weight_kernel(const __grid_constant_
 // the convolution kernel (forward and data gradient)
 // ---------------------------------------------------------------------------------------------------------
 struct ConvParams {
-  // private parameter block of the MMA-issue warp (uniform datapath: see mnb_conv_packed.cu for the rules)
+  // parameter block of the MMA warpgroups
   struct Mma {
     uint32_t n_items, chunks, ksteps, MT, Nt, npairs, st_mask, st_log2, stage16, a_mt16, a_term16, a_k16, b_off16,
-        b_tap16, b_k16, idesc, a_lbo, b_lbo, seg_len;
+        b_tap16, b_k16, a_lbo, b_lbo, seg_len;
     uint32_t ntmpl[MAXY];
-    // The MMA "program": one 32-bit word per (filter tap, piece pair) of a stage template = A offset | B offset << 16
-    // (16-byte units inside the stage); the issue loop is then  load word, two adds, MMA.  A single warp executes this
-    // loop serially, so every instruction in it costs MMA issue rate (measured: 45 uniform-datapath instructions per
-    // MMA = 420 cycles per MMA, tensor pipe 15 % busy).
+    // The MMA "program": one 32-bit word per (filter tap, piece pair, K-step) of a stage template = A offset | B offset << 16
+    // (16-byte units inside the stage); the issue loop is then  load word, two adds, MMA.
     uint16_t tmpl_begin[MAXY][MAXTMPL], tmpl_cnt[MAXY][MAXTMPL];   // in groups of four words
     alignas(16) uint4 prog4[MAXPROG / 4];                          // padded with 0xffffffff to whole groups
   } m;
@@ -725,9 +717,8 @@ struct ConvParams {
   int img_bytes[MAXY], y_off[MAXY];
   const uint8_t* w_img;
   // epilogue
-  int B, THH, BW, OHr, OWr, OH, OW, omul, ny, ng, Nt, NOUT, C8O, smem_bytes, tmem_cols, mode, zero_y[MAXY];
-  int nseg[MAXY];           // accumulation segments per work item (1 unless segmented)
-  int dbg;                  // MNB_PK_DEBUG (timing experiments only): 1 no epilogue stores, 2 no MMAs, 4 no TMEM loads
+  int B, THH, BW, OHr, OWr, OH, OW, omul, ny, ng, Nt, NOUT, C8O, smem_bytes, off_stg, mode;
+  int dbg;                  // MNB_PK_DEBUG (timing experiments only): 1 no epilogue stores, 2 no MMAs
   const float* n_scale;     // [NOUT] per-output-channel scale or NULL
   const float* a_scale;     // device scalar multiplied into n_scale, or NULL
   float a_scale_const;
@@ -744,32 +735,17 @@ struct ConvParams {
 };
 
 struct alignas(16) ConvShared {
-  uint64_t full[MAXST], empty[MAXST], acc_full[2], acc_empty[2];
-  uint32_t tmem_slot, abort;
+  uint64_t full[MAXST], empty[MAXST];
+  uint32_t abort;
   alignas(16) float epi_scale[256];
   alignas(16) float epi_bias[256];
 };
 
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-
 template <int NEPI>
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NEPI) : "memory"); }
 
-// Epilogue warps: one warp can only read the 32 TMEM lanes of its own quarter (warp % 4), and a lone warp per scheduler
-// issues its dependent tcgen05.ld -> fma -> st chains at ~0.3 instructions per cycle - ncu r3b: every forward / data-gradient
-// launch of the family sat at 42 - 47 k instructions per epilogue warp in 160 - 173 k cycles, tensor pipe 7 - 9 % busy, DRAM
-// 3.6 TB/s.  The un-segmented kernel therefore runs TWO warps per quarter (warps 4..7 take the even 16-column slots of an
-// item, warps 8..11 the odd ones); the segmented kernel keeps one (its 128 running sums per thread need the registers).
 // n = q * d + r for n < 2^22 through one float multiply (the compiler's 32-bit integer division is a ~25-instruction dependent
-// chain; the TMA-issuing lane ran ~2100 instructions per work item, most of them these, at one instruction every four cycles -
-// as long as a whole 3x3 g16 item takes: ncu r3b, source page).  q from the reciprocal is within +-1: corrected exactly.
+// chain, and the TMA-issuing lane decodes every work item with it).  q from the reciprocal is within +-1: corrected exactly.
 struct FastDiv {
   uint32_t d; float inv;
   __device__ __forceinline__ explicit FastDiv(int dd) : d((uint32_t)dd), inv(1.0f / (float)dd) {}
@@ -780,10 +756,15 @@ struct FastDiv {
   }
 };
 
-template <bool SEG> struct ConvCfg { static constexpr int EPIW = SEG ? 4 : 8, THREADS = 128 + 32 * EPIW; };
+constexpr int kConvThreads = 384;   // warp 0 TMA, warps 4..11 two MMA + epilogue warpgroups (warps 1..3 idle)
 
-template <bool SEG>   // SEG: segmented accumulation (split fp32 operands), the epilogue keeps the N tile in registers
-__global__ void __launch_bounds__(ConvCfg<SEG>::THREADS, 1)
+// Warpgroup wg issues the wgmma of GEMM rows 64*wg .. 64*wg+63 of every M tile of the item (accumulators in registers:
+// MT x NT / 2 per thread, plan: MT * Nt <= 128).  SEG: segmented accumulation (split fp32 operands): every segment of
+// at most seg_len stages starts from zero and is added into running sums with round-to-nearest fp32 adds.
+// Epilogue: 32 accumulator columns at a time through a 128 x 32 staging tile; thread et of the 256 then owns position
+// (et % 128) of the tile raster and one 16-column slot (et / 128) of the two.
+template <bool SEG, int NT>
+__global__ void __launch_bounds__(kConvThreads, 1)
 pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1,
                const __grid_constant__ CUtensorMap tmap2, const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -791,26 +772,17 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
-    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&sh.full[i], 1); tc::mbar_init(&sh.empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&sh.acc_full[i], 1); tc::mbar_init(&sh.acc_empty[i], 32 * ConvCfg<SEG>::EPIW); }
+    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&sh.full[i], 1); tc::mbar_init(&sh.empty[i], 8); }
     sh.abort = 0;
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tmap0);
     if (p.TA > 1) tc::prefetch_tmap(&tmap1);
     if (p.TA > 2) tc::prefetch_tmap(&tmap2);
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&sh.tmem_slot)),
-                 "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   // rows behind a box that only invalid accumulator rows read must at least be finite
-  for (int i = tid; i < p.smem_bytes / 16; i += ConvCfg<SEG>::THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < p.smem_bytes / 16; i += kConvThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = sh.tmem_slot;
 
   if (warp == 0) {
     // ================================================================= TMA producer
@@ -850,65 +822,12 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================================================= MMA issuer (warp-converged, lane 0 issues)
-
-    const uint32_t y = blockIdx.y;
-    const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), p.m.a_lbo, 128);
-    const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), p.m.b_lbo, 128) + (uint64_t)p.m.b_off16;
-    const uint32_t a_lo0 = (uint32_t)a_desc0, a_hi = (uint32_t)(a_desc0 >> 32), b_lo0 = (uint32_t)b_desc0, b_hi = (uint32_t)(b_desc0 >> 32);
-    uint32_t sc = 0, accq = 0;   // accq counts accumulator hand-offs (one per segment)
-    for (uint32_t it = blockIdx.x; it < p.m.n_items; it += gridDim.x) {
-      uint32_t started = 0, seg_pos = 0, open = 0;
-      for (uint32_t t = 0; t < p.m.ntmpl[y]; ++t) {
-        const uint32_t pb = p.m.tmpl_begin[y][t], pc = p.m.tmpl_cnt[y][t];
-        for (uint32_t cc = 0; cc < p.m.chunks; ++cc, ++sc) {
-          const uint32_t acc = accq & 1u, aph = (accq >> 1) & 1u;
-          if (!open) {   // first stage of a segment: the accumulator must have been drained
-            tc::mbar_wait_soft(&sh.acc_empty[acc], aph ^ 1u, p.err, 702, &sh.abort);
-            open = 1; started = 0;
-          }
-          const uint32_t slot = sc & p.m.st_mask, ph = (sc >> p.m.st_log2) & 1u;
-          tc::mbar_wait_soft(&sh.full[slot], ph, p.err, 703, &sh.abort);
-          tc::tc_fence_after();
-          const uint32_t s16 = slot * p.m.stage16;
-          for (uint32_t mt = 0; mt < p.m.MT; ++mt) {
-            const uint32_t d = tmem + (acc * p.m.MT + mt) * p.m.Nt;
-            const uint32_t a_base = a_lo0 + s16 + mt * p.m.a_mt16, b_base = b_lo0 + s16;
-            // flat program: one word per MMA of this stage template (tap x piece pair x K-step).  The first MMA of a
-            // segment overwrites the accumulator; the rest is a straight unrolled stream of independent
-            // load-word / add / add / MMA groups (a single warp issues them: dependent chains cost MMA rate)
-            if (!(p.dbg & 2)) {
-              tc::mma_f16_x4(d, a_base, a_hi, b_base, b_hi, p.m.idesc, p.m.prog4[pb], started);
-#pragma unroll 2
-              for (uint32_t e = 1; e < pc; ++e)
-                tc::mma_f16_x4(d, a_base, a_hi, b_base, b_hi, p.m.idesc, p.m.prog4[pb + e], 1u);
-            }
-          }
-          // MNB_PK_DEBUG bit 32 (with bit 2, timing experiments): plain mbarrier arrivals instead of tcgen05.commit
-          if (p.dbg & 32) { if (lane == 0) tc::mbar_arrive(&sh.empty[slot]); } else tc::mma_commit_elect(&sh.empty[slot]);
-          __syncwarp();
-          started = 1;
-          if (++seg_pos == p.m.seg_len) {   // segment complete: hand the accumulator to the epilogue
-            if (p.dbg & 32) { if (lane == 0) tc::mbar_arrive(&sh.acc_full[acc]); } else tc::mma_commit_elect(&sh.acc_full[acc]);
-            __syncwarp();
-            seg_pos = 0; open = 0; ++accq;
-          }
-        }
-      }
-      if (open || p.m.ntmpl[y] == 0) {      // last (partial) segment, or an output phase without any filter tap
-        const uint32_t acc = accq & 1u, aph = (accq >> 1) & 1u;
-        if (!open) tc::mbar_wait_soft(&sh.acc_empty[acc], aph ^ 1u, p.err, 702, &sh.abort);
-        if (p.dbg & 32) { if (lane == 0) tc::mbar_arrive(&sh.acc_full[acc]); } else tc::mma_commit_elect(&sh.acc_full[acc]);
-        __syncwarp();
-        ++accq;
-      }
-    }
   } else if (warp >= 4) {
-    // ================================================================= epilogue: TMEM -> scale/bias or STE -> fp32 NCHW
-    constexpr int NEPI = 32 * ConvCfg<SEG>::EPIW;
-    const int q = (warp - 4) & 3, half = (warp - 4) >> 2, et = tid - 128;   // TMEM lane quarter, slot parity (8 epilogue warps)
-    const int m = q * 32 + lane;                     // accumulator row = position of the zero-padded tile raster
+    // ================================================================= MMA warpgroups + epilogue
+    constexpr int NEPI = 256, NR = NT / 2, MAXMT = 128 / NT;
+    const int wg = (warp - 4) >> 2, et = tid - 128;
+    const int m = et & 127, half = et >> 7;          // epilogue: accumulator row (= tile raster position), slot parity
+    float* stage = reinterpret_cast<float*>(smem + p.off_stg);
     const int tb = m / (p.THH * p.BW);
     const int rem = m - tb * (p.THH * p.BW);
     const int th = rem / p.BW, wc = rem - th * p.BW;
@@ -922,7 +841,11 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
       pq = mnb_load_actq(p.post_q);
       if (p.post_q.mode == MNB_ACT_IAO && p.post_q.zero_point) pzp = __ldg(p.post_q.zero_point);
     }
-    uint32_t accq = 0;
+    const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), p.m.a_lbo, 128) + (uint64_t)(64 * wg);
+    const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), p.m.b_lbo, 128) + (uint64_t)p.m.b_off16;
+    const uint32_t a_lo0 = (uint32_t)a_desc0, b_lo0 = (uint32_t)b_desc0;
+    const uint64_t a_hi = a_desc0 & 0xffffffff00000000ull, b_hi = b_desc0 & 0xffffffff00000000ull;
+    uint32_t sc = 0;
     const FastDiv e_nt(p.n_ntiles), e_g(p.G), e_ct(p.col_tiles), e_rt(p.row_tiles);
     for (int it = blockIdx.x; it < p.n_items; it += gridDim.x) {
       uint32_t nt_u, r1_u, g_u, mg_u;
@@ -933,147 +856,181 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
       const int n_cnt = min(p.Nt, p.ng - nt * p.Nt);
       // per-channel constants of this N tile (the previous item's readers are done: barrier at the end of the loop body)
       for (int n = et; n < p.Nt; n += NEPI) {
-        float sc = 1.f, bs = 0.f;
+        float scv = 1.f, bs = 0.f;
         if (n < n_cnt) {
-          sc = p.n_scale ? __fmul_rn(a_sc, __ldg(p.n_scale + n_base + n)) : a_sc;
+          scv = p.n_scale ? __fmul_rn(a_sc, __ldg(p.n_scale + n_base + n)) : a_sc;
           if (p.bias) bs = __ldg(p.bias + n_base + n);
         }
-        sh.epi_scale[n] = sc; sh.epi_bias[n] = bs;
+        sh.epi_scale[n] = scv; sh.epi_bias[n] = bs;
       }
-      epi_bar_sync<NEPI>();
-      const int nseg = SEG ? p.nseg[y] : 1;
-      // running sums of the item's accumulator columns (segmented mode only: MT * Nt <= 128 -> 8 slots of 16 columns;
-      // slot = mt * (Nt / 16) + column chunk).  The slot loop is fully unrolled so that rs[][] stays in registers.
-      float rs[SEG ? 8 : 1][16];
-      const int nc16 = p.Nt >> 4, nslots = p.MT * nc16;
-      for (int seg = 0; seg < nseg; ++seg, ++accq) {
-        const uint32_t acc = accq & 1u, aph = (accq >> 1) & 1u;
-        if (!tc::mbar_wait(&sh.acc_full[acc], aph, p.err, 704)) goto done;
-        tc::tc_fence_after();
-        const bool last = seg == nseg - 1;
-        int mt_cur = -1;
-        bool valid = false;
-        float* orow = nullptr;
-        const uint8_t* brow = nullptr;
-        int64_t prow = 0;      // vector index of this thread's position in octet 0 of the consumer's operand plane
-        // one slot = 16 accumulator columns of one M tile.  Segmented kernels need rs[slot] with a compile-time index (8 slots,
-        // unrolled); the others run a ROLLED loop: unrolled 32 x, this body was 1 MB of SASS and the epilogue warps stalled
-        // on instruction fetch
-        auto do_slot = [&](const int slot, const int mt, const int c16, float (&rsl)[16]) {
-          const int n0 = c16 * 16;
-          if (mt != mt_cur) {   // output row of this thread in M tile mt
-            mt_cur = mt;
-            const int tile = mg * p.MT + mt;
-            uint32_t ct_u, r2_u, rt_u, bt_u;
-            e_ct.divmod((uint32_t)tile, r2_u, ct_u);
-            e_rt.divmod(r2_u, bt_u, rt_u);
-            const int ct = (int)ct_u, rt = (int)rt_u, bt = (int)bt_u;
-            const int b = bt * p.TB + tb, i = rt * p.TH + th, j = ct * p.Wt + wc;
-            valid = row_ok && tile < p.n_mtiles && b < p.B && i < p.OHr && j < p.OWr;
-            const int oh = i * p.omul + ya, ow = j * p.omul + yb;
-            orow = p.out ? p.out + ((int64_t)b * p.NOUT + n_base) * plane + (int64_t)oh * p.OW + ow : nullptr;
-            brow = p.bits8 ? p.bits8 + (int64_t)b * p.C8O * plane + (int64_t)oh * p.OW + ow : nullptr;
-            if (!SEG && p.post_out) {
-              if (p.post_split)   // octet index (h%2 * 2 + w%2) * C8 + c/8 of a [.., OH/2, OW/2] plane
-                prow = (((int64_t)b * 4 * p.C8O + ((oh & 1) * 2 + (ow & 1)) * p.C8O) * (p.OH >> 1) + (oh >> 1)) * (p.OW >> 1) + (ow >> 1);
-              else
-                prow = ((int64_t)b * p.C8O * p.OH + oh) * p.OW + ow;
+      // ---- MMAs of the item: every stage of every template, all M tiles
+      float acc[MAXMT][NR];
+      float rs[SEG ? MAXMT : 1][SEG ? NR : 1];
+#pragma unroll
+      for (int mt = 0; mt < MAXMT; ++mt) tc::zero_acc(acc[mt]);
+      if (SEG) {
+#pragma unroll
+        for (int mt = 0; mt < MAXMT; ++mt) tc::zero_acc(rs[mt]);
+      }
+      uint32_t seg_pos = 0;
+      for (uint32_t t = 0; t < p.m.ntmpl[y]; ++t) {
+        const uint32_t pb = p.m.tmpl_begin[y][t], pc = p.m.tmpl_cnt[y][t];
+        for (uint32_t cc = 0; cc < p.m.chunks; ++cc, ++sc) {
+          const uint32_t slot = sc & p.m.st_mask, ph = (sc >> p.m.st_log2) & 1u;
+          tc::mbar_wait_soft(&sh.full[slot], ph, p.err, 703, &sh.abort);
+          const uint32_t s16 = slot * p.m.stage16;
+          tc::wg_fence();
+#pragma unroll
+          for (int mt = 0; mt < MAXMT; ++mt) tc::fence_acc(acc[mt]);
+          if (!(p.dbg & 2)) {
+#pragma unroll
+            for (int mt = 0; mt < MAXMT; ++mt) {
+              if (mt >= (int)p.m.MT) break;
+              const uint32_t a_base = a_lo0 + s16 + (uint32_t)mt * p.m.a_mt16, b_base = b_lo0 + s16;
+              // flat program: one word per MMA of this stage template (tap x piece pair x K-step) = A offset | B offset << 16,
+              // padded with 0xffffffff to groups of four
+              for (uint32_t e = 0; e < pc; ++e) {
+                const uint4 w4 = p.m.prog4[pb + e];
+                const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                  if (w[k] == 0xffffffffu) continue;
+                  tc::Mma<NT>::template bf16<0, 0>(acc[mt], a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
+                                                    b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
+                }
+              }
             }
           }
-          uint32_t r[16];
-          if (!p.zero_y[y] && !(p.dbg & 4)) {
-            tmem_ld_32x16(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)((acc * p.MT + mt) * p.Nt + n0), r);
-            tc::tmem_ld_wait();
-          } else {
+          tc::wg_commit();
+          tc::wg_wait<0>();
 #pragma unroll
-            for (int k = 0; k < 16; ++k) r[k] = 0u;
-          }
-          if (SEG) {   // accumulate the segment (round-to-nearest fp32 adds), write only after the last one
+          for (int mt = 0; mt < MAXMT; ++mt) tc::fence_acc(acc[mt]);
+          __syncwarp();
+          if (lane == 0) tc::mbar_arrive(&sh.empty[slot]);   // this warp's reads of the stage are done
+          if (SEG && ++seg_pos == p.m.seg_len) {            // segment complete: into the running sums
+            seg_pos = 0;
 #pragma unroll
-            for (int k = 0; k < 16; ++k) {
-              const float v = seg == 0 ? __uint_as_float(r[k]) : __fadd_rn(rsl[k], __uint_as_float(r[k]));
-              rsl[k] = v;
-              r[k] = __float_as_uint(v);
+            for (int mt = 0; mt < MAXMT; ++mt) {
+#pragma unroll
+              for (int i = 0; i < NR; ++i) { rs[SEG ? mt : 0][SEG ? i : 0] = __fadd_rn(rs[SEG ? mt : 0][SEG ? i : 0], acc[mt][i]); acc[mt][i] = 0.f; }
             }
-            if (!last) return;
           }
-          if (!valid || n0 >= n_cnt || (p.dbg & 1)) return;
-          float sc[16], bs[16];
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const float4 a = *reinterpret_cast<const float4*>(&sh.epi_scale[n0 + 4 * v]);
-            const float4 c = *reinterpret_cast<const float4*>(&sh.epi_bias[n0 + 4 * v]);
-            sc[4 * v] = a.x; sc[4 * v + 1] = a.y; sc[4 * v + 2] = a.z; sc[4 * v + 3] = a.w;
-            bs[4 * v] = c.x; bs[4 * v + 1] = c.y; bs[4 * v + 2] = c.z; bs[4 * v + 3] = c.w;
-          }
-          float* op = orow + (int64_t)n0 * plane;
-          if (!SEG && p.post_out) {
-            // forward conv of a frozen inference graph: y = acc * scale + bias [-> ReLU] -> consumer's quantizer -> bf16 levels
-            float lev[16], yv[16];
-#pragma unroll
-            for (int k = 0; k < 16; ++k) {
-              const float v = fmaf(__uint_as_float(r[k]), sc[k], bs[k]);
-              if (orow && n0 + k < n_cnt) op[(int64_t)k * plane] = v;
-              yv[k] = p.post_relu ? fmaxf(v, 0.f) : v;
-            }
-            uint32_t passbits;
-            mnb_act_levels<16>(pq, yv, lev, passbits);
-#pragma unroll
-            for (int k = 0; k < 16; ++k) lev[k] = n0 + k < n_cnt ? lev[k] + pzp : 0.f;
-            const int64_t oct_stride = p.post_split ? (int64_t)(p.OH >> 1) * (p.OW >> 1) : plane;
-            const int oc8 = (n_base + n0) >> 3;
-            uint4* dst = p.post_out + prow + (int64_t)oc8 * oct_stride;
-            dst[0] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]), pack2(lev[6], lev[7]));
-            if (n0 + 8 < n_cnt)
-              dst[oct_stride] = make_uint4(pack2(lev[8], lev[9]), pack2(lev[10], lev[11]), pack2(lev[12], lev[13]), pack2(lev[14], lev[15]));
-          } else if (p.mode == 0 || !brow) {
-#pragma unroll
-            for (int k = 0; k < 16; ++k, op += plane)
-              if (n0 + k < n_cnt) *op = fmaf(__uint_as_float(r[k]), sc[k], bs[k]);
-          } else {
-            // STE of the activation quantizer that fed the forward conv: the reference computes ((g*s)*pass)/s (IAO) or
-            // (((g*s)/s)*pass)*0.1 (DoReFa); (g*s)/s is g to within one ulp, so g itself is passed
-            const int oc0 = (n_base + n0) >> 3;     // n_base + n0 is a multiple of 8 (checked on the host)
-            const uint32_t m0 = __ldg(brow + (int64_t)oc0 * plane);
-            const uint32_t m1 = (n0 + 8 < n_cnt) ? __ldg(brow + (int64_t)(oc0 + 1) * plane) : 0u;
-            const uint32_t mask = m0 | (m1 << 8);
-#pragma unroll
-            for (int k = 0; k < 16; ++k, op += plane)
-              if (n0 + k < n_cnt) *op = ((mask >> k) & 1u) ? __uint_as_float(r[k]) * p.gain : 0.f;
-          }
-                };
-        if (SEG) {
-          int mt = 0, c16 = 0;
-#pragma unroll
-          for (int slot = 0; slot < 8; ++slot) {
-            if (slot < nslots) do_slot(slot, mt, c16, rs[SEG ? slot : 0]);
-            if (++c16 == nc16) { c16 = 0; ++mt; }
-          }
-        } else {
-#pragma unroll 1
-          for (int mt = 0, slot = 0; mt < p.MT; ++mt)
-#pragma unroll 1
-            for (int c16 = 0; c16 < nc16; ++c16, ++slot)
-              if (ConvCfg<SEG>::EPIW == 4 || (slot & 1) == half) do_slot(slot, mt, c16, rs[0]);
         }
-        tc::tc_fence_before();
-        tc::mbar_arrive(&sh.acc_empty[acc]);
       }
-      epi_bar_sync<NEPI>();   // everyone is done with epi_scale / epi_bias of this item
+      if (SEG) {   // the last (partial) segment
+#pragma unroll
+        for (int mt = 0; mt < MAXMT; ++mt) {
+#pragma unroll
+          for (int i = 0; i < NR; ++i) rs[SEG ? mt : 0][SEG ? i : 0] = __fadd_rn(rs[SEG ? mt : 0][SEG ? i : 0], acc[mt][i]);
+        }
+      }
+      // ---- epilogue
+      int mt_cur = -1;
+      bool valid = false;
+      float* orow = nullptr;
+      const uint8_t* brow = nullptr;
+      int64_t prow = 0;      // vector index of this thread's position in octet 0 of the consumer's operand plane
+      // one slot = 16 accumulator columns of one M tile
+      auto do_slot = [&](const int mt, const int c16, const float (&r)[16]) {
+        const int n0 = c16 * 16;
+        if (mt != mt_cur) {   // output row of this thread in M tile mt
+          mt_cur = mt;
+          const int tile = mg * p.MT + mt;
+          uint32_t ct_u, r2_u, rt_u, bt_u;
+          e_ct.divmod((uint32_t)tile, r2_u, ct_u);
+          e_rt.divmod(r2_u, bt_u, rt_u);
+          const int ct = (int)ct_u, rt = (int)rt_u, bt = (int)bt_u;
+          const int b = bt * p.TB + tb, i = rt * p.TH + th, j = ct * p.Wt + wc;
+          valid = row_ok && tile < p.n_mtiles && b < p.B && i < p.OHr && j < p.OWr;
+          const int oh = i * p.omul + ya, ow = j * p.omul + yb;
+          orow = p.out ? p.out + ((int64_t)b * p.NOUT + n_base) * plane + (int64_t)oh * p.OW + ow : nullptr;
+          brow = p.bits8 ? p.bits8 + (int64_t)b * p.C8O * plane + (int64_t)oh * p.OW + ow : nullptr;
+          if (p.post_out) {
+            if (p.post_split)   // octet index (h%2 * 2 + w%2) * C8 + c/8 of a [.., OH/2, OW/2] plane
+              prow = (((int64_t)b * 4 * p.C8O + ((oh & 1) * 2 + (ow & 1)) * p.C8O) * (p.OH >> 1) + (oh >> 1)) * (p.OW >> 1) + (ow >> 1);
+            else
+              prow = ((int64_t)b * p.C8O * p.OH + oh) * p.OW + ow;
+          }
+        }
+        if (!valid || n0 >= n_cnt || (p.dbg & 1)) return;
+        float sc[16], bs[16];
+#pragma unroll
+        for (int v = 0; v < 4; ++v) {
+          const float4 a = *reinterpret_cast<const float4*>(&sh.epi_scale[n0 + 4 * v]);
+          const float4 c = *reinterpret_cast<const float4*>(&sh.epi_bias[n0 + 4 * v]);
+          sc[4 * v] = a.x; sc[4 * v + 1] = a.y; sc[4 * v + 2] = a.z; sc[4 * v + 3] = a.w;
+          bs[4 * v] = c.x; bs[4 * v + 1] = c.y; bs[4 * v + 2] = c.z; bs[4 * v + 3] = c.w;
+        }
+        float* op = orow + (int64_t)n0 * plane;
+        if (!SEG && p.post_out) {
+          // forward conv of a frozen inference graph: y = acc * scale + bias [-> ReLU] -> consumer's quantizer -> bf16 levels
+          float lev[16], yv[16];
+#pragma unroll
+          for (int k = 0; k < 16; ++k) {
+            const float v = fmaf(r[k], sc[k], bs[k]);
+            if (orow && n0 + k < n_cnt) op[(int64_t)k * plane] = v;
+            yv[k] = p.post_relu ? fmaxf(v, 0.f) : v;
+          }
+          uint32_t passbits;
+          mnb_act_levels<16>(pq, yv, lev, passbits);
+#pragma unroll
+          for (int k = 0; k < 16; ++k) lev[k] = n0 + k < n_cnt ? lev[k] + pzp : 0.f;
+          const int64_t oct_stride = p.post_split ? (int64_t)(p.OH >> 1) * (p.OW >> 1) : plane;
+          const int oc8 = (n_base + n0) >> 3;
+          uint4* dst = p.post_out + prow + (int64_t)oc8 * oct_stride;
+          dst[0] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]), pack2(lev[6], lev[7]));
+          if (n0 + 8 < n_cnt)
+            dst[oct_stride] = make_uint4(pack2(lev[8], lev[9]), pack2(lev[10], lev[11]), pack2(lev[12], lev[13]), pack2(lev[14], lev[15]));
+        } else if (p.mode == 0 || !brow) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k, op += plane)
+            if (n0 + k < n_cnt) *op = fmaf(r[k], sc[k], bs[k]);
+        } else {
+          // STE of the activation quantizer that fed the forward conv: the reference computes ((g*s)*pass)/s (IAO) or
+          // (((g*s)/s)*pass)*0.1 (DoReFa); (g*s)/s is g to within one ulp, so g itself is passed
+          const int oc0 = (n_base + n0) >> 3;     // n_base + n0 is a multiple of 8 (checked on the host)
+          const uint32_t m0 = __ldg(brow + (int64_t)oc0 * plane);
+          const uint32_t m1 = (n0 + 8 < n_cnt) ? __ldg(brow + (int64_t)(oc0 + 1) * plane) : 0u;
+          const uint32_t mask = m0 | (m1 << 8);
+#pragma unroll
+          for (int k = 0; k < 16; ++k, op += plane)
+            if (n0 + k < n_cnt) *op = ((mask >> k) & 1u) ? r[k] * p.gain : 0.f;
+        }
+      };
+      // columns of the item in M-tile-major order: L = mt * NT + n; round rnd stages L in [32 rnd, 32 rnd + 32)
+      const int ncols = (int)p.m.MT * NT;
+#pragma unroll
+      for (int rnd = 0; rnd < (MAXMT * NT + 31) / 32; ++rnd) {
+        if (32 * rnd >= ncols) break;
+        epi_bar_sync<NEPI>();   // every thread is done with the previous staging tile (and, first round, epi_scale is written)
+#pragma unroll
+        for (int mt = 0; mt < MAXMT; ++mt) {
+          const int lo = mt * NT > 32 * rnd ? mt * NT : 32 * rnd;
+          const int hi = (mt + 1) * NT < 32 * rnd + 32 ? (mt + 1) * NT : 32 * rnd + 32;
+          if (lo >= hi) continue;
+          float* dst = stage + (lo - 32 * rnd) * tc::kStageLd;
+          if constexpr (SEG) tc::frag_cols_to_smem(rs[mt], dst, tc::kStageLd, 64 * wg, lo - mt * NT, hi - lo);
+          else tc::frag_cols_to_smem(acc[mt], dst, tc::kStageLd, 64 * wg, lo - mt * NT, hi - lo);
+        }
+        epi_bar_sync<NEPI>();
+        const int L0 = 32 * rnd + 16 * half;
+        if (L0 < ncols) {
+          float r[16];
+#pragma unroll
+          for (int k = 0; k < 16; ++k) r[k] = stage[(16 * half + k) * tc::kStageLd + m];
+          do_slot(L0 / NT, (L0 % NT) >> 4, r);
+        }
+      }
+      epi_bar_sync<NEPI>();   // everyone is done with epi_scale / epi_bias and the staging tile of this item
     }
   }
 done:
-  tc::tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc::tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols));
-  }
 }
 
-// Map over term plane `t` of a packed tensor [b][octet][h][w][8 x bf16].  The TMA unit's cost is per box ROW (~12 cycles
-// per row and SM whatever its length: with the 16-byte channel octet as innermost dimension a 170-position x 16-channel
-// box took 4000 cycles), so the 16-byte pixels of one image row are declared as ONE dimension of 8-byte elements:
+// Map over term plane `t` of a packed tensor [b][octet][h][w][8 x bf16].  The TMA unit's cost is per box ROW whatever
+// its length (with the 16-byte channel octet as innermost dimension every position would be a row), so the 16-byte pixels
+// of one image row are declared as ONE dimension of 8-byte elements:
 // dims (2*W, H, B, octets), box (2*BW, rows, images, octets) - same shared-memory image [octet][image][row][col][16 B],
 // halo columns still zero-filled (start coordinate -2*wlo: a multiple of 16 bytes).
 static int make_pk_tmap(CUtensorMap* m, const void* base, int64_t plane_bytes, int t, int B, int C8tot, int H, int W,
@@ -1114,7 +1071,7 @@ struct WgPlan {
   int TA, TX, npairs, pair_a[MAXPAIR], pair_b[MAXPAIR];
   int tap_kph[MAXTAP], tap_off[MAXTAP];   // per tap: k-phase plane and start-row offset in the x block
   int kph_used[4], nkph_used, kph_slot[4];
-  int dy_box_bytes, x_box_bytes, dy_bytes, x_bytes, sub_bytes, stage_bytes, nstage, st_log2, smem_bytes, tmem_cols;
+  int dy_box_bytes, x_box_bytes, dy_bytes, x_bytes, sub_bytes, stage_bytes, nstage, st_log2, smem_bytes;
   int64_t partial_floats;
 };
 
@@ -1135,10 +1092,10 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
   p.cin_g = C / G; p.cout_g = K / G;
   if (G > 1 && ((p.cin_g % 8) || (p.cout_g % 8))) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: grouped conv needs channels per group % 8 == 0");
   // Small groups are MERGED: gm neighbouring groups form one 128-row accumulator block (rows = their output channels,
-  // columns = their input channels); an MMA costs 61 cycles whether it is 128 x 16 or 128 x 64, so computing the discarded
-  // off-diagonal blocks is free and the MMA count drops by gm.  The reduction kernel keeps the diagonal blocks only.
+  // columns = their input channels); a narrow MMA uses the tensor core poorly, so computing the discarded off-diagonal
+  // blocks costs little and the MMA count drops by gm.  The reduction kernel keeps the diagonal blocks only.
   p.gm = 1;
-  while (G % (p.gm * 2) == 0 && p.gm * 2 * p.cout_g <= 128 && p.gm * 2 * p.cin_g <= 256) p.gm *= 2;
+  while (G % (p.gm * 2) == 0 && p.gm * 2 * p.cout_g <= 128 && p.gm * 2 * p.cin_g <= 128) p.gm *= 2;
   if (const char* e = getenv("MNB_PK_WG_MERGE")) { if (atoi(e) == 0) p.gm = 1; }
   p.G = G / p.gm; p.cin_g *= p.gm; p.cout_g *= p.gm;
   p.K8 = ceil_div(K, 8); p.C8X = ceil_div(C, 8);
@@ -1162,24 +1119,19 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
   // raster: rows of BW >= Q + halo columns; TH * BW must be a multiple of 16 (MMA K-steps of 16 positions)
   const int need = p.Q + wlo + whi;
   if (need > 128) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: row wider than 128 positions");
-  // N tile over input channels and TAP GROUPS: one CTA accumulates tpg taps x Nc columns (<= 512 TMEM columns).  An MMA of
-  // N <= 64 costs the same 61 cycles as one of N = 128, so the N tile is made as wide as the layer allows (up to 256) and
-  // the taps are split over CTAs instead (each tap group re-reads the operands, mostly from L2): the MMA count is
-  // positions/16 x taps x pairs x ceil(C / Nc) - with Nc = 48 a 256-channel 3x3 layer issued six N = 48 MMAs where two
-  // tap groups of N = 256 do the same work at full tensor rate.
+  // N tile over input channels and TAP GROUPS: one CTA accumulates tpg taps x Nc columns (tpg x Nc <= 128: registers).
+  // Wide MMAs use the tensor core best, so the N tile is made as wide as the layer allows (up to 128) and the taps are split
+  // over CTAs instead (each tap group re-reads the operands, mostly from L2).
   int nc = std::min(nc_cap, round_up(p.cin_g, 16));
   if (const char* e = getenv("MNB_PK_WG_NC")) nc = std::max(16, std::min(nc, atoi(e) / 16 * 16));
   p.n_ctiles = ceil_div(p.cin_g, nc);
   p.Nc = round_up(ceil_div(p.cin_g, p.n_ctiles), 16);      // balance the tiles
   p.n_ctiles = ceil_div(p.cin_g, p.Nc);
   p.n_ktiles = ceil_div(p.cout_g, 128);
-  p.tpg = std::max(1, std::min(p.ntap, 512 / p.Nc));
+  p.tpg = std::max(1, std::min(p.ntap, 128 / p.Nc));       // accumulators: tpg x Nc / 2 registers per thread
   p.n_tg = ceil_div(p.ntap, p.tpg);
   p.tpg = ceil_div(p.ntap, p.n_tg);                        // balance the groups
-  int cols = 32;
-  while (cols < p.tpg * p.Nc) cols <<= 1;
-  if (cols > 512) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: accumulators exceed tensor memory");
-  p.tmem_cols = cols;
+  if (p.tpg * p.Nc > 128) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: accumulators exceed the register budget");
   // stage = NI sub-blocks (one image row-tile each): dy [TA][16 octets][rows_dy], x [TX][k-phase][Nc/8][rows_x].
   // Pick the raster (BW, TH) with the best useful fraction whose sub-block fits four times (else twice).
   auto sub_bytes_of = [&](int bw, int th) {
@@ -1222,8 +1174,8 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
   p.nstg_total = ceil_div(p.nsub, p.NI);
   const int n_kc = p.n_ktiles * p.n_ctiles * p.G * p.n_tg;
   p.splits = std::max(1, std::min(p.nstg_total, std::max(1, MNB_NUM_SMS / n_kc)));
-  // keep accumulation chains short: tcgen05.mma truncates the running fp32 sum after every instruction (a bias of
-  // ~2e-8 of |D| per MMA), so one accumulator takes <= ~192 MMAs; the partial sums are added with RN adds
+  // keep accumulation chains short (the tensor core does not round the running fp32 sum to nearest after every
+  // instruction): one accumulator takes <= ~256 MMAs; the partial sums are added with RN adds
   const int chain_per_stage = p.NI * (p.rows_dy / 16) * p.npairs;
   int chain_max = 256;
   if (const char* e = getenv("MNB_PK_WG_CHAIN")) chain_max = std::max(1, atoi(e));
@@ -1238,7 +1190,7 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
 // several times larger than one plane of integer levels)
 static int make_wg_plan(const mnb_conv_shape* s, int TA, int TX, WgPlan& p) {
   int rc = MNB_E_UNSUPPORTED;
-  for (int cap = 256; cap >= 16; cap /= 2) {
+  for (int cap = 128; cap >= 16; cap /= 2) {
     rc = make_wg_plan_nc(s, TA, TX, p, cap);
     if (rc != MNB_E_UNSUPPORTED) return rc;
   }
@@ -1248,26 +1200,31 @@ static int make_wg_plan(const mnb_conv_shape* s, int TA, int TX, WgPlan& p) {
 struct WgParams {
   struct Mma {
     uint32_t stg_per_split, nstg_total, NI, ksteps, ntap, tpg, n_tg, Nc, npairs, st_mask, st_log2, stage16, sub16, dy_term16, x_off16,
-        x_term16, x_kph16, idesc, dy_sbo, x_sbo, nsub;
+        x_term16, x_kph16, dy_sbo, x_sbo, nsub;
     uint32_t pair_a16[MAXPAIR], pair_b16[MAXPAIR];   // piece-plane offsets of the pairs (16-byte units)
-    // per (piece pair, tap group of this CTA, four taps): x-operand offsets = pair plane + k-phase slot + tap row offset,
-    // 0xffffffff behind the last tap of a group (one 128-bit constant load and one election per four MMAs)
+    // per (piece pair, tap group, tap): x-operand offsets = pair plane + k-phase slot + tap row offset, in groups of four
+    // (0xffffffff behind the last tap of a group)
     alignas(16) uint4 progb4[MAXPAIR * MAXTAP / 4 + MAXPAIR * 16];
     uint32_t g4;                        // uint4 entries per (pair, tap group) = ceil(tpg / 4)
   } m;
   int G, n_ktiles, n_ctiles, n_tg, tpg, splits, stg_per_split, nstg_total, NI, nsub, row_tiles, TA, TX, nkph_used, kph_used[4];
   int K8, C8X, cout_g8, cin_g8, Nc8, TH, hlo, wlo, stage_bytes, sub_bytes, dy_bytes, x_bytes, dy_box_bytes, x_box_bytes,
-      st_mask, st_log2, smem_bytes, tmem_cols, ntap, Nc, cout_g, cin_g;
+      st_mask, st_log2, smem_bytes, ntap, Nc, cout_g, cin_g;
   float* partial;
   int* err;
 };
 
 struct alignas(16) WgShared {
-  uint64_t full[MAXST], empty[MAXST], acc_full;
-  uint32_t tmem_slot, abort;
+  uint64_t full[MAXST], empty[MAXST];
+  uint32_t abort;
 };
 
-__global__ void __launch_bounds__(NTHREADS, 1)
+constexpr int kWgThreads = 384;   // warp 0 TMA, warps 4..11 two MMA warpgroups (warps 1..3 idle)
+
+// Warpgroup wg accumulates gradient channels (GEMM rows) 64*wg .. 64*wg+63 of the k tile for every tap of the CTA's tap
+// group: tpg x NC / 2 registers per thread (plan: tpg * Nc <= 128).
+template <int NC>
+__global__ void __launch_bounds__(kWgThreads, 1)
 pk_wgrad_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_constant__ CUtensorMap dy1,
                 const __grid_constant__ CUtensorMap dy2, const __grid_constant__ CUtensorMap x0,
                 const __grid_constant__ CUtensorMap x1, const __grid_constant__ CUtensorMap x2,
@@ -1276,25 +1233,16 @@ pk_wgrad_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_constant__
   __shared__ WgShared sh;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
-    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&sh.full[i], 1); tc::mbar_init(&sh.empty[i], 1); }
-    tc::mbar_init(&sh.acc_full, 1);
+    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&sh.full[i], 1); tc::mbar_init(&sh.empty[i], 8); }
     sh.abort = 0;
     tc::fence_barrier_init();
     tc::prefetch_tmap(&dy0); tc::prefetch_tmap(&x0);
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&sh.tmem_slot)),
-                 "r"((uint32_t)p.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   // every row an MMA can read must be finite (positions are the reduction dimension here): zero everything once,
   // the TMA boxes never touch the slack rows
-  for (int i = tid; i < p.smem_bytes / 16; i += NTHREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < p.smem_bytes / 16; i += kWgThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = sh.tmem_slot;
   // work item of this CTA: blockIdx.x = (((g * n_ktiles + kt) * n_ctiles + ct) * n_tg + tap group), blockIdx.y = split
   const int split = blockIdx.y;
   const int tg = blockIdx.x % p.n_tg;
@@ -1333,66 +1281,65 @@ pk_wgrad_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_constant__
         // sub-blocks of a short last stage keep their previous (finite) contents; the MMA loop skips them
       }
     }
-  } else if (warp == 1) {
-
-    const uint64_t a_desc0 = tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.m.dy_sbo);
+  } else if (warp >= 4) {
+    constexpr int NR = NC / 2, MAXTPG = 128 / NC;
+    const int wg = (warp - 4) >> 2;
+    const uint64_t a_desc0 = tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.m.dy_sbo) + (uint64_t)((8u * wg * p.m.dy_sbo) >> 4);
     const uint64_t b_desc0 = tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.m.x_sbo) + (uint64_t)p.m.x_off16;
-    const uint32_t a_lo0 = (uint32_t)a_desc0, a_hi = (uint32_t)(a_desc0 >> 32), b_lo0 = (uint32_t)b_desc0, b_hi = (uint32_t)(b_desc0 >> 32);
-    const uint32_t split_u = blockIdx.y;
+    const uint32_t a_lo0 = (uint32_t)a_desc0, b_lo0 = (uint32_t)b_desc0;
+    const uint64_t a_hi = a_desc0 & 0xffffffff00000000ull, b_hi = b_desc0 & 0xffffffff00000000ull;
+    const uint32_t* prog = reinterpret_cast<const uint32_t*>(p.m.progb4);
     const uint32_t tgm = blockIdx.x % p.m.n_tg;
-    const uint32_t t0m = tgm * p.m.tpg, tnm = min(p.m.tpg, p.m.ntap - t0m);
-    const uint32_t s0 = split_u * p.m.stg_per_split;
-    const uint32_t s1 = min(p.m.nstg_total, s0 + p.m.stg_per_split);
-    uint32_t sc = 0, accf = 0;
-    for (uint32_t stg = s0; stg < s1; ++stg, ++sc) {
+    const uint32_t tnm = min(p.m.tpg, p.m.ntap - tgm * p.m.tpg);
+    float acc[MAXTPG][NR];
+#pragma unroll
+    for (int t = 0; t < MAXTPG; ++t) tc::zero_acc(acc[t]);
+    uint32_t sc = 0;
+    for (int stg = stg0; stg < stg1; ++stg, ++sc) {
       const uint32_t slot = sc & p.m.st_mask, ph = (sc >> p.m.st_log2) & 1u;
       tc::mbar_wait_soft(&sh.full[slot], ph, p.err, 712, &sh.abort);
-      tc::tc_fence_after();
-      const uint32_t nsubs = min(p.m.NI, p.m.nsub - stg * p.m.NI);
+      const uint32_t nsubs = min(p.m.NI, p.m.nsub - (uint32_t)stg * p.m.NI);
+      tc::wg_fence();
+#pragma unroll
+      for (int t = 0; t < MAXTPG; ++t) tc::fence_acc(acc[t]);
       for (uint32_t si = 0; si < nsubs; ++si) {
         const uint32_t s16 = slot * p.m.stage16 + si * p.m.sub16;
         uint32_t arow = a_lo0 + s16, brow = b_lo0 + s16;
         for (uint32_t j = 0; j < p.m.ksteps; ++j, arow += 16u, brow += 16u) {
           for (uint32_t pr = 0; pr < p.m.npairs; ++pr) {
-            const uint32_t ad = arow + p.m.pair_a16[pr];
-            uint32_t d = tmem, e = (pr * p.m.n_tg + tgm) * p.m.g4;
-#pragma unroll 2
-            for (uint32_t t = 0; t < tnm; t += 4u, ++e, d += 4u * p.m.Nc)
-              tc::mma_f16_x4_taps(d, p.m.Nc, ad, a_hi, brow, b_hi, p.m.idesc, p.m.progb4[e], accf);
-            accf = 1u;   // every tap accumulator has been written once: accumulate from here on
+            const uint64_t ad = a_hi | (uint64_t)(arow + p.m.pair_a16[pr]);
+            const uint32_t* pw = prog + (size_t)(pr * p.m.n_tg + tgm) * p.m.g4 * 4;
+#pragma unroll
+            for (int t = 0; t < MAXTPG; ++t) {
+              if (t >= (int)tnm) break;
+              tc::Mma<NC>::template bf16<1, 1>(acc[t], ad, b_hi | (uint64_t)(brow + pw[t]), 1);
+            }
           }
         }
       }
-      tc::mma_commit_elect(&sh.empty[slot]);
-      __syncwarp();
-    }
-    tc::mma_commit_elect(&sh.acc_full);
-    __syncwarp();
-  } else if (warp >= 4) {
-    // partial[split][g][kt][ct][tap][c][k]: lanes = k -> coalesced
-    const int q = warp - 4;
-    const int kl = q * 32 + lane;
-    if (!tc::mbar_wait(&sh.acc_full, 0, p.err, 713)) goto done;
-    tc::tc_fence_after();
-    float* dst = p.partial + ((((int64_t)split * p.G + g) * p.n_ktiles + kt) * p.n_ctiles + ct) * (int64_t)(p.ntap * p.Nc * 128) +
-                 (int64_t)t0 * p.Nc * 128 + kl;
-    const bool any = stg1 > stg0;
-    for (int col = 0; col < tn * p.Nc; col += 16) {
-      uint32_t r[16];
-      tmem_ld_32x16(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)col, r);
-      tc::tmem_ld_wait();
+      tc::wg_commit();
+      tc::wg_wait<0>();
 #pragma unroll
-      for (int k = 0; k < 16; ++k) dst[(int64_t)(col + k) * 128] = any ? __uint_as_float(r[k]) : 0.f;
+      for (int t = 0; t < MAXTPG; ++t) tc::fence_acc(acc[t]);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&sh.empty[slot]);
     }
-    tc::tc_fence_before();
+    // partial[split][g][kt][ct][tap][c][k]: straight from the fragment (row = k, column = c)
+    float* dst = p.partial + ((((int64_t)split * p.G + g) * p.n_ktiles + kt) * p.n_ctiles + ct) * (int64_t)(p.ntap * p.Nc * 128) +
+                 (int64_t)t0 * p.Nc * 128;
+    const int fr = 64 * wg + 16 * ((warp - 4) & 3) + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+    for (int t = 0; t < MAXTPG; ++t) {
+      if (t >= tn) break;
+#pragma unroll
+      for (int j = 0; j < NR / 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          dst[(int64_t)(t * p.Nc + 8 * j + fc + (e & 1)) * 128 + fr + 8 * (e >> 1)] = acc[t][4 * j + e];
+    }
   }
 done:
-  tc::tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc::tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols));
-  }
 }
 
 // dw[k][c][tap] = mul(k) * sum over splits (fixed order: deterministic); mul = a_scale / kdiv[k] (either may be NULL).
@@ -1572,14 +1519,14 @@ extern "C" int mnb_bn_relu_quant_pack_fwd(const float* x, int32_t batch, int32_t
   return 0;
 }
 
-// host only: out[16] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, tmem_cols, TH, TB,
-//                       BW, n_mtiles, n_items, ny}
+// host only: out[16] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator columns
+//                       MT * Nt, TH, TB, BW, n_mtiles, n_items, ny}
 extern "C" int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out16) {
   pk::Plan p;
   if (int e = pk::make_plan(s, mode, terms_a, terms_w, p)) return e;
   if (out16) {
     const int v[16] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
-                       p.smem_bytes, p.tmem_cols, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny};
+                       p.smem_bytes, p.MT * p.Nt, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny};
     for (int i = 0; i < 16; ++i) out16[i] = v[i];
   }
   return 0;
@@ -1631,7 +1578,6 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   m.st_mask = pl.nstage - 1; m.st_log2 = pl.st_log2; m.stage16 = pl.stage_bytes >> 4;
   m.a_term16 = pl.a_bytes >> 4; m.a_mt16 = (pl.TA * pl.a_bytes) >> 4; m.a_k16 = 2 * pl.npos;
   m.b_off16 = pl.b_off >> 4; m.b_tap16 = (pl.CC / 8) * pl.Nt; m.b_k16 = 2 * pl.Nt;
-  m.idesc = tc::make_idesc(1, 1, 1, 128, (uint32_t)pl.Nt);
   m.a_lbo = (uint32_t)pl.npos * 16u; m.b_lbo = (uint32_t)pl.Nt * 16u;
   m.seg_len = (uint32_t)pl.seg_len;
   int nprog = 0;
@@ -1656,9 +1602,6 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
           }
     }
     p.img_bytes[y] = pl.img_bytes[y]; p.y_off[y] = pl.y_off[y];
-    p.zero_y[y] = pl.ntap[y] == 0;
-    const int nstages = pl.ntmpl[y] * pl.chunks;
-    p.nseg[y] = nstages == 0 ? 1 : (int)(((int64_t)nstages + pl.seg_len - 1) / pl.seg_len);
   }
   p.n_items = pl.n_items; p.n_ntiles = pl.n_ntiles; p.G = pl.G; p.MT = pl.MT; p.TA = pl.TA; p.chunks = pl.chunks;
   p.CC8 = pl.CC / 8; p.C8A = pl.C8A; p.kg8 = pl.kg / 8; p.stage_bytes = pl.stage_bytes; p.a_bytes = pl.a_bytes;
@@ -1667,7 +1610,7 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   p.n_mtiles = pl.n_mtiles;
   p.w_img = reinterpret_cast<const uint8_t*>(w_img);
   p.B = pl.B; p.THH = pl.THH; p.BW = pl.BW; p.OHr = pl.OHr; p.OWr = pl.OWr; p.OH = pl.OH; p.OW = pl.OW; p.omul = pl.omul; p.ny = pl.ny;
-  p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = (pl.NOUT + 7) / 8; p.smem_bytes = pl.smem_bytes; p.tmem_cols = pl.tmem_cols;
+  p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = (pl.NOUT + 7) / 8; p.smem_bytes = pl.smem_bytes; p.off_stg = pl.off_stg;
   p.mode = mode;
   p.n_scale = n_scale; p.a_scale = a_scale; p.a_scale_const = a_scale_const; p.bias = bias; p.bits8 = bits8; p.gain = gain;
   p.out = out; p.err = err_flag;
@@ -1685,14 +1628,17 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   if (pl.n_items >= (1 << 22) || pl.n_mtiles >= (1 << 22))     // FastDiv's exact range (fp32 reciprocal + one correction step)
     return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
   const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
-  if (pl.segmented) {
-    if (pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: segmented plan with Nt %d, MT %d", pl.Nt, pl.MT);
-    if (int e = set_max_smem(pk_conv_kernel<true>, kSmemBudget)) return e;
-    pk_conv_kernel<true><<<dim3(gx, pl.ny), ConvCfg<true>::THREADS, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
-  } else {
-    if (int e = set_max_smem(pk_conv_kernel<false>, kSmemBudget)) return e;
-    pk_conv_kernel<false><<<dim3(gx, pl.ny), ConvCfg<false>::THREADS, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
-  }
+  using ConvFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
+#define MNB_PK_CONV_FNS(SEG) {pk_conv_kernel<SEG, 16>, pk_conv_kernel<SEG, 32>, pk_conv_kernel<SEG, 48>, \
+                              pk_conv_kernel<SEG, 64>, pk_conv_kernel<SEG, 96>, pk_conv_kernel<SEG, 128>}
+  static const ConvFn fns[2][6] = {MNB_PK_CONV_FNS(false), MNB_PK_CONV_FNS(true)};
+#undef MNB_PK_CONV_FNS
+  int ki = -1;
+  for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
+  if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
+  const ConvFn fn = fns[pl.segmented ? 1 : 0][ki];
+  if (int e = set_max_smem(fn, kSmemBudget)) return e;
+  fn<<<dim3(gx, pl.ny), kConvThreads, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
   MNB_LAUNCHED(1);
   return 0;
 }
@@ -1736,7 +1682,6 @@ extern "C" int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t 
   m.Nc = pl.Nc; m.tpg = pl.tpg; m.n_tg = pl.n_tg; m.npairs = pl.npairs; m.st_mask = pl.nstage - 1; m.st_log2 = pl.st_log2; m.stage16 = pl.stage_bytes >> 4;
   m.sub16 = pl.sub_bytes >> 4; m.dy_term16 = pl.dy_bytes >> 4; m.x_off16 = (pl.TA * pl.dy_bytes) >> 4;
   m.x_term16 = (pl.nkph_used * pl.x_bytes) >> 4; m.x_kph16 = pl.x_bytes >> 4;
-  m.idesc = tc::make_idesc_major(1, 1, 1, 128, (uint32_t)pl.Nc, 1, 1);
   m.dy_sbo = (uint32_t)pl.rows_dy * 16u; m.x_sbo = (uint32_t)pl.rows_x * 16u; m.nsub = pl.nsub;
   for (int i = 0; i < pl.npairs; ++i) { m.pair_a16[i] = pl.pair_a[i] * m.dy_term16; m.pair_b16[i] = pl.pair_b[i] * m.x_term16; }
   {
@@ -1758,7 +1703,7 @@ extern "C" int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t 
   p.K8 = pl.K8; p.C8X = pl.C8X; p.cout_g8 = pl.cout_g / 8; p.cin_g8 = pl.cin_g / 8; p.Nc8 = pl.Nc / 8; p.TH = pl.TH; p.hlo = pl.hlo;
   p.wlo = pl.wlo; p.stage_bytes = pl.stage_bytes; p.sub_bytes = pl.sub_bytes; p.dy_bytes = pl.dy_bytes; p.x_bytes = pl.x_bytes;
   p.dy_box_bytes = pl.dy_box_bytes; p.x_box_bytes = pl.x_box_bytes; p.st_mask = pl.nstage - 1; p.st_log2 = pl.st_log2;
-  p.smem_bytes = pl.smem_bytes; p.tmem_cols = pl.tmem_cols; p.ntap = pl.ntap; p.Nc = pl.Nc; p.cout_g = pl.cout_g; p.cin_g = pl.cin_g;
+  p.smem_bytes = pl.smem_bytes; p.ntap = pl.ntap; p.Nc = pl.Nc; p.cout_g = pl.cout_g; p.cin_g = pl.cin_g;
   p.partial = reinterpret_cast<float*>(scratch); p.err = err_flag;
   CUtensorMap tdy[3], tx[3];
   const int64_t dy_plane = (int64_t)pl.B * pl.K8 * pl.P * pl.Q * 16;
@@ -1768,10 +1713,16 @@ extern "C" int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t 
     if (int e = make_pk_tmap(&tdy[t], dy_pk, dy_plane, t < pl.TA ? t : 0, pl.B, pl.K8, pl.P, pl.Q, pl.BW, pl.TH, 1, 16)) return e;
     if (int e = make_pk_tmap(&tx[t], x_pk, x_plane, t < pl.TX ? t : 0, pl.B, C8tot, pl.HX, pl.WX, pl.BW, pl.THH, 1, pl.Nc / 8)) return e;
   }
-  if (int e = set_max_smem(pk_wgrad_kernel, kSmemBudget)) return e;
+  using WgFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                        const CUtensorMap, const WgParams);
+  static const WgFn wfns[8] = {pk_wgrad_kernel<16>, pk_wgrad_kernel<32>, pk_wgrad_kernel<48>, pk_wgrad_kernel<64>,
+                               pk_wgrad_kernel<80>, pk_wgrad_kernel<96>, pk_wgrad_kernel<112>, pk_wgrad_kernel<128>};
+  if (pl.Nc % 16 || pl.Nc < 16 || pl.Nc > 128) return mnb_fail(MNB_E_ARG, "pk wgrad: plan with Nc %d", pl.Nc);
+  const WgFn wfn = wfns[pl.Nc / 16 - 1];
+  if (int e = set_max_smem(wfn, kSmemBudget)) return e;
   cudaStream_t st = (cudaStream_t)stream;
-  pk_wgrad_kernel<<<dim3(pl.G * pl.n_ktiles * pl.n_ctiles * pl.n_tg, pl.splits), NTHREADS, pl.smem_bytes, st>>>(tdy[0], tdy[1], tdy[2], tx[0],
-                                                                                                      tx[1], tx[2], p);
+  wfn<<<dim3(pl.G * pl.n_ktiles * pl.n_ctiles * pl.n_tg, pl.splits), kWgThreads, pl.smem_bytes, st>>>(tdy[0], tdy[1], tdy[2], tx[0],
+                                                                                                     tx[1], tx[2], p);
   {
     const int cout_o = pl.cout_g / pl.gm, cin_o = pl.cin_g / pl.gm;     // channels per original group
     const dim3 rgrid(cin_o * pl.ntap, (cout_o + 127) / 128, pl.G * pl.gm);

@@ -1,7 +1,7 @@
-// sm_100a building blocks for the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (TMEM alloc / mma / commit / ld) and the shared-memory / instruction descriptors.
-// Everything is inline PTX; the bit layouts follow the PTX ISA "tcgen05" matrix / instruction
-// descriptor tables (the same fields CuTe's mma_sm100_desc.hpp names).
+// sm_90a building blocks for the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor) and wgmma
+// (warpgroup MMA with register accumulators) with its shared-memory matrix descriptors.
+// Everything is inline PTX; the descriptor bit layout follows the PTX ISA "wgmma" matrix-descriptor table (the same
+// fields CuTe's mma_sm90_desc.hpp names).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -51,8 +51,7 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* e
 }
 
 // Bounded wait WITHOUT an early-exit branch: on timeout it records the error and simply returns, so the
-// caller's loops keep warp-uniform control flow (ptxas can then keep loop-carried address arithmetic in
-// uniform registers, which the single-thread tcgen05.mma issue path depends on).  After a timeout every
+// caller's loops keep warp-uniform control flow (a warpgroup must reach every wgmma together).  After a timeout every
 // later wait of the CTA returns after a short spin (shared `abort` flag): wrong results, but no hang.
 __device__ __forceinline__ void mbar_wait_soft(uint64_t* bar, uint32_t parity, int* err_flag, int code,
                                                volatile uint32_t* abort_flag) {
@@ -70,7 +69,7 @@ __device__ __forceinline__ void mbar_wait_soft(uint64_t* bar, uint32_t parity, i
   }
 }
 
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -111,195 +110,193 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
                : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-               "n"(NCOLS));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+// ------------------------------------------------------------------ wgmma
+// One warpgroup (4 consecutive warps, the first a multiple of 4) issues D[64 x N] (+)= A[64 x 16] * B[N x 16]^T with A and B
+// read from shared memory through descriptors; D lives in the registers of the 128 threads.  Fragment of one thread
+// (warp w of the warpgroup, lane l): d[4j + 2i + c] = D[16w + l/4 + 8i][8j + 2(l%4) + c].
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across wgmma issue and wg_wait (the asm outputs of an
+// issue are only valid after the wait that retires it)
+template <typename T, int NR>
+__device__ __forceinline__ void fence_acc(T (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+r"(reinterpret_cast<uint32_t(&)[NR]>(d)[i])::"memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS));
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; one thread issues on behalf of the CTA
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same instruction for warp-converged issue loops: every lane executes the (uniform) address
-// arithmetic so that ptxas keeps descriptors in uniform registers, and only the lane whose `guard`
-// is non-zero issues.  (Guarding the whole loop with `if (lane == 0)` instead makes every operand a
-// per-thread value: each MMA then pays an ELECT loop plus five R2UR broadcasts, ~150+ cycles.)
-__device__ __forceinline__ void mma_f16_guarded(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate, uint32_t guard) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(guard)
-      : "memory");
-}
-// Same, descriptors given as (low word, high word): only the 14-bit start-address field of the low word changes from
-// MMA to MMA, so issue loops carry 32-bit adds and the loop-invariant high words stay in uniform registers.
-__device__ __forceinline__ void mma_f16_guarded_lh(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                                   uint32_t b_hi, uint32_t idesc, uint32_t accumulate, uint32_t guard) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\tsetp.ne.b32 q, %7, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate), "r"(guard)
-      : "memory");
-}
-// Warp-converged issue with the hardware election inside the instruction group: `elect.sync` tells ptxas that exactly
-// one lane issues, so no per-lane ELECT / BRA.U.ANY loop is generated around the UTCHMMA and uniform operands stay in
-// uniform registers.  All 32 lanes must execute this (converged).
-__device__ __forceinline__ void mma_f16_elect_lh(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// FOUR MMAs of a host-built issue program in one instruction group: w.x .. w.w = (A offset | B offset << 16) in 16-byte
-// units relative to a_base / b_base, 0xffffffff = no MMA (padding of the program to a multiple of four).  One election
-// and one 128-bit constant load per four MMAs; the first MMA takes `accumulate_first`, the others accumulate.
-// (Measured on the one-word-per-iteration loop, ncu source view: ~105 issue cycles per MMA against 61 of tensor time -
-// the indexed constant load sat on the critical path of every MMA, plus ELECT / VOTEU / 4 x R2UR each.)
-__device__ __forceinline__ void mma_f16_x4(uint32_t d_tmem, uint32_t a_base, uint32_t a_hi, uint32_t b_base, uint32_t b_hi,
-                                           uint32_t idesc, uint4 w, uint32_t accumulate_first) {
-  asm volatile(
-      "{\n\t.reg .pred q, p0, e1, e2, e3, pt;\n\t.reg .b64 da, db;\n\t.reg .b32 al, bl;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p0, %10, 0;\n\t"
-      "setp.eq.b32 pt, %5, %5;\n\t"
-      "setp.ne.and.b32 e1, %7, 0xffffffff, q;\n\t"
-      "setp.ne.and.b32 e2, %8, 0xffffffff, q;\n\t"
-      "setp.ne.and.b32 e3, %9, 0xffffffff, q;\n\t"
-      "and.b32 al, %6, 0xffff;\n\tadd.u32 al, al, %1;\n\tshr.u32 bl, %6, 16;\n\tadd.u32 bl, bl, %3;\n\t"
-      "mov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p0;\n\t"
-      "and.b32 al, %7, 0xffff;\n\tadd.u32 al, al, %1;\n\tshr.u32 bl, %7, 16;\n\tadd.u32 bl, bl, %3;\n\t"
-      "mov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "@e1 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-      "and.b32 al, %8, 0xffff;\n\tadd.u32 al, al, %1;\n\tshr.u32 bl, %8, 16;\n\tadd.u32 bl, bl, %3;\n\t"
-      "mov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "@e2 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-      "and.b32 al, %9, 0xffff;\n\tadd.u32 al, al, %1;\n\tshr.u32 bl, %9, 16;\n\tadd.u32 bl, bl, %3;\n\t"
-      "mov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "@e3 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t}"
-      ::"r"(d_tmem), "r"(a_base), "r"(a_hi), "r"(b_base), "r"(b_hi), "r"(idesc), "r"(w.x), "r"(w.y), "r"(w.z), "r"(w.w),
-        "r"(accumulate_first)
-      : "memory");
-}
-// Up to four MMAs that share the A operand and the accumulate flag and differ in the B offset and the accumulator
-// (weight gradient: one accumulator per filter tap, d_tmem + i * d_step): boff.x .. boff.w are added to b_row,
-// 0xffffffff = no MMA.  One election / one 128-bit program load per group, see mma_f16_x4.
-__device__ __forceinline__ void mma_f16_x4_taps(uint32_t d_tmem, uint32_t d_step, uint32_t a_lo, uint32_t a_hi, uint32_t b_row,
-                                                uint32_t b_hi, uint32_t idesc, uint4 boff, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred q, p, e0, e1, e2, e3;\n\t.reg .b64 da, db;\n\t.reg .b32 bl, dd;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %11, 0;\n\t"
-      "setp.ne.and.b32 e0, %7, 0xffffffff, q;\n\t"
-      "setp.ne.and.b32 e1, %8, 0xffffffff, q;\n\t"
-      "setp.ne.and.b32 e2, %9, 0xffffffff, q;\n\t"
-      "setp.ne.and.b32 e3, %10, 0xffffffff, q;\n\t"
-      "mov.b64 da, {%2, %3};\n\t"
-      "add.u32 bl, %4, %7;\n\tmov.b64 db, {bl, %5};\n\t"
-      "@e0 tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %6, p;\n\t"
-      "add.u32 bl, %4, %8;\n\tmov.b64 db, {bl, %5};\n\tadd.u32 dd, %0, %1;\n\t"
-      "@e1 tcgen05.mma.cta_group::1.kind::f16 [dd], da, db, %6, p;\n\t"
-      "add.u32 bl, %4, %9;\n\tmov.b64 db, {bl, %5};\n\tadd.u32 dd, dd, %1;\n\t"
-      "@e2 tcgen05.mma.cta_group::1.kind::f16 [dd], da, db, %6, p;\n\t"
-      "add.u32 bl, %4, %10;\n\tmov.b64 db, {bl, %5};\n\tadd.u32 dd, dd, %1;\n\t"
-      "@e3 tcgen05.mma.cta_group::1.kind::f16 [dd], da, db, %6, p;\n\t}"
-      ::"r"(d_tmem), "r"(d_step), "r"(a_lo), "r"(a_hi), "r"(b_row), "r"(b_hi), "r"(idesc), "r"(boff.x), "r"(boff.y), "r"(boff.z),
-        "r"(boff.w), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                       uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread arrive on `bar` when they complete
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <typename T, int NR>
+__device__ __forceinline__ void zero_acc(T (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) d[i] = T(0);
 }
 
-// commit issued by the SAME elected lane as mma_f16_elect_lh (elect.sync is deterministic for a given member mask): the
-// commit tracks the MMAs of the executing thread only.  Warp-converged.
-__device__ __forceinline__ void mma_commit_elect(uint64_t* bar) {
+// bf16 x bf16 -> f32, N = 16 .. 160 in steps of 16 (the widths the kernels are instantiated for).  TA / TB: operand stored MN-major (1) or K-major (0).
+template <int N> struct Mma;
+template <> struct Mma<16> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<32> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<48> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[24], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<64> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<80> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[40], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, %43, %44;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<96> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<112> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[56], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, %59, %60;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<128> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<144> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[72], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n144k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, %72, %73, p, 1, 1, %75, %76;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+template <> struct Mma<160> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void bf16(float (&d)[80], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, %80, %81, p, 1, 1, %83, %84;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+  }
+};
+__device__ __forceinline__ void mma_s8_n128(int32_t (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-      ::"r"(smem_u32(bar))
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d)
       : "memory");
 }
 
-// TMEM -> registers: warp w (w % 4 selects the 32-lane quarter) reads 32 consecutive columns
-// of its 32 lanes; thread i gets lane (quarter*32 + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
+// columns [c0, c0 + nc) of the warpgroup's m64 x N fragment -> s[(col - c0) * ld + row0 + row] (column-major staging
+// tile: a thread that owns row m reads its columns conflict-free; ld = 4 (mod 32) keeps the fragment's scattered writes
+// conflict-free too).  c0 / nc should be compile-time constants after unrolling: the register index must be static.
+template <int NR>
+__device__ __forceinline__ void frag_cols_to_smem(const float (&d)[NR], float* s, int ld, int row0, int c0, int nc) {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int r = row0 + 16 * w + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < NR / 4; ++j) {
+    if (8 * j < c0 || 8 * j >= c0 + nc) continue;
+    float* p = s + (8 * j - c0 + c) * ld + r;
+    p[0] = d[4 * j]; p[ld] = d[4 * j + 1]; p[8] = d[4 * j + 2]; p[ld + 8] = d[4 * j + 3];
+  }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <int NR>
+__device__ __forceinline__ void frag_to_smem(const float (&d)[NR], float* s, int ld, int row0) {
+  frag_cols_to_smem(d, s, ld, row0, 0, 2 * NR);
+}
+constexpr int kStageLd = 132;   // 128-row staging tiles
+constexpr int kStageLd64 = 68;  // 64-row staging tiles
 
 // ------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor, K-major, no swizzle ("interleaved" canonical layout):
-//   core matrix = 8 rows x 16 bytes stored contiguously (row r at +16*r);
-//   SBO = byte distance between consecutive 8-row groups along M/N;
-//   LBO = byte distance between the two 16-byte K-chunks of one MMA K-step.
+// Shared-memory matrix descriptor, no swizzle ("interleaved" canonical layout), core matrix = 8 rows x 16 bytes stored
+// contiguously (row r at +16*r).
+//   K-major : LBO = byte distance between the two 16-byte K-chunks of one K16 step, SBO = between consecutive 8-row groups
+//   MN-major: 16-byte vectors hold 8 consecutive M (or N) elements, 8 consecutive K rows 16 bytes apart;
+//             LBO = byte distance between consecutive 8-row K groups, SBO = between consecutive 8-element M/N groups.
 __device__ __forceinline__ uint64_t smem_desc_kmajor_noswz(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  return d;                // base_offset = 0, lbo_mode = 0, layout_type = 0 (no swizzle)
+  return d;                // base_offset = 0, layout_type = 0 (no swizzle)
 }
-
-// Instruction descriptor (32-bit).  fmt: kind::f16 -> 0 F16, 1 BF16, 2 TF32 ; kind::i8 -> 0 U8, 1 S8.
-// cfmt: 0 F16, 1 F32, 2 S32.  Both operands K-major, dense, no negate, no saturate.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t cfmt, uint32_t afmt, uint32_t bfmt, uint32_t M,
-                                                  uint32_t N) {
-  return (cfmt << 4) | (afmt << 7) | (bfmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// same, with explicit operand majors (0 = K-major, 1 = MN-major)
-__host__ __device__ constexpr uint32_t make_idesc_major(uint32_t cfmt, uint32_t afmt, uint32_t bfmt, uint32_t M,
-                                                        uint32_t N, uint32_t a_mn, uint32_t b_mn) {
-  return make_idesc(cfmt, afmt, bfmt, M, N) | (a_mn << 15) | (b_mn << 16);
-}
-// MN-major no-swizzle canonical layout: 16-byte vectors hold 8 consecutive M (or N) elements,
-// 8 consecutive K rows are 16 bytes apart (128-byte core matrix);
-//   LBO = byte distance between consecutive 8-row K groups,
-//   SBO = byte distance between consecutive 8-element M/N groups.
-// The bit layout of the descriptor is the same as the K-major one.
 __device__ __forceinline__ uint64_t smem_desc_mnmajor_noswz(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return smem_desc_kmajor_noswz(saddr, lbo_bytes, sbo_bytes);
 }

@@ -2,8 +2,7 @@
 //
 // BASELINE.json north_star: "the wbwtab binary/ternary case additionally gets a bit-packed XNOR-popcount kernel picked
 // when ncu shows it beating the tensor-core path".  This file is that kernel; harness/xnor_probe.py times it against the
-// packed-operand tensor-core forward (mnb_pk.cu) layer by layer and functional.py picks per layer from the measured
-// table (DESIGN.md 4.12, profiles/r2_xnor_vs_tc.md).
+// packed-operand tensor-core forward (mnb_pk.cu) layer by layer and functional.xnor_preferred picks per layer (DESIGN.md 4.12).
 //
 // Reference math (WB:11-36, 55-75, 98-146, 181-195): y = bias + alpha[k] * sum_{c,r,s} a[c] * w[k][c][r][s] with
 // a = sign(x) in {-1, +1} (0 -> +1) and w in {-1, +1} (binary) or {-1, 0, +1} (ternary); out-of-image taps contribute 0.
@@ -96,9 +95,7 @@ __global__ void __launch_bounds__(128) pack_weight_kernel(const int16_t* __restr
 // forward: one thread = PX output pixels (256 apart: coalesced), looping over the output channels of its block's
 // (group, k-slice); the slice's weight words and per-channel constants sit in shared memory and are read as warp-wide
 // broadcasts (three 16-byte loads per channel for the 128-channel 1x1 layers, shared by the PX pixels), activation words stay
-// in registers.  First version (one pixel per thread, per-channel alpha / bias from global memory, border code compiled into
-// every variant): 44 instructions per output, issue-bound at 105 us on the 256-channel 1x1 layer (ncu r3c: 84 % issue
-// active) against a POPC floor of 58 us.
+// in registers: the kernel is instruction-issue bound, so per-output instructions are what this layout saves.
 // ------------------------------------------------------------------------------------------------------------------
 struct Params {
   const uint32_t* abits;
@@ -111,8 +108,7 @@ struct Params {
 };
 
 // pixels per thread: two where the receptive field is a few words (1x1 layers: the per-channel shared-memory loads and loop
-// overhead are shared), one where it is nine or more (3x3 / 5x5: 2 x 9 activation words + border state cost occupancy -
-// measured r3d: 123 vs 97 us on the 3x3 g16 layer)
+// overhead are shared), one where it is nine or more (3x3 / 5x5: 2 x 9 activation words + border state cost occupancy)
 template <int R_, int NW_> struct PxOf { static constexpr int value = (R_ * R_ * NW_ <= 8) ? 2 : 1; };
 
 // shared-memory record of one output channel: [S words TW][N words TW][popc(N) total, alpha, bias, 0][prefix table (R+1)^2]

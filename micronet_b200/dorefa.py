@@ -1,4 +1,4 @@
-"""DoReFa k-bit QAT modules on the B200 engine.
+"""DoReFa k-bit QAT modules on the H100 engine.
 
 Drop-in for the reference's ``micronet/compression/quantization/wqaq/dorefa/quantize.py``:
 same class names, constructor signatures (DF:77-91, DF:178-186), attribute names and

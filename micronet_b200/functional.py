@@ -292,14 +292,12 @@ def materialized(t):
 
 
 def xnor_preferred(sh, has_plane):
-    """MNB_XNOR=auto: take the XNOR-popcount forward for this wbwtab inference layer?  Decided from the layer-by-layer
-    measurement of harness/xnor_probe.py on B200 (profiles/r2_xnor_vs_tc.md, NIN-GC layers at batch 256):
+    """MNB_XNOR=auto: take the XNOR-popcount forward for this wbwtab inference layer?
 
-    * the two convolution kernels tie within ~7 % on the 1x1 layers (29 - 87 us vs 27 - 81 us) and split the 3x3 layers
-      (102 vs 83 us, 56 vs 58 us): both are dominated by the fp32 output they write, and B200's popc pipe (16 lanes / clk /
-      SM) gives the bit kernel no arithmetic edge over tcgen05 on +-1 operands;
-    * the operand it reads is 16 x smaller (1 bit vs one bf16 per activation): packing it from an fp32 tensor costs 11 - 50 us
-      against 25 - 156 us for the bf16 plane, so a layer that has to pack its own input is 1.08 - 1.79 x faster end to end.
+    * both convolution kernels are dominated by the fp32 output they write, and the popc pipe gives the bit kernel no
+      arithmetic edge over the tensor cores on +-1 operands;
+    * the operand it reads is 16 x smaller (1 bit vs one bf16 per activation), so a layer that has to pack its own input
+      saves most of its pack pass (harness/xnor_probe.py times both forms layer by layer; not yet measured on the H100).
 
     Hence: XNOR when the layer packs its own operand (no producer-written plane came with x), the tensor-core forward when a
     fused BatchNorm + binarizer already wrote the bf16 plane (the pack pass is free there)."""
@@ -424,8 +422,8 @@ class QuantConv2dFn(Function):
         ctx.pk = False
         if (L.XNOR_MODE != "off" and spec is None and w_int is not None and getattr(x, "_mnb_pm1", False)
                 and (no_grad or not any(ctx.needs_input_grad[:3])) and x.dtype == torch.float32 and not pre_relu):
-            # wbwtab inference forward on +-1 activations: bit-packed XNOR-popcount kernel where it was measured to beat the
-            # tensor-core forward (north_star; table: profiles/r2_xnor_vs_tc.md).  Same integer sums, same fmaf epilogue:
+            # wbwtab inference forward on +-1 activations: bit-packed XNOR-popcount kernel where it is expected to beat the
+            # tensor-core forward (xnor_preferred).  Same integer sums, same fmaf epilogue:
             # bit-identical to the packed-operand path.  Training steps never come here (their backward multiplies real-valued
             # gradients and wants the bf16 operand plane the forward already read).
             from . import xnor as XN
@@ -480,7 +478,7 @@ class QuantConv2dFn(Function):
                 elif rc != L.E_UNSUPPORTED:
                     L.check(rc, "pk_conv fwd (packed producer)")
         if not done and L.USE_TC and w_int is not None and x.dtype == torch.float32:
-            # fused tcgen05 path: quantize inside the operand staging of the tensor-core conv
+            # fused wgmma path: quantize inside the operand staging of the tensor-core conv
             qp = None
             if spec is not None:
                 qp = spec.struct()

@@ -1,10 +1,10 @@
-"""Integer-arithmetic-only (IAO) QAT / PTQ / QAFT modules on the B200 engine.
+"""Integer-arithmetic-only (IAO) QAT / PTQ / QAFT modules on the H100 engine.
 
 Drop-in for the reference's ``micronet/compression/quantization/wqaq/iao/quantize.py``:
 same class names, constructor signatures (IAO:326-346, 653-676, 998-1012), attribute names,
 registered buffers (so reference checkpoints load: IAO:45-60, 182-204, 247-286) and
 ``prepare`` rules (IAO:1501-1824).  Observers, scale / zero-point updates, fake-quant, the
-convolutions and their backward all run as sm_100a kernels with no host synchronisation."""
+convolutions and their backward all run as sm_90a kernels with no host synchronisation."""
 from __future__ import annotations
 
 import copy

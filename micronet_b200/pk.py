@@ -5,7 +5,7 @@ shared memory, stride 2, 5x5 filters, 4x4 or 224x224 images ...) and every fused
 
     pack_act    fp32 NCHW -> bf16 term planes [t][b][c/8][h][w][8] (fake-quantize, or exact split of an fp32 tensor)
     pack_weight integer levels / fp32 weights -> the bf16 operand image of one (shape, mode)
-    conv        TMA -> tcgen05.mma -> TMEM -> epilogue (forward: scale + bias; data gradient: STE mask)
+    conv        TMA -> wgmma (register accumulators) -> epilogue (forward: scale + bias; data gradient: STE mask)
     wgrad       the same boxes read as MN-major operands, split over the batch, deterministic reduction
 
 Reference math: F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen's

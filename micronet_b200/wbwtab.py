@@ -1,4 +1,4 @@
-"""Binary / ternary weight, binary activation QAT modules on the B200 engine.
+"""Binary / ternary weight, binary activation QAT modules on the H100 engine.
 
 Drop-in for the reference's ``micronet/compression/quantization/wbwtab/quantize.py``
 (constructor signatures WB:80, WB:106, WB:153-166; ``prepare`` rules WB:247-347)."""

@@ -21,7 +21,7 @@ reference on every quantity we compare.
 
 Pinning: the reference ships no golden vectors / known-answer tests
 (SURVEY.md §4, §8c).  The oracle is pinned against the reference ITSELF,
-imported unmodified from ``/root/reference`` in the build container by
+imported unmodified (a checkout named by ``MICRONET_REFERENCE``) by
 ``tests/golden/make_golden.py``; the resulting fixtures are committed under
 ``tests/golden/`` and checked by ``tests/test_oracle_golden.py`` (CPU suite).
 

@@ -21,7 +21,7 @@ def _no_tf32():
 
 def pytest_configure(config):
     _no_tf32()
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,4 +1,4 @@
-"""Case tables shared by ``make_golden.py`` (reference side, build container) and
+"""Case tables shared by ``make_golden.py`` (reference side) and
 the parity tests (oracle / CUDA side).  Pure data + a seeded input generator."""
 import torch
 

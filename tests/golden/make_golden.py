@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Generate the golden fixtures in this directory FROM THE REFERENCE ITSELF.
 
-Run in the build container only (it imports the unmodified reference from
-/root/reference, which does not exist on the GPU box):
+Needs a checkout of the reference (666DZY666/micronet @ c31cdd28); the tests only read the committed fixtures:
 
-    python tests/golden/make_golden.py
+    MICRONET_REFERENCE=<path to the checkout> python tests/golden/make_golden.py
 
 For every case below it instantiates the reference's own module
 (``micronet.compression.quantization.{wbwtab,wqaq.dorefa,wqaq.iao}.quantize``),
@@ -20,7 +19,9 @@ import sys
 import numpy as np
 import torch
 
-REF = os.environ.get("MICRONET_REFERENCE", "/root/reference")
+REF = os.environ.get("MICRONET_REFERENCE")
+if not REF:
+    sys.exit("make_golden.py: set MICRONET_REFERENCE to a checkout of 666DZY666/micronet @ c31cdd28")
 sys.path.insert(0, REF)
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Golden fixtures for the inference-graph converters (SURVEY 8 f3), generated FROM THE REFERENCE'S OWN bn_fuse SCRIPTS.
 
-Run in the build container only (imports the unmodified reference from /root/reference):
+Needs a checkout of the reference (MICRONET_REFERENCE=<path>, 666DZY666/micronet @ c31cdd28); the tests only read the
+committed fixtures:
 
     python tests/golden/make_golden_bnfuse.py
 
@@ -18,7 +19,9 @@ import sys
 import numpy as np
 import torch
 
-REF = os.environ.get("MICRONET_REFERENCE", "/root/reference")
+REF = os.environ.get("MICRONET_REFERENCE")
+if not REF:
+    sys.exit("make_golden_bnfuse.py: set MICRONET_REFERENCE to a checkout of 666DZY666/micronet @ c31cdd28")
 HERE = os.path.dirname(os.path.abspath(__file__))
 QDIR = os.path.join(REF, "micronet", "compression", "quantization")
 

@@ -1,16 +1,13 @@
-"""`QuantConvTranspose2d` on the CPU side (SURVEY 8 row f4): module surface / prepare() of all three schemes without a GPU, and -
-where the reference tree is present (build container only) - the evidence that the reference's OWN wbwtab / dorefa classes are
-not runnable under current PyTorch, which is why only the IAO one (IAO:510-636) has golden fixtures generated from the reference
-(tests/golden/layer_iao_convT_*.npz) and the other two are pinned on the oracle's quantizers composed with ATen."""
+"""`QuantConvTranspose2d` on the CPU side (SURVEY 8 row f4): module surface / prepare() of all three schemes without a GPU.
+The reference's own wbwtab / dorefa classes are not runnable under current PyTorch (they hand dilation / groups / bias to
+nn.ConvTranspose2d positionally in the wrong order), which is why only the IAO one (IAO:510-636) has golden fixtures generated
+from the reference (tests/golden/layer_iao_convT_*.npz) and the other two are pinned on the oracle's quantizers composed with
+ATen."""
 import copy
-import os
-import sys
 
 import pytest
 import torch
 import torch.nn as nn
-
-REF = os.environ.get("MICRONET_REFERENCE", "/root/reference")
 
 
 def _net():
@@ -40,23 +37,3 @@ def test_prepare_swaps_conv_transpose_in_every_scheme():
     for m in (d[2], w[2], i[2]):                                    # no CPU path: the engine refuses CPU tensors loudly
         with pytest.raises(Exception):
             m(torch.randn(1, 16, 4, 4))
-
-
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "micronet")), reason="reference tree not present (GPU box)")
-def test_reference_dorefa_and_wbwtab_conv_transpose_do_not_run():
-    sys.path.insert(0, REF)
-    try:
-        import micronet.compression.quantization.wbwtab.quantize as ref_wb
-        import micronet.compression.quantization.wqaq.dorefa.quantize as ref_df
-        import micronet.compression.quantization.wqaq.iao.quantize as ref_iao
-    finally:
-        sys.path.remove(REF)
-    x = torch.randn(2, 8, 5, 5)
-    m = ref_df.QuantConvTranspose2d(8, 6, 3, stride=2, padding=1, output_padding=1)
-    assert m.dilation == (True, True)          # `bias` landed in `dilation` (DF:142-153 vs nn.ConvTranspose2d's argument order)
-    with pytest.raises(TypeError):
-        m(x)
-    with pytest.raises(TypeError):
-        ref_wb.QuantConvTranspose2d(8, 6, 3, stride=2, padding=1, output_padding=1)(x)
-    y = ref_iao.QuantConvTranspose2d(8, 6, 3, stride=2, padding=1, output_padding=1)(x)   # keyword-correct: runs
-    assert tuple(y.shape) == (2, 6, 10, 10)

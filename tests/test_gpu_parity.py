@@ -1,4 +1,4 @@
-"""GPU parity suite (run on the B200 box): the CUDA engine, called through the C-ABI, against
+"""GPU parity suite (run on an H100): the CUDA engine, called through the C-ABI, against
  (a) the committed golden fixtures generated from the reference itself, and
  (b) the CPU oracle on seeded inputs.
 Bar (BASELINE.json north_star): integer quantized levels bit-exact, fp32 results within 1e-5

@@ -1,4 +1,4 @@
-"""Fused tcgen05 forward conv (mnb_fq_conv2d_fwd_tc) against the generic kernels, the standalone
+"""Fused wgmma forward conv (mnb_fq_conv2d_fwd_tc) against the generic kernels, the standalone
 quantizer kernel (codes / STE bits must be identical) and ATen-CPU conv2d."""
 import numpy as np
 import pytest
@@ -178,7 +178,7 @@ def test_tc_dgrad_matches_generic_and_cpu(shape, mode):
 @pytest.mark.parametrize("shape", SHAPES, ids=[str(s) for s in SHAPES])
 @pytest.mark.parametrize("mode", ["raw_pm1", "raw_fp32", "dorefa8", "iao_sym"])
 def test_tc_wgrad_matches_generic_and_cpu(shape, mode):
-    """dWq through the tensor-core wgrad (MN-major operands, TMEM-resident accumulators, deterministic
+    """dWq through the tensor-core wgrad (MN-major operands, register accumulators, deterministic
     two-stage reduction); raw fp32 inputs that are not bf16-exact take the device-side fallback."""
     from micronet_b200 import _lib as L, functional as F_
     from oracle import reference_port as O

@@ -1,4 +1,4 @@
-"""Hardware self-tests of the sm_100a building blocks (tcgen05 descriptors, TMA geometry)."""
+"""Hardware self-tests of the sm_90a building blocks (wgmma descriptors, TMA geometry)."""
 import ctypes as C
 
 import pytest

@@ -1,25 +1,14 @@
 """dorefa / wbwtab `QuantConvTranspose2d` (DF:125-174, WB:198-244; SURVEY 8 row f4).  The reference's own classes cannot serve as
 the oracle here: they pass (dilation, groups, bias) positionally in the wrong order to nn.ConvTranspose2d and their forward raises
-TypeError under current PyTorch (tests/test_conv_transpose_cpu.py shows it when /root/reference is present).  The engine modules
-implement the intent, so the check is the composition of the ORACLE's quantizers (pinned by the golden fixtures) with ATen's
-conv_transpose2d on the CPU.
-
-NOT YET RUN ON HARDWARE: these tests were written after the round's last GPU window (the one attempt, gpurun call 11, was cut by
-its 25-second limit during `import torch`).  They are therefore skipped unless MNB_RUN_UNVALIDATED=1 - an unvalidated test must
-not be able to turn the suite red - and they are the first thing to run in the next round.  The kernels underneath
-(functional.ConvTranspose2dFn and the dorefa / wbwtab quantizer Functions) are the ones tests/test_gpu_conv_transpose.py and
-tests/test_gpu_parity.py already pin; what is unvalidated is only the module-level composition."""
-import os
-
+TypeError under current PyTorch.  The engine modules implement the intent, so the check is the composition of the ORACLE's
+quantizers (pinned by the golden fixtures) with ATen's conv_transpose2d on the CPU."""
 import pytest
 import torch
 import torch.nn.functional as TF
 
 from tests.oracle_util import rel_err
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(os.environ.get("MNB_RUN_UNVALIDATED", "0") != "1",
-                                 reason="written after the round's last GPU window; set MNB_RUN_UNVALIDATED=1 to run")]
+pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 # Cin, Cout, k, stride, pad, output_padding, B, H
