@@ -348,6 +348,14 @@ int mnb_pk_pack_act_relu(const float* x, int32_t batch, int32_t channels, int32_
                          int32_t terms, const float* ch_scale, int32_t phase_split, int32_t relu, void* out_pk,
                          uint8_t* bits8, mnb_stream_t stream);
 int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out16); /* host only */
+/* host only, the plan mnb_pk_conv / mnb_pk_wgrad will run (same MNB_PK_* environment knobs); the first min(n, 21) resp.
+ * min(n, 10) fields are written:
+ *   mnb_pk_conv_plan_ex: the 16 fields of mnb_pk_conv_plan, then segmented, seg_len (stages per segment, 0 when not
+ *                        segmented), npairs (piece products per K-step), col_tiles, n_mgroups
+ *   mnb_pk_wgrad_plan  : Nc, n_ctiles, tpg (taps per CTA), n_tg (tap groups), gm (merged groups), splits (batch splits),
+ *                        NI (sub-blocks per stage), nstage, BW, TH */
+int mnb_pk_conv_plan_ex(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out, int32_t n);
+int mnb_pk_wgrad_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n);
 int64_t mnb_pk_wimage_bytes(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w);
 int mnb_pk_pack_weight(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, const int16_t* w_int,
                        const float* w_f32, const float* kzero, void* w_img, mnb_stream_t stream);

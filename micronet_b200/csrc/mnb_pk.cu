@@ -962,7 +962,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           bs[4 * v] = c.x; bs[4 * v + 1] = c.y; bs[4 * v + 2] = c.z; bs[4 * v + 3] = c.w;
         }
         float* op = orow + (int64_t)n0 * plane;
-        if (!SEG && p.post_out) {
+        if (!SEG && p.post_out) {   // (the host refuses a consumer plane on segmented plans)
           // forward conv of a frozen inference graph: y = acc * scale + bias [-> ReLU] -> consumer's quantizer -> bf16 levels
           float lev[16], yv[16];
 #pragma unroll
@@ -1519,17 +1519,24 @@ extern "C" int mnb_bn_relu_quant_pack_fwd(const float* x, int32_t batch, int32_t
   return 0;
 }
 
-// host only: out[16] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator columns
-//                       MT * Nt, TH, TB, BW, n_mtiles, n_items, ny}
-extern "C" int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out16) {
+// host only: out[0..15] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator
+//                          columns MT * Nt, TH, TB, BW, n_mtiles, n_items, ny},
+//            out[16..20] = {segmented, seg_len, npairs, col_tiles, n_mgroups}; the first min(n, 21) are written
+extern "C" int mnb_pk_conv_plan_ex(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out,
+                                   int32_t n) {
   pk::Plan p;
   if (int e = pk::make_plan(s, mode, terms_a, terms_w, p)) return e;
-  if (out16) {
-    const int v[16] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
-                       p.smem_bytes, p.MT * p.Nt, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny};
-    for (int i = 0; i < 16; ++i) out16[i] = v[i];
+  if (out) {
+    const int v[21] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
+                       p.smem_bytes, p.MT * p.Nt, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny,
+                       p.segmented, p.segmented ? p.seg_len : 0, p.npairs, p.col_tiles, p.n_mgroups};
+    for (int i = 0; i < std::min(n, 21); ++i) out[i] = v[i];
   }
   return 0;
+}
+
+extern "C" int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out16) {
+  return mnb_pk_conv_plan_ex(s, mode, terms_a, terms_w, out16, 16);
 }
 
 extern "C" int64_t mnb_pk_wimage_bytes(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w) {
@@ -1569,6 +1576,9 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     MNB_REQUIRE(post->q->bits >= 2 && post->q->bits <= 8, "pk conv: consumer levels must fit one bf16 piece (2..8 bits)");
     if (pl.G > 1 && (pl.ng % 8)) return unsupported("fused consumer of a grouped conv needs channels per group % 8 == 0");
     if (post->phase_split && ((pl.OH | pl.OW) & 1)) return unsupported("stride-2 consumer of an odd-sized plane");
+    // the consumer epilogue is compiled into the single-product kernels only: in the segmented ones (several piece
+    // products, e.g. an asymmetric-IAO producer whose levels take two pieces) it costs register spills on every launch
+    if (pl.segmented) return unsupported("fused consumer of a segmented (multi-piece) plan");
   }
   if (bits8 && pl.G > 1 && (pl.ng % 8)) return unsupported("STE mask of a grouped conv needs channels per group % 8 == 0");
   static ConvParams p;   // large POD: filled per call (single host thread per process)
@@ -1664,6 +1674,17 @@ extern "C" int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t t
   pk::WgPlan p;
   if (pk::make_wg_plan(s, terms_dy, terms_x, p)) return -1;
   return p.partial_floats * 4;
+}
+
+// host only: out = {Nc, n_ctiles, tpg, n_tg, gm, splits, NI, nstage, BW, TH}; the first min(n, 10) are written
+extern "C" int mnb_pk_wgrad_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n) {
+  pk::WgPlan p;
+  if (int e = pk::make_wg_plan(s, terms_dy, terms_x, p)) return e;
+  if (out) {
+    const int v[10] = {p.Nc, p.n_ctiles, p.tpg, p.n_tg, p.gm, p.splits, p.NI, p.nstage, p.BW, p.TH};
+    for (int i = 0; i < std::min(n, 10); ++i) out[i] = v[i];
+  }
+  return 0;
 }
 
 // dw[k][c][r][s] = mul(k) * sum_{b,p,q} dy[b,k,p,q] * x[b,c,p*st+r-pad, q*st+s-pad];  mul(k) = a_scale[0] / kdiv[k]

@@ -771,8 +771,10 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
     sh = _shape_struct(x.shape, wq.shape, stride, padding, dilation, groups)
     p, q = _out_hw(sh)
     out_shape = (x.shape[0], wq.shape[0], p, q)
-    fused = consumer is not None and consumer.accepts(out_shape)
     ta, tw = _pk_terms(spec, w_int)
+    # a segmented producer plan (two level pieces of an asymmetric quantizer) takes no fused consumer: the consumer packs
+    # its own operand from y
+    fused = consumer is not None and consumer.accepts(out_shape) and not PK.segmented(sh, 0, ta, tw)
     if (plane is None and not fused) or spec is None or w_int is None or L.PK_MODE == "off" or not PK.supported(sh, 0, ta, tw):
         if plane is not None:
             raise RuntimeError("micronet_b200: handed-over plane in front of a conv outside the packed-operand cover")

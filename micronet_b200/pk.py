@@ -33,6 +33,16 @@ def supported(sh, mode, terms_a, terms_w):
     return _plan_cache[k]
 
 
+def segmented(sh, mode, terms_a, terms_w):
+    """does the plan run segmented accumulation (several piece products per K-step, long K loop)?  Such plans take no
+    fused consumer (mnb_pk_conv_post refuses them).  Host-only plan query, cached."""
+    k = ("s", _key(sh), mode, terms_a, terms_w)
+    if k not in _plan_cache:
+        out = (C.c_int32 * 17)()
+        _plan_cache[k] = L.load().mnb_pk_conv_plan_ex(C.byref(sh), mode, terms_a, terms_w, out, 17) == 0 and out[16] != 0
+    return _plan_cache[k]
+
+
 def wgrad_supported(sh, terms_dy, terms_x):
     k = ("w", _key(sh), terms_dy, terms_x)
     if k not in _plan_cache:

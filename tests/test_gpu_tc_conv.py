@@ -1,5 +1,10 @@
 """Fused wgmma forward conv (mnb_fq_conv2d_fwd_tc) against the generic kernels, the standalone
-quantizer kernel (codes / STE bits must be identical) and ATen-CPU conv2d."""
+quantizer kernel (codes / STE bits must be identical) and ATen-CPU conv2d.
+
+The "tc" leg turns the packed-operand family off (L.PK_MODE = "off"): with a quantizer spec QuantConv2dFn would otherwise
+take that family first, whatever USE_TC says.  Inside the documented cover (DESIGN.md §4.1/§4.2) the leg must have run
+fwd_tc / dgrad_tc / wgrad_tc; the shapes instantiate every group width 16..160 of conv_tc_kernel, forward (K/g) and data
+gradient (C/g)."""
 import numpy as np
 import pytest
 import torch
@@ -22,19 +27,50 @@ SHAPES = [
     (2, 32, 16, 16, 32, 5, 1),       # 5x5
     (3, 48, 4, 4, 64, 1, 1),         # 4x4 images, 8 per tile
     (2, 16, 12, 12, 16, 3, 1),       # W not a power of two
+    (2, 48, 16, 16, 80, 3, 1),       # group widths: forward 80, data gradient 48
+    (2, 96, 16, 16, 112, 3, 1),      # 112 / 96
+    (2, 144, 8, 8, 48, 3, 1),        # 48 / 144
+    (2, 112, 8, 8, 144, 1, 1),       # 144 / 112
+    (2, 80, 8, 8, 96, 1, 1),         # 96 / 80
 ]
 
 
-def _run(x, wq, bias, w_int, w_scale, spec, R, G, use_tc):
+def _tc_cover(shape, which):
+    """inside the cover of the fused tensor-core kernels (DESIGN.md §4.1 / §4.2) for these stride-1 'same' shapes?"""
+    B, C, H, W, K, R, G = shape
+    if (C // G) % 16 or (K // G) % 16 or W > 64 or (W * 4) % 16:
+        return False
+    n = {"fwd": K // G, "dgrad": C // G, "wgrad": 0}[which]       # accumulator columns of the kernel instance
+    return n <= 160 and (which != "wgrad" or C // G <= 256)
+
+
+def _legs(use_tc):
+    """switch the engine to the fused tensor-core kernels (packed-operand family off) or to the generic fallback;
+    returns a restore function"""
     from micronet_b200 import _lib as L, functional as F_
+    old = (L.USE_TC, L.PK_MODE, F_.TIMER)
     L.USE_TC = use_tc
+    if use_tc:
+        L.PK_MODE = "off"
+    F_.TIMER = F_.KernelTimer()
+
+    def restore():
+        kinds = {k for k, _, _, _ in F_.TIMER.records}
+        L.USE_TC, L.PK_MODE, F_.TIMER = old
+        return kinds
+    return restore
+
+
+def _run(x, wq, bias, w_int, w_scale, spec, R, G, use_tc):
+    from micronet_b200 import functional as F_
+    restore = _legs(use_tc)
     try:
         xg = x.clone().requires_grad_(True)
         y = F_.quant_conv2d(xg, wq, bias, w_int, w_scale, spec, (1, 1), (R // 2, R // 2), (1, 1), G)
         torch.cuda.synchronize()
-        return y
     finally:
-        L.USE_TC = True
+        kinds = restore()
+    return y, kinds
 
 
 @pytest.mark.parametrize("shape", SHAPES, ids=[str(s) for s in SHAPES])
@@ -72,9 +108,12 @@ def test_tc_forward_matches_generic_and_cpu(shape, mode):
     err = L.tc_err_flag(torch.device(DEV))
     err.zero_()
     n0 = L.launch_count()
-    y_tc = _run(xd, wqd, bd, wid, wsd, spec, R, G, True)
+    y_tc, kinds = _run(xd, wqd, bd, wid, wsd, spec, R, G, True)
     assert err.item() == 0, f"tensor-core pipeline timed out, code {err.item()}"
-    y_gen = _run(xd, wqd, bd, wid, wsd, spec, R, G, False)
+    if _tc_cover(shape, "fwd"):
+        assert "fwd_tc" in kinds, kinds
+    assert not any(k.endswith("_pk") for k in kinds), kinds
+    y_gen, _ = _run(xd, wqd, bd, wid, wsd, spec, R, G, False)
     assert torch.isfinite(y_tc).all()
     # both paths are exact on integer levels; on raw fp32 they differ only by fp32 summation order
     assert rel_err(y_tc, y_gen) <= (5e-6 if mode == "raw_fp32" else 1e-6), f"tc vs generic {rel_err(y_tc, y_gen)}"
@@ -146,9 +185,9 @@ def test_tc_dgrad_matches_generic_and_cpu(shape, mode):
         spec = F_.ActSpec(L.ACT_IAO, qmin=-128, qmax=127, q_type=0, **{k: v.to(DEV) for k, v in bufs.items()})
     go = torch.randn(B, K, H, W, generator=g)
     err = L.tc_err_flag(torch.device(DEV)); err.zero_()
-    grads = {}
+    grads, kinds = {}, {}
     for use_tc in (True, False):
-        L.USE_TC = use_tc
+        restore = _legs(use_tc)
         try:
             xg = x.to(DEV).requires_grad_(True)
             y = F_.quant_conv2d(xg, wq.to(DEV), None, w_int.to(DEV), w_scale.to(DEV), spec, (1, 1), (R // 2, R // 2), (1, 1), G)
@@ -156,8 +195,11 @@ def test_tc_dgrad_matches_generic_and_cpu(shape, mode):
             torch.cuda.synchronize()
             grads[use_tc] = xg.grad.clone()
         finally:
-            L.USE_TC = True
+            kinds[use_tc] = restore()
     assert err.item() == 0, f"tensor-core pipeline timed out, code {err.item()}"
+    if _tc_cover(shape, "dgrad"):
+        assert "dgrad_tc" in kinds[True], kinds[True]
+    assert not any(k.endswith("_pk") for k in kinds[True]), kinds[True]
     assert rel_err(grads[True], grads[False]) <= 5e-6, rel_err(grads[True], grads[False])  # fp32 summation order
     # CPU: autograd of conv2d on the dequantized input
     from oracle import reference_port as O
@@ -201,9 +243,9 @@ def test_tc_wgrad_matches_generic_and_cpu(shape, mode):
         spec = F_.ActSpec(L.ACT_IAO, qmin=-128, qmax=127, q_type=0, **{k: v.to(DEV) for k, v in bufs.items()})
     go = torch.randn(B, K, H, W, generator=g)
     err = L.tc_err_flag(torch.device(DEV)); err.zero_()
-    grads = {}
+    grads, kinds = {}, {}
     for use_tc in (True, False):
-        L.USE_TC = use_tc
+        restore = _legs(use_tc)
         try:
             wg = wq.to(DEV).requires_grad_(True)
             y = F_.quant_conv2d(x.to(DEV), wg, None, w_int.to(DEV), w_scale.to(DEV), spec, (1, 1), (R // 2, R // 2), (1, 1), G)
@@ -211,8 +253,11 @@ def test_tc_wgrad_matches_generic_and_cpu(shape, mode):
             torch.cuda.synchronize()
             grads[use_tc] = wg.grad.clone()
         finally:
-            L.USE_TC = True
+            kinds[use_tc] = restore()
     assert err.item() == 0, f"tensor-core pipeline timed out, code {err.item()}"
+    if _tc_cover(shape, "wgrad") and mode != "raw_fp32":
+        assert "wgrad_tc" in kinds[True], kinds[True]
+    assert not any(k.endswith("_pk") for k in kinds[True]), kinds[True]
     assert torch.isfinite(grads[True]).all()
     assert rel_err(grads[True], grads[False]) <= 1e-5, rel_err(grads[True], grads[False])
     if mode.startswith("raw"):
