@@ -382,6 +382,36 @@ int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a,
                      const mnb_pk_post* post, int32_t* err_flag, mnb_stream_t stream);
 int mnb_quant_add_pack_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
                            const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post, mnb_stream_t stream);
+/* int8 operands for frozen inference graphs (symmetric IAO, IAO:214-240 with q_type 0): the forward conv of the family on
+ * s8 x s8 -> s32 wgmma (K32 MMAs, exact integer sums).  The result is  y = fmaf(float(sum), a_scale * n_scale[n], bias[n]),
+ * bit-identical to mnb_pk_conv on the same levels whenever its fp32 partial sums stay below 2^24, and exact (one rounding of
+ * the integer sum) above.  Cover: everything mnb_pk_conv covers in mode 0 with one piece per operand, grouped convs with
+ * C/g % 16 == 0, kg * R * S * 128 * 127 < 2^31; the quantizers must be symmetric IAO with 2..8 bits (levels in [-128, 127]),
+ * weight levels in [-127, 127].  Outside the cover every entry point returns MNB_E_UNSUPPORTED (or MNB_E_ARG for bad
+ * pointers) before launching anything.
+ *   int8 plane: pk8[b][ceil(C/16)][h][w][16] s8 levels (the byte geometry of the bf16 plane with 16 channels per 16 bytes);
+ *               phase_split: unit (h%2*2 + w%2)*ceil(C/16) + c/16 of an [H/2, W/2] tensor, as in mnb_pk_pack_act.
+ *   mnb_pk_i8_act_bytes        : bytes of one int8 plane.
+ *   mnb_pk_i8_pack_act         : fp32 NCHW [-> ReLU when relu != 0] -> int8 level plane (no STE bits: inference only).
+ *   mnb_pk_i8_conv_plan        : host only, the plan mnb_pk_i8_conv runs; same fields as mnb_pk_conv_plan_ex (CC counts
+ *                                channels: 32 per K-step).
+ *   mnb_pk_i8_wimage_bytes     : bytes of the int8 weight image (-1 outside the cover).
+ *   mnb_pk_i8_pack_weight      : i16 levels [K, C/g, R, S] -> int8 image [n-tile][group][stage][tap][c/16][n][16].
+ *   mnb_pk_i8_conv             : forward conv of an int8 plane; out may be NULL when post is given.  post: the consumer's
+ *                                plane is written as int8 (its quantizer symmetric IAO; producer and consumer channel
+ *                                offsets multiples of 16, i.e. grouped producers need K/g % 16 == 0).
+ *   mnb_quant_add_pack_i8_fwd  : mnb_quant_add_pack_fwd writing the consumer's int8 plane. */
+int64_t mnb_pk_i8_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w);
+int mnb_pk_i8_pack_act(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_act_qparams* qp,
+                       int32_t phase_split, int32_t relu, void* out_pk, mnb_stream_t stream);
+int mnb_pk_i8_conv_plan(const mnb_conv_shape* s, int32_t* out, int32_t n);
+int64_t mnb_pk_i8_wimage_bytes(const mnb_conv_shape* s);
+int mnb_pk_i8_pack_weight(const mnb_conv_shape* s, const int16_t* w_int, void* w_img, mnb_stream_t stream);
+int mnb_pk_i8_conv(const mnb_conv_shape* s, const void* a_pk, const void* w_img, const float* n_scale, const float* a_scale,
+                   float a_scale_const, const float* bias, float* out, const mnb_pk_post* post, int32_t* err_flag,
+                   mnb_stream_t stream);
+int mnb_quant_add_pack_i8_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
+                              const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post, mnb_stream_t stream);
 int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x);
 int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                  const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);

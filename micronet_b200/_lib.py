@@ -99,6 +99,13 @@ PROTOTYPES = {
     "mnb_bn_sign_pool_bwd_pack": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P]),
     "mnb_pk_conv_post": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P]),
     "mnb_quant_add_pack_fwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _ACTQ, _I, _P, C.POINTER(PkPost), _P]),
+    "mnb_pk_i8_act_bytes": (_L, [_I, _I, _I, _I]),
+    "mnb_pk_i8_pack_act": (C.c_int, [_P, _I, _I, _I, _I, _ACTQ, _I, _I, _P, _P]),
+    "mnb_pk_i8_conv_plan": (C.c_int, [_SHAPE, _P, _I]),
+    "mnb_pk_i8_wimage_bytes": (_L, [_SHAPE]),
+    "mnb_pk_i8_pack_weight": (C.c_int, [_SHAPE, _P, _P, _P]),
+    "mnb_pk_i8_conv": (C.c_int, [_SHAPE, _P, _P, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P]),
+    "mnb_quant_add_pack_i8_fwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _ACTQ, _I, _P, C.POINTER(PkPost), _P]),
     "mnb_pk_wgrad_scratch_bytes": (_L, [_SHAPE, _I, _I]),
     "mnb_pk_wgrad": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_xnor_supported": (C.c_int, [_SHAPE]),

@@ -66,6 +66,7 @@ struct Plan {
   int64_t wimg_bytes;
   int a_box_bytes, a_bytes, b_off, stage_bytes, nstage, st_log2, smem_bytes, off_stg;
   int segmented, seg_len;   // stages per accumulation segment (segmented mode)
+  int cpu;                  // channels per 16-byte unit of the operands: 8 (bf16), 16 (int8)
 };
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
@@ -86,13 +87,17 @@ static void make_pairs(int TA, int TBk, Plan& p) {
 static int unsupported(const char* why) { return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %s", why); }
 
 // mode 0: y = conv2d(x, w); mode 1: dx = conv_transpose(dy, w).  TA / TBk: term planes of the streamed / weight operand.
-static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p) {
+// cpu: channels per 16-byte operand unit - 8 for bf16 planes (K-step of 16 channels), 16 for int8 planes (K-step of 32
+// channels: one s8 K32 MMA reads the same 32 bytes per row as one bf16 K16 MMA, so every byte-level quantity below is
+// shared).  int8 plans are forward, single-product (TA = TBk = 1) and never segmented.
+static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p, int cpu = 8) {
   MNB_REQUIRE(s != nullptr, "conv shape is NULL");
   memset(&p, 0, sizeof(p));
   const int C = s->in_c, K = s->out_c, G = s->groups, H = s->in_h, W = s->in_w, R = s->ker_h, S = s->ker_w;
   MNB_REQUIRE(s->batch > 0 && C > 0 && K > 0 && H > 0 && W > 0 && G > 0 && C % G == 0 && K % G == 0 && R > 0 && S > 0,
               "bad conv shape");
   MNB_REQUIRE(TA >= 1 && TA <= 3 && TBk >= 1 && TBk <= 3, "term counts must be 1..3");
+  MNB_REQUIRE(cpu == 8 || (cpu == 16 && mode == 0 && TA == 1 && TBk == 1), "int8 plans are single-product forward plans");
   if (s->dil_h != 1 || s->dil_w != 1) return unsupported("dilation != 1");
   if (s->stride_h != s->stride_w || (s->stride_h != 1 && s->stride_h != 2)) return unsupported("stride must be 1 or 2");
   const int st = s->stride_h, ph_ = s->pad_h, pw_ = s->pad_w;
@@ -102,19 +107,23 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   if (st == 2 && ((H | W) & 1)) return unsupported("stride 2 needs even H and W");
   const int cin_g = C / G, cout_g = K / G;
   p.mode = mode; p.B = s->batch; p.G = G; p.R = R; p.S = S; p.stride = st;
-  p.TA = TA; p.TBk = TBk;
+  p.TA = TA; p.TBk = TBk; p.cpu = cpu;
   make_pairs(TA, TBk, p);
   if (mode == 0) {
     p.kg = cin_g; p.ng = cout_g; p.NOUT = K;
     p.nkph = st == 2 ? 4 : 1;
-    p.HA = H / st; p.WA = W / st; p.C8A = ceil_div(C, 8);
+    p.HA = H / st; p.WA = W / st; p.C8A = ceil_div(C, cpu);
     p.OHr = P; p.OWr = Q; p.OH = P; p.OW = Q; p.omul = 1; p.ny = 1;
   } else {
     p.kg = cout_g; p.ng = cin_g; p.NOUT = C;
     p.nkph = 1; p.HA = P; p.WA = Q; p.C8A = ceil_div(K, 8);
     p.OHr = H / st; p.OWr = W / st; p.OH = H; p.OW = W; p.omul = st; p.ny = st == 2 ? 4 : 1;
   }
-  if (G > 1 && (p.kg % 8)) return unsupported("grouped conv needs GEMM-K channels per group % 8 == 0");
+  if (G > 1 && (p.kg % cpu))
+    return unsupported(cpu == 8 ? "grouped conv needs GEMM-K channels per group % 8 == 0"
+                                : "grouped int8 conv needs GEMM-K channels per group % 16 == 0");
+  // s32 accumulators: |level| <= 128 (activations) times |level| <= 127 (symmetric weights) over kg x taps products
+  if (cpu == 16 && (int64_t)p.kg * R * S * 128 * 127 > (int64_t)INT32_MAX) return unsupported("int8 sums could overflow s32");
   // ---- taps: (k-phase, shift) of every filter tap, per output phase
   struct Tap { int kph, sh, sw, r, s; };
   Tap taps[MAXY][MAXTAP];
@@ -242,15 +251,15 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   p.n_mgroups = ceil_div(p.n_mtiles, p.MT);
   p.n_items = p.n_mgroups * p.n_ntiles * G;
   // ---- K chunking and tap groups: one stage = MT * TA boxes of CC channels + the weights of (chunk, tap group)
-  const int nk16 = ceil_div(p.kg, 16);
+  const int nk16 = ceil_div(p.kg, 2 * cpu);      // K-steps (16 bf16 / 32 int8 channels = 32 bytes per row)
   int maxtap_kph = 1;
   for (int y = 0; y < p.ny; ++y)
     for (int i = 0, run = 0; i < p.ntap[y]; ++i) {
       run = (i > 0 && taps[y][i].kph == taps[y][i - 1].kph) ? run + 1 : 1;
       maxtap_kph = std::max(maxtap_kph, run);
     }
-  const int a16 = p.MT * TA * round_up(2 * p.npos * 16, 128);     // A bytes per 16 channels (2 octets)
-  auto b16 = [&](int tg) { return TBk * tg * 2 * p.Nt * 16; };   // B bytes per 16 channels
+  const int a16 = p.MT * TA * round_up(2 * p.npos * 16, 128);     // A bytes per K-step (2 units)
+  auto b16 = [&](int tg) { return TBk * tg * 2 * p.Nt * 16; };   // B bytes per K-step
   const int stage_target = 56 * 1024;
   int TG = std::min(maxtap_kph, 25);
   while (TG > 1 && a16 + b16(TG) > stage_target) --TG;
@@ -259,8 +268,8 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
   cc16 = std::min(cc16, 16);
   p.chunks = ceil_div(nk16, cc16);
   cc16 = ceil_div(nk16, p.chunks);            // balance the chunks
-  p.CC = cc16 * 16; p.ksteps = cc16;
-  p.a_box_bytes = (p.CC / 8) * p.npos * 16;
+  p.CC = cc16 * 2 * cpu; p.ksteps = cc16;
+  p.a_box_bytes = (p.CC / cpu) * p.npos * 16;
   p.a_bytes = round_up(p.a_box_bytes, 128);
   p.b_off = p.MT * TA * p.a_bytes;
   // ---- stage templates and the weight-image layout
@@ -274,7 +283,7 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
       if (nt >= MAXTMPL) return unsupported("too many tap groups");
       Tmpl& t = p.tmpl[y][nt++];
       t.kph = taps[y][i].kph; t.tap0 = i; t.ntap = j - i;
-      t.blk_bytes = TBk * t.ntap * (p.CC / 8) * p.Nt * 16;
+      t.blk_bytes = TBk * t.ntap * (p.CC / cpu) * p.Nt * 16;
       t.blk_off = off;
       off += p.chunks * t.blk_bytes;
       max_blk = std::max(max_blk, t.blk_bytes);
@@ -319,6 +328,16 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
+}
+
+// four integer levels (exact floats in [-128, 127]) -> four s8 bytes, first in the lowest byte
+__device__ __forceinline__ uint32_t pack4_s8(float a, float b, float c, float d) {
+  return ((uint32_t)__float2int_rn(a) & 0xffu) | (((uint32_t)__float2int_rn(b) & 0xffu) << 8) |
+         (((uint32_t)__float2int_rn(c) & 0xffu) << 16) | ((uint32_t)__float2int_rn(d) << 24);
+}
+__device__ __forceinline__ uint4 pack16_s8(const float (&l)[16]) {
+  return make_uint4(pack4_s8(l[0], l[1], l[2], l[3]), pack4_s8(l[4], l[5], l[6], l[7]), pack4_s8(l[8], l[9], l[10], l[11]),
+                    pack4_s8(l[12], l[13], l[14], l[15]));
 }
 
 // fp32 NCHW -> bf16 term planes [t][b][octet][h][w][8]; one thread = one pixel of one channel octet.
@@ -390,6 +409,42 @@ __global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__
   }
 }
 
+// fp32 NCHW -> int8 level plane [b][c/16][h][w][16] of a symmetric IAO quantizer (levels in [-128, 127]): the levels of
+// pack_act_kernel<1> with one piece, stored as s8; one thread = one pixel of one 16-channel unit.  phase_split: unit index
+// (h%2 * 2 + w%2) * C16 + c/16 of a [.., H/2, W/2] plane (stride-2 consumers).  No STE bits (inference only).
+__global__ void __launch_bounds__(256) pack_act_i8_kernel(const float* __restrict__ x, int B, int C, int H, int W, int C16,
+                                                          mnb_act_qparams qp, int phase_split, int relu, uint4* __restrict__ out) {
+  const MnbActQ q = mnb_load_actq(qp);
+  const float zp = qp.zero_point ? __ldg(qp.zero_point) : 0.f;
+  const uint32_t HW = (uint32_t)H * (uint32_t)W;
+  const uint32_t plane = blockIdx.y * blockDim.y + threadIdx.y;                 // b * C16 + c16
+  if (plane >= (uint32_t)B * (uint32_t)C16) return;
+  const uint32_t b = plane / (uint32_t)C16, c16 = plane - b * (uint32_t)C16;
+  for (uint32_t pos = blockIdx.x * blockDim.x + threadIdx.x; pos < HW; pos += gridDim.x * blockDim.x) {
+    const float* src = x + ((int64_t)b * C + c16 * 16) * HW + pos;
+    float v[16], lev[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      float val = (int)c16 * 16 + j < C ? __ldg(src + (int64_t)j * HW) : 0.f;
+      if (relu) val = fmaxf(val, 0.f);
+      v[j] = val;
+    }
+    uint32_t passbits;
+    mnb_act_levels<16>(q, v, lev, passbits);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) lev[j] = (int)c16 * 16 + j < C ? lev[j] + zp : 0.f;
+    int64_t dst;
+    if (phase_split) {
+      const uint32_t h = pos / (uint32_t)W, w = pos - h * (uint32_t)W;
+      const uint32_t u = ((h & 1u) * 2u + (w & 1u)) * (uint32_t)C16 + c16;
+      dst = (((int64_t)b * 4 * C16 + u) * (H >> 1) + (h >> 1)) * (W >> 1) + (w >> 1);
+    } else {
+      dst = (int64_t)plane * HW + pos;
+    }
+    out[dst] = pack16_s8(lev);
+  }
+}
+
 // BatchNorm2d + ReLU + DoReFa activation quantizer + operand packing in ONE pass (SURVEY.md 8 f2 for the DoReFa blocks
 // conv -> nn.BatchNorm2d -> nn.ReLU -> [channel_shuffle] -> QuantConv2d, nin_gc.py:53-59 + DF:36-46): reads the conv output
 // once, writes the integer levels of the NEXT conv's activation quantizer as its packed bf16 plane (2 B / element, in the
@@ -437,8 +492,10 @@ __global__ void __launch_bounds__(256) bn_relu_quant_pack_kernel(const float* __
 }
 
 // IAO QuantAdd of a frozen inference graph + the consuming conv's quantizer and operand packing in one pass (see
-// mnb_quant_add_pack_fwd): one thread = one pixel of one channel octet, same arithmetic as quant_add_fwd_kernel
-// (mnb_quant.cu) followed by pack_act_kernel<1>.
+// mnb_quant_add_pack_fwd): one thread = one pixel of one 16-byte unit of the consumer's plane (CPU = 8 channels as bf16,
+// or 16 channels as int8 for an int8 consumer), same arithmetic as quant_add_fwd_kernel (mnb_quant.cu) followed by
+// pack_act_kernel<1> / pack_act_i8_kernel.
+template <int CPU>
 __global__ void __launch_bounds__(256) quant_add_pack_kernel(const float* __restrict__ a, const float* __restrict__ b, int B, int C,
                                                              int H, int W, int C8, mnb_act_qparams qadd, int relu,
                                                              float* __restrict__ out, mnb_act_qparams qnext, int next_relu,
@@ -450,22 +507,22 @@ __global__ void __launch_bounds__(256) quant_add_pack_kernel(const float* __rest
   if (plane >= (uint32_t)B * (uint32_t)C8) return;
   const uint32_t bi = plane / (uint32_t)C8, c8 = plane - bi * (uint32_t)C8;
   for (uint32_t pos = blockIdx.x * blockDim.x + threadIdx.x; pos < HW; pos += gridDim.x * blockDim.x) {
-    const int64_t base = ((int64_t)bi * C + c8 * 8) * HW + pos;
-    float va[8], vb[8], lev[8];
+    const int64_t base = ((int64_t)bi * C + c8 * CPU) * HW + pos;
+    float va[CPU], vb[CPU], lev[CPU];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const bool live = (int)c8 * 8 + j < C;
+    for (int j = 0; j < CPU; ++j) {
+      const bool live = (int)c8 * CPU + j < C;
       va[j] = live ? __ldg(a + base + (int64_t)j * HW) : 0.f;
       vb[j] = live ? __ldg(b + base + (int64_t)j * HW) : 0.f;
     }
     // Q(a), Q(b): the level as a float (IAO: clamp(round(x/s - zp)), value = (level + zp) * s; DoReFa: value = level * s)
-    float la[8], lb[8], sum[8];
+    float la[CPU], lb[CPU], sum[CPU];
     uint32_t pbits;
-    mnb_act_levels<8>(q, va, la, pbits);
-    mnb_act_levels<8>(q, vb, lb, pbits);
+    mnb_act_levels<CPU>(q, va, la, pbits);
+    mnb_act_levels<CPU>(q, vb, lb, pbits);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const bool live = (int)c8 * 8 + j < C;
+    for (int j = 0; j < CPU; ++j) {
+      const bool live = (int)c8 * CPU + j < C;
       float oa, ob;
       if (q.mode == MNB_ACT_DOREFA) { oa = __fmul_rn(la[j], q.s); ob = __fmul_rn(lb[j], q.s); }
       else { oa = __fmul_rn(__fadd_rn(la[j], q.zp), q.s); ob = __fmul_rn(__fadd_rn(lb[j], q.zp), q.s); }
@@ -474,9 +531,9 @@ __global__ void __launch_bounds__(256) quant_add_pack_kernel(const float* __rest
       if (live) out[base + (int64_t)j * HW] = t;
       sum[j] = next_relu ? fmaxf(t, 0.f) : t;
     }
-    mnb_act_levels<8>(qn, sum, lev, pbits);
+    mnb_act_levels<CPU>(qn, sum, lev, pbits);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) lev[j] = ((int)c8 * 8 + j < C) ? lev[j] + zpn : 0.f;
+    for (int j = 0; j < CPU; ++j) lev[j] = ((int)c8 * CPU + j < C) ? lev[j] + zpn : 0.f;
     int64_t dst;
     if (phase_split) {
       const uint32_t h = pos / (uint32_t)W, w = pos - h * (uint32_t)W;
@@ -485,7 +542,8 @@ __global__ void __launch_bounds__(256) quant_add_pack_kernel(const float* __rest
     } else {
       dst = (int64_t)plane * HW + pos;
     }
-    out_pk[dst] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]), pack2(lev[6], lev[7]));
+    if constexpr (CPU == 16) out_pk[dst] = pack16_s8(lev);
+    else out_pk[dst] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]), pack2(lev[6], lev[7]));
   }
 }
 
@@ -639,7 +697,9 @@ struct PackWParams {
   int cin_g, cout_g;
 };
 
-// weights (int16 levels or fp32) -> bf16 image of the plan; one thread = one 16-byte vector (8 GEMM-K channels)
+// weights (int16 levels or fp32) -> bf16 image of the plan; one thread = one 16-byte vector (8 GEMM-K channels).
+// CPU = 16: int16 levels in [-127, 127] -> int8 image [n-tile][group][stage][tap][c/16][n][16] (16 GEMM-K channels per vector).
+template <int CPU>
 __global__ void __launch_bounds__(256) pack_weight_kernel(const __grid_constant__ PackWParams pp, uint4* __restrict__ out) {
   const Plan& p = pp.pl;
   const int64_t total = p.wimg_bytes / 16;
@@ -660,7 +720,7 @@ __global__ void __launch_bounds__(256) pack_weight_kernel(const __grid_constant_
     rem -= tp.blk_off;
     const int cc = rem / tp.blk_bytes;
     rem -= cc * tp.blk_bytes;
-    const int per_tap = (p.CC / 8) * p.Nt * 16, per_term = tp.ntap * per_tap;
+    const int per_tap = (p.CC / CPU) * p.Nt * 16, per_term = tp.ntap * per_tap;
     const int term = rem / per_term;
     rem -= term * per_term;
     const int tapi = rem / per_tap;
@@ -668,10 +728,10 @@ __global__ void __launch_bounds__(256) pack_weight_kernel(const __grid_constant_
     const int c8l = rem / (p.Nt * 16), n = (rem - c8l * (p.Nt * 16)) / 16;
     const int r = p.tap_r[y][tp.tap0 + tapi], s = p.tap_s[y][tp.tap0 + tapi];
     const int nn = nt * p.Nt + n;                 // GEMM-N channel within the group
-    float val[8];
+    float val[CPU];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int kk = cc * p.CC + c8l * 8 + e;     // GEMM-K channel within the group
+    for (int e = 0; e < CPU; ++e) {
+      const int kk = cc * p.CC + c8l * CPU + e;   // GEMM-K channel within the group
       float x = 0.f;
       if (kk < p.kg && nn < p.ng) {
         int64_t src;
@@ -683,16 +743,20 @@ __global__ void __launch_bounds__(256) pack_weight_kernel(const __grid_constant_
       }
       val[e] = x;
     }
-    uint32_t pk4[4];
-    for (int tm = 0; tm <= term; ++tm) {
+    if constexpr (CPU == 16) {
+      out[v] = pack16_s8(val);
+    } else {
+      uint32_t pk4[4];
+      for (int tm = 0; tm <= term; ++tm) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        pk4[j] = pack2(val[2 * j], val[2 * j + 1]);
-        val[2 * j] -= __uint_as_float(pk4[j] << 16);
-        val[2 * j + 1] -= __uint_as_float(pk4[j] & 0xffff0000u);
+        for (int j = 0; j < 4; ++j) {
+          pk4[j] = pack2(val[2 * j], val[2 * j + 1]);
+          val[2 * j] -= __uint_as_float(pk4[j] << 16);
+          val[2 * j + 1] -= __uint_as_float(pk4[j] & 0xffff0000u);
+        }
       }
+      out[v] = make_uint4(pk4[0], pk4[1], pk4[2], pk4[3]);
     }
-    out[v] = make_uint4(pk4[0], pk4[1], pk4[2], pk4[3]);
   }
 }
 
@@ -727,7 +791,8 @@ struct ConvParams {
   float gain;               // dgrad: factor on passed gradients (DoReFa 0.1)
   float* out;               // fp32 NCHW result, or NULL when only the packed output below is wanted
   // fused consumer (inference graphs): the epilogue also applies [ReLU +] the NEXT conv's activation quantizer and writes
-  // that conv's operand plane [b][c/8][h][w][8] bf16 (space-to-depth phase planes for a stride-2 consumer)
+  // that conv's operand plane [b][c/8][h][w][8] bf16, or [b][c/16][h][w][16] int8 in the int8 kernels (space-to-depth
+  // phase planes for a stride-2 consumer; C8O = 16-byte units per position)
   uint4* post_out;
   mnb_act_qparams post_q;
   int post_relu, post_split;
@@ -763,7 +828,9 @@ constexpr int kConvThreads = 384;   // warp 0 TMA, warps 4..11 two MMA + epilogu
 // at most seg_len stages starts from zero and is added into running sums with round-to-nearest fp32 adds.
 // Epilogue: 32 accumulator columns at a time through a 128 x 32 staging tile; thread et of the 256 then owns position
 // (et % 128) of the tile raster and one 16-column slot (et / 128) of the two.
-template <bool SEG, int NT>
+// I8: int8 operands (16 channels per 16-byte unit, s8 K32 MMAs into s32 accumulators, exact); the sums are converted to
+// fp32 once (__int2float_rn) ahead of the same epilogue, and a consumer plane is written as int8.
+template <bool SEG, int NT, bool I8 = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1,
                const __grid_constant__ CUtensorMap tmap2, const __grid_constant__ ConvParams p) {
@@ -895,8 +962,12 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
                   if (w[k] == 0xffffffffu) continue;
-                  tc::Mma<NT>::template bf16<0, 0>(acc[mt], a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
-                                                    b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
+                  if constexpr (I8)   // s32 accumulators in the registers of acc (zero bits = 0 either way)
+                    tc::Mma<NT>::s8(reinterpret_cast<int32_t(&)[NR]>(acc[mt]), a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
+                                    b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
+                  else
+                    tc::Mma<NT>::template bf16<0, 0>(acc[mt], a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
+                                                      b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
                 }
               }
             }
@@ -922,6 +993,13 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
         for (int mt = 0; mt < MAXMT; ++mt) {
 #pragma unroll
           for (int i = 0; i < NR; ++i) rs[SEG ? mt : 0][SEG ? i : 0] = __fadd_rn(rs[SEG ? mt : 0][SEG ? i : 0], acc[mt][i]);
+        }
+      }
+      if constexpr (I8) {   // exact s32 sums -> fp32, rounded once (exact below 2^24, where the bf16 kernels agree)
+#pragma unroll
+        for (int mt = 0; mt < MAXMT; ++mt) {
+#pragma unroll
+          for (int i = 0; i < NR; ++i) acc[mt][i] = __int2float_rn(__float_as_int(acc[mt][i]));
         }
       }
       // ---- epilogue
@@ -976,11 +1054,15 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
 #pragma unroll
           for (int k = 0; k < 16; ++k) lev[k] = n0 + k < n_cnt ? lev[k] + pzp : 0.f;
           const int64_t oct_stride = p.post_split ? (int64_t)(p.OH >> 1) * (p.OW >> 1) : plane;
-          const int oc8 = (n_base + n0) >> 3;
-          uint4* dst = p.post_out + prow + (int64_t)oc8 * oct_stride;
-          dst[0] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]), pack2(lev[6], lev[7]));
-          if (n0 + 8 < n_cnt)
-            dst[oct_stride] = make_uint4(pack2(lev[8], lev[9]), pack2(lev[10], lev[11]), pack2(lev[12], lev[13]), pack2(lev[14], lev[15]));
+          if constexpr (I8) {   // one 16-channel unit (n_base + n0 is a multiple of 16: checked on the host)
+            p.post_out[prow + (int64_t)((n_base + n0) >> 4) * oct_stride] = pack16_s8(lev);
+          } else {
+            const int oc8 = (n_base + n0) >> 3;
+            uint4* dst = p.post_out + prow + (int64_t)oc8 * oct_stride;
+            dst[0] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]), pack2(lev[6], lev[7]));
+            if (n0 + 8 < n_cnt)
+              dst[oct_stride] = make_uint4(pack2(lev[8], lev[9]), pack2(lev[10], lev[11]), pack2(lev[12], lev[13]), pack2(lev[14], lev[15]));
+          }
         } else if (p.mode == 0 || !brow) {
 #pragma unroll
           for (int k = 0; k < 16; ++k, op += plane)
@@ -1382,6 +1464,55 @@ __global__ void __launch_bounds__(128) wg_reduce_kernel(const float* __restrict_
 // =========================================================================================================
 // C-ABI
 // =========================================================================================================
+// launch geometry of the packers that give one thread one position of one (image, 16-byte unit) plane: block =
+// (positions, planes), small images put several planes into one 256-thread block.  false: the planes exceed the grid.
+static bool unit_grid(int batch, int units, int hw, dim3& blocks, dim3& threads) {
+  const int tx = std::min(256, (hw + 31) / 32 * 32), ty = 256 / tx;     // threads along positions / planes per block
+  const int planes = batch * units, gy = (planes + ty - 1) / ty;
+  const int bx = std::max(1, std::min((hw + tx - 1) / tx, std::max(1, (MNB_NUM_SMS * 16) / std::max(1, gy))));
+  blocks = dim3(bx, gy); threads = dim3(tx, ty);
+  return gy <= 65535;
+}
+
+// the quantizers whose levels fit s8 (symmetric IAO, 2..8 bits): the only ones an int8 plane holds
+static bool i8_quantizer(const mnb_act_qparams* q) {
+  return q->mode == MNB_ACT_IAO && q->q_type == 0 && q->bits >= 2 && q->bits <= 8 && q->qmin >= -128 && q->qmax <= 127;
+}
+
+// mnb_quant_add_pack_fwd (CPU = 8: bf16 consumer plane) and mnb_quant_add_pack_i8_fwd (CPU = 16: int8 consumer plane)
+template <int CPU>
+static int quant_add_pack(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
+                          const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post, mnb_stream_t stream) {
+  MNB_REQUIRE(a && b && qp && out && post && post->q && post->out_pk, "NULL quant_add_pack pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad quant_add_pack shape");
+  MNB_REQUIRE(qp->mode == MNB_ACT_DOREFA || qp->mode == MNB_ACT_IAO, "QuantAdd takes a DoReFa or IAO quantizer");
+  if (CPU == 16) {
+    if (!i8_quantizer(post->q)) return mnb_fail(MNB_E_UNSUPPORTED, "int8 consumer plane needs a symmetric IAO quantizer with 2..8 bits");
+  } else {
+    MNB_REQUIRE(post->q->mode == MNB_ACT_DOREFA || post->q->mode == MNB_ACT_IAO, "consumer quantizer must be DoReFa or IAO");
+  }
+  MNB_REQUIRE(post->q->bits >= 2 && post->q->bits <= 8 && qp->bits >= 2 && qp->bits <= 8, "quantizers must have 2..8 bits");
+  MNB_REQUIRE((reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "packed tensor must be 16-byte aligned");
+  if (post->phase_split) MNB_REQUIRE(((h | w) & 1) == 0, "phase split needs even H and W");
+  const int units = (channels + CPU - 1) / CPU;
+  dim3 blocks, threads;
+  if (!unit_grid(batch, units, h * w, blocks, threads))
+    return mnb_fail(MNB_E_UNSUPPORTED, "quant_add_pack: %d (image, unit) planes exceed the grid", batch * units);
+  pk::quant_add_pack_kernel<CPU><<<blocks, threads, 0, (cudaStream_t)stream>>>(
+      a, b, batch, channels, h, w, units, *qp, relu, out, *post->q, post->relu, post->phase_split,
+      reinterpret_cast<uint4*>(post->out_pk));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+// the first min(n, 21) fields of mnb_pk_conv_plan_ex / mnb_pk_i8_conv_plan
+static void plan_fields(const pk::Plan& p, int32_t* out, int32_t n) {
+  const int v[21] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
+                     p.smem_bytes, p.MT * p.Nt, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny,
+                     p.segmented, p.segmented ? p.seg_len : 0, p.npairs, p.col_tiles, p.n_mgroups};
+  for (int i = 0; i < std::min(n, 21); ++i) out[i] = v[i];
+}
+
 extern "C" int64_t mnb_pk_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t terms) {
   return (int64_t)terms * batch * ((channels + 7) / 8) * h * w * 16;
 }
@@ -1402,12 +1533,9 @@ extern "C" int mnb_pk_pack_act_relu(const float* x, int32_t batch, int32_t chann
   const int C8 = (channels + 7) / 8;
   const int64_t plane_vecs = (int64_t)batch * C8 * h * w;
   MNB_REQUIRE((int64_t)batch * C8 <= 65535 * 8 && (int64_t)h * w < (1ll << 31), "pk_pack_act: too many (image, octet) planes");
-  const int hw = h * w;
-  const int tx = std::min(256, (hw + 31) / 32 * 32), ty = 256 / tx;     // threads along positions / planes per block
-  const int planes = batch * C8, gy = (planes + ty - 1) / ty;
-  const int bx = std::max(1, std::min((hw + tx - 1) / tx, std::max(1, (MNB_NUM_SMS * 16) / std::max(1, gy))));
-  if (gy > 65535) return mnb_fail(MNB_E_UNSUPPORTED, "pk_pack_act: %d (image, octet) planes exceed the grid", planes);
-  const dim3 blocks(bx, gy), threads(tx, ty);
+  dim3 blocks, threads;
+  if (!unit_grid(batch, C8, h * w, blocks, threads))
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_pack_act: %d (image, octet) planes exceed the grid", batch * C8);
   cudaStream_t st = (cudaStream_t)stream;
   if (qp) {
     MNB_REQUIRE(qp->mode == MNB_ACT_DOREFA || qp->mode == MNB_ACT_IAO || qp->mode == MNB_ACT_SIGN, "unknown activation quantizer");
@@ -1479,24 +1607,7 @@ extern "C" int mnb_bn_sign_pool_bwd_pack(const float* g, const uint32_t* pass_bi
 extern "C" int mnb_quant_add_pack_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
                                       const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post,
                                       mnb_stream_t stream) {
-  MNB_REQUIRE(a && b && qp && out && post && post->q && post->out_pk, "NULL quant_add_pack pointer");
-  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad quant_add_pack shape");
-  MNB_REQUIRE(qp->mode == MNB_ACT_DOREFA || qp->mode == MNB_ACT_IAO, "QuantAdd takes a DoReFa or IAO quantizer");
-  MNB_REQUIRE(post->q->mode == MNB_ACT_DOREFA || post->q->mode == MNB_ACT_IAO, "consumer quantizer must be DoReFa or IAO");
-  MNB_REQUIRE(post->q->bits >= 2 && post->q->bits <= 8 && qp->bits >= 2 && qp->bits <= 8, "quantizers must have 2..8 bits");
-  MNB_REQUIRE((reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "packed tensor must be 16-byte aligned");
-  if (post->phase_split) MNB_REQUIRE(((h | w) & 1) == 0, "phase split needs even H and W");
-  const int C8 = (channels + 7) / 8;
-  const int hw = h * w;
-  const int tx = std::min(256, (hw + 31) / 32 * 32), ty = 256 / tx;
-  const int planes = batch * C8, gy = (planes + ty - 1) / ty;
-  const int bx = std::max(1, std::min((hw + tx - 1) / tx, std::max(1, (MNB_NUM_SMS * 16) / std::max(1, gy))));
-  if (gy > 65535) return mnb_fail(MNB_E_UNSUPPORTED, "quant_add_pack: %d (image, octet) planes exceed the grid", planes);
-  pk::quant_add_pack_kernel<<<dim3(bx, gy), dim3(tx, ty), 0, (cudaStream_t)stream>>>(
-      a, b, batch, channels, h, w, C8, *qp, relu, out, *post->q, post->relu, post->phase_split,
-      reinterpret_cast<uint4*>(post->out_pk));
-  MNB_LAUNCHED(1);
-  return 0;
+  return quant_add_pack<8>(a, b, batch, channels, h, w, qp, relu, out, post, stream);
 }
 
 extern "C" int mnb_bn_relu_quant_pack_fwd(const float* x, int32_t batch, int32_t channels, int32_t hw, const float* mean,
@@ -1526,12 +1637,7 @@ extern "C" int mnb_pk_conv_plan_ex(const mnb_conv_shape* s, int32_t mode, int32_
                                    int32_t n) {
   pk::Plan p;
   if (int e = pk::make_plan(s, mode, terms_a, terms_w, p)) return e;
-  if (out) {
-    const int v[21] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
-                       p.smem_bytes, p.MT * p.Nt, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny,
-                       p.segmented, p.segmented ? p.seg_len : 0, p.npairs, p.col_tiles, p.n_mgroups};
-    for (int i = 0; i < std::min(n, 21); ++i) out[i] = v[i];
-  }
+  if (out) plan_fields(p, out, n);
   return 0;
 }
 
@@ -1556,7 +1662,7 @@ extern "C" int mnb_pk_pack_weight(const mnb_conv_shape* s, int32_t mode, int32_t
   pp.cin_g = s->in_c / s->groups; pp.cout_g = s->out_c / s->groups;
   const int64_t vecs = pp.pl.wimg_bytes / 16;
   const int blocks = (int)std::min<int64_t>((vecs + 255) / 256, (int64_t)MNB_NUM_SMS * 8);
-  pk::pack_weight_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(pp, reinterpret_cast<uint4*>(w_img));
+  pk::pack_weight_kernel<8><<<blocks, 256, 0, (cudaStream_t)stream>>>(pp, reinterpret_cast<uint4*>(w_img));
   MNB_LAUNCHED(1);
   return 0;
 }
@@ -1564,11 +1670,18 @@ extern "C" int mnb_pk_pack_weight(const mnb_conv_shape* s, int32_t mode, int32_t
 static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
                         int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
                         const float* bias, const uint8_t* bits8, float gain, float* out, const mnb_pk_post* post,
-                        int32_t* err_flag, mnb_stream_t stream) {
+                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8) {
   using namespace pk;
   MNB_REQUIRE(s && a_pk && w_img && (out || post) && err_flag, "NULL pk_conv pointer");
   Plan pl;
-  if (int e = make_plan(s, mode, terms_a, terms_w, pl)) return e;
+  if (int e = make_plan(s, mode, terms_a, terms_w, pl, cpu)) return e;
+  if (post && cpu == 16) {   // int8 consumer plane: s8 levels of a symmetric IAO quantizer, 16-channel units
+    MNB_REQUIRE(post->q && post->out_pk && (reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "pk conv: consumer plane / quantizer");
+    if (post->q->mode != MNB_ACT_IAO || post->q->q_type != 0 || post->q->bits < 2 || post->q->bits > 8 || post->q->qmin < -128 ||
+        post->q->qmax > 127)
+      return unsupported("int8 consumer plane needs a symmetric IAO quantizer with 2..8 bits");
+    if (pl.G > 1 && (pl.ng % 16)) return unsupported("int8 consumer plane of a grouped conv needs channels per group % 16 == 0");
+  }
   if (post) {
     MNB_REQUIRE(mode == 0 && !bits8, "pk conv: a fused consumer is a forward-only (inference) option");
     MNB_REQUIRE(post->q && post->out_pk && (reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "pk conv: consumer plane / quantizer");
@@ -1587,7 +1700,7 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   m.n_items = pl.n_items; m.chunks = pl.chunks; m.ksteps = pl.ksteps; m.MT = pl.MT; m.Nt = pl.Nt; m.npairs = pl.npairs;
   m.st_mask = pl.nstage - 1; m.st_log2 = pl.st_log2; m.stage16 = pl.stage_bytes >> 4;
   m.a_term16 = pl.a_bytes >> 4; m.a_mt16 = (pl.TA * pl.a_bytes) >> 4; m.a_k16 = 2 * pl.npos;
-  m.b_off16 = pl.b_off >> 4; m.b_tap16 = (pl.CC / 8) * pl.Nt; m.b_k16 = 2 * pl.Nt;
+  m.b_off16 = pl.b_off >> 4; m.b_tap16 = (pl.CC / cpu) * pl.Nt; m.b_k16 = 2 * pl.Nt;
   m.a_lbo = (uint32_t)pl.npos * 16u; m.b_lbo = (uint32_t)pl.Nt * 16u;
   m.seg_len = (uint32_t)pl.seg_len;
   int nprog = 0;
@@ -1614,13 +1727,13 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     p.img_bytes[y] = pl.img_bytes[y]; p.y_off[y] = pl.y_off[y];
   }
   p.n_items = pl.n_items; p.n_ntiles = pl.n_ntiles; p.G = pl.G; p.MT = pl.MT; p.TA = pl.TA; p.chunks = pl.chunks;
-  p.CC8 = pl.CC / 8; p.C8A = pl.C8A; p.kg8 = pl.kg / 8; p.stage_bytes = pl.stage_bytes; p.a_bytes = pl.a_bytes;
+  p.CC8 = pl.CC / cpu; p.C8A = pl.C8A; p.kg8 = pl.kg / cpu; p.stage_bytes = pl.stage_bytes; p.a_bytes = pl.a_bytes;
   p.a_box_bytes = pl.a_box_bytes; p.b_off = pl.b_off; p.st_mask = pl.nstage - 1; p.st_log2 = pl.st_log2;
   p.Wt = pl.Wt; p.TH = pl.TH; p.TB = pl.TB; p.wlo = pl.wlo; p.hlo = pl.hlo; p.col_tiles = pl.col_tiles; p.row_tiles = pl.row_tiles;
   p.n_mtiles = pl.n_mtiles;
   p.w_img = reinterpret_cast<const uint8_t*>(w_img);
   p.B = pl.B; p.THH = pl.THH; p.BW = pl.BW; p.OHr = pl.OHr; p.OWr = pl.OWr; p.OH = pl.OH; p.OW = pl.OW; p.omul = pl.omul; p.ny = pl.ny;
-  p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = (pl.NOUT + 7) / 8; p.smem_bytes = pl.smem_bytes; p.off_stg = pl.off_stg;
+  p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = ceil_div(pl.NOUT, cpu); p.smem_bytes = pl.smem_bytes; p.off_stg = pl.off_stg;
   p.mode = mode;
   p.n_scale = n_scale; p.a_scale = a_scale; p.a_scale_const = a_scale_const; p.bias = bias; p.bits8 = bits8; p.gain = gain;
   p.out = out; p.err = err_flag;
@@ -1633,20 +1746,20 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   const int64_t plane_bytes = (int64_t)pl.B * C8tot * pl.HA * pl.WA * 16;
   for (int t = 0; t < 3; ++t) {
     const int tt = t < pl.TA ? t : 0;
-    if (int e = make_pk_tmap(&tm[t], a_pk, plane_bytes, tt, pl.B, C8tot, pl.HA, pl.WA, pl.BW, pl.THH, pl.TB, pl.CC / 8)) return e;
+    if (int e = make_pk_tmap(&tm[t], a_pk, plane_bytes, tt, pl.B, C8tot, pl.HA, pl.WA, pl.BW, pl.THH, pl.TB, pl.CC / cpu)) return e;
   }
   if (pl.n_items >= (1 << 22) || pl.n_mtiles >= (1 << 22))     // FastDiv's exact range (fp32 reciprocal + one correction step)
     return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
   const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
   using ConvFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
-#define MNB_PK_CONV_FNS(SEG) {pk_conv_kernel<SEG, 16>, pk_conv_kernel<SEG, 32>, pk_conv_kernel<SEG, 48>, \
-                              pk_conv_kernel<SEG, 64>, pk_conv_kernel<SEG, 96>, pk_conv_kernel<SEG, 128>}
-  static const ConvFn fns[2][6] = {MNB_PK_CONV_FNS(false), MNB_PK_CONV_FNS(true)};
+#define MNB_PK_CONV_FNS(SEG, I8) {pk_conv_kernel<SEG, 16, I8>, pk_conv_kernel<SEG, 32, I8>, pk_conv_kernel<SEG, 48, I8>, \
+                                  pk_conv_kernel<SEG, 64, I8>, pk_conv_kernel<SEG, 96, I8>, pk_conv_kernel<SEG, 128, I8>}
+  static const ConvFn fns[3][6] = {MNB_PK_CONV_FNS(false, false), MNB_PK_CONV_FNS(true, false), MNB_PK_CONV_FNS(false, true)};
 #undef MNB_PK_CONV_FNS
   int ki = -1;
   for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
   if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
-  const ConvFn fn = fns[pl.segmented ? 1 : 0][ki];
+  const ConvFn fn = fns[cpu == 16 ? 2 : (pl.segmented ? 1 : 0)][ki];
   if (int e = set_max_smem(fn, kSmemBudget)) return e;
   fn<<<dim3(gx, pl.ny), kConvThreads, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
   MNB_LAUNCHED(1);
@@ -1668,6 +1781,70 @@ extern "C" int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32
   MNB_REQUIRE(post, "NULL consumer description");
   return pk_conv_impl(s, 0, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, out, post,
                       err_flag, stream);
+}
+
+// ---- int8 operands (inference): symmetric IAO levels as s8, s8 x s8 -> s32 wgmma
+
+extern "C" int64_t mnb_pk_i8_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w) {
+  return (int64_t)batch * ((channels + 15) / 16) * h * w * 16;
+}
+
+extern "C" int mnb_pk_i8_pack_act(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_act_qparams* qp,
+                                  int32_t phase_split, int32_t relu, void* out_pk, mnb_stream_t stream) {
+  MNB_REQUIRE(x && qp && out_pk, "NULL pk_i8_pack_act pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad pk_i8_pack_act arguments");
+  MNB_REQUIRE((reinterpret_cast<uintptr_t>(out_pk) & 15) == 0, "packed tensor must be 16-byte aligned");
+  if (!i8_quantizer(qp)) return mnb_fail(MNB_E_UNSUPPORTED, "int8 plane needs a symmetric IAO quantizer with 2..8 bits");
+  if (phase_split) MNB_REQUIRE(((h | w) & 1) == 0, "phase split needs even H and W");
+  MNB_REQUIRE((int64_t)h * w < (1ll << 31), "pk_i8_pack_act: plane too large");
+  const int C16 = (channels + 15) / 16;
+  dim3 blocks, threads;
+  if (!unit_grid(batch, C16, h * w, blocks, threads))
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_i8_pack_act: %d (image, unit) planes exceed the grid", batch * C16);
+  pk::pack_act_i8_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(x, batch, channels, h, w, C16, *qp, phase_split,
+                                                                               relu, reinterpret_cast<uint4*>(out_pk));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int mnb_pk_i8_conv_plan(const mnb_conv_shape* s, int32_t* out, int32_t n) {
+  pk::Plan p;
+  if (int e = pk::make_plan(s, 0, 1, 1, p, 16)) return e;
+  if (out) plan_fields(p, out, n);
+  return 0;
+}
+
+extern "C" int64_t mnb_pk_i8_wimage_bytes(const mnb_conv_shape* s) {
+  pk::Plan p;
+  if (pk::make_plan(s, 0, 1, 1, p, 16)) return -1;
+  return p.wimg_bytes;
+}
+
+extern "C" int mnb_pk_i8_pack_weight(const mnb_conv_shape* s, const int16_t* w_int, void* w_img, mnb_stream_t stream) {
+  MNB_REQUIRE(w_int, "NULL pk_i8_pack_weight levels");
+  MNB_REQUIRE(w_img && (reinterpret_cast<uintptr_t>(w_img) & 15) == 0, "weight image must be 16-byte aligned");
+  pk::PackWParams pp;
+  if (int e = pk::make_plan(s, 0, 1, 1, pp.pl, 16)) return e;
+  pp.w_int = w_int; pp.w_f32 = nullptr; pp.kzero = nullptr;
+  pp.cin_g = s->in_c / s->groups; pp.cout_g = s->out_c / s->groups;
+  const int64_t vecs = pp.pl.wimg_bytes / 16;
+  const int blocks = (int)std::min<int64_t>((vecs + 255) / 256, (int64_t)MNB_NUM_SMS * 8);
+  pk::pack_weight_kernel<16><<<blocks, 256, 0, (cudaStream_t)stream>>>(pp, reinterpret_cast<uint4*>(w_img));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int mnb_pk_i8_conv(const mnb_conv_shape* s, const void* a_pk, const void* w_img, const float* n_scale,
+                              const float* a_scale, float a_scale_const, const float* bias, float* out, const mnb_pk_post* post,
+                              int32_t* err_flag, mnb_stream_t stream) {
+  MNB_REQUIRE(out || post, "pk_i8_conv: NULL out needs a consumer plane (post)");
+  return pk_conv_impl(s, 0, a_pk, 1, w_img, 1, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, out, post, err_flag, stream, 16);
+}
+
+extern "C" int mnb_quant_add_pack_i8_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
+                                         const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post,
+                                         mnb_stream_t stream) {
+  return quant_add_pack<16>(a, b, batch, channels, h, w, qp, relu, out, post, stream);
 }
 
 extern "C" int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x) {

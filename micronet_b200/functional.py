@@ -722,12 +722,22 @@ def conv_transpose2d(x, w, bias, stride, padding, output_padding, groups, dilati
 # --------------------------------------------------------------------------
 class Consumer:
     """the quantized conv that reads a producer's output next (set up by iao.freeze_inference): its frozen activation
-    quantizer, the nn.ReLU in between (folded away), its geometry, and whether anybody else needs the fp32 tensor"""
+    quantizer, the nn.ReLU in between (folded away), its geometry, whether anybody else needs the fp32 tensor, and
+    whether it was frozen with int8 operands (``int8``: then ``format`` tells which plane it reads)"""
 
-    def __init__(self, module, spec, relu, only, w_shape, stride, padding, dilation, groups, int_weights):
+    def __init__(self, module, spec, relu, only, w_shape, stride, padding, dilation, groups, int_weights, int8=False):
         self.module, self.spec, self.relu, self.only = module, spec, bool(relu), bool(only)
         self.w_shape, self.stride, self.padding, self.dilation, self.groups = w_shape, stride, padding, dilation, groups
-        self.int_weights = int_weights
+        self.int_weights, self.int8 = int_weights, bool(int8)
+
+    def format(self, act_shape):
+        """operand plane the consumer's forward reads for this activation: "i8" (int8 conv), "bf16" (packed-operand conv
+        with a one-piece plane) or None (a producer cannot write its operand).  frozen_conv takes the same decision."""
+        if self.int8 and act_shape[1] == self.w_shape[1] * self.groups:
+            sh = _shape_struct(act_shape, self.w_shape, self.stride, self.padding, self.dilation, self.groups)
+            if _i8_route(self.spec, self.int_weights, sh):
+                return "i8"
+        return "bf16" if self.accepts(act_shape) else None
 
     def accepts(self, act_shape):
         """will the consumer's forward run on the packed-operand family with a one-piece plane of this activation?"""
@@ -757,24 +767,50 @@ def handed_plane(module, x):
     return None
 
 
-def _tag(y, consumer, plane):
-    y._mnb_pk_pre = (consumer.module, plane, y._version)
+def _tag(y, consumer, plane, fmt="bf16"):
+    y._mnb_pk_pre = (consumer.module, plane, y._version, fmt)
     return y
 
 
+def _i8_route(spec, w_int, sh):
+    """does a conv frozen with int8=True run this forward on the int8 kernels?  Symmetric IAO activations with 2..8 bits
+    and levels in [-128, 127] (the quantizer test of the C side: an asymmetric quantizer reports q_type 0 until its first
+    update_qparams, its level range tells), integer weights (the module checks they are symmetric with 2..8 bits) and a
+    shape the int8 plan takes; everything else keeps the bf16 path."""
+    from . import pk as PK
+    return (spec is not None and bool(w_int is not None) and spec.mode == L.ACT_IAO and spec.q_type == 0 and 2 <= spec.bits <= 8
+            and -128 <= spec.qmin and spec.qmax <= 127 and L.PK_MODE != "off" and PK.i8_supported(sh))
+
+
+def _i8_producer_writes_plane(out_channels, groups):
+    """can an int8 conv's epilogue write its consumer's int8 plane?  It stores whole 16-channel units, so every N tile
+    must start on one: a grouped producer needs output channels per group % 16 == 0 (mnb_pk_i8_conv refuses others)"""
+    return groups == 1 or (out_channels // groups) % 16 == 0
+
+
 @torch.no_grad()
-def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, consumer=None):
+def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, consumer=None,
+                int8=False):
     """eval forward of a frozen quantized conv.  ``plane``: operand plane its producer already wrote (x holds no data
-    then); ``consumer``: write the next conv's plane from the epilogue (mnb_pk_conv_post)."""
+    then); ``consumer``: write the next conv's plane from the epilogue (mnb_pk_conv_post); ``int8``: the module was frozen
+    with int8 operands (the int8 kernels run where _i8_route allows)."""
     from . import pk as PK
     stride, padding, dilation = tuple(stride), tuple(padding), tuple(dilation)
     sh = _shape_struct(x.shape, wq.shape, stride, padding, dilation, groups)
     p, q = _out_hw(sh)
     out_shape = (x.shape[0], wq.shape[0], p, q)
+    fmt = "i8" if int8 and _i8_route(spec, w_int, sh) else "bf16"
+    if plane is not None and x._mnb_pk_pre[3] != fmt:
+        raise RuntimeError(f"micronet_b200: a {x._mnb_pk_pre[3]} operand plane reached a conv that reads {fmt}")
+    # a producer hands its consumer a plane only when both run the same format; otherwise the consumer packs its own
+    cfmt = consumer.format(out_shape) if consumer is not None else None
+    if fmt == "i8":
+        hand = cfmt == "i8" and _i8_producer_writes_plane(wq.shape[0], groups)
+        return _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_relu, consumer if hand else None)
     ta, tw = _pk_terms(spec, w_int)
     # a segmented producer plan (two level pieces of an asymmetric quantizer) takes no fused consumer: the consumer packs
     # its own operand from y
-    fused = consumer is not None and consumer.accepts(out_shape) and not PK.segmented(sh, 0, ta, tw)
+    fused = cfmt == "bf16" and not PK.segmented(sh, 0, ta, tw)
     if (plane is None and not fused) or spec is None or w_int is None or L.PK_MODE == "off" or not PK.supported(sh, 0, ta, tw):
         if plane is not None:
             raise RuntimeError("micronet_b200: handed-over plane in front of a conv outside the packed-operand cover")
@@ -808,10 +844,41 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
     return _tag(y, consumer, cplane)
 
 
+def _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_relu, consumer):
+    """frozen_conv on the int8 kernels (mnb_pk_i8_*); ``consumer``: an int8 consumer whose plane the epilogue writes"""
+    from . import pk as PK
+    dev = w_int.device
+    if plane is None:
+        L.require_cuda(x, w_int)
+        plane = PK.pack_act_i8(x.contiguous(), spec.struct(), phase_split=sh.stride_h == 2, relu=pre_relu)
+    cache = getattr(w_int, "_mnb_pk_cache", None)
+    ckey = (PK._key(sh), "i8")
+    w_img = cache.get(ckey) if cache is not None else None
+    if w_img is None:
+        w_img = PK.pack_weight_i8(sh, w_int)
+        if cache is not None:
+            cache[ckey] = w_img
+    if consumer is None:
+        y = torch.empty(out_shape, dtype=torch.float32, device=dev)
+        L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=spec.scale, bias=bias)),
+                "pk_i8_conv")
+        return y
+    y = None if consumer.only else torch.empty(out_shape, dtype=torch.float32, device=dev)
+    cplane = PK.consumer_plane_i8(*out_shape, dev)
+    post = (consumer.spec.struct(), cplane, consumer.relu, consumer.split)
+    L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=spec.scale, bias=bias,
+                                                       post=post)), "pk_i8_conv")
+    if y is None:
+        y = torch.empty(out_shape, dtype=torch.float32, device="meta")
+    return _tag(y, consumer, cplane, "i8")
+
+
 @torch.no_grad()
 def frozen_quant_add(a, b, spec, relu, consumer=None):
-    """eval forward of a frozen QuantAdd; with a ``consumer`` the kernel also writes the next conv's operand plane"""
-    if consumer is None or not consumer.accepts(tuple(a.shape)) or a.dim() != 4:
+    """eval forward of a frozen QuantAdd; with a ``consumer`` the kernel also writes the next conv's operand plane, in the
+    format that conv reads (bf16 or int8)"""
+    cfmt = consumer.format(tuple(a.shape)) if consumer is not None and a.dim() == 4 else None
+    if cfmt is None:
         return QuantAddFn.apply(a, b, spec, relu)
     from . import pk as PK
     L.require_cuda(a, b)
@@ -819,13 +886,14 @@ def frozen_quant_add(a, b, spec, relu, consumer=None):
     a, b = a.contiguous(), b.contiguous()
     assert a.shape == b.shape, "QuantAdd: operand shapes differ"
     out = torch.empty_like(a)
-    cplane = PK.consumer_plane(*a.shape, a.device)
+    i8 = cfmt == "i8"
+    cplane = (PK.consumer_plane_i8 if i8 else PK.consumer_plane)(*a.shape, a.device)
     qp, cqp = spec.struct(), consumer.spec.struct()
     post = L.PkPost(C.pointer(cqp), 1 if (consumer.relu and not relu) else 0, 1 if consumer.split else 0, cplane.data_ptr())
-    L.check(lib.mnb_quant_add_pack_fwd(a.data_ptr(), b.data_ptr(), a.shape[0], a.shape[1], a.shape[2], a.shape[3],
-                                       C.byref(qp), 1 if relu else 0, out.data_ptr(), C.byref(post), L.stream()),
-            "quant_add_pack_fwd")
-    return _tag(out, consumer, cplane)
+    fn = lib.mnb_quant_add_pack_i8_fwd if i8 else lib.mnb_quant_add_pack_fwd
+    L.check(fn(a.data_ptr(), b.data_ptr(), a.shape[0], a.shape[1], a.shape[2], a.shape[3], C.byref(qp), 1 if relu else 0,
+               out.data_ptr(), C.byref(post), L.stream()), "quant_add_pack_i8_fwd" if i8 else "quant_add_pack_fwd")
+    return _tag(out, consumer, cplane, cfmt)
 
 
 def quant_linear(x, wq, bias, w_int, w_scale, spec):

@@ -239,6 +239,13 @@ def _weight_quantizer(w_bits, q_type, q_level, weight_observer, out_channels, qa
     return cls(bits=w_bits, observer=observer, activation_weight_flag=0, qaft=qaft)
 
 
+def _int8_ok(conv):
+    """was ``conv`` frozen with int8=True, with integer weights that fit s8 (symmetric, 2..8 bits)?  Its activation
+    quantizer and shape are checked per call (functional._i8_route)."""
+    wq = conv.weight_quantizer
+    return bool(conv.__dict__.get("_int8", False)) and not conv.quant_inference and wq.symmetric and 2 <= wq.bits <= 8
+
+
 def _consumer_of(producer):
     """F_.Consumer for the conv that freeze_inference linked behind ``producer`` (None without a link)"""
     link = producer.__dict__.get("_post_consumer")
@@ -251,7 +258,7 @@ def _consumer_of(producer):
     if aq.bits == 32 or wq.bits == 32 or not wq.symmetric:
         return None
     return F_.Consumer(nxt, aq.act_spec(), nxt.__dict__.get("_pre_relu", False), only, tuple(nxt.weight.shape), tuple(nxt.stride),
-                       tuple(nxt.padding), tuple(nxt.dilation), nxt.groups, True)
+                       tuple(nxt.padding), tuple(nxt.dilation), nxt.groups, True, int8=_int8_ok(nxt))
 
 
 # ********************* quantized conv / linear *********************
@@ -306,7 +313,7 @@ class QuantConv2d(nn.Conv2d):
         spec = aq.act_spec() if plane is not None else aq.prepare_activation(input)
         return F_.frozen_conv(input, plane, wq, bias, w_int, w_scale, spec, self.stride, self.padding, self.dilation,
                               self.groups, pre_relu=self.__dict__.get("_pre_relu", False),
-                              consumer=_consumer_of(self))
+                              consumer=_consumer_of(self), int8=_int8_ok(self))
 
     def forward(self, input):
         if self._use_frozen():
@@ -612,7 +619,7 @@ def add_quant_op(module, a_bits=8, w_bits=8, q_type=0, q_level=0, weight_observe
             add_quant_op(child, **kw)
 
 
-def freeze_inference(model, enable=True, handoff=True):
+def freeze_inference(model, enable=True, handoff=True, int8=False):
     """Opt-in inference fast path for an IAO-prepared model in eval mode (BASELINE.json configs[4], iao/main.py:511-519):
     * every quant conv folds + quantizes its weights and packs their tensor-core image ONCE (re-done when a parameter or
       buffer is written in place);
@@ -622,10 +629,14 @@ def freeze_inference(model, enable=True, handoff=True):
     * ``handoff``: producers write the bf16 operand plane of the conv that consumes them (conv epilogue -> next conv of an
       nn.Sequential, QuantAdd -> first conv of the next residual block; mnb_pk_conv_post / mnb_quant_add_pack_fwd), so those
       convs need no separate quantize + pack pass and the Sequential intermediates are never written as fp32.
+    * ``int8``: every quant conv with a symmetric activation quantizer (q_type 0) and symmetric weights of 2..8 bits runs
+      its forward on int8 operands (s8 x s8 -> s32 wgmma, mnb_pk_i8_conv) where the int8 plan covers its shape; the others
+      keep the bf16 path.  Hand-offs then carry the plane format the consumer reads.
     Outputs are bit-identical to the un-frozen eval forward; ``enable=False`` restores the modules."""
     for m in model.modules():
         if isinstance(m, (QuantConv2d, QuantLinear, QuantAdd)):
             m.__dict__["_frozen_inference"] = bool(enable)
+            m.__dict__["_int8"] = bool(enable and int8)
             m.__dict__.pop("_frozen", None)
             m.__dict__.pop("_pre_relu", None)
             m.__dict__.pop("_fuse_relu", None)

@@ -100,6 +100,56 @@ def conv_post(sh, a_pk, terms_a, w_img, terms_w, out, post_qp, post_plane, post_
                                 L.tc_err_flag(a_pk.device).data_ptr(), L.stream())
 
 
+# ---- int8 operands (frozen inference graphs, symmetric IAO): planes [b][c/16][h][w][16] s8, s8 x s8 -> s32 wgmma
+def i8_plan(sh):
+    """plan of mnb_pk_i8_conv as a list of the 21 mnb_pk_conv_plan_ex fields, None outside the int8 cover (host only)"""
+    out = (C.c_int32 * 21)()
+    return list(out) if L.load().mnb_pk_i8_conv_plan(C.byref(sh), out, 21) == 0 else None
+
+
+def i8_supported(sh):
+    """does mnb_pk_i8_conv cover this forward shape?  (host-only plan query, cached)"""
+    k = ("i8", _key(sh))
+    if k not in _plan_cache:
+        _plan_cache[k] = L.load().mnb_pk_i8_conv_plan(C.byref(sh), None, 0) == 0
+    return _plan_cache[k]
+
+
+def consumer_plane_i8(b, c, h, w, device):
+    """empty int8 operand plane of a conv that reads a [b, c, h, w] activation"""
+    return torch.empty(int(L.load().mnb_pk_i8_act_bytes(b, c, h, w)), dtype=torch.uint8, device=device)
+
+
+def pack_act_i8(x, qp, phase_split=False, relu=False):
+    """fp32 NCHW -> int8 level plane of a symmetric IAO quantizer"""
+    b, c, h, w = x.shape
+    out = consumer_plane_i8(b, c, h, w, x.device)
+    L.check(L.load().mnb_pk_i8_pack_act(x.data_ptr(), b, c, h, w, C.byref(qp), 1 if phase_split else 0, 1 if relu else 0,
+                                        out.data_ptr(), L.stream()), "pk_i8_pack_act")
+    return out
+
+
+def pack_weight_i8(sh, w_int):
+    nbytes = int(L.load().mnb_pk_i8_wimage_bytes(C.byref(sh)))
+    if nbytes < 0:
+        raise ValueError("micronet_b200.pk: shape outside the cover of the int8 convolution")
+    img = torch.empty(nbytes, dtype=torch.uint8, device=w_int.device)
+    L.check(L.load().mnb_pk_i8_pack_weight(C.byref(sh), w_int.data_ptr(), img.data_ptr(), L.stream()), "pk_i8_pack_weight")
+    return img
+
+
+def conv_i8(sh, a_pk, w_img, out, n_scale=None, a_scale=None, a_scale_const=1.0, bias=None, post=None):
+    """forward conv of an int8 plane; ``post`` = (quantizer struct, int8 plane, relu, phase split) of the consumer whose
+    plane the epilogue writes as well (out may then be None).  Returns the C status."""
+    pp = None
+    if post is not None:
+        qp, plane, relu, split = post
+        pp = C.byref(L.PkPost(C.pointer(qp), 1 if relu else 0, 1 if split else 0, plane.data_ptr()))
+    return L.load().mnb_pk_i8_conv(C.byref(sh), a_pk.data_ptr(), w_img.data_ptr(), L.ptr(n_scale), L.ptr(a_scale),
+                                   float(a_scale_const), L.ptr(bias), L.ptr(out), pp, L.tc_err_flag(a_pk.device).data_ptr(),
+                                   L.stream())
+
+
 def wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
     lib = L.load()
     nbytes = int(lib.mnb_pk_wgrad_scratch_bytes(C.byref(sh), terms_dy, terms_x))
