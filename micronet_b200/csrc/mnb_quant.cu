@@ -608,6 +608,7 @@ extern "C" int mnb_iao_weight_fwd(const float* w, int64_t numel, int32_t out_c, 
 extern "C" int mnb_iao_weight_bwd(const float* g_wq, const uint8_t* pass, const float* scale, int64_t numel,
                                   int32_t out_c, int32_t rows, float* dw, mnb_stream_t stream) {
   MNB_REQUIRE(g_wq && pass && scale && dw && numel > 0 && out_c > 0 && numel % out_c == 0, "bad IAO weight-bwd arguments");
+  MNB_REQUIRE(rows == 1 || rows == out_c, "rows must be 1 or out_c, got %d for out_c = %d", rows, out_c);
   int blocks = (int)std::min<int64_t>(mnb_ceil_div(numel, 256), MNB_NUM_SMS * 8);
   iao_weight_bwd_kernel<<<blocks, 256, 0, S(stream)>>>(g_wq, pass, scale, numel, numel / out_c, rows, dw);
   MNB_LAUNCHED(1);
