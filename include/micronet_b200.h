@@ -415,6 +415,15 @@ int mnb_quant_add_pack_i8_fwd(const float* a, const float* b, int32_t batch, int
 int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x);
 int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                  const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);
+/* mnb_pk_wgrad for narrow grouped 3x3 layers (stride 1, 16 input / 32 output channels per group, groups % 4 == 0): one CTA
+ * keeps all nine taps of four groups in registers, so every operand byte is loaded once.  Same arguments as mnb_pk_wgrad
+ * and the same result bit for bit (same accumulation chains, batch splits and reduction order); MNB_E_UNSUPPORTED (nothing
+ * launched) outside that cover.
+ * mnb_pk_wgrad_taps_plan (host only): out = {blocks, splits, NI, nstage, BW, TH, stages per split, smem bytes,
+ * accumulators per MMA thread, scratch bytes (lo 31 bits), scratch bytes (hi), npairs}; the first min(n, 12) are written. */
+int mnb_pk_wgrad_taps_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n);
+int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
+                      const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * Bit-packed XNOR-popcount forward for wbwtab layers (mnb_xnor.cu): binary activations (WB:11-36, sign with 0 -> +1)

@@ -108,6 +108,8 @@ PROTOTYPES = {
     "mnb_quant_add_pack_i8_fwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _ACTQ, _I, _P, C.POINTER(PkPost), _P]),
     "mnb_pk_wgrad_scratch_bytes": (_L, [_SHAPE, _I, _I]),
     "mnb_pk_wgrad": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "mnb_pk_wgrad_taps_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),
+    "mnb_pk_wgrad_taps": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_xnor_supported": (C.c_int, [_SHAPE]),
     "mnb_xnor_act_bytes": (_L, [_I, _I, _I, _I, _I]),
     "mnb_xnor_pack_act": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
@@ -214,6 +216,9 @@ PK_TERMS_BWD = int(os.environ.get("MNB_PK_TERMS_BWD", "2"))
 # with BOTH operands written by the producers: +-1 planes forward (mnb_bn_sign_fwd_packed), gradient pieces backward
 # (mnb_bn_sign_bwd_pack); 3x3 layers take it in any case.  MNB_PK_WBWTAB=0 keeps every wbwtab layer on the fused kernels.
 PK_WBWTAB = os.environ.get("MNB_PK_WBWTAB", "1") == "1"
+# weight gradient of narrow grouped 3x3 layers (16 / 32 channels per group) on mnb_pk_wgrad_taps, all taps of a CTA in
+# registers; MNB_PK_WG_TAPS=0 keeps them on mnb_pk_wgrad (to compare the two in one process)
+PK_WG_TAPS = os.environ.get("MNB_PK_WG_TAPS", "1") != "0"
 
 # bit-packed XNOR-popcount forward for wbwtab inference (mnb_xnor.cu): "auto" = the layers where it is expected to beat the
 # tensor-core forward (functional.xnor_preferred), "all" = wherever it has cover, "off" = never

@@ -1459,6 +1459,165 @@ __global__ void __launch_bounds__(128) wg_reduce_kernel(const float* __restrict_
   dw[((int64_t)kout * cin_g + c) * ntap + tap] = acc;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// weight gradient of narrow grouped 3x3 convolutions with every filter tap in registers
+// ---------------------------------------------------------------------------------------------------------
+// pk_wgrad_kernel merges four groups of 16 input / 32 output channels into one 128 x 64 accumulator block per tap and keeps
+// tpg x Nc <= 128 accumulator columns, so such a layer runs as 5 tap groups, each re-reading every operand byte, with 3/4
+// of its MMAs landing in discarded off-diagonal blocks.  Here one CTA owns the same 4-group block for ALL nine taps: MMA
+// warpgroup wg multiplies its 64 dy rows (groups 2wg, 2wg + 1) by those two groups' 32 x columns only (m64n32k16, half of
+// the products discarded instead of 3/4), 9 x 16 = 144 fp32 accumulators per thread, so each stage is loaded once.
+// The register file is split with setmaxnreg: TMA warpgroup 40, MMA warpgroups 232 (128 * 40 + 256 * 232 = 384 * 168).
+constexpr int kTapsN = 9;                                     // taps held in registers: 3 x 3 filters
+constexpr int kTapsCin = 16, kTapsCout = 32, kTapsGm = 4;     // channels per group; groups per CTA block
+constexpr int kTapsTmaRegs = 40, kTapsMmaRegs = 232;
+
+// The cover: stride 1, 3 x 3, 16 / 32 channels per group, groups % 4 == 0.  The raster, the stages and the batch splits
+// are those of make_wg_plan for the same shape, so every accumulator runs the same chain of MMAs in the same order and
+// the splits are reduced in the same order: the result is bit for bit that of pk_wgrad_kernel.  Only the ring depth
+// differs (any count up to MAXST instead of 2, 4 or 8: it does not change the arithmetic).
+static int make_wgt_plan(const mnb_conv_shape* s, int TA, int TX, WgPlan& p) {
+  MNB_REQUIRE(s != nullptr, "conv shape is NULL");
+  MNB_REQUIRE(TA >= 1 && TA <= 3 && TX >= 1 && TX <= 3, "term counts must be 1..3");
+  const int C = s->in_c, K = s->out_c, G = s->groups;
+  MNB_REQUIRE(s->batch > 0 && C > 0 && K > 0 && s->in_h > 0 && s->in_w > 0 && G > 0 && C % G == 0 && K % G == 0,
+              "bad conv shape");
+  auto no = [](const char* why) { return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad taps: %s", why); };
+  if (s->ker_h != 3 || s->ker_w != 3) return no("filter is not 3x3");
+  if (s->stride_h != 1 || s->stride_w != 1 || s->dil_h != 1 || s->dil_w != 1) return no("stride or dilation != 1");
+  if (s->pad_h < 0 || s->pad_w < 0 || s->pad_h > 2 || s->pad_w > 2) return no("padding outside 0..2");
+  if (C / G != kTapsCin || K / G != kTapsCout || G % kTapsGm) return no("needs 16 / 32 channels per group and groups % 4 == 0");
+  if (int e = make_wg_plan(s, TA, TX, p)) return e;
+  // the same block as pk_wgrad_kernel's: 4 merged groups, one 128-channel k tile, one 64-channel c tile (MNB_PK_WG_* knobs
+  // that change it leave the shape to pk_wgrad_kernel)
+  if (p.gm != kTapsGm || p.Nc != 64 || p.n_ctiles != 1 || p.n_ktiles != 1 || p.nkph_used != 1) return no("merged block");
+  p.tpg = kTapsN; p.n_tg = 1;
+  p.nstage = std::min(MAXST, (kSmemBudget - 1024) / p.stage_bytes);
+  p.smem_bytes = p.nstage * p.stage_bytes + 1024;
+  p.partial_floats = (int64_t)p.splits * p.G * kTapsN * p.Nc * 128;
+  return 0;
+}
+
+// tc::fence_acc for fp32 accumulators kept as "f" registers: the "+r" form moves every accumulator between register
+// classes around each MMA, and ptxas then waits for every wgmma before the next one
+__device__ __forceinline__ void fence_f32(float (&d)[16]) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+struct WgtParams {
+  uint32_t stg_per_split, nstg_total, NI, nsub, ksteps, npairs, nstage, stage16, sub16, dy_sbo, x_sbo, x_off16;
+  uint32_t pair_a16[MAXPAIR], pair_b16[MAXPAIR];   // dy / x piece-plane offsets of each piece pair (16-byte units)
+  uint32_t tap16[kTapsN];                          // x start-row offset of each tap (16-byte units)
+  int row_tiles, TA, TX, TH, hlo, wlo, stage_bytes, sub_bytes, dy_bytes, x_bytes, dy_box_bytes, x_box_bytes, smem_bytes;
+  float* partial;
+  int* err;
+};
+
+constexpr int kWgtThreads = 384;   // warpgroup 0: TMA (warp 0, lane 0), warpgroups 1, 2: MMA
+
+// CTA (blockIdx.x = 4-group block, blockIdx.y = batch split).  partial[split][block][tap][c 0..63][k 0..127] as
+// wg_reduce_kernel reads it (G = blocks, one k tile, one c tile, Nc = 64); only the diagonal (same group) 32 x 16 blocks are
+// written, the reduction reads nothing else.
+__global__ void __launch_bounds__(kWgtThreads, 1)
+pk_wgrad_taps_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_constant__ CUtensorMap dy1,
+                     const __grid_constant__ CUtensorMap dy2, const __grid_constant__ CUtensorMap x0,
+                     const __grid_constant__ CUtensorMap x1, const __grid_constant__ CUtensorMap x2,
+                     const __grid_constant__ WgtParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ WgShared sh;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&sh.full[i], 1); tc::mbar_init(&sh.empty[i], 8); }
+    sh.abort = 0;
+    tc::fence_barrier_init();
+    tc::prefetch_tmap(&dy0); tc::prefetch_tmap(&x0);
+  }
+  // every row an MMA can read must be finite (positions are the reduction dimension): zero everything once
+  for (int i = tid; i < p.smem_bytes / 16; i += kWgtThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+  const int blk = blockIdx.x, split = blockIdx.y;
+  const uint32_t stg0 = (uint32_t)split * p.stg_per_split, stg1 = min(p.nstg_total, stg0 + p.stg_per_split);
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kTapsTmaRegs));
+    if (warp == 0 && lane == 0) {
+      uint32_t slot = 0, ph = 0;
+      const int k8 = blk * (kTapsGm * kTapsCout / 8), c8 = blk * (kTapsGm * kTapsCin / 8);
+      for (uint32_t stg = stg0; stg < stg1; ++stg) {
+        if (!tc::mbar_wait(&sh.empty[slot], ph ^ 1u, p.err, 721)) break;
+        const int sub0 = (int)(stg * p.NI), nsubs = min((int)p.NI, (int)p.nsub - sub0);
+        tc::mbar_arrive_expect_tx(&sh.full[slot], (uint32_t)(nsubs * (p.TA * p.dy_box_bytes + p.TX * p.x_box_bytes)));
+        for (int si = 0; si < nsubs; ++si) {
+          const int sub = sub0 + si;
+          const int b = sub / p.row_tiles, h0 = (sub - b * p.row_tiles) * p.TH;
+          uint8_t* sb = smem + (size_t)slot * p.stage_bytes + (size_t)si * p.sub_bytes;
+          tc::tma_load_4d(sb, &dy0, &sh.full[slot], 0, h0, b, k8);
+          if (p.TA > 1) tc::tma_load_4d(sb + p.dy_bytes, &dy1, &sh.full[slot], 0, h0, b, k8);
+          if (p.TA > 2) tc::tma_load_4d(sb + 2 * p.dy_bytes, &dy2, &sh.full[slot], 0, h0, b, k8);
+          uint8_t* xb = sb + (size_t)p.TA * p.dy_bytes;
+          tc::tma_load_4d(xb, &x0, &sh.full[slot], -2 * p.wlo, h0 - p.hlo, b, c8);
+          if (p.TX > 1) tc::tma_load_4d(xb + p.x_bytes, &x1, &sh.full[slot], -2 * p.wlo, h0 - p.hlo, b, c8);
+          if (p.TX > 2) tc::tma_load_4d(xb + 2 * p.x_bytes, &x2, &sh.full[slot], -2 * p.wlo, h0 - p.hlo, b, c8);
+        }
+        // sub-blocks of a short last stage keep their previous (finite) contents; the MMA loop skips them
+        if (++slot == p.nstage) { slot = 0; ph ^= 1u; }
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTapsMmaRegs));
+    const int wg = (warp - 4) >> 2, w4 = (warp - 4) & 3;
+    // A: the warpgroup's 64 dy channels (octets 8wg ..), B: its two groups' 32 x channels (octets 4wg ..)
+    const uint64_t a_desc0 = tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.dy_sbo) + (uint64_t)((8u * wg * p.dy_sbo) >> 4);
+    const uint64_t b_desc0 =
+        tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.x_sbo) + (uint64_t)(p.x_off16 + ((4u * wg * p.x_sbo) >> 4));
+    const uint32_t a_lo0 = (uint32_t)a_desc0, b_lo0 = (uint32_t)b_desc0;
+    const uint64_t a_hi = a_desc0 & 0xffffffff00000000ull, b_hi = b_desc0 & 0xffffffff00000000ull;
+    float acc[kTapsN][16];
+#pragma unroll
+    for (int t = 0; t < kTapsN; ++t) tc::zero_acc(acc[t]);
+    uint32_t slot = 0, ph = 0;
+    for (uint32_t stg = stg0; stg < stg1; ++stg) {
+      tc::mbar_wait_soft(&sh.full[slot], ph, p.err, 722, &sh.abort);
+      const uint32_t nsubs = min(p.NI, p.nsub - stg * p.NI);
+      tc::wg_fence();
+#pragma unroll
+      for (int t = 0; t < kTapsN; ++t) fence_f32(acc[t]);
+      for (uint32_t si = 0; si < nsubs; ++si) {
+        const uint32_t s16 = slot * p.stage16 + si * p.sub16;
+        for (uint32_t j = 0; j < p.ksteps; ++j) {
+          for (uint32_t pr = 0; pr < p.npairs; ++pr) {
+            const uint64_t ad = a_hi | (uint64_t)(a_lo0 + s16 + 16u * j + p.pair_a16[pr]);
+            const uint32_t bb = b_lo0 + s16 + 16u * j + p.pair_b16[pr];
+#pragma unroll
+            for (int t = 0; t < kTapsN; ++t) tc::Mma<32>::bf16<1, 1>(acc[t], ad, b_hi | (uint64_t)(bb + p.tap16[t]), 1);
+          }
+        }
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+#pragma unroll
+      for (int t = 0; t < kTapsN; ++t) fence_f32(acc[t]);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&sh.empty[slot]);
+      if (++slot == p.nstage) { slot = 0; ph ^= 1u; }
+    }
+    // fragment d[4j + 2i + c] = D[16 w4 + lane/4 + 8i][8j + 2(lane%4) + c]: rows of group (w4 >> 1), columns of group (j >> 1)
+    float* dst = p.partial + ((int64_t)split * gridDim.x + blk) * (int64_t)(kTapsN * 64 * 128);
+    const int kr = 64 * wg + 16 * w4 + (lane >> 2), cb = 32 * wg + 2 * (lane & 3);
+#pragma unroll
+    for (int t = 0; t < kTapsN; ++t)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if ((j >> 1) != (w4 >> 1)) continue;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) dst[(int64_t)(t * 64 + cb + 8 * j + (e & 1)) * 128 + kr + 8 * (e >> 1)] = acc[t][4 * j + e];
+      }
+  }
+  __syncthreads();
+}
+
 }  // namespace pk
 
 // =========================================================================================================
@@ -1927,6 +2086,60 @@ extern "C" int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t 
     wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, pl.gm, pl.n_ktiles, pl.n_ctiles, pl.ntap, pl.Nc, cout_o,
                                             cin_o, a_scale, kdiv, dw);
   }
+  MNB_LAUNCHED(2);
+  return 0;
+}
+
+// host only: out = {blocks, splits, NI, nstage, BW, TH, stg_per_split, smem_bytes, accumulators per MMA thread,
+//                   scratch bytes (lo), scratch bytes (hi), npairs}; the first min(n, 12) are written
+extern "C" int mnb_pk_wgrad_taps_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n) {
+  pk::WgPlan p;
+  if (int e = pk::make_wgt_plan(s, terms_dy, terms_x, p)) return e;
+  if (out) {
+    const int64_t sb = p.partial_floats * 4;
+    const int v[12] = {p.G, p.splits, p.NI, p.nstage, p.BW, p.TH, p.stg_per_split, p.smem_bytes, pk::kTapsN * 16,
+                       (int)(sb & 0x7fffffff), (int)(sb >> 31), p.npairs};
+    for (int i = 0; i < std::min(n, 12); ++i) out[i] = v[i];
+  }
+  return 0;
+}
+
+// mnb_pk_wgrad for the shapes of mnb_pk_wgrad_taps_plan's cover (same operands, the same result bit for bit: same chains,
+// same batch splits, same reduction); scratch: the plan's scratch bytes
+extern "C" int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
+                                 const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag,
+                                 mnb_stream_t stream) {
+  using namespace pk;
+  MNB_REQUIRE(s && dy_pk && x_pk && dw && scratch && err_flag, "NULL pk_wgrad_taps pointer");
+  WgPlan pl;
+  if (int e = make_wgt_plan(s, terms_dy, terms_x, pl)) return e;
+  WgtParams p;
+  memset(&p, 0, sizeof(p));
+  p.stg_per_split = pl.stg_per_split; p.nstg_total = pl.nstg_total; p.NI = pl.NI; p.nsub = pl.nsub; p.ksteps = pl.rows_dy / 16;
+  p.npairs = pl.npairs; p.nstage = pl.nstage; p.stage16 = pl.stage_bytes >> 4; p.sub16 = pl.sub_bytes >> 4;
+  p.dy_sbo = (uint32_t)pl.rows_dy * 16u; p.x_sbo = (uint32_t)pl.rows_x * 16u; p.x_off16 = (pl.TA * pl.dy_bytes) >> 4;
+  for (int i = 0; i < pl.npairs; ++i) {
+    p.pair_a16[i] = (uint32_t)(pl.pair_a[i] * pl.dy_bytes) >> 4;
+    p.pair_b16[i] = (uint32_t)(pl.pair_b[i] * pl.x_bytes) >> 4;
+  }
+  for (int t = 0; t < kTapsN; ++t) p.tap16[t] = (uint32_t)pl.tap_off[t];
+  p.row_tiles = pl.row_tiles; p.TA = pl.TA; p.TX = pl.TX; p.TH = pl.TH; p.hlo = pl.hlo; p.wlo = pl.wlo;
+  p.stage_bytes = pl.stage_bytes; p.sub_bytes = pl.sub_bytes; p.dy_bytes = pl.dy_bytes; p.x_bytes = pl.x_bytes;
+  p.dy_box_bytes = pl.dy_box_bytes; p.x_box_bytes = pl.x_box_bytes; p.smem_bytes = pl.smem_bytes;
+  p.partial = reinterpret_cast<float*>(scratch); p.err = err_flag;
+  CUtensorMap tdy[3], tx[3];
+  const int64_t dy_plane = (int64_t)pl.B * pl.K8 * pl.P * pl.Q * 16;
+  const int64_t x_plane = (int64_t)pl.B * pl.C8X * pl.HX * pl.WX * 16;
+  for (int t = 0; t < 3; ++t) {
+    if (int e = make_pk_tmap(&tdy[t], dy_pk, dy_plane, t < pl.TA ? t : 0, pl.B, pl.K8, pl.P, pl.Q, pl.BW, pl.TH, 1, 16)) return e;
+    if (int e = make_pk_tmap(&tx[t], x_pk, x_plane, t < pl.TX ? t : 0, pl.B, pl.C8X, pl.HX, pl.WX, pl.BW, pl.THH, 1, 8)) return e;
+  }
+  if (int e = set_max_smem(pk_wgrad_taps_kernel, kSmemBudget)) return e;
+  cudaStream_t st = (cudaStream_t)stream;
+  pk_wgrad_taps_kernel<<<dim3(pl.G, pl.splits), kWgtThreads, pl.smem_bytes, st>>>(tdy[0], tdy[1], tdy[2], tx[0], tx[1], tx[2], p);
+  const dim3 rgrid(kTapsCin * kTapsN, 1, pl.G * kTapsGm);
+  wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, kTapsGm, 1, 1, kTapsN, pl.Nc, kTapsCout, kTapsCin, a_scale,
+                                          kdiv, dw);
   MNB_LAUNCHED(2);
   return 0;
 }

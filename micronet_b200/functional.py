@@ -394,8 +394,10 @@ def _pk_backward(ctx, dy):
         if spec is not None:
             a_scale = ctx.pk_a_scale if spec.mode == L.ACT_IAO else _dorefa_scale_tensor(spec.bits, dy.device)
         tx = min(ctx.pk_ta, T)     # a 3-piece saved input contributes its two leading pieces
-        L.check(_timed("wgrad_pk", sh, lambda: PK.wgrad(sh, dy_pk, T, ctx.pk_x, tx, dwq, a_scale=a_scale,
-                                                        kdiv=ctx.w_scale if fold else None)), "pk_wgrad")
+        kdiv = ctx.w_scale if fold else None
+        # narrow grouped 3x3 layers: all taps of a CTA in registers (same kernel-table kind; its rows are those layers' shapes)
+        fn = PK.wgrad_taps if L.PK_WG_TAPS and PK.wgrad_taps_plan(sh, T, tx) is not None else PK.wgrad
+        L.check(_timed("wgrad_pk", sh, lambda: fn(sh, dy_pk, T, ctx.pk_x, tx, dwq, a_scale=a_scale, kdiv=kdiv)), "pk_wgrad")
     return dx, dwq
 
 

@@ -7,6 +7,7 @@ shared memory, stride 2, 5x5 filters, 4x4 or 224x224 images ...) and every fused
     pack_weight integer levels / fp32 weights -> the bf16 operand image of one (shape, mode)
     conv        TMA -> wgmma (register accumulators) -> epilogue (forward: scale + bias; data gradient: STE mask)
     wgrad       the same boxes read as MN-major operands, split over the batch, deterministic reduction
+    wgrad_taps  wgrad of narrow grouped 3x3 layers with all nine taps of a CTA in registers
 
 Reference math: F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen's
 convolution_backward."""
@@ -158,3 +159,29 @@ def wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
     ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dw.device)
     return lib.mnb_pk_wgrad(C.byref(sh), dy_pk.data_ptr(), terms_dy, x_pk.data_ptr(), terms_x, L.ptr(a_scale),
                             L.ptr(kdiv), dw.data_ptr(), ws.data_ptr(), L.tc_err_flag(dw.device).data_ptr(), L.stream())
+
+
+def wgrad_taps_plan(sh, terms_dy, terms_x):
+    """plan of mnb_pk_wgrad_taps as a dict, None outside its cover (host-only plan query, cached)"""
+    k = ("wt", _key(sh), terms_dy, terms_x)
+    if k not in _plan_cache:
+        out = (C.c_int32 * 12)()
+        ok = L.load().mnb_pk_wgrad_taps_plan(C.byref(sh), terms_dy, terms_x, out, 12) == 0
+        names = ("blocks", "splits", "NI", "nstage", "BW", "TH", "stg_per_split", "smem_bytes", "acc_regs")
+        plan = None
+        if ok:
+            plan = dict(zip(names, out[:9]))
+            plan["scratch_bytes"] = out[9] | (out[10] << 31)
+            plan["npairs"] = out[11]
+        _plan_cache[k] = plan
+    return _plan_cache[k]
+
+
+def wgrad_taps(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
+    """mnb_pk_wgrad_taps: same operands as wgrad and the same result bit for bit; returns the C status"""
+    plan = wgrad_taps_plan(sh, terms_dy, terms_x)
+    if plan is None:
+        return L.E_UNSUPPORTED
+    ws = torch.empty(plan["scratch_bytes"], dtype=torch.uint8, device=dw.device)
+    return L.load().mnb_pk_wgrad_taps(C.byref(sh), dy_pk.data_ptr(), terms_dy, x_pk.data_ptr(), terms_x, L.ptr(a_scale),
+                                      L.ptr(kdiv), dw.data_ptr(), ws.data_ptr(), L.tc_err_flag(dw.device).data_ptr(), L.stream())
