@@ -1498,13 +1498,6 @@ static int make_wgt_plan(const mnb_conv_shape* s, int TA, int TX, WgPlan& p) {
   return 0;
 }
 
-// tc::fence_acc for fp32 accumulators kept as "f" registers: the "+r" form moves every accumulator between register
-// classes around each MMA, and ptxas then waits for every wgmma before the next one
-__device__ __forceinline__ void fence_f32(float (&d)[16]) {
-#pragma unroll
-  for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
 struct WgtParams {
   uint32_t stg_per_split, nstg_total, NI, nsub, ksteps, npairs, nstage, stage16, sub16, dy_sbo, x_sbo, x_off16;
   uint32_t pair_a16[MAXPAIR], pair_b16[MAXPAIR];   // dy / x piece-plane offsets of each piece pair (16-byte units)
@@ -1583,7 +1576,7 @@ pk_wgrad_taps_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_const
       const uint32_t nsubs = min(p.NI, p.nsub - stg * p.NI);
       tc::wg_fence();
 #pragma unroll
-      for (int t = 0; t < kTapsN; ++t) fence_f32(acc[t]);
+      for (int t = 0; t < kTapsN; ++t) tc::fence_acc(acc[t]);
       for (uint32_t si = 0; si < nsubs; ++si) {
         const uint32_t s16 = slot * p.stage16 + si * p.sub16;
         for (uint32_t j = 0; j < p.ksteps; ++j) {
@@ -1598,7 +1591,7 @@ pk_wgrad_taps_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_const
       tc::wg_commit();
       tc::wg_wait<0>();
 #pragma unroll
-      for (int t = 0; t < kTapsN; ++t) fence_f32(acc[t]);
+      for (int t = 0; t < kTapsN; ++t) tc::fence_acc(acc[t]);
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(&sh.empty[slot]);
       if (++slot == p.nstage) { slot = 0; ph ^= 1u; }

@@ -119,11 +119,15 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator reads / writes across wgmma issue and wg_wait (the asm outputs of an
-// issue are only valid after the wait that retires it)
+// issue are only valid after the wait that retires it).  Each accumulator is pinned in the register class its Mma wrapper
+// uses ("f" for fp32, "r" for s32): a class change between two MMAs makes ptxas retire every wgmma before the next one
+// (C7517, a WARPGROUP.DEPBAR after each HGMMA).
+__device__ __forceinline__ void fence_reg(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+__device__ __forceinline__ void fence_reg(int32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
 template <typename T, int NR>
 __device__ __forceinline__ void fence_acc(T (&d)[NR]) {
 #pragma unroll
-  for (int i = 0; i < NR; ++i) asm volatile("" : "+r"(reinterpret_cast<uint32_t(&)[NR]>(d)[i])::"memory");
+  for (int i = 0; i < NR; ++i) fence_reg(d[i]);
 }
 template <typename T, int NR>
 __device__ __forceinline__ void zero_acc(T (&d)[NR]) {
