@@ -69,6 +69,14 @@ struct MnbMin { template <typename T> __device__ T operator()(T a, T b) const { 
 struct MnbMax { template <typename T> __device__ T operator()(T a, T b) const { return a > b ? a : b; } };
 struct MnbSum { template <typename T> __device__ T operator()(T a, T b) const { return a + b; } };
 
+// The centred gradient of the BatchNorm backward, g_masked - dbeta / N - xhat * dgamma / N, with its rounding pinned: one
+// subtraction, then one fma.  Every apply pass of the fused producers (mnb_fused.cu, and the _pack passes of mnb_pk.cu that
+// write the same dx as packed pieces) calls this, so they all produce the same fp32 dx bit for bit; written as a plain
+// expression, nvcc's fma contraction was free to round it differently in each kernel.
+__device__ __forceinline__ float bn_bwd_centre(float g, float db, float xhat, float dg) {
+  return fmaf(-xhat, dg, __fsub_rn(g, db));
+}
+
 // ---- the activation quantizer, shared by the standalone kernel and the fused conv loaders ----
 struct MnbActQ {
   int mode, qmin, qmax;

@@ -194,10 +194,10 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __r
                 v3 = (nib & 8u) ? gv.w : 0.f;
           if (training) {
             const float4 xv = __ldg(x4 + fi4);
-            v0 = v0 - db - ((xv.x - mu) * is) * dg;
-            v1 = v1 - db - ((xv.y - mu) * is) * dg;
-            v2 = v2 - db - ((xv.z - mu) * is) * dg;
-            v3 = v3 - db - ((xv.w - mu) * is) * dg;
+            v0 = bn_bwd_centre(v0, db, (xv.x - mu) * is, dg);
+            v1 = bn_bwd_centre(v1, db, (xv.y - mu) * is, dg);
+            v2 = bn_bwd_centre(v2, db, (xv.z - mu) * is, dg);
+            v3 = bn_bwd_centre(v3, db, (xv.w - mu) * is, dg);
           }
           const float4 o = make_float4(k * v0, k * v1, k * v2, k * v3);
           dx4[fi4] = o;
@@ -215,7 +215,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __r
         const int64_t fi = off + i;
         const bool pass = (__ldg(bits + (fi >> 5)) >> (fi & 31)) & 1u;
         float v = pass ? __ldg(g + goff + i) : 0.f;
-        if (training) v = v - db - ((__ldg(x + fi) - mu) * is) * dg;
+        if (training) v = bn_bwd_centre(v, db, (__ldg(x + fi) - mu) * is, dg);
         v = k * v;
         dx[fi] = v;
         f += v;
@@ -451,7 +451,7 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_apply_kernel(const float
       const float4 r0 = __ldg(x + i0), r1 = __ldg(x + i1);
       const float xs[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
 #pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] = v[e] - db - ((xs[e] - mu) * is) * dg;
+      for (int e = 0; e < 8; ++e) v[e] = bn_bwd_centre(v[e], db, (xs[e] - mu) * is, dg);
     }
     const float4 o0 = make_float4(k * v[0], k * v[1], k * v[2], k * v[3]), o1 = make_float4(k * v[4], k * v[5], k * v[6], k * v[7]);
     dx[i0] = o0;

@@ -603,7 +603,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __re
 #pragma unroll
       for (int i = 0; i < VEC; ++i) {
         float t = ((bw[j] >> i) & 1u) ? gf[i] : 0.f;
-        t = t - db - ((xf[i] - mu) * is) * dg;
+        t = bn_bwd_centre(t, db, (xf[i] - mu) * is, dg);
         t = k * t;
         df[i] = t;
         v[i][j] = ch_scale ? __fmul_rn(t, sc) : t;
@@ -669,7 +669,7 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_pack_kernel(const float2
         float t = 0.f;
         if ((uint32_t)e == e0 && ((nib >> e) & 1u)) t = gv.x;
         if ((uint32_t)e == e1 && ((nib >> e) & 1u)) t = gv.y;
-        t = t - db - ((xs[e] - mu) * is) * dg;
+        t = bn_bwd_centre(t, db, (xs[e] - mu) * is, dg);
         t = k * t;
         v[e][q] = ch_scale ? __fmul_rn(t, sc) : t;
       }
