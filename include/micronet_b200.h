@@ -343,6 +343,45 @@ int mnb_bn_sign_pool_bwd_pack(const float* g, const uint32_t* pass_bits, const u
                               int32_t channels, int32_t H, int32_t W, const float* mean, const float* invstd,
                               const float* gamma, const float* dgamma, const float* dbeta, int32_t out_shuffle_groups,
                               const float* ch_scale, int32_t terms, void* dy_packed, mnb_stream_t stream);
+/* Int16 hand-off between a wbwtab conv and its BatchNorm + binarizer (the conv's only reader).  On a +-1 activation plane
+ * and integer weight levels the conv's sums are exact integers; mnb_pk_conv_codes stores them as int16 `codes`
+ * [B][K][OH][OW] instead of the fp32 output, plus dec[2][K] = (a_scale * n_scale[k], bias[k]), the epilogue's pair, so that
+ * x = fmaf(code, dec[k], dec[K + k]) is mnb_pk_conv's fp32 output bit for bit.  Refused with MNB_E_UNSUPPORTED (nothing
+ * launched) unless (C/g) * R * S * level_bound <= 32767 (level_bound = max |weight level|), terms_a = terms_w = 1 and the
+ * plan is not segmented.  The _codes producers below are their fp32 namesakes reading x through that decode, with the
+ * same element-to-thread mapping and summation order (identical results); codes need half the alignment x needs there. */
+int mnb_pk_conv_codes(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
+                      const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, int32_t level_bound,
+                      int16_t* codes, float* dec, int32_t* err_flag, mnb_stream_t stream);
+/* x = fmaf(codes, dec[c], dec[C + c]) as fp32 [batch, channels, hw] */
+int mnb_codes_decode(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t hw, float* x,
+                     mnb_stream_t stream);
+int mnb_bn_batch_stats_codes(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t hw, double eps,
+                             double momentum, float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                             float* mean_invstd, void* scratch, mnb_stream_t stream);
+int mnb_bn_sign_fwd_packed_codes(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t hw,
+                                 const float* mean, const float* invstd, const float* gamma, const float* beta,
+                                 int32_t out_shuffle_groups, float* y, uint32_t* pass_bits, void* x_packed, mnb_stream_t stream);
+int mnb_bn_sign_bwd_codes(const float* g, const uint32_t* pass_bits, const int16_t* codes, const float* dec, int32_t batch,
+                          int32_t channels, int32_t hw, const float* mean, const float* invstd, const float* gamma,
+                          int32_t training, int32_t out_shuffle_groups, float* dx, float* dgamma, float* dbeta,
+                          float* dx_channel_sum, void* scratch, mnb_stream_t stream);
+int mnb_bn_sign_pool_fwd_codes(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t H, int32_t W,
+                               const float* mean, const float* invstd, const float* gamma, const float* beta,
+                               int32_t out_shuffle_groups, float* y, uint32_t* pass_bits, uint8_t* argmax, mnb_stream_t stream);
+int mnb_bn_sign_pool_bwd_codes(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const int16_t* codes,
+                               const float* dec, int32_t batch, int32_t channels, int32_t H, int32_t W, const float* mean,
+                               const float* invstd, const float* gamma, int32_t training, int32_t out_shuffle_groups, float* dx,
+                               float* dgamma, float* dbeta, float* dx_channel_sum, void* scratch, mnb_stream_t stream);
+int mnb_bn_sign_bwd_pack_codes(const float* g, const uint32_t* pass_bits, const int16_t* codes, const float* dec, int32_t batch,
+                               int32_t channels, int32_t hw, const float* mean, const float* invstd, const float* gamma,
+                               const float* dgamma, const float* dbeta, int32_t out_shuffle_groups, const float* ch_scale,
+                               int32_t terms, float* dx, void* dy_packed, mnb_stream_t stream);
+int mnb_bn_sign_pool_bwd_pack_codes(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const int16_t* codes,
+                                    const float* dec, int32_t batch, int32_t channels, int32_t H, int32_t W, const float* mean,
+                                    const float* invstd, const float* gamma, const float* dgamma, const float* dbeta,
+                                    int32_t out_shuffle_groups, const float* ch_scale, int32_t terms, void* dy_packed,
+                                    mnb_stream_t stream);
 /* mnb_pk_pack_act with a preceding nn.ReLU folded in (relu != 0: x is clamped at 0 before it is quantized / split) */
 int mnb_pk_pack_act_relu(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_act_qparams* qp,
                          int32_t terms, const float* ch_scale, int32_t phase_split, int32_t relu, void* out_pk,

@@ -98,6 +98,16 @@ PROTOTYPES = {
     "mnb_bn_sign_bwd_pack": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P, _P]),
     "mnb_bn_sign_pool_bwd_pack": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P]),
     "mnb_pk_conv_post": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P]),
+    "mnb_pk_conv_codes": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _I, _P, _P, _P, _P]),
+    "mnb_codes_decode": (C.c_int, [_P, _P, _I, _I, _I, _P, _P]),
+    "mnb_bn_batch_stats_codes": (C.c_int, [_P, _P, _I, _I, _I, _D, _D, _P, _P, _P, _P, _P, _P]),
+    "mnb_bn_sign_fwd_packed_codes": (C.c_int, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
+    "mnb_bn_sign_bwd_codes": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "mnb_bn_sign_pool_fwd_codes": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
+    "mnb_bn_sign_pool_bwd_codes": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "mnb_bn_sign_bwd_pack_codes": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P, _P]),
+    "mnb_bn_sign_pool_bwd_pack_codes": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P,
+                                                  _P]),
     "mnb_quant_add_pack_fwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _ACTQ, _I, _P, C.POINTER(PkPost), _P]),
     "mnb_pk_i8_act_bytes": (_L, [_I, _I, _I, _I]),
     "mnb_pk_i8_pack_act": (C.c_int, [_P, _I, _I, _I, _I, _ACTQ, _I, _I, _P, _P]),

@@ -77,6 +77,45 @@ __device__ __forceinline__ float bn_bwd_centre(float g, float db, float xhat, fl
   return fmaf(-xhat, dg, __fsub_rn(g, db));
 }
 
+// ---- the x operand of the fused BatchNorm producers: fp32 values (XT = float), or the exact int16 accumulator codes of a
+// wbwtab convolution (XT = int16_t, written by mnb_pk_conv_codes) with the per-channel decode pair dec[c] / dec[C + c] that
+// conv's epilogue used: x = fmaf(code, dec[c], dec[C + c]) is the value its fp32 epilogue stores, bit for bit.  Loads are
+// VEC elements wide (16 bytes of fp32 = 8 bytes of codes); nothing else of a producer depends on XT.
+struct XDec { float s, b; };
+template <typename XT> struct XVec;
+template <> struct XVec<float> { typedef float t1; typedef float2 t2; typedef float4 t4; };
+template <> struct XVec<int16_t> { typedef short t1; typedef short2 t2; typedef short4 t4; };
+
+template <typename XT>
+__device__ __forceinline__ XDec x_dec(const float* dec, int channels, int c) {
+  if constexpr (sizeof(XT) == 4) return XDec{1.f, 0.f};
+  else return XDec{__ldg(dec + c), __ldg(dec + channels + c)};
+}
+template <typename XT>
+__device__ __forceinline__ float x_val(XT q, XDec d) {
+  if constexpr (sizeof(XT) == 4) return q;
+  else return fmaf((float)q, d.s, d.b);
+}
+template <int VEC, typename XT>
+__device__ __forceinline__ void x_load(const XT* p, XDec d, float (&v)[VEC]) {
+  if constexpr (VEC == 1) {
+    v[0] = x_val<XT>(__ldg(reinterpret_cast<const typename XVec<XT>::t1*>(p)), d);
+  } else if constexpr (VEC == 2) {
+    const typename XVec<XT>::t2 t = __ldg(reinterpret_cast<const typename XVec<XT>::t2*>(p));
+    v[0] = x_val<XT>(t.x, d); v[1] = x_val<XT>(t.y, d);
+  } else {
+    static_assert(VEC == 4, "x_load: 1, 2 or 4 elements");
+    const typename XVec<XT>::t4 t = __ldg(reinterpret_cast<const typename XVec<XT>::t4*>(p));
+    v[0] = x_val<XT>(t.x, d); v[1] = x_val<XT>(t.y, d); v[2] = x_val<XT>(t.z, d); v[3] = x_val<XT>(t.w, d);
+  }
+}
+template <typename XT>
+__device__ __forceinline__ float4 x_load4(const XT* p, XDec d) {
+  float v[4];
+  x_load<4>(p, d, v);
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+
 // ---- the activation quantizer, shared by the standalone kernel and the fused conv loaders ----
 struct MnbActQ {
   int mode, qmin, qmax;

@@ -85,9 +85,11 @@ __global__ void __launch_bounds__(256) bn_sign_fwd_kernel(const float* __restric
 
 // ------------------------------------------------------------------ BatchNorm + sign, backward
 // pass 1: dbeta = sum g*pass, dgamma = sum g*pass*xhat per channel.  `g` is indexed through the output permutation.
-template <bool VEC>
+// XT = int16_t (here and in every kernel below): x as a wbwtab conv's codes + decode pair `dec` (mnb_common.cuh x_load).
+template <bool VEC, typename XT>
 __global__ void __launch_bounds__(256) bn_sign_bwd_reduce_kernel(const float* __restrict__ g, const uint32_t* __restrict__ bits,
-                                                                 const float* __restrict__ x, int batch, int channels, int hw,
+                                                                 const XT* __restrict__ x, const float* __restrict__ dec,
+                                                                 int batch, int channels, int hw,
                                                                  int sg, const float* __restrict__ mean,
                                                                  const float* __restrict__ invstd, float* __restrict__ dgamma,
                                                                  float* __restrict__ dbeta, uint32_t* counters,
@@ -97,12 +99,12 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_reduce_kernel(const float* __
   const int c = blockIdx.x, sp = blockIdx.y, nsp = gridDim.y;
   const int oc = (int)shuffled_channel((uint32_t)c, (uint32_t)sg, (uint32_t)(channels / sg));
   const float mu = __ldg(mean + c), is = __ldg(invstd + c);
+  const XDec d = x_dec<XT>(dec, channels, c);
   const int b_lo = (int)((int64_t)batch * sp / nsp), b_hi = (int)((int64_t)batch * (sp + 1) / nsp);
   double s1, s2;
   if (VEC) {
     const uint32_t hw4 = (uint32_t)hw >> 2, total = (uint32_t)(b_hi - b_lo) * hw4;
     const float4* g4 = reinterpret_cast<const float4*>(g);
-    const float4* x4 = reinterpret_cast<const float4*>(x);
     float f1[2] = {0.f, 0.f}, f2[2] = {0.f, 0.f};
     for (uint32_t t0 = threadIdx.x; t0 < total; t0 += 2 * blockDim.x) {
 #pragma unroll
@@ -113,7 +115,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_reduce_kernel(const float* __
           const uint32_t fi4 = ((uint32_t)(b_lo + b) * channels + c) * hw4 + i;
           const uint32_t go4 = ((uint32_t)(b_lo + b) * channels + oc) * hw4 + i;
           const uint32_t nib = (__ldg(bits + (fi4 >> 3)) >> (4 * (fi4 & 7))) & 15u;
-          const float4 gv = __ldg(g4 + go4), xv = __ldg(x4 + fi4);
+          const float4 gv = __ldg(g4 + go4), xv = x_load4(x + 4 * fi4, d);
           const float g0 = (nib & 1u) ? gv.x : 0.f, g1 = (nib & 2u) ? gv.y : 0.f, g2 = (nib & 4u) ? gv.z : 0.f,
                       g3 = (nib & 8u) ? gv.w : 0.f;
           f1[u] += (g0 + g1) + (g2 + g3);
@@ -133,7 +135,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_reduce_kernel(const float* __
         const bool pass = (__ldg(bits + (fi >> 5)) >> (fi & 31)) & 1u;
         const float gv = pass ? __ldg(g + goff + i) : 0.f;
         f1 += gv;
-        f2 += gv * ((__ldg(x + fi) - mu) * is);
+        f2 += gv * ((x_val<XT>(__ldg(x + fi), d) - mu) * is);
       }
       s1 += (double)f1; s2 += (double)f2;
     }
@@ -158,9 +160,10 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_reduce_kernel(const float* __
 
 // pass 2: dx = gamma * invstd * (g*pass - dbeta/N - xhat * dgamma/N)  (training) or gamma * invstd * g*pass (eval),
 // plus the per-channel sum of the dx values just written (what the producing convolution needs as its bias gradient).
-template <bool VEC>
+template <bool VEC, typename XT>
 __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __restrict__ g, const uint32_t* __restrict__ bits,
-                                                                const float* __restrict__ x, int batch, int channels, int hw,
+                                                                const XT* __restrict__ x, const float* __restrict__ dec,
+                                                                int batch, int channels, int hw,
                                                                 int sg, float inv_count, const float* __restrict__ mean,
                                                                 const float* __restrict__ invstd, const float* __restrict__ gamma,
                                                                 const float* __restrict__ dgamma, const float* __restrict__ dbeta,
@@ -172,12 +175,12 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __r
   const int oc = (int)shuffled_channel((uint32_t)c, (uint32_t)sg, (uint32_t)(channels / sg));
   const float mu = __ldg(mean + c), is = __ldg(invstd + c), k = __ldg(gamma + c) * is;
   const float db = training ? __ldg(dbeta + c) * inv_count : 0.f, dg = training ? __ldg(dgamma + c) * inv_count : 0.f;
+  const XDec d = x_dec<XT>(dec, channels, c);
   const int b_lo = (int)((int64_t)batch * sp / nsp), b_hi = (int)((int64_t)batch * (sp + 1) / nsp);
   double s;
   if (VEC) {
     const uint32_t hw4 = (uint32_t)hw >> 2, total = (uint32_t)(b_hi - b_lo) * hw4;
     const float4* g4 = reinterpret_cast<const float4*>(g);
-    const float4* x4 = reinterpret_cast<const float4*>(x);
     float4* dx4 = reinterpret_cast<float4*>(dx);
     float f[2] = {0.f, 0.f};
     for (uint32_t t0 = threadIdx.x; t0 < total; t0 += 2 * blockDim.x) {
@@ -193,7 +196,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __r
           float v0 = (nib & 1u) ? gv.x : 0.f, v1 = (nib & 2u) ? gv.y : 0.f, v2 = (nib & 4u) ? gv.z : 0.f,
                 v3 = (nib & 8u) ? gv.w : 0.f;
           if (training) {
-            const float4 xv = __ldg(x4 + fi4);
+            const float4 xv = x_load4(x + 4 * fi4, d);
             v0 = bn_bwd_centre(v0, db, (xv.x - mu) * is, dg);
             v1 = bn_bwd_centre(v1, db, (xv.y - mu) * is, dg);
             v2 = bn_bwd_centre(v2, db, (xv.z - mu) * is, dg);
@@ -215,7 +218,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __r
         const int64_t fi = off + i;
         const bool pass = (__ldg(bits + (fi >> 5)) >> (fi & 31)) & 1u;
         float v = pass ? __ldg(g + goff + i) : 0.f;
-        if (training) v = bn_bwd_centre(v, db, (__ldg(x + fi) - mu) * is, dg);
+        if (training) v = bn_bwd_centre(v, db, (x_val<XT>(__ldg(x + fi), d) - mu) * is, dg);
         v = k * v;
         dx[fi] = v;
         f += v;
@@ -239,9 +242,11 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_apply_kernel(const float* __r
   counters[c] = 0;
 }
 
-static bool planes_vectorizable(int64_t n, int hw, const void* a, const void* b, const void* c) {
+// a, b, c: fp32 planes read / written 16 bytes at a time; x (optional): the x operand of element type XT, 4 elements at a time
+template <typename XT = float>
+static bool planes_vectorizable(int64_t n, int hw, const void* a, const void* b, const void* c, const XT* x = nullptr) {
   return (hw & 3) == 0 && n < (1ll << 31) &&
-         (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15) == 0;
+         (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15) == 0 && ((uintptr_t)x & (4 * sizeof(XT) - 1)) == 0;
 }
 // (channels x splits) blocks: about two waves of 8 resident 256-thread blocks per SM, so that every block streams
 // >= ~100 KB (small blocks spend as long being scheduled as loading)
@@ -270,10 +275,11 @@ extern "C" int mnb_bn_sign_fwd(const float* x, int32_t batch, int32_t channels, 
   return 0;
 }
 
-extern "C" int mnb_bn_sign_bwd(const float* g, const uint32_t* pass_bits, const float* x, int32_t batch, int32_t channels,
-                               int32_t hw, const float* mean, const float* invstd, const float* gamma, int32_t training,
-                               int32_t out_shuffle_groups, float* dx, float* dgamma, float* dbeta, float* dx_channel_sum,
-                               void* scratch, mnb_stream_t stream) {
+template <typename XT>
+static int bn_sign_bwd(const float* g, const uint32_t* pass_bits, const XT* x, const float* dec, int32_t batch, int32_t channels,
+                       int32_t hw, const float* mean, const float* invstd, const float* gamma, int32_t training,
+                       int32_t out_shuffle_groups, float* dx, float* dgamma, float* dbeta, float* dx_channel_sum, void* scratch,
+                       mnb_stream_t stream) {
   MNB_REQUIRE(g && pass_bits && x && mean && invstd && gamma && dx && dgamma && dbeta && scratch, "NULL bn_sign_bwd pointer");
   MNB_REQUIRE(batch > 0 && channels > 0 && channels <= 8192 && hw > 0, "bad bn_sign_bwd shape");
   MNB_REQUIRE(out_shuffle_groups >= 1 && channels % out_shuffle_groups == 0, "shuffle groups %d do not divide %d channels",
@@ -285,23 +291,40 @@ extern "C" int mnb_bn_sign_bwd(const float* g, const uint32_t* pass_bits, const 
   double* partial = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 49152);
   const dim3 grid(channels, splits);
   const float inv_count = 1.f / (float)per;
-  if (planes_vectorizable(n, hw, x, g, dx)) {
-    bn_sign_bwd_reduce_kernel<true><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, batch, channels, hw, out_shuffle_groups, mean,
-                                                                 invstd, dgamma, dbeta, counters, partial);
+  if (planes_vectorizable(n, hw, g, dx, nullptr, x)) {
+    bn_sign_bwd_reduce_kernel<true, XT><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, dec, batch, channels, hw, out_shuffle_groups,
+                                                                     mean, invstd, dgamma, dbeta, counters, partial);
     if (training == 2) { MNB_LAUNCHED(1); return 0; }   // reduce pass only: the caller applies (mnb_bn_sign_bwd_pack)
-    bn_sign_bwd_apply_kernel<true><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, batch, channels, hw, out_shuffle_groups,
-                                                                inv_count, mean, invstd, gamma, dgamma, dbeta, training, dx,
-                                                                dx_channel_sum, counters, partial);
+    bn_sign_bwd_apply_kernel<true, XT><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, dec, batch, channels, hw, out_shuffle_groups,
+                                                                    inv_count, mean, invstd, gamma, dgamma, dbeta, training, dx,
+                                                                    dx_channel_sum, counters, partial);
   } else {
-    bn_sign_bwd_reduce_kernel<false><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, batch, channels, hw, out_shuffle_groups, mean,
-                                                                  invstd, dgamma, dbeta, counters, partial);
+    bn_sign_bwd_reduce_kernel<false, XT><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, dec, batch, channels, hw, out_shuffle_groups,
+                                                                      mean, invstd, dgamma, dbeta, counters, partial);
     if (training == 2) { MNB_LAUNCHED(1); return 0; }
-    bn_sign_bwd_apply_kernel<false><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, batch, channels, hw, out_shuffle_groups,
-                                                                 inv_count, mean, invstd, gamma, dgamma, dbeta, training, dx,
-                                                                 dx_channel_sum, counters, partial);
+    bn_sign_bwd_apply_kernel<false, XT><<<grid, 256, 0, S(stream)>>>(g, pass_bits, x, dec, batch, channels, hw, out_shuffle_groups,
+                                                                     inv_count, mean, invstd, gamma, dgamma, dbeta, training, dx,
+                                                                     dx_channel_sum, counters, partial);
   }
   MNB_LAUNCHED(2);
   return 0;
+}
+
+extern "C" int mnb_bn_sign_bwd(const float* g, const uint32_t* pass_bits, const float* x, int32_t batch, int32_t channels,
+                               int32_t hw, const float* mean, const float* invstd, const float* gamma, int32_t training,
+                               int32_t out_shuffle_groups, float* dx, float* dgamma, float* dbeta, float* dx_channel_sum,
+                               void* scratch, mnb_stream_t stream) {
+  return bn_sign_bwd<float>(g, pass_bits, x, nullptr, batch, channels, hw, mean, invstd, gamma, training, out_shuffle_groups, dx,
+                            dgamma, dbeta, dx_channel_sum, scratch, stream);
+}
+
+extern "C" int mnb_bn_sign_bwd_codes(const float* g, const uint32_t* pass_bits, const int16_t* codes, const float* dec,
+                                     int32_t batch, int32_t channels, int32_t hw, const float* mean, const float* invstd,
+                                     const float* gamma, int32_t training, int32_t out_shuffle_groups, float* dx, float* dgamma,
+                                     float* dbeta, float* dx_channel_sum, void* scratch, mnb_stream_t stream) {
+  MNB_REQUIRE(dec, "NULL decode pair");
+  return bn_sign_bwd<int16_t>(g, pass_bits, codes, dec, batch, channels, hw, mean, invstd, gamma, training, out_shuffle_groups, dx,
+                              dgamma, dbeta, dx_channel_sum, scratch, stream);
 }
 
 // ------------------------------------------------------------------ BatchNorm + sign + MaxPool2d(2, 2) in one pass
@@ -316,7 +339,9 @@ __device__ __forceinline__ uint32_t first_max_of_signs(bool p0, bool p1, bool p2
   return p0 ? 0u : (p1 ? 1u : (p2 ? 2u : (p3 ? 3u : 0u)));
 }
 
-__global__ void __launch_bounds__(256) bn_sign_pool_fwd_kernel(const float4* __restrict__ x, uint32_t n_pairs, PoolGeom gm,
+template <typename XT>
+__global__ void __launch_bounds__(256) bn_sign_pool_fwd_kernel(const XT* __restrict__ x, const float* __restrict__ dec,
+                                                               uint32_t n_pairs, PoolGeom gm,
                                                                const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                float2* __restrict__ y, uchar2* __restrict__ arg,
@@ -333,7 +358,8 @@ __global__ void __launch_bounds__(256) bn_sign_pool_fwd_kernel(const float4* __r
       const uint32_t b = plane / gm.channels, c = plane - b * gm.channels;
       i0 = (plane * gm.H + 2 * oh) * gm.W4 + j;
       const float mu = __ldg(mean + c), sc = __ldg(gamma + c) * __ldg(invstd + c), be = __ldg(beta + c);
-      const float4 r0 = __ldg(x + i0), r1 = __ldg(x + i0 + gm.W4);
+      const XDec d = x_dec<XT>(dec, (int)gm.channels, (int)c);
+      const float4 r0 = x_load4(x + 4 * i0, d), r1 = x_load4(x + 4 * (i0 + gm.W4), d);
       const float v[8] = {fmaf(r0.x - mu, sc, be), fmaf(r0.y - mu, sc, be), fmaf(r0.z - mu, sc, be), fmaf(r0.w - mu, sc, be),
                           fmaf(r1.x - mu, sc, be), fmaf(r1.y - mu, sc, be), fmaf(r1.z - mu, sc, be), fmaf(r1.w - mu, sc, be)};
       bool pos[8];
@@ -356,9 +382,10 @@ __global__ void __launch_bounds__(256) bn_sign_pool_fwd_kernel(const float4* __r
 }
 
 // pass 1 of the backward: dbeta = sum gm, dgamma = sum gm * xhat with gm = pooled gradient at the window winner x pass bit
+template <typename XT>
 __global__ void __launch_bounds__(256) bn_sign_pool_bwd_reduce_kernel(const float2* __restrict__ g, const uchar2* __restrict__ arg,
-                                                                      const uint8_t* __restrict__ bits8, const float* __restrict__ x,
-                                                                      int batch, PoolGeom gm, const float* __restrict__ mean,
+                                                                      const uint8_t* __restrict__ bits8, const XT* __restrict__ x,
+                                                                      const float* __restrict__ dec, int batch, PoolGeom gm, const float* __restrict__ mean,
                                                                       const float* __restrict__ invstd, float* __restrict__ dgamma,
                                                                       float* __restrict__ dbeta, uint32_t* counters, double* partial) {
   __shared__ double red[32];
@@ -366,6 +393,7 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_reduce_kernel(const floa
   const uint32_t c = blockIdx.x, sp = blockIdx.y, nsp = gridDim.y;
   const uint32_t oc = shuffled_channel(c, gm.sg, gm.channels / gm.sg);
   const float mu = __ldg(mean + c), is = __ldg(invstd + c);
+  const XDec d = x_dec<XT>(dec, (int)gm.channels, (int)c);
   const uint32_t b_lo = (uint32_t)((int64_t)batch * sp / nsp), b_hi = (uint32_t)((int64_t)batch * (sp + 1) / nsp);
   const uint32_t per_img = gm.OH * gm.OW2, total = (b_hi - b_lo) * per_img;
   float f1[2] = {0.f, 0.f}, f2[2] = {0.f, 0.f};
@@ -387,7 +415,7 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_reduce_kernel(const floa
           const bool pass = (bits8[i4 >> 1] >> (4u * (i4 & 1u) + col)) & 1u;
           const float gmv = pass ? (w ? gv.y : gv.x) : 0.f;
           f1[u] += gmv;
-          f2[u] += gmv * ((__ldg(x + 4u * i4 + col) - mu) * is);
+          f2[u] += gmv * ((x_val<XT>(__ldg(x + 4u * i4 + col), d) - mu) * is);
         }
       }
     }
@@ -411,9 +439,10 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_reduce_kernel(const floa
 }
 
 // pass 2: dx over the full-resolution plane (+ its channel sums)
+template <typename XT>
 __global__ void __launch_bounds__(256) bn_sign_pool_bwd_apply_kernel(const float2* __restrict__ g, const uchar2* __restrict__ arg,
-                                                                     const uint8_t* __restrict__ bits8, const float4* __restrict__ x,
-                                                                     int batch, PoolGeom gm, float inv_count,
+                                                                     const uint8_t* __restrict__ bits8, const XT* __restrict__ x,
+                                                                     const float* __restrict__ dec, int batch, PoolGeom gm, float inv_count,
                                                                      const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                      const float* __restrict__ gamma, const float* __restrict__ dgamma,
                                                                      const float* __restrict__ dbeta, int training,
@@ -425,6 +454,7 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_apply_kernel(const float
   const uint32_t oc = shuffled_channel(c, gm.sg, gm.channels / gm.sg);
   const float mu = __ldg(mean + c), is = __ldg(invstd + c), k = __ldg(gamma + c) * is;
   const float db = training ? __ldg(dbeta + c) * inv_count : 0.f, dg = training ? __ldg(dgamma + c) * inv_count : 0.f;
+  const XDec d = x_dec<XT>(dec, (int)gm.channels, (int)c);
   const uint32_t b_lo = (uint32_t)((int64_t)batch * sp / nsp), b_hi = (uint32_t)((int64_t)batch * (sp + 1) / nsp);
   const uint32_t per_img = gm.OH * gm.OW2, total = (b_hi - b_lo) * per_img;
   float f = 0.f;
@@ -448,7 +478,7 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_apply_kernel(const float
       }
     }
     if (training) {
-      const float4 r0 = __ldg(x + i0), r1 = __ldg(x + i1);
+      const float4 r0 = x_load4(x + 4 * i0, d), r1 = x_load4(x + 4 * i1, d);
       const float xs[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
 #pragma unroll
       for (int e = 0; e < 8; ++e) v[e] = bn_bwd_centre(v[e], db, (xs[e] - mu) * is, dg);
@@ -474,35 +504,55 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_apply_kernel(const float
   counters[c] = 0;
 }
 
-static int pool_geom(int batch, int channels, int H, int W, int sg, const void* a, const void* b, const void* c, PoolGeom& gm) {
+// x: 4-element loads of element type XT; a, b: fp32 tensors accessed 16 bytes at a time
+template <typename XT>
+static int pool_geom(int batch, int channels, int H, int W, int sg, const XT* x, const void* a, const void* b, PoolGeom& gm) {
   MNB_REQUIRE(batch > 0 && channels > 0 && channels <= 8192 && H > 0 && W > 0, "bad bn_sign_pool shape");
   MNB_REQUIRE(sg >= 1 && channels % sg == 0, "shuffle groups %d do not divide %d channels", sg, channels);
   if ((H & 1) || (W & 7) || (int64_t)batch * channels * H * W >= (1ll << 31) ||
-      (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15))
+      (((uintptr_t)a | (uintptr_t)b) & 15) || ((uintptr_t)x & (4 * sizeof(XT) - 1)))
     return mnb_fail(MNB_E_UNSUPPORTED, "bn_sign_pool needs even H, W %% 8 == 0, < 2^31 elements, 16-byte aligned tensors");
   gm = PoolGeom{(uint32_t)channels, (uint32_t)H, (uint32_t)(W / 4), (uint32_t)(H / 2), (uint32_t)(W / 4), (uint32_t)sg};
+  return 0;
+}
+
+template <typename XT>
+static int bn_sign_pool_fwd(const XT* x, const float* dec, int32_t batch, int32_t channels, int32_t H, int32_t W, const float* mean,
+                            const float* invstd, const float* gamma, const float* beta, int32_t out_shuffle_groups, float* y,
+                            uint32_t* pass_bits, uint8_t* argmax, mnb_stream_t stream) {
+  MNB_REQUIRE(x && mean && invstd && gamma && beta && y && pass_bits && argmax, "NULL bn_sign_pool_fwd pointer");
+  PoolGeom gm;
+  if (int e = pool_geom(batch, channels, H, W, out_shuffle_groups, x, y, nullptr, gm)) return e;
+  const uint32_t n_pairs = (uint32_t)((int64_t)batch * channels * gm.OH * gm.OW2);
+  int blocks = (int)std::min<int64_t>(mnb_ceil_div(n_pairs, 256), MNB_NUM_SMS * 16);
+  bn_sign_pool_fwd_kernel<XT><<<blocks, 256, 0, S(stream)>>>(x, dec, n_pairs, gm, mean, invstd, gamma, beta,
+                                                             reinterpret_cast<float2*>(y), reinterpret_cast<uchar2*>(argmax),
+                                                             reinterpret_cast<uint8_t*>(pass_bits));
+  MNB_LAUNCHED(1);
   return 0;
 }
 
 extern "C" int mnb_bn_sign_pool_fwd(const float* x, int32_t batch, int32_t channels, int32_t H, int32_t W, const float* mean,
                                     const float* invstd, const float* gamma, const float* beta, int32_t out_shuffle_groups,
                                     float* y, uint32_t* pass_bits, uint8_t* argmax, mnb_stream_t stream) {
-  MNB_REQUIRE(x && mean && invstd && gamma && beta && y && pass_bits && argmax, "NULL bn_sign_pool_fwd pointer");
-  PoolGeom gm;
-  if (int e = pool_geom(batch, channels, H, W, out_shuffle_groups, x, y, nullptr, gm)) return e;
-  const uint32_t n_pairs = (uint32_t)((int64_t)batch * channels * gm.OH * gm.OW2);
-  int blocks = (int)std::min<int64_t>(mnb_ceil_div(n_pairs, 256), MNB_NUM_SMS * 16);
-  bn_sign_pool_fwd_kernel<<<blocks, 256, 0, S(stream)>>>(reinterpret_cast<const float4*>(x), n_pairs, gm, mean, invstd, gamma, beta,
-                                                         reinterpret_cast<float2*>(y), reinterpret_cast<uchar2*>(argmax),
-                                                         reinterpret_cast<uint8_t*>(pass_bits));
-  MNB_LAUNCHED(1);
-  return 0;
+  return bn_sign_pool_fwd<float>(x, nullptr, batch, channels, H, W, mean, invstd, gamma, beta, out_shuffle_groups, y, pass_bits,
+                                 argmax, stream);
 }
 
-extern "C" int mnb_bn_sign_pool_bwd(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const float* x, int32_t batch,
-                                    int32_t channels, int32_t H, int32_t W, const float* mean, const float* invstd,
-                                    const float* gamma, int32_t training, int32_t out_shuffle_groups, float* dx, float* dgamma,
-                                    float* dbeta, float* dx_channel_sum, void* scratch, mnb_stream_t stream) {
+extern "C" int mnb_bn_sign_pool_fwd_codes(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t H,
+                                          int32_t W, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                                          int32_t out_shuffle_groups, float* y, uint32_t* pass_bits, uint8_t* argmax,
+                                          mnb_stream_t stream) {
+  MNB_REQUIRE(dec, "NULL decode pair");
+  return bn_sign_pool_fwd<int16_t>(codes, dec, batch, channels, H, W, mean, invstd, gamma, beta, out_shuffle_groups, y, pass_bits,
+                                   argmax, stream);
+}
+
+template <typename XT>
+static int bn_sign_pool_bwd(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const XT* x, const float* dec,
+                            int32_t batch, int32_t channels, int32_t H, int32_t W, const float* mean, const float* invstd,
+                            const float* gamma, int32_t training, int32_t out_shuffle_groups, float* dx, float* dgamma,
+                            float* dbeta, float* dx_channel_sum, void* scratch, mnb_stream_t stream) {
   MNB_REQUIRE(g && pass_bits && argmax && x && mean && invstd && gamma && dx && dgamma && dbeta && scratch,
               "NULL bn_sign_pool_bwd pointer");
   PoolGeom gm;
@@ -514,17 +564,34 @@ extern "C" int mnb_bn_sign_pool_bwd(const float* g, const uint32_t* pass_bits, c
   double* partial = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 49152);
   const dim3 grid(channels, splits);
   const uint8_t* bits8 = reinterpret_cast<const uint8_t*>(pass_bits);
-  bn_sign_pool_bwd_reduce_kernel<<<grid, 256, 0, S(stream)>>>(reinterpret_cast<const float2*>(g),
-                                                              reinterpret_cast<const uchar2*>(argmax), bits8, x, batch, gm, mean,
-                                                              invstd, dgamma, dbeta, counters, partial);
+  bn_sign_pool_bwd_reduce_kernel<XT><<<grid, 256, 0, S(stream)>>>(reinterpret_cast<const float2*>(g),
+                                                                  reinterpret_cast<const uchar2*>(argmax), bits8, x, dec, batch, gm,
+                                                                  mean, invstd, dgamma, dbeta, counters, partial);
   if (training == 2) { MNB_LAUNCHED(1); return 0; }   // reduce pass only: the caller applies (mnb_bn_sign_pool_bwd_pack)
-  bn_sign_pool_bwd_apply_kernel<<<grid, 256, 0, S(stream)>>>(reinterpret_cast<const float2*>(g),
-                                                             reinterpret_cast<const uchar2*>(argmax), bits8,
-                                                             reinterpret_cast<const float4*>(x), batch, gm, 1.f / (float)per, mean,
-                                                             invstd, gamma, dgamma, dbeta, training,
-                                                             reinterpret_cast<float4*>(dx), dx_channel_sum, counters, partial);
+  bn_sign_pool_bwd_apply_kernel<XT><<<grid, 256, 0, S(stream)>>>(reinterpret_cast<const float2*>(g),
+                                                                 reinterpret_cast<const uchar2*>(argmax), bits8, x, dec, batch, gm,
+                                                                 1.f / (float)per, mean, invstd, gamma, dgamma, dbeta, training,
+                                                                 reinterpret_cast<float4*>(dx), dx_channel_sum, counters, partial);
   MNB_LAUNCHED(2);
   return 0;
+}
+
+extern "C" int mnb_bn_sign_pool_bwd(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const float* x, int32_t batch,
+                                    int32_t channels, int32_t H, int32_t W, const float* mean, const float* invstd,
+                                    const float* gamma, int32_t training, int32_t out_shuffle_groups, float* dx, float* dgamma,
+                                    float* dbeta, float* dx_channel_sum, void* scratch, mnb_stream_t stream) {
+  return bn_sign_pool_bwd<float>(g, pass_bits, argmax, x, nullptr, batch, channels, H, W, mean, invstd, gamma, training,
+                                 out_shuffle_groups, dx, dgamma, dbeta, dx_channel_sum, scratch, stream);
+}
+
+extern "C" int mnb_bn_sign_pool_bwd_codes(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const int16_t* codes,
+                                          const float* dec, int32_t batch, int32_t channels, int32_t H, int32_t W,
+                                          const float* mean, const float* invstd, const float* gamma, int32_t training,
+                                          int32_t out_shuffle_groups, float* dx, float* dgamma, float* dbeta,
+                                          float* dx_channel_sum, void* scratch, mnb_stream_t stream) {
+  MNB_REQUIRE(dec, "NULL decode pair");
+  return bn_sign_pool_bwd<int16_t>(g, pass_bits, argmax, codes, dec, batch, channels, H, W, mean, invstd, gamma, training,
+                                   out_shuffle_groups, dx, dgamma, dbeta, dx_channel_sum, scratch, stream);
 }
 
 // ------------------------------------------------------------------ MaxPool2d with a one-byte window index
@@ -686,6 +753,27 @@ extern "C" int mnb_maxpool2d_bwd(const float* g, const uint8_t* argmax, int32_t 
     maxpool_bwd_kernel<<<blocks, 256, 0, S(stream)>>>(g, argmax, n_in, channels, H, W, OH, OW, kernel, stride, pad,
                                                       out_shuffle_groups, dx);
   }
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+// ------------------------------------------------------------------ int16 codes of a wbwtab conv -> its fp32 output
+// (functional.materialized: the values for readers outside the _codes producers; the same fmaf as the conv's epilogue)
+__global__ void __launch_bounds__(256) codes_decode_kernel(const int16_t* __restrict__ codes, const float* __restrict__ dec,
+                                                           int64_t n, int channels, int hw, float* __restrict__ x) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int c = (int)((i / hw) % channels);
+    x[i] = x_val<int16_t>(__ldg(codes + i), x_dec<int16_t>(dec, channels, c));
+  }
+}
+
+extern "C" int mnb_codes_decode(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t hw, float* x,
+                                mnb_stream_t stream) {
+  MNB_REQUIRE(codes && dec && x && batch > 0 && channels > 0 && hw > 0, "bad codes_decode arguments");
+  const int64_t n = (int64_t)batch * channels * hw;
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(n, 256), MNB_NUM_SMS * 8);
+  codes_decode_kernel<<<blocks, 256, 0, S(stream)>>>(codes, dec, n, channels, hw, x);
   MNB_LAUNCHED(1);
   return 0;
 }

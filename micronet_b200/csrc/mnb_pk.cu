@@ -560,9 +560,11 @@ template <> struct PkVec<4> { typedef float4 type; };
 // One warp = 32 * VEC consecutive pixels of one channel octet (the conv's own channel order; g is read in the shuffled
 // order); a lane owns VEC consecutive pixels: 16-byte loads of g and x (VEC = 4), one word of pass bits per channel, VEC
 // consecutive 16-byte pixels per piece plane (one pixel per thread with 4-byte loads is far below HBM bandwidth).
-template <int VEC>
+// XT = int16_t (also in the pooled form below): x as a wbwtab conv's codes + decode pair `dec` (mnb_common.cuh x_load).
+template <int VEC, typename XT>
 __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __restrict__ g, const uint32_t* __restrict__ bits,
-                                                               const float* __restrict__ x, int batch, int channels, int hw,
+                                                               const XT* __restrict__ x, const float* __restrict__ dec,
+                                                               int batch, int channels, int hw,
                                                                int sg, float inv_count, const float* __restrict__ mean,
                                                                const float* __restrict__ invstd, const float* __restrict__ gamma,
                                                                const float* __restrict__ dgamma, const float* __restrict__ dbeta,
@@ -578,7 +580,8 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __re
     const int64_t pl = w / chunks;                                // b * c8n + c8
     const int c8 = (int)(pl % c8n), b = (int)(pl / c8n);
     const int pos = (ch * 32 + lane) * VEC;
-    T gv[8], xv[8];
+    T gv[8];
+    float xf[8][VEC];
     uint32_t bw[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -586,7 +589,7 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __re
       const int oc = sg > 1 ? (c % cpg) * sg + c / cpg : c;      // out[:, a*sg + b] = in[:, b*cpg + a]
       const int64_t fi = ((int64_t)b * channels + c) * hw + pos;
       gv[j] = __ldg(reinterpret_cast<const T*>(g + ((int64_t)b * channels + oc) * hw + pos));
-      xv[j] = __ldg(reinterpret_cast<const T*>(x + fi));
+      x_load<VEC>(x + fi, x_dec<XT>(dec, channels, c), xf[j]);
       bw[j] = __ldg(bits + (fi >> 5)) >> (fi & 31);              // bit i = pass flag of pixel pos + i
     }
     float v[VEC][8];
@@ -597,13 +600,12 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __re
       const float db = __ldg(dbeta + c) * inv_count, dg = __ldg(dgamma + c) * inv_count;
       const float sc = ch_scale ? __ldg(ch_scale + c) : 1.f;
       const float* gf = reinterpret_cast<const float*>(&gv[j]);
-      const float* xf = reinterpret_cast<const float*>(&xv[j]);
       T dv;
       float* df = reinterpret_cast<float*>(&dv);
 #pragma unroll
       for (int i = 0; i < VEC; ++i) {
         float t = ((bw[j] >> i) & 1u) ? gf[i] : 0.f;
-        t = bn_bwd_centre(t, db, (xf[i] - mu) * is, dg);
+        t = bn_bwd_centre(t, db, (xf[j][i] - mu) * is, dg);
         t = k * t;
         df[i] = t;
         v[i][j] = ch_scale ? __fmul_rn(t, sc) : t;
@@ -632,9 +634,10 @@ __global__ void __launch_bounds__(256) bn_sign_bwd_pack_kernel(const float* __re
 // adjacent pooling windows (4 x 2 pixels) of the 8 channels of one octet: per channel one float2 of the pooled gradient
 // (read in the shuffled order), the two window arg-max bytes, the pass nibbles and two float4 of x; per piece plane two
 // runs of 4 consecutive 16-byte pixels.  Layouts of arg / bits8 as written by bn_sign_pool_fwd_kernel (mnb_fused.cu).
+template <typename XT>
 __global__ void __launch_bounds__(256) bn_sign_pool_bwd_pack_kernel(const float2* __restrict__ g, const uchar2* __restrict__ arg,
-                                                                    const uint8_t* __restrict__ bits8, const float4* __restrict__ x,
-                                                                    int batch, int channels, int H, int W4, int sg, float inv_count,
+                                                                    const uint8_t* __restrict__ bits8, const XT* __restrict__ x,
+                                                                    const float* __restrict__ dec, int batch, int channels, int H, int W4, int sg, float inv_count,
                                                                     const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                     const float* __restrict__ gamma, const float* __restrict__ dgamma,
                                                                     const float* __restrict__ dbeta, const float* __restrict__ ch_scale,
@@ -657,7 +660,8 @@ __global__ void __launch_bounds__(256) bn_sign_pool_bwd_pack_kernel(const float2
       const uchar2 a = arg[((size_t)plane * OH + oh) * OW2 + j];
       const uint32_t i0 = (plane * (uint32_t)H + 2u * oh) * (uint32_t)W4 + j, i1 = i0 + (uint32_t)W4;
       const uint32_t n0 = (bits8[i0 >> 1] >> (4u * (i0 & 1u))) & 15u, n1 = (bits8[i1 >> 1] >> (4u * (i1 & 1u))) & 15u;
-      const float4 r0 = __ldg(x + i0), r1 = __ldg(x + i1);
+      const XDec d = x_dec<XT>(dec, channels, (int)c);
+      const float4 r0 = x_load4(x + 4 * i0, d), r1 = x_load4(x + 4 * i1, d);
       const float mu = __ldg(mean + c), is = __ldg(invstd + c), k = __ldg(gamma + c) * is;
       const float db = __ldg(dbeta + c) * inv_count, dg = __ldg(dgamma + c) * inv_count;
       const float sc = ch_scale ? __ldg(ch_scale + c) : 1.f;
@@ -790,6 +794,10 @@ struct ConvParams {
   const uint8_t* bits8;     // dgrad STE mask [B][C8O][OH][OW] or NULL
   float gain;               // dgrad: factor on passed gradients (DoReFa 0.1)
   float* out;               // fp32 NCHW result, or NULL when only the packed output below is wanted
+  // int16 codes (mnb_pk_conv_codes, single-product forward plans only): the exact integer sums as NCHW int16 instead of out,
+  // and dec[2][NOUT] = the (scale, bias) pair of the epilogue, so that a reader rebuilds out as fmaf(code, scale, bias)
+  int16_t* codes;
+  float* dec;
   // fused consumer (inference graphs): the epilogue also applies [ReLU +] the NEXT conv's activation quantizer and writes
   // that conv's operand plane [b][c/8][h][w][8] bf16, or [b][c/16][h][w][16] int8 in the int8 kernels (space-to-depth
   // phase planes for a stride-2 consumer; C8O = 16-byte units per position)
@@ -929,6 +937,9 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           if (p.bias) bs = __ldg(p.bias + n_base + n);
         }
         sh.epi_scale[n] = scv; sh.epi_bias[n] = bs;
+        if constexpr (!SEG && !I8) {   // one snapshot of the decode pair: from the items of M group 0
+          if (p.dec && mg == 0 && y == 0 && n < n_cnt) { p.dec[n_base + n] = scv; p.dec[p.NOUT + n_base + n] = bs; }
+        }
       }
       // ---- MMAs of the item: every stage of every template, all M tiles
       float acc[MAXMT][NR];
@@ -1005,7 +1016,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
       // ---- epilogue
       int mt_cur = -1;
       bool valid = false;
-      float* orow = nullptr;
+      int64_t orow = 0;      // element offset of this thread's output position in channel n_base of out / codes
       const uint8_t* brow = nullptr;
       int64_t prow = 0;      // vector index of this thread's position in octet 0 of the consumer's operand plane
       // one slot = 16 accumulator columns of one M tile
@@ -1021,7 +1032,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           const int b = bt * p.TB + tb, i = rt * p.TH + th, j = ct * p.Wt + wc;
           valid = row_ok && tile < p.n_mtiles && b < p.B && i < p.OHr && j < p.OWr;
           const int oh = i * p.omul + ya, ow = j * p.omul + yb;
-          orow = p.out ? p.out + ((int64_t)b * p.NOUT + n_base) * plane + (int64_t)oh * p.OW + ow : nullptr;
+          orow = ((int64_t)b * p.NOUT + n_base) * plane + (int64_t)oh * p.OW + ow;
           brow = p.bits8 ? p.bits8 + (int64_t)b * p.C8O * plane + (int64_t)oh * p.OW + ow : nullptr;
           if (p.post_out) {
             if (p.post_split)   // octet index (h%2 * 2 + w%2) * C8 + c/8 of a [.., OH/2, OW/2] plane
@@ -1031,6 +1042,13 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           }
         }
         if (!valid || n0 >= n_cnt || (p.dbg & 1)) return;
+        if (!SEG && !I8 && p.codes) {   // exact integer sums (|r| <= 32767: checked on the host) as int16
+          int16_t* cp = p.codes + orow + (int64_t)n0 * plane;
+#pragma unroll
+          for (int k = 0; k < 16; ++k, cp += plane)
+            if (n0 + k < n_cnt) *cp = (int16_t)__float2int_rn(r[k]);
+          return;
+        }
         float sc[16], bs[16];
 #pragma unroll
         for (int v = 0; v < 4; ++v) {
@@ -1039,14 +1057,14 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           sc[4 * v] = a.x; sc[4 * v + 1] = a.y; sc[4 * v + 2] = a.z; sc[4 * v + 3] = a.w;
           bs[4 * v] = c.x; bs[4 * v + 1] = c.y; bs[4 * v + 2] = c.z; bs[4 * v + 3] = c.w;
         }
-        float* op = orow + (int64_t)n0 * plane;
+        float* op = p.out + orow + (int64_t)n0 * plane;
         if (!SEG && p.post_out) {   // (the host refuses a consumer plane on segmented plans)
           // forward conv of a frozen inference graph: y = acc * scale + bias [-> ReLU] -> consumer's quantizer -> bf16 levels
           float lev[16], yv[16];
 #pragma unroll
           for (int k = 0; k < 16; ++k) {
             const float v = fmaf(r[k], sc[k], bs[k]);
-            if (orow && n0 + k < n_cnt) op[(int64_t)k * plane] = v;
+            if (p.out && n0 + k < n_cnt) op[(int64_t)k * plane] = v;
             yv[k] = p.post_relu ? fmaxf(v, 0.f) : v;
           }
           uint32_t passbits;
@@ -1704,10 +1722,11 @@ extern "C" int mnb_pk_pack_act_relu(const float* x, int32_t batch, int32_t chann
   return 0;
 }
 
-extern "C" int mnb_bn_sign_bwd_pack(const float* g, const uint32_t* pass_bits, const float* x, int32_t batch, int32_t channels,
-                                    int32_t hw, const float* mean, const float* invstd, const float* gamma, const float* dgamma,
-                                    const float* dbeta, int32_t out_shuffle_groups, const float* ch_scale, int32_t terms,
-                                    float* dx, void* dy_packed, mnb_stream_t stream) {
+template <typename XT>
+static int bn_sign_bwd_pack(const float* g, const uint32_t* pass_bits, const XT* x, const float* dec, int32_t batch,
+                            int32_t channels, int32_t hw, const float* mean, const float* invstd, const float* gamma,
+                            const float* dgamma, const float* dbeta, int32_t out_shuffle_groups, const float* ch_scale,
+                            int32_t terms, float* dx, void* dy_packed, mnb_stream_t stream) {
   MNB_REQUIRE(g && pass_bits && x && mean && invstd && gamma && dgamma && dbeta && dy_packed, "NULL bn_sign_bwd_pack pointer");
   MNB_REQUIRE(batch > 0 && channels > 0 && hw > 0 && terms >= 1 && terms <= 3, "bad bn_sign_bwd_pack arguments");
   MNB_REQUIRE(out_shuffle_groups >= 1 && channels % out_shuffle_groups == 0, "shuffle groups %d do not divide %d channels",
@@ -1717,18 +1736,62 @@ extern "C" int mnb_bn_sign_bwd_pack(const float* g, const uint32_t* pass_bits, c
   if (hw % 32) return mnb_fail(MNB_E_UNSUPPORTED, "packed BatchNorm backward needs H*W %% 32 == 0");
   const int c8n = channels / 8;
   auto al = [](const void* p, int a) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(a - 1)) == 0; };
-  const int vec = (hw % 128 == 0 && al(g, 16) && al(x, 16) && al(dx, 16)) ? 4 : ((hw % 64 == 0 && al(g, 8) && al(x, 8) && al(dx, 8)) ? 2 : 1);
+  constexpr int xs = (int)sizeof(XT);   // x is loaded VEC elements at a time
+  const int vec = (hw % 128 == 0 && al(g, 16) && al(x, 4 * xs) && al(dx, 16)) ? 4
+                  : ((hw % 64 == 0 && al(g, 8) && al(x, 2 * xs) && al(dx, 8)) ? 2 : 1);
   const int64_t warps = (int64_t)batch * c8n * (hw / (32 * vec));
   const int blocks = (int)std::min<int64_t>(mnb_ceil_div(warps, 8), (int64_t)MNB_NUM_SMS * 8);
   const float inv_count = 1.f / (float)((int64_t)batch * hw);
   uint4* outp = reinterpret_cast<uint4*>(dy_packed);
   const int64_t plane_vecs = (int64_t)batch * c8n * hw;
   cudaStream_t st = (cudaStream_t)stream;
-#define MNB_BWD_PACK(V)                                                                                                      \
-  pk::bn_sign_bwd_pack_kernel<V><<<blocks, 256, 0, st>>>(g, pass_bits, x, batch, channels, hw, out_shuffle_groups, inv_count, \
-                                                         mean, invstd, gamma, dgamma, dbeta, ch_scale, terms, dx, outp, plane_vecs)
+#define MNB_BWD_PACK(V)                                                                                                          \
+  pk::bn_sign_bwd_pack_kernel<V, XT><<<blocks, 256, 0, st>>>(g, pass_bits, x, dec, batch, channels, hw, out_shuffle_groups,     \
+                                                             inv_count, mean, invstd, gamma, dgamma, dbeta, ch_scale, terms, dx, \
+                                                             outp, plane_vecs)
   if (vec == 4) MNB_BWD_PACK(4); else if (vec == 2) MNB_BWD_PACK(2); else MNB_BWD_PACK(1);
 #undef MNB_BWD_PACK
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int mnb_bn_sign_bwd_pack(const float* g, const uint32_t* pass_bits, const float* x, int32_t batch, int32_t channels,
+                                    int32_t hw, const float* mean, const float* invstd, const float* gamma, const float* dgamma,
+                                    const float* dbeta, int32_t out_shuffle_groups, const float* ch_scale, int32_t terms,
+                                    float* dx, void* dy_packed, mnb_stream_t stream) {
+  return bn_sign_bwd_pack<float>(g, pass_bits, x, nullptr, batch, channels, hw, mean, invstd, gamma, dgamma, dbeta,
+                                 out_shuffle_groups, ch_scale, terms, dx, dy_packed, stream);
+}
+
+extern "C" int mnb_bn_sign_bwd_pack_codes(const float* g, const uint32_t* pass_bits, const int16_t* codes, const float* dec,
+                                          int32_t batch, int32_t channels, int32_t hw, const float* mean, const float* invstd,
+                                          const float* gamma, const float* dgamma, const float* dbeta, int32_t out_shuffle_groups,
+                                          const float* ch_scale, int32_t terms, float* dx, void* dy_packed, mnb_stream_t stream) {
+  MNB_REQUIRE(dec, "NULL decode pair");
+  return bn_sign_bwd_pack<int16_t>(g, pass_bits, codes, dec, batch, channels, hw, mean, invstd, gamma, dgamma, dbeta,
+                                   out_shuffle_groups, ch_scale, terms, dx, dy_packed, stream);
+}
+
+template <typename XT>
+static int bn_sign_pool_bwd_pack(const float* g, const uint32_t* pass_bits, const uint8_t* argmax, const XT* x, const float* dec,
+                                 int32_t batch, int32_t channels, int32_t H, int32_t W, const float* mean, const float* invstd,
+                                 const float* gamma, const float* dgamma, const float* dbeta, int32_t out_shuffle_groups,
+                                 const float* ch_scale, int32_t terms, void* dy_packed, mnb_stream_t stream) {
+  MNB_REQUIRE(g && pass_bits && argmax && x && mean && invstd && gamma && dgamma && dbeta && dy_packed, "NULL bn_sign_pool_bwd_pack pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && H > 0 && W > 0 && terms >= 1 && terms <= 3, "bad bn_sign_pool_bwd_pack arguments");
+  MNB_REQUIRE(out_shuffle_groups >= 1 && channels % out_shuffle_groups == 0, "shuffle groups %d do not divide %d channels",
+              out_shuffle_groups, channels);
+  if ((H & 1) || (W & 7) || channels % 8 || (int64_t)batch * channels * H * W >= (1ll << 31) ||
+      (reinterpret_cast<uintptr_t>(x) & (4 * sizeof(XT) - 1)) || (reinterpret_cast<uintptr_t>(dy_packed) & 15) ||
+      (reinterpret_cast<uintptr_t>(g) & 7))
+    return mnb_fail(MNB_E_UNSUPPORTED, "packed pooled BatchNorm backward needs even H, W %% 8 == 0, channels %% 8 == 0, aligned tensors");
+  const int c8n = channels / 8;
+  const int64_t total = (int64_t)batch * c8n * (H / 2) * (W / 4);
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 8);
+  pk::bn_sign_pool_bwd_pack_kernel<XT><<<blocks, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const float2*>(g), reinterpret_cast<const uchar2*>(argmax), reinterpret_cast<const uint8_t*>(pass_bits),
+      x, dec, batch, channels, H, W / 4, out_shuffle_groups, 1.f / (float)((int64_t)batch * H * W), mean,
+      invstd, gamma, dgamma, dbeta, ch_scale, terms, reinterpret_cast<uint4*>(dy_packed), (int64_t)batch * c8n * H * W);
   MNB_LAUNCHED(1);
   return 0;
 }
@@ -1738,22 +1801,18 @@ extern "C" int mnb_bn_sign_pool_bwd_pack(const float* g, const uint32_t* pass_bi
                                          const float* invstd, const float* gamma, const float* dgamma, const float* dbeta,
                                          int32_t out_shuffle_groups, const float* ch_scale, int32_t terms, void* dy_packed,
                                          mnb_stream_t stream) {
-  MNB_REQUIRE(g && pass_bits && argmax && x && mean && invstd && gamma && dgamma && dbeta && dy_packed, "NULL bn_sign_pool_bwd_pack pointer");
-  MNB_REQUIRE(batch > 0 && channels > 0 && H > 0 && W > 0 && terms >= 1 && terms <= 3, "bad bn_sign_pool_bwd_pack arguments");
-  MNB_REQUIRE(out_shuffle_groups >= 1 && channels % out_shuffle_groups == 0, "shuffle groups %d do not divide %d channels",
-              out_shuffle_groups, channels);
-  if ((H & 1) || (W & 7) || channels % 8 || (int64_t)batch * channels * H * W >= (1ll << 31) ||
-      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy_packed)) & 15) || (reinterpret_cast<uintptr_t>(g) & 7))
-    return mnb_fail(MNB_E_UNSUPPORTED, "packed pooled BatchNorm backward needs even H, W %% 8 == 0, channels %% 8 == 0, aligned tensors");
-  const int c8n = channels / 8;
-  const int64_t total = (int64_t)batch * c8n * (H / 2) * (W / 4);
-  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 8);
-  pk::bn_sign_pool_bwd_pack_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const float2*>(g), reinterpret_cast<const uchar2*>(argmax), reinterpret_cast<const uint8_t*>(pass_bits),
-      reinterpret_cast<const float4*>(x), batch, channels, H, W / 4, out_shuffle_groups, 1.f / (float)((int64_t)batch * H * W), mean,
-      invstd, gamma, dgamma, dbeta, ch_scale, terms, reinterpret_cast<uint4*>(dy_packed), (int64_t)batch * c8n * H * W);
-  MNB_LAUNCHED(1);
-  return 0;
+  return bn_sign_pool_bwd_pack<float>(g, pass_bits, argmax, x, nullptr, batch, channels, H, W, mean, invstd, gamma, dgamma, dbeta,
+                                      out_shuffle_groups, ch_scale, terms, dy_packed, stream);
+}
+
+extern "C" int mnb_bn_sign_pool_bwd_pack_codes(const float* g, const uint32_t* pass_bits, const uint8_t* argmax,
+                                               const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t H,
+                                               int32_t W, const float* mean, const float* invstd, const float* gamma,
+                                               const float* dgamma, const float* dbeta, int32_t out_shuffle_groups,
+                                               const float* ch_scale, int32_t terms, void* dy_packed, mnb_stream_t stream) {
+  MNB_REQUIRE(dec, "NULL decode pair");
+  return bn_sign_pool_bwd_pack<int16_t>(g, pass_bits, argmax, codes, dec, batch, channels, H, W, mean, invstd, gamma, dgamma,
+                                        dbeta, out_shuffle_groups, ch_scale, terms, dy_packed, stream);
 }
 
 extern "C" int mnb_quant_add_pack_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
@@ -1822,11 +1881,17 @@ extern "C" int mnb_pk_pack_weight(const mnb_conv_shape* s, int32_t mode, int32_t
 static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
                         int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
                         const float* bias, const uint8_t* bits8, float gain, float* out, const mnb_pk_post* post,
-                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8) {
+                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8, int16_t* codes = nullptr, float* dec = nullptr) {
   using namespace pk;
-  MNB_REQUIRE(s && a_pk && w_img && (out || post) && err_flag, "NULL pk_conv pointer");
+  MNB_REQUIRE(s && a_pk && w_img && (out || post || codes) && err_flag, "NULL pk_conv pointer");
   Plan pl;
   if (int e = make_plan(s, mode, terms_a, terms_w, pl, cpu)) return e;
+  if (codes) {
+    MNB_REQUIRE(mode == 0 && cpu == 8 && !out && !post && !bits8 && dec, "pk conv: int16 codes are a plain forward output");
+    // the int16 store is compiled into the single-product kernels only; one piece per operand keeps the sums exact integers
+    if (pl.segmented || terms_a != 1 || terms_w != 1)
+      return unsupported("int16 codes need one activation piece, one weight piece and a non-segmented plan");
+  }
   if (post && cpu == 16) {   // int8 consumer plane: s8 levels of a symmetric IAO quantizer, 16-channel units
     MNB_REQUIRE(post->q && post->out_pk && (reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "pk conv: consumer plane / quantizer");
     if (post->q->mode != MNB_ACT_IAO || post->q->q_type != 0 || post->q->bits < 2 || post->q->bits > 8 || post->q->qmin < -128 ||
@@ -1888,7 +1953,7 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = ceil_div(pl.NOUT, cpu); p.smem_bytes = pl.smem_bytes; p.off_stg = pl.off_stg;
   p.mode = mode;
   p.n_scale = n_scale; p.a_scale = a_scale; p.a_scale_const = a_scale_const; p.bias = bias; p.bits8 = bits8; p.gain = gain;
-  p.out = out; p.err = err_flag;
+  p.out = out; p.err = err_flag; p.codes = codes; p.dec = dec;
   if (post) {
     p.post_out = reinterpret_cast<uint4*>(post->out_pk); p.post_q = *post->q; p.post_relu = post->relu; p.post_split = post->phase_split;
   }
@@ -1933,6 +1998,19 @@ extern "C" int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32
   MNB_REQUIRE(post, "NULL consumer description");
   return pk_conv_impl(s, 0, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, out, post,
                       err_flag, stream);
+}
+
+extern "C" int mnb_pk_conv_codes(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
+                                 const float* n_scale, const float* a_scale, float a_scale_const, const float* bias,
+                                 int32_t level_bound, int16_t* codes, float* dec, int32_t* err_flag, mnb_stream_t stream) {
+  MNB_REQUIRE(s && codes && dec, "NULL pk_conv_codes pointer");
+  MNB_REQUIRE(level_bound >= 1 && s->groups >= 1, "pk_conv_codes: level bound %d", level_bound);
+  // |sum| <= (C/g) * R * S * max|level| for a +-1 activation plane: the bound under which every sum is an exact int16
+  if ((int64_t)(s->in_c / s->groups) * s->ker_h * s->ker_w * level_bound > 32767)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_conv_codes: sums of %d x %d x %d terms of level %d may exceed int16", s->in_c / s->groups,
+                    s->ker_h, s->ker_w, level_bound);
+  return pk_conv_impl(s, 0, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, nullptr, nullptr,
+                      err_flag, stream, 8, codes, dec);
 }
 
 // ---- int8 operands (inference): symmetric IAO levels as s8, s8 x s8 -> s32 wgmma

@@ -624,8 +624,11 @@ struct MnbBnUpdate {
   float* running_mean; float* running_var; long long* num_batches_tracked;
 };
 
-__global__ void __launch_bounds__(256) channel_stats_kernel(const float* __restrict__ x, int batch, int channels,
-                                                            int hw, int as_mean_var, float* __restrict__ stats,
+// XT = int16_t: x as the codes of a wbwtab conv with their decode pair `dec` (mnb_common.cuh x_load); the loads are half as
+// wide, the element-to-accumulator mapping and every sum are those of the fp32 form.
+template <typename XT>
+__global__ void __launch_bounds__(256) channel_stats_kernel(const XT* __restrict__ x, const float* __restrict__ dec, int batch,
+                                                            int channels, int hw, int as_mean_var, float* __restrict__ stats,
                                                             uint32_t* counters, double* partial, MnbBnUpdate bn) {
   __shared__ double red[32];
   __shared__ bool last;
@@ -635,14 +638,14 @@ __global__ void __launch_bounds__(256) channel_stats_kernel(const float* __restr
   // Sums are taken of (x - pivot), pivot = the channel's first value: sum(x^2) - N mean^2 in fp32 partials cancels
   // catastrophically when |mean| >> std (a conv with a large bias); the shifted form is exact to fp32 rounding of the
   // deviations (as_mean_var == 0, plain sums for bias gradients, keeps pivot 0).
-  const float pivot = as_mean_var ? __ldg(x + (int64_t)c * hw) : 0.f;
+  const XDec d = x_dec<XT>(dec, channels, c);
+  const float pivot = as_mean_var ? x_val<XT>(__ldg(x + (int64_t)c * hw), d) : 0.f;
   // images [b_lo, b_hi) of this split.  The (image, offset) pairs of the split are walked as one flat index
   // space so that small planes (8x8) still keep every thread loading; fp32 partials per thread, fp64 across.
   const int b_lo = (int)((int64_t)batch * sp / nsp), b_hi = (int)((int64_t)batch * (sp + 1) / nsp);
-  const bool vec = (hw & 3) == 0 && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
+  const bool vec = (hw & 3) == 0 && ((reinterpret_cast<uintptr_t>(x) & (4 * sizeof(XT) - 1)) == 0);
   if (vec) {
     const uint32_t hw4 = (uint32_t)hw >> 2, total = (uint32_t)(b_hi - b_lo) * hw4;
-    const float4* base = reinterpret_cast<const float4*>(x);
     float f1[4] = {0.f, 0.f, 0.f, 0.f}, f2[4] = {0.f, 0.f, 0.f, 0.f};
     for (uint32_t t0 = threadIdx.x; t0 < total; t0 += 4 * blockDim.x) {
 #pragma unroll
@@ -650,7 +653,7 @@ __global__ void __launch_bounds__(256) channel_stats_kernel(const float* __restr
         const uint32_t t = t0 + u * blockDim.x;
         if (t < total) {
           const uint32_t b = t / hw4, i = t - b * hw4;
-          float4 v = __ldg(base + ((int64_t)(b_lo + b) * channels + c) * hw4 + i);
+          float4 v = x_load4(x + 4 * (((int64_t)(b_lo + b) * channels + c) * hw4 + i), d);
           v.x -= pivot; v.y -= pivot; v.z -= pivot; v.w -= pivot;
           f1[u] += (v.x + v.y) + (v.z + v.w);
           f2[u] += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
@@ -661,10 +664,10 @@ __global__ void __launch_bounds__(256) channel_stats_kernel(const float* __restr
     s2 = ((double)f2[0] + (double)f2[1]) + ((double)f2[2] + (double)f2[3]);
   } else {
     for (int b = b_lo; b < b_hi; ++b) {
-      const float* plane = x + ((int64_t)b * channels + c) * hw;
+      const XT* plane = x + ((int64_t)b * channels + c) * hw;
       float f1 = 0.f, f2 = 0.f;
       for (int i = threadIdx.x; i < hw; i += blockDim.x) {
-        const float v = __ldg(plane + i) - pivot;
+        const float v = x_val<XT>(__ldg(plane + i), d) - pivot;
         f1 += v; f2 += v * v;
       }
       s1 += (double)f1;
@@ -739,15 +742,16 @@ extern "C" int mnb_channel_stats(const float* x, int32_t batch, int32_t channels
   uint32_t* counters = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(scratch) + 16384);
   double* partial = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 49152);
   MNB_REQUIRE(as_mean_var >= 0 && as_mean_var <= 2, "as_mean_var must be 0, 1 or 2");
-  channel_stats_kernel<<<dim3(channels, splits), 256, 0, S(stream)>>>(x, batch, channels, hw, as_mean_var, stats,
-                                                                       counters, partial, MnbBnUpdate{});
+  channel_stats_kernel<float><<<dim3(channels, splits), 256, 0, S(stream)>>>(x, nullptr, batch, channels, hw, as_mean_var,
+                                                                              stats, counters, partial, MnbBnUpdate{});
   MNB_LAUNCHED(1);
   return 0;
 }
 
-extern "C" int mnb_bn_batch_stats(const float* x, int32_t batch, int32_t channels, int32_t hw, double eps, double momentum,
-                                  float* running_mean, float* running_var, int64_t* num_batches_tracked,
-                                  float* mean_invstd, void* scratch, mnb_stream_t stream) {
+template <typename XT>
+static int bn_batch_stats(const XT* x, const float* dec, int32_t batch, int32_t channels, int32_t hw, double eps, double momentum,
+                          float* running_mean, float* running_var, int64_t* num_batches_tracked, float* mean_invstd,
+                          void* scratch, mnb_stream_t stream) {
   MNB_REQUIRE(x && running_mean && running_var && mean_invstd && scratch && batch > 0 && channels > 0 && hw > 0,
               "bad bn_batch_stats arguments");
   MNB_REQUIRE(channels <= 8192, "bn_batch_stats supports at most 8192 channels, got %d", channels);
@@ -758,10 +762,25 @@ extern "C" int mnb_bn_batch_stats(const float* x, int32_t batch, int32_t channel
   uint32_t* counters = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(scratch) + 16384);
   double* partial = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 49152);
   MnbBnUpdate bn{eps, (float)momentum, running_mean, running_var, reinterpret_cast<long long*>(num_batches_tracked)};
-  channel_stats_kernel<<<dim3(channels, splits), 256, 0, S(stream)>>>(x, batch, channels, hw, 3, mean_invstd, counters,
-                                                                       partial, bn);
+  channel_stats_kernel<XT><<<dim3(channels, splits), 256, 0, S(stream)>>>(x, dec, batch, channels, hw, 3, mean_invstd, counters,
+                                                                           partial, bn);
   MNB_LAUNCHED(1);
   return 0;
+}
+
+extern "C" int mnb_bn_batch_stats(const float* x, int32_t batch, int32_t channels, int32_t hw, double eps, double momentum,
+                                  float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                                  float* mean_invstd, void* scratch, mnb_stream_t stream) {
+  return bn_batch_stats<float>(x, nullptr, batch, channels, hw, eps, momentum, running_mean, running_var, num_batches_tracked,
+                               mean_invstd, scratch, stream);
+}
+
+extern "C" int mnb_bn_batch_stats_codes(const int16_t* codes, const float* dec, int32_t batch, int32_t channels, int32_t hw,
+                                        double eps, double momentum, float* running_mean, float* running_var,
+                                        int64_t* num_batches_tracked, float* mean_invstd, void* scratch, mnb_stream_t stream) {
+  MNB_REQUIRE(dec, "NULL decode pair");
+  return bn_batch_stats<int16_t>(codes, dec, batch, channels, hw, eps, momentum, running_mean, running_var, num_batches_tracked,
+                                 mean_invstd, scratch, stream);
 }
 
 extern "C" int mnb_channel_stats_bwd(const float* x, const float* mean, const float* dmean, const float* dvar,

@@ -282,8 +282,16 @@ def channel_sums(x4):
 
 def materialized(t):
     """the values of a producer output: ``t`` itself, or - for a plane-only output of a fused BatchNorm + binarizer (its fp32
-    storage was never written) - the +-1 tensor rebuilt from the bf16 operand plane [b][c/8][h][w][8].  Plumbing for tests,
-    hooks and convs outside the packed-operand cover; the training step never calls it."""
+    storage was never written) - the +-1 tensor rebuilt from the bf16 operand plane [b][c/8][h][w][8], or - for a wbwtab conv
+    that handed its output to its BatchNorm as int16 codes (``codes_out``) - that output decoded with the conv epilogue's own
+    fmaf.  Plumbing for tests, hooks and readers outside the fused producers; the training step never calls it."""
+    codes = getattr(t, "_mnb_codes", None)
+    if codes is not None:
+        b, c = t.shape[0], t.shape[1]
+        out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
+        L.check(L.load().mnb_codes_decode(codes[0].data_ptr(), codes[1].data_ptr(), b, c, t.numel() // (b * c), out.data_ptr(),
+                                          L.stream()), "codes_decode")
+        return out
     if not getattr(t, "_mnb_plane_only", False):
         return t
     b, c, h, w = t.shape
@@ -315,9 +323,13 @@ def _pk_terms(spec, w_int, pm1=False):
     return ta, (1 if w_int is not None else T)
 
 
-def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, need_dx, prepacked=None, pre_relu=False, pm1=False):
+def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, need_dx, prepacked=None, pre_relu=False, pm1=False,
+                codes_out=False):
     """forward on the packed-operand tensor-core family; returns False when the shape is outside its cover.
-    ``prepacked``: the operand plane a fused producer (fused.BNReluQuantFn) already wrote - x itself holds no data then."""
+    ``prepacked``: the operand plane a fused producer (fused.BNReluQuantFn) already wrote - x itself holds no data then.
+    ``codes_out`` (wbwtab layer on a +-1 input whose only reader is its fused BatchNorm + binarizer): the exact integer sums
+    go out as int16 codes with their decode pair, tagged on y as ``_mnb_codes``; y itself is then not written.  Shapes the
+    int16 hand-off does not cover write y as usual."""
     from . import pk as PK
     ta, tw = _pk_terms(spec, w_int, pm1)
     if not PK.supported(sh, 0, ta, tw):
@@ -350,8 +362,18 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, need_dx, prepacke
             a_scale = spec.scale.clone() if (need_dx or ctx.needs_input_grad[1]) else spec.scale
         elif spec.mode == L.ACT_DOREFA:
             a_const = 1.0 / float(2 ** spec.bits - 1)
-    rc = _timed("fwd_pk", sh, lambda: PK.conv(sh, 0, x_pk, ta, w_img, tw, y, n_scale=w_scale if w_int is not None else None,
-                                              a_scale=a_scale, a_scale_const=a_const, bias=bias))
+    rc = L.E_UNSUPPORTED
+    if codes_out and w_int is not None and ta == 1 and tw == 1:
+        codes = torch.empty(y.shape, dtype=torch.int16, device=y.device)
+        dec = torch.empty(2 * y.shape[1], dtype=torch.float32, device=y.device)
+        rc = _timed("fwd_pk", sh, lambda: PK.conv_codes(sh, x_pk, w_img, codes, dec, n_scale=w_scale, a_scale=a_scale,
+                                                        a_scale_const=a_const, bias=bias))
+        if rc == 0:
+            y._mnb_codes = (codes, dec)
+    if rc == L.E_UNSUPPORTED:
+        rc = _timed("fwd_pk", sh, lambda: PK.conv(sh, 0, x_pk, ta, w_img, tw, y,
+                                                  n_scale=w_scale if w_int is not None else None,
+                                                  a_scale=a_scale, a_scale_const=a_const, bias=bias))
     if rc == L.E_UNSUPPORTED:
         return False
     L.check(rc, "pk_conv fwd")
@@ -406,7 +428,8 @@ class QuantConv2dFn(Function):
     and the clip-STE fused into dgrad.  ``spec`` None => x is used as fp32 (wbwtab, a_bits=32)."""
 
     @staticmethod
-    def forward(ctx, x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, no_grad=False):
+    def forward(ctx, x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, no_grad=False,
+                codes_out=False):
         L.require_cuda(x, wq)
         assert not (pre_relu and any(ctx.needs_input_grad)), "the folded ReLU is an inference-only fusion"
         lib = L.load()
@@ -455,7 +478,7 @@ class QuantConv2dFn(Function):
             if pm1_plane is not None and pm1_plane.numel() != x.numel() * 2:
                 pm1_plane = None
             done = _pk_forward(ctx, x, wq, bias, w_int, w_scale, None, sh, y, ctx.needs_input_grad[0], prepacked=pm1_plane,
-                               pm1=True)
+                               pm1=True, codes_out=codes_out)
         if (not done and L.PK_MODE != "off" and spec is None and w_int is None and x.dtype == torch.float32
                 and getattr(x, "_mnb_pm1", False) and not pre_relu):
             # un-quantized conv behind a binarizer (the 10-way head of a wbwtab model, fused.EnginePmConv2d): the +-1 input is
@@ -554,7 +577,7 @@ class QuantConv2dFn(Function):
             db = presummed if presummed is not None and presummed.numel() == dy.shape[1] else channel_sums(dy)
         if ctx.pk:
             dx, dwq = _pk_backward(ctx, dy)
-            return dx, dwq, db, None, None, None, None, None, None, None, None, None
+            return dx, dwq, db, None, None, None, None, None, None, None, None, None, None
         if ctx.needs_input_grad[0]:
             dx = torch.empty((sh.batch, sh.in_c, sh.in_h, sh.in_w), dtype=torch.float32, device=dy.device)
             qp = spec.struct() if spec is not None else None
@@ -615,14 +638,14 @@ class QuantConv2dFn(Function):
                 L.check(_timed("wgrad", sh, lambda: lib.mnb_conv2d_wgrad(
                     C.byref(sh), dy.data_ptr(), C.byref(ops), dwq.data_ptr(), ws.data_ptr(), L.stream())),
                     "conv2d_wgrad")
-        return dx, dwq, db, None, None, None, None, None, None, None, None, None
+        return dx, dwq, db, None, None, None, None, None, None, None, None, None, None
 
 
-def quant_conv2d(x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False):
+def quant_conv2d(x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, codes_out=False):
     # (autograd runs a Function's forward with grad mode off and needs_input_grad ignores torch.no_grad(): whether this call
     # will ever be differentiated is only known out here)
     return QuantConv2dFn.apply(x, wq, bias, w_int, w_scale, spec, tuple(stride), tuple(padding),
-                               tuple(dilation), groups, pre_relu, not torch.is_grad_enabled())
+                               tuple(dilation), groups, pre_relu, not torch.is_grad_enabled(), codes_out)
 
 
 # --------------------------------------------------------------------------

@@ -29,24 +29,40 @@ import torch.nn.functional as TF
 from . import _lib as L
 
 
+def _xargs(lib, name, x, codes):
+    """(entry point, leading x arguments) of a producer call: the fp32 form on x, or its _codes form on the int16 codes and
+    decode pair that the producing wbwtab conv handed over instead of writing x"""
+    if codes is None:
+        return getattr(lib, name), (x.data_ptr(),)
+    return getattr(lib, name + "_codes"), (codes[0].data_ptr(), codes[1].data_ptr())
+
+
 class BNSignFn(Function):
     """sign(batch_norm(x)) [-> max_pool2d(2, 2)] [-> channel_shuffle] with the saturate STE"""
 
     @staticmethod
     def forward(ctx, x, gamma, beta, mean, invstd, training, shuffle_groups, pool, plane_only=False):
+        from . import functional as F_
         lib = L.load()
         x = x.contiguous()
         b, c = x.shape[0], x.shape[1]
         hw = x.numel() // (b * c)
+        # the conv that produced x ran on the packed-operand family (functional.QuantConv2dFn tags its output): its
+        # gradient operand is written by this backward, pre-multiplied with the conv's per-channel weight scale
+        pk_conv = getattr(x, "_mnb_pk_conv", None)
+        codes = getattr(x, "_mnb_codes", None)     # x holds no data: the conv handed over int16 codes (functional._pk_forward)
+        if codes is not None and not pool and (L.USE_PACKED or not (L.PK_WBWTAB and c % 8 == 0 and hw % 32 == 0
+                                                                    and x.dim() == 4 and L.PK_MODE != "off")):
+            x, codes = F_.materialized(x), None     # below, only the packed producer reads codes
         bits = torch.empty((x.numel() + 31) // 32, dtype=torch.int32, device=x.device)
         arg = None
         if pool:
             h, w = x.shape[2], x.shape[3]
             y = torch.empty((b, c, h // 2, w // 2), dtype=x.dtype, device=x.device)
             arg = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)
-            L.check(lib.mnb_bn_sign_pool_fwd(x.data_ptr(), b, c, h, w, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
-                                             beta.data_ptr(), shuffle_groups, y.data_ptr(), bits.data_ptr(), arg.data_ptr(),
-                                             L.stream()), "bn_sign_pool_fwd")
+            fn, xa = _xargs(lib, "mnb_bn_sign_pool_fwd", x, codes)
+            L.check(fn(*xa, b, c, h, w, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(), beta.data_ptr(), shuffle_groups,
+                       y.data_ptr(), bits.data_ptr(), arg.data_ptr(), L.stream()), "bn_sign_pool_fwd")
         else:
             y = torch.empty_like(x)
             packed = None
@@ -57,9 +73,9 @@ class BNSignFn(Function):
                 # plane_only (set by the rewrite pass when the ONLY reader is a conv of the packed-operand family): the fp32
                 # tensor is a shape-carrying placeholder, 4 of the 10 bytes per element this pass moved are never written
                 skip_y = bool(plane_only) and L.PLANE_ONLY
-                rc = lib.mnb_bn_sign_fwd_packed(x.data_ptr(), b, c, hw, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
-                                                beta.data_ptr(), shuffle_groups, None if skip_y else y.data_ptr(),
-                                                bits.data_ptr(), plane.data_ptr(), L.stream())
+                fn, xa = _xargs(lib, "mnb_bn_sign_fwd_packed", x, codes)
+                rc = fn(*xa, b, c, hw, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(), beta.data_ptr(), shuffle_groups,
+                        None if skip_y else y.data_ptr(), bits.data_ptr(), plane.data_ptr(), L.stream())
                 if rc == 0:
                     y._mnb_pk_pm1 = plane
                     if skip_y:
@@ -67,6 +83,8 @@ class BNSignFn(Function):
                     packed = False          # done (not the experimental bf16 tensor of MNB_PACKED_OPERANDS)
                 elif rc != L.E_UNSUPPORTED:
                     L.check(rc, "bn_sign_fwd_packed")
+                elif codes is not None:
+                    x, codes = F_.materialized(x), None
             if packed is None and L.USE_PACKED and c % 8 == 0 and hw % 32 == 0:
                 # experimental (MNB_PACKED_OPERANDS=1): also emit the bf16 position-major operand of the next conv
                 packed = torch.empty(x.numel(), dtype=torch.bfloat16, device=x.device)
@@ -86,9 +104,7 @@ class BNSignFn(Function):
         y._mnb_pm1 = True        # exactly +-1: a consuming conv may pack it as ONE bf16 piece
         ctx.save_for_backward(x, gamma, mean, invstd)
         ctx.bits, ctx.arg, ctx.training, ctx.shuffle_groups = bits, arg, training, shuffle_groups
-        # the conv that produced x ran on the packed-operand family (functional.QuantConv2dFn tags its output): its
-        # gradient operand is written by this backward, pre-multiplied with the conv's per-channel weight scale
-        ctx.pk_conv = getattr(x, "_mnb_pk_conv", None)
+        ctx.pk_conv, ctx.codes = pk_conv, codes    # the backward reads x through the same codes
         return y
 
     @staticmethod
@@ -107,44 +123,44 @@ class BNSignFn(Function):
             # pooled producer behind a conv of the packed-operand family: reduce pass (dgamma, dbeta), then the apply pass
             # writes the full-resolution gradient straight as that conv's packed operand (no fp32 dx, no pack pass)
             w_scale, T = ctx.pk_conv
-            L.check(lib.mnb_bn_sign_pool_bwd(g.data_ptr(), ctx.bits.data_ptr(), ctx.arg.data_ptr(), x.data_ptr(), b, c,
-                                             x.shape[2], x.shape[3], mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
-                                             2, ctx.shuffle_groups, dx.data_ptr(), dgamma.data_ptr(),
-                                             dbeta.data_ptr(), None, scratch.data_ptr(), L.stream()), "bn_sign_pool_bwd (reduce)")
+            fn, xa = _xargs(lib, "mnb_bn_sign_pool_bwd", x, ctx.codes)
+            L.check(fn(g.data_ptr(), ctx.bits.data_ptr(), ctx.arg.data_ptr(), *xa, b, c, x.shape[2], x.shape[3],
+                       mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(), 2, ctx.shuffle_groups, dx.data_ptr(),
+                       dgamma.data_ptr(), dbeta.data_ptr(), None, scratch.data_ptr(), L.stream()), "bn_sign_pool_bwd (reduce)")
             dy_pk = torch.empty(T * x.numel() * 2, dtype=torch.uint8, device=x.device)
-            L.check(lib.mnb_bn_sign_pool_bwd_pack(g.data_ptr(), ctx.bits.data_ptr(), ctx.arg.data_ptr(), x.data_ptr(), b, c,
-                                                  x.shape[2], x.shape[3], mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
-                                                  dgamma.data_ptr(), dbeta.data_ptr(), ctx.shuffle_groups, L.ptr(w_scale), T,
-                                                  dy_pk.data_ptr(), L.stream()), "bn_sign_pool_bwd_pack")
+            fn, xa = _xargs(lib, "mnb_bn_sign_pool_bwd_pack", x, ctx.codes)
+            L.check(fn(g.data_ptr(), ctx.bits.data_ptr(), ctx.arg.data_ptr(), *xa, b, c, x.shape[2], x.shape[3],
+                       mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
+                       ctx.shuffle_groups, L.ptr(w_scale), T, dy_pk.data_ptr(), L.stream()), "bn_sign_pool_bwd_pack")
             dx_sum.zero_()
             dx._mnb_pk_dy = (dy_pk, T, w_scale)     # dx itself is NOT written: its only reader is that conv's backward
         elif ctx.arg is not None:
-            L.check(lib.mnb_bn_sign_pool_bwd(g.data_ptr(), ctx.bits.data_ptr(), ctx.arg.data_ptr(), x.data_ptr(), b, c,
-                                             x.shape[2], x.shape[3], mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
-                                             1 if ctx.training else 0, ctx.shuffle_groups, dx.data_ptr(), dgamma.data_ptr(),
-                                             dbeta.data_ptr(), dx_sum.data_ptr(), scratch.data_ptr(), L.stream()),
+            fn, xa = _xargs(lib, "mnb_bn_sign_pool_bwd", x, ctx.codes)
+            L.check(fn(g.data_ptr(), ctx.bits.data_ptr(), ctx.arg.data_ptr(), *xa, b, c, x.shape[2], x.shape[3],
+                       mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(), 1 if ctx.training else 0, ctx.shuffle_groups,
+                       dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), dx_sum.data_ptr(), scratch.data_ptr(), L.stream()),
                     "bn_sign_pool_bwd")
         elif ctx.pk_conv is not None and ctx.training and c % 8 == 0 and "mnb_bn_sign_bwd_pack" in L.PROTOTYPES:
             # reduce pass of mnb_bn_sign_bwd (dgamma, dbeta), then the apply pass that writes dx as the producing conv's packed
             # gradient operand.  The channel sums of dx (that conv's bias gradient) are exactly zero behind a training-mode
             # BatchNorm; the reference's value is the rounding noise of that sum.
             w_scale, T = ctx.pk_conv
-            L.check(lib.mnb_bn_sign_bwd(g.data_ptr(), ctx.bits.data_ptr(), x.data_ptr(), b, c, hw, mean.data_ptr(),
-                                        invstd.data_ptr(), gamma.data_ptr(), 2, ctx.shuffle_groups,
-                                        dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), None,
-                                        scratch.data_ptr(), L.stream()), "bn_sign_bwd (reduce)")
+            fn, xa = _xargs(lib, "mnb_bn_sign_bwd", x, ctx.codes)
+            L.check(fn(g.data_ptr(), ctx.bits.data_ptr(), *xa, b, c, hw, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
+                       2, ctx.shuffle_groups, dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), None, scratch.data_ptr(),
+                       L.stream()), "bn_sign_bwd (reduce)")
             dy_pk = torch.empty(T * x.numel() * 2, dtype=torch.uint8, device=x.device)
-            L.check(lib.mnb_bn_sign_bwd_pack(g.data_ptr(), ctx.bits.data_ptr(), x.data_ptr(), b, c, hw, mean.data_ptr(),
-                                             invstd.data_ptr(), gamma.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
-                                             ctx.shuffle_groups, L.ptr(w_scale), T, None, dy_pk.data_ptr(), L.stream()),
-                    "bn_sign_bwd_pack")
+            fn, xa = _xargs(lib, "mnb_bn_sign_bwd_pack", x, ctx.codes)
+            L.check(fn(g.data_ptr(), ctx.bits.data_ptr(), *xa, b, c, hw, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
+                       dgamma.data_ptr(), dbeta.data_ptr(), ctx.shuffle_groups, L.ptr(w_scale), T, None, dy_pk.data_ptr(),
+                       L.stream()), "bn_sign_bwd_pack")
             dx_sum.zero_()
             dx._mnb_pk_dy = (dy_pk, T, w_scale)     # dx itself is NOT written: its only reader is that conv's backward
         else:
-            L.check(lib.mnb_bn_sign_bwd(g.data_ptr(), ctx.bits.data_ptr(), x.data_ptr(), b, c, hw, mean.data_ptr(),
-                                        invstd.data_ptr(), gamma.data_ptr(), 1 if ctx.training else 0, ctx.shuffle_groups,
-                                        dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), dx_sum.data_ptr(),
-                                        scratch.data_ptr(), L.stream()), "bn_sign_bwd")
+            fn, xa = _xargs(lib, "mnb_bn_sign_bwd", x, ctx.codes)
+            L.check(fn(g.data_ptr(), ctx.bits.data_ptr(), *xa, b, c, hw, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
+                       1 if ctx.training else 0, ctx.shuffle_groups, dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
+                       dx_sum.data_ptr(), scratch.data_ptr(), L.stream()), "bn_sign_bwd")
         # picked up by QuantConv2dFn.backward when this dx is its grad_output (saves its own channel-sum pass)
         dx._mnb_channel_sum = dx_sum
         return dx, dgamma, dbeta, None, None, None, None, None, None
@@ -169,10 +185,10 @@ class BatchNormBinarize2d(nn.BatchNorm2d):
             x = input.detach().contiguous()
             b, c = x.shape[0], x.shape[1]
             stats = torch.empty(2 * c, dtype=torch.float32, device=x.device)
-            L.check(lib.mnb_bn_batch_stats(x.data_ptr(), b, c, x.numel() // (b * c), float(self.eps), float(self.momentum),
-                                           self.running_mean.data_ptr(), self.running_var.data_ptr(),
-                                           self.num_batches_tracked.data_ptr(), stats.data_ptr(),
-                                           L.scratch(x.device, c).data_ptr(), L.stream()), "bn_batch_stats")
+            fn, xa = _xargs(lib, "mnb_bn_batch_stats", x, getattr(input, "_mnb_codes", None))
+            L.check(fn(*xa, b, c, x.numel() // (b * c), float(self.eps), float(self.momentum), self.running_mean.data_ptr(),
+                       self.running_var.data_ptr(), self.num_batches_tracked.data_ptr(), stats.data_ptr(),
+                       L.scratch(x.device, c).data_ptr(), L.stream()), "bn_batch_stats")
             mean, invstd = stats[:c], stats[c:]
         else:
             mean = self.running_mean
@@ -553,6 +569,24 @@ def _mark_plane_only(module: nn.Module):
             prod.plane_only = True
 
 
+def _mark_codes_out(module: nn.Module):
+    """wbwtab conv (binary / ternary weights, trained) whose only reader is the BatchNormBinarize2d of its own block - the
+    reference's conv-bn-act block runs its children in order - and whose sums fit in int16: the conv hands its output to
+    that producer as int16 codes (functional._pk_forward, codes_out), 2 bytes per element on every pass instead of 4."""
+    from .pk import codes_fit
+    from .wbwtab import QuantConv2d as WbConv
+    for m in module.modules():
+        if not hasattr(m, "channel_shuffle_flag"):
+            continue
+        kids = [k for k in m.children() if not isinstance(k, nn.Identity)]
+        if len(kids) != 2 or not isinstance(kids[0], WbConv) or not isinstance(kids[1], BatchNormBinarize2d):
+            continue
+        conv = kids[0]
+        if conv.weight_quantizer.W in (2, 3) and not conv.quant_inference and codes_fit(conv.in_channels, conv.groups,
+                                                                                        conv.kernel_size):
+            conv.codes_out = True
+
+
 def fuse_wbwtab_blocks(model: nn.Module, fold_shuffle: bool = True) -> nn.Module:
     _fuse_pairs(model)
     _fold_pools(model)
@@ -560,6 +594,7 @@ def fuse_wbwtab_blocks(model: nn.Module, fold_shuffle: bool = True) -> nn.Module
     if fold_shuffle:
         _fold_shuffles(model)
     _mark_plane_only(model)
+    _mark_codes_out(model)
     return model
 
 

@@ -86,6 +86,20 @@ def conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, n_scale=None, a_scale=Non
                            L.tc_err_flag(out.device).data_ptr(), L.stream())
 
 
+def conv_codes(sh, a_pk, w_img, codes, dec, n_scale=None, a_scale=None, a_scale_const=1.0, bias=None, level_bound=1):
+    """forward conv of one +-1 piece against one piece of integer weight levels (|level| <= level_bound) whose exact sums go
+    out as int16 ``codes`` plus the epilogue's decode pair ``dec`` [2, K] (mnb_pk_conv_codes); returns the C status"""
+    return L.load().mnb_pk_conv_codes(C.byref(sh), a_pk.data_ptr(), 1, w_img.data_ptr(), 1, L.ptr(n_scale), L.ptr(a_scale),
+                                      float(a_scale_const), L.ptr(bias), int(level_bound), codes.data_ptr(), dec.data_ptr(),
+                                      L.tc_err_flag(codes.device).data_ptr(), L.stream())
+
+
+def codes_fit(in_channels, groups, kernel_size, level_bound=1):
+    """the int16 bound of mnb_pk_conv_codes: every sum of (C/g) * R * S terms +-1 x level fits in an int16"""
+    r, s = (kernel_size, kernel_size) if isinstance(kernel_size, int) else kernel_size
+    return (in_channels // groups) * r * s * level_bound <= 32767
+
+
 def consumer_plane(b, c, h, w, device):
     """empty operand plane (one bf16 piece) of a conv that reads a [b, c, h, w] activation"""
     return torch.empty(int(L.load().mnb_pk_act_bytes(b, c, h, w, 1)), dtype=torch.uint8, device=device)

@@ -47,6 +47,8 @@ class WeightQuantizer(nn.Module):
 
 
 class QuantConv2d(nn.Conv2d):
+    codes_out = False   # set by fused.fuse_wbwtab_blocks: the only reader is this block's BatchNormBinarize2d (int16 hand-off)
+
     def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1,
                  bias=True, padding_mode="zeros", W=2, quant_inference=False):
         super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, groups, bias,
@@ -62,7 +64,7 @@ class QuantConv2d(nn.Conv2d):
         # the input is NOT quantized here (WB:181-195): it is whatever the previous block produced
         # (+-1 after an ActivationQuantizer(A=2), plain fp32 when A == 32)
         return F_.quant_conv2d(input, wq, self.bias, w_int, w_scale, None, self.stride, self.padding,
-                               self.dilation, self.groups)
+                               self.dilation, self.groups, codes_out=bool(self.codes_out) and w_int is not None)
 
 
 class QuantConvTranspose2d(nn.ConvTranspose2d):
