@@ -481,6 +481,37 @@ int64_t mnb_xnor_wimage_bytes(const mnb_conv_shape* s);
 int mnb_xnor_pack_weight(const mnb_conv_shape* s, const int16_t* w_int, void* w_img, mnb_stream_t stream);
 int mnb_xnor_conv_fwd(const mnb_conv_shape* s, const void* a_bits, const void* w_img, const float* alpha, const float* bias,
                       float* y, mnb_stream_t stream);
+/* Frozen wbwtab inference graphs (wbwtab.freeze_inference): the producer writes its consumer's operand, so no fp32 tensor
+ * crosses between two binarized layers.  The value v = fmaf(sum, alpha[k], bias[k]) of mnb_xnor_conv_fwd goes through
+ *   [eval BatchNorm: v = fmaf(v - mean[k], gamma[k] * invstd[k], beta[k]), the op sequence of mnb_bn_sign_fwd_packed]
+ *   -> sign bit !(v < 0) (WB:11-36: 0 and -0.0 -> +1) [-> MaxPool2d(2, 2): OR of the window's bits] [-> channel shuffle:
+ *   channel c to (c mod C/sg) * sg + c div (C/sg), the producers' out_shuffle_groups]
+ * and is stored in the consumer's format:
+ *   MNB_XNOR_BITS       the bit plane of mnb_xnor_pack_act for a consumer with out_groups groups (zeroed and OR-ed into on
+ *                       the stream: bitwise deterministic);
+ *   MNB_XNOR_PM1_BF16   the +-1 bf16 plane [b][c/8][h][w][8] of mnb_bn_sign_fwd_packed (no pool; C % 8 == 0, 16-byte aligned).
+ *   mnb_xnor_post_bytes    : bytes of conv_post's output (-1 outside the cover: conv shape, odd plane under a pool, ...).
+ *   mnb_xnor_conv_post     : the convolution with that epilogue.
+ *   mnb_xnor_pack_act_post : fp32 NCHW [B, C, H, W] (the un-quantized stem's output) -> the same epilogue -> bit plane.
+ * Refusals (nothing launched): MNB_E_ARG for a malformed description (format, shuffle / consumer groups that do not divide C,
+ * partial BatchNorm pointers), MNB_E_UNSUPPORTED outside the cover (conv shape, a pool over an odd plane, bf16 with a pool). */
+#define MNB_XNOR_BITS 0
+#define MNB_XNOR_PM1_BF16 1
+typedef struct mnb_xnor_post {
+  int32_t format;          /* MNB_XNOR_BITS or MNB_XNOR_PM1_BF16 */
+  int32_t out_groups;      /* bits: the consumer conv's group count (C_out % out_groups == 0) */
+  int32_t shuffle_groups;  /* 1 = none */
+  int32_t pool2;           /* 1: MaxPool2d(2, 2) folded in (even P and Q) */
+  const float* bn_mean;    /* NULL: no BatchNorm; otherwise all four, [C_out] */
+  const float* bn_invstd;
+  const float* bn_gamma;
+  const float* bn_beta;
+} mnb_xnor_post;
+int64_t mnb_xnor_post_bytes(const mnb_conv_shape* s, const mnb_xnor_post* post);
+int mnb_xnor_conv_post(const mnb_conv_shape* s, const void* a_bits, const void* w_img, const float* alpha, const float* bias,
+                       const mnb_xnor_post* post, void* out, mnb_stream_t stream);
+int mnb_xnor_pack_act_post(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_xnor_post* post,
+                           void* out_bits, mnb_stream_t stream);
 
 /* Optimizer step of the QAT loop (torch.optim.Adam semantics, L2 weight decay, no amsgrad;
  * wbwtab/main.py:84,331-339) over one flat fp32 parameter / gradient bucket: a single launch. */

@@ -32,6 +32,15 @@ class PkPost(C.Structure):
     _fields_ = [("q", C.POINTER(ActQParams)), ("relu", C.c_int32), ("phase_split", C.c_int32), ("out_pk", C.c_void_p)]
 
 
+XNOR_BITS, XNOR_PM1_BF16 = 0, 1
+
+
+class XnorPost(C.Structure):
+    """mnb_xnor_post: the epilogue of a frozen wbwtab layer (BatchNorm, pool, shuffle) and its consumer's operand format"""
+    _fields_ = [("format", C.c_int32), ("out_groups", C.c_int32), ("shuffle_groups", C.c_int32), ("pool2", C.c_int32),
+                ("bn_mean", C.c_void_p), ("bn_invstd", C.c_void_p), ("bn_gamma", C.c_void_p), ("bn_beta", C.c_void_p)]
+
+
 class ConvOperands(C.Structure):
     _fields_ = [("a_codes", C.c_void_p), ("a_f32", C.c_void_p), ("a_offset", C.c_int32),
                 ("a_offset_zp", C.c_void_p), ("a_scale", C.c_void_p), ("w_int", C.c_void_p),
@@ -126,6 +135,9 @@ PROTOTYPES = {
     "mnb_xnor_wimage_bytes": (_L, [_SHAPE]),
     "mnb_xnor_pack_weight": (C.c_int, [_SHAPE, _P, _P, _P]),
     "mnb_xnor_conv_fwd": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),
+    "mnb_xnor_post_bytes": (_L, [_SHAPE, C.POINTER(XnorPost)]),
+    "mnb_xnor_conv_post": (C.c_int, [_SHAPE, _P, _P, _P, _P, C.POINTER(XnorPost), _P, _P]),
+    "mnb_xnor_pack_act_post": (C.c_int, [_P, _I, _I, _I, _I, C.POINTER(XnorPost), _P, _P]),
     "mnb_set_tc_profile_buffer": (None, [_P]),
     "mnb_selftest_mma_rate": (C.c_int, [_I, _I, _I, _I, _I, _P, _P, _P]),
     "mnb_selftest_umma": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),

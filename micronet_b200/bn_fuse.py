@@ -7,6 +7,8 @@
   the weights stay +-1 / ternary and only the bias changes (channels with gamma < 0 flip the sign of weight and bias);
   the rest is the ordinary fold.  Fused convs 2 .. bin_bn_fuse_num become ``wbwtab.QuantConv2d(quant_inference=True)``,
   the others plain ``nn.Conv2d``; the BatchNorm is replaced by ``nn.Identity``.
+* ``wbwtab_quantize_inference_weights`` - the weight step that follows in the reference (
+  ``bn_fused_model_test.py:191-194``): every wbwtab ``QuantConv2d`` stores its quantized weight alpha_k * {-1, 0, +1}.
 * ``iao_model_bn_fuse`` - ``wqaq/iao/bn_fuse/bn_fuse.py:20-73``.  Every ``iao.QuantBNFuseConv2d`` becomes an
   ``iao.QuantConv2d(quant_inference=True, bias=True)`` holding the folded weight / bias (running statistics) and the
   calibrated scale / zero-point buffers of both quantizers.
@@ -113,4 +115,15 @@ def iao_model_bn_fuse(model, inplace=False):
     if not inplace:
         model = copy.deepcopy(model)
     _iao_walk(model)
+    return model
+
+
+@torch.no_grad()
+def wbwtab_quantize_inference_weights(model):
+    """the second step of the reference's deployment flow (``wbwtab/bn_fuse/bn_fused_model_test.py:191-194``): every wbwtab
+    ``QuantConv2d`` of a BN-fused model stores its quantized weight, ``m.weight.data = m.weight_quantizer(m.weight)``, so a
+    ``quant_inference`` layer holds alpha_k * {-1, 0, +1} (what ``wbwtab.freeze_inference`` runs on the XNOR kernels)"""
+    for m in model.modules():
+        if isinstance(m, _wb.QuantConv2d):
+            m.weight.data = m.weight_quantizer(m.weight)
     return model

@@ -105,7 +105,43 @@ struct Params {
   const float* bias;    // [K] or NULL
   float* y;
   int B, G, cin_g, cout_g, H, W, P, Q, R, S, stride, pad, kb, ksplit;
+  // sign-bit epilogue (conv_kernel<..., true>, mnb_xnor_conv_post): BatchNorm constants (mean NULL = none), the consumer's
+  // output format, unit geometry and the 2x2 pool
+  const float *bn_mean, *bn_invstd, *bn_gamma, *bn_beta;
+  void* out;
+  int fmt, sg, out_cin_g, out_nw, pool;
 };
+
+// destination of output channel c in the consumer's plane, packed as (unit << 5) | bit: unit = (group, word) of the bit plane
+// or the channel octet of the bf16 plane.  The producer's channel shuffle moves channel c to (c mod C/sg) * sg + c div (C/sg).
+__host__ __device__ inline int post_dest(int c, int K, int fmt, int sg, int out_cin_g, int out_nw) {
+  const int cpg = K / sg;
+  const int cd = sg > 1 ? (c % cpg) * sg + c / cpg : c;
+  if (fmt == MNB_XNOR_PM1_BF16) return ((cd >> 3) << 5) | (cd & 7);
+  const int g = cd / out_cin_g, r = cd - g * out_cin_g;
+  return ((g * out_nw + (r >> 5)) << 5) | (r & 31);
+}
+
+// flush one destination unit of one output pixel: OR the collected sign bits into the (zeroed) bit plane, or store the
+// +-1 channels of the octet as bf16 (one 16-byte store when this thread holds all eight)
+__device__ __forceinline__ void post_flush(const Params& p, int64_t base, int64_t unit_stride, int unit, uint32_t bits,
+                                           uint32_t have) {
+  if (unit < 0) return;
+  if (p.fmt == MNB_XNOR_BITS) {
+    if (bits) atomicOr(reinterpret_cast<uint32_t*>(p.out) + base + (int64_t)unit * unit_stride, bits);
+    return;
+  }
+  uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + (base + (int64_t)unit * unit_stride) * 8;
+  if (have == 0xFFu) {
+    uint32_t h[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) h[j] = (bits >> j) & 1u ? 0x3F80u : 0xBF80u;
+    *reinterpret_cast<uint4*>(o) = make_uint4(h[0] | (h[1] << 16), h[2] | (h[3] << 16), h[4] | (h[5] << 16), h[6] | (h[7] << 16));
+  } else {
+    for (int j = 0; j < 8; ++j)
+      if ((have >> j) & 1u) o[j] = (bits >> j) & 1u ? 0x3F80u : 0xBF80u;
+  }
+}
 
 // pixels per thread: two where the receptive field is a few words (1x1 layers: the per-channel shared-memory loads and loop
 // overhead are shared), one where it is nine or more (3x3 / 5x5: 2 x 9 activation words + border state cost occupancy)
@@ -120,7 +156,7 @@ struct Rec {
   static constexpr int WORDS = 2 * TWP + 4 + ((TAB + 3) & ~3);
 };
 
-template <int R_, int NW_, bool BORDER>
+template <int R_, int NW_, bool BORDER, bool POST>
 __global__ void __launch_bounds__(NTHREADS) conv_kernel(const Params p) {
   constexpr int PX = PxOf<R_, NW_>::value;
   typedef Rec<R_, NW_> RC;
@@ -130,6 +166,18 @@ __global__ void __launch_bounds__(NTHREADS) conv_kernel(const Params p) {
   const int g = blockIdx.y / p.ksplit, ks = blockIdx.y % p.ksplit;
   const int k0 = g * p.cout_g + ks * p.kb;                // first output channel of this block
   const int kcnt = min(p.kb, p.cout_g - ks * p.kb);
+  // POST: per channel {mean, gamma * invstd, beta, destination} after the records (the BN+sign producers' constants)
+  float4* pcst = reinterpret_cast<float4*>(smem + p.kb * RC::WORDS);
+  if (POST) {
+    const int K = p.G * p.cout_g;
+    for (int e = threadIdx.x; e < kcnt; e += NTHREADS) {
+      const int c = k0 + e;
+      float4 v = make_float4(0.f, 1.f, 0.f, 0.f);
+      if (p.bn_mean) v = make_float4(__ldg(p.bn_mean + c), __ldg(p.bn_gamma + c) * __ldg(p.bn_invstd + c), __ldg(p.bn_beta + c), 0.f);
+      v.w = __int_as_float(post_dest(c, K, p.fmt, p.sg, p.out_cin_g, p.out_nw));
+      pcst[e] = v;
+    }
+  }
   for (int e = threadIdx.x; e < kcnt * RC::WORDS; e += NTHREADS) {
     const int k = e / RC::WORDS, o = e - k * RC::WORDS;
     uint32_t v = 0;
@@ -151,6 +199,11 @@ __global__ void __launch_bounds__(NTHREADS) conv_kernel(const Params p) {
   float* yp[PX];
   int r0[PX], r1[PX], s0[PX], s1[PX];
   bool border[PX];
+  int64_t obase[PX];
+  int cu[PX];                 // POST: destination unit being collected (-1: none), its bits and the channels seen
+  uint32_t cb[PX], chv[PX];
+  const int64_t out_hw = POST && p.pool ? (int64_t)(p.P >> 1) * (p.Q >> 1) : (int64_t)PQ;
+  const int units = !POST ? 0 : p.fmt == MNB_XNOR_BITS ? p.out_nw * ((p.G * p.cout_g) / p.out_cin_g) : (p.G * p.cout_g) >> 3;
 #pragma unroll
   for (int x = 0; x < PX; ++x) {
     const int64_t pix = ((int64_t)blockIdx.x * PX + x) * NTHREADS + threadIdx.x;
@@ -174,7 +227,14 @@ __global__ void __launch_bounds__(NTHREADS) conv_kernel(const Params p) {
     r0[x] = max(0, -ih0); r1[x] = max(r0[x], min(R_, p.H - ih0));
     s0[x] = max(0, -iw0); s1[x] = max(s0[x], min(R_, p.W - iw0));
     border[x] = BORDER && ((r0[x] != 0) || (r1[x] != R_) || (s0[x] != 0) || (s1[x] != R_));
-    yp[x] = p.y + ((int64_t)b * p.G * p.cout_g + k0) * PQ + pq;
+    if (POST) {
+      // destination pixel (pooled: the 2x2 window's output) and the offset of unit 0 of this image
+      const int opq = p.pool ? (op >> 1) * (p.Q >> 1) + (oq >> 1) : pq;
+      obase[x] = (int64_t)b * units * out_hw + opq;
+      cu[x] = -1; cb[x] = 0u; chv[x] = 0u;
+    } else {
+      yp[x] = p.y + ((int64_t)b * p.G * p.cout_g + k0) * PQ + pq;
+    }
   }
 
 #pragma unroll 2
@@ -197,18 +257,79 @@ __global__ void __launch_bounds__(NTHREADS) conv_kernel(const Params p) {
                          P[r0[x] * (R_ + 1) + s0[x]];
         acc += P[R_ * (R_ + 1) + R_] - rect;
       }
-      if (live[x]) yp[x][(int64_t)k * PQ] = fmaf((float)acc, al, bs);
+      if (!POST) {
+        if (live[x]) yp[x][(int64_t)k * PQ] = fmaf((float)acc, al, bs);
+      } else {
+        // the BN+sign producers' op sequence (mnb_conv_packed.cu): bn = fmaf(v - mean, gamma * invstd, beta), bit = !(bn < 0)
+        const float4 pc = pcst[k];
+        float v = fmaf((float)acc, al, bs);
+        if (p.bn_mean) v = fmaf(v - pc.x, pc.y, pc.z);
+        const int dest = __float_as_int(pc.w), unit = dest >> 5, j = dest & 31;
+        if (unit != cu[x]) {
+          if (live[x]) post_flush(p, obase[x], out_hw, cu[x], cb[x], chv[x]);
+          cu[x] = unit; cb[x] = 0u; chv[x] = 0u;
+        }
+        cb[x] |= (v < 0.f ? 0u : 1u) << j;
+        chv[x] |= 1u << j;
+      }
     }
+  }
+  if (POST) {
+#pragma unroll
+    for (int x = 0; x < PX; ++x)
+      if (live[x]) post_flush(p, obase[x], out_hw, cu[x], cb[x], chv[x]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// stem producer: fp32 NCHW [-> eval BatchNorm] -> sign [-> 2x2 max-pool] [-> channel shuffle] -> the consumer's bit plane.
+// One thread per output word, gathering its (up to) 32 channels through the inverse shuffle; the pooled bit is the OR of the
+// window's four sign bits (the max of +-1 values).
+// ------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(NTHREADS) pack_act_post_kernel(const float* __restrict__ x, int B, int Cc, int H, int W,
+                                                                 int G, int sg, int pool, const float* __restrict__ mean,
+                                                                 const float* __restrict__ invstd,
+                                                                 const float* __restrict__ gamma,
+                                                                 const float* __restrict__ beta, uint32_t* __restrict__ out) {
+  const int cin_g = Cc / G, nw = words_per_group(cin_g), cpg = Cc / sg;
+  const int OH = pool ? H / 2 : H, OW = pool ? W / 2 : W, OHW = OH * OW, HW = H * W;
+  const int64_t total = (int64_t)B * G * nw * OHW;
+  for (int64_t i = (int64_t)blockIdx.x * NTHREADS + threadIdx.x; i < total; i += (int64_t)gridDim.x * NTHREADS) {
+    const int opix = (int)(i % OHW);
+    int64_t t = i / OHW;
+    const int n = (int)(t % nw); t /= nw;
+    const int g = (int)(t % G);
+    const int b = (int)(t / G);
+    const int oh = opix / OW, ow = opix % OW;
+    const int pix = pool ? (2 * oh) * W + 2 * ow : opix;
+    const int c0 = n * 32, cnt = min(32, cin_g - c0);
+    uint32_t word = 0;
+    for (int j = 0; j < cnt; ++j) {
+      const int cd = g * cin_g + c0 + j;
+      const int c = sg > 1 ? (cd % sg) * cpg + cd / sg : cd;   // inverse of the producer's shuffle
+      const float* src = x + ((int64_t)b * Cc + c) * HW + pix;
+      float mu = 0.f, k = 1.f, be = 0.f;
+      if (mean) { mu = __ldg(mean + c); k = __ldg(gamma + c) * __ldg(invstd + c); be = __ldg(beta + c); }
+      uint32_t bit = 0;
+      for (int q = 0; q < (pool ? 4 : 1); ++q) {
+        float v = __ldg(src + (q >> 1) * W + (q & 1));
+        if (mean) v = fmaf(v - mu, k, be);
+        bit |= v < 0.f ? 0u : 1u;
+      }
+      word |= bit << j;
+    }
+    out[i] = word;
   }
 }
 
 typedef void (*KernelFn)(const Params);
-static KernelFn pick(int R, int nw, bool border, int* rec_words, int* px = nullptr) {
-#define XN_CASE(r, n)                                                                     \
-  if (R == r && nw == n) {                                                                \
-    if (rec_words) *rec_words = Rec<r, n>::WORDS;                                         \
-    if (px) *px = PxOf<r, n>::value;                                                      \
-    return border ? conv_kernel<r, n, true> : conv_kernel<r, n, false>;                   \
+static KernelFn pick(int R, int nw, bool border, int* rec_words, int* px = nullptr, bool post = false) {
+#define XN_CASE(r, n)                                                                                 \
+  if (R == r && nw == n) {                                                                            \
+    if (rec_words) *rec_words = Rec<r, n>::WORDS;                                                     \
+    if (px) *px = PxOf<r, n>::value;                                                                  \
+    if (post) return border ? conv_kernel<r, n, true, true> : conv_kernel<r, n, false, true>;         \
+    return border ? conv_kernel<r, n, true, false> : conv_kernel<r, n, false, false>;                 \
   }
   XN_CASE(1, 1) XN_CASE(1, 2) XN_CASE(1, 3) XN_CASE(1, 4) XN_CASE(1, 8)
   XN_CASE(3, 1) XN_CASE(3, 2) XN_CASE(3, 4)
@@ -227,6 +348,75 @@ static int check_shape(const mnb_conv_shape* s) {
   if (pick(s->ker_h, words_per_group(s->in_c / s->groups), true, nullptr) == nullptr) return MNB_E_UNSUPPORTED;
   const int P = (s->in_h + 2 * s->pad_h - s->ker_h) / s->stride_h + 1, Q = (s->in_w + 2 * s->pad_w - s->ker_w) / s->stride_w + 1;
   if (P <= 0 || Q <= 0) return MNB_E_UNSUPPORTED;
+  return 0;
+}
+
+// post: NULL for the fp32 output of mnb_xnor_conv_fwd.  The shape has passed check_shape (and check_post when post is set).
+static int launch(const mnb_conv_shape* s, const void* a_bits, const void* w_img, const float* alpha, const float* bias,
+                  const mnb_xnor_post* post, void* out, mnb_stream_t stream) {
+  Params p;
+  p.B = s->batch; p.G = s->groups; p.cin_g = s->in_c / s->groups; p.cout_g = s->out_c / s->groups;
+  p.H = s->in_h; p.W = s->in_w; p.R = s->ker_h; p.S = s->ker_w; p.stride = s->stride_h; p.pad = s->pad_h;
+  p.P = (p.H + 2 * p.pad - p.R) / p.stride + 1;
+  p.Q = (p.W + 2 * p.pad - p.S) / p.stride + 1;
+  const int nw = words_per_group(p.cin_g), TW = p.R * p.S * nw;
+  // border handling only where a tap can leave the image (never for an un-padded filter that fits)
+  const bool border = p.pad > 0 || (p.P - 1) * p.stride + p.R > p.H || (p.Q - 1) * p.stride + p.S > p.W;
+  int rec_words = 0, px = 1;
+  KernelFn fn = pick(p.R, nw, border, &rec_words, &px, post != nullptr);
+  const int per_k = rec_words * 4 + (post ? 16 : 0);     // shared-memory bytes per output channel
+  const int64_t npix = (int64_t)p.B * p.P * p.Q;
+  const int pblocks = (int)((npix + NTHREADS * px - 1) / (NTHREADS * px));
+  // k-slices: enough blocks for ~4 per SM, at most 40 KB of channel records per block
+  int ksplit = 1;
+  while (p.cout_g / ksplit > 8 && ((int64_t)pblocks * p.G * ksplit < 4 * MNB_NUM_SMS ||
+                                   (int64_t)((p.cout_g + ksplit - 1) / ksplit) * per_k > 40 * 1024))
+    ++ksplit;
+  p.kb = (p.cout_g + ksplit - 1) / ksplit;
+  p.ksplit = (p.cout_g + p.kb - 1) / p.kb;
+  const size_t smem = (size_t)p.kb * per_k;
+  if (smem > 48 * 1024) return MNB_E_UNSUPPORTED;
+  const uint32_t* words = (const uint32_t*)w_img;
+  p.abits = (const uint32_t*)a_bits;
+  p.wwords = words;
+  p.wtabs = (const int32_t*)(words + (int64_t)s->out_c * 2 * TW);
+  p.alpha = alpha; p.bias = bias;
+  p.y = post ? nullptr : (float*)out;
+  p.bn_mean = p.bn_invstd = p.bn_gamma = p.bn_beta = nullptr;
+  p.out = nullptr;
+  p.fmt = p.sg = p.out_cin_g = p.out_nw = p.pool = 0;
+  if (post) {
+    p.bn_mean = post->bn_mean; p.bn_invstd = post->bn_invstd; p.bn_gamma = post->bn_gamma; p.bn_beta = post->bn_beta;
+    p.out = out;
+    p.fmt = post->format; p.sg = post->shuffle_groups; p.pool = post->pool2;
+    p.out_cin_g = s->out_c / post->out_groups; p.out_nw = words_per_group(p.out_cin_g);
+  }
+  dim3 grid((unsigned)pblocks, (unsigned)(p.G * p.ksplit));
+  if (grid.y > 65535) return MNB_E_UNSUPPORTED;
+  fn<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+// the consumer description of mnb_xnor_conv_post / mnb_xnor_pack_act_post for C producer channels on a P x Q plane
+// (P = Q = 0: plane size not known yet, only the channel rules are checked)
+static int check_post(const mnb_xnor_post* post, int C, int P, int Q) {
+  MNB_REQUIRE(post != nullptr, "xnor post: null consumer description");
+  MNB_REQUIRE(post->format == MNB_XNOR_BITS || post->format == MNB_XNOR_PM1_BF16, "xnor post: unknown format %d", post->format);
+  MNB_REQUIRE(post->shuffle_groups >= 1 && C % post->shuffle_groups == 0, "xnor post: shuffle groups %d do not divide %d channels",
+              post->shuffle_groups, C);
+  MNB_REQUIRE(post->pool2 == 0 || post->pool2 == 1, "xnor post: pool2 must be 0 or 1");
+  const bool any_bn = post->bn_mean || post->bn_invstd || post->bn_gamma || post->bn_beta;
+  MNB_REQUIRE(!any_bn || (post->bn_mean && post->bn_invstd && post->bn_gamma && post->bn_beta),
+              "xnor post: BatchNorm needs all four of mean, invstd, gamma, beta");
+  if (post->format == MNB_XNOR_BITS) {
+    MNB_REQUIRE(post->out_groups >= 1 && C % post->out_groups == 0, "xnor post: consumer groups %d do not divide %d channels",
+                post->out_groups, C);
+  } else {
+    if (post->pool2) return mnb_fail(MNB_E_UNSUPPORTED, "xnor post: the bf16 plane takes no folded pool");
+    if (C % 8) return mnb_fail(MNB_E_UNSUPPORTED, "xnor post: the bf16 plane needs C %% 8 == 0");
+  }
+  if (post->pool2 && ((P | Q) & 1)) return mnb_fail(MNB_E_UNSUPPORTED, "xnor post: a 2x2 pool over an odd plane (%d x %d)", P, Q);
   return 0;
 }
 
@@ -280,35 +470,50 @@ int mnb_xnor_conv_fwd(const mnb_conv_shape* s, const void* a_bits, const void* w
   const int rc = xnor::check_shape(s);
   if (rc != 0) return rc;
   MNB_REQUIRE(a_bits && w_img && y, "xnor_conv_fwd: null pointer");
-  xnor::Params p;
-  p.B = s->batch; p.G = s->groups; p.cin_g = s->in_c / s->groups; p.cout_g = s->out_c / s->groups;
-  p.H = s->in_h; p.W = s->in_w; p.R = s->ker_h; p.S = s->ker_w; p.stride = s->stride_h; p.pad = s->pad_h;
-  p.P = (p.H + 2 * p.pad - p.R) / p.stride + 1;
-  p.Q = (p.W + 2 * p.pad - p.S) / p.stride + 1;
-  const int nw = xnor::words_per_group(p.cin_g), TW = p.R * p.S * nw;
-  // border handling only where a tap can leave the image (never for an un-padded filter that fits)
-  const bool border = p.pad > 0 || (p.P - 1) * p.stride + p.R > p.H || (p.Q - 1) * p.stride + p.S > p.W;
-  int rec_words = 0, px = 1;
-  xnor::KernelFn fn = xnor::pick(p.R, nw, border, &rec_words, &px);
-  const int64_t npix = (int64_t)p.B * p.P * p.Q;
-  const int pblocks = (int)((npix + xnor::NTHREADS * px - 1) / (xnor::NTHREADS * px));
-  // k-slices: enough blocks for ~4 per SM, at most 40 KB of channel records per block
-  int ksplit = 1;
-  while (p.cout_g / ksplit > 8 && ((int64_t)pblocks * p.G * ksplit < 4 * MNB_NUM_SMS ||
-                                   (int64_t)((p.cout_g + ksplit - 1) / ksplit) * rec_words * 4 > 40 * 1024))
-    ++ksplit;
-  p.kb = (p.cout_g + ksplit - 1) / ksplit;
-  p.ksplit = (p.cout_g + p.kb - 1) / p.kb;
-  const size_t smem = (size_t)p.kb * rec_words * 4;
-  if (smem > 48 * 1024) return MNB_E_UNSUPPORTED;
-  const uint32_t* words = (const uint32_t*)w_img;
-  p.abits = (const uint32_t*)a_bits;
-  p.wwords = words;
-  p.wtabs = (const int32_t*)(words + (int64_t)s->out_c * 2 * TW);
-  p.alpha = alpha; p.bias = bias; p.y = y;
-  dim3 grid((unsigned)pblocks, (unsigned)(p.G * p.ksplit));
-  if (grid.y > 65535) return MNB_E_UNSUPPORTED;
-  fn<<<grid, xnor::NTHREADS, smem, (cudaStream_t)stream>>>(p);
+  return xnor::launch(s, a_bits, w_img, alpha, bias, nullptr, y, stream);
+}
+
+int64_t mnb_xnor_post_bytes(const mnb_conv_shape* s, const mnb_xnor_post* post) {
+  if (xnor::check_shape(s) != 0 || xnor::check_post(post, s->out_c, 0, 0) != 0) return -1;
+  const int P = (s->in_h + 2 * s->pad_h - s->ker_h) / s->stride_h + 1, Q = (s->in_w + 2 * s->pad_w - s->ker_w) / s->stride_w + 1;
+  if (post->pool2 && ((P | Q) & 1)) return -1;
+  const int OH = post->pool2 ? P / 2 : P, OW = post->pool2 ? Q / 2 : Q;
+  if (post->format == MNB_XNOR_PM1_BF16) return (int64_t)s->batch * s->out_c * OH * OW * 2;
+  return mnb_xnor_act_bytes(s->batch, s->out_c, OH, OW, post->out_groups);
+}
+
+int mnb_xnor_conv_post(const mnb_conv_shape* s, const void* a_bits, const void* w_img, const float* alpha, const float* bias,
+                       const mnb_xnor_post* post, void* out, mnb_stream_t stream) {
+  int rc = xnor::check_shape(s);
+  if (rc != 0) return rc;
+  MNB_REQUIRE(a_bits && w_img && out, "xnor_conv_post: null pointer");
+  const int P = (s->in_h + 2 * s->pad_h - s->ker_h) / s->stride_h + 1, Q = (s->in_w + 2 * s->pad_w - s->ker_w) / s->stride_w + 1;
+  rc = xnor::check_post(post, s->out_c, P, Q);
+  if (rc != 0) return rc;
+  if (post->format == MNB_XNOR_PM1_BF16 && (reinterpret_cast<uintptr_t>(out) & 15))
+    return mnb_fail(MNB_E_UNSUPPORTED, "xnor_conv_post: the bf16 plane must be 16-byte aligned");
+  if (post->format == MNB_XNOR_BITS) {
+    // bits are OR-ed in (several blocks, and the four pixels of a pooled window, write one word): zero the plane first
+    const int64_t nbytes = mnb_xnor_post_bytes(s, post);
+    cudaError_t e = cudaMemsetAsync(out, 0, (size_t)nbytes, (cudaStream_t)stream);
+    if (e != cudaSuccess) return mnb_fail((int)e, "xnor_conv_post: memset failed: %s", cudaGetErrorString(e));
+  }
+  return xnor::launch(s, a_bits, w_img, alpha, bias, post, out, stream);
+}
+
+int mnb_xnor_pack_act_post(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_xnor_post* post,
+                           void* out_bits, mnb_stream_t stream) {
+  MNB_REQUIRE(x && out_bits, "xnor_pack_act_post: null pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "xnor_pack_act_post: bad shape");
+  const int rc = xnor::check_post(post, channels, h, w);
+  if (rc != 0) return rc;
+  if (post->format != MNB_XNOR_BITS) return mnb_fail(MNB_E_UNSUPPORTED, "xnor_pack_act_post: writes bit planes only");
+  const int OH = post->pool2 ? h / 2 : h, OW = post->pool2 ? w / 2 : w;
+  const int64_t total = mnb_xnor_act_bytes(batch, channels, OH, OW, post->out_groups) / 4;
+  const int blocks = (int)std::min<int64_t>((total + xnor::NTHREADS - 1) / xnor::NTHREADS, (int64_t)MNB_NUM_SMS * 16);
+  xnor::pack_act_post_kernel<<<blocks, xnor::NTHREADS, 0, (cudaStream_t)stream>>>(
+      x, batch, channels, h, w, post->out_groups, post->shuffle_groups, post->pool2, post->bn_mean, post->bn_invstd,
+      post->bn_gamma, post->bn_beta, (uint32_t*)out_bits);
   MNB_LAUNCHED(1);
   return 0;
 }

@@ -284,7 +284,12 @@ def materialized(t):
     """the values of a producer output: ``t`` itself, or - for a plane-only output of a fused BatchNorm + binarizer (its fp32
     storage was never written) - the +-1 tensor rebuilt from the bf16 operand plane [b][c/8][h][w][8], or - for a wbwtab conv
     that handed its output to its BatchNorm as int16 codes (``codes_out``) - that output decoded with the conv epilogue's own
-    fmaf.  Plumbing for tests, hooks and readers outside the fused producers; the training step never calls it."""
+    fmaf, or - for the output of a frozen wbwtab layer (wbwtab.freeze_inference) - the +-1 tensor its consumer's bit plane
+    encodes.  Plumbing for tests, hooks and readers outside the fused producers; the training step never calls it."""
+    xbits = getattr(t, "_mnb_xbits", None)
+    if xbits is not None:
+        from . import xnor as XN
+        return XN.unpack(xbits[1], t.shape, xbits[3])
     codes = getattr(t, "_mnb_codes", None)
     if codes is not None:
         b, c = t.shape[0], t.shape[1]

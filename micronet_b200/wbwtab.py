@@ -26,6 +26,9 @@ class ActivationQuantizer(nn.Module):
         return y
 
     def forward(self, input):
+        frozen = self.__dict__.get("_mnb_xnor")     # set by freeze_inference: this binarizer writes its consumer's bit plane
+        if frozen is not None:
+            return frozen(self, input)
         return self.binary(input) if self.A == 2 else self.relu(input)
 
 
@@ -57,6 +60,9 @@ class QuantConv2d(nn.Conv2d):
         self.weight_quantizer = WeightQuantizer(W=W)
 
     def forward(self, input):
+        frozen = self.__dict__.get("_mnb_xnor")     # set by freeze_inference: XNOR conv writing its consumer's operand
+        if frozen is not None:
+            return frozen(self, input)
         if not self.quant_inference:
             wq, w_int, w_scale = self.weight_quantizer.quantize(self.weight)
         else:
@@ -135,4 +141,321 @@ def prepare(model, inplace=False, A=2, W=2, quant_inference=False, fuse_bn=False
     if fuse_bn and A == 2:
         from .fused import fuse_wbwtab_blocks
         fuse_wbwtab_blocks(model)
+    return model
+
+
+# --------------------------------------------------------------------------
+# frozen inference graphs on bit planes
+# --------------------------------------------------------------------------
+def frozen_levels(conv):
+    """(w_int i16 [K, C/g, R, S], alpha f32 [K]) of a wbwtab conv for the XNOR kernels, or None when its weights cannot be
+    frozen.  A ``quant_inference`` layer holds alpha_k * {-1, 0, +1} (bn_fuse.wbwtab_quantize_inference_weights): the levels
+    are recovered exactly, anything else (raw fp32 weights, NaN) is refused.  A QAT layer takes them from its weight
+    quantizer (W = 2 centres the parameter in place, as every forward of the un-frozen layer does); a NaN alpha (an all-zero
+    ternary channel, 0 / 0) is refused: a sign bit cannot carry NaN."""
+    import torch
+    if conv.quant_inference:
+        w = conv.weight.detach()
+        alpha = w.abs().amax(dim=(1, 2, 3))
+        a4 = alpha.view(-1, 1, 1, 1)
+        lv = torch.where(a4 > 0, w / torch.where(a4 > 0, a4, torch.ones_like(a4)), torch.zeros_like(w)).round()
+        if not torch.equal(lv * a4, w):
+            return None
+        w_int = lv.to(torch.int16)
+    else:
+        if conv.weight_quantizer.W not in (2, 3):
+            return None
+        _, w_int, alpha = conv.weight_quantizer.quantize(conv.weight)
+        w_int, alpha = w_int.detach(), alpha.detach()
+    if not bool(torch.isfinite(alpha).all()):
+        return None
+    return w_int, alpha
+
+
+def _freezable(conv):
+    """structural test of frozen_levels that needs no kernel: geometry inside the XNOR cover and, for a QAT ternary layer,
+    no all-zero channel (its alpha is 0 / 0)"""
+    import torch
+    from . import xnor as XN
+    if not isinstance(conv, QuantConv2d) or conv.padding_mode != "zeros" or isinstance(conv.padding, str):
+        return False
+    k = conv.kernel_size[0]
+    sh = L.ConvShape(1, conv.in_channels, max(8, k), max(8, k), conv.out_channels, k, conv.kernel_size[1], conv.stride[0],
+                     conv.stride[1], conv.padding[0], conv.padding[1], conv.dilation[0], conv.dilation[1], conv.groups)
+    if not XN.supported(sh):
+        return False
+    if conv.quant_inference:
+        return frozen_levels(conv) is not None
+    if conv.weight_quantizer.W == 3:
+        return bool((conv.weight.detach().abs().amax(dim=(1, 2, 3)) > 0).all())
+    return conv.weight_quantizer.W == 2
+
+
+class _Link:
+    """what a frozen producer writes for its consumer: format (bit plane for a frozen XNOR conv, bf16 +-1 plane for the
+    un-quantized head), the consumer's groups, and the modules the epilogue stands for (the eval BatchNorm of a
+    BatchNormBinarize2d or an ActivationQuantizer, a 2x2 max-pool, the consumer block's channel shuffle)"""
+
+    def __init__(self, consumer, fmt, out_groups, act, pool, shuffle_groups):
+        self.consumer, self.fmt, self.out_groups = consumer, fmt, out_groups
+        self.act, self.pool, self.sg = act, pool, shuffle_groups
+
+    @property
+    def pool2(self):
+        from .fused import BatchNormBinarize2d
+        return bool(self.act.pool2) if isinstance(self.act, BatchNormBinarize2d) else self.pool is not None
+
+    def post(self):
+        """(mnb_xnor_post, the tensors it points to)"""
+        import torch
+        from . import xnor as XN
+        from .fused import BatchNormBinarize2d
+        bn = None
+        if isinstance(self.act, BatchNormBinarize2d):
+            a = self.act      # eval BatchNorm: running statistics, invstd exactly as BatchNormBinarize2d computes it
+            bn = (a.running_mean, torch.rsqrt(a.running_var + a.eps), a.weight.detach(), a.bias.detach())
+        return XN.post_struct(self.fmt, self.out_groups, self.sg, self.pool2, bn), bn
+
+    def out_shape(self, b, c, h, w):
+        return (b, c, h // 2, w // 2) if self.pool2 else (b, c, h, w)
+
+    def tail(self, y):
+        """the absorbed modules, run as they would run un-frozen (planes the kernels refuse at run time)"""
+        from .fused import BatchNormBinarize2d
+        if isinstance(self.act, BatchNormBinarize2d):
+            y = self.act._forward(y)             # BatchNorm + sign [+ pool] [+ shuffle]
+        else:
+            y = self.act.binary(y)
+            if self.pool is not None:
+                y = self.pool(y)
+            if self.sg > 1:
+                b, c = y.shape[0], y.shape[1]
+                y = y.view(b, self.sg, c // self.sg, *y.shape[2:]).transpose(1, 2).contiguous().view(y.shape)
+                y._mnb_pm1 = True
+        return y
+
+    def tag(self, plane, shape, device):
+        import torch
+        if self.fmt == L.XNOR_BITS:
+            y = torch.empty(shape, dtype=torch.float32, device="meta")     # shape only: the data lives in the bit plane
+            y._mnb_xbits = (self.consumer, plane, y._version, self.out_groups)
+            return y
+        y = torch.empty(shape, dtype=torch.float32, device=device)          # the placeholder of a plane-only producer
+        y._mnb_pk_pm1, y._mnb_plane_only, y._mnb_pm1 = plane, True, True
+        return y
+
+
+def _out_buffer(nbytes, fmt, device):
+    import torch
+    if fmt == L.XNOR_BITS:
+        return torch.empty(nbytes // 4, dtype=torch.int32, device=device)
+    return torch.empty(nbytes, dtype=torch.uint8, device=device)
+
+
+def _handed_bits(module, x):
+    """the bit plane a frozen producer wrote for ``module``, if ``x`` is that producer's unmodified output"""
+    pre = getattr(x, "_mnb_xbits", None)
+    if pre is not None and pre[0] is module and x._version == pre[2] and pre[3] == module.groups:
+        return pre[1]
+    return None
+
+
+def _check_eval(m):
+    if m.training:
+        raise RuntimeError("micronet_b200: this module is frozen for inference (wbwtab.freeze_inference); call "
+                           "freeze_inference(model, enable=False) before training it")
+
+
+def _frozen_conv_operands(conv):
+    """(w_int, alpha, bias, XNOR weight image) computed once; re-done when a parameter or buffer is written in place"""
+    key = tuple(t._version for t in list(conv.parameters()) + list(conv.buffers()))
+    fr = conv.__dict__.get("_mnb_xnor_ops")
+    if fr is None or fr[0] != key:
+        lv = frozen_levels(conv)
+        if lv is None:
+            raise RuntimeError("micronet_b200: the weights of a frozen wbwtab layer changed to values the XNOR kernel cannot "
+                               "hold (NaN alpha or not alpha * {-1, 0, 1}); call wbwtab.freeze_inference(model) again")
+        key = tuple(t._version for t in list(conv.parameters()) + list(conv.buffers()))   # W = 2 centres in place
+        fr = (key, lv[0], lv[1], None if conv.bias is None else conv.bias.detach(), {})
+        conv.__dict__["_mnb_xnor_ops"] = fr
+    return fr[1:]
+
+
+def _frozen_conv_forward(link, conv, x):
+    """XNOR conv whose epilogue applies the absorbed BatchNorm / binarizer / pool / shuffle and writes the consumer's operand"""
+    from . import xnor as XN
+    _check_eval(conv)
+    w_int, alpha, bias, images = _frozen_conv_operands(conv)
+    sh = F_._shape_struct(x.shape, conv.weight.shape, conv.stride, conv.padding, conv.dilation, conv.groups)
+    post, keep = link.post()
+    nbytes = XN.post_bytes(sh, post)
+    if nbytes >= 0:
+        plane = _handed_bits(conv, x)
+        if plane is None:
+            plane = XN.pack_act(F_.materialized(x).contiguous(), conv.groups)
+        if "w_img" not in images:
+            images["w_img"] = XN.pack_weight(sh, w_int)
+        out = _out_buffer(nbytes, link.fmt, alpha.device)
+        rc = F_._timed("fwd_xnor_post", sh, lambda: XN.conv_post(sh, plane, images["w_img"], post, out, alpha=alpha, bias=bias))
+        del keep
+        if rc == 0:
+            p, q = F_._out_hw(sh)
+            return link.tag(out, link.out_shape(x.shape[0], conv.out_channels, p, q), alpha.device)
+        if rc != L.E_UNSUPPORTED:
+            L.check(rc, "xnor_conv_post")
+    # outside the kernel's cover: the un-frozen layer, then the modules its epilogue stands for
+    wq = w_int.float() * alpha.view(-1, 1, 1, 1)
+    y = F_.quant_conv2d(F_.materialized(x), wq, bias, w_int, alpha, None, conv.stride, conv.padding, conv.dilation, conv.groups)
+    return link.tail(y)
+
+
+def _frozen_stem_forward(link, act, x):
+    """the binarizer behind the un-quantized stem conv: [eval BatchNorm] + sign [+ pool] [+ shuffle] straight into the
+    first XNOR layer's bit plane"""
+    import torch
+    from . import xnor as XN
+    _check_eval(act)
+    x = F_.materialized(x)
+    if x.dim() == 4 and x.is_cuda and x.dtype == torch.float32:
+        b, c, h, w = x.shape
+        post, keep = link.post()
+        oh, ow = (h // 2, w // 2) if link.pool2 else (h, w)
+        nbytes = int(L.load().mnb_xnor_act_bytes(b, c, oh, ow, link.out_groups))
+        if nbytes >= 0 and not (link.pool2 and (h | w) & 1):
+            out = _out_buffer(nbytes, L.XNOR_BITS, x.device)
+            x = x.contiguous()
+            rc = XN.pack_act_post(x, post, out)
+            del keep
+            if rc == 0:
+                return link.tag(out, (b, c, oh, ow), x.device)
+            if rc != L.E_UNSUPPORTED:
+                L.check(rc, "xnor_pack_act_post")
+    return link.tail(x)
+
+
+def _absorbed(m, x):
+    _check_eval(m)
+    return x
+
+
+def _blocks(seq):
+    """[(index in kids, name, block, conv, binarizer)] of the conv-bn-act blocks of an nn.Sequential that end in a binarizer
+    (BatchNormBinarize2d, or a BatchNorm-fused conv followed by ActivationQuantizer(A=2))"""
+    from .fused import BatchNormBinarize2d
+    out = []
+    kids = [(n, k) for n, k in seq.named_children() if not isinstance(k, nn.Identity)]
+    for i, (name, blk) in enumerate(kids):
+        if not hasattr(blk, "channel_shuffle_flag"):
+            continue
+        parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
+        if len(parts) != 2 or not isinstance(parts[0], nn.Conv2d):
+            continue
+        act = parts[1]
+        if isinstance(act, BatchNormBinarize2d) or (type(act) is ActivationQuantizer and act.A == 2):
+            out.append((i, name, blk, parts[0], act))
+    return kids, out
+
+
+def _head_conv(conv):
+    from .fused import EnginePmConv2d
+    return (type(conv) in (nn.Conv2d, EnginePmConv2d) and conv.in_channels % 8 == 0 and conv.padding_mode == "zeros"
+            and not isinstance(conv.padding, str))
+
+
+def _undo(model):
+    for kind, obj, key, val in reversed(model.__dict__.pop("_mnb_xnor_undo", [])):
+        if kind == "child":
+            obj._modules[key] = val
+        elif kind == "attr":
+            setattr(obj, key, val)
+        else:
+            obj.__dict__.pop(key, None)
+
+
+def freeze_inference(model, enable=True):
+    """Inference on bit planes for a wbwtab model in eval mode (NIN-GC-style ``nn.Sequential`` of conv-bn-act blocks):
+    every binary / ternary conv whose output is binarized for a consumer runs the XNOR-popcount kernel with its weights
+    quantized and packed ONCE (re-done when a parameter is written in place), and its epilogue writes the consumer's operand
+    directly - the sign bits of the next XNOR layer (mnb_xnor_conv_post), or the +-1 bf16 plane of the un-quantized head -
+    so no fp32 activation crosses between two binarized layers.  The binarizer behind the stem conv writes the first
+    layer's bit plane (mnb_xnor_pack_act_post).  Covered graphs:
+    * the QAT graph with fused producers (``prepare(..., fuse_bn=True)``, then ``.eval()``): each layer's
+      BatchNormBinarize2d (running statistics, folded pool, channel shuffle) moves into the conv's epilogue;
+    * the reference's deployment graph (``prepare(quant_inference=True)`` -> ``bn_fuse.wbwtab_model_bn_fuse`` ->
+      ``bn_fuse.wbwtab_quantize_inference_weights``): the ActivationQuantizer, the following MaxPool2d(2, 2) and the next
+      block's channel shuffle move into the epilogue, and the BatchNorm-fused head conv reads the +-1 plane on the
+      packed-operand tensor cores (fused.EnginePmConv2d).
+    A layer whose weights are not of the form alpha_k * {-1, 0, +1} with a finite alpha (raw fp32 weights, an all-zero
+    ternary channel) stays un-frozen, and so does every producer without a frozen consumer.  A consumer takes a plane only
+    from the unmodified tagged producer output; anything else reads ``functional.materialized`` of what it receives.  The
+    logits equal the un-frozen eval forward's bit for bit (same integer sums, same fmaf, same BatchNorm op sequence).
+    Parameters, buffers and state_dict keys are unchanged; ``enable=False`` restores the modules (needed before training)."""
+    from .fused import BatchNormBinarize2d, EngineMaxPool2d, EnginePmConv2d, _pool_cfg
+    _undo(model)
+    if not enable:
+        return model
+    undo = model.__dict__.setdefault("_mnb_xnor_undo", [])
+    for seq in [m for m in model.modules() if isinstance(m, nn.Sequential)]:
+        kids, blocks = _blocks(seq)
+        frozen = set()
+        links = []
+        # from the last block back: a producer is frozen only when its consumer reads what it writes
+        for i, name, blk, conv, act in reversed(blocks):
+            j, pool = i + 1, None
+            if (j < len(kids) and type(kids[j][1]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j][1]) == (2, 2, 0)
+                    and not isinstance(act, BatchNormBinarize2d)):
+                pool, j = kids[j], j + 1
+            if j >= len(kids):
+                continue
+            nxt = kids[j][1]
+            shuffled = bool(getattr(nxt, "channel_shuffle_flag", 0)) and int(getattr(nxt, "shuffle_groups", 1)) > 1
+            if isinstance(act, BatchNormBinarize2d) and shuffled:
+                continue        # a shuffle the fused producer did not take (not a graph prepare(fuse_bn=True) builds)
+            nparts = [k for k in nxt.children() if not isinstance(k, nn.Identity)] if hasattr(nxt, "channel_shuffle_flag") else []
+            cconv = nparts[0] if nparts and isinstance(nparts[0], nn.Conv2d) else None
+            if cconv is None:
+                continue
+            sg = int(nxt.shuffle_groups) if shuffled else (int(act.out_shuffle_groups) if isinstance(act, BatchNormBinarize2d) else 1)
+            link = None
+            if cconv in frozen:
+                link = _Link(cconv, L.XNOR_BITS, cconv.groups, act, pool[1] if pool else None, sg)
+            elif _head_conv(cconv) and not isinstance(cconv, QuantConv2d) and sg == 1 and pool is None and not (
+                    isinstance(act, BatchNormBinarize2d) and act.pool2):
+                link = _Link(cconv, L.XNOR_PM1_BF16, 1, act, None, 1)
+            if link is None:
+                continue
+            if isinstance(conv, QuantConv2d):
+                if not _freezable(conv):
+                    continue
+                frozen.add(conv)
+                links.append(("conv", conv, link, pool, nxt, shuffled, kids[j][0]))
+            elif link.fmt == L.XNOR_BITS and type(conv) is not QuantConv2d:
+                links.append(("stem", act, link, pool, nxt, shuffled, kids[j][0]))
+        for kind, mod, link, pool, nxt, shuffled, nxt_name in links:
+            if kind == "conv":
+                mod.__dict__["_mnb_xnor"] = lambda m, x, link=link: _frozen_conv_forward(link, m, x)
+                undo.append(("dict", mod, "_mnb_xnor", None))
+                undo.append(("dict", mod, "_mnb_xnor_ops", None))
+                link.act.__dict__["_mnb_xnor"] = _absorbed       # its work is done in the conv's epilogue
+                undo.append(("dict", link.act, "_mnb_xnor", None))
+            else:
+                mod.__dict__["_mnb_xnor"] = lambda m, x, link=link: _frozen_stem_forward(link, m, x)
+                undo.append(("dict", mod, "_mnb_xnor", None))
+            if pool is not None:
+                undo.append(("child", seq, pool[0], pool[1]))
+                seq._modules[pool[0]] = nn.Identity()
+            if shuffled:
+                undo.append(("attr", nxt, "channel_shuffle_flag", nxt.channel_shuffle_flag))
+                nxt.channel_shuffle_flag = 0
+            if link.fmt == L.XNOR_PM1_BF16 and type(link.consumer) is nn.Conv2d:
+                # the BatchNorm-fused head reads the +-1 plane on the packed-operand family (same parameters)
+                h = link.consumer
+                pm = EnginePmConv2d(h.in_channels, h.out_channels, h.kernel_size, h.stride, h.padding, h.dilation, h.groups,
+                                    h.bias is not None, h.padding_mode)
+                pm.weight, pm.bias = h.weight, h.bias
+                pm.train(h.training)
+                for n, k in nxt.named_children():
+                    if k is h:
+                        undo.append(("child", nxt, n, h))
+                        nxt._modules[n] = pm
     return model

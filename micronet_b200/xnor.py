@@ -48,3 +48,37 @@ def pack_weight(sh, w_int):
 def conv(sh, a_bits, w_img, out, alpha=None, bias=None):
     return L.load().mnb_xnor_conv_fwd(C.byref(sh), a_bits.data_ptr(), w_img.data_ptr(), L.ptr(alpha), L.ptr(bias),
                                       out.data_ptr(), L.stream())
+
+
+def post_struct(fmt, out_groups=1, shuffle_groups=1, pool2=False, bn=None):
+    """mnb_xnor_post: ``bn`` = (mean, invstd, gamma, beta) fp32 [C] device tensors of an eval BatchNorm, or None"""
+    ptrs = [None] * 4 if bn is None else [t.data_ptr() for t in bn]
+    return L.XnorPost(fmt, int(out_groups), int(shuffle_groups), 1 if pool2 else 0, *ptrs)
+
+
+def post_bytes(sh, post):
+    return int(L.load().mnb_xnor_post_bytes(C.byref(sh), C.byref(post)))
+
+
+def conv_post(sh, a_bits, w_img, post, out, alpha=None, bias=None):
+    """the convolution with the sign-bit epilogue: ``out`` (post_bytes(sh, post) bytes) receives the consumer's operand"""
+    return L.load().mnb_xnor_conv_post(C.byref(sh), a_bits.data_ptr(), w_img.data_ptr(), L.ptr(alpha), L.ptr(bias),
+                                       C.byref(post), out.data_ptr(), L.stream())
+
+
+def pack_act_post(x, post, out):
+    b, c, h, w = x.shape
+    return L.load().mnb_xnor_pack_act_post(x.data_ptr(), b, c, h, w, C.byref(post), out.data_ptr(), L.stream())
+
+
+def unpack(bits, shape, groups):
+    """bit plane u32 [B][G][ceil(C/g / 32)][H][W] -> the +-1 fp32 tensor [B, C, H, W] it encodes (for readers outside the
+    frozen graph: tests, hooks, a module the plane was not written for)"""
+    b, c, h, w = shape
+    cg = c // groups
+    nw = (cg + 31) // 32
+    words = bits.view(b, groups, nw, h, w)
+    ch = torch.arange(c, device=bits.device)
+    sel = words[:, ch // cg, (ch % cg) // 32]                                  # [B, C, H, W] word of each channel
+    bit = (sel >> (ch % 32).view(1, c, 1, 1).to(torch.int32)) & 1
+    return (bit * 2 - 1).float()
