@@ -415,6 +415,19 @@ typedef struct mnb_pk_post {
   int32_t relu;             /* an nn.ReLU sits between producer and consumer */
   int32_t phase_split;
   void* out_pk;             /* mnb_pk_act_bytes(B, C_out, OH, OW, 1) bytes, 16-byte aligned */
+  /* Trailing fields, zero = absent (mnb_pk_conv_post and mnb_pk_i8_conv only; the QuantAdd producers ignore them):
+   * eval BatchNorm2d between the conv and the [ReLU +] quantizer, y' = fmaf(y - mean, gamma * invstd, beta) - the op
+   * sequence of mnb_bn_relu_quant_pack_fwd, so a DoReFa block conv -> nn.BatchNorm2d -> nn.ReLU -> QuantConv2d
+   * (nin.py / nin_gc.py conv-bn-relu blocks, DF:36-46) writes the levels that producer writes from the fp32 output, bit for
+   * bit.  All four NULL or all four [C_out]; a partial set is MNB_E_ARG.
+   * shuffle_groups > 1: the consumer block's channel_shuffle (nin_gc.py:14-22) - producer channel c is stored as consumer
+   * channel (c % cpg) * sg + c / cpg, cpg = C_out / sg.  MNB_E_UNSUPPORTED unless sg divides C_out, C_out fills whole
+   * 16-byte units (8 bf16 / 16 int8 channels) and phase_split is 0. */
+  const float* bn_mean;
+  const float* bn_invstd;
+  const float* bn_gamma;
+  const float* bn_beta;
+  int32_t shuffle_groups;
 } mnb_pk_post;
 int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
                      const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, float* out,
@@ -451,6 +464,23 @@ int mnb_pk_i8_conv(const mnb_conv_shape* s, const void* a_pk, const void* w_img,
                    mnb_stream_t stream);
 int mnb_quant_add_pack_i8_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
                               const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post, mnb_stream_t stream);
+/* Frozen DoReFa inference graphs (the reference's quant_inference flow, wqaq/dorefa/quant_model_test/quant_model_test.py:185-194).
+ * int8 planes also hold DoReFa levels 0 .. 2^a - 1 for a = 2..7 (DF:36-46); weight levels +-(2^w - 1) fit s8 for w <= 7.
+ * 8-bit DoReFa activations stay on the bf16 planes: every int8 entry point refuses them with MNB_E_UNSUPPORTED.
+ *   mnb_bn_relu_quant_pack_i8_fwd : mnb_bn_relu_quant_pack_fwd (same BatchNorm, ReLU and shuffle sequence) writing the int8
+ *                                   plane of a DoReFa quantizer with 2..7 bits; no STE bits (inference only).  Needs
+ *                                   C % 16 == 0 and H*W % 32 == 0, else MNB_E_UNSUPPORTED.
+ *   mnb_pk_plane_maxpool          : max_pool2d(k, stride s, padding p) of a level plane (int8 != 0: int8 [b][c/16][h][w][16],
+ *                                   else bf16 [b][c/8][h][w][8]) into the same layout at the pooled size, padding skipped.
+ *                                   Exact for every plane a quantizer writes: DoReFa's floor(clamp(0.1 x, 0, 1) / s + 0.5)
+ *                                   and ReLU are monotone non-decreasing, so Q(maxpool(relu(y))) == maxpool(Q(relu(y))).
+ *                                   Square windows with 2 * p <= k (nin.py:51/56, nin_gc.py:126/131); the output feeds a
+ *                                   stride-1 consumer (no phase split). */
+int mnb_bn_relu_quant_pack_i8_fwd(const float* x, int32_t batch, int32_t channels, int32_t hw, const float* mean,
+                                  const float* invstd, const float* gamma, const float* beta, const mnb_act_qparams* qp,
+                                  int32_t out_shuffle_groups, void* x_packed, mnb_stream_t stream);
+int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s, int32_t p,
+                         int32_t int8, void* out_pk, mnb_stream_t stream);
 int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x);
 int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                  const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);

@@ -28,8 +28,11 @@ class ActQParams(C.Structure):
 
 
 class PkPost(C.Structure):
-    """mnb_pk_post: the consumer of a frozen-inference producer (its quantizer and operand plane)"""
-    _fields_ = [("q", C.POINTER(ActQParams)), ("relu", C.c_int32), ("phase_split", C.c_int32), ("out_pk", C.c_void_p)]
+    """mnb_pk_post: the consumer of a frozen-inference producer (its quantizer and operand plane); the trailing fields (eval
+    BatchNorm, channel shuffle) are absent when left at zero"""
+    _fields_ = [("q", C.POINTER(ActQParams)), ("relu", C.c_int32), ("phase_split", C.c_int32), ("out_pk", C.c_void_p),
+                ("bn_mean", C.c_void_p), ("bn_invstd", C.c_void_p), ("bn_gamma", C.c_void_p), ("bn_beta", C.c_void_p),
+                ("shuffle_groups", C.c_int32)]
 
 
 XNOR_BITS, XNOR_PM1_BF16 = 0, 1
@@ -125,6 +128,8 @@ PROTOTYPES = {
     "mnb_pk_i8_pack_weight": (C.c_int, [_SHAPE, _P, _P, _P]),
     "mnb_pk_i8_conv": (C.c_int, [_SHAPE, _P, _P, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P]),
     "mnb_quant_add_pack_i8_fwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _ACTQ, _I, _P, C.POINTER(PkPost), _P]),
+    "mnb_bn_relu_quant_pack_i8_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _ACTQ, _I, _P, _P]),
+    "mnb_pk_plane_maxpool": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "mnb_pk_wgrad_scratch_bytes": (_L, [_SHAPE, _I, _I]),
     "mnb_pk_wgrad": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_pk_wgrad_taps_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),

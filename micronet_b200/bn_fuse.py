@@ -127,3 +127,15 @@ def wbwtab_quantize_inference_weights(model):
         if isinstance(m, _wb.QuantConv2d):
             m.weight.data = m.weight_quantizer(m.weight)
     return model
+
+
+@torch.no_grad()
+def dorefa_quantize_inference_weights(model):
+    """the weight step of the reference's DoReFa deployment flow (``wqaq/dorefa/quant_model_test/quant_model_test.py:
+    191-194``): every DoReFa ``QuantConv2d`` stores its quantized weight, ``m.weight.data = m.weight_quantizer(m.weight)``, so
+    a ``quant_inference`` layer holds the levels (2 k - n) / n, n = 2^w - 1, that ``dorefa.freeze_inference`` recovers"""
+    from . import dorefa as _df
+    for m in model.modules():
+        if isinstance(m, _df.QuantConv2d):
+            m.weight.data = m.weight_quantizer(m.weight)
+    return model

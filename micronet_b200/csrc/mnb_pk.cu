@@ -415,7 +415,7 @@ __global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__
 __global__ void __launch_bounds__(256) pack_act_i8_kernel(const float* __restrict__ x, int B, int C, int H, int W, int C16,
                                                           mnb_act_qparams qp, int phase_split, int relu, uint4* __restrict__ out) {
   const MnbActQ q = mnb_load_actq(qp);
-  const float zp = qp.zero_point ? __ldg(qp.zero_point) : 0.f;
+  const float zp = (qp.mode == MNB_ACT_IAO && qp.zero_point) ? __ldg(qp.zero_point) : 0.f;
   const uint32_t HW = (uint32_t)H * (uint32_t)W;
   const uint32_t plane = blockIdx.y * blockDim.y + threadIdx.y;                 // b * C16 + c16
   if (plane >= (uint32_t)B * (uint32_t)C16) return;
@@ -488,6 +488,75 @@ __global__ void __launch_bounds__(256) bn_relu_quant_pack_kernel(const float* __
     }
     xp[((int64_t)b * c8n + oc8) * hw + pos] = make_uint4(pack2(lev[0], lev[1]), pack2(lev[2], lev[3]), pack2(lev[4], lev[5]),
                                                           pack2(lev[6], lev[7]));
+  }
+}
+
+// bn_relu_quant_pack_kernel writing the int8 plane [b][c/16][hw][16] of a DoReFa quantizer with 2..7 bits (inference only:
+// no STE bits); same BatchNorm, ReLU and shuffle sequence.  One warp = 32 consecutive positions of one output unit.
+__global__ void __launch_bounds__(256) bn_relu_quant_pack_i8_kernel(const float* __restrict__ x, int batch, int channels, int hw,
+                                                                    int sg, const float* __restrict__ mean,
+                                                                    const float* __restrict__ invstd,
+                                                                    const float* __restrict__ gamma,
+                                                                    const float* __restrict__ beta, mnb_act_qparams qp,
+                                                                    uint4* __restrict__ xp) {
+  const int lane = threadIdx.x & 31;
+  const int c16n = channels / 16, p32n = hw / 32, cpg = channels / sg;
+  const int64_t items = (int64_t)batch * c16n * p32n;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const MnbActQ q = mnb_load_actq(qp);
+  for (int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < items; w += nwarps) {
+    const int p32 = (int)(w % p32n);
+    const int64_t t = w / p32n;
+    const int oc16 = (int)(t % c16n), b = (int)(t / c16n);
+    const int pos = p32 * 32 + lane;
+    float lev[16], yv[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int oc = oc16 * 16 + j;
+      const int c = sg > 1 ? (oc % sg) * cpg + oc / sg : oc;
+      const int64_t fi = ((int64_t)b * channels + c) * hw + pos;
+      yv[j] = fmaxf(fmaf(__ldg(x + fi) - __ldg(mean + c), __ldg(gamma + c) * __ldg(invstd + c), __ldg(beta + c)), 0.f);
+    }
+    uint32_t passbits;
+    mnb_act_levels<16>(q, yv, lev, passbits);
+    xp[((int64_t)b * c16n + oc16) * hw + pos] = pack16_s8(lev);
+  }
+}
+
+// window max of a level plane [b][unit][H][W][16 B] (bf16 or s8 levels), unit by unit, padding skipped: the plane of
+// max_pool2d(k, s, p) of the decoded activations, because every quantizer whose levels a plane holds is monotone
+// non-decreasing.  One thread = one output position of one unit.
+template <bool I8>
+__global__ void __launch_bounds__(256) plane_maxpool_kernel(const uint4* __restrict__ in, int64_t planes, int H, int W, int k,
+                                                            int s, int pad, int OH, int OW, uint4* __restrict__ out) {
+  const int64_t total = planes * OH * OW;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int ow = (int)(idx % OW);
+    const int64_t t = idx / OW;
+    const int oh = (int)(t % OH);
+    const uint4* src = in + (t / OH) * H * W;
+    const int h0 = oh * s - pad, w0 = ow * s - pad;
+    uint4 m = make_uint4(0, 0, 0, 0);
+    bool first = true;
+    for (int i = max(h0, 0); i < min(h0 + k, H); ++i)
+      for (int j = max(w0, 0); j < min(w0 + k, W); ++j) {
+        const uint4 v = __ldg(src + (int64_t)i * W + j);
+        if (first) { m = v; first = false; continue; }
+        uint32_t* mm = reinterpret_cast<uint32_t*>(&m);
+        const uint32_t* vv = reinterpret_cast<const uint32_t*>(&v);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          if constexpr (I8) {
+            mm[e] = __vmaxs4(mm[e], vv[e]);
+          } else {
+            __nv_bfloat162 a = *reinterpret_cast<__nv_bfloat162*>(&mm[e]);
+            const __nv_bfloat162 b = *reinterpret_cast<const __nv_bfloat162*>(&vv[e]);
+            a = __hmax2(a, b);
+            mm[e] = *reinterpret_cast<uint32_t*>(&a);
+          }
+        }
+      }
+    out[idx] = m;
   }
 }
 
@@ -804,6 +873,10 @@ struct ConvParams {
   uint4* post_out;
   mnb_act_qparams post_q;
   int post_relu, post_split;
+  // eval BatchNorm between the conv and the consumer's [ReLU +] quantizer (all four or none) and the consumer block's
+  // channel shuffle (post_sg > 1: producer channel c lands at consumer channel (c % cpg) * sg + c / cpg, cpg = NOUT / sg)
+  const float *post_mean, *post_invstd, *post_gamma, *post_beta;
+  int post_sg;
   int* err;
 };
 
@@ -812,6 +885,7 @@ struct alignas(16) ConvShared {
   uint32_t abort;
   alignas(16) float epi_scale[256];
   alignas(16) float epi_bias[256];
+  uint16_t epi_dst[256];     // consumer channel of each channel of the N tile (shuffled consumer plane only)
 };
 
 template <int NEPI>
@@ -838,7 +912,10 @@ constexpr int kConvThreads = 384;   // warp 0 TMA, warps 4..11 two MMA + epilogu
 // (et % 128) of the tile raster and one 16-column slot (et / 128) of the two.
 // I8: int8 operands (16 channels per 16-byte unit, s8 K32 MMAs into s32 accumulators, exact); the sums are converted to
 // fp32 once (__int2float_rn) ahead of the same epilogue, and a consumer plane is written as int8.
-template <bool SEG, int NT, bool I8 = false>
+// XPOST (forward with a consumer plane only): the consumer plane with an eval BatchNorm and / or a channel shuffle in front of
+// the quantizer.  Instances of their own: with both epilogues in one instance the plain consumer plane's code (the IAO frozen
+// graphs) loses registers to the other and ran 22-25% slower on frozen ResNet-18 (DESIGN.md 4.15).
+template <bool SEG, int NT, bool I8 = false, bool XPOST = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1,
                const __grid_constant__ CUtensorMap tmap2, const __grid_constant__ ConvParams p) {
@@ -937,6 +1014,12 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           if (p.bias) bs = __ldg(p.bias + n_base + n);
         }
         sh.epi_scale[n] = scv; sh.epi_bias[n] = bs;
+        if constexpr (XPOST) {
+          if (p.post_sg > 1 && n < n_cnt) {
+            const int c = n_base + n, cpg = p.NOUT / p.post_sg;
+            sh.epi_dst[n] = (uint16_t)((c % cpg) * p.post_sg + c / cpg);
+          }
+        }
         if constexpr (!SEG && !I8) {   // one snapshot of the decode pair: from the items of M group 0
           if (p.dec && mg == 0 && y == 0 && n < n_cnt) { p.dec[n_base + n] = scv; p.dec[p.NOUT + n_base + n] = bs; }
         }
@@ -1047,6 +1130,70 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
 #pragma unroll
           for (int k = 0; k < 16; ++k, cp += plane)
             if (n0 + k < n_cnt) *cp = (int16_t)__float2int_rn(r[k]);
+          return;
+        }
+        if constexpr (XPOST) {
+          float* op0 = p.out + orow + (int64_t)n0 * plane;
+          // consumer plane with an eval BatchNorm in front of the [ReLU +] quantizer (the op sequence of
+          // bn_relu_quant_pack_kernel) and / or the consumer block's channel shuffle.  Four chunks of four channels (the
+          // quantizer is elementwise) with the packed words carried over: few values are live at a time, which keeps these
+          // instances free of spills.
+          const int64_t oct_stride = p.post_split ? (int64_t)(p.OH >> 1) * (p.OW >> 1) : plane;
+          uint32_t pw[4];     // packed words of the current 16-byte unit (bf16: 8 channels, int8: 16 channels)
+#pragma unroll
+          for (int qc = 0; qc < 4; ++qc) {
+            if (!I8 && qc >= 2 && n0 + 8 >= n_cnt) break;
+            float lev[4], yv[4];
+            // 16-byte loads of the chunk's per-channel constants (BatchNorm arrays: 16-byte aligned, C_out % 4 == 0, checked
+            // on the host; a chunk past the tile's last channel re-reads the first one)
+            const float4 sc4 = *reinterpret_cast<const float4*>(&sh.epi_scale[n0 + 4 * qc]);
+            const float4 bs4 = *reinterpret_cast<const float4*>(&sh.epi_bias[n0 + 4 * qc]);
+            const float scv[4] = {sc4.x, sc4.y, sc4.z, sc4.w}, bsv[4] = {bs4.x, bs4.y, bs4.z, bs4.w};
+            float mu[4] = {0.f, 0.f, 0.f, 0.f}, gs[4] = {0.f, 0.f, 0.f, 0.f}, be[4] = {0.f, 0.f, 0.f, 0.f};
+            if (p.post_mean) {
+              const int c0 = n_base + n0 + (n0 + 4 * qc < n_cnt ? 4 * qc : 0);
+              const float4 m4 = __ldg(reinterpret_cast<const float4*>(p.post_mean + c0));
+              const float4 g4 = __ldg(reinterpret_cast<const float4*>(p.post_gamma + c0));
+              const float4 i4 = __ldg(reinterpret_cast<const float4*>(p.post_invstd + c0));
+              const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.post_beta + c0));
+              mu[0] = m4.x; mu[1] = m4.y; mu[2] = m4.z; mu[3] = m4.w;
+              gs[0] = __fmul_rn(g4.x, i4.x); gs[1] = __fmul_rn(g4.y, i4.y); gs[2] = __fmul_rn(g4.z, i4.z); gs[3] = __fmul_rn(g4.w, i4.w);
+              be[0] = b4.x; be[1] = b4.y; be[2] = b4.z; be[3] = b4.w;
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const int k = 4 * qc + j;
+              float v = fmaf(r[k], scv[j], bsv[j]);
+              if (p.out && n0 + k < n_cnt) op0[(int64_t)k * plane] = v;
+              if (p.post_mean) v = fmaf(__fsub_rn(v, mu[j]), gs[j], be[j]);
+              yv[j] = p.post_relu ? fmaxf(v, 0.f) : v;
+            }
+            uint32_t passbits;
+            mnb_act_levels<4>(pq, yv, lev, passbits);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) lev[j] = n0 + 4 * qc + j < n_cnt ? lev[j] + pzp : 0.f;
+            if (p.post_sg > 1) {   // consecutive channels land in different consumer units: one element at a time
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                if (n0 + 4 * qc + j >= n_cnt) continue;
+                const int oc = sh.epi_dst[n0 + 4 * qc + j];
+                if constexpr (I8)
+                  reinterpret_cast<int8_t*>(p.post_out)[(prow + (int64_t)(oc >> 4) * oct_stride) * 16 + (oc & 15)] =
+                      (int8_t)__float2int_rn(lev[j]);
+                else
+                  reinterpret_cast<__nv_bfloat16*>(p.post_out)[(prow + (int64_t)(oc >> 3) * oct_stride) * 8 + (oc & 7)] =
+                      __float2bfloat16_rn(lev[j]);
+              }
+            } else if constexpr (I8) {   // one 16-channel unit (n_base + n0 is a multiple of 16: checked on the host)
+              pw[qc] = pack4_s8(lev[0], lev[1], lev[2], lev[3]);
+              if (qc == 3) p.post_out[prow + (int64_t)((n_base + n0) >> 4) * oct_stride] = make_uint4(pw[0], pw[1], pw[2], pw[3]);
+            } else {
+              pw[2 * (qc & 1)] = pack2(lev[0], lev[1]);
+              pw[2 * (qc & 1) + 1] = pack2(lev[2], lev[3]);
+              if (qc & 1)
+                p.post_out[prow + (int64_t)(((n_base + n0) >> 3) + (qc >> 1)) * oct_stride] = make_uint4(pw[0], pw[1], pw[2], pw[3]);
+            }
+          }
           return;
         }
         float sc[16], bs[16];
@@ -1644,10 +1791,15 @@ static bool unit_grid(int batch, int units, int hw, dim3& blocks, dim3& threads)
   return gy <= 65535;
 }
 
-// the quantizers whose levels fit s8 (symmetric IAO, 2..8 bits): the only ones an int8 plane holds
+// the quantizers whose levels fit s8: symmetric IAO with 2..8 bits, DoReFa with 2..7 bits (levels 0 .. 2^a - 1); the only
+// ones an int8 plane holds
 static bool i8_quantizer(const mnb_act_qparams* q) {
+  if (q->mode == MNB_ACT_DOREFA) return q->bits >= 2 && q->bits <= 7;
   return q->mode == MNB_ACT_IAO && q->q_type == 0 && q->bits >= 2 && q->bits <= 8 && q->qmin >= -128 && q->qmax <= 127;
 }
+static const char* const kI8QuantizerRule =
+    "int8 plane needs a symmetric IAO quantizer with 2..8 bits or a DoReFa quantizer with 2..7 bits (8-bit DoReFa levels "
+    "reach 255)";
 
 // mnb_quant_add_pack_fwd (CPU = 8: bf16 consumer plane) and mnb_quant_add_pack_i8_fwd (CPU = 16: int8 consumer plane)
 template <int CPU>
@@ -1657,7 +1809,7 @@ static int quant_add_pack(const float* a, const float* b, int32_t batch, int32_t
   MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad quant_add_pack shape");
   MNB_REQUIRE(qp->mode == MNB_ACT_DOREFA || qp->mode == MNB_ACT_IAO, "QuantAdd takes a DoReFa or IAO quantizer");
   if (CPU == 16) {
-    if (!i8_quantizer(post->q)) return mnb_fail(MNB_E_UNSUPPORTED, "int8 consumer plane needs a symmetric IAO quantizer with 2..8 bits");
+    if (!i8_quantizer(post->q)) return mnb_fail(MNB_E_UNSUPPORTED, "quant_add_pack: %s", kI8QuantizerRule);
   } else {
     MNB_REQUIRE(post->q->mode == MNB_ACT_DOREFA || post->q->mode == MNB_ACT_IAO, "consumer quantizer must be DoReFa or IAO");
   }
@@ -1841,6 +1993,47 @@ extern "C" int mnb_bn_relu_quant_pack_fwd(const float* x, int32_t batch, int32_t
   return 0;
 }
 
+extern "C" int mnb_bn_relu_quant_pack_i8_fwd(const float* x, int32_t batch, int32_t channels, int32_t hw, const float* mean,
+                                             const float* invstd, const float* gamma, const float* beta,
+                                             const mnb_act_qparams* qp, int32_t out_shuffle_groups, void* x_packed,
+                                             mnb_stream_t stream) {
+  MNB_REQUIRE(x && mean && invstd && gamma && beta && qp && x_packed, "NULL bn_relu_quant_pack_i8 pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && hw > 0, "bad bn_relu_quant_pack_i8 shape");
+  MNB_REQUIRE(out_shuffle_groups >= 1 && channels % out_shuffle_groups == 0, "shuffle groups %d do not divide %d channels",
+              out_shuffle_groups, channels);
+  if (qp->mode != MNB_ACT_DOREFA || !i8_quantizer(qp))
+    return mnb_fail(MNB_E_UNSUPPORTED, "bn_relu_quant_pack_i8: the int8 producer takes a DoReFa quantizer with 2..7 bits");
+  if (channels % 16 || hw % 32 || (reinterpret_cast<uintptr_t>(x_packed) & 15))
+    return mnb_fail(MNB_E_UNSUPPORTED, "int8 producer needs channels %% 16 == 0, H*W %% 32 == 0, 16-byte aligned output");
+  const int64_t warps = (int64_t)batch * (channels / 16) * (hw / 32);
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(warps, 8), (int64_t)MNB_NUM_SMS * 16);
+  pk::bn_relu_quant_pack_i8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, batch, channels, hw, out_shuffle_groups, mean,
+                                                                          invstd, gamma, beta, *qp,
+                                                                          reinterpret_cast<uint4*>(x_packed));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
+                                    int32_t s, int32_t p, int32_t int8, void* out_pk, mnb_stream_t stream) {
+  MNB_REQUIRE(in_pk && out_pk && in_pk != out_pk, "NULL or aliased pk_plane_maxpool pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad pk_plane_maxpool shape");
+  MNB_REQUIRE(((reinterpret_cast<uintptr_t>(in_pk) | reinterpret_cast<uintptr_t>(out_pk)) & 15) == 0,
+              "packed tensors must be 16-byte aligned");
+  if (k < 1 || s < 1 || p < 0 || 2 * p > k || h + 2 * p < k || w + 2 * p < k)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool: kernel %d, stride %d, padding %d on %d x %d (needs 2 * p <= k)", k, s,
+                    p, h, w);
+  const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
+  const int64_t planes = (int64_t)batch * ((channels + (int8 ? 15 : 7)) / (int8 ? 16 : 8));
+  const int64_t total = planes * oh * ow;
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 16);
+  auto kern = int8 ? pk::plane_maxpool_kernel<true> : pk::plane_maxpool_kernel<false>;
+  kern<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint4*>(in_pk), planes, h, w, k, s, p, oh, ow,
+                                                 reinterpret_cast<uint4*>(out_pk));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
 // host only: out[0..15] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator
 //                          columns MT * Nt, TH, TB, BW, n_mtiles, n_items, ny},
 //            out[16..20] = {segmented, seg_len, npairs, col_tiles, n_mgroups}; the first min(n, 21) are written
@@ -1892,11 +2085,25 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     if (pl.segmented || terms_a != 1 || terms_w != 1)
       return unsupported("int16 codes need one activation piece, one weight piece and a non-segmented plan");
   }
-  if (post && cpu == 16) {   // int8 consumer plane: s8 levels of a symmetric IAO quantizer, 16-channel units
+  if (post) {   // BatchNorm and channel shuffle in front of the consumer's quantizer
+    const int nbn = (post->bn_mean != nullptr) + (post->bn_invstd != nullptr) + (post->bn_gamma != nullptr) + (post->bn_beta != nullptr);
+    MNB_REQUIRE(nbn == 0 || nbn == 4, "pk conv: the consumer's BatchNorm needs all four of mean, invstd, gamma, beta");
+    if (nbn) {
+      MNB_REQUIRE(((reinterpret_cast<uintptr_t>(post->bn_mean) | reinterpret_cast<uintptr_t>(post->bn_invstd) |
+                    reinterpret_cast<uintptr_t>(post->bn_gamma) | reinterpret_cast<uintptr_t>(post->bn_beta)) & 15) == 0,
+                  "pk conv: the consumer's BatchNorm arrays must be 16-byte aligned");
+      if (pl.NOUT % 4) return unsupported("the consumer's BatchNorm needs output channels % 4 == 0");
+    }
+    MNB_REQUIRE(post->shuffle_groups >= 0, "pk conv: shuffle groups %d", post->shuffle_groups);
+    if (post->shuffle_groups > 1) {
+      if (pl.NOUT % post->shuffle_groups) return unsupported("shuffle groups do not divide the output channels");
+      if (post->phase_split) return unsupported("channel shuffle in front of a stride-2 consumer");
+      if (pl.NOUT % cpu) return unsupported("shuffled consumer plane needs output channels % channels per unit == 0");
+    }
+  }
+  if (post && cpu == 16) {   // int8 consumer plane: s8 levels, 16-channel units
     MNB_REQUIRE(post->q && post->out_pk && (reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "pk conv: consumer plane / quantizer");
-    if (post->q->mode != MNB_ACT_IAO || post->q->q_type != 0 || post->q->bits < 2 || post->q->bits > 8 || post->q->qmin < -128 ||
-        post->q->qmax > 127)
-      return unsupported("int8 consumer plane needs a symmetric IAO quantizer with 2..8 bits");
+    if (!i8_quantizer(post->q)) return unsupported(kI8QuantizerRule);
     if (pl.G > 1 && (pl.ng % 16)) return unsupported("int8 consumer plane of a grouped conv needs channels per group % 16 == 0");
   }
   if (post) {
@@ -1956,6 +2163,8 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   p.out = out; p.err = err_flag; p.codes = codes; p.dec = dec;
   if (post) {
     p.post_out = reinterpret_cast<uint4*>(post->out_pk); p.post_q = *post->q; p.post_relu = post->relu; p.post_split = post->phase_split;
+    p.post_mean = post->bn_mean; p.post_invstd = post->bn_invstd; p.post_gamma = post->bn_gamma; p.post_beta = post->bn_beta;
+    p.post_sg = post->shuffle_groups;
   }
   { static const int dbg = [] { const char* e = getenv("MNB_PK_DEBUG"); return e ? atoi(e) : 0; }(); p.dbg = dbg; }
   CUtensorMap tm[3];
@@ -1969,14 +2178,17 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
   const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
   using ConvFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
-#define MNB_PK_CONV_FNS(SEG, I8) {pk_conv_kernel<SEG, 16, I8>, pk_conv_kernel<SEG, 32, I8>, pk_conv_kernel<SEG, 48, I8>, \
-                                  pk_conv_kernel<SEG, 64, I8>, pk_conv_kernel<SEG, 96, I8>, pk_conv_kernel<SEG, 128, I8>}
-  static const ConvFn fns[3][6] = {MNB_PK_CONV_FNS(false, false), MNB_PK_CONV_FNS(true, false), MNB_PK_CONV_FNS(false, true)};
+#define MNB_PK_CONV_FNS(SEG, I8, X) {pk_conv_kernel<SEG, 16, I8, X>, pk_conv_kernel<SEG, 32, I8, X>, pk_conv_kernel<SEG, 48, I8, X>, \
+                                     pk_conv_kernel<SEG, 64, I8, X>, pk_conv_kernel<SEG, 96, I8, X>, pk_conv_kernel<SEG, 128, I8, X>}
+  static const ConvFn fns[5][6] = {MNB_PK_CONV_FNS(false, false, false), MNB_PK_CONV_FNS(true, false, false),
+                                   MNB_PK_CONV_FNS(false, true, false), MNB_PK_CONV_FNS(false, false, true),
+                                   MNB_PK_CONV_FNS(false, true, true)};
 #undef MNB_PK_CONV_FNS
   int ki = -1;
   for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
   if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
-  const ConvFn fn = fns[cpu == 16 ? 2 : (pl.segmented ? 1 : 0)][ki];
+  const bool xpost = post && (post->bn_mean || post->shuffle_groups > 1);   // (segmented plans refuse a post above)
+  const ConvFn fn = fns[cpu == 16 ? (xpost ? 4 : 2) : (pl.segmented ? 1 : (xpost ? 3 : 0))][ki];
   if (int e = set_max_smem(fn, kSmemBudget)) return e;
   fn<<<dim3(gx, pl.ny), kConvThreads, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
   MNB_LAUNCHED(1);
@@ -2024,7 +2236,7 @@ extern "C" int mnb_pk_i8_pack_act(const float* x, int32_t batch, int32_t channel
   MNB_REQUIRE(x && qp && out_pk, "NULL pk_i8_pack_act pointer");
   MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad pk_i8_pack_act arguments");
   MNB_REQUIRE((reinterpret_cast<uintptr_t>(out_pk) & 15) == 0, "packed tensor must be 16-byte aligned");
-  if (!i8_quantizer(qp)) return mnb_fail(MNB_E_UNSUPPORTED, "int8 plane needs a symmetric IAO quantizer with 2..8 bits");
+  if (!i8_quantizer(qp)) return mnb_fail(MNB_E_UNSUPPORTED, "pk_i8_pack_act: %s", kI8QuantizerRule);
   if (phase_split) MNB_REQUIRE(((h | w) & 1) == 0, "phase split needs even H and W");
   MNB_REQUIRE((int64_t)h * w < (1ll << 31), "pk_i8_pack_act: plane too large");
   const int C16 = (channels + 15) / 16;

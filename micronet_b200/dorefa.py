@@ -64,6 +64,8 @@ class QuantConv2d(nn.Conv2d):
         self.weight_quantizer = WeightQuantizer(w_bits=w_bits)
 
     def forward(self, input):
+        if "_mnb_frozen" in self.__dict__:      # set by freeze_inference
+            return _frozen_conv_forward(self, input)
         spec = self.activation_quantizer.spec()
         if not self.quant_inference:
             wq, w_int, w_scale = self.weight_quantizer.quantize(self.weight)
@@ -159,4 +161,270 @@ def prepare(model, inplace=False, a_bits=8, w_bits=8, quant_inference=False, fus
     if fuse:
         from .fused import fuse_blocks
         fuse_blocks(model)
+    return model
+
+
+# --------------------------------------------------------------------------
+# frozen inference graphs on level planes
+# --------------------------------------------------------------------------
+def frozen_levels(conv):
+    """(wq, w_int i16 [K, C/g, R, S], w_scale f32 [K]) of a DoReFa conv with 2..8-bit weights, or None when its weights cannot be
+    frozen.  A QAT layer takes them from its weight quantizer (DF:50-73).  A ``quant_inference`` layer holds that quantizer's
+    output (bn_fuse.dorefa_quantize_inference_weights, quant_model_test.py:191-194): v = 2 k / n - 1 with n = 2^w - 1, so the
+    level is the odd integer round(v * n); anything else (raw fp32 weights, NaN) is refused."""
+    import torch
+    bits = conv.weight_quantizer.w_bits
+    if not 2 <= bits <= 8:
+        return None
+    if not conv.quant_inference:
+        wq, w_int, w_scale = conv.weight_quantizer.quantize(conv.weight)
+        return wq.detach(), w_int.detach(), w_scale.detach()
+    n = float(2 ** bits - 1)
+    v = conv.weight.detach()
+    lv = torch.round(v * n)
+    tol = 4 * torch.finfo(torch.float32).eps       # the reconstruction must match v to fp32 rounding
+    ok = (bool(torch.isfinite(v).all()) and bool((lv.abs() <= n).all()) and bool((lv.remainder(2) == 1).all())
+          and bool(((lv / n - v).abs() <= tol).all()))
+    if not ok:
+        return None
+    return v, lv.to(torch.int16), torch.full((v.shape[0],), 1.0 / n, dtype=torch.float32, device=v.device)
+
+
+def _freezable(conv):
+    if not isinstance(conv, QuantConv2d) or conv.padding_mode != "zeros" or isinstance(conv.padding, str):
+        return False
+    if not (2 <= conv.activation_quantizer.a_bits <= 8 and 2 <= conv.weight_quantizer.w_bits <= 8):
+        return False
+    return not conv.quant_inference or frozen_levels(conv) is not None
+
+
+def _check_eval(m):
+    if m.training:
+        raise RuntimeError("micronet_b200: this module is frozen for inference (dorefa.freeze_inference); call "
+                           "freeze_inference(model, enable=False) before training it")
+
+
+def _frozen_operands(conv):
+    """(wq, w_int, w_scale, bias) computed once; re-done when a parameter or buffer is written in place"""
+    key = tuple(t._version for t in list(conv.parameters()) + list(conv.buffers()))
+    fr = conv.__dict__.get("_mnb_ops")
+    if fr is None or fr[0] != key:
+        lv = frozen_levels(conv)
+        if lv is None:
+            raise RuntimeError("micronet_b200: the weights of a frozen DoReFa layer changed to values that are not weight "
+                               "quantizer levels; call dorefa.freeze_inference(model) again")
+        lv[1]._mnb_pk_cache = {}          # the packed weight images are built once per shape (functional.frozen_conv)
+        fr = (key,) + tuple(lv) + (None if conv.bias is None else conv.bias.detach(),)
+        conv.__dict__["_mnb_ops"] = fr
+    return fr[1:]
+
+
+def _shuffle(x, groups):
+    b, c = x.shape[0], x.shape[1]
+    return x.view(b, groups, c // groups, *x.shape[2:]).transpose(1, 2).contiguous().view(x.shape)
+
+
+class _Link:
+    """a producer -> consumer hand-off of a frozen graph: the consumer conv, the eval BatchNorm and ReLU the producer applies,
+    the consumer block's channel shuffle and the max-pool in between, which runs on the level plane"""
+
+    def __init__(self, cconv, bn, relu, sg, pool):
+        self.cconv, self.bn, self.relu, self.sg, self.pool = cconv, bn, relu, sg, pool
+        self.target = pool[0] if pool is not None else cconv
+        self._invstd = None
+
+    def consumer(self):
+        import torch
+        bn, c = self.bn, self.cconv
+        rv = bn.running_var
+        key = (rv.data_ptr(), rv._version, float(bn.eps))
+        if self._invstd is None or self._invstd[0] != key:
+            self._invstd = (key, torch.rsqrt(rv + bn.eps))     # as the un-frozen eval BatchNormReluQuant2d computes it
+        stats = (bn.running_mean, self._invstd[1], bn.weight.detach(), bn.bias.detach())
+        return F_.Consumer(c, c.activation_quantizer.spec(), self.relu, True, tuple(c.weight.shape), tuple(c.stride),
+                           tuple(c.padding), tuple(c.dilation), c.groups, True, int8=c.__dict__["_mnb_frozen"]["int8"],
+                           bn=stats, shuffle_groups=self.sg, pool=self.pool)
+
+
+def _frozen_conv_forward(conv, x):
+    """eval forward of a frozen DoReFa conv: cached weight levels, the plane its producer wrote (if it got one) and, with a
+    link, its consumer's plane written by the epilogue (BatchNorm, ReLU and shuffle folded in)"""
+    _check_eval(conv)
+    wq, w_int, w_scale, bias = _frozen_operands(conv)
+    spec = conv.activation_quantizer.spec()
+    plane = F_.handed_plane(conv, x)
+    if plane is None:
+        if getattr(x, "_mnb_pk_q", None) is not None:     # a BatchNormReluQuant2d that ran un-linked wrote this conv's plane
+            return F_.quant_conv2d(x, wq, bias, w_int, w_scale, spec, conv.stride, conv.padding, conv.dilation, conv.groups)
+        x = F_.materialized(x)
+        sg = conv.__dict__.get("_mnb_in_shuffle", 1)
+        if sg > 1:
+            x = _shuffle(x, sg)       # the block's channel shuffle that freeze_inference moved into the producer
+    info = conv.__dict__["_mnb_frozen"]
+    link = info.get("link")
+    return F_.frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, conv.stride, conv.padding, conv.dilation, conv.groups,
+                          consumer=link.consumer() if link is not None else None, int8=info["int8"])
+
+
+def _absorbed_forward(m, target, x):
+    """BatchNorm / ReLU whose work a producer did for ``target``: pass its tagged output through, run as usual otherwise"""
+    pre = getattr(x, "_mnb_pk_pre", None)
+    if pre is not None and pre[0] is target:
+        _check_eval(m)
+        return x
+    return type(m).forward(m, x)
+
+
+def _pool_forward(pool, link, x):
+    """the max-pool between a producer and its consumer: mnb_pk_plane_maxpool on the producer's level plane"""
+    import torch
+    from . import pk as PK
+    plane = F_.handed_plane(pool, x)
+    if plane is None:
+        return type(pool).forward(pool, x)
+    _check_eval(pool)
+    _, k, s, p = link.pool
+    b, c, h, w = x.shape
+    fmt = x._mnb_pk_pre[3]
+    out = F_._timed("plane_pool", L.ConvShape(b, c, h, w, c, k, k, s, s, p, p, 1, 1, 1),
+                    lambda: PK.plane_maxpool(plane, b, c, h, w, k, s, p, int8=fmt == "i8"))
+    y = torch.empty((b, c, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1), dtype=torch.float32, device="meta")
+    y._mnb_pk_pre = (link.cconv, out, y._version, fmt)
+    return y
+
+
+def _stem_forward(bn, link, x):
+    """eval BatchNorm + ReLU behind the un-quantized stem conv, written straight as the first quantized conv's level plane
+    (mnb_bn_relu_quant_pack_fwd / _i8_fwd) with the consumer block's shuffle"""
+    import ctypes as C
+    import torch
+    from . import pk as PK
+    _check_eval(bn)
+    x = F_.materialized(x)
+    if x.dim() == 4 and x.is_cuda and x.dtype == torch.float32:
+        consumer = link.consumer()
+        fmt = consumer.format(tuple(x.shape))
+        if fmt is not None:
+            b, c, h, w = x.shape
+            x = x.contiguous()
+            mean, invstd, gamma, beta = (t.data_ptr() for t in consumer.bn)
+            qp = consumer.spec.struct()
+            lib = L.load()
+            if fmt == "i8":
+                plane = PK.consumer_plane_i8(b, c, h, w, x.device)
+                rc = lib.mnb_bn_relu_quant_pack_i8_fwd(x.data_ptr(), b, c, h * w, mean, invstd, gamma, beta, C.byref(qp),
+                                                       consumer.sg, plane.data_ptr(), L.stream())
+            else:
+                plane = PK.consumer_plane(b, c, h, w, x.device)
+                bits = torch.empty((x.numel() + 31) // 32, dtype=torch.int32, device=x.device)   # STE mask (unused)
+                rc = lib.mnb_bn_relu_quant_pack_fwd(x.data_ptr(), b, c, h * w, mean, invstd, gamma, beta, C.byref(qp),
+                                                    consumer.sg, plane.data_ptr(), bits.data_ptr(), L.stream())
+            if rc == 0:
+                return F_._tag(torch.empty(x.shape, dtype=torch.float32, device="meta"), consumer, plane, fmt)
+            if rc != L.E_UNSUPPORTED:
+                L.check(rc, "bn_relu_quant_pack (stem)")
+    return type(bn).forward(bn, x)
+
+
+def _conv_bn_act(blk):
+    """(conv, BatchNorm, nn.ReLU or None, relu applied?) of one of the reference's conv-bn-relu blocks, else None"""
+    from .fused import BatchNormReluQuant2d
+    if not hasattr(blk, "channel_shuffle_flag"):
+        return None
+    parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
+    if len(parts) not in (2, 3) or not isinstance(parts[0], nn.Conv2d):
+        return None
+    bn, act = parts[1], (parts[2] if len(parts) == 3 else None)
+    if type(bn) not in (nn.BatchNorm2d, BatchNormReluQuant2d) or not (bn.affine and bn.track_running_stats):
+        return None
+    if act is not None and (type(act) is not nn.ReLU or isinstance(bn, BatchNormReluQuant2d)):
+        return None
+    return parts[0], bn, act, act is not None or isinstance(bn, BatchNormReluQuant2d)
+
+
+def _undo(model):
+    for rec in reversed(model.__dict__.pop("_mnb_dorefa_undo", [])):
+        if rec[0] == "attr":
+            setattr(rec[1], rec[2], rec[3])
+        else:
+            rec[1].__dict__.pop(rec[2], None)
+
+
+def freeze_inference(model, enable=True, int8=False):
+    """Inference on level planes for a DoReFa model in eval mode (NIN / NIN-GC-style ``nn.Sequential`` of conv-bn-relu
+    blocks; the reference times this graph in wqaq/dorefa/quant_model_test/quant_model_test.py:185-194):
+    * every eval-mode QuantConv2d with 2..8-bit quantizers quantizes and packs its weights ONCE (re-done when a parameter or
+      buffer is written in place);
+    * linking, from the conv-bn-relu block (QuantConv2d, nn.BatchNorm2d or fused.BatchNormReluQuant2d, nn.ReLU or nothing) to
+      the first conv of the next block, when that conv is frozen and any max-pool in between is square with 2 * p <= k and
+      feeds a stride-1 conv: the producer conv's epilogue applies the eval BatchNorm (running statistics), the ReLU, the
+      consumer's quantizer and the next block's channel shuffle and writes the consumer's level plane (mnb_pk_conv_post /
+      mnb_pk_i8_conv); the pool runs on that plane (mnb_pk_plane_maxpool); no fp32 activation is written in between;
+    * the un-quantized stem conv's BatchNorm + ReLU write the first quantized conv's plane (mnb_bn_relu_quant_pack_fwd or
+      its int8 form); the last conv of the model writes fp32 as before;
+    * ``int8``: convs with activation and weight quantizers of at most 7 bits run on int8 operands where the int8 plan
+      covers them (NIN-GC W4A4); 8-bit layers keep the bf16 planes.
+    Covered graphs: ``prepare(...)`` and ``prepare(..., fuse=True)`` in eval mode, and the deployment graph
+    ``prepare(quant_inference=True)`` -> ``bn_fuse.dorefa_quantize_inference_weights``; a layer whose weights are not
+    quantizer levels (raw fp32 weights) stays un-frozen, and so does the producer in front of it.
+    A consumer takes a plane only from the unmodified tagged producer output; when the kernels refuse a shape at run time the
+    absorbed modules run as usual.  Numerics (DESIGN.md 4.15): the levels equal the fused BatchNormReluQuant2d's bit for bit;
+    where the un-frozen graph ran ATen's BatchNorm a level on a rounding boundary may differ by one.  Parameters, buffers
+    and state_dict keys are unchanged; ``enable=False`` restores the modules (needed before training)."""
+    import functools
+    from .fused import EngineFloatConv2d, EngineMaxPool2d, _pool_cfg
+    _undo(model)
+    if not enable:
+        return model
+    undo = model.__dict__.setdefault("_mnb_dorefa_undo", [])
+    frozen = set()
+    for m in model.modules():
+        if isinstance(m, QuantConv2d) and not m.training and _freezable(m):
+            small = m.activation_quantizer.a_bits <= 7 and m.weight_quantizer.w_bits <= 7
+            m.__dict__["_mnb_frozen"] = {"int8": bool(int8) and small, "link": None}
+            undo += [("dict", m, "_mnb_frozen"), ("dict", m, "_mnb_ops")]
+            frozen.add(m)
+
+    def override(m, fn):
+        m.__dict__["forward"] = fn
+        undo.append(("dict", m, "forward"))
+
+    for seq in [m for m in model.modules() if isinstance(m, nn.Sequential)]:
+        kids = [k for k in seq.children() if not isinstance(k, nn.Identity)]
+        for i, blk in enumerate(kids):
+            cba = _conv_bn_act(blk)
+            if cba is None:
+                continue
+            conv, bn, act, relu = cba
+            j, pool = i + 1, None
+            if j < len(kids) and type(kids[j]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j]) is not None:
+                pool, j = kids[j], j + 1
+            if j >= len(kids) or not hasattr(kids[j], "channel_shuffle_flag"):
+                continue
+            nxt = kids[j]
+            nparts = [k for k in nxt.children() if not isinstance(k, nn.Identity)]
+            cconv = nparts[0] if nparts else None
+            if cconv not in frozen or (pool is not None and tuple(cconv.stride) != (1, 1)):
+                continue
+            flag_sg = int(nxt.shuffle_groups) if nxt.channel_shuffle_flag and int(getattr(nxt, "shuffle_groups", 1)) > 1 else 1
+            fold_sg = int(getattr(pool if pool is not None else bn, "out_shuffle_groups", 1))   # folded by fuse=True
+            stem = type(conv) in (nn.Conv2d, EngineFloatConv2d)
+            if not (conv in frozen or (stem and relu and (pool is not None or tuple(cconv.stride) == (1, 1)))):
+                continue
+            link = _Link(cconv, bn, relu, max(flag_sg, fold_sg), None if pool is None else (pool,) + _pool_cfg(pool))
+            target = link.target
+            if stem:
+                override(bn, functools.partial(_stem_forward, bn, link))
+            else:
+                conv.__dict__["_mnb_frozen"]["link"] = link
+                override(bn, functools.partial(_absorbed_forward, bn, target))
+            if act is not None:
+                override(act, functools.partial(_absorbed_forward, act, target))
+            if pool is not None:
+                override(pool, functools.partial(_pool_forward, pool, link))
+            if flag_sg > 1:
+                undo.append(("attr", nxt, "channel_shuffle_flag", nxt.channel_shuffle_flag))
+                nxt.channel_shuffle_flag = 0
+                cconv.__dict__["_mnb_in_shuffle"] = flag_sg     # applied by the consumer when no plane comes
+                undo.append(("dict", cconv, "_mnb_in_shuffle"))
     return model

@@ -755,14 +755,31 @@ class Consumer:
     quantizer, the nn.ReLU in between (folded away), its geometry, whether anybody else needs the fp32 tensor, and
     whether it was frozen with int8 operands (``int8``: then ``format`` tells which plane it reads)"""
 
-    def __init__(self, module, spec, relu, only, w_shape, stride, padding, dilation, groups, int_weights, int8=False):
+    def __init__(self, module, spec, relu, only, w_shape, stride, padding, dilation, groups, int_weights, int8=False, bn=None,
+                 shuffle_groups=1, pool=None):
         self.module, self.spec, self.relu, self.only = module, spec, bool(relu), bool(only)
         self.w_shape, self.stride, self.padding, self.dilation, self.groups = w_shape, stride, padding, dilation, groups
         self.int_weights, self.int8 = int_weights, bool(int8)
+        # DoReFa graphs (dorefa.freeze_inference): the eval BatchNorm (mean, invstd, gamma, beta) the producer's epilogue applies
+        # before the ReLU, the consumer block's channel shuffle, and a max-pool in between: pool = (module, k, s, p), run as
+        # mnb_pk_plane_maxpool on the producer's full-resolution plane, so the producer tags its output for that module
+        self.bn, self.sg, self.pool = bn, int(shuffle_groups), pool
+        self.target = module if pool is None else pool[0]
 
-    def format(self, act_shape):
-        """operand plane the consumer's forward reads for this activation: "i8" (int8 conv), "bf16" (packed-operand conv
+    def read_shape(self, out_shape):
+        """the activation the consumer reads when the producer writes ``out_shape``"""
+        if self.pool is None:
+            return tuple(out_shape)
+        _, k, s, p = self.pool
+        b, c, h, w = out_shape
+        return (b, c, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1)
+
+    def format(self, out_shape):
+        """operand plane the consumer's forward reads for this producer output: "i8" (int8 conv), "bf16" (packed-operand conv
         with a one-piece plane) or None (a producer cannot write its operand).  frozen_conv takes the same decision."""
+        act_shape = self.read_shape(out_shape)
+        if self.sg > 1 and (out_shape[1] % 16 or out_shape[1] % self.sg or self.split):
+            return None       # the epilogue stores a shuffled plane of whole units only, never phase-split
         if self.int8 and act_shape[1] == self.w_shape[1] * self.groups:
             sh = _shape_struct(act_shape, self.w_shape, self.stride, self.padding, self.dilation, self.groups)
             if _i8_route(self.spec, self.int_weights, sh):
@@ -784,7 +801,7 @@ class Consumer:
 
     @property
     def split(self):
-        return self.stride[0] == 2
+        return self.stride[0] == 2 and self.pool is None
 
 
 def handed_plane(module, x):
@@ -798,18 +815,23 @@ def handed_plane(module, x):
 
 
 def _tag(y, consumer, plane, fmt="bf16"):
-    y._mnb_pk_pre = (consumer.module, plane, y._version, fmt)
+    y._mnb_pk_pre = (consumer.target, plane, y._version, fmt)
     return y
 
 
 def _i8_route(spec, w_int, sh):
     """does a conv frozen with int8=True run this forward on the int8 kernels?  Symmetric IAO activations with 2..8 bits
     and levels in [-128, 127] (the quantizer test of the C side: an asymmetric quantizer reports q_type 0 until its first
-    update_qparams, its level range tells), integer weights (the module checks they are symmetric with 2..8 bits) and a
-    shape the int8 plan takes; everything else keeps the bf16 path."""
+    update_qparams, its level range tells) or DoReFa activations with 2..7 bits (levels 0 .. 2^a - 1), integer weights (the
+    module checks they fit s8) and a shape the int8 plan takes; everything else keeps the bf16 path."""
     from . import pk as PK
-    return (spec is not None and bool(w_int is not None) and spec.mode == L.ACT_IAO and spec.q_type == 0 and 2 <= spec.bits <= 8
-            and -128 <= spec.qmin and spec.qmax <= 127 and L.PK_MODE != "off" and PK.i8_supported(sh))
+    if spec is None or w_int is None or L.PK_MODE == "off":
+        return False
+    if spec.mode == L.ACT_DOREFA:
+        ok = 2 <= spec.bits <= 7
+    else:
+        ok = spec.mode == L.ACT_IAO and spec.q_type == 0 and 2 <= spec.bits <= 8 and -128 <= spec.qmin and spec.qmax <= 127
+    return ok and PK.i8_supported(sh)
 
 
 def _i8_producer_writes_plane(out_channels, groups):
@@ -867,7 +889,8 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
     cplane = PK.consumer_plane(*out_shape, dev)
     cqp = consumer.spec.struct()
     L.check(_timed("fwd_pk", sh, lambda: PK.conv_post(sh, plane, ta, w_img, tw, y, cqp, cplane, consumer.relu, consumer.split,
-                                                      n_scale=w_scale, a_scale=a_scale, a_scale_const=a_const, bias=bias)),
+                                                      n_scale=w_scale, a_scale=a_scale, a_scale_const=a_const, bias=bias,
+                                                      bn=consumer.bn, shuffle_groups=consumer.sg)),
             "pk_conv_post")
     if y is None:
         y = torch.empty(out_shape, dtype=torch.float32, device="meta")   # shape only: the data lives in the consumer's plane
@@ -888,16 +911,19 @@ def _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_rel
         w_img = PK.pack_weight_i8(sh, w_int)
         if cache is not None:
             cache[ckey] = w_img
+    # activation scale: IAO's device scalar, DoReFa's 1 / (2^a - 1)
+    a_scale = spec.scale if spec.mode == L.ACT_IAO else None
+    a_const = 1.0 / float(2 ** spec.bits - 1) if spec.mode == L.ACT_DOREFA else 1.0
     if consumer is None:
         y = torch.empty(out_shape, dtype=torch.float32, device=dev)
-        L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=spec.scale, bias=bias)),
-                "pk_i8_conv")
+        L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=a_scale,
+                                                           a_scale_const=a_const, bias=bias)), "pk_i8_conv")
         return y
     y = None if consumer.only else torch.empty(out_shape, dtype=torch.float32, device=dev)
     cplane = PK.consumer_plane_i8(*out_shape, dev)
-    post = (consumer.spec.struct(), cplane, consumer.relu, consumer.split)
-    L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=spec.scale, bias=bias,
-                                                       post=post)), "pk_i8_conv")
+    post = (consumer.spec.struct(), cplane, consumer.relu, consumer.split, consumer.bn, consumer.sg)
+    L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=a_scale,
+                                                       a_scale_const=a_const, bias=bias, post=post)), "pk_i8_conv")
     if y is None:
         y = torch.empty(out_shape, dtype=torch.float32, device="meta")
     return _tag(y, consumer, cplane, "i8")

@@ -105,11 +105,20 @@ def consumer_plane(b, c, h, w, device):
     return torch.empty(int(L.load().mnb_pk_act_bytes(b, c, h, w, 1)), dtype=torch.uint8, device=device)
 
 
+def post_struct(qp, plane, relu, split, bn=None, shuffle_groups=1):
+    """mnb_pk_post of a consumer; ``bn`` = (mean, invstd, gamma, beta) of an eval BatchNorm in front of its [ReLU +] quantizer"""
+    post = L.PkPost(C.pointer(qp), 1 if relu else 0, 1 if split else 0, plane.data_ptr())
+    if bn is not None:
+        post.bn_mean, post.bn_invstd, post.bn_gamma, post.bn_beta = (t.data_ptr() for t in bn)
+    post.shuffle_groups = int(shuffle_groups)
+    return post
+
+
 def conv_post(sh, a_pk, terms_a, w_img, terms_w, out, post_qp, post_plane, post_relu, post_split, n_scale=None, a_scale=None,
-              a_scale_const=1.0, bias=None):
+              a_scale_const=1.0, bias=None, bn=None, shuffle_groups=1):
     """forward conv whose epilogue also writes the consumer's operand plane (frozen inference graphs); out may be None"""
     lib = L.load()
-    post = L.PkPost(C.pointer(post_qp), 1 if post_relu else 0, 1 if post_split else 0, post_plane.data_ptr())
+    post = post_struct(post_qp, post_plane, post_relu, post_split, bn, shuffle_groups)
     return lib.mnb_pk_conv_post(C.byref(sh), a_pk.data_ptr(), terms_a, w_img.data_ptr(), terms_w, L.ptr(n_scale), L.ptr(a_scale),
                                 float(a_scale_const), L.ptr(bias), L.ptr(out), C.byref(post),
                                 L.tc_err_flag(a_pk.device).data_ptr(), L.stream())
@@ -144,6 +153,15 @@ def pack_act_i8(x, qp, phase_split=False, relu=False):
     return out
 
 
+def plane_maxpool(plane, b, c, h, w, k, s, p, int8=False):
+    """max_pool2d(k, s, p) of a level plane of a [b, c, h, w] activation (mnb_pk_plane_maxpool) -> the pooled plane"""
+    oh, ow = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    out = (consumer_plane_i8 if int8 else consumer_plane)(b, c, oh, ow, plane.device)
+    L.check(L.load().mnb_pk_plane_maxpool(plane.data_ptr(), b, c, h, w, k, s, p, 1 if int8 else 0, out.data_ptr(), L.stream()),
+            "pk_plane_maxpool")
+    return out
+
+
 def pack_weight_i8(sh, w_int):
     nbytes = int(L.load().mnb_pk_i8_wimage_bytes(C.byref(sh)))
     if nbytes < 0:
@@ -154,12 +172,11 @@ def pack_weight_i8(sh, w_int):
 
 
 def conv_i8(sh, a_pk, w_img, out, n_scale=None, a_scale=None, a_scale_const=1.0, bias=None, post=None):
-    """forward conv of an int8 plane; ``post`` = (quantizer struct, int8 plane, relu, phase split) of the consumer whose
-    plane the epilogue writes as well (out may then be None).  Returns the C status."""
+    """forward conv of an int8 plane; ``post`` = (quantizer struct, int8 plane, relu, phase split[, BatchNorm tensors,
+    shuffle groups]) of the consumer whose plane the epilogue writes as well (out may then be None).  Returns the C status."""
     pp = None
     if post is not None:
-        qp, plane, relu, split = post
-        pp = C.byref(L.PkPost(C.pointer(qp), 1 if relu else 0, 1 if split else 0, plane.data_ptr()))
+        pp = C.byref(post_struct(*post))
     return L.load().mnb_pk_i8_conv(C.byref(sh), a_pk.data_ptr(), w_img.data_ptr(), L.ptr(n_scale), L.ptr(a_scale),
                                    float(a_scale_const), L.ptr(bias), L.ptr(out), pp, L.tc_err_flag(a_pk.device).data_ptr(),
                                    L.stream())
