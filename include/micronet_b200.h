@@ -287,7 +287,12 @@ int mnb_bn_sign_fwd_packed(const float* x, int32_t batch, int32_t channels, int3
  * Cover: groups 1, stride 1, dilation 1, 'same' odd square filter, C*R*S <= 128, Cout <= 256, 128 % W == 0,
  * (H*W) % 128 == 0; anything else returns MNB_E_UNSUPPORTED (-2).
  *   fwd   : y = conv2d(x, w) + bias (bias may be NULL)
- *   wgrad : dw = corr(x, dy);  scratch >= mnb_fconv2d_wgrad_tc_scratch_bytes(s) (-1: unsupported)        */
+ *   wgrad : dw = corr(x, dy);  scratch >= mnb_fconv2d_wgrad_tc_scratch_bytes(s) (-1: unsupported)
+ *   mnb_fconv2d_plan: host only, the plan the forward (wgrad = 0) or weight gradient (wgrad != 0) will run; the first
+ *                     min(n, 8) of  NP (padded Cout), KP (padded C*R*S), TH (rows per 128-position tile), n_tiles, grid
+ *                     (CTAs), nbuf_a (forward operand buffers), smem_bytes, patch_floats (C * (TH + R - 1) * (W + R - 1))
+ *                     are written.  Refusals as for the launching entry points.                                          */
+int mnb_fconv2d_plan(const mnb_conv_shape* s, int32_t wgrad, int32_t* out, int32_t n);
 int mnb_fconv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const float* w, const float* bias, float* y,
                        int32_t* err_flag, mnb_stream_t stream);
 int64_t mnb_fconv2d_wgrad_tc_scratch_bytes(const mnb_conv_shape* s);

@@ -91,6 +91,7 @@ PROTOTYPES = {
     "mnb_bn_sign_pool_fwd": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
     "mnb_bn_sign_pool_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_bn_sign_fwd_packed": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
+    "mnb_fconv2d_plan": (C.c_int, [_SHAPE, _I, _P, _I]),
     "mnb_fconv2d_fwd_tc": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),
     "mnb_fconv2d_wgrad_tc_scratch_bytes": (_L, [_SHAPE]),
     "mnb_fconv2d_wgrad_tc": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),

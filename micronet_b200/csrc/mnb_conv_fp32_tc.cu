@@ -512,6 +512,16 @@ static int debug_mask() {
 
 }  // namespace tcfp32
 
+extern "C" int mnb_fconv2d_plan(const mnb_conv_shape* s, int32_t wgrad, int32_t* out, int32_t n) {
+  tcfp32::Params p{};
+  int smem_bytes = 0;
+  if (int e = tcfp32::plan(s, wgrad != 0, p, smem_bytes)) return e;
+  const int v[8] = {p.NP, p.KP, p.TH, p.n_tiles, tcfp32::grid_size(p), p.nbuf_a, smem_bytes, p.C * p.PH * p.PW};
+  if (out)
+    for (int i = 0; i < std::min(n, 8); ++i) out[i] = v[i];
+  return 0;
+}
+
 extern "C" int mnb_fconv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const float* w, const float* bias, float* y,
                                   int32_t* err_flag, mnb_stream_t stream) {
   using namespace tcfp32;
