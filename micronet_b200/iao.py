@@ -530,9 +530,12 @@ class QuantAdd(nn.Module):
             # feed the STE range of a backward pass, so a frozen inference model (freeze_inference) skips them
             self.observer_res(res)
             self.observer_shortcut(shortcut)
+            # in place (the reference rebinds the attributes): a CUDA graph captured here keeps writing the buffers it
+            # captured, so a rebinding eager step between replays would leave the module holding a stale range
             obs = q.observer
-            obs.min_val = torch.min(self.observer_res.min_val, self.observer_shortcut.min_val)
-            obs.max_val = torch.max(self.observer_res.max_val, self.observer_shortcut.max_val)
+            with torch.no_grad():
+                torch.minimum(self.observer_res.min_val, self.observer_shortcut.min_val, out=obs.min_val)
+                torch.maximum(self.observer_res.max_val, self.observer_shortcut.max_val, out=obs.max_val)
         if q.bits == 32:
             return res + shortcut
         q._check_bits()
