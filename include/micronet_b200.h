@@ -498,6 +498,22 @@ int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, c
 int mnb_pk_wgrad_taps_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n);
 int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                       const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);
+/* Forward and data gradient of the same narrow grouped 3x3 layers (stride 1, padding 0..2, 16 input / 32 output channels per
+ * group, groups % 4 == 0) with whole images as M tiles and a CTA per block of groups whose weights stay in shared memory.
+ * Forward: one activation piece and one weight piece (mnb_pk_gc3_conv mode 0 = mnb_pk_conv mode 0, mnb_pk_gc3_conv_codes =
+ * mnb_pk_conv_codes); data gradient: two dy pieces and one weight piece on an un-segmented plan (mnb_pk_gc3_conv mode 1 =
+ * mnb_pk_conv mode 1).  Same arguments, same weight image (mnb_pk_pack_weight) and the same result bit for bit: every
+ * element sees the MMA chain of mnb_pk_conv's plan.  MNB_E_UNSUPPORTED (nothing launched) outside that cover.
+ * mnb_pk_gc3_plan (host only): out[0..9] = {groups per CTA block, images per M tile, m64 blocks per M tile, stages, smem
+ * bytes, CTAs, image tiles, MMAs per chain, N tile, MMA warpgroups (stages are a multiple of it)}, then per MMA of the chain in issue order (tap r * 3 + s,
+ * streamed-operand piece, weight piece, 16-channel K-step); the first n are written. */
+int mnb_pk_gc3_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out, int32_t n);
+int mnb_pk_gc3_conv(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
+                    const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, const uint8_t* bits8,
+                    float gain, float* out, int32_t* err_flag, mnb_stream_t stream);
+int mnb_pk_gc3_conv_codes(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
+                          const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, int32_t level_bound,
+                          int16_t* codes, float* dec, int32_t* err_flag, mnb_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * Bit-packed XNOR-popcount forward for wbwtab layers (mnb_xnor.cu): binary activations (WB:11-36, sign with 0 -> +1)

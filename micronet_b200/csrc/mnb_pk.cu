@@ -1776,6 +1776,318 @@ pk_wgrad_taps_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_const
   __syncthreads();
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// forward and data gradient of narrow grouped 3x3 convolutions with whole images as M tiles
+// ---------------------------------------------------------------------------------------------------------
+// pk_conv_kernel tiles these layers (16 / 32 channels per group) into 128-row M tiles of a few image rows: a 16 x 16 image
+// takes three row tiles (7 + 7 + 2 rows), an 8 x 8 image fills half of one, and every work item is 9..36 short MMAs followed
+// by an epilogue that both MMA warpgroups wait for.  Here a CTA owns GB consecutive groups for the whole launch (their
+// weight images stay in shared memory) and walks over image tiles: one stage = the zero-padded boxes of TB whole images
+// with the channels of all GB groups, the M tile = the image raster itself (ceil(rows / 64) m64 blocks, no row tiles).
+// The three MMA warpgroups take turns on the stages: while one runs its epilogue the others issue MMAs.  The
+// epilogue goes through a per-warpgroup staging tile [image][channel][position], so that the output of one (image, group)
+// - a contiguous NCHW run of ng * H * W elements - leaves in 16-byte stores.
+// Every output element sees the MMA chain of make_plan's plan for the same shape (taps, piece pairs, K-steps and their
+// order; one N tile of exactly the group's channels), so the result is bit for bit that of pk_conv_kernel (DESIGN.md 4.9).
+constexpr int kGc3MaxMb = 8;                       // m64 blocks per M tile
+constexpr int kGc3MaxProg = 128;                   // MMAs per accumulator chain
+constexpr int kGc3Cons = 3;                        // MMA + epilogue warpgroups
+constexpr int kGc3Threads = 128 * (1 + kGc3Cons);  // warpgroup 0: TMA (warp 0, lane 0), warpgroups 1 .. 3: MMA + epilogue
+constexpr int kGc3SmemBudget = 227 * 1024 - 4096;  // dynamic shared memory (the static part holds barriers and constants)
+// registers: 128 * 40 + 384 * 152 <= 65536; the accumulators of an M tile are (m64 blocks) x NT / 2 per thread
+constexpr int kGc3TmaRegs = 40, kGc3MmaRegs = 152;
+__host__ __device__ constexpr int gc3_max_mb(int nt) { return nt == 32 ? 6 : kGc3MaxMb; }
+
+struct Gc3Plan {
+  Plan pl;                  // make_plan's plan of the same (shape, mode, pieces): the chain and the weight image
+  int GB, nblk, TB, n_tiles, cpb, BW, THH, npos, nmb, plane, SP;
+  int a_box_bytes, a_piece_bytes, stage_bytes, nstage, w_bytes, stg_bytes, off_stage, off_stg, off_rowmap, smem_bytes;
+  int nprog;
+  uint32_t prog[kGc3MaxProg];               // A offset | B offset << 16 (16-byte units) of each MMA of the chain, in order
+  int16_t chain[kGc3MaxProg][4];            // (tap r * S + s, piece of A, piece of B, K-step) of each MMA (plan queries)
+};
+
+struct Gc3Params {
+  uint32_t prog[kGc3MaxProg];
+  int nprog, mode, TA, GB, ng, kg8, NOUT, B, TB, n_tiles, cpb, nmb, npos, BW, THH, OH, OW, plane, SP, C8O, wlo, hlo;
+  int a_box_bytes, a_piece_bytes, stage_bytes, nstage, w_bytes, img_bytes, stg_bytes, off_stage, off_stg, off_rowmap, smem_bytes;
+  const uint8_t* w_img;
+  const float* n_scale;
+  const float* a_scale;
+  float a_scale_const;
+  const float* bias;
+  const uint8_t* bits8;
+  float gain;
+  float* out;
+  int16_t* codes;
+  float* dec;
+  int* err;
+};
+
+static int make_gc3_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Gc3Plan& g) {
+  MNB_REQUIRE(s != nullptr, "conv shape is NULL");
+  MNB_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (forward) or 1 (data gradient)");
+  MNB_REQUIRE(TA >= 1 && TA <= 3 && TBk >= 1 && TBk <= 3, "term counts must be 1..3");
+  memset(&g, 0, sizeof(g));
+  auto no = [](const char* why) { return mnb_fail(MNB_E_UNSUPPORTED, "pk gc3: %s", why); };
+  const int C = s->in_c, K = s->out_c, G = s->groups;
+  MNB_REQUIRE(s->batch > 0 && C > 0 && K > 0 && s->in_h > 0 && s->in_w > 0 && G > 0 && C % G == 0 && K % G == 0,
+              "bad conv shape");
+  if (s->ker_h != 3 || s->ker_w != 3) return no("filter is not 3x3");
+  if (s->stride_h != 1 || s->stride_w != 1 || s->dil_h != 1 || s->dil_w != 1) return no("stride or dilation != 1");
+  if (s->pad_h < 0 || s->pad_w < 0 || s->pad_h > 2 || s->pad_w > 2) return no("padding outside 0..2");
+  if (C / G != 16 || K / G != 32 || G % 4) return no("needs 16 / 32 channels per group and groups % 4 == 0");
+  if (mode == 0 && (TA != 1 || TBk != 1)) return no("the forward takes one activation piece and one weight piece");
+  if (mode == 1 && (TA != 2 || TBk != 1)) return no("the data gradient takes two dy pieces and one weight piece");
+  Plan& p = g.pl;
+  if (int e = make_plan(s, mode, TA, TBk, p)) return e;
+  if (p.segmented || p.ny != 1 || p.nkph != 1 || p.n_ntiles != 1 || p.Nt != p.ng) return no("plan is segmented or tiled along N");
+  // raster: whole images, row pitch BW, TB images per M tile
+  g.BW = p.OWr + p.wlo + p.whi; g.THH = p.OHr + p.hlo + p.hhi; g.plane = p.OHr * p.OWr;
+  if (2 * g.BW > 256 || g.THH > 256) return no("image larger than one box");
+  g.SP = g.plane + ((4 - g.plane % 16) + 16) % 16;     // channel pitch of the staging tile: = 4 (mod 16), conflict-free writes
+  const int kg8 = p.kg / 8, img_bytes = p.img_bytes[0];
+  const int static_slack = 1024;
+  double best = -1;
+  for (int pass = 0; pass < 2 && best < 0; ++pass) {
+    // stages: a multiple of kGc3Cons, so that every ring slot belongs to ONE warpgroup (stage k -> slot k % nstage, warpgroup
+    // k % kGc3Cons).  A slot shared by two warpgroups would let the consumer of stage k + nstage wait on full[slot] while
+    // stage k's load is still in flight: the phase it waits for has the parity of the phase before stage k, the wait would
+    // pass at once, and its arrivals on empty[slot] would release stage k's slot early.  Within one warpgroup the waits on
+    // a slot are ordered, so a waiter is never more than one phase ahead.
+    const int min_st = pass == 0 ? 2 * kGc3Cons : kGc3Cons;
+    for (int tb = std::min(p.B, 16); tb >= 1; --tb) {
+      const int rows = (tb - 1) * g.THH * g.BW + (p.OHr - 1) * g.BW + p.OWr;
+      const int nmb = ceil_div(rows, 64);
+      if (nmb > gc3_max_mb(p.Nt)) continue;
+      const double eff = (double)tb * g.plane / (64.0 * nmb);
+      if (eff <= best + 1e-9) continue;
+      for (int gb = 4; gb >= 1; gb /= 2) {
+        if (G % gb) continue;
+        const int npos = tb * g.THH * g.BW;
+        const int box = gb * kg8 * npos * 16, piece = round_up(box, 128);
+        const int stage = round_up(TA * piece, 1024);
+        const int wb = round_up(gb * img_bytes, 1024);
+        const int stg = round_up(tb * p.ng * g.SP * 4, 128);
+        // MMAs of invalid rows read up to nmb * 64 + the largest tap offset rows past the start of the last octet
+        const int over = std::max(0, nmb * 64 + (p.hlo + p.hhi) * g.BW + p.wlo + p.whi - npos);
+        const int slack = round_up(over * 16 + 16, 1024);
+        const int rowmap = kGc3MaxMb * 64 * 4;
+        const int fixed = wb + slack + kGc3Cons * stg + rowmap + static_slack;
+        const int nst = std::min(MAXST, (kGc3SmemBudget - fixed) / stage) / kGc3Cons * kGc3Cons;
+        if (nst < min_st) continue;
+        best = eff;
+        g.TB = tb; g.nmb = nmb; g.npos = npos; g.GB = gb; g.a_box_bytes = box; g.a_piece_bytes = piece; g.stage_bytes = stage;
+        g.nstage = nst; g.w_bytes = gb * img_bytes; g.stg_bytes = stg;
+        g.off_stage = wb; g.off_stg = wb + nst * stage + slack; g.off_rowmap = g.off_stg + kGc3Cons * stg;
+        g.smem_bytes = g.off_rowmap + rowmap;
+        break;
+      }
+    }
+  }
+  if (best < 0) return no("no image tile fits the accumulators and shared memory");
+  if (g.npos * 16 >= (1 << 18) || g.stage_bytes * g.nstage + g.w_bytes > (1 << 18)) return no("descriptor range");
+  g.nblk = G / g.GB;
+  g.n_tiles = ceil_div(p.B, g.TB);
+  g.cpb = std::max(1, std::min(g.n_tiles, MNB_NUM_SMS / g.nblk));
+  // the chain of make_plan: stage templates -> K chunks -> piece pairs (small products first) -> taps -> K-steps, the issue
+  // order of pk_conv_kernel's program; A offsets for this raster, B offsets into the plan's weight image of one group
+  const int ph = s->pad_h, pw = s->pad_w;
+  const int b_tap16 = (p.CC / 8) * p.Nt, a_piece16 = g.a_piece_bytes >> 4;
+  g.nprog = 0;
+  for (int t = 0; t < p.ntmpl[0]; ++t) {
+    const Tmpl& tp = p.tmpl[0][t];
+    for (int cc = 0; cc < p.chunks; ++cc)
+      for (int pr = 0; pr < p.npairs; ++pr)
+        for (int i = 0; i < tp.ntap; ++i)
+          for (int j = 0; j < p.ksteps; ++j) {
+            if (g.nprog >= kGc3MaxProg) return no("MMA chain longer than 128");
+            const int r = p.tap_r[0][tp.tap0 + i], q = p.tap_s[0][tp.tap0 + i];
+            const int sh = mode == 0 ? r - ph : ph - r, sw = mode == 0 ? q - pw : pw - q;
+            const int ks = cc * p.ksteps + j;
+            const int a16 = (sh + p.hlo) * g.BW + (sw + p.wlo) + p.pair_a[pr] * a_piece16 + ks * 2 * g.npos;
+            const int b16 = (tp.blk_off + cc * tp.blk_bytes) / 16 + i * b_tap16 + p.pair_b[pr] * tp.ntap * b_tap16 + j * 2 * p.Nt;
+            if (a16 > 0xffff || b16 > 0xffff) return no("MMA offset overflow");
+            g.chain[g.nprog][0] = (int16_t)(r * 3 + q); g.chain[g.nprog][1] = (int16_t)p.pair_a[pr];
+            g.chain[g.nprog][2] = (int16_t)p.pair_b[pr]; g.chain[g.nprog][3] = (int16_t)ks;
+            g.prog[g.nprog++] = (uint32_t)a16 | ((uint32_t)b16 << 16);
+          }
+  }
+  return 0;
+}
+
+__device__ __forceinline__ void gc3_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// One output element of the epilogue, exactly as pk_conv_kernel's do_slot computes it (r: the accumulator).
+struct Gc3Out {
+  const Gc3Params& p;
+  const float* sc;
+  const float* bs;
+  __device__ __forceinline__ float f32(float r, int n, int b, int ch, int pos) const {
+    if (p.mode == 1 && p.bits8) {
+      const uint32_t m = __ldg(p.bits8 + ((int64_t)b * p.C8O + (ch >> 3)) * p.plane + pos);
+      return ((m >> (ch & 7)) & 1u) ? r * p.gain : 0.f;
+    }
+    return fmaf(r, sc[n], bs[n]);
+  }
+};
+
+template <int NT>
+__global__ void __launch_bounds__(kGc3Threads, 1)
+pk_gc3_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, const __grid_constant__ Gc3Params p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ uint64_t full[MAXST], empty[MAXST], wfull;
+  __shared__ uint32_t abort_flag;
+  __shared__ alignas(16) float s_scale[128], s_bias[128];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int blk = blockIdx.x / p.cpb, cta = blockIdx.x - blk * p.cpb;   // group block; CTA within the block
+  const int n_base = blk * p.GB * p.ng;                                 // first output channel of the block
+  int* rowmap = reinterpret_cast<int*>(smem + p.off_rowmap);
+  if (tid == 0) {
+    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&full[i], 1); tc::mbar_init(&empty[i], 4); }
+    tc::mbar_init(&wfull, 1);
+    abort_flag = 0;
+    tc::fence_barrier_init();
+    tc::prefetch_tmap(&tm0);
+    if (p.TA > 1) tc::prefetch_tmap(&tm1);
+  }
+  // rows behind the boxes that only invalid accumulator rows read must be finite
+  for (int i = tid; i < p.off_rowmap / 16; i += kGc3Threads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  // M row -> staging index image * ng * SP + position, or -1 for a halo / padding row
+  for (int m = tid; m < kGc3MaxMb * 64; m += kGc3Threads) {
+    const int img = p.THH * p.BW, tb = m / img, rem = m - tb * img, th = rem / p.BW, wc = rem - th * p.BW;
+    rowmap[m] = (tb < p.TB && th < p.OH && wc < p.OW) ? tb * p.ng * p.SP + th * p.OW + wc : -1;
+  }
+  {
+    const float a_sc = p.a_scale ? __ldg(p.a_scale) : p.a_scale_const;
+    for (int n = tid; n < p.GB * p.ng; n += kGc3Threads) {
+      const float scv = p.n_scale ? __fmul_rn(a_sc, __ldg(p.n_scale + n_base + n)) : a_sc;
+      const float bsv = p.bias ? __ldg(p.bias + n_base + n) : 0.f;
+      s_scale[n] = scv; s_bias[n] = bsv;
+      if (p.dec && cta == 0) { p.dec[n_base + n] = scv; p.dec[p.NOUT + n_base + n] = bsv; }
+    }
+  }
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGc3TmaRegs));
+    if (warp == 0 && lane == 0) {
+      tc::mbar_arrive_expect_tx(&wfull, (uint32_t)p.w_bytes);
+      tc::bulk_load_1d(smem, p.w_img + (size_t)blk * p.w_bytes, (uint32_t)p.w_bytes, &wfull);
+      const int c8 = blk * p.GB * p.kg8;
+      uint32_t slot = 0, ph = 0;
+      for (int t = cta; t < p.n_tiles; t += p.cpb) {
+        if (!tc::mbar_wait(&empty[slot], ph ^ 1u, p.err, 731)) break;
+        tc::mbar_arrive_expect_tx(&full[slot], (uint32_t)(p.TA * p.a_box_bytes));
+        uint8_t* sb = smem + p.off_stage + (size_t)slot * p.stage_bytes;
+        tc::tma_load_4d(sb, &tm0, &full[slot], -2 * p.wlo, -p.hlo, t * p.TB, c8);
+        if (p.TA > 1) tc::tma_load_4d(sb + p.a_piece_bytes, &tm1, &full[slot], -2 * p.wlo, -p.hlo, t * p.TB, c8);
+        if (++slot == (uint32_t)p.nstage) { slot = 0; ph ^= 1u; }
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kGc3MmaRegs));
+    constexpr int NR = NT / 2, MAXMB = gc3_max_mb(NT);
+    const int wg = (warp - 4) >> 2, w4 = (warp - 4) & 3, et = tid - 128 * (wg + 1);
+    float* stg = reinterpret_cast<float*>(smem + p.off_stg + (size_t)wg * p.stg_bytes);
+    const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), (uint32_t)p.npos * 16u, 128);
+    const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), (uint32_t)NT * 16u, 128);
+    const uint32_t a_lo0 = (uint32_t)a_desc0, b_lo0 = (uint32_t)b_desc0;
+    const uint64_t a_hi = a_desc0 & 0xffffffff00000000ull, b_hi = b_desc0 & 0xffffffff00000000ull;
+    const int fr = 16 * w4 + (lane >> 2), fc = 2 * (lane & 3);      // fragment row / column of d[0]
+    const FastDiv d_plane(p.plane);
+    tc::mbar_wait_soft(&wfull, 0, p.err, 733, &abort_flag);
+    // this warpgroup's stages: every kGc3Cons-th one of the CTA's sequence (k = wg, wg + kGc3Cons, ...)
+    for (int k = wg, t = cta + wg * p.cpb; t < p.n_tiles; k += kGc3Cons, t += kGc3Cons * p.cpb) {
+      const uint32_t slot = (uint32_t)k % (uint32_t)p.nstage, ph = ((uint32_t)k / (uint32_t)p.nstage) & 1u;
+      tc::mbar_wait_soft(&full[slot], ph, p.err, 732, &abort_flag);
+      const uint32_t s16 = (uint32_t)(p.off_stage + (int)slot * p.stage_bytes) >> 4;
+      for (int gl = 0; gl < p.GB; ++gl) {
+        float acc[MAXMB][NR];
+#pragma unroll
+        for (int mb = 0; mb < MAXMB; ++mb) tc::zero_acc(acc[mb]);
+        tc::wg_fence();
+#pragma unroll
+        for (int mb = 0; mb < MAXMB; ++mb) tc::fence_acc(acc[mb]);
+        const uint32_t a_base = a_lo0 + s16 + (uint32_t)(gl * p.kg8 * p.npos), b_base = b_lo0 + (uint32_t)((gl * p.img_bytes) >> 4);
+#pragma unroll
+        for (int mb = 0; mb < MAXMB; ++mb) {
+          if (mb >= p.nmb) break;
+          for (int e = 0; e < p.nprog; ++e) {
+            const uint32_t w = p.prog[e];
+            tc::Mma<NT>::template bf16<0, 0>(acc[mb], a_hi | (uint64_t)(a_base + 64u * mb + (w & 0xffffu)),
+                                              b_hi | (uint64_t)(b_base + (w >> 16)), 1);
+          }
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+#pragma unroll
+        for (int mb = 0; mb < MAXMB; ++mb) tc::fence_acc(acc[mb]);
+        if (gl == p.GB - 1) {   // this warp's reads of the stage are done
+          __syncwarp();
+          if (lane == 0) tc::mbar_arrive(&empty[slot]);
+        }
+        gc3_bar(1 + wg);        // the previous copy-out is done with the staging tile
+#pragma unroll
+        for (int mb = 0; mb < MAXMB; ++mb) {
+          if (mb >= p.nmb) break;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int dst = rowmap[64 * mb + fr + 8 * i];
+            if (dst < 0) continue;
+#pragma unroll
+            for (int j = 0; j < NR / 4; ++j) {
+              stg[dst + (8 * j + fc) * p.SP] = acc[mb][4 * j + 2 * i];
+              stg[dst + (8 * j + fc + 1) * p.SP] = acc[mb][4 * j + 2 * i + 1];
+            }
+          }
+        }
+        gc3_bar(1 + wg);
+        // copy-out: image b of the tile, channels ch0 .. ch0 + ng: one contiguous NCHW run of ng * plane elements
+        const int ch0 = n_base + gl * p.ng, E = p.ng * p.plane;
+        const float* sc = s_scale + gl * p.ng;
+        const float* bs = s_bias + gl * p.ng;
+        const Gc3Out og{p, sc, bs};
+        for (int tb = 0; tb < p.TB; ++tb) {
+          const int b = t * p.TB + tb;
+          if (b >= p.B) break;
+          const float* src = stg + tb * p.ng * p.SP;
+          if (p.codes) {
+            uint4* dst = reinterpret_cast<uint4*>(p.codes + ((int64_t)b * p.NOUT + ch0) * p.plane);
+            for (int v = et; v < E / 8; v += 128) {
+              uint32_t n, pos;
+              d_plane.divmod((uint32_t)(8 * v), n, pos);
+              uint32_t wv[4];
+#pragma unroll
+              for (int i = 0; i < 8; ++i) {
+                const uint32_t c = (uint32_t)(int16_t)__float2int_rn(src[n * p.SP + pos]) & 0xffffu;
+                wv[i >> 1] = (i & 1) ? (wv[i >> 1] | (c << 16)) : c;
+                if (++pos == (uint32_t)p.plane) { pos = 0; ++n; }
+              }
+              dst[v] = make_uint4(wv[0], wv[1], wv[2], wv[3]);
+            }
+          } else {
+            float4* dst = reinterpret_cast<float4*>(p.out + ((int64_t)b * p.NOUT + ch0) * p.plane);
+            for (int v = et; v < E / 4; v += 128) {
+              uint32_t n, pos;
+              d_plane.divmod((uint32_t)(4 * v), n, pos);
+              float r[4];
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                r[i] = og.f32(src[n * p.SP + pos], (int)n, b, ch0 + (int)n, (int)pos);
+                if (++pos == (uint32_t)p.plane) { pos = 0; ++n; }
+              }
+              dst[v] = make_float4(r[0], r[1], r[2], r[3]);
+            }
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();
+}
+
 }  // namespace pk
 
 // =========================================================================================================
@@ -2425,4 +2737,83 @@ extern "C" int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int
                                           kdiv, dw);
   MNB_LAUNCHED(2);
   return 0;
+}
+
+// ---- forward and data gradient of narrow grouped 3x3 convolutions (pk_gc3_kernel)
+
+// host only: out[0..9] = {groups per CTA block, images per M tile, m64 blocks per M tile, stages, shared-memory bytes, CTAs,
+// image tiles, MMAs per accumulator chain, N tile, MMA warpgroups}, then 4 values per MMA of the chain in issue order:
+// (filter tap r * 3 + s, piece of the streamed operand, piece of the weights, 16-channel K-step); the first n are written
+extern "C" int mnb_pk_gc3_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out, int32_t n) {
+  static pk::Gc3Plan g;   // large POD (single host thread per process)
+  if (int e = pk::make_gc3_plan(s, mode, terms_a, terms_w, g)) return e;
+  if (out) {
+    const int v[10] = {g.GB, g.TB, g.nmb, g.nstage, g.smem_bytes, g.nblk * g.cpb, g.n_tiles, g.nprog, g.pl.Nt, pk::kGc3Cons};
+    for (int i = 0; i < std::min(n, 10); ++i) out[i] = v[i];
+    for (int i = 10; i < n && (i - 10) / 4 < g.nprog; ++i) out[i] = g.chain[(i - 10) / 4][(i - 10) % 4];
+  }
+  return 0;
+}
+
+static int pk_gc3_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
+                       const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, const uint8_t* bits8,
+                       float gain, float* out, int16_t* codes, float* dec, int32_t* err_flag, mnb_stream_t stream) {
+  using namespace pk;
+  MNB_REQUIRE(s && a_pk && w_img && (out != nullptr) != (codes != nullptr) && err_flag, "NULL pk_gc3 pointer");
+  static Gc3Plan g;
+  if (int e = make_gc3_plan(s, mode, terms_a, terms_w, g)) return e;
+  MNB_REQUIRE(g.nstage % kGc3Cons == 0, "pk gc3: %d stages are not a whole number per MMA warpgroup", g.nstage);
+  const Plan& pl = g.pl;
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (!al16(a_pk) || !al16(w_img) || !al16(out ? (const void*)out : (const void*)codes))
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk gc3: operands and output must be 16-byte aligned");
+  static Gc3Params p;
+  memset(&p, 0, sizeof(p));
+  for (int i = 0; i < g.nprog; ++i) p.prog[i] = g.prog[i];
+  p.nprog = g.nprog; p.mode = mode; p.TA = terms_a; p.GB = g.GB; p.ng = pl.ng; p.kg8 = pl.kg / 8; p.NOUT = pl.NOUT; p.B = pl.B;
+  p.TB = g.TB; p.n_tiles = g.n_tiles; p.cpb = g.cpb; p.nmb = g.nmb; p.npos = g.npos; p.BW = g.BW; p.THH = g.THH; p.OH = pl.OHr;
+  p.OW = pl.OWr; p.plane = g.plane; p.SP = g.SP; p.C8O = ceil_div(pl.NOUT, 8); p.wlo = pl.wlo; p.hlo = pl.hlo;
+  p.a_box_bytes = g.a_box_bytes; p.a_piece_bytes = g.a_piece_bytes; p.stage_bytes = g.stage_bytes; p.nstage = g.nstage;
+  p.w_bytes = g.w_bytes; p.img_bytes = pl.img_bytes[0]; p.stg_bytes = g.stg_bytes; p.off_stage = g.off_stage; p.off_stg = g.off_stg;
+  p.off_rowmap = g.off_rowmap; p.smem_bytes = g.smem_bytes;
+  p.w_img = reinterpret_cast<const uint8_t*>(w_img);
+  p.n_scale = n_scale; p.a_scale = a_scale; p.a_scale_const = a_scale_const; p.bias = bias; p.bits8 = mode == 1 ? bits8 : nullptr;
+  p.gain = gain; p.out = out; p.codes = codes; p.dec = dec; p.err = err_flag;
+  CUtensorMap tm[2];
+  const int64_t plane_bytes = (int64_t)pl.B * pl.C8A * pl.HA * pl.WA * 16;
+  for (int t = 0; t < 2; ++t)
+    if (int e = make_pk_tmap(&tm[t], a_pk, plane_bytes, t < terms_a ? t : 0, pl.B, pl.C8A, pl.HA, pl.WA, g.BW, g.THH, g.TB,
+                             g.GB * p.kg8))
+      return e;
+  auto fn = pl.Nt == 32 ? pk_gc3_kernel<32> : pk_gc3_kernel<16>;
+  if (pl.Nt != 16 && pl.Nt != 32) return mnb_fail(MNB_E_ARG, "pk gc3: plan with Nt %d", pl.Nt);
+  if (int e = set_max_smem(fn, kGc3SmemBudget)) return e;
+  fn<<<g.nblk * g.cpb, kGc3Threads, g.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], p);
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+// mnb_pk_conv (mode 0: fp32 forward, mode 1: data gradient) for the shapes of mnb_pk_gc3_plan's cover: the same operands, weight
+// image and epilogue arguments, the same result bit for bit
+extern "C" int mnb_pk_gc3_conv(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
+                               int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
+                               const float* bias, const uint8_t* bits8, float gain, float* out, int32_t* err_flag,
+                               mnb_stream_t stream) {
+  MNB_REQUIRE(out, "NULL pk_gc3_conv output");
+  return pk_gc3_impl(s, mode, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, bits8, gain, out, nullptr,
+                     nullptr, err_flag, stream);
+}
+
+// mnb_pk_conv_codes for the forward shapes of mnb_pk_gc3_plan's cover: the same codes and decode pair
+extern "C" int mnb_pk_gc3_conv_codes(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img,
+                                     int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
+                                     const float* bias, int32_t level_bound, int16_t* codes, float* dec, int32_t* err_flag,
+                                     mnb_stream_t stream) {
+  MNB_REQUIRE(s && codes && dec, "NULL pk_gc3_conv_codes pointer");
+  MNB_REQUIRE(level_bound >= 1 && s->groups >= 1, "pk_gc3_conv_codes: level bound %d", level_bound);
+  if ((int64_t)(s->in_c / s->groups) * s->ker_h * s->ker_w * level_bound > 32767)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_gc3_conv_codes: sums of %d x %d x %d terms of level %d may exceed int16",
+                    s->in_c / s->groups, s->ker_h, s->ker_w, level_bound);
+  return pk_gc3_impl(s, 0, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, nullptr, codes, dec,
+                     err_flag, stream);
 }

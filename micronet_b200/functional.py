@@ -371,14 +371,24 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, need_dx, prepacke
     if codes_out and w_int is not None and ta == 1 and tw == 1:
         codes = torch.empty(y.shape, dtype=torch.int16, device=y.device)
         dec = torch.empty(2 * y.shape[1], dtype=torch.float32, device=y.device)
-        rc = _timed("fwd_pk", sh, lambda: PK.conv_codes(sh, x_pk, w_img, codes, dec, n_scale=w_scale, a_scale=a_scale,
-                                                        a_scale_const=a_const, bias=bias))
+        # narrow grouped 3x3 layers: whole images as M tiles (same kernel-table kind, the same codes); whatever that kernel
+        # refuses goes to mnb_pk_conv_codes
+        fns = ([PK.gc3_conv_codes] if L.PK_GC3 and PK.gc3_plan(sh, 0, 1, 1) is not None else []) + [PK.conv_codes]
+        for fn in fns:
+            rc = _timed("fwd_pk", sh, lambda fn=fn: fn(sh, x_pk, w_img, codes, dec, n_scale=w_scale, a_scale=a_scale,
+                                                       a_scale_const=a_const, bias=bias))
+            if rc != L.E_UNSUPPORTED:
+                break
         if rc == 0:
             y._mnb_codes = (codes, dec)
     if rc == L.E_UNSUPPORTED:
-        rc = _timed("fwd_pk", sh, lambda: PK.conv(sh, 0, x_pk, ta, w_img, tw, y,
-                                                  n_scale=w_scale if w_int is not None else None,
-                                                  a_scale=a_scale, a_scale_const=a_const, bias=bias))
+        fns = ([PK.gc3_conv] if L.PK_GC3 and PK.gc3_plan(sh, 0, ta, tw) is not None else []) + [PK.conv]
+        for fn in fns:
+            rc = _timed("fwd_pk", sh, lambda fn=fn: fn(sh, 0, x_pk, ta, w_img, tw, y,
+                                                       n_scale=w_scale if w_int is not None else None,
+                                                       a_scale=a_scale, a_scale_const=a_const, bias=bias))
+            if rc != L.E_UNSUPPORTED:
+                break
     if rc == L.E_UNSUPPORTED:
         return False
     L.check(rc, "pk_conv fwd")
@@ -413,8 +423,13 @@ def _pk_backward(ctx, dy):
         gain = 0.1 if (spec is not None and spec.mode == L.ACT_DOREFA) else 1.0
         # a fused producer applies the STE mask itself (it owns the mask bits): plain data gradient times the quantizer's gain
         plain_gain = gain if ctx.pk_prepacked else 1.0
-        L.check(_timed("dgrad_pk", sh, lambda: PK.conv(sh, 1, dy_pk, T, w_img, tw, dx, bits8=ctx.pk_bits8, gain=gain,
-                                                       a_scale_const=plain_gain)), "pk_conv dgrad")
+        fns = ([PK.gc3_conv] if L.PK_GC3 and PK.gc3_plan(sh, 1, T, tw) is not None else []) + [PK.conv]
+        for fn in fns:   # whatever mnb_pk_gc3_conv refuses goes to mnb_pk_conv
+            rc = _timed("dgrad_pk", sh, lambda fn=fn: fn(sh, 1, dy_pk, T, w_img, tw, dx, bits8=ctx.pk_bits8, gain=gain,
+                                                         a_scale_const=plain_gain))
+            if rc != L.E_UNSUPPORTED:
+                break
+        L.check(rc, "pk_conv dgrad")
     if need_dw:
         dwq = torch.empty_like(ctx.wq)
         a_scale = None

@@ -8,6 +8,7 @@ shared memory, stride 2, 5x5 filters, 4x4 or 224x224 images ...) and every fused
     conv        TMA -> wgmma (register accumulators) -> epilogue (forward: scale + bias; data gradient: STE mask)
     wgrad       the same boxes read as MN-major operands, split over the batch, deterministic reduction
     wgrad_taps  wgrad of narrow grouped 3x3 layers with all nine taps of a CTA in registers
+    gc3_conv    forward / data gradient of the same layers with whole images as M tiles (same result as conv)
 
 Reference math: F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen's
 convolution_backward."""
@@ -216,3 +217,35 @@ def wgrad_taps(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
     ws = torch.empty(plan["scratch_bytes"], dtype=torch.uint8, device=dw.device)
     return L.load().mnb_pk_wgrad_taps(C.byref(sh), dy_pk.data_ptr(), terms_dy, x_pk.data_ptr(), terms_x, L.ptr(a_scale),
                                       L.ptr(kdiv), dw.data_ptr(), ws.data_ptr(), L.tc_err_flag(dw.device).data_ptr(), L.stream())
+
+
+def gc3_plan(sh, mode, terms_a, terms_w):
+    """plan of mnb_pk_gc3_conv as a dict, None outside its cover (host-only plan query, cached).  ``chain``: the MMAs of
+    one accumulator in issue order as (filter tap r * 3 + s, streamed-operand piece, weight piece, 16-channel K-step)"""
+    k = ("g3", _key(sh), mode, terms_a, terms_w)
+    if k not in _plan_cache:
+        out = (C.c_int32 * (10 + 4 * 128))()
+        ok = L.load().mnb_pk_gc3_plan(C.byref(sh), mode, terms_a, terms_w, out, len(out)) == 0
+        plan = None
+        if ok:
+            names = ("groups_per_block", "images_per_tile", "m_blocks", "nstage", "smem_bytes", "ctas", "tiles", "chain_len",
+                     "Nt", "mma_warpgroups")
+            plan = dict(zip(names, out[:10]))
+            plan["chain"] = [tuple(out[10 + 4 * i:14 + 4 * i]) for i in range(plan["chain_len"])]
+        _plan_cache[k] = plan
+    return _plan_cache[k]
+
+
+def gc3_conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, n_scale=None, a_scale=None, a_scale_const=1.0, bias=None,
+             bits8=None, gain=1.0):
+    """mnb_pk_gc3_conv: same arguments as conv and the same result bit for bit; returns the C status"""
+    return L.load().mnb_pk_gc3_conv(C.byref(sh), mode, a_pk.data_ptr(), terms_a, w_img.data_ptr(), terms_w, L.ptr(n_scale),
+                                    L.ptr(a_scale), float(a_scale_const), L.ptr(bias), L.ptr(bits8), float(gain),
+                                    out.data_ptr(), L.tc_err_flag(out.device).data_ptr(), L.stream())
+
+
+def gc3_conv_codes(sh, a_pk, w_img, codes, dec, n_scale=None, a_scale=None, a_scale_const=1.0, bias=None, level_bound=1):
+    """mnb_pk_gc3_conv_codes: same arguments as conv_codes and the same codes and decode pair; returns the C status"""
+    return L.load().mnb_pk_gc3_conv_codes(C.byref(sh), a_pk.data_ptr(), 1, w_img.data_ptr(), 1, L.ptr(n_scale), L.ptr(a_scale),
+                                          float(a_scale_const), L.ptr(bias), int(level_bound), codes.data_ptr(), dec.data_ptr(),
+                                          L.tc_err_flag(codes.device).data_ptr(), L.stream())
