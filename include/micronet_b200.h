@@ -486,6 +486,21 @@ int mnb_bn_relu_quant_pack_i8_fwd(const float* x, int32_t batch, int32_t channel
                                   int32_t out_shuffle_groups, void* x_packed, mnb_stream_t stream);
 int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s, int32_t p,
                          int32_t int8, void* out_pk, mnb_stream_t stream);
+/* Frozen IAO inference graphs of NIN / NIN-GC (nin.py:51/55, nin_gc.py:88/119): the pool between two conv-bn-relu blocks is a
+ * QuantMaxPool2d (IAO:1285-1343) with a quantizer of its own, so the producer's epilogue writes the POOL quantizer's levels
+ * L and the next conv quantizes the pooled values again.  Both maps are exact functions of L: the pool writes
+ * v = fl((L + zp_p) * s_p) (ActQuantFn), and the consumer's level of v is monotone non-decreasing in L (s_p > 0), so
+ * Q_c(maxpool(Q_p(relu(y)))) == T[maxpool(L)] with a 256-entry table T.
+ *   mnb_pk_plane_maxpool_requant : mnb_pk_plane_maxpool of a plane of the pool quantizer's levels (same layouts, same cover,
+ *                                  int8 in -> int8 out, bf16 in -> bf16 out), each window max written through T as the
+ *                                  consumer's plane.  Every CTA builds T in shared memory from the device scalars with the
+ *                                  fp32 op sequence of the engine's IAO quantizer (__fdiv_rn, round half away, clamp), so
+ *                                  the result is the consumer's pack_act of max_pool2d(ActQuantFn(x)) bit for bit.  Both
+ *                                  quantizers must be IAO with q_type 0 and 2..8 bits (zero_point 0, levels in
+ *                                  [-128, 127]); anything else returns MNB_E_UNSUPPORTED before launching. */
+int mnb_pk_plane_maxpool_requant(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s,
+                                 int32_t p, int32_t int8, const mnb_act_qparams* q_in, const mnb_act_qparams* q_out, void* out_pk,
+                                 mnb_stream_t stream);
 int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x);
 int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                  const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);

@@ -131,6 +131,7 @@ PROTOTYPES = {
     "mnb_quant_add_pack_i8_fwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _ACTQ, _I, _P, C.POINTER(PkPost), _P]),
     "mnb_bn_relu_quant_pack_i8_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _ACTQ, _I, _P, _P]),
     "mnb_pk_plane_maxpool": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "mnb_pk_plane_maxpool_requant": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _ACTQ, _ACTQ, _P, _P]),
     "mnb_pk_wgrad_scratch_bytes": (_L, [_SHAPE, _I, _I]),
     "mnb_pk_wgrad": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_pk_wgrad_taps_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),

@@ -523,12 +523,33 @@ __global__ void __launch_bounds__(256) bn_relu_quant_pack_i8_kernel(const float*
   }
 }
 
+// The requantizing table of an IAO max-pool (mnb_pk_plane_maxpool_requant), one entry per stored level P in [-128, 127]
+// (entry P + 128): the pool quantizer's dequantized value v = fl((P + zp_in) * s_in), exactly what ActQuantFn writes
+// (act_quant_fwd_kernel), requantized by the consumer's quantizer with the exact op sequence of mnb_act_quantize_one
+// (__fdiv_rn, mnb_round_half_away, clamp) and stored as the consumer's plane value fl(level + zp_out): bf16 bits, or the
+// s8 byte in the low 8 bits.  Symmetric quantizers have zero_point 0, so P is the pool quantizer's level itself.
+template <bool I8>
+__device__ __forceinline__ void build_requant_table(const mnb_act_qparams& qin, const mnb_act_qparams& qout, uint16_t* tab) {
+  const MnbActQ a = mnb_load_actq(qin), b = mnb_load_actq(qout);
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+    const float lev = (float)min(max(i - 128, a.qmin), a.qmax);
+    const float v = __fmul_rn(__fadd_rn(lev, a.zp), a.s);
+    bool pass;
+    float xq;
+    const float o = __fadd_rn((float)(mnb_act_quantize_one(b, v, pass, xq) + b.qmin), b.zp);
+    if constexpr (I8) tab[i] = (uint16_t)((uint32_t)__float2int_rn(o) & 0xffu);
+    else tab[i] = __bfloat16_as_ushort(__float2bfloat16_rn(o));
+  }
+}
+
 // window max of a level plane [b][unit][H][W][16 B] (bf16 or s8 levels), unit by unit, padding skipped: the plane of
 // max_pool2d(k, s, p) of the decoded activations, because every quantizer whose levels a plane holds is monotone
-// non-decreasing.  One thread = one output position of one unit.
-template <bool I8>
-__global__ void __launch_bounds__(256) plane_maxpool_kernel(const uint4* __restrict__ in, int64_t planes, int H, int W, int k,
-                                                            int s, int pad, int OH, int OW, uint4* __restrict__ out) {
+// non-decreasing.  One thread = one output position of one unit.  REQ: the window max goes out through the requantizing
+// table ``tab`` of an IAO pool quantizer -> consumer quantizer pair (build_requant_table; monotone as well, so it commutes
+// with the max).
+template <bool I8, bool REQ>
+__device__ __forceinline__ void plane_maxpool_body(const uint4* __restrict__ in, int64_t planes, int H, int W, int k, int s,
+                                                   int pad, int OH, int OW, uint4* __restrict__ out, const uint16_t* tab) {
   const int64_t total = planes * OH * OW;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int ow = (int)(idx % OW);
@@ -556,8 +577,44 @@ __global__ void __launch_bounds__(256) plane_maxpool_kernel(const uint4* __restr
           }
         }
       }
+    if constexpr (REQ) {
+      uint32_t* mm = reinterpret_cast<uint32_t*>(&m);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const uint32_t v = mm[e];
+        if constexpr (I8) {      // s8 level + 128 == its byte with the sign bit flipped
+          const uint32_t x = v ^ 0x80808080u;
+          mm[e] = (uint32_t)tab[x & 0xffu] | ((uint32_t)tab[(x >> 8) & 0xffu] << 8) |
+                  ((uint32_t)tab[(x >> 16) & 0xffu] << 16) | ((uint32_t)tab[x >> 24] << 24);
+        } else {                 // bf16 holding an integer level in [-128, 127]
+          const int lo = min(max(__float2int_rz(__uint_as_float(v << 16)) + 128, 0), 255);
+          const int hi = min(max(__float2int_rz(__uint_as_float(v & 0xffff0000u)) + 128, 0), 255);
+          mm[e] = (uint32_t)tab[lo] | ((uint32_t)tab[hi] << 16);
+        }
+      }
+    }
     out[idx] = m;
   }
+}
+
+template <bool I8>
+__global__ void __launch_bounds__(256) plane_maxpool_kernel(const uint4* __restrict__ in, int64_t planes, int H, int W, int k,
+                                                            int s, int pad, int OH, int OW, uint4* __restrict__ out) {
+  plane_maxpool_body<I8, false>(in, planes, H, W, k, s, pad, OH, OW, out, nullptr);
+}
+
+// the IAO pool (IAO:1285-1343) between two frozen convs: table built once per CTA, then the window max through it
+template <bool I8>
+__global__ void __launch_bounds__(256) plane_maxpool_requant_kernel(const uint4* __restrict__ in, int64_t planes, int H, int W,
+                                                                    int k, int s, int pad, int OH, int OW,
+                                                                    uint4* __restrict__ out, mnb_act_qparams qin,
+                                                                    mnb_act_qparams qout) {
+  // 512 bytes, the kernel's only shared memory.  ptxas reports 1024: this file's dynamic shared array (pk::smem) is aligned
+  // to 1024 bytes, so every kernel's static shared memory is rounded up to that alignment.
+  __shared__ uint16_t tab[256];
+  build_requant_table<I8>(qin, qout, tab);
+  __syncthreads();
+  plane_maxpool_body<I8, true>(in, planes, H, W, k, s, pad, OH, OW, out, tab);
 }
 
 // IAO QuantAdd of a frozen inference graph + the consuming conv's quantizer and operand packing in one pass (see
@@ -2326,8 +2383,10 @@ extern "C" int mnb_bn_relu_quant_pack_i8_fwd(const float* x, int32_t batch, int3
   return 0;
 }
 
-extern "C" int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
-                                    int32_t s, int32_t p, int32_t int8, void* out_pk, mnb_stream_t stream) {
+// mnb_pk_plane_maxpool (q_in == NULL) and mnb_pk_plane_maxpool_requant: same cover, same grid
+static int plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s,
+                         int32_t p, int32_t int8, const mnb_act_qparams* q_in, const mnb_act_qparams* q_out, void* out_pk,
+                         mnb_stream_t stream) {
   MNB_REQUIRE(in_pk && out_pk && in_pk != out_pk, "NULL or aliased pk_plane_maxpool pointer");
   MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad pk_plane_maxpool shape");
   MNB_REQUIRE(((reinterpret_cast<uintptr_t>(in_pk) | reinterpret_cast<uintptr_t>(out_pk)) & 15) == 0,
@@ -2335,15 +2394,42 @@ extern "C" int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t ch
   if (k < 1 || s < 1 || p < 0 || 2 * p > k || h + 2 * p < k || w + 2 * p < k)
     return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool: kernel %d, stride %d, padding %d on %d x %d (needs 2 * p <= k)", k, s,
                     p, h, w);
+  if (q_in) {
+    for (const mnb_act_qparams* q : {q_in, q_out})
+      if (q->mode != MNB_ACT_IAO || q->q_type != 0 || q->bits < 2 || q->bits > 8 || q->qmin < -128 || q->qmax > 127)
+        return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool_requant: both quantizers must be symmetric IAO (q_type 0) with "
+                                           "2..8 bits and levels in [-128, 127]");
+    MNB_REQUIRE(q_in->scale && q_in->zero_point && q_in->obs_min && q_in->obs_max && q_out->scale && q_out->zero_point &&
+                    q_out->obs_min && q_out->obs_max,
+                "NULL IAO quantizer scalar");
+  }
   const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
   const int64_t planes = (int64_t)batch * ((channels + (int8 ? 15 : 7)) / (int8 ? 16 : 8));
   const int64_t total = planes * oh * ow;
   const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 16);
-  auto kern = int8 ? pk::plane_maxpool_kernel<true> : pk::plane_maxpool_kernel<false>;
-  kern<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint4*>(in_pk), planes, h, w, k, s, p, oh, ow,
-                                                 reinterpret_cast<uint4*>(out_pk));
+  const uint4* src = reinterpret_cast<const uint4*>(in_pk);
+  uint4* dst = reinterpret_cast<uint4*>(out_pk);
+  if (q_in) {
+    auto kern = int8 ? pk::plane_maxpool_requant_kernel<true> : pk::plane_maxpool_requant_kernel<false>;
+    kern<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, planes, h, w, k, s, p, oh, ow, dst, *q_in, *q_out);
+  } else {
+    auto kern = int8 ? pk::plane_maxpool_kernel<true> : pk::plane_maxpool_kernel<false>;
+    kern<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, planes, h, w, k, s, p, oh, ow, dst);
+  }
   MNB_LAUNCHED(1);
   return 0;
+}
+
+extern "C" int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
+                                    int32_t s, int32_t p, int32_t int8, void* out_pk, mnb_stream_t stream) {
+  return plane_maxpool(in_pk, batch, channels, h, w, k, s, p, int8, nullptr, nullptr, out_pk, stream);
+}
+
+extern "C" int mnb_pk_plane_maxpool_requant(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
+                                            int32_t s, int32_t p, int32_t int8, const mnb_act_qparams* q_in,
+                                            const mnb_act_qparams* q_out, void* out_pk, mnb_stream_t stream) {
+  MNB_REQUIRE(q_in && q_out, "NULL pk_plane_maxpool_requant quantizer");
+  return plane_maxpool(in_pk, batch, channels, h, w, k, s, p, int8, q_in, q_out, out_pk, stream);
 }
 
 // host only: out[0..15] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator

@@ -11,6 +11,7 @@ import copy
 import torch.nn as nn
 
 from . import _lib as L
+from . import frozen_graph as FG
 from . import functional as F_
 
 
@@ -219,18 +220,12 @@ def _frozen_operands(conv):
     return fr[1:]
 
 
-def _shuffle(x, groups):
-    b, c = x.shape[0], x.shape[1]
-    return x.view(b, groups, c // groups, *x.shape[2:]).transpose(1, 2).contiguous().view(x.shape)
-
-
-class _Link:
-    """a producer -> consumer hand-off of a frozen graph: the consumer conv, the eval BatchNorm and ReLU the producer applies,
-    the consumer block's channel shuffle and the max-pool in between, which runs on the level plane"""
+class _Link(FG.Link):
+    """frozen_graph.Link whose producer applies the eval BatchNorm (running statistics) before the ReLU and the consumer's
+    DoReFa quantizer; a max-pool in between runs as mnb_pk_plane_maxpool"""
 
     def __init__(self, cconv, bn, relu, sg, pool):
-        self.cconv, self.bn, self.relu, self.sg, self.pool = cconv, bn, relu, sg, pool
-        self.target = pool[0] if pool is not None else cconv
+        super().__init__(cconv, bn, relu, sg, pool)
         self._invstd = None
 
     def consumer(self):
@@ -259,38 +254,16 @@ def _frozen_conv_forward(conv, x):
         x = F_.materialized(x)
         sg = conv.__dict__.get("_mnb_in_shuffle", 1)
         if sg > 1:
-            x = _shuffle(x, sg)       # the block's channel shuffle that freeze_inference moved into the producer
+            x = FG.shuffle(x, sg)     # the block's channel shuffle that freeze_inference moved into the producer
     info = conv.__dict__["_mnb_frozen"]
     link = info.get("link")
     return F_.frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, conv.stride, conv.padding, conv.dilation, conv.groups,
                           consumer=link.consumer() if link is not None else None, int8=info["int8"])
 
 
-def _absorbed_forward(m, target, x):
-    """BatchNorm / ReLU whose work a producer did for ``target``: pass its tagged output through, run as usual otherwise"""
-    pre = getattr(x, "_mnb_pk_pre", None)
-    if pre is not None and pre[0] is target:
-        _check_eval(m)
-        return x
-    return type(m).forward(m, x)
-
-
-def _pool_forward(pool, link, x):
-    """the max-pool between a producer and its consumer: mnb_pk_plane_maxpool on the producer's level plane"""
-    import torch
+def _plane_pool(plane, b, c, h, w, k, s, p, int8):
     from . import pk as PK
-    plane = F_.handed_plane(pool, x)
-    if plane is None:
-        return type(pool).forward(pool, x)
-    _check_eval(pool)
-    _, k, s, p = link.pool
-    b, c, h, w = x.shape
-    fmt = x._mnb_pk_pre[3]
-    out = F_._timed("plane_pool", L.ConvShape(b, c, h, w, c, k, k, s, s, p, p, 1, 1, 1),
-                    lambda: PK.plane_maxpool(plane, b, c, h, w, k, s, p, int8=fmt == "i8"))
-    y = torch.empty((b, c, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1), dtype=torch.float32, device="meta")
-    y._mnb_pk_pre = (link.cconv, out, y._version, fmt)
-    return y
+    return PK.plane_maxpool(plane, b, c, h, w, k, s, p, int8=int8)
 
 
 def _stem_forward(bn, link, x):
@@ -329,25 +302,18 @@ def _stem_forward(bn, link, x):
 def _conv_bn_act(blk):
     """(conv, BatchNorm, nn.ReLU or None, relu applied?) of one of the reference's conv-bn-relu blocks, else None"""
     from .fused import BatchNormReluQuant2d
-    if not hasattr(blk, "channel_shuffle_flag"):
+    bp = FG.block_parts(blk)
+    if bp is None or len(bp[1]) not in (1, 2):
         return None
-    parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
-    if len(parts) not in (2, 3) or not isinstance(parts[0], nn.Conv2d):
-        return None
-    bn, act = parts[1], (parts[2] if len(parts) == 3 else None)
+    bn, act = bp[1][0], (bp[1][1] if len(bp[1]) == 2 else None)
     if type(bn) not in (nn.BatchNorm2d, BatchNormReluQuant2d) or not (bn.affine and bn.track_running_stats):
         return None
     if act is not None and (type(act) is not nn.ReLU or isinstance(bn, BatchNormReluQuant2d)):
         return None
-    return parts[0], bn, act, act is not None or isinstance(bn, BatchNormReluQuant2d)
+    return bp[0], bn, act, act is not None or isinstance(bn, BatchNormReluQuant2d)
 
 
-def _undo(model):
-    for rec in reversed(model.__dict__.pop("_mnb_dorefa_undo", [])):
-        if rec[0] == "attr":
-            setattr(rec[1], rec[2], rec[3])
-        else:
-            rec[1].__dict__.pop(rec[2], None)
+_UNDO = "_mnb_dorefa_undo"
 
 
 def freeze_inference(model, enable=True, int8=False):
@@ -371,60 +337,41 @@ def freeze_inference(model, enable=True, int8=False):
     absorbed modules run as usual.  Numerics (DESIGN.md 4.15): the levels equal the fused BatchNormReluQuant2d's bit for bit;
     where the un-frozen graph ran ATen's BatchNorm a level on a rounding boundary may differ by one.  Parameters, buffers
     and state_dict keys are unchanged; ``enable=False`` restores the modules (needed before training)."""
-    import functools
     from .fused import EngineFloatConv2d, EngineMaxPool2d, _pool_cfg
-    _undo(model)
+    FG.undo(model, _UNDO)
     if not enable:
         return model
-    undo = model.__dict__.setdefault("_mnb_dorefa_undo", [])
+    rw = FG.Rewrite(model, _UNDO)
     frozen = set()
     for m in model.modules():
         if isinstance(m, QuantConv2d) and not m.training and _freezable(m):
             small = m.activation_quantizer.a_bits <= 7 and m.weight_quantizer.w_bits <= 7
             m.__dict__["_mnb_frozen"] = {"int8": bool(int8) and small, "link": None}
-            undo += [("dict", m, "_mnb_frozen"), ("dict", m, "_mnb_ops")]
+            rw.forget(m, "_mnb_frozen", "_mnb_ops")
             frozen.add(m)
 
-    def override(m, fn):
-        m.__dict__["forward"] = fn
-        undo.append(("dict", m, "forward"))
+    def pool_cfg(k):
+        return _pool_cfg(k) if type(k) in (nn.MaxPool2d, EngineMaxPool2d) else None
 
-    for seq in [m for m in model.modules() if isinstance(m, nn.Sequential)]:
-        kids = [k for k in seq.children() if not isinstance(k, nn.Identity)]
-        for i, blk in enumerate(kids):
-            cba = _conv_bn_act(blk)
-            if cba is None:
-                continue
-            conv, bn, act, relu = cba
-            j, pool = i + 1, None
-            if j < len(kids) and type(kids[j]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j]) is not None:
-                pool, j = kids[j], j + 1
-            if j >= len(kids) or not hasattr(kids[j], "channel_shuffle_flag"):
-                continue
-            nxt = kids[j]
-            nparts = [k for k in nxt.children() if not isinstance(k, nn.Identity)]
-            cconv = nparts[0] if nparts else None
-            if cconv not in frozen or (pool is not None and tuple(cconv.stride) != (1, 1)):
-                continue
-            flag_sg = int(nxt.shuffle_groups) if nxt.channel_shuffle_flag and int(getattr(nxt, "shuffle_groups", 1)) > 1 else 1
-            fold_sg = int(getattr(pool if pool is not None else bn, "out_shuffle_groups", 1))   # folded by fuse=True
-            stem = type(conv) in (nn.Conv2d, EngineFloatConv2d)
-            if not (conv in frozen or (stem and relu and (pool is not None or tuple(cconv.stride) == (1, 1)))):
-                continue
-            link = _Link(cconv, bn, relu, max(flag_sg, fold_sg), None if pool is None else (pool,) + _pool_cfg(pool))
-            target = link.target
-            if stem:
-                override(bn, functools.partial(_stem_forward, bn, link))
-            else:
-                conv.__dict__["_mnb_frozen"]["link"] = link
-                override(bn, functools.partial(_absorbed_forward, bn, target))
-            if act is not None:
-                override(act, functools.partial(_absorbed_forward, act, target))
-            if pool is not None:
-                override(pool, functools.partial(_pool_forward, pool, link))
-            if flag_sg > 1:
-                undo.append(("attr", nxt, "channel_shuffle_flag", nxt.channel_shuffle_flag))
-                nxt.channel_shuffle_flag = 0
-                cconv.__dict__["_mnb_in_shuffle"] = flag_sg     # applied by the consumer when no plane comes
-                undo.append(("dict", cconv, "_mnb_in_shuffle"))
+    for (conv, bn, act, relu), pool, cfg, nxt, cconv in FG.block_pairs(model, _conv_bn_act, pool_cfg):
+        if cconv not in frozen or (pool is not None and tuple(cconv.stride) != (1, 1)):
+            continue
+        flag_sg = FG.block_shuffle(nxt)
+        fold_sg = int(getattr(pool if pool is not None else bn, "out_shuffle_groups", 1))   # folded by fuse=True
+        stem = type(conv) in (nn.Conv2d, EngineFloatConv2d)
+        if not (conv in frozen or (stem and relu and (pool is not None or tuple(cconv.stride) == (1, 1)))):
+            continue
+        link = _Link(cconv, bn, relu, max(flag_sg, fold_sg), None if pool is None else (pool,) + cfg)
+        target = link.target
+        if stem:
+            rw.override(bn, _stem_forward, bn, link)
+        else:
+            conv.__dict__["_mnb_frozen"]["link"] = link
+            rw.override(bn, FG.absorbed_forward, _check_eval, bn, target)
+        if act is not None:
+            rw.override(act, FG.absorbed_forward, _check_eval, act, target)
+        if pool is not None:
+            rw.override(pool, FG.pool_forward, _check_eval, _plane_pool, pool, link)
+        if flag_sg > 1:
+            rw.move_shuffle(nxt, cconv, flag_sg)
     return model

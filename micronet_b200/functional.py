@@ -771,7 +771,7 @@ class Consumer:
     whether it was frozen with int8 operands (``int8``: then ``format`` tells which plane it reads)"""
 
     def __init__(self, module, spec, relu, only, w_shape, stride, padding, dilation, groups, int_weights, int8=False, bn=None,
-                 shuffle_groups=1, pool=None):
+                 shuffle_groups=1, pool=None, post_spec=None, formats=None):
         self.module, self.spec, self.relu, self.only = module, spec, bool(relu), bool(only)
         self.w_shape, self.stride, self.padding, self.dilation, self.groups = w_shape, stride, padding, dilation, groups
         self.int_weights, self.int8 = int_weights, bool(int8)
@@ -780,6 +780,11 @@ class Consumer:
         # mnb_pk_plane_maxpool on the producer's full-resolution plane, so the producer tags its output for that module
         self.bn, self.sg, self.pool = bn, int(shuffle_groups), pool
         self.target = module if pool is None else pool[0]
+        # the quantizer whose levels the producer writes: the consumer's own, or - IAO graphs (iao.freeze_inference) - that of
+        # the QuantMaxPool2d in between, whose pool kernel requantizes them to the consumer's (mnb_pk_plane_maxpool_requant)
+        self.post_spec = spec if post_spec is None else post_spec
+        # the plane formats this link hands over (None: any); for any other format the producer writes fp32
+        self.formats = formats
 
     def read_shape(self, out_shape):
         """the activation the consumer reads when the producer writes ``out_shape``"""
@@ -795,11 +800,14 @@ class Consumer:
         act_shape = self.read_shape(out_shape)
         if self.sg > 1 and (out_shape[1] % 16 or out_shape[1] % self.sg or self.split):
             return None       # the epilogue stores a shuffled plane of whole units only, never phase-split
+        fmt = None
         if self.int8 and act_shape[1] == self.w_shape[1] * self.groups:
             sh = _shape_struct(act_shape, self.w_shape, self.stride, self.padding, self.dilation, self.groups)
             if _i8_route(self.spec, self.int_weights, sh):
-                return "i8"
-        return "bf16" if self.accepts(act_shape) else None
+                fmt = "i8"
+        if fmt is None and self.accepts(act_shape):
+            fmt = "bf16"
+        return fmt if self.formats is None or fmt in self.formats else None
 
     def accepts(self, act_shape):
         """will the consumer's forward run on the packed-operand family with a one-piece plane of this activation?"""
@@ -902,7 +910,7 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
         return y
     y = None if consumer.only else torch.empty(out_shape, dtype=torch.float32, device=dev)
     cplane = PK.consumer_plane(*out_shape, dev)
-    cqp = consumer.spec.struct()
+    cqp = consumer.post_spec.struct()
     L.check(_timed("fwd_pk", sh, lambda: PK.conv_post(sh, plane, ta, w_img, tw, y, cqp, cplane, consumer.relu, consumer.split,
                                                       n_scale=w_scale, a_scale=a_scale, a_scale_const=a_const, bias=bias,
                                                       bn=consumer.bn, shuffle_groups=consumer.sg)),
@@ -936,7 +944,7 @@ def _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_rel
         return y
     y = None if consumer.only else torch.empty(out_shape, dtype=torch.float32, device=dev)
     cplane = PK.consumer_plane_i8(*out_shape, dev)
-    post = (consumer.spec.struct(), cplane, consumer.relu, consumer.split, consumer.bn, consumer.sg)
+    post = (consumer.post_spec.struct(), cplane, consumer.relu, consumer.split, consumer.bn, consumer.sg)
     L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=a_scale,
                                                        a_scale_const=a_const, bias=bias, post=post)), "pk_i8_conv")
     if y is None:

@@ -14,6 +14,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
+from . import frozen_graph as FG
 from . import functional as F_
 
 
@@ -251,12 +252,14 @@ def _consumer_of(producer):
     link = producer.__dict__.get("_post_consumer")
     if link is None:
         return None
-    nxt, only = link
+    nxt, only = (link.cconv, True) if isinstance(link, _BlockLink) else link
     if not nxt._use_frozen() or nxt.quant_inference:
         return None
     aq, wq = nxt.activation_quantizer, nxt.weight_quantizer
     if aq.bits == 32 or wq.bits == 32 or not wq.symmetric:
         return None
+    if isinstance(link, _BlockLink):
+        return link.consumer(aq.act_spec(), _int8_ok(nxt))
     return F_.Consumer(nxt, aq.act_spec(), nxt.__dict__.get("_pre_relu", False), only, tuple(nxt.weight.shape), tuple(nxt.stride),
                        tuple(nxt.padding), tuple(nxt.dilation), nxt.groups, True, int8=_int8_ok(nxt))
 
@@ -304,11 +307,19 @@ class QuantConv2d(nn.Conv2d):
     def _use_frozen(self):
         return self.__dict__.get("_frozen_inference", False) and not self.training and not torch.is_grad_enabled()
 
+    def _in_shuffle(self, x):
+        """the channel shuffle of this conv's block that freeze_inference moved into the producer's epilogue, applied here
+        when the producer wrote fp32 instead (no plane came, or the module runs un-frozen)"""
+        sg = self.__dict__.get("_mnb_in_shuffle", 1)
+        return x if sg == 1 else FG.shuffle(F_.materialized(x), sg)
+
     def _frozen_forward(self, input, make):
         """eval forward of a frozen module: cached quantized weights, the operand plane its producer may have written
         (F_.handed_plane) and the plane it writes for its own consumer (freeze_inference's ``_post_consumer``)"""
         wq, w_int, w_scale, bias = self._frozen_operands(make)
         plane = F_.handed_plane(self, input)
+        if plane is None:
+            input = self._in_shuffle(input)
         aq = self.activation_quantizer
         spec = aq.act_spec() if plane is not None else aq.prepare_activation(input)
         return F_.frozen_conv(input, plane, wq, bias, w_int, w_scale, spec, self.stride, self.padding, self.dilation,
@@ -318,7 +329,7 @@ class QuantConv2d(nn.Conv2d):
     def forward(self, input):
         if self._use_frozen():
             return self._frozen_forward(input, lambda: (self.weight, self.bias))
-        return self._quant_conv(input, self.weight, self.bias)
+        return self._quant_conv(self._in_shuffle(input), self.weight, self.bias)
 
 
 class QuantConvTranspose2d(nn.ConvTranspose2d):
@@ -392,6 +403,7 @@ class QuantBNFuseConv2d(QuantConv2d):
     def forward(self, input):
         if self._use_frozen():   # eval / running statistics (IAO:903-935), folded and quantized once
             return self._frozen_forward(input, self._fold_running)
+        input = self._in_shuffle(input)
         use_batch = (not self.qaft) and self.training
         if use_batch:
             # un-quantised conv only to obtain the BN batch statistics (IAO:843-855)
@@ -635,7 +647,18 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
     * ``int8``: every quant conv with a symmetric activation quantizer (q_type 0) and symmetric weights of 2..8 bits runs
       its forward on int8 operands (s8 x s8 -> s32 wgmma, mnb_pk_i8_conv) where the int8 plan covers its shape; the others
       keep the bf16 path.  Hand-offs then carry the plane format the consumer reads.
+    * ``handoff``, NIN / NIN-GC-style graphs (``nn.Sequential`` of conv-bn-relu blocks, nin.py / nin_gc.py, prepared with
+      ``bn_fuse=True``): a block (conv, nn.Identity or nothing, nn.ReLU) is linked to the first conv of the next block when
+      both convs and any QuantMaxPool2d in between have symmetric (q_type 0) IAO quantizers and the pool is square with
+      2 * p <= k in front of a stride-1 conv.  The producer's epilogue applies the ReLU, the next block's channel shuffle and
+      the pool's quantizer (the consumer's without a pool) and writes a level plane; the pool max-pools that plane and
+      requantizes it to the consumer's levels (mnb_pk_plane_maxpool_requant).  No fp32 activation is written in between.
+      A link whose consumer block shuffles its input is taken only where it pays (DESIGN.md 4.16): the shuffled epilogue
+      stores one element at a time, so such a link is made only across a pool (whose fake-quant and max-pool passes it
+      saves) and only for an int8 plane (1-byte stores); the others write fp32 as before.
+      Blocks with a live nn.BatchNorm2d (``bn_fuse=False``) and asymmetric quantizers keep the fp32 path.
     Outputs are bit-identical to the un-frozen eval forward; ``enable=False`` restores the modules."""
+    FG.undo(model, _UNDO)
     for m in model.modules():
         if isinstance(m, (QuantConv2d, QuantLinear, QuantAdd)):
             m.__dict__["_frozen_inference"] = bool(enable)
@@ -665,7 +688,92 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
             m._modules["act"] = nn.Identity()
     if enable and handoff:
         _link_consumers(model)
+        _link_blocks(model)
     return model
+
+
+_UNDO = "_mnb_iao_undo"
+
+
+class _BlockLink(FG.Link):
+    """frozen_graph.Link of two conv-bn-relu blocks of an IAO graph: the producer applies the ReLU, the consumer block's
+    shuffle and the IAO quantizer of the QuantMaxPool2d in between (the consumer's without one).  A shuffled link hands
+    over int8 planes only (_shuffled_link_pays)."""
+
+    def consumer(self, spec, int8):
+        c = self.cconv
+        pool_spec = None if self.pool is None else self.pool[0].activation_quantizer.act_spec()
+        return F_.Consumer(c, spec, True, True, tuple(c.weight.shape), tuple(c.stride), tuple(c.padding), tuple(c.dilation),
+                           c.groups, True, int8=int8, shuffle_groups=self.sg, pool=self.pool, post_spec=pool_spec,
+                           formats=None if self.sg == 1 else ("i8",))
+
+
+def _shuffled_link_pays(pool, cconv):
+    """link a producer to a consumer block that shuffles its input?  The shuffled epilogue stores one level at a time
+    (2 bytes scattered per element for a bf16 plane, 1 for int8), where the fp32 path runs the conv with its plain epilogue
+    (or pk_gc3_kernel for the narrow grouped 3x3 layers), ATen ReLU, the shuffle copy and the consumer's pack.  Measured on
+    an H100 (DESIGN.md 4.16) this pays only when the link also replaces a pool's fake-quant and max-pool passes and the
+    plane is int8: so a pool in between and a consumer frozen with int8 operands (the link then hands over int8 planes
+    only; in any other format the producer writes fp32)."""
+    return pool is not None and _int8_ok(cconv)
+
+
+def _sym_quantizer(q):
+    return isinstance(q, Quantizer) and q.symmetric and 2 <= q.bits <= 8
+
+
+def _block_conv(conv):
+    """can ``conv`` produce or consume a level plane of a block link?  A frozen eval-mode conv with symmetric 2..8-bit IAO
+    quantizers and integer weights (no ``quant_inference``)"""
+    return (isinstance(conv, QuantConv2d) and conv.__dict__.get("_frozen_inference", False) and not conv.training
+            and not conv.quant_inference and _sym_quantizer(conv.activation_quantizer)
+            and _sym_quantizer(conv.weight_quantizer))
+
+
+def _conv_relu(blk):
+    """(conv, nn.ReLU) of a conv-bn-relu block whose BatchNorm prepare(bn_fuse=True) folded into the conv, else None"""
+    bp = FG.block_parts(blk)
+    if bp is None or len(bp[1]) != 1 or type(bp[1][0]) is not nn.ReLU:
+        return None
+    return bp[0], bp[1][0]
+
+
+def _pool_cover(m):
+    """(k, s, p) of a QuantMaxPool2d that mnb_pk_plane_maxpool_requant runs, else None"""
+    from .fused import _pool_cfg
+    if type(m) is not QuantMaxPool2d or m.training or not _sym_quantizer(m.activation_quantizer):
+        return None
+    return _pool_cfg(m)
+
+
+def _requant_pool(link, plane, b, c, h, w, k, s, p, int8):
+    from . import pk as PK
+    q_in = link.pool[0].activation_quantizer.act_spec().struct()
+    q_out = link.cconv.activation_quantizer.act_spec().struct()
+    return PK.plane_maxpool_requant(plane, b, c, h, w, k, s, p, q_in, q_out, int8=int8)
+
+
+def _no_check(m):
+    """absorbed IAO modules run un-frozen in training mode: a producer tags its output only on the frozen eval path"""
+
+
+def _link_blocks(model):
+    """block -> block links of NIN / NIN-GC-style graphs (see freeze_inference); recorded for ``enable=False``"""
+    import functools
+    rw = FG.Rewrite(model, _UNDO)
+    for (conv, relu), pool, cfg, nxt, cconv in FG.block_pairs(model, _conv_relu, _pool_cover):
+        if not (_block_conv(conv) and _block_conv(cconv)) or (pool is not None and tuple(cconv.stride) != (1, 1)):
+            continue
+        sg = FG.block_shuffle(nxt)
+        if sg > 1 and not _shuffled_link_pays(pool, cconv):
+            continue
+        link = _BlockLink(cconv, None, relu, sg, None if pool is None else (pool,) + cfg)
+        rw.set_dict(conv, "_post_consumer", link)
+        rw.override(relu, FG.absorbed_forward, _no_check, relu, link.target)
+        if pool is not None:
+            rw.override(pool, FG.pool_forward, _no_check, functools.partial(_requant_pool, link), pool, link)
+        if sg > 1:
+            rw.move_shuffle(nxt, cconv, sg)
 
 
 def _first_quant_conv(seq):

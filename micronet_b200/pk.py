@@ -163,6 +163,16 @@ def plane_maxpool(plane, b, c, h, w, k, s, p, int8=False):
     return out
 
 
+def plane_maxpool_requant(plane, b, c, h, w, k, s, p, q_in, q_out, int8=False):
+    """the IAO QuantMaxPool2d between two frozen convs on a plane of its own quantizer's levels (q_in, an ActQParams):
+    max_pool2d(k, s, p), requantized to the consumer's quantizer q_out (mnb_pk_plane_maxpool_requant) -> the consumer's plane"""
+    oh, ow = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    out = (consumer_plane_i8 if int8 else consumer_plane)(b, c, oh, ow, plane.device)
+    L.check(L.load().mnb_pk_plane_maxpool_requant(plane.data_ptr(), b, c, h, w, k, s, p, 1 if int8 else 0, C.byref(q_in),
+                                                  C.byref(q_out), out.data_ptr(), L.stream()), "pk_plane_maxpool_requant")
+    return out
+
+
 def pack_weight_i8(sh, w_int):
     nbytes = int(L.load().mnb_pk_i8_wimage_bytes(C.byref(sh)))
     if nbytes < 0:
