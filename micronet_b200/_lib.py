@@ -230,9 +230,6 @@ def tc_check(device=None):
 E_UNSUPPORTED = -2
 KEEP_DEBUG = False   # tests only: modules keep the fake-quantized weight of their last call
 USE_TC = os.environ.get("MNB_DISABLE_TC", "0") != "1"
-# packed bf16 operands from the BN+binarizer producer to the next conv's forward (experimental, opt-in with
-# MNB_PACKED_OPERANDS=1): the producer's extra 2 B / element plane costs more than the conv gains
-USE_PACKED = os.environ.get("MNB_PACKED_OPERANDS", "0") == "1"
 # packed-operand tensor-core family (mnb_pk.cu): "auto" = wherever the fused kernels have no cover and for every fused-quantizer
 # layer; "all" = every conv it supports; "off" = never
 PK_MODE = os.environ.get("MNB_PK", "auto")

@@ -328,14 +328,14 @@ def _pk_terms(spec, w_int, pm1=False):
     return ta, (1 if w_int is not None else T)
 
 
-def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, need_dx, prepacked=None, pre_relu=False, pm1=False,
-                codes_out=False):
+def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, pre_relu=False, pm1=False, codes_out=False):
     """forward on the packed-operand tensor-core family; returns False when the shape is outside its cover.
     ``prepacked``: the operand plane a fused producer (fused.BNReluQuantFn) already wrote - x itself holds no data then.
     ``codes_out`` (wbwtab layer on a +-1 input whose only reader is its fused BatchNorm + binarizer): the exact integer sums
     go out as int16 codes with their decode pair, tagged on y as ``_mnb_codes``; y itself is then not written.  Shapes the
     int16 hand-off does not cover write y as usual."""
     from . import pk as PK
+    need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
     ta, tw = _pk_terms(spec, w_int, pm1)
     if not PK.supported(sh, 0, ta, tw):
         return False
@@ -343,64 +343,47 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, need_dx, prepacke
     Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
     if need_dx and not PK.supported(sh, 1, Tb, 1 if w_int is not None else Tb):
         return False
-    if ctx.needs_input_grad[1] and not PK.wgrad_supported(sh, Tb, min(ta, Tb)):
+    if need_dw and not PK.wgrad_supported(sh, Tb, min(ta, Tb)):
         return False
     qp = spec.struct() if spec is not None else None
-    split = sh.stride_h == 2
     if prepacked is not None:
         x_pk, bits8 = prepacked, None      # the producer keeps the STE mask for its own backward
     else:
-        x_pk, bits8 = PK.pack_act(x, qp, ta, phase_split=split, want_bits=need_dx, relu=pre_relu)
-    # frozen (inference) modules hang a dict on their cached weight tensor: the packed image is then built once
-    src = w_int if w_int is not None else wq
-    cache = getattr(src, "_mnb_pk_cache", None)
-    ckey = (PK._key(sh), ta, tw)
-    w_img = cache.get(ckey) if cache is not None else None
-    if w_img is None:
-        w_img = PK.pack_weight(sh, 0, ta, tw, w_int=w_int, w_f32=None if w_int is not None else wq)
-        if cache is not None:
-            cache[ckey] = w_img
-    a_scale, a_const = None, 1.0
-    if spec is not None:
-        if spec.mode == L.ACT_IAO:
-            # backward must see the forward-time scale (the reference clones it too); no clone needed without autograd
-            a_scale = spec.scale.clone() if (need_dx or ctx.needs_input_grad[1]) else spec.scale
-        elif spec.mode == L.ACT_DOREFA:
-            a_const = 1.0 / float(2 ** spec.bits - 1)
+        x_pk, bits8 = PK.pack_act(x, qp, ta, phase_split=sh.stride_h == 2, want_bits=need_dx, relu=pre_relu)
+    w_img = PK.weight_image(sh, ta, tw, w_int=w_int, w_f32=None if w_int is not None else wq)
+    # backward must see the forward-time scale (the reference clones it too); no clone needed without autograd
+    a_scale, a_const = PK.act_scale(spec, clone=need_dx or need_dw)
     rc = L.E_UNSUPPORTED
     if codes_out and w_int is not None and ta == 1 and tw == 1:
         codes = torch.empty(y.shape, dtype=torch.int16, device=y.device)
         dec = torch.empty(2 * y.shape[1], dtype=torch.float32, device=y.device)
-        # narrow grouped 3x3 layers: whole images as M tiles (same kernel-table kind, the same codes); whatever that kernel
-        # refuses goes to mnb_pk_conv_codes
-        fns = ([PK.gc3_conv_codes] if L.PK_GC3 and PK.gc3_plan(sh, 0, 1, 1) is not None else []) + [PK.conv_codes]
-        for fn in fns:
-            rc = _timed("fwd_pk", sh, lambda fn=fn: fn(sh, x_pk, w_img, codes, dec, n_scale=w_scale, a_scale=a_scale,
-                                                       a_scale_const=a_const, bias=bias))
-            if rc != L.E_UNSUPPORTED:
-                break
+        rc = _timed("fwd_pk", sh, lambda: PK.run_conv_codes(sh, x_pk, w_img, codes, dec, n_scale=w_scale, a_scale=a_scale,
+                                                            a_scale_const=a_const, bias=bias))
         if rc == 0:
             y._mnb_codes = (codes, dec)
     if rc == L.E_UNSUPPORTED:
-        fns = ([PK.gc3_conv] if L.PK_GC3 and PK.gc3_plan(sh, 0, ta, tw) is not None else []) + [PK.conv]
-        for fn in fns:
-            rc = _timed("fwd_pk", sh, lambda fn=fn: fn(sh, 0, x_pk, ta, w_img, tw, y,
-                                                       n_scale=w_scale if w_int is not None else None,
-                                                       a_scale=a_scale, a_scale_const=a_const, bias=bias))
-            if rc != L.E_UNSUPPORTED:
-                break
+        rc = _timed("fwd_pk", sh, lambda: PK.run_conv(sh, 0, x_pk, ta, w_img, tw, y,
+                                                      n_scale=w_scale if w_int is not None else None, a_scale=a_scale,
+                                                      a_scale_const=a_const, bias=bias))
     if rc == L.E_UNSUPPORTED:
         return False
     L.check(rc, "pk_conv fwd")
-    ctx.pk = True
-    ctx.pk_x, ctx.pk_ta, ctx.pk_bits8, ctx.pk_a_scale, ctx.pk_prepacked = x_pk, ta, bits8, a_scale, prepacked is not None
+    ctx.pk_x, ctx.pk_ta, ctx.pk_bits8, ctx.pk_prepacked = x_pk, ta, bits8, prepacked is not None
+    # the quantizer's STE gain on the data gradient, and the scale of the saved activation levels in the weight gradient
+    ctx.pk_gain = 0.1 if (spec is not None and spec.mode == L.ACT_DOREFA) else 1.0
+    ctx.pk_wg_scale = None
+    if spec is not None:
+        ctx.pk_wg_scale = a_scale if spec.mode == L.ACT_IAO else _dorefa_scale_tensor(spec.bits, x.device)
+    if spec is None and w_int is not None and need_dw:
+        # a fused BatchNorm + binarizer consuming y may write this layer's gradient operand itself (fused.BNSignFn)
+        y._mnb_pk_conv = (w_scale if need_dx else None, Tb)
     return True
 
 
 def _pk_backward(ctx, dy):
     """data and weight gradients of a layer whose forward ran on the packed-operand path"""
     from . import pk as PK
-    sh, spec = ctx.sh, ctx.spec
+    sh = ctx.sh
     T = min(L.PK_TERMS, L.PK_TERMS_BWD)     # pieces of dy and of an fp32 second operand (see _lib.PK_TERMS_BWD)
     int_w = ctx.w_int is not None
     need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
@@ -420,244 +403,273 @@ def _pk_backward(ctx, dy):
         w_img = PK.pack_weight(sh, 1, T, tw, w_int=ctx.w_int, w_f32=None if int_w else ctx.wq,
                                kzero=ctx.w_scale if int_w else None)
         dx = torch.empty((sh.batch, sh.in_c, sh.in_h, sh.in_w), dtype=torch.float32, device=dy.device)
-        gain = 0.1 if (spec is not None and spec.mode == L.ACT_DOREFA) else 1.0
         # a fused producer applies the STE mask itself (it owns the mask bits): plain data gradient times the quantizer's gain
-        plain_gain = gain if ctx.pk_prepacked else 1.0
-        fns = ([PK.gc3_conv] if L.PK_GC3 and PK.gc3_plan(sh, 1, T, tw) is not None else []) + [PK.conv]
-        for fn in fns:   # whatever mnb_pk_gc3_conv refuses goes to mnb_pk_conv
-            rc = _timed("dgrad_pk", sh, lambda fn=fn: fn(sh, 1, dy_pk, T, w_img, tw, dx, bits8=ctx.pk_bits8, gain=gain,
-                                                         a_scale_const=plain_gain))
-            if rc != L.E_UNSUPPORTED:
-                break
-        L.check(rc, "pk_conv dgrad")
+        plain_gain = ctx.pk_gain if ctx.pk_prepacked else 1.0
+        L.check(_timed("dgrad_pk", sh, lambda: PK.run_conv(sh, 1, dy_pk, T, w_img, tw, dx, bits8=ctx.pk_bits8, gain=ctx.pk_gain,
+                                                           a_scale_const=plain_gain)), "pk_conv dgrad")
     if need_dw:
         dwq = torch.empty_like(ctx.wq)
-        a_scale = None
-        if spec is not None:
-            a_scale = ctx.pk_a_scale if spec.mode == L.ACT_IAO else _dorefa_scale_tensor(spec.bits, dy.device)
         tx = min(ctx.pk_ta, T)     # a 3-piece saved input contributes its two leading pieces
         kdiv = ctx.w_scale if fold else None
-        # narrow grouped 3x3 layers: all taps of a CTA in registers (same kernel-table kind; its rows are those layers' shapes)
-        fn = PK.wgrad_taps if L.PK_WG_TAPS and PK.wgrad_taps_plan(sh, T, tx) is not None else PK.wgrad
-        L.check(_timed("wgrad_pk", sh, lambda: fn(sh, dy_pk, T, ctx.pk_x, tx, dwq, a_scale=a_scale, kdiv=kdiv)), "pk_wgrad")
+        L.check(_timed("wgrad_pk", sh, lambda: PK.run_wgrad(sh, dy_pk, T, ctx.pk_x, tx, dwq, a_scale=ctx.pk_wg_scale,
+                                                            kdiv=kdiv)), "pk_wgrad")
     return dx, dwq
+
+
+def _xnor_forward(x, w_int, w_scale, bias, sh, y, groups):
+    """wbwtab inference forward on +-1 activations: bit-packed XNOR-popcount kernel where it is expected to beat the
+    tensor-core forward (xnor_preferred).  Same integer sums, same fmaf epilogue: bit-identical to the packed-operand
+    path.  Only taken where no backward follows (training steps multiply real-valued gradients and want the bf16 operand
+    plane the forward already read), so it saves nothing."""
+    from . import xnor as XN
+    if not (XN.supported(sh) and (L.XNOR_MODE == "all" or xnor_preferred(sh, getattr(x, "_mnb_pk_pm1", None) is not None))):
+        return False
+    a_bits = XN.pack_act(materialized(x), groups)
+    rc = _timed("fwd_xnor", sh, lambda: XN.conv(sh, a_bits, XN.pack_weight(sh, w_int), y, alpha=w_scale, bias=bias))
+    if rc == L.E_UNSUPPORTED:
+        return False
+    L.check(rc, "xnor_conv_fwd")
+    return True
+
+
+def _save_unpacked(ctx, x, spec, codes, bits, keep_x):
+    """what the backward of the round-1, fconv and generic families reads: the quantizer with its forward-time parameters
+    (the forward kernel may have refreshed them), its u8 codes and STE mask bits, and the fp32 input where a kernel reads it"""
+    if spec is not None and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]):
+        spec = spec.frozen()
+    ctx.spec, ctx.codes, ctx.bits = spec, codes, bits
+    ctx.x = x if keep_x else None
+
+
+def _act_operands(spec, codes, x):
+    """ConvOperands with the activation side filled in: the u8 codes of the quantizer ``spec`` or the fp32 tensor x"""
+    ops = L.ConvOperands()
+    if codes is None:
+        ops.a_f32 = x.data_ptr()
+        return ops
+    ops.a_codes, ops.a_offset = codes.data_ptr(), spec.code_offset
+    if spec.mode == L.ACT_IAO:
+        ops.a_offset_zp, ops.a_scale = L.ptr(spec.zero_point), L.ptr(spec.scale)
+    elif spec.mode == L.ACT_DOREFA:
+        ops.a_scale = _dorefa_scale_tensor(spec.bits, codes.device).data_ptr()
+    return ops
+
+
+def _tc_forward(ctx, x, w_int, w_scale, bias, spec, sh, y):
+    """round-1 fused wgmma forward (mnb_fq_conv2d_fwd_tc): the activation quantizer runs inside the operand staging of the
+    tensor-core conv and also writes the u8 codes and STE mask bits the backward reads.  False outside its cover."""
+    lib = L.load()
+    qp = codes = bits = None
+    if spec is not None:
+        qp = spec.struct()
+        codes = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
+        if ctx.needs_input_grad[0]:
+            bits = torch.zeros((x.numel() + 31) // 32, dtype=torch.int32, device=x.device)
+    wpack = torch.empty(w_int.numel(), dtype=torch.int16, device=x.device)
+    rc = _timed("fwd_tc", sh, lambda: lib.mnb_fq_conv2d_fwd_tc(
+        C.byref(sh), x.data_ptr(), None if qp is None else C.byref(qp), w_int.data_ptr(),
+        w_scale.data_ptr(), L.ptr(bias), y.data_ptr(), L.ptr(codes), L.ptr(bits), wpack.data_ptr(),
+        L.tc_err_flag(x.device).data_ptr(), L.stream()))
+    if rc == L.E_UNSUPPORTED:
+        return False
+    L.check(rc, "fq_conv2d_fwd_tc")
+    _save_unpacked(ctx, x, spec, codes, bits, keep_x=True)
+    return True
+
+
+def _fconv_forward(ctx, x, wq, bias, sh, y):
+    """un-quantized input with few channels (first layer): fp32-accurate im2col conv on the tensor cores
+    (mnb_fconv2d_fwd_tc).  False outside its cover."""
+    lib = L.load()
+    rc = _timed("fconv_fwd_tc", sh, lambda: lib.mnb_fconv2d_fwd_tc(
+        C.byref(sh), x.data_ptr(), wq.data_ptr(), L.ptr(bias), y.data_ptr(), L.tc_err_flag(x.device).data_ptr(), L.stream()))
+    if rc == L.E_UNSUPPORTED:
+        return False
+    L.check(rc, "fconv2d_fwd_tc")
+    _save_unpacked(ctx, x, None, None, None, keep_x=True)
+    return True
+
+
+def _generic_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, keep_x):
+    """implicit-GEMM forward of any shape (mnb_conv2d_fwd) on the codes of the standalone quantizer kernel"""
+    lib = L.load()
+    codes = bits = None
+    if spec is not None:
+        codes, bits, _ = act_quant_raw(x, spec, True, ctx.needs_input_grad[0], False)
+    ops = _act_operands(spec, codes, x)
+    if codes is not None and w_int is not None:
+        ops.w_int, ops.w_scale = w_int.data_ptr(), w_scale.data_ptr()
+    else:
+        ops.w_f32 = wq.data_ptr()
+    ops.bias = L.ptr(bias)
+    L.check(_timed("fwd", sh, lambda: lib.mnb_conv2d_fwd(C.byref(sh), C.byref(ops), y.data_ptr(), L.stream())), "conv2d_fwd")
+    _save_unpacked(ctx, x, spec, codes, bits, keep_x=keep_x or codes is None)
+
+
+def _dgrad(ctx, dy, tc):
+    """data gradient of an unpacked layer: mnb_conv2d_dgrad_tc first when ``tc`` (integer weights), mnb_conv2d_dgrad for
+    whatever it refuses"""
+    lib = L.load()
+    sh, spec = ctx.sh, ctx.spec
+    dx = torch.empty((sh.batch, sh.in_c, sh.in_h, sh.in_w), dtype=torch.float32, device=dy.device)
+    qp = spec.struct() if spec is not None else None
+    bits_ptr = ctx.bits.data_ptr() if spec is not None else None
+    rc = L.E_UNSUPPORTED
+    if tc:
+        wpack = torch.empty(ctx.w_int.numel(), dtype=torch.int16, device=dy.device)
+        rc = _timed("dgrad_tc", sh, lambda: lib.mnb_conv2d_dgrad_tc(
+            C.byref(sh), dy.data_ptr(), ctx.w_int.data_ptr(), ctx.w_scale.data_ptr(), bits_ptr,
+            None if qp is None else C.byref(qp), dx.data_ptr(), wpack.data_ptr(),
+            L.tc_err_flag(dy.device).data_ptr(), L.stream()))
+    if rc == L.E_UNSUPPORTED:
+        rc = _timed("dgrad", sh, lambda: lib.mnb_conv2d_dgrad(
+            C.byref(sh), dy.data_ptr(), ctx.wq.data_ptr(), bits_ptr, None if qp is None else C.byref(qp),
+            dx.data_ptr(), L.stream()))
+    L.check(rc, "conv2d_dgrad")
+    return dx
+
+
+def _wgrad(ctx, dy, tc):
+    """weight gradient of an unpacked layer: mnb_conv2d_wgrad_tc first when ``tc`` (integer weights; raw fp32 activations
+    that are not bf16-exact then take mnb_conv2d_wgrad_cond, on the device), mnb_conv2d_wgrad for whatever it refuses"""
+    lib = L.load()
+    sh, spec = ctx.sh, ctx.spec
+    dwq = torch.empty_like(ctx.wq)
+    ops = _act_operands(spec, ctx.codes, ctx.x)
+    nbytes = int(lib.mnb_wgrad_scratch_bytes(C.byref(sh)))
+    tbytes = int(lib.mnb_wgrad_tc_scratch_bytes(C.byref(sh))) if tc else 0
+    if tbytes > 0:
+        qp = spec.struct() if spec is not None else None
+        ws = torch.empty(max(tbytes, nbytes, 4), dtype=torch.uint8, device=dy.device)
+        inexact = torch.zeros(1, dtype=torch.int32, device=dy.device)
+        rc = _timed("wgrad_tc", sh, lambda: lib.mnb_conv2d_wgrad_tc(
+            C.byref(sh), dy.data_ptr(), ctx.x.data_ptr(), None if qp is None else C.byref(qp),
+            dwq.data_ptr(), ws.data_ptr(), inexact.data_ptr(), L.tc_err_flag(dy.device).data_ptr(), L.stream()))
+        if rc == 0:
+            if spec is None:
+                L.check(lib.mnb_conv2d_wgrad_cond(C.byref(sh), dy.data_ptr(), C.byref(ops), dwq.data_ptr(),
+                                                  ws.data_ptr(), inexact.data_ptr(), L.stream()), "conv2d_wgrad_cond")
+            return dwq
+        if rc != L.E_UNSUPPORTED:
+            L.check(rc, "conv2d_wgrad_tc")
+    ws = torch.empty(max(nbytes, 4), dtype=torch.uint8, device=dy.device)
+    L.check(_timed("wgrad", sh, lambda: lib.mnb_conv2d_wgrad(
+        C.byref(sh), dy.data_ptr(), C.byref(ops), dwq.data_ptr(), ws.data_ptr(), L.stream())), "conv2d_wgrad")
+    return dwq
+
+
+def _fconv_wgrad(ctx, dy):
+    """weight gradient on mnb_fconv2d_wgrad_tc; None where it has no plan"""
+    lib = L.load()
+    sh = ctx.sh
+    fbytes = int(lib.mnb_fconv2d_wgrad_tc_scratch_bytes(C.byref(sh)))
+    if fbytes < 0:
+        return None
+    dwq = torch.empty_like(ctx.wq)
+    ws = torch.empty(max(fbytes, 4), dtype=torch.uint8, device=dy.device)
+    L.check(_timed("fconv_wgrad_tc", sh, lambda: lib.mnb_fconv2d_wgrad_tc(
+        C.byref(sh), dy.data_ptr(), ctx.x.data_ptr(), dwq.data_ptr(), ws.data_ptr(), L.tc_err_flag(dy.device).data_ptr(),
+        L.stream())), "fconv2d_wgrad_tc")
+    return dwq
 
 
 class QuantConv2dFn(Function):
     """y = conv2d(Q_a(x), wq, bias) with the activation quantizer fused on the input side
-    and the clip-STE fused into dgrad.  ``spec`` None => x is used as fp32 (wbwtab, a_bits=32)."""
+    and the clip-STE fused into dgrad.  ``spec`` None => x is used as fp32 (wbwtab, a_bits=32).
+
+    The forward picks one kernel family and records it as ``ctx.family``; the backward runs that family's gradients
+    (DESIGN.md 4.9, "Dispatch")."""
 
     @staticmethod
     def forward(ctx, x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, no_grad=False,
                 codes_out=False):
         L.require_cuda(x, wq)
         assert not (pre_relu and any(ctx.needs_input_grad)), "the folded ReLU is an inference-only fusion"
-        lib = L.load()
-        packed = getattr(x, "_mnb_packed", None) if L.USE_PACKED else None   # experimental, see fused.BNSignFn
         x = x.contiguous()
         wq = wq.contiguous()
         sh = _shape_struct(x.shape, wq.shape, stride, padding, dilation, groups)
         p, q = _out_hw(sh)
         y = torch.empty((x.shape[0], wq.shape[0], p, q), dtype=torch.float32, device=x.device)
-        codes = bits = None
-        a_scale = None
-        if spec is not None and spec.mode != L.ACT_SIGN:
-            a_scale = spec.scale if spec.mode == L.ACT_IAO else _dorefa_scale_tensor(spec.bits, x.device)
-        done = False
-        ctx.pk = False
-        if (L.XNOR_MODE != "off" and spec is None and w_int is not None and getattr(x, "_mnb_pm1", False)
-                and (no_grad or not any(ctx.needs_input_grad[:3])) and x.dtype == torch.float32 and not pre_relu):
-            # wbwtab inference forward on +-1 activations: bit-packed XNOR-popcount kernel where it is expected to beat the
-            # tensor-core forward (xnor_preferred).  Same integer sums, same fmaf epilogue:
-            # bit-identical to the packed-operand path.  Training steps never come here (their backward multiplies real-valued
-            # gradients and wants the bf16 operand plane the forward already read).
-            from . import xnor as XN
-            if XN.supported(sh) and (L.XNOR_MODE == "all" or xnor_preferred(sh, getattr(x, "_mnb_pk_pm1", None) is not None)):
-                a_bits = XN.pack_act(materialized(x), groups)
-                rc = _timed("fwd_xnor", sh, lambda: XN.conv(sh, a_bits, XN.pack_weight(sh, w_int), y, alpha=w_scale, bias=bias))
-                if rc == 0:
-                    done = True
-                elif rc != L.E_UNSUPPORTED:
-                    L.check(rc, "xnor_conv_fwd")
+        ctx.sh, ctx.wq, ctx.has_bias = sh, wq, bias is not None
+        ctx.w_int, ctx.w_scale = (w_int, w_scale) if w_int is not None else (None, None)
+        pk_on = L.PK_MODE != "off"
+        pm1 = x.dtype == torch.float32 and getattr(x, "_mnb_pm1", False)   # exactly +-1 (a binarizer's output)
+        pm1_plane = getattr(x, "_mnb_pk_pm1", None)   # that +-1 tensor as the bf16 plane a fused BatchNorm + binarizer wrote
+        plane = pm1_plane if (pm1_plane is not None and pm1_plane.numel() == x.numel() * 2) else None
         pkq = getattr(x, "_mnb_pk_q", None)   # operand plane written by a fused BN + ReLU + quantizer producer
-        if pkq is not None and not done:
+        plane_only = getattr(x, "_mnb_plane_only", False)
+        if (L.XNOR_MODE != "off" and spec is None and w_int is not None and pm1 and not pre_relu
+                and (no_grad or not any(ctx.needs_input_grad[:3])) and _xnor_forward(x, w_int, w_scale, bias, sh, y, groups)):
+            family = "xnor"
+        elif pkq is not None:
             if spec is None or spec.mode != L.ACT_DOREFA or spec.bits != pkq[1] or w_int is None:
                 raise RuntimeError("micronet_b200: a fused producer's packed output reached a conv with another quantizer")
-            done = _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, ctx.needs_input_grad[0], prepacked=pkq[0])
-            if not done:
+            if not _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=pkq[0]):
                 raise RuntimeError("micronet_b200: fused producer output in front of a conv outside the packed-operand cover")
-        if (not done and L.PK_MODE != "off" and x.dtype == torch.float32 and (L.PK_MODE == "all" or spec is not None)
-                and not getattr(x, "_mnb_plane_only", False)):
-            done = _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, ctx.needs_input_grad[0], pre_relu=pre_relu)
-        pm1_plane = getattr(x, "_mnb_pk_pm1", None)
-        if (not done and L.PK_WBWTAB and L.PK_MODE != "off" and spec is None and w_int is not None and x.dtype == torch.float32
-                and getattr(x, "_mnb_pm1", False) and (pm1_plane is not None or sh.ker_h * sh.ker_w > 1)):
-            # wbwtab layer behind a fused BatchNorm + binarizer: +-1 input (one exact bf16 piece).  With the producer's plane
-            # the layer is pure TMA -> MMA; 3x3 layers win on the packed-operand family even when they pack themselves
-            # (measured per layer, DESIGN.md 6).  Falls through to the fused kernels when the shape is outside the cover.
-            if pm1_plane is not None and pm1_plane.numel() != x.numel() * 2:
-                pm1_plane = None
-            done = _pk_forward(ctx, x, wq, bias, w_int, w_scale, None, sh, y, ctx.needs_input_grad[0], prepacked=pm1_plane,
-                               pm1=True, codes_out=codes_out)
-        if (not done and L.PK_MODE != "off" and spec is None and w_int is None and x.dtype == torch.float32
-                and getattr(x, "_mnb_pm1", False) and not pre_relu):
-            # un-quantized conv behind a binarizer (the 10-way head of a wbwtab model, fused.EnginePmConv2d): the +-1 input is
-            # ONE exact bf16 piece - the producer's plane when it wrote one - against exact pieces of the fp32 weights
-            plane = pm1_plane if (pm1_plane is not None and pm1_plane.numel() == x.numel() * 2) else None
-            done = _pk_forward(ctx, x, wq, bias, None, None, None, sh, y, ctx.needs_input_grad[0], prepacked=plane, pm1=True)
-        if not done and getattr(x, "_mnb_plane_only", False):
-            x = materialized(x)   # outside the packed-operand cover (rare): the kernels below read the fp32 values
-        if not done and pre_relu:
-            x = torch.relu(x)     # outside the packed-operand cover: the folded ReLU as its own pass
-        if not done and packed is not None and spec is None and w_int is not None and packed.numel() == x.numel() \
-                and L.PK_MODE != "off" and sh.stride_h == 1:
-            # the BatchNorm + binarizer producer also wrote its +-1 output as the bf16 plane the packed-operand family
-            # reads (fused.BNSignFn): forward = TMA -> MMA -> epilogue on 2 B/element, no pack pass, no converter warps.
-            # The backward of this layer stays on the fused kernels below (they re-read the fp32 tensor).
-            from . import pk as PK
-            if PK.supported(sh, 0, 1, 1):
-                w_img = PK.pack_weight(sh, 0, 1, 1, w_int=w_int)
-                rc = _timed("fwd_pk", sh, lambda: PK.conv(sh, 0, packed, 1, w_img, 1, y, n_scale=w_scale, bias=bias))
-                if rc == 0:
-                    done = True
-                elif rc != L.E_UNSUPPORTED:
-                    L.check(rc, "pk_conv fwd (packed producer)")
-        if not done and L.USE_TC and w_int is not None and x.dtype == torch.float32:
-            # fused wgmma path: quantize inside the operand staging of the tensor-core conv
-            qp = None
-            if spec is not None:
-                qp = spec.struct()
-                codes = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
-                if ctx.needs_input_grad[0]:
-                    bits = torch.zeros((x.numel() + 31) // 32, dtype=torch.int32, device=x.device)
-            wpack = torch.empty(w_int.numel(), dtype=torch.int16, device=x.device)
-            rc = _timed("fwd_tc", sh, lambda: lib.mnb_fq_conv2d_fwd_tc(
-                C.byref(sh), x.data_ptr(), None if qp is None else C.byref(qp), w_int.data_ptr(),
-                w_scale.data_ptr(), L.ptr(bias), y.data_ptr(), L.ptr(codes), L.ptr(bits), wpack.data_ptr(),
-                L.tc_err_flag(x.device).data_ptr(), L.stream()))
-            if rc == 0:
-                done = True
-            elif rc == L.E_UNSUPPORTED:
-                codes = bits = None
+            family = "pk"
+        elif ((pk_on and x.dtype == torch.float32 and (L.PK_MODE == "all" or spec is not None) and not plane_only
+               and _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, pre_relu=pre_relu))
+              # wbwtab layer behind a fused BatchNorm + binarizer: +-1 input (one exact bf16 piece).  With the producer's
+              # plane the layer is pure TMA -> MMA; 3x3 layers win on the packed-operand family even when they pack
+              # themselves (measured per layer, DESIGN.md 6).  Outside the cover: the round-1 fused kernels below.
+              or (L.PK_WBWTAB and pk_on and spec is None and w_int is not None and pm1
+                  and (pm1_plane is not None or sh.ker_h * sh.ker_w > 1)
+                  and _pk_forward(ctx, x, wq, bias, w_int, w_scale, None, sh, y, prepacked=plane, pm1=True,
+                                  codes_out=codes_out))
+              # un-quantized conv behind a binarizer (the 10-way head of a wbwtab model, fused.EnginePmConv2d): the +-1
+              # input is ONE exact bf16 piece - the producer's plane when it wrote one - against exact pieces of the fp32
+              # weights
+              or (pk_on and spec is None and w_int is None and pm1 and not pre_relu
+                  and _pk_forward(ctx, x, wq, bias, None, None, None, sh, y, prepacked=plane, pm1=True))):
+            family = "pk"
+        else:
+            # outside the packed-operand cover: the kernels below read the fp32 values, with the folded ReLU as its own pass
+            if plane_only:
+                x = materialized(x)
+            if pre_relu:
+                x = torch.relu(x)
+            f32 = x.dtype == torch.float32
+            if L.USE_TC and w_int is not None and f32 and _tc_forward(ctx, x, w_int, w_scale, bias, spec, sh, y):
+                family = "tc"
+            elif L.USE_TC and spec is None and f32 and _fconv_forward(ctx, x, wq, bias, sh, y):
+                family = "fconv"
+            elif pk_on and f32 and _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y):
+                family = "pk"
             else:
-                L.check(rc, "fq_conv2d_fwd_tc")
-        ctx.fconv = False
-        if not done and L.USE_TC and spec is None and x.dtype == torch.float32:
-            # un-quantized input with few channels (first layer): fp32-accurate im2col conv on the tensor cores
-            rc = _timed("fconv_fwd_tc", sh, lambda: lib.mnb_fconv2d_fwd_tc(
-                C.byref(sh), x.data_ptr(), wq.data_ptr(), L.ptr(bias), y.data_ptr(),
-                L.tc_err_flag(x.device).data_ptr(), L.stream()))
-            if rc == 0:
-                done = ctx.fconv = True
-            elif rc != L.E_UNSUPPORTED:
-                L.check(rc, "fconv2d_fwd_tc")
-        if not done and L.PK_MODE != "off" and x.dtype == torch.float32:
-            done = _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, ctx.needs_input_grad[0])
-        if not done:
-            ops = L.ConvOperands()
-            if spec is not None:
-                codes, bits, _ = act_quant_raw(x, spec, True, ctx.needs_input_grad[0], False)
-                ops.a_codes = codes.data_ptr()
-                ops.a_offset = spec.code_offset
-                ops.a_offset_zp = L.ptr(spec.zero_point) if spec.mode == L.ACT_IAO else None
-                ops.a_scale = L.ptr(a_scale)
-            else:
-                ops.a_f32 = x.data_ptr()
-            if codes is not None and w_int is not None:
-                ops.w_int, ops.w_scale = w_int.data_ptr(), w_scale.data_ptr()
-            else:
-                ops.w_f32 = wq.data_ptr()
-            ops.bias = L.ptr(bias)
-            L.check(_timed("fwd", sh, lambda: lib.mnb_conv2d_fwd(C.byref(sh), C.byref(ops), y.data_ptr(), L.stream())),
-                    "conv2d_fwd")
-        if spec is not None and not ctx.pk and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]):
-            spec = spec.frozen()   # backward re-quantizes / masks with the forward-time parameters
-            if spec.mode == L.ACT_IAO:
-                a_scale = spec.scale
-        ctx.sh, ctx.spec, ctx.a_scale = sh, spec, a_scale
-        ctx.codes, ctx.bits = codes, bits
-        ctx.x = x if (not ctx.pk and (codes is None or (L.USE_TC and w_int is not None))) else None
-        ctx.wq = wq
-        ctx.w_int, ctx.w_scale = (w_int, w_scale) if w_int is not None else (None, None)
-        ctx.has_bias = bias is not None
-        if ctx.pk and spec is None and w_int is not None and ctx.needs_input_grad[1]:
-            # a fused BatchNorm + binarizer consuming y may write this layer's gradient operand itself (fused.BNSignFn)
-            y._mnb_pk_conv = (w_scale if ctx.needs_input_grad[0] else None, min(L.PK_TERMS, L.PK_TERMS_BWD))
+                # the round-1 backward kernels also cover shapes whose forward they refuse (the data gradient reads K
+                # channels and writes C): with integer weights the layer takes the round-1 backward
+                tc = L.USE_TC and w_int is not None
+                _generic_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, keep_x=tc)
+                family = "tc" if tc else "generic"
+        ctx.family = family
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        lib = L.load()
         # a fused BatchNorm+binarize consumer already reduced its dx (= this dy) over (B, H, W): fused.BNSignFn
         presummed = getattr(dy, "_mnb_channel_sum", None)
         dy = dy.contiguous()
-        sh, spec = ctx.sh, ctx.spec
-        dx = dwq = db = None
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        db = None
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = presummed if presummed is not None and presummed.numel() == dy.shape[1] else channel_sums(dy)
-        if ctx.pk:
+        dx = dwq = None
+        if ctx.family == "pk":
             dx, dwq = _pk_backward(ctx, dy)
-            return dx, dwq, db, None, None, None, None, None, None, None, None, None, None
-        if ctx.needs_input_grad[0]:
-            dx = torch.empty((sh.batch, sh.in_c, sh.in_h, sh.in_w), dtype=torch.float32, device=dy.device)
-            qp = spec.struct() if spec is not None else None
-            bits_ptr = ctx.bits.data_ptr() if spec is not None else None
-            rc = L.E_UNSUPPORTED
-            if L.USE_TC and ctx.w_int is not None:
-                wpack = torch.empty(ctx.w_int.numel(), dtype=torch.int16, device=dy.device)
-                rc = _timed("dgrad_tc", sh, lambda: lib.mnb_conv2d_dgrad_tc(
-                    C.byref(sh), dy.data_ptr(), ctx.w_int.data_ptr(), ctx.w_scale.data_ptr(), bits_ptr,
-                    None if qp is None else C.byref(qp), dx.data_ptr(), wpack.data_ptr(),
-                    L.tc_err_flag(dy.device).data_ptr(), L.stream()))
-            if rc == L.E_UNSUPPORTED:
-                rc = _timed("dgrad", sh, lambda: lib.mnb_conv2d_dgrad(
-                    C.byref(sh), dy.data_ptr(), ctx.wq.data_ptr(), bits_ptr, None if qp is None else C.byref(qp),
-                    dx.data_ptr(), L.stream()))
-            L.check(rc, "conv2d_dgrad")
-        if ctx.needs_input_grad[1]:
-            dwq = torch.empty_like(ctx.wq)
-            ops = L.ConvOperands()
-            if ctx.codes is not None:
-                ops.a_codes = ctx.codes.data_ptr()
-                ops.a_offset = spec.code_offset
-                ops.a_offset_zp = L.ptr(spec.zero_point) if spec.mode == L.ACT_IAO else None
-                ops.a_scale = L.ptr(ctx.a_scale)
-            else:
-                ops.a_f32 = ctx.x.data_ptr()
-            nbytes = int(lib.mnb_wgrad_scratch_bytes(C.byref(sh)))
-            done = False
-            if ctx.fconv:
-                fbytes = int(lib.mnb_fconv2d_wgrad_tc_scratch_bytes(C.byref(sh)))
-                if fbytes >= 0:
-                    ws = torch.empty(max(fbytes, 4), dtype=torch.uint8, device=dy.device)
-                    L.check(_timed("fconv_wgrad_tc", sh, lambda: lib.mnb_fconv2d_wgrad_tc(
-                        C.byref(sh), dy.data_ptr(), ctx.x.data_ptr(), dwq.data_ptr(), ws.data_ptr(),
-                        L.tc_err_flag(dy.device).data_ptr(), L.stream())), "fconv2d_wgrad_tc")
-                    done = True
-            if not done and L.USE_TC and ctx.w_int is not None and ctx.x is not None:
-                tbytes = int(lib.mnb_wgrad_tc_scratch_bytes(C.byref(sh)))
-                if tbytes > 0:
-                    qp = spec.struct() if spec is not None else None
-                    ws = torch.empty(max(tbytes, nbytes, 4), dtype=torch.uint8, device=dy.device)
-                    inexact = torch.zeros(1, dtype=torch.int32, device=dy.device)
-                    rc = _timed("wgrad_tc", sh, lambda: lib.mnb_conv2d_wgrad_tc(
-                        C.byref(sh), dy.data_ptr(), ctx.x.data_ptr(), None if qp is None else C.byref(qp),
-                        dwq.data_ptr(), ws.data_ptr(), inexact.data_ptr(), L.tc_err_flag(dy.device).data_ptr(),
-                        L.stream()))
-                    if rc == 0:
-                        done = True
-                        if spec is None:
-                            # raw fp32 activations that are not bf16-exact: device-side fallback, no host sync
-                            L.check(lib.mnb_conv2d_wgrad_cond(C.byref(sh), dy.data_ptr(), C.byref(ops), dwq.data_ptr(),
-                                                              ws.data_ptr(), inexact.data_ptr(), L.stream()),
-                                    "conv2d_wgrad_cond")
-                    elif rc != L.E_UNSUPPORTED:
-                        L.check(rc, "conv2d_wgrad_tc")
-            if not done:
-                ws = torch.empty(max(nbytes, 4), dtype=torch.uint8, device=dy.device)
-                L.check(_timed("wgrad", sh, lambda: lib.mnb_conv2d_wgrad(
-                    C.byref(sh), dy.data_ptr(), C.byref(ops), dwq.data_ptr(), ws.data_ptr(), L.stream())),
-                    "conv2d_wgrad")
+        elif ctx.family == "tc":
+            dx = _dgrad(ctx, dy, tc=True) if need_dx else None
+            dwq = _wgrad(ctx, dy, tc=True) if need_dw else None
+        elif ctx.family == "fconv":
+            # integer weights (a wbwtab layer the round-1 forward refused): the round-1 kernels may still take the gradients
+            tc = ctx.w_int is not None
+            dx = _dgrad(ctx, dy, tc) if need_dx else None
+            if need_dw:
+                dwq = _fconv_wgrad(ctx, dy)
+                if dwq is None:
+                    dwq = _wgrad(ctx, dy, tc)
+        else:
+            dx = _dgrad(ctx, dy, tc=False) if need_dx else None
+            dwq = _wgrad(ctx, dy, tc=False) if need_dw else None
         return dx, dwq, db, None, None, None, None, None, None, None, None, None, None
 
 
@@ -894,15 +906,8 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
     if plane is None:
         L.require_cuda(x, wq)
         plane, _ = PK.pack_act(x.contiguous(), spec.struct(), ta, phase_split=sh.stride_h == 2, relu=pre_relu)
-    cache = getattr(w_int, "_mnb_pk_cache", None)
-    ckey = (PK._key(sh), ta, tw)
-    w_img = cache.get(ckey) if cache is not None else None
-    if w_img is None:
-        w_img = PK.pack_weight(sh, 0, ta, tw, w_int=w_int)
-        if cache is not None:
-            cache[ckey] = w_img
-    a_scale = spec.scale if spec.mode == L.ACT_IAO else None
-    a_const = 1.0 / float(2 ** spec.bits - 1) if spec.mode == L.ACT_DOREFA else 1.0
+    w_img = PK.weight_image(sh, ta, tw, w_int=w_int)
+    a_scale, a_const = PK.act_scale(spec)
     if not fused:
         y = torch.empty(out_shape, dtype=torch.float32, device=dev)
         L.check(_timed("fwd_pk", sh, lambda: PK.conv(sh, 0, plane, ta, w_img, tw, y, n_scale=w_scale, a_scale=a_scale,
@@ -927,16 +932,8 @@ def _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_rel
     if plane is None:
         L.require_cuda(x, w_int)
         plane = PK.pack_act_i8(x.contiguous(), spec.struct(), phase_split=sh.stride_h == 2, relu=pre_relu)
-    cache = getattr(w_int, "_mnb_pk_cache", None)
-    ckey = (PK._key(sh), "i8")
-    w_img = cache.get(ckey) if cache is not None else None
-    if w_img is None:
-        w_img = PK.pack_weight_i8(sh, w_int)
-        if cache is not None:
-            cache[ckey] = w_img
-    # activation scale: IAO's device scalar, DoReFa's 1 / (2^a - 1)
-    a_scale = spec.scale if spec.mode == L.ACT_IAO else None
-    a_const = 1.0 / float(2 ** spec.bits - 1) if spec.mode == L.ACT_DOREFA else 1.0
+    w_img = PK.weight_image(sh, w_int=w_int, i8=True)
+    a_scale, a_const = PK.act_scale(spec)
     if consumer is None:
         y = torch.empty(out_shape, dtype=torch.float32, device=dev)
         L.check(_timed("fwd_pk_i8", sh, lambda: PK.conv_i8(sh, plane, w_img, y, n_scale=w_scale, a_scale=a_scale,

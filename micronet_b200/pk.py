@@ -10,6 +10,9 @@ shared memory, stride 2, 5x5 filters, 4x4 or 224x224 images ...) and every fused
     wgrad_taps  wgrad of narrow grouped 3x3 layers with all nine taps of a CTA in registers
     gc3_conv    forward / data gradient of the same layers with whole images as M tiles (same result as conv)
 
+The layers of the engine go through run_conv / run_conv_codes / run_wgrad, which pick among those kernels (``PK_GC3``,
+``PK_WG_TAPS``); the single-kernel calls stay for tests and probes that compare the kernels directly.
+
 Reference math: F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen's
 convolution_backward."""
 from __future__ import annotations
@@ -77,6 +80,31 @@ def pack_weight(sh, mode, terms_a, terms_w, w_int=None, w_f32=None, kzero=None):
     L.check(lib.mnb_pk_pack_weight(C.byref(sh), mode, terms_a, terms_w, L.ptr(w_int), L.ptr(w_f32), L.ptr(kzero),
                                    img.data_ptr(), L.stream()), "pk_pack_weight")
     return img
+
+
+def weight_image(sh, terms_a=1, terms_w=1, w_int=None, w_f32=None, i8=False):
+    """forward weight image of pack_weight (or of pack_weight_i8 with ``i8``).  Frozen (inference) modules hang a dict
+    ``_mnb_pk_cache`` on their cached weight tensor: the image is then built once per shape."""
+    src = w_int if w_int is not None else w_f32
+    cache = getattr(src, "_mnb_pk_cache", None)
+    key = (_key(sh), "i8") if i8 else (_key(sh), terms_a, terms_w)
+    img = cache.get(key) if cache is not None else None
+    if img is None:
+        img = pack_weight_i8(sh, w_int) if i8 else pack_weight(sh, 0, terms_a, terms_w, w_int=w_int, w_f32=w_f32)
+        if cache is not None:
+            cache[key] = img
+    return img
+
+
+def act_scale(spec, clone=False):
+    """(a_scale, a_scale_const) of the forward epilogues for the activation quantizer ``spec`` (functional.ActSpec or None):
+    IAO's device scalar - a private copy with ``clone``, for a backward that must see the forward-time scale - or DoReFa's
+    1 / (2^a - 1)"""
+    if spec is not None and spec.mode == L.ACT_IAO:
+        return (spec.scale.clone() if clone else spec.scale), 1.0
+    if spec is not None and spec.mode == L.ACT_DOREFA:
+        return None, 1.0 / float(2 ** spec.bits - 1)
+    return None, 1.0
 
 
 def conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, n_scale=None, a_scale=None, a_scale_const=1.0, bias=None,
@@ -259,3 +287,30 @@ def gc3_conv_codes(sh, a_pk, w_img, codes, dec, n_scale=None, a_scale=None, a_sc
     return L.load().mnb_pk_gc3_conv_codes(C.byref(sh), a_pk.data_ptr(), 1, w_img.data_ptr(), 1, L.ptr(n_scale), L.ptr(a_scale),
                                           float(a_scale_const), L.ptr(bias), int(level_bound), codes.data_ptr(), dec.data_ptr(),
                                           L.tc_err_flag(codes.device).data_ptr(), L.stream())
+
+
+# ---- kernel choice of the engine's layers
+def run_conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, **epilogue):
+    """forward (mode 0) or data gradient (mode 1) with conv's arguments: on gc3_conv where its plan covers the shape and
+    PK_GC3 allows, on conv otherwise and for whatever gc3_conv refuses.  Returns the C status."""
+    if L.PK_GC3 and gc3_plan(sh, mode, terms_a, terms_w) is not None:
+        rc = gc3_conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, **epilogue)
+        if rc != L.E_UNSUPPORTED:
+            return rc
+    return conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, **epilogue)
+
+
+def run_conv_codes(sh, a_pk, w_img, codes, dec, **epilogue):
+    """conv_codes with the same choice as run_conv: gc3_conv_codes first where it applies.  Returns the C status."""
+    if L.PK_GC3 and gc3_plan(sh, 0, 1, 1) is not None:
+        rc = gc3_conv_codes(sh, a_pk, w_img, codes, dec, **epilogue)
+        if rc != L.E_UNSUPPORTED:
+            return rc
+    return conv_codes(sh, a_pk, w_img, codes, dec, **epilogue)
+
+
+def run_wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
+    """weight gradient with wgrad's arguments: on wgrad_taps where its plan covers the shape and PK_WG_TAPS allows, on
+    wgrad otherwise.  Returns the C status."""
+    fn = wgrad_taps if L.PK_WG_TAPS and wgrad_taps_plan(sh, terms_dy, terms_x) is not None else wgrad
+    return fn(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=a_scale, kdiv=kdiv)

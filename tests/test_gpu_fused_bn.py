@@ -296,6 +296,38 @@ def test_wbwtab_layer_between_two_fused_producers_on_the_packed_operand_family(c
     L.tc_check()
 
 
+# B, C, H, W, K, R, groups, shuffle groups of the producer
+PLANE_FED = [(4, 256, 32, 32, 256, 1, 2, 1), (4, 256, 32, 32, 256, 1, 2, 2), (4, 512, 16, 16, 512, 1, 4, 16),
+             (5, 1024, 8, 8, 1024, 1, 8, 32), (4, 256, 16, 16, 512, 3, 16, 2), (4, 512, 8, 8, 1024, 3, 32, 4),
+             (3, 64, 16, 16, 32, 3, 1, 1)]
+
+
+@pytest.mark.parametrize("case", PLANE_FED, ids=[str(c) for c in PLANE_FED])
+def test_plane_fed_conv_matches_fp64(case):
+    """BatchNormBinarize2d writes its +-1 output also as the bf16 operand plane of the next conv; a wbwtab conv fed by that
+    plane (packed-operand family, no pack pass) equals an fp64 convolution of the fp32 +-1 tensor"""
+    import torch.nn.functional as TF
+    from micronet_b200 import _lib as L, functional as F_
+    from micronet_b200.fused import BatchNormBinarize2d
+    B, C, H, W, K, R, G, sg = case
+    torch.manual_seed(sum(case))
+    bn = BatchNormBinarize2d(C).to(DEV).train()
+    bn.out_shuffle_groups = sg
+    with torch.no_grad():
+        bn.weight.copy_(torch.rand(C) + 0.5)
+        bn.bias.copy_(torch.randn(C) * 0.3)
+    y = bn((torch.randn(B, C, H, W) * 1.5).to(DEV))
+    assert getattr(y, "_mnb_pk_pm1", None) is not None, "producer did not write the operand plane"
+    w_int = torch.randint(-1, 2, (K, C // G, R, R), dtype=torch.int16).to(DEV)
+    w_scale = (torch.rand(K) * 0.02 + 0.001).to(DEV)
+    bias = torch.randn(K).to(DEV)
+    wq = w_int.float() * w_scale.view(-1, 1, 1, 1)
+    out = F_.quant_conv2d(y, wq, bias, w_int, w_scale, None, (1, 1), (R // 2, R // 2), (1, 1), G)
+    L.tc_check()
+    ref = TF.conv2d(y.detach().double().cpu(), wq.double().cpu(), bias.double().cpu(), 1, R // 2, 1, G)
+    assert rel_err(out.detach(), ref) < 2e-6
+
+
 @pytest.mark.parametrize("shape", [(8, 1024, 8, 8, 10, 1), (4, 256, 16, 16, 24, 3)], ids=["head1x1", "3x3"])
 def test_unquantized_conv_behind_a_binarizer_runs_on_the_packed_family(shape):
     """fused.EnginePmConv2d (the fp32 10-way head of a wbwtab model, WB:247-331 leaves it un-quantized): BatchNorm+binarizer

@@ -270,3 +270,33 @@ def test_tc_wgrad_matches_generic_and_cpu(shape, mode):
     wr = wq.clone().double().requires_grad_(True)
     TF.conv2d(xq.double(), wr, None, 1, R // 2, 1, G).backward(go.double())
     assert rel_err(grads[True], wr.grad) <= 1e-5, rel_err(grads[True], wr.grad)
+
+
+def test_backward_stays_on_the_family_of_the_forward():
+    """the backward of a layer whose forward ran on the fused tensor-core kernels runs dgrad_tc / wgrad_tc even when
+    L.USE_TC changes between forward and backward, with the gradients of a run that never changes it"""
+    from micronet_b200 import _lib as L, functional as F_
+    B, C, H, W, K, R, G = SHAPES[0]
+    g = torch.Generator().manual_seed(11)
+    x = (torch.randn(B, C, H, W, generator=g) * 4).to(DEV)
+    w_int = torch.randint(-127, 128, (K, C // G, R, R), generator=g, dtype=torch.int16).to(DEV)
+    w_scale = (torch.rand(K, generator=g) * 0.02 + 0.001).to(DEV)
+    wq = w_int.float() * w_scale.view(-1, 1, 1, 1)
+    go = torch.randn(B, K, H, W, generator=g).to(DEV)
+    spec = F_.ActSpec(L.ACT_DOREFA, bits=8)
+    grads, kinds = {}, {}
+    for flip in (False, True):
+        restore = _legs(True)
+        try:
+            xg, wg = x.clone().requires_grad_(True), wq.clone().requires_grad_(True)
+            y = F_.quant_conv2d(xg, wg, None, w_int, w_scale, spec, (1, 1), (R // 2, R // 2), (1, 1), G)
+            if flip:
+                L.USE_TC = False
+            y.backward(go)
+            torch.cuda.synchronize()
+            grads[flip] = (xg.grad, wg.grad)
+        finally:
+            kinds[flip] = restore()
+        assert {"fwd_tc", "dgrad_tc", "wgrad_tc"} <= kinds[flip], (flip, kinds[flip])
+    L.tc_check()
+    assert torch.equal(grads[True][0], grads[False][0]) and torch.equal(grads[True][1], grads[False][1])
