@@ -391,6 +391,16 @@ int mnb_bn_sign_pool_bwd_pack_codes(const float* g, const uint32_t* pass_bits, c
 int mnb_pk_pack_act_relu(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_act_qparams* qp,
                          int32_t terms, const float* ch_scale, int32_t phase_split, int32_t relu, void* out_pk,
                          uint8_t* bits8, mnb_stream_t stream);
+/* Group-padded planes of a grouped conv (DESIGN.md 4.17): mnb_pk_pack_act_relu for the operand of a conv with `groups` groups.
+ * Group g's channel j sits at plane channel g * round_up(channels / groups, 8) + j; the padding channels are zero in every
+ * plane and in bits8 [b][groups * ceil(channels / groups / 8)][h][w].  With channels / groups % 8 == 0 (or groups == 1) this
+ * is the plane of mnb_pk_pack_act.  mnb_pk_conv, mnb_pk_wgrad and mnb_pk_pack_weight read grouped operands in this layout
+ * (mode 0: the input's channels per group, mode 1 and the weight gradient's dy: the output's).  out_pk:
+ * mnb_pk_grouped_act_bytes() bytes (-1: groups do not divide channels). */
+int64_t mnb_pk_grouped_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t terms, int32_t groups);
+int mnb_pk_pack_act_grouped(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_act_qparams* qp,
+                            int32_t terms, const float* ch_scale, int32_t phase_split, int32_t relu, void* out_pk,
+                            uint8_t* bits8, int32_t groups, mnb_stream_t stream);
 int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out16); /* host only */
 /* host only, the plan mnb_pk_conv / mnb_pk_wgrad will run (same MNB_PK_* environment knobs); the first min(n, 21) resp.
  * min(n, 10) fields are written:

@@ -102,6 +102,8 @@ PROTOTYPES = {
     "mnb_pk_pack_act": (C.c_int, [_P, _I, _I, _I, _I, _ACTQ, _I, _P, _I, _P, _P, _P]),
     "mnb_bn_relu_quant_pack_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _ACTQ, _I, _P, _P, _P]),
     "mnb_pk_pack_act_relu": (C.c_int, [_P, _I, _I, _I, _I, _ACTQ, _I, _P, _I, _I, _P, _P, _P]),
+    "mnb_pk_grouped_act_bytes": (_L, [_I, _I, _I, _I, _I, _I]),
+    "mnb_pk_pack_act_grouped": (C.c_int, [_P, _I, _I, _I, _I, _ACTQ, _I, _P, _I, _I, _P, _P, _I, _P]),
     "mnb_pk_conv_plan": (C.c_int, [_SHAPE, _I, _I, _I, _P]),
     "mnb_pk_conv_plan_ex": (C.c_int, [_SHAPE, _I, _I, _I, _P, _I]),
     "mnb_pk_wgrad_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),

@@ -119,9 +119,10 @@ static int make_plan(const mnb_conv_shape* s, int mode, int TA, int TBk, Plan& p
     p.nkph = 1; p.HA = P; p.WA = Q; p.C8A = ceil_div(K, 8);
     p.OHr = H / st; p.OWr = W / st; p.OH = H; p.OW = W; p.omul = st; p.ny = st == 2 ? 4 : 1;
   }
-  if (G > 1 && (p.kg % cpu))
-    return unsupported(cpu == 8 ? "grouped conv needs GEMM-K channels per group % 8 == 0"
-                                : "grouped int8 conv needs GEMM-K channels per group % 16 == 0");
+  if (cpu == 16 && G > 1 && (p.kg % cpu)) return unsupported("grouped int8 conv needs GEMM-K channels per group % 16 == 0");
+  // bf16 planes of a grouped conv are group-padded: group g's K-octets start at octet g * ceil(kg / 8) (DESIGN.md 4.17;
+  // the same octets as ceil(C / 8) whenever kg % 8 == 0 or G == 1)
+  if (cpu == 8) p.C8A = G * ceil_div(p.kg, 8);
   // s32 accumulators: |level| <= 128 (activations) times |level| <= 127 (symmetric weights) over kg x taps products
   if (cpu == 16 && (int64_t)p.kg * R * S * 128 * 127 > (int64_t)INT32_MAX) return unsupported("int8 sums could overflow s32");
   // ---- taps: (k-phase, shift) of every filter tap, per output phase
@@ -345,11 +346,13 @@ __device__ __forceinline__ uint4 pack16_s8(const float (&l)[16]) {
 //   QUANT = 1: plane 0.. hold the fake-quantized integer level e = code + a_off (+ zero point) (exact; two pieces when
 //              |e| can exceed 256), bits8[b][c/8][h][w] bit j = STE pass flag of channel 8*(c/8) + j
 // phase_split: octet index (h%2 * 2 + w%2) * C8 + c/8 of a [.., H/2, W/2] plane (stride-2 consumers)
-template <int QUANT>
-__global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__ x, int B, int C, int H, int W, int C8,
-                                                       int terms, const float* __restrict__ ch_scale, mnb_act_qparams qp,
-                                                       int a_off, int phase_split, uint4* __restrict__ out,
-                                                       int64_t plane_vecs, uint8_t* __restrict__ bits8, int relu) {
+// GROUPED: the group-padded plane of a grouped conv with cg channels per group, cg % 8 != 0: group g's channel j sits at
+// plane channel g * kg8 * 8 + j (kg8 = ceil(cg / 8) octets per group), the padding channels are zero in every plane and mask.
+template <int QUANT, bool GROUPED>
+__device__ __forceinline__ void pack_act_body(const float* __restrict__ x, int B, int C, int H, int W, int C8, int terms,
+                                              const float* __restrict__ ch_scale, mnb_act_qparams qp, int phase_split,
+                                              uint4* __restrict__ out, int64_t plane_vecs, uint8_t* __restrict__ bits8, int relu,
+                                              int cg, int kg8) {
   MnbActQ q;
   float zp = 0.f;
   if (QUANT) {
@@ -362,17 +365,25 @@ __global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__
   const uint32_t plane = blockIdx.y * blockDim.y + threadIdx.y;                 // b * C8 + c8
   if (plane >= (uint32_t)B * (uint32_t)C8) return;
   const uint32_t b = plane / (uint32_t)C8, c8 = plane - b * (uint32_t)C8;
+  // first channel of the octet, and (GROUPED) its index inside its group: channels jb + j >= cg are padding
+  uint32_t cb = c8 * 8, jb = 0;
+  if (GROUPED) {
+    const uint32_t g = c8 / (uint32_t)kg8;
+    jb = (c8 - g * (uint32_t)kg8) * 8;
+    cb = g * (uint32_t)cg + jb;
+  }
   for (uint32_t pos = blockIdx.x * blockDim.x + threadIdx.x; pos < HW; pos += gridDim.x * blockDim.x) {
     const int64_t idx = (int64_t)plane * HW + pos;
     float v[8];
     uint32_t passbits = 0;
-    const float* src = x + ((int64_t)b * C + c8 * 8) * HW + pos;
+    const float* src = x + ((int64_t)b * C + (GROUPED ? cb : c8 * 8)) * HW + pos;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const int c = (int)c8 * 8 + j;
-      float val = c < C ? __ldg(src + (int64_t)j * HW) : 0.f;
+      const int c = GROUPED ? (int)cb + j : (int)c8 * 8 + j;
+      const bool in = GROUPED ? (int)jb + j < cg : c < C;
+      float val = in ? __ldg(src + (int64_t)j * HW) : 0.f;
       if (relu) val = fmaxf(val, 0.f);          // a preceding nn.ReLU folded into the packer (inference graphs)
-      if (!QUANT && ch_scale) val = c < C ? __fmul_rn(val, __ldg(ch_scale + c)) : 0.f;
+      if (!QUANT && ch_scale) val = in ? __fmul_rn(val, __ldg(ch_scale + c)) : 0.f;
       v[j] = val;
     }
     if (QUANT) {   // level itself (code + a_off) as a float, eight channels in straight-line code
@@ -381,7 +392,7 @@ __global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__
       uint32_t live = 0;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const bool in = (int)c8 * 8 + j < C;
+        const bool in = GROUPED ? (int)jb + j < cg : (int)c8 * 8 + j < C;
         v[j] = in ? lev[j] + zp : 0.f;
         live |= in ? (1u << j) : 0u;
       }
@@ -407,6 +418,23 @@ __global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__
     }
     if (QUANT && bits8) bits8[idx] = (uint8_t)passbits;
   }
+}
+
+template <int QUANT>
+__global__ void __launch_bounds__(256) pack_act_kernel(const float* __restrict__ x, int B, int C, int H, int W, int C8,
+                                                       int terms, const float* __restrict__ ch_scale, mnb_act_qparams qp,
+                                                       int a_off, int phase_split, uint4* __restrict__ out,
+                                                       int64_t plane_vecs, uint8_t* __restrict__ bits8, int relu) {
+  pack_act_body<QUANT, false>(x, B, C, H, W, C8, terms, ch_scale, qp, phase_split, out, plane_vecs, bits8, relu, 0, 1);
+}
+
+// C8 = groups * kg8 octets per position
+template <int QUANT>
+__global__ void __launch_bounds__(256) pack_act_grouped_kernel(const float* __restrict__ x, int B, int C, int H, int W, int C8,
+                                                               int terms, const float* __restrict__ ch_scale, mnb_act_qparams qp,
+                                                               int phase_split, uint4* __restrict__ out, int64_t plane_vecs,
+                                                               uint8_t* __restrict__ bits8, int relu, int cg, int kg8) {
+  pack_act_body<QUANT, true>(x, B, C, H, W, C8, terms, ch_scale, qp, phase_split, out, plane_vecs, bits8, relu, cg, kg8);
 }
 
 // fp32 NCHW -> int8 level plane [b][c/16][h][w][16] of a symmetric IAO quantizer (levels in [-128, 127]): the levels of
@@ -1292,7 +1320,9 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
         } else {
           // STE of the activation quantizer that fed the forward conv: the reference computes ((g*s)*pass)/s (IAO) or
           // (((g*s)/s)*pass)*0.1 (DoReFa); (g*s)/s is g to within one ulp, so g itself is passed
-          const int oc0 = (n_base + n0) >> 3;     // n_base + n0 is a multiple of 8 (checked on the host)
+          // mask octet of channel nt * Nt + n0 of group g (a multiple of 8) in the group-padded mask: C8O / G octets per group
+          // (the int8 instances run forward plans only)
+          const int oc0 = I8 ? (n_base + n0) >> 3 : g * (p.C8O / p.G) + ((nt * p.Nt + n0) >> 3);
           const uint32_t m0 = __ldg(brow + (int64_t)oc0 * plane);
           const uint32_t m1 = (n0 + 8 < n_cnt) ? __ldg(brow + (int64_t)(oc0 + 1) * plane) : 0u;
           const uint32_t mask = m0 | (m1 << 8);
@@ -1369,7 +1399,8 @@ static int set_max_smem(K kernel, int bytes) {
 struct WgPlan {
   int B, G, R, S, stride, ntap;
   int P, Q, K8, HX, WX, C8X, nkph;      // dy dims / octets; x planes as stored
-  int cin_g, cout_g, gm;       // channels per (merged) group; gm = original groups per merged group
+  int cin_g, cout_g, gm;       // plane channels per (merged) group; gm = original groups per merged group
+  int cin_o, cout_o;           // channels per original group
   int hlo, hhi, wlo, whi, BW, TH, THH, rows_dy, rows_x, row_tiles;
   int Nc, n_ctiles, n_ktiles, tpg, n_tg, NI, nsub, nstg_total, splits, stg_per_split;
   int TA, TX, npairs, pair_a[MAXPAIR], pair_b[MAXPAIR];
@@ -1393,8 +1424,9 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
   p.B = s->batch; p.G = G; p.R = R; p.S = S; p.stride = st; p.ntap = R * S;
   p.P = (H + 2 * ph_ - R) / st + 1; p.Q = (W + 2 * pw_ - S) / st + 1;
   if (p.P < 1 || p.Q < 1) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: empty output");
-  p.cin_g = C / G; p.cout_g = K / G;
-  if (G > 1 && ((p.cin_g % 8) || (p.cout_g % 8))) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: grouped conv needs channels per group % 8 == 0");
+  p.cin_o = C / G; p.cout_o = K / G;
+  // group-padded planes (DESIGN.md 4.17): a group spans round_up(channels per group, 8) plane channels on either side
+  p.cin_g = G > 1 ? round_up(p.cin_o, 8) : p.cin_o; p.cout_g = G > 1 ? round_up(p.cout_o, 8) : p.cout_o;
   // Small groups are MERGED: gm neighbouring groups form one 128-row accumulator block (rows = their output channels,
   // columns = their input channels); a narrow MMA uses the tensor core poorly, so computing the discarded off-diagonal
   // blocks costs little and the MMA count drops by gm.  The reduction kernel keeps the diagonal blocks only.
@@ -1402,7 +1434,7 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
   while (G % (p.gm * 2) == 0 && p.gm * 2 * p.cout_g <= 128 && p.gm * 2 * p.cin_g <= 128) p.gm *= 2;
   if (const char* e = getenv("MNB_PK_WG_MERGE")) { if (atoi(e) == 0) p.gm = 1; }
   p.G = G / p.gm; p.cin_g *= p.gm; p.cout_g *= p.gm;
-  p.K8 = ceil_div(K, 8); p.C8X = ceil_div(C, 8);
+  p.K8 = ceil_div(p.G * p.cout_g, 8); p.C8X = ceil_div(p.G * p.cin_g, 8);
   p.nkph = st == 2 ? 4 : 1; p.HX = H / st; p.WX = W / st;
   p.TA = TA; p.TX = TX;
   { Plan tmp; memset(&tmp, 0, sizeof(tmp)); make_pairs(TA, TX, tmp); p.npairs = tmp.npairs;
@@ -1651,10 +1683,11 @@ done:
 // One block = the 128 output channels of a k tile for ONE (input channel, tap): the partials are read along k, their
 // contiguous dimension (512-byte runs per warp), four splits in flight per thread; |W| threads in total.
 __global__ void __launch_bounds__(128) wg_reduce_kernel(const float* __restrict__ partial, int splits, int G, int gm, int n_ktiles,
-                                                        int n_ctiles, int ntap, int Nc, int cout_g, int cin_g,
-                                                        const float* __restrict__ a_scale, const float* __restrict__ kdiv,
-                                                        float* __restrict__ dw) {
-  // cout_g / cin_g: channels per ORIGINAL group.  grid = (cin_g * ntap, k tiles of the original group, original groups)
+                                                        int n_ctiles, int ntap, int Nc, int cout_g, int cin_g, int cout_p,
+                                                        int cin_p, const float* __restrict__ a_scale,
+                                                        const float* __restrict__ kdiv, float* __restrict__ dw) {
+  // cout_g / cin_g: channels per ORIGINAL group; cout_p / cin_p: the plane channels it spans (group-padded planes: rounded
+  // up to 8, only the real (k, c) entries are read).  grid = (cin_g * ntap, k tiles of the original group, original groups)
   const int go = blockIdx.z, ktile = blockIdx.y;
   const int c = blockIdx.x / ntap, tap = blockIdx.x - c * ntap;
   const int g = go / gm, gi = go - g * gm;
@@ -1662,7 +1695,7 @@ __global__ void __launch_bounds__(128) wg_reduce_kernel(const float* __restrict_
   if (kk >= cout_g) return;
   const int64_t tile = (int64_t)ntap * Nc * 128;
   const int64_t split_stride = (int64_t)G * n_ktiles * n_ctiles * tile;
-  const int km = gi * cout_g + kk, cm = gi * cin_g + c;     // row / column inside the merged group
+  const int km = gi * cout_p + kk, cm = gi * cin_p + c;     // row / column inside the merged group
   const int kt = km >> 7, kl = km & 127, ct = cm / Nc, cl = cm - ct * Nc;
   const float* src = partial + (((int64_t)g * n_ktiles + kt) * n_ctiles + ct) * tile + ((int64_t)tap * Nc + cl) * 128 + kl;
   float acc = 0.f;
@@ -2243,6 +2276,44 @@ extern "C" int mnb_pk_pack_act_relu(const float* x, int32_t batch, int32_t chann
   return 0;
 }
 
+extern "C" int64_t mnb_pk_grouped_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t terms, int32_t groups) {
+  if (groups < 1 || channels % groups) return -1;
+  return (int64_t)terms * batch * groups * ((channels / groups + 7) / 8) * h * w * 16;
+}
+
+extern "C" int mnb_pk_pack_act_grouped(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w,
+                                       const mnb_act_qparams* qp, int32_t terms, const float* ch_scale, int32_t phase_split,
+                                       int32_t relu, void* out_pk, uint8_t* bits8, int32_t groups, mnb_stream_t stream) {
+  MNB_REQUIRE(x && out_pk, "NULL pk_pack_act_grouped pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0 && terms >= 1 && terms <= 3 && groups >= 1 && channels % groups == 0,
+              "bad pk_pack_act_grouped arguments");
+  MNB_REQUIRE((reinterpret_cast<uintptr_t>(out_pk) & 15) == 0, "packed tensor must be 16-byte aligned");
+  if (phase_split) MNB_REQUIRE(((h | w) & 1) == 0, "phase split needs even H and W");
+  const int cg = channels / groups;
+  if (groups == 1 || cg % 8 == 0)   // the padded layout is the plain one: one kernel for it
+    return mnb_pk_pack_act_relu(x, batch, channels, h, w, qp, terms, ch_scale, phase_split, relu, out_pk, bits8, stream);
+  const int kg8 = (cg + 7) / 8, C8 = groups * kg8;
+  const int64_t plane_vecs = (int64_t)batch * C8 * h * w;
+  MNB_REQUIRE((int64_t)batch * C8 <= 65535 * 8 && (int64_t)h * w < (1ll << 31), "pk_pack_act_grouped: too many (image, octet) planes");
+  dim3 blocks, threads;
+  if (!unit_grid(batch, C8, h * w, blocks, threads))
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_pack_act_grouped: %d (image, octet) planes exceed the grid", batch * C8);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (qp) {
+    MNB_REQUIRE(qp->mode == MNB_ACT_DOREFA || qp->mode == MNB_ACT_IAO || qp->mode == MNB_ACT_SIGN, "unknown activation quantizer");
+    if (qp->mode == MNB_ACT_DOREFA) MNB_REQUIRE(qp->bits >= 2 && qp->bits <= 8, "DoReFa a_bits must be in [2,8]");
+    pk::pack_act_grouped_kernel<1><<<blocks, threads, 0, st>>>(x, batch, channels, h, w, C8, terms, nullptr, *qp, phase_split,
+                                                               reinterpret_cast<uint4*>(out_pk), plane_vecs, bits8, relu, cg, kg8);
+  } else {
+    mnb_act_qparams none{};
+    pk::pack_act_grouped_kernel<0><<<blocks, threads, 0, st>>>(x, batch, channels, h, w, C8, terms, ch_scale, none, phase_split,
+                                                               reinterpret_cast<uint4*>(out_pk), plane_vecs, nullptr, relu, cg,
+                                                               kg8);
+  }
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
 template <typename XT>
 static int bn_sign_bwd_pack(const float* g, const uint32_t* pass_bits, const XT* x, const float* dec, int32_t batch,
                             int32_t channels, int32_t hw, const float* mean, const float* invstd, const float* gamma,
@@ -2515,7 +2586,6 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     // products, e.g. an asymmetric-IAO producer whose levels take two pieces) it costs register spills on every launch
     if (pl.segmented) return unsupported("fused consumer of a segmented (multi-piece) plan");
   }
-  if (bits8 && pl.G > 1 && (pl.ng % 8)) return unsupported("STE mask of a grouped conv needs channels per group % 8 == 0");
   static ConvParams p;   // large POD: filled per call (single host thread per process)
   memset(&p, 0, sizeof(p));
   ConvParams::Mma& m = p.m;
@@ -2549,13 +2619,14 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     p.img_bytes[y] = pl.img_bytes[y]; p.y_off[y] = pl.y_off[y];
   }
   p.n_items = pl.n_items; p.n_ntiles = pl.n_ntiles; p.G = pl.G; p.MT = pl.MT; p.TA = pl.TA; p.chunks = pl.chunks;
-  p.CC8 = pl.CC / cpu; p.C8A = pl.C8A; p.kg8 = pl.kg / cpu; p.stage_bytes = pl.stage_bytes; p.a_bytes = pl.a_bytes;
+  p.CC8 = pl.CC / cpu; p.C8A = pl.C8A; p.kg8 = ceil_div(pl.kg, cpu); p.stage_bytes = pl.stage_bytes; p.a_bytes = pl.a_bytes;
   p.a_box_bytes = pl.a_box_bytes; p.b_off = pl.b_off; p.st_mask = pl.nstage - 1; p.st_log2 = pl.st_log2;
   p.Wt = pl.Wt; p.TH = pl.TH; p.TB = pl.TB; p.wlo = pl.wlo; p.hlo = pl.hlo; p.col_tiles = pl.col_tiles; p.row_tiles = pl.row_tiles;
   p.n_mtiles = pl.n_mtiles;
   p.w_img = reinterpret_cast<const uint8_t*>(w_img);
   p.B = pl.B; p.THH = pl.THH; p.BW = pl.BW; p.OHr = pl.OHr; p.OWr = pl.OWr; p.OH = pl.OH; p.OW = pl.OW; p.omul = pl.omul; p.ny = pl.ny;
-  p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = ceil_div(pl.NOUT, cpu); p.smem_bytes = pl.smem_bytes; p.off_stg = pl.off_stg;
+  // units per position of the output-side planes: the STE mask of a data gradient is group-padded like its operand plane
+  p.ng = pl.ng; p.Nt = pl.Nt; p.NOUT = pl.NOUT; p.C8O = cpu == 8 ? pl.G * ceil_div(pl.ng, 8) : ceil_div(pl.NOUT, cpu); p.smem_bytes = pl.smem_bytes; p.off_stg = pl.off_stg;
   p.mode = mode;
   p.n_scale = n_scale; p.a_scale = a_scale; p.a_scale_const = a_scale_const; p.bias = bias; p.bits8 = bits8; p.gain = gain;
   p.out = out; p.err = err_flag; p.codes = codes; p.dec = dec;
@@ -2762,10 +2833,9 @@ extern "C" int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t 
   wfn<<<dim3(pl.G * pl.n_ktiles * pl.n_ctiles * pl.n_tg, pl.splits), kWgThreads, pl.smem_bytes, st>>>(tdy[0], tdy[1], tdy[2], tx[0],
                                                                                                      tx[1], tx[2], p);
   {
-    const int cout_o = pl.cout_g / pl.gm, cin_o = pl.cin_g / pl.gm;     // channels per original group
-    const dim3 rgrid(cin_o * pl.ntap, (cout_o + 127) / 128, pl.G * pl.gm);
-    wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, pl.gm, pl.n_ktiles, pl.n_ctiles, pl.ntap, pl.Nc, cout_o,
-                                            cin_o, a_scale, kdiv, dw);
+    const dim3 rgrid(pl.cin_o * pl.ntap, (pl.cout_o + 127) / 128, pl.G * pl.gm);
+    wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, pl.gm, pl.n_ktiles, pl.n_ctiles, pl.ntap, pl.Nc, pl.cout_o,
+                                            pl.cin_o, pl.cout_g / pl.gm, pl.cin_g / pl.gm, a_scale, kdiv, dw);
   }
   MNB_LAUNCHED(2);
   return 0;
@@ -2819,8 +2889,8 @@ extern "C" int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int
   cudaStream_t st = (cudaStream_t)stream;
   pk_wgrad_taps_kernel<<<dim3(pl.G, pl.splits), kWgtThreads, pl.smem_bytes, st>>>(tdy[0], tdy[1], tdy[2], tx[0], tx[1], tx[2], p);
   const dim3 rgrid(kTapsCin * kTapsN, 1, pl.G * kTapsGm);
-  wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, kTapsGm, 1, 1, kTapsN, pl.Nc, kTapsCout, kTapsCin, a_scale,
-                                          kdiv, dw);
+  wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, kTapsGm, 1, 1, kTapsN, pl.Nc, kTapsCout, kTapsCin, kTapsCout,
+                                          kTapsCin, a_scale, kdiv, dw);
   MNB_LAUNCHED(2);
   return 0;
 }

@@ -349,7 +349,8 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, p
     if prepacked is not None:
         x_pk, bits8 = prepacked, None      # the producer keeps the STE mask for its own backward
     else:
-        x_pk, bits8 = PK.pack_act(x, qp, ta, phase_split=sh.stride_h == 2, want_bits=need_dx, relu=pre_relu)
+        x_pk, bits8 = PK.pack_act(x, qp, ta, phase_split=sh.stride_h == 2, want_bits=need_dx, relu=pre_relu,
+                                  groups=sh.groups)
     w_img = PK.weight_image(sh, ta, tw, w_int=w_int, w_f32=None if w_int is not None else wq)
     # backward must see the forward-time scale (the reference clones it too); no clone needed without autograd
     a_scale, a_const = PK.act_scale(spec, clone=need_dx or need_dw)
@@ -374,8 +375,9 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, p
     ctx.pk_wg_scale = None
     if spec is not None:
         ctx.pk_wg_scale = a_scale if spec.mode == L.ACT_IAO else _dorefa_scale_tensor(spec.bits, x.device)
-    if spec is None and w_int is not None and need_dw:
-        # a fused BatchNorm + binarizer consuming y may write this layer's gradient operand itself (fused.BNSignFn)
+    if spec is None and w_int is not None and need_dw and not PK.padded(sh.out_c, sh.groups):
+        # a fused BatchNorm + binarizer consuming y may write this layer's gradient operand itself (fused.BNSignFn; plain
+        # planes only: a group-padded dy plane is packed here)
         y._mnb_pk_conv = (w_scale if need_dx else None, Tb)
     return True
 
@@ -392,11 +394,11 @@ def _pk_backward(ctx, dy):
     fold = int_w and need_dx
     pre = getattr(dy, "_mnb_pk_dy", None)     # written by the consumer's fused BatchNorm backward (fused.BNSignFn): dy holds no data
     if pre is not None:
-        if pre[1] != T or (pre[2] is not None) != fold:
+        if pre[1] != T or (pre[2] is not None) != fold or PK.padded(sh.out_c, sh.groups):
             raise RuntimeError("micronet_b200: packed gradient operand does not match this layer's backward configuration")
         dy_pk = pre[0]
     else:
-        dy_pk, _ = PK.pack_act(dy, None, T, ch_scale=ctx.w_scale if fold else None)
+        dy_pk, _ = PK.pack_act(dy, None, T, ch_scale=ctx.w_scale if fold else None, groups=sh.groups)
     dx = dwq = None
     if need_dx:
         tw = 1 if int_w else T
@@ -583,6 +585,7 @@ class QuantConv2dFn(Function):
     @staticmethod
     def forward(ctx, x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, no_grad=False,
                 codes_out=False):
+        from . import pk as PK
         L.require_cuda(x, wq)
         assert not (pre_relu and any(ctx.needs_input_grad)), "the folded ReLU is an inference-only fusion"
         x = x.contiguous()
@@ -595,9 +598,15 @@ class QuantConv2dFn(Function):
         pk_on = L.PK_MODE != "off"
         pm1 = x.dtype == torch.float32 and getattr(x, "_mnb_pm1", False)   # exactly +-1 (a binarizer's output)
         pm1_plane = getattr(x, "_mnb_pk_pm1", None)   # that +-1 tensor as the bf16 plane a fused BatchNorm + binarizer wrote
-        plane = pm1_plane if (pm1_plane is not None and pm1_plane.numel() == x.numel() * 2) else None
+        # producers write plain planes: a conv that reads a group-padded plane (pk.padded) packs its own
+        padded_in = PK.padded(sh.in_c, sh.groups)
+        plane = pm1_plane if (pm1_plane is not None and not padded_in and pm1_plane.numel() == x.numel() * 2) else None
         pkq = getattr(x, "_mnb_pk_q", None)   # operand plane written by a fused BN + ReLU + quantizer producer
+        if pkq is not None and padded_in:
+            raise RuntimeError("micronet_b200: a fused producer's packed output reached a conv that reads group-padded planes")
         plane_only = getattr(x, "_mnb_plane_only", False)
+        if plane_only and padded_in:
+            x, plane_only = materialized(x), False
         if (L.XNOR_MODE != "off" and spec is None and w_int is not None and pm1 and not pre_relu
                 and (no_grad or not any(ctx.needs_input_grad[:3])) and _xnor_forward(x, w_int, w_scale, bias, sh, y, groups)):
             family = "xnor"
@@ -612,8 +621,9 @@ class QuantConv2dFn(Function):
               # wbwtab layer behind a fused BatchNorm + binarizer: +-1 input (one exact bf16 piece).  With the producer's
               # plane the layer is pure TMA -> MMA; 3x3 layers win on the packed-operand family even when they pack
               # themselves (measured per layer, DESIGN.md 6).  Outside the cover: the round-1 fused kernels below.
+              # Group-padded layers (no producer plane, no round-1 cover) take it too
               or (L.PK_WBWTAB and pk_on and spec is None and w_int is not None and pm1
-                  and (pm1_plane is not None or sh.ker_h * sh.ker_w > 1)
+                  and (pm1_plane is not None or sh.ker_h * sh.ker_w > 1 or padded_in)
                   and _pk_forward(ctx, x, wq, bias, w_int, w_scale, None, sh, y, prepacked=plane, pm1=True,
                                   codes_out=codes_out))
               # un-quantized conv behind a binarizer (the 10-way head of a wbwtab model, fused.EnginePmConv2d): the +-1
@@ -687,7 +697,8 @@ def _pk_plain(sh, mode, a, w, out, T):
     """fp32 x fp32 convolution (mode 0) / data gradient (mode 1) of shape ``sh`` on the packed-operand tensor-core family:
     both operands as T exact bf16 pieces.  False when the shape is outside its cover."""
     from . import pk as PK
-    if L.PK_MODE == "off" or not PK.supported(sh, mode, T, T):
+    # (group-padded shapes keep the generic kernels here: the transposed conv's planes are not packed group-padded)
+    if L.PK_MODE == "off" or PK.padded_conv(sh) or not PK.supported(sh, mode, T, T):
         return False
     a_pk, _ = PK.pack_act(a, None, T, phase_split=(mode == 0 and sh.stride_h == 2))
     w_img = PK.pack_weight(sh, mode, T, T, w_f32=w)
@@ -752,7 +763,7 @@ class ConvTranspose2dFn(Function):
         if ctx.needs_input_grad[1]:
             gw = torch.empty_like(w)
             done = False
-            if L.PK_MODE != "off" and PK.wgrad_supported(sh, T, T):
+            if L.PK_MODE != "off" and not PK.padded_conv(sh) and PK.wgrad_supported(sh, T, T):
                 x_pk, _ = PK.pack_act(x, None, T)                                   # S's output-gradient operand
                 g_pk, _ = PK.pack_act(gy, None, T, phase_split=sh.stride_h == 2)    # S's input operand
                 rc = _timed("wgrad_pk", sh, lambda: PK.wgrad(sh, x_pk, T, g_pk, T, gw))
@@ -829,6 +840,8 @@ class Consumer:
             return False
         if act_shape[1] != self.w_shape[1] * self.groups:
             return False
+        if PK.padded(act_shape[1], self.groups):     # producers write plain planes; this conv reads a group-padded one
+            return False
         sh = _shape_struct(act_shape, self.w_shape, self.stride, self.padding, self.dilation, self.groups)
         if sh.stride_h == 2 and ((act_shape[2] | act_shape[3]) & 1):
             return False
@@ -896,8 +909,9 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
         return _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_relu, consumer if hand else None)
     ta, tw = _pk_terms(spec, w_int)
     # a segmented producer plan (two level pieces of an asymmetric quantizer) takes no fused consumer: the consumer packs
-    # its own operand from y
-    fused = cfmt == "bf16" and not PK.segmented(sh, 0, ta, tw)
+    # its own operand from y.  Nor does a grouped producer with output channels per group % 8 != 0 (mnb_pk_conv_post stores
+    # whole octets of a group)
+    fused = cfmt == "bf16" and not PK.segmented(sh, 0, ta, tw) and not PK.padded(sh.out_c, groups)
     if (plane is None and not fused) or spec is None or w_int is None or L.PK_MODE == "off" or not PK.supported(sh, 0, ta, tw):
         if plane is not None:
             raise RuntimeError("micronet_b200: handed-over plane in front of a conv outside the packed-operand cover")
@@ -905,7 +919,7 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
     dev = wq.device
     if plane is None:
         L.require_cuda(x, wq)
-        plane, _ = PK.pack_act(x.contiguous(), spec.struct(), ta, phase_split=sh.stride_h == 2, relu=pre_relu)
+        plane, _ = PK.pack_act(x.contiguous(), spec.struct(), ta, phase_split=sh.stride_h == 2, relu=pre_relu, groups=groups)
     w_img = PK.weight_image(sh, ta, tw, w_int=w_int)
     a_scale, a_const = PK.act_scale(spec)
     if not fused:

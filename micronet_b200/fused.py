@@ -27,6 +27,7 @@ import ctypes as C
 import torch.nn.functional as TF
 
 from . import _lib as L
+from . import pk as PK
 
 
 def _xargs(lib, name, x, codes):
@@ -519,6 +520,8 @@ def _fuse_dorefa_producers(module: nn.Module):
         a_bits = int(conv.activation_quantizer.a_bits) if isinstance(conv, DorefaConv) else 0
         if not (2 <= a_bits <= 8) or conv.in_channels % 8 or tuple(conv.stride) != (1, 1) or conv.quant_inference:
             continue
+        if PK.padded(conv.in_channels, conv.groups):     # the producer writes a plain plane, the conv reads a group-padded one
+            continue
         if not hasattr(prev, "channel_shuffle_flag"):
             continue
         names = [n for n, k in prev.named_children() if not isinstance(k, nn.Identity)]
@@ -553,7 +556,7 @@ def _mark_plane_only(module: nn.Module):
         prod, conv = _tail_producer(prev), _first_conv(nxt)
         if not isinstance(prod, BatchNormBinarize2d) or prod.pool2 or conv is None:
             continue
-        if getattr(nxt, "channel_shuffle_flag", 0) or conv.in_channels % 8:
+        if getattr(nxt, "channel_shuffle_flag", 0) or conv.in_channels % 8 or PK.padded(conv.in_channels, conv.groups):
             continue
         if isinstance(conv, WbConv):
             ok = conv.weight_quantizer.W in (2, 3) and not conv.quant_inference

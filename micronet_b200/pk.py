@@ -55,18 +55,35 @@ def wgrad_supported(sh, terms_dy, terms_x):
     return _plan_cache[k] >= 0
 
 
-def pack_act(x, qp, terms, ch_scale=None, phase_split=False, want_bits=False, relu=False):
-    """-> (planes u8[terms * B * ceil(C/8) * H * W * 16], bits8 u8[B, ceil(C/8), H, W] or None)"""
+def padded(channels, groups):
+    """is the operand plane of a grouped conv reading ``channels`` channels group-padded (DESIGN.md 4.17)?  Then its
+    layout differs from a plain plane of the same tensor, and no plane in the plain layout may be handed to that conv."""
+    return groups > 1 and (channels // groups) % 8 != 0
+
+
+def padded_conv(sh):
+    """does any operand plane of conv ``sh`` (x: input channels per group, dy: output channels per group) use the padded layout?"""
+    return padded(sh.in_c, sh.groups) or padded(sh.out_c, sh.groups)
+
+
+def pack_act(x, qp, terms, ch_scale=None, phase_split=False, want_bits=False, relu=False, groups=1):
+    """-> (planes u8[terms * B * ceil(C/8) * H * W * 16], bits8 u8[B, ceil(C/8), H, W] or None).  ``groups``: the plane is the
+    operand of a grouped conv; group-padded (mnb_pk_pack_act_grouped) where C / groups % 8 != 0, the plain plane otherwise."""
     lib = L.load()
     b, c, h, w = x.shape
-    nbytes = int(lib.mnb_pk_act_bytes(b, c, h, w, terms))
+    pad = padded(c, groups)
+    c8 = groups * ((c // groups + 7) // 8) if pad else (c + 7) // 8
+    nbytes = int(lib.mnb_pk_grouped_act_bytes(b, c, h, w, terms, groups) if pad else lib.mnb_pk_act_bytes(b, c, h, w, terms))
     out = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
     bits = None
     if qp is not None and want_bits:
-        bits = torch.empty((b, (c + 7) // 8, h, w), dtype=torch.uint8, device=x.device)
-    L.check(lib.mnb_pk_pack_act_relu(x.data_ptr(), b, c, h, w, None if qp is None else C.byref(qp), terms, L.ptr(ch_scale),
-                                     1 if phase_split else 0, 1 if relu else 0, out.data_ptr(), L.ptr(bits), L.stream()),
-            "pk_pack_act")
+        bits = torch.empty((b, c8, h, w), dtype=torch.uint8, device=x.device)
+    args = (x.data_ptr(), b, c, h, w, None if qp is None else C.byref(qp), terms, L.ptr(ch_scale), 1 if phase_split else 0,
+            1 if relu else 0, out.data_ptr(), L.ptr(bits))
+    if pad:
+        L.check(lib.mnb_pk_pack_act_grouped(*args, groups, L.stream()), "pk_pack_act_grouped")
+    else:
+        L.check(lib.mnb_pk_pack_act_relu(*args, L.stream()), "pk_pack_act")
     return out, bits
 
 
