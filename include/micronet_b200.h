@@ -295,7 +295,22 @@ int mnb_bn_sign_fwd_packed(const float* x, int32_t batch, int32_t channels, int3
 int mnb_fconv2d_plan(const mnb_conv_shape* s, int32_t wgrad, int32_t* out, int32_t n);
 int mnb_fconv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const float* w, const float* bias, float* y,
                        int32_t* err_flag, mnb_stream_t stream);
+/* mnb_fconv2d_fwd_wg: the same forward on two MMA warpgroups, 64-position tiles and one MMA over all output channels;
+ * bit for bit mnb_fconv2d_fwd_tc's y.  Cover: that of mnb_fconv2d_fwd_tc with W <= 64, Cout > 128, where 3 im2col
+ * buffers fit in shared memory (the 3 -> 192 / 256 5x5 stems at 32 x 32); anything else returns MNB_E_UNSUPPORTED before
+ * any launch.
+ *   mnb_fconv2d_wg_plan: host only, its plan in the fields of mnb_fconv2d_plan (TH: rows per 64-position tile, NP: the MMA
+ *                        width 192 or 256, nbuf_a: im2col buffers).                                                          */
+int mnb_fconv2d_wg_plan(const mnb_conv_shape* s, int32_t* out, int32_t n);
+int mnb_fconv2d_fwd_wg(const mnb_conv_shape* s, const float* x, const float* w, const float* bias, float* y,
+                       int32_t* err_flag, mnb_stream_t stream);
 int64_t mnb_fconv2d_wgrad_tc_scratch_bytes(const mnb_conv_shape* s);
+/* mnb_fconv2d_wgrad_wg: the same weight gradient on two MMA warpgroups with the running sums in registers; bit for bit
+ * mnb_fconv2d_wgrad_tc's dw (same plan, partials and reduction).  Cover: that of mnb_fconv2d_wgrad_tc with 65 <= C*R*S <= 80
+ * and Cout > 128 (the 3 -> 192 / 256 5x5 stems); scratch >= mnb_fconv2d_wgrad_wg_scratch_bytes(s) (-1: unsupported).                          */
+int64_t mnb_fconv2d_wgrad_wg_scratch_bytes(const mnb_conv_shape* s);
+int mnb_fconv2d_wgrad_wg(const mnb_conv_shape* s, const float* dy, const float* x, float* dw, void* scratch,
+                         int32_t* err_flag, mnb_stream_t stream);
 int mnb_fconv2d_wgrad_tc(const mnb_conv_shape* s, const float* dy, const float* x, float* dw, void* scratch,
                          int32_t* err_flag, mnb_stream_t stream);
 

@@ -93,8 +93,12 @@ PROTOTYPES = {
     "mnb_bn_sign_fwd_packed": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
     "mnb_fconv2d_plan": (C.c_int, [_SHAPE, _I, _P, _I]),
     "mnb_fconv2d_fwd_tc": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),
+    "mnb_fconv2d_wg_plan": (C.c_int, [_SHAPE, _P, _I]),
+    "mnb_fconv2d_fwd_wg": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),
     "mnb_fconv2d_wgrad_tc_scratch_bytes": (_L, [_SHAPE]),
     "mnb_fconv2d_wgrad_tc": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),
+    "mnb_fconv2d_wgrad_wg_scratch_bytes": (_L, [_SHAPE]),
+    "mnb_fconv2d_wgrad_wg": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P]),
     "mnb_maxpool2d_fwd": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "mnb_maxpool2d_bwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "mnb_adam_step": (C.c_int, [_P, _P, _P, _P, _L, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _I, _P]),

@@ -92,24 +92,26 @@ __device__ __forceinline__ float patch_element(const Params& p, int i, int b, in
   const int h = h0 - p.pad + pr, w = pc - p.pad;
   return (h >= 0 && h < p.H && w >= 0 && w < p.W) ? __ldg(p.x + (((int64_t)b * p.C + c) * p.H + h) * p.W + w) : 0.f;
 }
-__device__ __forceinline__ void patch_fetch(const Params& p, int tile, int ct, int nconv, float (&v)[PF]) {
+template <int NPF = PF>
+__device__ __forceinline__ void patch_fetch(const Params& p, int tile, int ct, int nconv, float (&v)[NPF]) {
   const int b = tile / p.tiles_per_img, h0 = (tile - b * p.tiles_per_img) * p.TH;
   const int n = p.C * p.PH * p.PW;
 #pragma unroll
-  for (int k = 0; k < PF; ++k) {
+  for (int k = 0; k < NPF; ++k) {
     const int i = ct + k * nconv;
     v[k] = i < n ? patch_element(p, i, b, h0) : 0.f;
   }
 }
-__device__ __forceinline__ void patch_commit(const Params& p, float* patch, int tile, int ct, int nconv, const float (&v)[PF]) {
+template <int NPF = PF>
+__device__ __forceinline__ void patch_commit(const Params& p, float* patch, int tile, int ct, int nconv, const float (&v)[NPF]) {
   const int b = tile / p.tiles_per_img, h0 = (tile - b * p.tiles_per_img) * p.TH;
   const int n = p.C * p.PH * p.PW;
 #pragma unroll
-  for (int k = 0; k < PF; ++k) {
+  for (int k = 0; k < NPF; ++k) {
     const int i = ct + k * nconv;
     if (i < n) patch[i] = v[k];
   }
-  for (int i = ct + PF * nconv; i < n; i += nconv) patch[i] = patch_element(p, i, b, h0);
+  for (int i = ct + NPF * nconv; i < n; i += nconv) patch[i] = patch_element(p, i, b, h0);
 }
 
 // ------------------------------------------------------------------------------------------------ forward
@@ -504,7 +506,393 @@ static int plan(const mnb_conv_shape* s, bool wgrad, Params& p, int& smem_bytes)
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ forward, two MMA warpgroups
+// fwd_kernel runs a 128-position tile as 8 slabs of 32 channels on one warpgroup (MMA, wait, staging epilogue, one after
+// another), and at the bench stems only one im2col buffer fits next to its weight image.  Here a tile is 64 positions and
+// one m64nN MMA spans every output channel (N = Cout rounded up to 192 or 256), so A is read once per K-step
+// instead of once per slab; two MMA warpgroups take alternate tiles, so one runs its epilogue while the other issues MMAs,
+// and 3..4 im2col buffers let the converters build tile t + 2 meanwhile.  The epilogue stores straight from the fragment:
+// the 8 row-lanes of a column are 8 consecutive positions of one channel, whole 32-byte sectors of y.
+// Every output element sees fwd_kernel's chain: a zeroed accumulator, the kProdA / kProdB products in order with the
+// same K-steps over the same split3_pair pieces (zero beyond KR and Cout), then + bias in fp32.  An MMA's result for one
+// element does not depend on the N width or the 64-row block it is issued with (DESIGN.md 4.9), so y is bit for bit
+// fwd_kernel's.  The plan never covers a shape fwd_kernel refuses.
+// Measured on an H100 SXM (700 W), batch 256, 32 x 32: 3 -> 256 5x5 252 -> 164 us, 3 -> 192 5x5 194 -> 135 us per launch.
+constexpr int FWG_THREADS = 384;   // warpgroup 0: im2col converters; warpgroups 1, 2: MMA + epilogue on alternate tiles
+constexpr int FWG_NCONV = 128;
+constexpr int FWG_PF = 6;          // FWG_PF * FWG_NCONV >= the bench stems' 648-float patch: no element waits on its load
+constexpr int FWG_MAXBUF = 4;
+constexpr int FWG_CONV_REGS = 56, FWG_MMA_REGS = 224;   // 128 * 56 + 256 * 224 <= 65536 (m64n256: 128 accumulators)
+
+struct alignas(16) FwgShared {
+  uint64_t full[FWG_MAXBUF], empty[FWG_MAXBUF];
+  uint32_t abort;
+};
+
+template <int N>
+__global__ void __launch_bounds__(FWG_THREADS, 1) fwd_wg_kernel(const Params p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ FwgShared sh;
+  __shared__ __align__(16) float epi_bias[N];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint8_t* bop = smem + p.off_b;
+  uint8_t* aop = smem + p.off_a;
+  int* tab = reinterpret_cast<int*>(smem + p.off_tab);
+  const int kchunks = p.KP / 8;
+
+  if (tid == 0) {
+    for (int i = 0; i < FWG_MAXBUF; ++i) {
+      tc::mbar_init(&sh.full[i], FWG_NCONV / 32); tc::mbar_init(&sh.empty[i], 4);
+    }
+    sh.abort = 0;
+    tc::fence_barrier_init();
+  }
+  for (int n = tid; n < N; n += FWG_THREADS) epi_bias[n] = (p.bias && n < p.K) ? __ldg(p.bias + n) : 0.f;
+  // resident B operand, as in fwd_kernel with NP = N
+  for (int i = tid; i < kchunks * N; i += FWG_THREADS) {
+    const int j = i / N, n = i - j * N;
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int kk = j * 8 + e;
+      v[e] = (n < p.K && kk < p.KR) ? __ldg(p.w + (int64_t)n * p.KR + kk) : 0.f;
+    }
+    store_split8(v, bop + (size_t)i * 16, p.b_term_bytes);
+  }
+  for (int kk = tid; kk < p.KP; kk += FWG_THREADS) {
+    int off = -1;
+    if (kk < p.KR) {
+      const int s = kk % p.R, t = kk / p.R;
+      const int r = t % p.R, c = t / p.R;
+      off = (c * p.PH + r) * p.PW + s;
+    }
+    tab[kk] = off;
+  }
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+  // local tile t of this CTA = tile blockIdx.x + t * gridDim.x, im2col buffer t % nbuf_a, MMA warpgroup t % 2
+  const int n_local = (int)blockIdx.x < p.n_tiles ? (p.n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+
+  if (warp < FWG_NCONV / 32) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(FWG_CONV_REGS));
+    // ================================================================= converters: patch -> im2col A operand
+    const int ct = tid;
+    float* patch0 = reinterpret_cast<float*>(smem + p.off_patch);
+    const int items = 64 * kchunks;
+    const int patch_floats = p.patch_bytes / 4;
+    float pre[FWG_PF];
+    if (n_local > 0) {
+      patch_fetch(p, blockIdx.x, ct, FWG_NCONV, pre);
+      patch_commit(p, patch0, blockIdx.x, ct, FWG_NCONV, pre);
+    }
+    for (int t = 0; t < n_local; ++t) {
+      const int tile = (int)blockIdx.x + t * (int)gridDim.x;
+      const float* patch = patch0 + (size_t)(t & 1) * patch_floats;
+      conv_bar_sync(FWG_NCONV);   // every converter committed its part of this tile's patch
+      const int next = tile + (int)gridDim.x;
+      if (next < p.n_tiles) patch_fetch(p, next, ct, FWG_NCONV, pre);
+      const int ab = t % p.nbuf_a;
+      const uint32_t aph = (uint32_t)(t / p.nbuf_a) & 1u;
+      if (!tc::mbar_wait(&sh.empty[ab], aph ^ 1u, p.err, 506)) break;
+      uint8_t* abuf = aop + (size_t)ab * p.a_buf_bytes;
+      for (int i = ct; i < items; i += FWG_NCONV) {
+        const int j = i >> 6, m = i & 63;
+        const int base = (m / p.W) * p.PW + (m % p.W);
+        int off[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) off[e] = tab[j * 8 + e];
+        float v[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = off[e] >= 0 ? patch[off[e] + base] : 0.f;
+        store_split8(v, abuf + (size_t)i * 16, p.a_term_bytes);
+      }
+      tc::fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&sh.full[ab]);
+      if (next < p.n_tiles) patch_commit(p, patch0 + (size_t)((t + 1) & 1) * patch_floats, next, ct, FWG_NCONV, pre);
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(FWG_MMA_REGS));
+    // ================================================================= MMA warpgroups: wgmma -> + bias -> y (NCHW)
+    const int wg = (warp - FWG_NCONV / 32) >> 2, w4 = warp & 3;
+    const int64_t plane = (int64_t)p.H * p.W;
+    const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(aop), 64u * 16u, 128u);
+    const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(bop), (uint32_t)N * 16u, 128u);
+    const uint32_t a_term16 = (uint32_t)p.a_term_bytes >> 4, b_term16 = (uint32_t)p.b_term_bytes >> 4;
+    const uint32_t a_buf16 = (uint32_t)p.a_buf_bytes >> 4;
+    const uint32_t a_step16 = 2u * 64u, b_step16 = 2u * (uint32_t)N;   // one K16 step = two 8-wide chunks
+    const int ksteps = p.KP / 16;
+    // fragment: acc[4j + 2i + c] = D[row 16 w4 + lane / 4 + 8i][column 8j + 2 (lane % 4) + c]
+    const int fr = 16 * w4 + (lane >> 2), fc = 2 * (lane & 3);
+    for (int t = wg; t < n_local; t += 2) {
+      const int tile = (int)blockIdx.x + t * (int)gridDim.x;
+      const int ab = t % p.nbuf_a;
+      tc::mbar_wait_soft(&sh.full[ab], (uint32_t)(t / p.nbuf_a) & 1u, p.err, 505, &sh.abort);
+      float acc[N / 2];
+      tc::zero_acc(acc);
+      tc::wg_fence();
+      tc::fence_acc(acc);
+#pragma unroll
+      for (int q = 0; q < 6; ++q) {
+        const uint64_t aq = a_desc0 + (uint64_t)((uint32_t)ab * a_buf16 + (uint32_t)kProdA[q] * a_term16);
+        const uint64_t bq = b_desc0 + (uint64_t)((uint32_t)kProdB[q] * b_term16);
+        for (int ks = 0; ks < ksteps; ++ks)
+          tc::Mma<N>::template bf16<0, 0>(acc, aq + (uint64_t)((uint32_t)ks * a_step16), bq + (uint64_t)((uint32_t)ks * b_step16), 1);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&sh.empty[ab]);   // the tile's MMAs retired: its operand buffer is free
+      const int b = tile / p.tiles_per_img, h0 = (tile - b * p.tiles_per_img) * p.TH;
+      float* dst = p.y + (int64_t)b * p.K * plane + (int64_t)h0 * p.W + fr;
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) {
+        const int n = 8 * j + fc;
+        const float2 bs = *reinterpret_cast<const float2*>(&epi_bias[n]);
+        float* o = dst + (int64_t)n * plane;
+        if (n < p.K) { o[0] = __fadd_rn(acc[4 * j], bs.x); o[8] = __fadd_rn(acc[4 * j + 2], bs.x); }
+        if (n + 1 < p.K) { o[plane] = __fadd_rn(acc[4 * j + 1], bs.y); o[plane + 8] = __fadd_rn(acc[4 * j + 3], bs.y); }
+      }
+    }
+  }
+  __syncthreads();
+}
+
 static int grid_size(const Params& p) { return std::max(1, std::min(p.n_tiles, MNB_NUM_SMS)); }
+
+// plan of fwd_wg_kernel: fwd_kernel's cover (whose checks it runs first) where a 64-position tile holds whole rows
+// (W <= 64) and at least 3 im2col buffers fit next to the weight image
+static int plan_wg(const mnb_conv_shape* s, Params& p, int& smem_bytes) {
+  if (int e = plan(s, false, p, smem_bytes)) return e;
+  auto unsupported = [](const char* why) { return mnb_fail(MNB_E_UNSUPPORTED, "fp32 tc conv (two warpgroups): %s", why); };
+  if (64 % p.W) return unsupported("image rows do not tile into 64 positions");
+  // at narrow N a tile's MMAs are too short to hide the converters and the epilogue: the 3 -> 64 stem measured slower
+  if (p.K <= 128) return unsupported("128 output channels or fewer");
+  p.TH = 64 / p.W;
+  p.PH = p.TH + 2 * p.pad;
+  p.tiles_per_img = p.H / p.TH;
+  p.n_tiles = p.B * p.tiles_per_img;
+  p.patch_bytes = (p.C * p.PH * p.PW * 4 + 8 * 4 + 15) / 16 * 16;
+  p.NP = p.K <= 192 ? 192 : 256;
+  const int kchunks = p.KP / 8;
+  p.b_term_bytes = kchunks * p.NP * 16;
+  p.a_term_bytes = kchunks * 64 * 16;
+  p.a_buf_bytes = 3 * p.a_term_bytes;
+  p.off_b = 0;
+  p.off_a = 3 * p.b_term_bytes;
+  for (p.nbuf_a = FWG_MAXBUF; p.nbuf_a >= 3; --p.nbuf_a) {
+    p.off_patch = p.off_a + p.nbuf_a * p.a_buf_bytes;
+    p.off_tab = p.off_patch + 2 * p.patch_bytes;
+    smem_bytes = p.off_tab + p.KP * 4;
+    if (smem_bytes <= kMaxDynSmem) break;
+  }
+  if (p.nbuf_a < 3) return unsupported("shared memory budget (3 im2col buffers)");
+  return 0;
+}
+
+template <int N>
+static int launch_fwd_wg(const Params& p, int smem_bytes, mnb_stream_t stream) {
+  static bool attr_set = false;   // one per instantiation
+  if (!attr_set) {
+    cudaError_t ce = cudaFuncSetAttribute(fwd_wg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+    if (ce != cudaSuccess) return mnb_fail((int)ce, "cudaFuncSetAttribute: %s", cudaGetErrorString(ce));
+    attr_set = true;
+  }
+  fwd_wg_kernel<N><<<grid_size(p), FWG_THREADS, smem_bytes, (cudaStream_t)stream>>>(p);
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ weight gradient, two MMA warpgroups
+// wgrad_kernel issues m64n32 over KP = 80 in three slabs (96 columns for 80), waits after every 24 MMAs and then adds each
+// fragment into a running sum in shared memory (4-way bank conflicts on every read and write).  Here two MMA warpgroups
+// each own every other 64-channel block (blocks wg, wg + 2) and one m64nKP MMA spans all im2col columns; the running sums
+// stay in registers (a (channel, kk) element lives in the same thread of the same fragment for the whole launch), and a
+// ring of 3 dy / Xcol stages lets warpgroup 0 convert two steps ahead.
+// Bit identity with wgrad_kernel: the same plan (tiles, grid, CTA i takes tiles i, i + grid, ...), the same 32-position
+// steps in order, per step and element one 12-MMA chain (kProdA / kProdB order, 2 K-steps each) from a zeroed
+// accumulator added with __fadd_rn into a running sum that starts at 0, one partial per CTA, reduce_partials_kernel.
+constexpr int WWG_THREADS = 384;   // warpgroup 0: converters (dy split + im2col of x); warpgroups 1, 2: MMA
+constexpr int WWG_NCONV = 128;
+constexpr int WWG_DMAX = 8;        // dy items (channel, 8 positions) per converter and step: 4 * Cout <= 8 * 128
+constexpr int WWG_NBUF = 3;
+constexpr int WWG_KP = 80;         // the 3 x 5 x 5 stems
+
+template <int KP>
+__global__ void __launch_bounds__(WWG_THREADS, 1) wgrad_wg_kernel(const Params p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ FwgShared sh;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint8_t* bop = smem + p.off_b;   // Xcol^T : [buf][piece][pos / 8][kk][8 pos]
+  uint8_t* aop = smem + p.off_a;   // dy     : [buf][piece][pos / 8][channel][8 pos]
+  int* tab = reinterpret_cast<int*>(smem + p.off_tab);
+  const int nsub = 128 / SUB;
+  const int b_buf_bytes = 3 * p.b_term_bytes;
+
+  if (tid == 0) {
+    for (int i = 0; i < WWG_NBUF; ++i) {
+      tc::mbar_init(&sh.full[i], WWG_NCONV / 32); tc::mbar_init(&sh.empty[i], 8);
+    }
+    sh.abort = 0;
+    tc::fence_barrier_init();
+  }
+  // operand buffers start as zeros: channel rows >= Cout and im2col rows >= KR are never written
+  for (int i = tid; i < WWG_NBUF * (p.a_buf_bytes + b_buf_bytes) / 16; i += WWG_THREADS)
+    reinterpret_cast<uint4*>(smem + p.off_b)[i] = make_uint4(0, 0, 0, 0);
+  for (int kk = tid; kk < p.KP; kk += WWG_THREADS) {
+    int off = -1;
+    if (kk < p.KR) {
+      const int s = kk % p.R, t = kk / p.R;
+      const int r = t % p.R, c = t / p.R;
+      off = (c * p.PH + r) * p.PW + s;
+    }
+    tab[kk] = off;
+  }
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+
+  if (warp >= 4) {
+    // ================================================================= MMA warpgroups: wgmma -> register running sums -> partial dw
+    const int wg = (warp - 4) >> 2, w4 = warp & 3;
+    const uint64_t a_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(aop), (uint32_t)p.NP * 16u, 128u);
+    const uint64_t b_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(bop), (uint32_t)KP * 16u, 128u);
+    const uint32_t a_term16 = (uint32_t)p.a_term_bytes >> 4, b_term16 = (uint32_t)p.b_term_bytes >> 4;
+    const uint32_t a_buf16 = (uint32_t)p.a_buf_bytes >> 4, b_buf16 = (uint32_t)b_buf_bytes >> 4;
+    const uint32_t a_step16 = 2u * (uint32_t)p.NP, b_step16 = 2u * (uint32_t)KP;
+    float sum0[KP / 2], sum1[KP / 2];   // blocks wg, wg + 2
+    tc::zero_acc(sum0); tc::zero_acc(sum1);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+      for (int sub = 0; sub < nsub; ++sub, ++it) {
+        const uint32_t ob = it % WWG_NBUF, oph = (it / WWG_NBUF) & 1u;
+        tc::mbar_wait_soft(&sh.full[ob], oph, p.err, 515, &sh.abort);
+#pragma unroll 1
+        for (int mb = 0; mb < 2; ++mb) {   // 64-channel blocks wg, wg + 2; rolled: two chains in one block serialise the wgmma
+          float acc[KP / 2];
+          tc::zero_acc(acc);
+          tc::wg_fence();
+          tc::fence_acc(acc);
+#pragma unroll
+          for (int q = 0; q < 6; ++q) {
+            const uint64_t aq = a_desc0 + (uint64_t)(ob * a_buf16 + (uint32_t)kProdA[q] * a_term16 + (uint32_t)(wg + 2 * mb) * 64u);
+            const uint64_t bq = b_desc0 + (uint64_t)(ob * b_buf16 + (uint32_t)kProdB[q] * b_term16);
+#pragma unroll
+            for (int ks = 0; ks < SUB / 16; ++ks)
+              tc::Mma<KP>::template bf16<0, 0>(acc, aq + (uint64_t)((uint32_t)ks * a_step16), bq + (uint64_t)((uint32_t)ks * b_step16), 1);
+          }
+          tc::wg_commit();
+          tc::wg_wait<0>();
+          tc::fence_acc(acc);
+#pragma unroll
+          for (int i = 0; i < KP / 2; ++i) {
+            if (mb == 0) sum0[i] = __fadd_rn(sum0[i], acc[i]);
+            else sum1[i] = __fadd_rn(sum1[i], acc[i]);
+          }
+        }
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&sh.empty[ob]);
+      }
+    }
+    // fragment: sum[mb][4j + 2i + c] = dw[channel 64 (wg + 2 mb) + 16 w4 + lane / 4 + 8i][kk 8j + 2 (lane % 4) + c]
+    float* mine = p.partial + (int64_t)blockIdx.x * p.K * p.KR;
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+      for (int e = 0; e < KP / 2; ++e) {
+        const int n = 64 * (wg + 2 * mb) + 16 * w4 + (lane >> 2) + 8 * ((e >> 1) & 1);
+        const int kk = 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
+        if (n < p.K && kk < p.KR) mine[(int64_t)n * p.KR + kk] = mb == 0 ? sum0[e] : sum1[e];
+      }
+    }
+  } else {
+    // ================================================================= converters: wgrad_kernel's, with each step's dy loaded
+    // when the step starts (a register copy of the next step's dy does not fit next to it): the ring runs them ahead
+    const int ct = tid;
+    float* patch0 = reinterpret_cast<float*>(smem + p.off_patch);
+    const int64_t plane = (int64_t)p.H * p.W;
+    const int d_items = p.K * (SUB / 8), x_items = p.KR * (SUB / 8);
+    const int patch_floats = p.patch_bytes / 4;
+    float4 dpre[WWG_DMAX][2];
+    auto fetch_dy = [&](int tile, int sub) {
+      const int b = tile / p.tiles_per_img, h0 = (tile - b * p.tiles_per_img) * p.TH;
+      const float* dy_tile = p.dy + (int64_t)b * p.K * plane + (int64_t)h0 * p.W + sub * SUB;
+#pragma unroll
+      for (int k = 0; k < WWG_DMAX; ++k) {
+        const int i = ct + k * WWG_NCONV;
+        if (i < d_items) {
+          const int n = i / (SUB / 8), j = i - n * (SUB / 8);
+          const float4* src = reinterpret_cast<const float4*>(dy_tile + (int64_t)n * plane + j * 8);
+          dpre[k][0] = __ldg(src); dpre[k][1] = __ldg(src + 1);
+        }
+      }
+    };
+    float pre[PF];
+    if ((int)blockIdx.x < p.n_tiles) {
+      patch_fetch(p, blockIdx.x, ct, WWG_NCONV, pre);
+      patch_commit(p, patch0, blockIdx.x, ct, WWG_NCONV, pre);
+    }
+    uint32_t it = 0, t = 0;
+    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x, ++t) {
+      const float* patch = patch0 + (size_t)(t & 1u) * patch_floats;
+      conv_bar_sync(WWG_NCONV);
+      const int next = tile + (int)gridDim.x;
+      if (next < p.n_tiles) patch_fetch(p, next, ct, WWG_NCONV, pre);
+      for (int sub = 0; sub < nsub; ++sub, ++it) {
+        const uint32_t ob = it % WWG_NBUF, oph = (it / WWG_NBUF) & 1u;
+        fetch_dy(tile, sub);
+        const auto& dcur = dpre;
+        if (!tc::mbar_wait(&sh.empty[ob], oph ^ 1u, p.err, 516)) goto done;
+        uint8_t* abuf = aop + (size_t)ob * p.a_buf_bytes;
+        uint8_t* bbuf = bop + (size_t)ob * b_buf_bytes;
+#pragma unroll
+        for (int k = 0; k < WWG_DMAX; ++k) {
+          const int i = ct + k * WWG_NCONV;
+          if (i < d_items) {
+            const int n = i / (SUB / 8), j = i - n * (SUB / 8);
+            const float v[8] = {dcur[k][0].x, dcur[k][0].y, dcur[k][0].z, dcur[k][0].w,
+                                dcur[k][1].x, dcur[k][1].y, dcur[k][1].z, dcur[k][1].w};
+            store_split8(v, abuf + ((size_t)j * p.NP + n) * 16, p.a_term_bytes);
+          }
+        }
+        for (int i = ct; i < x_items; i += WWG_NCONV) {
+          const int kk = i / (SUB / 8), j = i - kk * (SUB / 8);
+          const int m = sub * SUB + j * 8;
+          const float* src = patch + tab[kk] + (m / p.W) * p.PW + (m % p.W);
+          float v[8];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[e] = src[e];
+          store_split8(v, bbuf + ((size_t)j * KP + kk) * 16, p.b_term_bytes);
+        }
+        tc::fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&sh.full[ob]);
+      }
+      if (next < p.n_tiles) patch_commit(p, patch0 + (size_t)((t + 1) & 1u) * patch_floats, next, ct, WWG_NCONV, pre);
+    }
+  }
+done:
+  __syncthreads();
+}
+
+// plan of wgrad_wg_kernel: wgrad_kernel's plan (whose tiles, grid and partials it keeps) at KP = 80 and 129..256 output
+// channels (four 64-channel blocks, two per MMA warpgroup: a branch around a block would serialise the wgmma), with a ring of 3
+// stages in place of 2 stages and the shared-memory running sum
+static int plan_wgrad_wg(const mnb_conv_shape* s, Params& p, int& smem_bytes) {
+  if (int e = plan(s, true, p, smem_bytes)) return e;
+  if (p.KP != WWG_KP) return mnb_fail(MNB_E_UNSUPPORTED, "fp32 tc wgrad (two warpgroups): C*R*S not in 65..80");
+  if (p.NP != 256) return mnb_fail(MNB_E_UNSUPPORTED, "fp32 tc wgrad (two warpgroups): 128 output channels or fewer");
+  p.off_b = 0;
+  p.off_a = WWG_NBUF * 3 * p.b_term_bytes;
+  p.off_patch = p.off_a + WWG_NBUF * p.a_buf_bytes;
+  p.off_tab = p.off_patch + 2 * p.patch_bytes;
+  p.sum_bytes = 0;
+  p.nbuf_a = WWG_NBUF;
+  smem_bytes = p.off_tab + p.KP * 4;
+  if (smem_bytes > kMaxDynSmem) return mnb_fail(MNB_E_UNSUPPORTED, "fp32 tc wgrad (two warpgroups): shared memory budget");
+  return 0;
+}
+
 static int debug_mask() {
   static const int m = [] { const char* e = getenv("MNB_FCONV_DEBUG"); return e ? atoi(e) : 0; }();
   return m;
@@ -541,6 +929,27 @@ extern "C" int mnb_fconv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const
   return 0;
 }
 
+extern "C" int mnb_fconv2d_wg_plan(const mnb_conv_shape* s, int32_t* out, int32_t n) {
+  tcfp32::Params p{};
+  int smem_bytes = 0;
+  if (int e = tcfp32::plan_wg(s, p, smem_bytes)) return e;
+  const int v[8] = {p.NP, p.KP, p.TH, p.n_tiles, tcfp32::grid_size(p), p.nbuf_a, smem_bytes, p.C * p.PH * p.PW};
+  if (out)
+    for (int i = 0; i < std::min(n, 8); ++i) out[i] = v[i];
+  return 0;
+}
+
+extern "C" int mnb_fconv2d_fwd_wg(const mnb_conv_shape* s, const float* x, const float* w, const float* bias, float* y,
+                                  int32_t* err_flag, mnb_stream_t stream) {
+  using namespace tcfp32;
+  MNB_REQUIRE(s && x && w && y && err_flag, "NULL pointer");
+  Params p{};
+  int smem_bytes = 0;
+  if (int e = plan_wg(s, p, smem_bytes)) return e;
+  p.x = x; p.w = w; p.bias = bias; p.y = y; p.err = err_flag;
+  return p.NP == 192 ? launch_fwd_wg<192>(p, smem_bytes, stream) : launch_fwd_wg<256>(p, smem_bytes, stream);
+}
+
 extern "C" int64_t mnb_fconv2d_wgrad_tc_scratch_bytes(const mnb_conv_shape* s) {
   tcfp32::Params p{};
   int smem = 0;
@@ -566,6 +975,37 @@ extern "C" int mnb_fconv2d_wgrad_tc(const mnb_conv_shape* s, const float* dy, co
   const int grid = grid_size(p);
   cudaStream_t st = (cudaStream_t)stream;
   wgrad_kernel<<<grid, NTHREADS, smem_bytes, st>>>(p);
+  const int n = p.K * p.KR;
+  reduce_partials_kernel<<<std::min(mnb_ceil_div(n, 256), MNB_NUM_SMS * 4), 256, 0, st>>>(p.partial, n, grid, dw);
+  MNB_LAUNCHED(2);
+  return 0;
+}
+
+extern "C" int64_t mnb_fconv2d_wgrad_wg_scratch_bytes(const mnb_conv_shape* s) {
+  tcfp32::Params p{};
+  int smem = 0;
+  if (tcfp32::plan_wgrad_wg(s, p, smem)) return -1;
+  return (int64_t)tcfp32::grid_size(p) * p.K * p.KR * 4;
+}
+
+extern "C" int mnb_fconv2d_wgrad_wg(const mnb_conv_shape* s, const float* dy, const float* x, float* dw, void* scratch,
+                                    int32_t* err_flag, mnb_stream_t stream) {
+  using namespace tcfp32;
+  MNB_REQUIRE(s && dy && x && dw && scratch && err_flag, "NULL pointer");
+  MNB_REQUIRE((reinterpret_cast<uintptr_t>(dy) & 15) == 0, "dy must be 16-byte aligned");
+  Params p{};
+  int smem_bytes = 0;
+  if (int e = plan_wgrad_wg(s, p, smem_bytes)) return e;
+  p.x = x; p.dy = dy; p.partial = reinterpret_cast<float*>(scratch); p.err = err_flag;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t ce = cudaFuncSetAttribute(wgrad_wg_kernel<WWG_KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+    if (ce != cudaSuccess) return mnb_fail((int)ce, "cudaFuncSetAttribute: %s", cudaGetErrorString(ce));
+    attr_set = true;
+  }
+  const int grid = grid_size(p);
+  cudaStream_t st = (cudaStream_t)stream;
+  wgrad_wg_kernel<WWG_KP><<<grid, WWG_THREADS, smem_bytes, st>>>(p);
   const int n = p.K * p.KR;
   reduce_partials_kernel<<<std::min(mnb_ceil_div(n, 256), MNB_NUM_SMS * 4), 256, 0, st>>>(p.partial, n, grid, dw);
   MNB_LAUNCHED(2);

@@ -479,12 +479,43 @@ def _tc_forward(ctx, x, w_int, w_scale, bias, spec, sh, y):
     return True
 
 
-def _fconv_forward(ctx, x, wq, bias, sh, y):
-    """un-quantized input with few channels (first layer): fp32-accurate im2col conv on the tensor cores
-    (mnb_fconv2d_fwd_tc).  False outside its cover."""
+def fconv_fwd(sh, x, w, bias, y, kind=None):
+    """fp32-accurate im2col conv of an un-quantized input with few channels (first layer) on the tensor cores:
+    mnb_fconv2d_fwd_wg where its plan covers the shape, mnb_fconv2d_fwd_tc otherwise (the same bits).  Returns the entry
+    point's code: MNB_E_UNSUPPORTED outside both covers.  ``kind``: record the launch under it in TIMER."""
     lib = L.load()
-    rc = _timed("fconv_fwd_tc", sh, lambda: lib.mnb_fconv2d_fwd_tc(
-        C.byref(sh), x.data_ptr(), wq.data_ptr(), L.ptr(bias), y.data_ptr(), L.tc_err_flag(x.device).data_ptr(), L.stream()))
+    args = (C.byref(sh), x.data_ptr(), w.data_ptr(), L.ptr(bias), y.data_ptr(), L.tc_err_flag(x.device).data_ptr(),
+            L.stream())
+
+    def run():
+        rc = lib.mnb_fconv2d_fwd_wg(*args)
+        return lib.mnb_fconv2d_fwd_tc(*args) if rc == L.E_UNSUPPORTED else rc
+    return run() if kind is None else _timed(kind, sh, run)
+
+
+def fconv_wgrad(sh, dy, x, dw, kind=None):
+    """weight gradient of the fconv_fwd layer: mnb_fconv2d_wgrad_wg where its plan covers the shape,
+    mnb_fconv2d_wgrad_tc otherwise (the same bits); False where neither has a plan.  ``kind`` as for fconv_fwd."""
+    lib = L.load()
+    entry = lib.mnb_fconv2d_wgrad_wg
+    fbytes = int(lib.mnb_fconv2d_wgrad_wg_scratch_bytes(C.byref(sh)))
+    if fbytes < 0:
+        entry = lib.mnb_fconv2d_wgrad_tc
+        fbytes = int(lib.mnb_fconv2d_wgrad_tc_scratch_bytes(C.byref(sh)))
+    if fbytes < 0:
+        return False
+    ws = torch.empty(max(fbytes, 4), dtype=torch.uint8, device=dy.device)
+
+    def run():
+        return entry(C.byref(sh), dy.data_ptr(), x.data_ptr(), dw.data_ptr(), ws.data_ptr(),
+                     L.tc_err_flag(dy.device).data_ptr(), L.stream())
+    L.check(run() if kind is None else _timed(kind, sh, run), "fconv2d_wgrad")
+    return True
+
+
+def _fconv_forward(ctx, x, wq, bias, sh, y):
+    """un-quantized input with few channels (first layer): fconv_fwd.  False outside its cover."""
+    rc = fconv_fwd(sh, x, wq, bias, y, "fconv_fwd_tc")
     if rc == L.E_UNSUPPORTED:
         return False
     L.check(rc, "fconv2d_fwd_tc")
@@ -561,18 +592,9 @@ def _wgrad(ctx, dy, tc):
 
 
 def _fconv_wgrad(ctx, dy):
-    """weight gradient on mnb_fconv2d_wgrad_tc; None where it has no plan"""
-    lib = L.load()
-    sh = ctx.sh
-    fbytes = int(lib.mnb_fconv2d_wgrad_tc_scratch_bytes(C.byref(sh)))
-    if fbytes < 0:
-        return None
+    """weight gradient on fconv_wgrad; None where it has no plan"""
     dwq = torch.empty_like(ctx.wq)
-    ws = torch.empty(max(fbytes, 4), dtype=torch.uint8, device=dy.device)
-    L.check(_timed("fconv_wgrad_tc", sh, lambda: lib.mnb_fconv2d_wgrad_tc(
-        C.byref(sh), dy.data_ptr(), ctx.x.data_ptr(), dwq.data_ptr(), ws.data_ptr(), L.tc_err_flag(dy.device).data_ptr(),
-        L.stream())), "fconv2d_wgrad_tc")
-    return dwq
+    return dwq if fconv_wgrad(ctx.sh, dy, ctx.x, dwq, "fconv_wgrad_tc") else None
 
 
 class QuantConv2dFn(Function):

@@ -334,19 +334,18 @@ class EngineMaxPool2d(nn.MaxPool2d):
 
 
 class FloatConvFn(Function):
-    """fp32 conv2d with few input channels on the tensor-core im2col path (mnb_fconv2d_*_tc);
+    """fp32 conv2d with few input channels on the tensor-core im2col path (functional.fconv_fwd / fconv_wgrad);
     shapes outside its cover run ATen's convolution (what the reference runs for this layer)."""
 
     @staticmethod
     def forward(ctx, x, w, bias, padding):
-        lib = L.load()
+        from .functional import fconv_fwd
         x, w = x.contiguous(), w.contiguous()
         b, c, h, wd = x.shape
         k, _, r, s_ = w.shape
         sh = L.ConvShape(b, c, h, wd, k, r, s_, 1, 1, padding, padding, 1, 1, 1)
         y = torch.empty((b, k, h, wd), dtype=torch.float32, device=x.device)
-        rc = lib.mnb_fconv2d_fwd_tc(C.byref(sh), x.data_ptr(), w.data_ptr(), L.ptr(bias), y.data_ptr(),
-                                    L.tc_err_flag(x.device).data_ptr(), L.stream())
+        rc = fconv_fwd(sh, x, w, bias, y)
         ctx.engine = rc == 0
         if rc == L.E_UNSUPPORTED:
             y = TF.conv2d(x, w, bias, 1, padding)
@@ -358,7 +357,7 @@ class FloatConvFn(Function):
 
     @staticmethod
     def backward(ctx, dy):
-        lib = L.load()
+        from .functional import fconv_wgrad
         x, w = ctx.saved_tensors
         presummed = getattr(dy, "_mnb_channel_sum", None)
         dy = dy.contiguous()
@@ -366,14 +365,8 @@ class FloatConvFn(Function):
         if ctx.needs_input_grad[0]:
             dx = torch.nn.grad.conv2d_input(x.shape, w, dy, 1, ctx.padding)
         if ctx.needs_input_grad[1]:
-            need = int(lib.mnb_fconv2d_wgrad_tc_scratch_bytes(C.byref(ctx.sh))) if ctx.engine else -1
-            if need >= 0:
-                dw = torch.empty_like(w)
-                scratch = torch.empty(need, dtype=torch.uint8, device=dy.device)
-                L.check(lib.mnb_fconv2d_wgrad_tc(C.byref(ctx.sh), dy.data_ptr(), x.data_ptr(), dw.data_ptr(),
-                                                 scratch.data_ptr(), L.tc_err_flag(dy.device).data_ptr(), L.stream()),
-                        "fconv2d_wgrad_tc")
-            else:
+            dw = torch.empty_like(w)
+            if not (ctx.engine and fconv_wgrad(ctx.sh, dy, x, dw)):
                 dw = torch.nn.grad.conv2d_weight(x, w.shape, dy, 1, ctx.padding)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             if presummed is not None and presummed.numel() == dy.shape[1]:
