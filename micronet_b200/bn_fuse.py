@@ -12,6 +12,8 @@
 * ``iao_model_bn_fuse`` - ``wqaq/iao/bn_fuse/bn_fuse.py:20-73``.  Every ``iao.QuantBNFuseConv2d`` becomes an
   ``iao.QuantConv2d(quant_inference=True, bias=True)`` holding the folded weight / bias (running statistics) and the
   calibrated scale / zero-point buffers of both quantizers.
+* ``iao_quantize_inference_weights`` - its weight step (``bn_fused_model_test.py:199-201``): every such conv stores its
+  fake-quantized weight, which ``iao.freeze_inference`` runs on the integer levels.
 
 The reference scripts read ``W`` / bit widths / ``q_type`` / ``q_level`` from their command line; here they are arguments
 (wbwtab) or read off the module being replaced (iao)."""
@@ -138,4 +140,17 @@ def dorefa_quantize_inference_weights(model):
     for m in model.modules():
         if isinstance(m, _df.QuantConv2d):
             m.weight.data = m.weight_quantizer(m.weight)
+    return model
+
+
+@torch.no_grad()
+def iao_quantize_inference_weights(model):
+    """the weight step of the reference's IAO deployment flow (``wqaq/iao/bn_fuse/bn_fused_model_test.py:199-201``, on the
+    model in eval mode): every IAO ``QuantConv2d`` with ``quant_inference=True`` (``iao_model_bn_fuse``'s output) stores
+    ``m.weight_quantizer(m.weight)`` with the stored scale / zero point and no observer or qparam update, per-channel and
+    per-layer alike, so it holds the levels ``fl(L * s)`` that ``iao.freeze_inference`` recovers.  Evaluated with
+    ``iao.stored_fake_quant`` (torch ops, the kernels' op sequence), so a model converted on the CPU takes the step there."""
+    for m in model.modules():
+        if isinstance(m, _iao.QuantConv2d) and m.quant_inference and m.weight_quantizer.bits != 32:
+            m.weight.data = _iao.stored_fake_quant(m.weight_quantizer, m.weight)[0]
     return model

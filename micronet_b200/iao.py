@@ -240,11 +240,58 @@ def _weight_quantizer(w_bits, q_type, q_level, weight_observer, out_channels, qa
     return cls(bits=w_bits, observer=observer, activation_weight_flag=0, qaft=qaft)
 
 
+def stored_fake_quant(quantizer, w):
+    """the weight fake-quant of the reference's eval forward (IAO:214-240: no observer or qparam update) with the stored
+    scale / zero point, in torch ops so that it runs wherever the converter does: (clamp(r, qmin, qmax) + zp) * s with
+    r = sign(v) * floor(|v| + 0.5), v = w / s - zp - the op sequence of iao_weight_fwd_kernel and act_quant_fwd_kernel
+    (per-channel and per-layer weights).  -> (fake-quantized ``w``, un-clamped levels r)"""
+    v = w / quantizer.scale - quantizer.zero_point
+    r = torch.sign(v) * torch.floor(v.abs() + 0.5)
+    return (r.clamp(quantizer.qmin, quantizer.qmax) + quantizer.zero_point) * quantizer.scale, r
+
+
+def _holds_levels(conv):
+    """does the weight of a ``quant_inference`` conv with a symmetric 2..8-bit weight quantizer hold that quantizer's output
+    (bn_fuse.iao_quantize_inference_weights)?  Finite, every level in range, and quantizing it again reproduces it bit for
+    bit; raw folded fp32 weights fail the last test."""
+    q = conv.weight_quantizer
+    if not (conv.quant_inference and _sym_quantizer(q)):
+        return False
+    w = conv.weight.detach()
+    wq, r = stored_fake_quant(q, w)
+    return bool(torch.isfinite(w).all()) and bool(((r >= q.qmin) & (r <= q.qmax)).all()) and torch.equal(wq, w)
+
+
+def _int_weights(conv):
+    """does ``conv`` run on integer weights when frozen?  A QAT conv quantizes its own; a ``quant_inference`` conv only when
+    freeze_inference found its stored weight to be its quantizer's levels (``_int_levels``, DESIGN.md 4.18)"""
+    return not conv.quant_inference or conv.__dict__.get("_int_levels") is not None
+
+
+_OPEN_RANGE = {}    # device -> (-inf, +inf) observer range of _frozen_spec
+
+
+def _frozen_spec(conv, spec):
+    """the activation spec of a frozen conv's forward and of the epilogue that writes its plane.  A deployment conv with
+    levels gets an unbounded observer range in place of its own: the converter does not copy the observer (neither does
+    the reference's), so its range is [0, 0], and the range only feeds the STE mask, which no frozen forward reads - but
+    the epilogues' level certification (mnb_act_levels) re-derives every level within rounding distance of the range's
+    ends exactly, i.e. every zero that a ReLU left, which made the linked convs 2.8x slower (DESIGN.md 4.18).  Levels are
+    unchanged: that path only decides how they are computed."""
+    if spec is None or conv.__dict__.get("_int_levels") is None:
+        return spec
+    dev = spec.scale.device
+    if dev not in _OPEN_RANGE:
+        _OPEN_RANGE[dev] = (torch.full((1,), -float("inf"), device=dev), torch.full((1,), float("inf"), device=dev))
+    return F_.ActSpec(spec.mode, spec.bits, spec.qmin, spec.qmax, spec.q_type, spec.scale, spec.zero_point,
+                      *_OPEN_RANGE[dev])
+
+
 def _int8_ok(conv):
     """was ``conv`` frozen with int8=True, with integer weights that fit s8 (symmetric, 2..8 bits)?  Its activation
     quantizer and shape are checked per call (functional._i8_route)."""
     wq = conv.weight_quantizer
-    return bool(conv.__dict__.get("_int8", False)) and not conv.quant_inference and wq.symmetric and 2 <= wq.bits <= 8
+    return bool(conv.__dict__.get("_int8", False)) and _int_weights(conv) and wq.symmetric and 2 <= wq.bits <= 8
 
 
 def _consumer_of(producer):
@@ -253,14 +300,15 @@ def _consumer_of(producer):
     if link is None:
         return None
     nxt, only = (link.cconv, True) if isinstance(link, _BlockLink) else link
-    if not nxt._use_frozen() or nxt.quant_inference:
+    if not nxt._use_frozen() or not _int_weights(nxt):
         return None
     aq, wq = nxt.activation_quantizer, nxt.weight_quantizer
     if aq.bits == 32 or wq.bits == 32 or not wq.symmetric:
         return None
+    spec = _frozen_spec(nxt, aq.act_spec())
     if isinstance(link, _BlockLink):
-        return link.consumer(aq.act_spec(), _int8_ok(nxt))
-    return F_.Consumer(nxt, aq.act_spec(), nxt.__dict__.get("_pre_relu", False), only, tuple(nxt.weight.shape), tuple(nxt.stride),
+        return link.consumer(spec, _int8_ok(nxt))
+    return F_.Consumer(nxt, spec, nxt.__dict__.get("_pre_relu", False), only, tuple(nxt.weight.shape), tuple(nxt.stride),
                        tuple(nxt.padding), tuple(nxt.dilation), nxt.groups, True, int8=_int8_ok(nxt))
 
 
@@ -296,6 +344,8 @@ class QuantConv2d(nn.Conv2d):
             weight, bias = make()
             if not self.quant_inference:
                 wq, w_int, w_scale = self.weight_quantizer.quantize_weight(weight)
+            elif _int_weights(self):
+                wq, w_int, w_scale = self._stored_levels(weight)
             else:
                 wq, w_int, w_scale = weight, None, None
             wq = wq.detach()
@@ -303,6 +353,16 @@ class QuantConv2d(nn.Conv2d):
             fr = (key, wq, w_int, w_scale, None if bias is None else bias.detach())
             self.__dict__["_frozen"] = fr
         return fr[1:]
+
+    def _stored_levels(self, weight):
+        """(wq, w_int, w_scale) of a ``quant_inference`` conv whose stored weight freeze_inference accepted as levels: the
+        weight quantizer run on it (levels clamped to range), which must give the stored weight back bit for bit.  A weight
+        written since with other values is refused: the planes this conv reads and writes assume those levels."""
+        wq, w_int, w_scale = self.weight_quantizer.quantize_weight(weight)
+        if not (bool(torch.isfinite(weight).all()) and torch.equal(wq, weight)):
+            raise RuntimeError(f"micronet_b200: the weight of {self.__dict__['_int_levels']!r} no longer holds its weight "
+                               "quantizer's levels; call iao.freeze_inference(model) again")
+        return wq, w_int, w_scale
 
     def _use_frozen(self):
         return self.__dict__.get("_frozen_inference", False) and not self.training and not torch.is_grad_enabled()
@@ -321,7 +381,7 @@ class QuantConv2d(nn.Conv2d):
         if plane is None:
             input = self._in_shuffle(input)
         aq = self.activation_quantizer
-        spec = aq.act_spec() if plane is not None else aq.prepare_activation(input)
+        spec = _frozen_spec(self, aq.act_spec() if plane is not None else aq.prepare_activation(input))
         return F_.frozen_conv(input, plane, wq, bias, w_int, w_scale, spec, self.stride, self.padding, self.dilation,
                               self.groups, pre_relu=self.__dict__.get("_pre_relu", False),
                               consumer=_consumer_of(self), int8=_int8_ok(self))
@@ -657,9 +717,16 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
       stores one element at a time, so such a link is made only across a pool (whose fake-quant and max-pool passes it
       saves) and only for an int8 plane (1-byte stores); the others write fp32 as before.
       Blocks with a live nn.BatchNorm2d (``bn_fuse=False``) and asymmetric quantizers keep the fp32 path.
-    Outputs are bit-identical to the un-frozen eval forward; ``enable=False`` restores the modules."""
+    * deployment graphs (``bn_fuse.iao_model_bn_fuse`` -> ``bn_fuse.iao_quantize_inference_weights``): an eval-mode
+      ``quant_inference`` conv with a symmetric 2..8-bit weight quantizer whose stored weight is that quantizer's output
+      (finite, levels in range, re-quantized bit for bit) runs on those integer levels and links like the QAT conv it came
+      from; its logits are bitwise those of the frozen QAT graph (DESIGN.md 4.18).  Any other ``quant_inference`` conv (raw
+      folded weights, asymmetric weights) keeps its fp32 weight and is not linked; a later in-place write of a weight that
+      no longer verifies raises at the next forward.
+    Outputs are bit-identical to the un-frozen eval forward (a deployment graph's: to the frozen QAT graph's);
+    ``enable=False`` restores the modules."""
     FG.undo(model, _UNDO)
-    for m in model.modules():
+    for name, m in model.named_modules():
         if isinstance(m, (QuantConv2d, QuantLinear, QuantAdd)):
             m.__dict__["_frozen_inference"] = bool(enable)
             m.__dict__["_int8"] = bool(enable and int8)
@@ -667,6 +734,9 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
             m.__dict__.pop("_pre_relu", None)
             m.__dict__.pop("_fuse_relu", None)
             m.__dict__.pop("_post_consumer", None)
+            m.__dict__.pop("_int_levels", None)
+            if enable and isinstance(m, QuantConv2d) and not m.training and _holds_levels(m):
+                m.__dict__["_int_levels"] = name or type(m).__name__    # named in the error of a later mismatch
     for m in model.modules():
         saved = m.__dict__.setdefault("_mnb_saved_relus", {})
         for name, relu in list(saved.items()):       # undo an earlier rewrite first
@@ -677,7 +747,7 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
         if isinstance(m, nn.Sequential):
             kids = [(n, k) for n, k in m.named_children() if not isinstance(k, nn.Identity)]
             for (n0, k0), (n1, k1) in zip(kids, kids[1:]):
-                if type(k0) is nn.ReLU and isinstance(k1, QuantConv2d) and not k1.quant_inference:
+                if type(k0) is nn.ReLU and isinstance(k1, QuantConv2d) and _int_weights(k1):
                     k1.__dict__["_pre_relu"] = True
                     saved[n0] = k0
                     m._modules[n0] = nn.Identity()
@@ -724,9 +794,9 @@ def _sym_quantizer(q):
 
 def _block_conv(conv):
     """can ``conv`` produce or consume a level plane of a block link?  A frozen eval-mode conv with symmetric 2..8-bit IAO
-    quantizers and integer weights (no ``quant_inference``)"""
+    quantizers and integer weights (_int_weights)"""
     return (isinstance(conv, QuantConv2d) and conv.__dict__.get("_frozen_inference", False) and not conv.training
-            and not conv.quant_inference and _sym_quantizer(conv.activation_quantizer)
+            and _int_weights(conv) and _sym_quantizer(conv.activation_quantizer)
             and _sym_quantizer(conv.weight_quantizer))
 
 
