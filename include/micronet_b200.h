@@ -153,8 +153,8 @@ int mnb_iao_weight_bwd(const float* g_wq, const uint8_t* pass, const float* scal
  *                                        value = e_a * a_scale[0]; a_offset_zp (device scalar,
  *                                        may be NULL) is added to a_offset (IAO zero_point);
  *                      else            : a_f32 raw fp32 activations.
- * Weight operand:      w_int != NULL && a_codes != NULL : exact integer path, s32 accumulate,
- *                                        y = bias + acc * a_scale * w_scale[k];
+ * Weight operand:      w_int != NULL && a_codes != NULL : exact integer path, s64 accumulate,
+ *                                        y = bias + acc * (a_scale * w_scale[k]), acc rounded once;
  *                      else            : w_f32 fp32 weights, fp32 accumulate.
  * ---------------------------------------------------------------------- */
 typedef struct {

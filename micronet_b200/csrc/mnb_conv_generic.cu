@@ -1,6 +1,6 @@
 // Generic implicit-GEMM convolution kernels (any stride / padding / dilation / groups).
 //
-// This is the shape-agnostic path of the engine: forward (exact s32 accumulation when both
+// This is the shape-agnostic path of the engine: forward (exact integer accumulation when both
 // operands are integer levels, fp32 otherwise), dgrad fused with the activation STE mask, and
 // split-K wgrad with a deterministic two-stage reduction.  Hot, regular shapes are taken by the
 // wgmma tensor-core kernels (mnb_conv_tc_fwd.cu, mnb_conv_tc_wgrad.cu, mnb_pk.cu); everything else (C_in = 3 stems, 10-way heads,
@@ -30,9 +30,11 @@ static int make_geom(const mnb_conv_shape* s, ConvGeom& g) {
   MNB_REQUIRE(g.B > 0 && g.C > 0 && g.H > 0 && g.W > 0 && g.K > 0 && g.R > 0 && g.S > 0, "non-positive conv dims");
   MNB_REQUIRE(g.sh > 0 && g.sw > 0 && g.dh > 0 && g.dw > 0 && g.ph >= 0 && g.pw >= 0, "bad stride/dilation/padding");
   MNB_REQUIRE(g.G > 0 && g.C % g.G == 0 && g.K % g.G == 0, "channels (%d,%d) not divisible by groups %d", g.C, g.K, g.G);
-  g.P = (g.H + 2 * g.ph - g.dh * (g.R - 1) - 1) / g.sh + 1;
-  g.Q = (g.W + 2 * g.pw - g.dw * (g.S - 1) - 1) / g.sw + 1;
-  MNB_REQUIRE(g.P > 0 && g.Q > 0, "empty conv output");
+  // (tested before dividing: C division truncates, so a filter one row longer than the padded image would give P = 1)
+  const int h_span = g.H + 2 * g.ph - g.dh * (g.R - 1) - 1, w_span = g.W + 2 * g.pw - g.dw * (g.S - 1) - 1;
+  MNB_REQUIRE(h_span >= 0 && w_span >= 0, "empty conv output");
+  g.P = h_span / g.sh + 1;
+  g.Q = w_span / g.sw + 1;
   g.Cg = g.C / g.G; g.Ng = g.K / g.G; g.RS = g.R * g.S;
   return 0;
 }
@@ -69,11 +71,15 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(FwdArgs a) {
 
   const int bk = tid & (BK - 1), bn0 = tid >> 4;  // B: k fastest
 
-  Acc acc[4][TN];
+  // Integer levels: each BK chunk sums into an int partial (16 products of |w| <= 32767 and |e| <= 255 + |offset| +
+  // |zero_point| stay far below 2^31) that is folded into a 64-bit running sum, so the sum is exact for any Cg*R*S.
+  constexpr bool kInt = std::is_integral<Acc>::value;
+  using Sum = typename std::conditional<kInt, long long, float>::type;
+  Sum acc[4][TN];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int j = 0; j < TN; ++j) acc[i][j] = (Acc)0;
+    for (int j = 0; j < TN; ++j) acc[i][j] = (Sum)0;
 
   for (int k0 = 0; k0 < Kd; k0 += BK) {
 #pragma unroll
@@ -110,6 +116,11 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(FwdArgs a) {
       Bs[bk][nn] = v;
     }
     __syncthreads();
+    Acc part[4][TN];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < TN; ++j) part[i][j] = (Acc)0;
 #pragma unroll
     for (int kk = 0; kk < BK; ++kk) {
       Acc av[4], bv[TN];
@@ -120,7 +131,16 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(FwdArgs a) {
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < TN; ++j) acc[i][j] += av[i] * bv[j];
+        for (int j = 0; j < TN; ++j) {
+          if constexpr (kInt) part[i][j] += av[i] * bv[j];
+          else acc[i][j] += av[i] * bv[j];
+        }
+    }
+    if constexpr (kInt) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < TN; ++j) acc[i][j] += part[i][j];
     }
     __syncthreads();
   }
@@ -132,14 +152,14 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(FwdArgs a) {
     const int ch = grp * g.Ng + n;
     const float bsv = a.bias ? __ldg(a.bias + ch) : 0.f;
     float sc = 1.f;
-    if constexpr (std::is_integral<Acc>::value) sc = __fmul_rn(a_sc, __ldg(a.w_scale + ch));
+    if constexpr (kInt) sc = __fmul_rn(a_sc, __ldg(a.w_scale + ch));
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int mm = m0 + tx + 16 * i;
       if (mm >= M) continue;
       const int b = mm / PQ, pq = mm - b * PQ;
       float v;
-      if constexpr (std::is_integral<Acc>::value) v = __fadd_rn(__fmul_rn((float)acc[i][j], sc), bsv);
+      if constexpr (kInt) v = __fadd_rn(__fmul_rn((float)acc[i][j], sc), bsv);
       else v = (float)acc[i][j] + bsv;
       a.y[((int64_t)b * g.K + ch) * PQ + pq] = v;
     }

@@ -54,6 +54,7 @@ def test_conv_transpose_fn_matches_fp64(shape):
     assert rel_err(be.grad, bd.grad) <= 1e-5
     if dil == 1 and Ci >= 16:
         assert {"dgrad_pk", "fwd_pk", "wgrad_pk"} <= kinds, kinds       # the tensor-core family, roles swapped
+        assert not {"dgrad", "fwd", "wgrad"} & kinds, kinds             # (a _pk kind is recorded even when it refused)
     if dil == 2:
         assert {"dgrad", "fwd", "wgrad"} <= kinds, kinds
 
