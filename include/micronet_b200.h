@@ -589,7 +589,7 @@ int mnb_xnor_conv_fwd(const mnb_conv_shape* s, const void* a_bits, const void* w
 #define MNB_XNOR_BITS 0
 #define MNB_XNOR_PM1_BF16 1
 typedef struct mnb_xnor_post {
-  int32_t format;          /* MNB_XNOR_BITS or MNB_XNOR_PM1_BF16 */
+  int32_t format;          /* MNB_XNOR_BITS or MNB_XNOR_PM1_BF16 (mnb_b1_*: also MNB_XNOR_B1_PLANE) */
   int32_t out_groups;      /* bits: the consumer conv's group count (C_out % out_groups == 0) */
   int32_t shuffle_groups;  /* 1 = none */
   int32_t pool2;           /* 1: MaxPool2d(2, 2) folded in (even P and Q) */
@@ -603,6 +603,46 @@ int mnb_xnor_conv_post(const mnb_conv_shape* s, const void* a_bits, const void* 
                        const mnb_xnor_post* post, void* out, mnb_stream_t stream);
 int mnb_xnor_pack_act_post(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_xnor_post* post,
                            void* out_bits, mnb_stream_t stream);
+
+/* ------------------------------------------------------------------------
+ * Binary tensor-core forward for wbwtab layers (mnb_b1.cu): the exact integer sum of mnb_xnor_conv_fwd / mnb_pk_conv
+ * (WB:11-36, 55-75, 181-195) on wgmma m64nNk256.s32.b1.b1.and.popc, for the layers outside the XNOR kernel's cover
+ * (NIN's 1x1 / 3x3 / 5x5 layers of 160 and 192 channels, models/nin.py; deployed as by wbwtab/bn_fuse).
+ *   b1 plane : [B][G * u][H][W][16 bytes], u = ceil(C/g / 64) units per group; a unit holds 64 channels of one pixel,
+ *              bits 0-63 p = [value is +1], bits 64-127 n = [value is -1] (bit j of the 64 = channel 64 i + j of the group).
+ *              p = n = 0 is a 0: image halo (zero-filled by the TMA unit), channel padding up to a whole unit, and each
+ *              group starting on a unit boundary - the zero padding of the reference's +-1 tensor, with no border tables.
+ *   w_img    : mnb_b1_wimage_bytes() bytes from the i16 levels {-1, 0, +1} [K][C/g][R][S]: P = [w == +1], M = [w == -1];
+ *              output channel k owns two adjacent B columns plus = [P | M] and minus = [M | P], so
+ *              D_plus - D_minus = sum (P - M)(p - n) = sum w * a exactly.
+ * y = fmaf(sum, alpha[k], bias[k]) equals mnb_xnor_conv_fwd's and mnb_pk_conv's result bit for bit.  Cover: stride 1,
+ * dilation 1, square filters up to 7 x 7 with pad <= R / 2, any C/g and K/g; else MNB_E_UNSUPPORTED (mnb_b1_supported: 1 / 0).
+ *   mnb_b1_pack_act       : fp32 NCHW -> b1 plane (sign with 0 -> +1, NaN -> +1, like the engine's other binarizers).
+ *   mnb_b1_pack_act_post  : fp32 NCHW -> [eval BatchNorm] -> sign [-> 2x2 max-pool] [-> channel shuffle] -> the consumer's
+ *                           b1 plane (format MNB_XNOR_B1_PLANE, out_groups = the consumer's groups).
+ *   mnb_b1_conv_fwd       : fp32 NCHW output.  err_flag: device int set on a pipeline timeout (as mnb_pk_conv's).
+ *   mnb_b1_conv_post      : the epilogue of mnb_xnor_conv_post (BatchNorm, sign, OR-pool, shuffle) into MNB_XNOR_BITS,
+ *                           MNB_XNOR_PM1_BF16 or MNB_XNOR_B1_PLANE (bitwise deterministic: the plane is pre-filled, then
+ *                           OR / AND-ed into, one word per output pixel and run of channels).
+ *   mnb_b1_plane_maxpool  : MaxPool2d(k, s, p) (2p <= k, floor mode) on a b1 plane: p = OR of the in-image p bits,
+ *                           n = (OR n) & !p - the max of +-1 values, padding channels stay zero.
+ * mnb_xnor_conv_post / mnb_xnor_pack_act_post refuse MNB_XNOR_B1_PLANE (MNB_E_ARG).                                     */
+#define MNB_XNOR_B1_PLANE 2
+int mnb_b1_supported(const mnb_conv_shape* s);
+int64_t mnb_b1_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t groups);
+int mnb_b1_pack_act(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t groups, void* out_plane,
+                    mnb_stream_t stream);
+int mnb_b1_pack_act_post(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_xnor_post* post,
+                         void* out_plane, mnb_stream_t stream);
+int64_t mnb_b1_wimage_bytes(const mnb_conv_shape* s);
+int mnb_b1_pack_weight(const mnb_conv_shape* s, const int16_t* w_int, void* w_img, mnb_stream_t stream);
+int mnb_b1_conv_fwd(const mnb_conv_shape* s, const void* a_plane, const void* w_img, const float* alpha, const float* bias,
+                    float* y, int32_t* err_flag, mnb_stream_t stream);
+int64_t mnb_b1_post_bytes(const mnb_conv_shape* s, const mnb_xnor_post* post);
+int mnb_b1_conv_post(const mnb_conv_shape* s, const void* a_plane, const void* w_img, const float* alpha, const float* bias,
+                     const mnb_xnor_post* post, void* out, int32_t* err_flag, mnb_stream_t stream);
+int mnb_b1_plane_maxpool(const void* in_plane, int32_t batch, int32_t channels, int32_t groups, int32_t h, int32_t w, int32_t k,
+                         int32_t s, int32_t p, void* out_plane, mnb_stream_t stream);
 
 /* Optimizer step of the QAT loop (torch.optim.Adam semantics, L2 weight decay, no amsgrad;
  * wbwtab/main.py:84,331-339) over one flat fp32 parameter / gradient bucket: a single launch. */

@@ -285,11 +285,16 @@ def materialized(t):
     storage was never written) - the +-1 tensor rebuilt from the bf16 operand plane [b][c/8][h][w][8], or - for a wbwtab conv
     that handed its output to its BatchNorm as int16 codes (``codes_out``) - that output decoded with the conv epilogue's own
     fmaf, or - for the output of a frozen wbwtab layer (wbwtab.freeze_inference) - the +-1 tensor its consumer's bit plane
-    encodes.  Plumbing for tests, hooks and readers outside the fused producers; the training step never calls it."""
+    encodes (bit plane or b1 plane).  Plumbing for tests, hooks and readers outside the fused producers; the training step
+    never calls it."""
     xbits = getattr(t, "_mnb_xbits", None)
     if xbits is not None:
         from . import xnor as XN
         return XN.unpack(xbits[1], t.shape, xbits[3])
+    b1p = getattr(t, "_mnb_b1", None)
+    if b1p is not None:
+        from . import b1 as B1
+        return B1.unpack(b1p[1], t.shape, b1p[3])
     codes = getattr(t, "_mnb_codes", None)
     if codes is not None:
         b, c = t.shape[0], t.shape[1]

@@ -172,23 +172,30 @@ def frozen_levels(conv):
     return w_int, alpha
 
 
-def _freezable(conv):
-    """structural test of frozen_levels that needs no kernel: geometry inside the XNOR cover and, for a QAT ternary layer,
-    no all-zero channel (its alpha is 0 / 0)"""
-    import torch
-    from . import xnor as XN
+def _frozen_kernel(conv):
+    """the kernel a frozen layer runs, from its geometry: "xnor" inside the XNOR kernel's cover, else "b1" inside the binary
+    tensor-core convolution's (DESIGN.md 4.19), else None; None also when frozen_levels would refuse the weights (for a QAT
+    ternary layer: an all-zero channel, alpha 0 / 0)"""
+    from . import b1 as B1, xnor as XN
     if not isinstance(conv, QuantConv2d) or conv.padding_mode != "zeros" or isinstance(conv.padding, str):
-        return False
+        return None
     k = conv.kernel_size[0]
     sh = L.ConvShape(1, conv.in_channels, max(8, k), max(8, k), conv.out_channels, k, conv.kernel_size[1], conv.stride[0],
                      conv.stride[1], conv.padding[0], conv.padding[1], conv.dilation[0], conv.dilation[1], conv.groups)
-    if not XN.supported(sh):
-        return False
+    kind = "xnor" if XN.supported(sh) else ("b1" if B1.supported(sh) else None)
+    if kind is None:
+        return None
     if conv.quant_inference:
-        return frozen_levels(conv) is not None
-    if conv.weight_quantizer.W == 3:
-        return bool((conv.weight.detach().abs().amax(dim=(1, 2, 3)) > 0).all())
-    return conv.weight_quantizer.W == 2
+        ok = frozen_levels(conv) is not None
+    elif conv.weight_quantizer.W == 3:
+        ok = bool((conv.weight.detach().abs().amax(dim=(1, 2, 3)) > 0).all())
+    else:
+        ok = conv.weight_quantizer.W == 2
+    return kind if ok else None
+
+
+def _freezable(conv):
+    return _frozen_kernel(conv) is not None
 
 
 class _Link:
@@ -236,6 +243,10 @@ class _Link:
 
     def tag(self, plane, shape, device):
         import torch
+        if self.fmt == L.XNOR_B1_PLANE:
+            y = torch.empty(shape, dtype=torch.float32, device="meta")     # shape only: the data lives in the b1 plane
+            y._mnb_b1 = (self.consumer, plane, y._version, self.out_groups)
+            return y
         if self.fmt == L.XNOR_BITS:
             y = torch.empty(shape, dtype=torch.float32, device="meta")     # shape only: the data lives in the bit plane
             y._mnb_xbits = (self.consumer, plane, y._version, self.out_groups)
@@ -247,7 +258,7 @@ class _Link:
 
 def _out_buffer(nbytes, fmt, device):
     import torch
-    if fmt == L.XNOR_BITS:
+    if fmt in (L.XNOR_BITS, L.XNOR_B1_PLANE):
         return torch.empty(nbytes // 4, dtype=torch.int32, device=device)
     return torch.empty(nbytes, dtype=torch.uint8, device=device)
 
@@ -258,6 +269,46 @@ def _handed_bits(module, x):
     if pre is not None and pre[0] is module and x._version == pre[2] and pre[3] == module.groups:
         return pre[1]
     return None
+
+
+def _handed_b1(module, x):
+    """the b1 plane a frozen producer (or a plane pool) wrote for ``module``, if ``x`` is that unmodified output"""
+    pre = getattr(x, "_mnb_b1", None)
+    if pre is not None and pre[0] is module and x._version == pre[2] and pre[3] == module.groups:
+        return pre[1]
+    return None
+
+
+class _PlanePool(nn.Module):
+    """a MaxPool2d(k, s, p) between a frozen producer and a frozen b1 consumer: the pool of the +-1 tensor taken on its b1
+    plane (mnb_b1_plane_maxpool); any other input runs the original pool"""
+
+    def __init__(self, pool, consumer):
+        super().__init__()
+        self.__dict__["pool"], self.__dict__["consumer"] = pool, consumer      # not sub-modules: state_dict unchanged
+        self.k, self.s, self.p = _pool_cfg_b1(pool)
+
+    def forward(self, x):
+        import torch
+        from . import b1 as B1
+        _check_eval(self)
+        pre = getattr(x, "_mnb_b1", None)
+        if pre is not None and pre[0] is self and x._version == pre[2]:
+            rc, out, shape = B1.plane_maxpool(pre[1], x.shape, pre[3], self.k, self.s, self.p)
+            if rc == 0:
+                y = torch.empty(shape, dtype=torch.float32, device="meta")
+                y._mnb_b1 = (self.consumer, out, y._version, pre[3])
+                return y
+            if rc != L.E_UNSUPPORTED:
+                L.check(rc, "b1_plane_maxpool")
+        return self.pool(F_.materialized(x))
+
+
+def _pool_cfg_b1(pool):
+    from .fused import EngineMaxPool2d, _pool_cfg
+    if type(pool) not in (nn.MaxPool2d, EngineMaxPool2d) or int(getattr(pool, "out_shuffle_groups", 1)) != 1:
+        return None
+    return _pool_cfg(pool)
 
 
 def _check_eval(m):
@@ -281,28 +332,30 @@ def _frozen_conv_operands(conv):
     return fr[1:]
 
 
-def _frozen_conv_forward(link, conv, x):
-    """XNOR conv whose epilogue applies the absorbed BatchNorm / binarizer / pool / shuffle and writes the consumer's operand"""
-    from . import xnor as XN
+def _frozen_conv_forward(link, conv, x, kind="xnor"):
+    """XNOR (or, outside its cover, binary tensor-core) conv whose epilogue applies the absorbed BatchNorm / binarizer /
+    pool / shuffle and writes the consumer's operand"""
+    from . import b1 as B1, xnor as XN
+    K = B1 if kind == "b1" else XN
     _check_eval(conv)
     w_int, alpha, bias, images = _frozen_conv_operands(conv)
     sh = F_._shape_struct(x.shape, conv.weight.shape, conv.stride, conv.padding, conv.dilation, conv.groups)
     post, keep = link.post()
-    nbytes = XN.post_bytes(sh, post)
+    nbytes = K.post_bytes(sh, post)
     if nbytes >= 0:
-        plane = _handed_bits(conv, x)
+        plane = _handed_b1(conv, x) if kind == "b1" else _handed_bits(conv, x)
         if plane is None:
-            plane = XN.pack_act(F_.materialized(x).contiguous(), conv.groups)
+            plane = K.pack_act(F_.materialized(x).contiguous(), conv.groups)
         if "w_img" not in images:
-            images["w_img"] = XN.pack_weight(sh, w_int)
+            images["w_img"] = K.pack_weight(sh, w_int)
         out = _out_buffer(nbytes, link.fmt, alpha.device)
-        rc = F_._timed("fwd_xnor_post", sh, lambda: XN.conv_post(sh, plane, images["w_img"], post, out, alpha=alpha, bias=bias))
+        rc = F_._timed(f"fwd_{kind}_post", sh, lambda: K.conv_post(sh, plane, images["w_img"], post, out, alpha=alpha, bias=bias))
         del keep
         if rc == 0:
             p, q = F_._out_hw(sh)
             return link.tag(out, link.out_shape(x.shape[0], conv.out_channels, p, q), alpha.device)
         if rc != L.E_UNSUPPORTED:
-            L.check(rc, "xnor_conv_post")
+            L.check(rc, f"{kind}_conv_post")
     # outside the kernel's cover: the un-frozen layer, then the modules its epilogue stands for
     wq = w_int.float() * alpha.view(-1, 1, 1, 1)
     y = F_.quant_conv2d(F_.materialized(x), wq, bias, w_int, alpha, None, conv.stride, conv.padding, conv.dilation, conv.groups)
@@ -313,29 +366,36 @@ def _frozen_stem_forward(link, act, x):
     """the binarizer behind the un-quantized stem conv: [eval BatchNorm] + sign [+ pool] [+ shuffle] straight into the
     first XNOR layer's bit plane"""
     import torch
-    from . import xnor as XN
+    from . import b1 as B1, xnor as XN
+    K = B1 if link.fmt == L.XNOR_B1_PLANE else XN
     _check_eval(act)
     x = F_.materialized(x)
     if x.dim() == 4 and x.is_cuda and x.dtype == torch.float32:
         b, c, h, w = x.shape
         post, keep = link.post()
         oh, ow = (h // 2, w // 2) if link.pool2 else (h, w)
-        nbytes = int(L.load().mnb_xnor_act_bytes(b, c, oh, ow, link.out_groups))
+        nbytes = int((L.load().mnb_b1_act_bytes if K is B1 else L.load().mnb_xnor_act_bytes)(b, c, oh, ow, link.out_groups))
         if nbytes >= 0 and not (link.pool2 and (h | w) & 1):
-            out = _out_buffer(nbytes, L.XNOR_BITS, x.device)
+            out = _out_buffer(nbytes, link.fmt, x.device)
             x = x.contiguous()
-            rc = XN.pack_act_post(x, post, out)
+            rc = K.pack_act_post(x, post, out)
             del keep
             if rc == 0:
                 return link.tag(out, (b, c, oh, ow), x.device)
             if rc != L.E_UNSUPPORTED:
-                L.check(rc, "xnor_pack_act_post")
+                L.check(rc, "pack_act_post")
     return link.tail(x)
 
 
 def _absorbed(m, x):
     _check_eval(m)
     return x
+
+
+def _block_parts(blk):
+    """[conv, act] of a conv-bn-act block: NIN-GC's (with channel_shuffle_flag) or the reference nin.py one (without)"""
+    parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
+    return parts if len(parts) == 2 and isinstance(parts[0], nn.Conv2d) else None
 
 
 def _blocks(seq):
@@ -345,10 +405,8 @@ def _blocks(seq):
     out = []
     kids = [(n, k) for n, k in seq.named_children() if not isinstance(k, nn.Identity)]
     for i, (name, blk) in enumerate(kids):
-        if not hasattr(blk, "channel_shuffle_flag"):
-            continue
-        parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
-        if len(parts) != 2 or not isinstance(parts[0], nn.Conv2d):
+        parts = _block_parts(blk)
+        if parts is None:
             continue
         act = parts[1]
         if isinstance(act, BatchNormBinarize2d) or (type(act) is ActivationQuantizer and act.A == 2):
@@ -374,7 +432,8 @@ def _undo(model):
 
 def freeze_inference(model, enable=True):
     """Inference on bit planes for a wbwtab model in eval mode (NIN-GC-style ``nn.Sequential`` of conv-bn-act blocks):
-    every binary / ternary conv whose output is binarized for a consumer runs the XNOR-popcount kernel with its weights
+    every binary / ternary conv whose output is binarized for a consumer runs the XNOR-popcount kernel (outside its cover,
+    e.g. NIN's 160 / 192-channel layers: the binary tensor-core convolution, DESIGN.md 4.19) with its weights
     quantized and packed ONCE (re-done when a parameter is written in place), and its epilogue writes the consumer's operand
     directly - the sign bits of the next XNOR layer (mnb_xnor_conv_post), or the +-1 bf16 plane of the un-quantized head -
     so no fp32 activation crosses between two binarized layers.  The binarizer behind the stem conv writes the first
@@ -397,27 +456,34 @@ def freeze_inference(model, enable=True):
     undo = model.__dict__.setdefault("_mnb_xnor_undo", [])
     for seq in [m for m in model.modules() if isinstance(m, nn.Sequential)]:
         kids, blocks = _blocks(seq)
-        frozen = set()
+        frozen = {}             # conv -> the kernel it runs frozen ("xnor" / "b1")
         links = []
         # from the last block back: a producer is frozen only when its consumer reads what it writes
         for i, name, blk, conv, act in reversed(blocks):
-            j, pool = i + 1, None
+            j, pool, ppool = i + 1, None, None
             if (j < len(kids) and type(kids[j][1]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j][1]) == (2, 2, 0)
                     and not isinstance(act, BatchNormBinarize2d)):
                 pool, j = kids[j], j + 1
+            elif j < len(kids) and _pool_cfg_b1(kids[j][1]) is not None and _pool_cfg_b1(kids[j][1]) != (2, 2, 0):
+                ppool, j = kids[j], j + 1     # taken on the consumer's b1 plane (mnb_b1_plane_maxpool), if it has one
             if j >= len(kids):
                 continue
             nxt = kids[j][1]
             shuffled = bool(getattr(nxt, "channel_shuffle_flag", 0)) and int(getattr(nxt, "shuffle_groups", 1)) > 1
             if isinstance(act, BatchNormBinarize2d) and shuffled:
                 continue        # a shuffle the fused producer did not take (not a graph prepare(fuse_bn=True) builds)
-            nparts = [k for k in nxt.children() if not isinstance(k, nn.Identity)] if hasattr(nxt, "channel_shuffle_flag") else []
+            nparts = [k for k in nxt.children() if not isinstance(k, nn.Identity)]
             cconv = nparts[0] if nparts and isinstance(nparts[0], nn.Conv2d) else None
             if cconv is None:
                 continue
             sg = int(nxt.shuffle_groups) if shuffled else (int(act.out_shuffle_groups) if isinstance(act, BatchNormBinarize2d) else 1)
+            ckind = frozen.get(cconv)
+            if ppool is not None and ckind != "b1":
+                continue        # a pool the epilogue cannot take and no b1 plane to take it on
             link = None
-            if cconv in frozen:
+            if ckind == "b1":
+                link = _Link(cconv, L.XNOR_B1_PLANE, cconv.groups, act, pool[1] if pool else None, sg)
+            elif ckind == "xnor":
                 link = _Link(cconv, L.XNOR_BITS, cconv.groups, act, pool[1] if pool else None, sg)
             elif _head_conv(cconv) and not isinstance(cconv, QuantConv2d) and sg == 1 and pool is None and not (
                     isinstance(act, BatchNormBinarize2d) and act.pool2):
@@ -425,15 +491,26 @@ def freeze_inference(model, enable=True):
             if link is None:
                 continue
             if isinstance(conv, QuantConv2d):
-                if not _freezable(conv):
+                kind = _frozen_kernel(conv)
+                # an XNOR producer has no b1-plane epilogue: in front of a b1 consumer it runs un-frozen
+                if kind is None or (kind == "xnor" and link.fmt == L.XNOR_B1_PLANE):
                     continue
-                frozen.add(conv)
-                links.append(("conv", conv, link, pool, nxt, shuffled, kids[j][0]))
-            elif link.fmt == L.XNOR_BITS and type(conv) is not QuantConv2d:
-                links.append(("stem", act, link, pool, nxt, shuffled, kids[j][0]))
-        for kind, mod, link, pool, nxt, shuffled, nxt_name in links:
+                frozen[conv] = kind
+                links.append(("conv", conv, link, pool, nxt, shuffled, ppool, kind))
+            elif link.fmt in (L.XNOR_BITS, L.XNOR_B1_PLANE) and type(conv) is not QuantConv2d:
+                links.append(("stem", act, link, pool, nxt, shuffled, ppool, None))
+        for kind, mod, link, pool, nxt, shuffled, ppool, ckind in links:
+            if ppool is not None:
+                # the pool reads what the producer writes and hands its pooled plane to the consumer
+                pp = _PlanePool(ppool[1], link.consumer)
+                pp.train(ppool[1].training)
+                link.consumer = pp
+                undo.append(("child", seq, ppool[0], ppool[1]))
+                seq._modules[ppool[0]] = pp
             if kind == "conv":
-                mod.__dict__["_mnb_xnor"] = lambda m, x, link=link: _frozen_conv_forward(link, m, x)
+                mod.__dict__["_mnb_xnor"] = lambda m, x, link=link, k=ckind: _frozen_conv_forward(link, m, x, k)
+                mod.__dict__["_mnb_frozen_plan"] = (ckind, link.fmt)     # the kernel and hand-off format (introspection)
+                undo.append(("dict", mod, "_mnb_frozen_plan", None))
                 undo.append(("dict", mod, "_mnb_xnor", None))
                 undo.append(("dict", mod, "_mnb_xnor_ops", None))
                 link.act.__dict__["_mnb_xnor"] = _absorbed       # its work is done in the conv's epilogue
