@@ -603,6 +603,12 @@ int mnb_xnor_conv_post(const mnb_conv_shape* s, const void* a_bits, const void* 
                        const mnb_xnor_post* post, void* out, mnb_stream_t stream);
 int mnb_xnor_pack_act_post(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_xnor_post* post,
                            void* out_bits, mnb_stream_t stream);
+/* host only, the plan mnb_xnor_conv_fwd (post NULL) / mnb_xnor_conv_post runs, from the function their launcher uses:
+ * out[0..9] = {R, NW (32-channel words per group), border, px (pixels per thread), post, ksplit (k-slices per group),
+ * kb (output channels per k-slice, the last one ragged when K/g % kb != 0), pblocks (pixel blocks), shared-memory bytes,
+ * refused}.  refused = 1: the launch returns MNB_E_UNSUPPORTED although mnb_xnor_supported is 1 (shared memory over 48 KB
+ * or more than 65535 (group, k-slice) blocks).  Returns MNB_E_UNSUPPORTED outside the cover and check_post's refusals. */
+int mnb_xnor_plan(const mnb_conv_shape* s, const mnb_xnor_post* post, int32_t* out);
 
 /* ------------------------------------------------------------------------
  * Binary tensor-core forward for wbwtab layers (mnb_b1.cu): the exact integer sum of mnb_xnor_conv_fwd / mnb_pk_conv
@@ -638,6 +644,12 @@ int64_t mnb_b1_wimage_bytes(const mnb_conv_shape* s);
 int mnb_b1_pack_weight(const mnb_conv_shape* s, const int16_t* w_int, void* w_img, mnb_stream_t stream);
 int mnb_b1_conv_fwd(const mnb_conv_shape* s, const void* a_plane, const void* w_img, const float* alpha, const float* bias,
                     float* y, int32_t* err_flag, mnb_stream_t stream);
+/* host only, the plan mnb_b1_conv_fwd (post NULL) / mnb_b1_conv_post runs (the launcher's own plan function):
+ * out[0..16] = {Nt (B columns of the N tile: kernel instance), n_ntiles, u (64-channel units per group), ksteps, G,
+ * col_tiles, Wt (output columns per tile), BW (box width with halo), TH (output rows per tile), TB (images per M tile),
+ * row_tiles, n_mtiles, TG (taps per stage), ntg (tap groups), nstage (pipeline stages), post, dynamic shared-memory bytes}.
+ * Returns MNB_E_UNSUPPORTED outside the cover and check_post's refusals. */
+int mnb_b1_plan(const mnb_conv_shape* s, const mnb_xnor_post* post, int32_t* out);
 int64_t mnb_b1_post_bytes(const mnb_conv_shape* s, const mnb_xnor_post* post);
 int mnb_b1_conv_post(const mnb_conv_shape* s, const void* a_plane, const void* w_img, const float* alpha, const float* bias,
                      const mnb_xnor_post* post, void* out, int32_t* err_flag, mnb_stream_t stream);

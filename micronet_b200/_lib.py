@@ -154,6 +154,7 @@ PROTOTYPES = {
     "mnb_xnor_post_bytes": (_L, [_SHAPE, C.POINTER(XnorPost)]),
     "mnb_xnor_conv_post": (C.c_int, [_SHAPE, _P, _P, _P, _P, C.POINTER(XnorPost), _P, _P]),
     "mnb_xnor_pack_act_post": (C.c_int, [_P, _I, _I, _I, _I, C.POINTER(XnorPost), _P, _P]),
+    "mnb_xnor_plan": (C.c_int, [_SHAPE, C.POINTER(XnorPost), _P]),
     "mnb_b1_supported": (C.c_int, [_SHAPE]),
     "mnb_b1_act_bytes": (_L, [_I, _I, _I, _I, _I]),
     "mnb_b1_pack_act": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
@@ -161,6 +162,7 @@ PROTOTYPES = {
     "mnb_b1_wimage_bytes": (_L, [_SHAPE]),
     "mnb_b1_pack_weight": (C.c_int, [_SHAPE, _P, _P, _P]),
     "mnb_b1_conv_fwd": (C.c_int, [_SHAPE, _P, _P, _P, _P, _P, _P, _P]),
+    "mnb_b1_plan": (C.c_int, [_SHAPE, C.POINTER(XnorPost), _P]),
     "mnb_b1_post_bytes": (_L, [_SHAPE, C.POINTER(XnorPost)]),
     "mnb_b1_conv_post": (C.c_int, [_SHAPE, _P, _P, _P, _P, C.POINTER(XnorPost), _P, _P, _P]),
     "mnb_b1_plane_maxpool": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),

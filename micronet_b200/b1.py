@@ -25,6 +25,21 @@ def supported(sh):
     return _sup_cache[k]
 
 
+PLAN_FIELDS = ("Nt", "n_ntiles", "u", "ksteps", "G", "col_tiles", "Wt", "BW", "TH", "TB", "row_tiles", "n_mtiles", "TG",
+               "ntg", "nstage", "post", "smem")
+
+
+def plan(sh, post=None):
+    """the launch plan of ``conv`` (post None) / ``conv_post`` for shape ``sh`` (mnb_b1_plan, host only): a dict of
+    PLAN_FIELDS, or None outside the cover"""
+    out = (C.c_int32 * len(PLAN_FIELDS))()
+    rc = L.load().mnb_b1_plan(C.byref(sh), None if post is None else C.byref(post), out)
+    if rc == L.E_UNSUPPORTED:
+        return None
+    L.check(rc, "b1_plan")
+    return dict(zip(PLAN_FIELDS, out))
+
+
 def act_bytes(b, c, h, w, groups):
     return int(L.load().mnb_b1_act_bytes(b, c, h, w, groups))
 

@@ -624,6 +624,21 @@ int mnb_b1_pack_weight(const mnb_conv_shape* s, const int16_t* w_int, void* w_im
   return 0;
 }
 
+int mnb_b1_plan(const mnb_conv_shape* s, const mnb_xnor_post* post, int32_t* out) {
+  b1::Plan pl;
+  int rc = b1::make_plan(s, pl);
+  if (rc != 0) return rc;
+  MNB_REQUIRE(out != nullptr, "b1_plan: null output");
+  if (post) {
+    rc = b1::check_post(post, s->out_c, pl.P, pl.Q);
+    if (rc != 0) return rc;
+  }
+  const int32_t v[] = {pl.Nt, pl.n_ntiles, pl.u, pl.ksteps, pl.G, pl.col_tiles, pl.Wt, pl.BW, pl.TH, pl.TB, pl.row_tiles,
+                       pl.n_mtiles, pl.TG, pl.ntg, pl.nstage, post != nullptr, pl.smem_bytes};
+  for (int i = 0; i < 17; ++i) out[i] = v[i];
+  return 0;
+}
+
 int mnb_b1_conv_fwd(const mnb_conv_shape* s, const void* a_plane, const void* w_img, const float* alpha, const float* bias,
                     float* y, int32_t* err_flag, mnb_stream_t stream) {
   return b1::run_conv(s, a_plane, w_img, alpha, bias, nullptr, y, err_flag, stream);

@@ -351,31 +351,51 @@ static int check_shape(const mnb_conv_shape* s) {
   return 0;
 }
 
+// the launch configuration of a shape that has passed check_shape: kernel instance, k-slices, grid and shared memory
+struct Plan {
+  int P, Q, nw, border, px, post, ksplit, kb, pblocks, smem, grid_y;
+  bool refused;              // shared memory or grid beyond what the launch allows: MNB_E_UNSUPPORTED, nothing launched
+  KernelFn fn;
+};
+
+static void make_plan(const mnb_conv_shape* s, bool post, Plan& pl) {
+  const int cout_g = s->out_c / s->groups, R = s->ker_h;
+  pl.P = (s->in_h + 2 * s->pad_h - R) / s->stride_h + 1;
+  pl.Q = (s->in_w + 2 * s->pad_w - s->ker_w) / s->stride_w + 1;
+  pl.nw = words_per_group(s->in_c / s->groups);
+  // border handling only where a tap can leave the image (never for an un-padded filter that fits)
+  pl.border = s->pad_h > 0 || (pl.P - 1) * s->stride_h + R > s->in_h || (pl.Q - 1) * s->stride_w + s->ker_w > s->in_w;
+  pl.post = post;
+  int rec_words = 0;
+  pl.px = 1;
+  pl.fn = pick(R, pl.nw, pl.border, &rec_words, &pl.px, post);
+  const int per_k = rec_words * 4 + (post ? 16 : 0);     // shared-memory bytes per output channel
+  const int64_t npix = (int64_t)s->batch * pl.P * pl.Q;
+  pl.pblocks = (int)((npix + NTHREADS * pl.px - 1) / (NTHREADS * pl.px));
+  // k-slices: enough blocks for ~4 per SM, at most 40 KB of channel records per block
+  int ksplit = 1;
+  while (cout_g / ksplit > 8 && ((int64_t)pl.pblocks * s->groups * ksplit < 4 * MNB_NUM_SMS ||
+                                 (int64_t)((cout_g + ksplit - 1) / ksplit) * per_k > 40 * 1024))
+    ++ksplit;
+  pl.kb = (cout_g + ksplit - 1) / ksplit;
+  pl.ksplit = (cout_g + pl.kb - 1) / pl.kb;
+  pl.smem = pl.kb * per_k;
+  pl.grid_y = s->groups * pl.ksplit;
+  pl.refused = pl.smem > 48 * 1024 || pl.grid_y > 65535;
+}
+
 // post: NULL for the fp32 output of mnb_xnor_conv_fwd.  The shape has passed check_shape (and check_post when post is set).
 static int launch(const mnb_conv_shape* s, const void* a_bits, const void* w_img, const float* alpha, const float* bias,
                   const mnb_xnor_post* post, void* out, mnb_stream_t stream) {
+  Plan pl;
+  make_plan(s, post != nullptr, pl);
+  if (pl.refused) return MNB_E_UNSUPPORTED;
   Params p;
   p.B = s->batch; p.G = s->groups; p.cin_g = s->in_c / s->groups; p.cout_g = s->out_c / s->groups;
   p.H = s->in_h; p.W = s->in_w; p.R = s->ker_h; p.S = s->ker_w; p.stride = s->stride_h; p.pad = s->pad_h;
-  p.P = (p.H + 2 * p.pad - p.R) / p.stride + 1;
-  p.Q = (p.W + 2 * p.pad - p.S) / p.stride + 1;
-  const int nw = words_per_group(p.cin_g), TW = p.R * p.S * nw;
-  // border handling only where a tap can leave the image (never for an un-padded filter that fits)
-  const bool border = p.pad > 0 || (p.P - 1) * p.stride + p.R > p.H || (p.Q - 1) * p.stride + p.S > p.W;
-  int rec_words = 0, px = 1;
-  KernelFn fn = pick(p.R, nw, border, &rec_words, &px, post != nullptr);
-  const int per_k = rec_words * 4 + (post ? 16 : 0);     // shared-memory bytes per output channel
-  const int64_t npix = (int64_t)p.B * p.P * p.Q;
-  const int pblocks = (int)((npix + NTHREADS * px - 1) / (NTHREADS * px));
-  // k-slices: enough blocks for ~4 per SM, at most 40 KB of channel records per block
-  int ksplit = 1;
-  while (p.cout_g / ksplit > 8 && ((int64_t)pblocks * p.G * ksplit < 4 * MNB_NUM_SMS ||
-                                   (int64_t)((p.cout_g + ksplit - 1) / ksplit) * per_k > 40 * 1024))
-    ++ksplit;
-  p.kb = (p.cout_g + ksplit - 1) / ksplit;
-  p.ksplit = (p.cout_g + p.kb - 1) / p.kb;
-  const size_t smem = (size_t)p.kb * per_k;
-  if (smem > 48 * 1024) return MNB_E_UNSUPPORTED;
+  p.P = pl.P; p.Q = pl.Q;
+  p.kb = pl.kb; p.ksplit = pl.ksplit;
+  const int TW = p.R * p.S * pl.nw;
   const uint32_t* words = (const uint32_t*)w_img;
   p.abits = (const uint32_t*)a_bits;
   p.wwords = words;
@@ -391,9 +411,8 @@ static int launch(const mnb_conv_shape* s, const void* a_bits, const void* w_img
     p.fmt = post->format; p.sg = post->shuffle_groups; p.pool = post->pool2;
     p.out_cin_g = s->out_c / post->out_groups; p.out_nw = words_per_group(p.out_cin_g);
   }
-  dim3 grid((unsigned)pblocks, (unsigned)(p.G * p.ksplit));
-  if (grid.y > 65535) return MNB_E_UNSUPPORTED;
-  fn<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
+  dim3 grid((unsigned)pl.pblocks, (unsigned)pl.grid_y);
+  pl.fn<<<grid, NTHREADS, (size_t)pl.smem, (cudaStream_t)stream>>>(p);
   MNB_LAUNCHED(1);
   return 0;
 }
@@ -499,6 +518,21 @@ int mnb_xnor_conv_post(const mnb_conv_shape* s, const void* a_bits, const void* 
     if (e != cudaSuccess) return mnb_fail((int)e, "xnor_conv_post: memset failed: %s", cudaGetErrorString(e));
   }
   return xnor::launch(s, a_bits, w_img, alpha, bias, post, out, stream);
+}
+
+int mnb_xnor_plan(const mnb_conv_shape* s, const mnb_xnor_post* post, int32_t* out) {
+  int rc = xnor::check_shape(s);
+  if (rc != 0) return rc;
+  MNB_REQUIRE(out != nullptr, "xnor_plan: null output");
+  xnor::Plan pl;
+  xnor::make_plan(s, post != nullptr, pl);
+  if (post) {
+    rc = xnor::check_post(post, s->out_c, pl.P, pl.Q);
+    if (rc != 0) return rc;
+  }
+  const int32_t v[] = {s->ker_h, pl.nw, pl.border, pl.px, pl.post, pl.ksplit, pl.kb, pl.pblocks, pl.smem, pl.refused};
+  for (int i = 0; i < 10; ++i) out[i] = v[i];
+  return 0;
 }
 
 int mnb_xnor_pack_act_post(const float* x, int32_t batch, int32_t channels, int32_t h, int32_t w, const mnb_xnor_post* post,

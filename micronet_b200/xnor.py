@@ -24,6 +24,20 @@ def supported(sh):
     return _sup_cache[k]
 
 
+PLAN_FIELDS = ("R", "NW", "border", "px", "post", "ksplit", "kb", "pblocks", "smem", "refused")
+
+
+def plan(sh, post=None):
+    """the launch plan of ``conv`` (post None) / ``conv_post`` for shape ``sh`` (mnb_xnor_plan, host only): a dict of
+    PLAN_FIELDS, or None outside the cover.  ``refused`` 1: the launch returns MNB_E_UNSUPPORTED."""
+    out = (C.c_int32 * len(PLAN_FIELDS))()
+    rc = L.load().mnb_xnor_plan(C.byref(sh), None if post is None else C.byref(post), out)
+    if rc == L.E_UNSUPPORTED:
+        return None
+    L.check(rc, "xnor_plan")
+    return dict(zip(PLAN_FIELDS, out))
+
+
 def pack_act(x, groups):
     lib = L.load()
     b, c, h, w = x.shape
@@ -80,5 +94,5 @@ def unpack(bits, shape, groups):
     words = bits.view(b, groups, nw, h, w)
     ch = torch.arange(c, device=bits.device)
     sel = words[:, ch // cg, (ch % cg) // 32]                                  # [B, C, H, W] word of each channel
-    bit = (sel >> (ch % 32).view(1, c, 1, 1).to(torch.int32)) & 1
+    bit = (sel >> ((ch % cg) % 32).view(1, c, 1, 1).to(torch.int32)) & 1           # bit of the channel within its group
     return (bit * 2 - 1).float()

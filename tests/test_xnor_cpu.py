@@ -91,6 +91,23 @@ def test_xnor_arithmetic_model_matches_a_convolution(case):
     assert np.array_equal(got, ref.astype(np.int64))
 
 
+@pytest.mark.parametrize("cg,groups", [(24, 3), (77, 2), (81, 2), (16, 16), (64, 2)])
+def test_unpack_reads_each_channel_at_its_bit_within_the_group(cg, groups):
+    """xnor.unpack (functional.materialized of a frozen layer's bit plane) against the layout of the numpy packer above:
+    channel j of a group sits at bit j % 32 of word j // 32, also when C/g is not a multiple of 32 (the pruned NIN-GC)"""
+    from micronet_b200 import xnor as X
+    g = torch.Generator().manual_seed(cg * groups)
+    x = torch.randn(2, cg * groups, 3, 5, generator=g)
+    nw = (cg + 31) // 32
+    words = np.zeros((2, groups, nw, 3, 5), dtype=np.uint64)
+    for gi in range(groups):
+        for n in range(nw):
+            ch = x[:, gi * cg + 32 * n: gi * cg + min(32 * n + 32, cg)].numpy()
+            words[:, gi, n] = _pack_bits(np.moveaxis(~(ch < 0), 1, -1))
+    bits = torch.from_numpy(words.astype(np.uint32).view(np.int32).reshape(-1))
+    assert torch.equal(X.unpack(bits, x.shape, groups), torch.where(x < 0, -1.0, 1.0))
+
+
 def test_xnor_host_queries():
     from micronet_b200 import _lib as L
     lib = L.load()
