@@ -458,6 +458,14 @@ typedef struct mnb_pk_post {
   const float* bn_gamma;
   const float* bn_beta;
   int32_t shuffle_groups;
+  /* terms_out > 0 with q == NULL (mnb_pk_conv_post only): no consumer quantizer - the consumer reads the fp32 value
+   * [ReLU](BatchNorm(y)) itself as terms_out (1..3) exact bf16 pieces, the term planes mnb_pk_pack_act writes from that
+   * tensor (qp == NULL), out_pk then holding terms_out planes of mnb_pk_act_bytes(B, C_out, OH, OW, 1) bytes each.  The
+   * frozen wbwtab graphs of fp32-activation models (prepare(A=32, W=2|3)): a binary / ternary conv -> nn.BatchNorm2d ->
+   * ReLU (WB:79-94, A=32) -> [channel_shuffle] -> the next QuantConv2d, which feeds its fp32 input to F.conv2d (WB:181-195).
+   * Same cover and refusals as the quantized consumer plane, and output channels per group % 8 != 0 (grouped or not) is
+   * MNB_E_UNSUPPORTED; q == NULL with terms_out == 0 (or q with terms_out != 0) and terms_out > 3 are MNB_E_ARG. */
+  int32_t terms_out;
 } mnb_pk_post;
 int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
                      const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, float* out,
@@ -526,6 +534,24 @@ int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int
 int mnb_pk_plane_maxpool_requant(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s,
                                  int32_t p, int32_t int8, const mnb_act_qparams* q_in, const mnb_act_qparams* q_out, void* out_pk,
                                  mnb_stream_t stream);
+/* Frozen wbwtab inference graphs with fp32 activations (prepare(A=32, W=2|3), WB:79-94: the "activation quantizer" is a ReLU):
+ * activations cross between layers as term planes (terms exact bf16 pieces, the mnb_pk_pack_act layout with qp == NULL).
+ *   mnb_pk_plane_maxpool_terms : max_pool2d(k, s, p) of the fp32 tensor a term plane holds (nin.py:51/56 3x3/2/1, nin_gc.py
+ *                                2x2/2/0, replacing ATen's max-pool of the ReLU output and the next conv's pack): values
+ *                                rebuilt exactly, window max with ATen's rule (first of equal values, NaN propagates),
+ *                                written as `terms` pieces of the pooled size.  Bitwise mnb_pk_pack_act of ATen max_pool2d of
+ *                                the decoded tensor.  Same cover as mnb_pk_plane_maxpool (square windows, 2 * p <= k, stride-1
+ *                                consumer); MNB_E_UNSUPPORTED outside it.
+ *   mnb_bn_relu_pack_terms_fwd : eval BatchNorm y' = fmaf(y - mean, gamma * invstd, beta) (all four NULL: none) [-> ReLU]
+ *                                [-> the consumer block's channel shuffle] of an fp32 NCHW tensor written as the consumer's
+ *                                `terms` term planes: the stem producer (fp32 stem conv -> nn.BatchNorm2d -> ReLU ->
+ *                                first QuantConv2d), the op sequence of mnb_pk_conv_post with terms_out.  channels % 8 == 0,
+ *                                shuffle groups dividing channels, else MNB_E_UNSUPPORTED; a partial BatchNorm set is MNB_E_ARG. */
+int mnb_pk_plane_maxpool_terms(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s,
+                               int32_t p, int32_t terms, void* out_pk, mnb_stream_t stream);
+int mnb_bn_relu_pack_terms_fwd(const float* x, int32_t batch, int32_t channels, int32_t hw, const float* mean,
+                               const float* invstd, const float* gamma, const float* beta, int32_t relu,
+                               int32_t out_shuffle_groups, int32_t terms, void* x_packed, mnb_stream_t stream);
 int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x);
 int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                  const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);

@@ -29,10 +29,10 @@ class ActQParams(C.Structure):
 
 class PkPost(C.Structure):
     """mnb_pk_post: the consumer of a frozen-inference producer (its quantizer and operand plane); the trailing fields (eval
-    BatchNorm, channel shuffle) are absent when left at zero"""
+    BatchNorm, channel shuffle, term planes of a consumer without a quantizer) are absent when left at zero"""
     _fields_ = [("q", C.POINTER(ActQParams)), ("relu", C.c_int32), ("phase_split", C.c_int32), ("out_pk", C.c_void_p),
                 ("bn_mean", C.c_void_p), ("bn_invstd", C.c_void_p), ("bn_gamma", C.c_void_p), ("bn_beta", C.c_void_p),
-                ("shuffle_groups", C.c_int32)]
+                ("shuffle_groups", C.c_int32), ("terms_out", C.c_int32)]
 
 
 XNOR_BITS, XNOR_PM1_BF16, XNOR_B1_PLANE = 0, 1, 2
@@ -138,6 +138,8 @@ PROTOTYPES = {
     "mnb_bn_relu_quant_pack_i8_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _ACTQ, _I, _P, _P]),
     "mnb_pk_plane_maxpool": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "mnb_pk_plane_maxpool_requant": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _ACTQ, _ACTQ, _P, _P]),
+    "mnb_pk_plane_maxpool_terms": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "mnb_bn_relu_pack_terms_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "mnb_pk_wgrad_scratch_bytes": (_L, [_SHAPE, _I, _I]),
     "mnb_pk_wgrad": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_pk_wgrad_taps_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),

@@ -645,6 +645,87 @@ __global__ void __launch_bounds__(256) plane_maxpool_requant_kernel(const uint4*
   plane_maxpool_body<I8, true>(in, planes, H, W, k, s, pad, OH, OW, out, tab);
 }
 
+// the exact split of pack_act_body: piece t of each of 8 values into unit dst[t * term_vecs], residues carried over
+__device__ __forceinline__ void store_terms8(float (&v)[8], int terms, uint4* __restrict__ dst, int64_t term_vecs) {
+  for (int tm = 0; tm < terms; ++tm) {
+    uint32_t pk4[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      pk4[j] = pack2(v[2 * j], v[2 * j + 1]);
+      v[2 * j] -= __uint_as_float(pk4[j] << 16);
+      v[2 * j + 1] -= __uint_as_float(pk4[j] & 0xffff0000u);
+    }
+    dst[(int64_t)tm * term_vecs] = make_uint4(pk4[0], pk4[1], pk4[2], pk4[3]);
+  }
+}
+
+// max_pool2d(k, s, p) of an fp32 tensor held as `terms` exact bf16 pieces [t][b][c/8][H][W][8] (mnb_pk_plane_maxpool_terms):
+// each value is rebuilt as p0 + p1 + p2 (exact: the pieces are the successive rounding residues of pack_act_body), the window
+// max is taken with ATen's rule (row-major window order, the first of equal values stays, NaN wins) and split again.  One
+// thread = one output position of one 8-channel unit.
+__global__ void __launch_bounds__(256) plane_maxpool_terms_kernel(const uint4* __restrict__ in, int64_t planes, int H, int W,
+                                                                  int k, int s, int pad, int OH, int OW, int terms,
+                                                                  uint4* __restrict__ out) {
+  const int64_t total = planes * OH * OW, in_vecs = planes * H * W;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int ow = (int)(idx % OW);
+    const int64_t t = idx / OW;
+    const int oh = (int)(t % OH);
+    const uint4* src = in + (t / OH) * H * W;
+    const int h0 = oh * s - pad, w0 = ow * s - pad;
+    float m[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m[e] = -INFINITY;     // ATen's start value: the first window value always replaces it
+    for (int i = max(h0, 0); i < min(h0 + k, H); ++i)
+      for (int j = max(w0, 0); j < min(w0 + k, W); ++j) {
+        const uint4* px = src + (int64_t)i * W + j;
+        float v[8];
+#pragma unroll
+        for (int tm = 0; tm < 3; ++tm) {
+          if (tm >= terms) break;
+          const uint4 u = __ldg(px + (int64_t)tm * in_vecs);
+          const float f[8] = {__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                              __uint_as_float(u.y & 0xffff0000u), __uint_as_float(u.z << 16), __uint_as_float(u.z & 0xffff0000u),
+                              __uint_as_float(u.w << 16), __uint_as_float(u.w & 0xffff0000u)};
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[e] = tm ? v[e] + f[e] : f[e];
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          if (v[e] > m[e] || v[e] != v[e]) m[e] = v[e];
+      }
+    store_terms8(m, terms, out + idx, total);
+  }
+}
+
+// eval BatchNorm [-> ReLU] [-> channel shuffle] of an fp32 NCHW tensor into the consumer's term planes (mnb_bn_relu_pack_terms_fwd):
+// the op sequence of the XTERMS conv epilogue.  One thread = one position of one consumer 8-channel unit; a block's threads
+// take consecutive positions, so each channel's loads coalesce.
+__global__ void __launch_bounds__(256) bn_relu_pack_terms_kernel(const float* __restrict__ x, int batch, int channels, int hw,
+                                                                 int sg, const float* __restrict__ mean,
+                                                                 const float* __restrict__ invstd,
+                                                                 const float* __restrict__ gamma,
+                                                                 const float* __restrict__ beta, int relu, int terms,
+                                                                 uint4* __restrict__ xp) {
+  const int c8n = channels / 8, cpg = channels / sg;
+  const int64_t total = (int64_t)batch * c8n * hw;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int pos = (int)(idx % hw);
+    const int64_t t = idx / hw;
+    const int oc8 = (int)(t % c8n), b = (int)(t / c8n);
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int oc = oc8 * 8 + j;
+      const int c = sg > 1 ? (oc % sg) * cpg + oc / sg : oc;   // inverse of out[:, a*sg + b] = in[:, b*cpg + a]
+      float y = __ldg(x + ((int64_t)b * channels + c) * hw + pos);
+      if (mean) y = fmaf(__fsub_rn(y, __ldg(mean + c)), __fmul_rn(__ldg(gamma + c), __ldg(invstd + c)), __ldg(beta + c));
+      v[j] = relu ? fmaxf(y, 0.f) : y;
+    }
+    store_terms8(v, terms, xp + idx, total);
+  }
+}
+
 // IAO QuantAdd of a frozen inference graph + the consuming conv's quantizer and operand packing in one pass (see
 // mnb_quant_add_pack_fwd): one thread = one pixel of one 16-byte unit of the consumer's plane (CPU = 8 channels as bf16,
 // or 16 channels as int8 for an int8 consumer), same arithmetic as quant_add_fwd_kernel (mnb_quant.cu) followed by
@@ -963,6 +1044,9 @@ struct ConvParams {
   const float *post_mean, *post_invstd, *post_gamma, *post_beta;
   int post_sg;
   int* err;
+  // XTERMS instances (no consumer quantizer): the consumer's fp32 operand as post_terms exact bf16 pieces (after err, so
+  // the parameter offsets of every other instance stay as they were)
+  int post_terms;
 };
 
 struct alignas(16) ConvShared {
@@ -1000,7 +1084,10 @@ constexpr int kConvThreads = 384;   // warp 0 TMA, warps 4..11 two MMA + epilogu
 // XPOST (forward with a consumer plane only): the consumer plane with an eval BatchNorm and / or a channel shuffle in front of
 // the quantizer.  Instances of their own: with both epilogues in one instance the plain consumer plane's code (the IAO frozen
 // graphs) loses registers to the other and ran 22-25% slower on frozen ResNet-18 (DESIGN.md 4.15).
-template <bool SEG, int NT, bool I8 = false, bool XPOST = false>
+// XTERMS (bf16 forward with a consumer plane only, no consumer quantizer): [eval BatchNorm] [-> ReLU] [-> shuffle] and the
+// value's exact split into post_terms bf16 pieces, the term planes mnb_pk_pack_act writes from the same fp32 tensor (frozen
+// wbwtab graphs with fp32 activations, DESIGN.md 4.20).  Instances of their own for the same reason.
+template <bool SEG, int NT, bool I8 = false, bool XPOST = false, bool XTERMS = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1,
                const __grid_constant__ CUtensorMap tmap2, const __grid_constant__ ConvParams p) {
@@ -1074,7 +1161,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
     const float a_sc = p.a_scale ? __ldg(p.a_scale) : p.a_scale_const;
     MnbActQ pq;
     float pzp = 0.f;
-    if (p.post_out) {
+    if (!XTERMS && p.post_out) {
       pq = mnb_load_actq(p.post_q);
       if (p.post_q.mode == MNB_ACT_IAO && p.post_q.zero_point) pzp = __ldg(p.post_q.zero_point);
     }
@@ -1099,7 +1186,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           if (p.bias) bs = __ldg(p.bias + n_base + n);
         }
         sh.epi_scale[n] = scv; sh.epi_bias[n] = bs;
-        if constexpr (XPOST) {
+        if constexpr (XPOST || XTERMS) {
           if (p.post_sg > 1 && n < n_cnt) {
             const int c = n_base + n, cpg = p.NOUT / p.post_sg;
             sh.epi_dst[n] = (uint16_t)((c % cpg) * p.post_sg + c / cpg);
@@ -1215,6 +1302,60 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
 #pragma unroll
           for (int k = 0; k < 16; ++k, cp += plane)
             if (n0 + k < n_cnt) *cp = (int16_t)__float2int_rn(r[k]);
+          return;
+        }
+        if constexpr (XTERMS) {
+          // one 8-channel unit at a time (C_out per group % 8 == 0, refused otherwise on the host: an octet is all valid or
+          // all past the tile): the value after [BatchNorm] [ReLU], split into pieces exactly as pack_act_body splits an
+          // fp32 tensor
+          float* op0 = p.out + orow + (int64_t)n0 * plane;
+          const int64_t oct_stride = p.post_split ? (int64_t)(p.OH >> 1) * (p.OW >> 1) : plane;
+          const int64_t term_vecs = (int64_t)p.B * p.C8O * plane;     // 16-byte units per term plane
+#pragma unroll
+          for (int o = 0; o < 2; ++o) {
+            if (n0 + 8 * o >= n_cnt) break;
+            float v[8];
+#pragma unroll
+            for (int h4 = 0; h4 < 2; ++h4) {
+              const int k0 = 8 * o + 4 * h4;
+              const float4 sc4 = *reinterpret_cast<const float4*>(&sh.epi_scale[n0 + k0]);
+              const float4 bs4 = *reinterpret_cast<const float4*>(&sh.epi_bias[n0 + k0]);
+              const float scv[4] = {sc4.x, sc4.y, sc4.z, sc4.w}, bsv[4] = {bs4.x, bs4.y, bs4.z, bs4.w};
+              float mu[4] = {0.f, 0.f, 0.f, 0.f}, gs[4] = {0.f, 0.f, 0.f, 0.f}, be[4] = {0.f, 0.f, 0.f, 0.f};
+              if (p.post_mean) {   // 16-byte aligned arrays, C_out % 4 == 0 (checked on the host)
+                const int c0 = n_base + n0 + k0;
+                const float4 m4 = __ldg(reinterpret_cast<const float4*>(p.post_mean + c0));
+                const float4 g4 = __ldg(reinterpret_cast<const float4*>(p.post_gamma + c0));
+                const float4 i4 = __ldg(reinterpret_cast<const float4*>(p.post_invstd + c0));
+                const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.post_beta + c0));
+                mu[0] = m4.x; mu[1] = m4.y; mu[2] = m4.z; mu[3] = m4.w;
+                gs[0] = __fmul_rn(g4.x, i4.x); gs[1] = __fmul_rn(g4.y, i4.y); gs[2] = __fmul_rn(g4.z, i4.z); gs[3] = __fmul_rn(g4.w, i4.w);
+                be[0] = b4.x; be[1] = b4.y; be[2] = b4.z; be[3] = b4.w;
+              }
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                float t = fmaf(r[k0 + j], scv[j], bsv[j]);
+                if (p.out) op0[(int64_t)(k0 + j) * plane] = t;
+                if (p.post_mean) t = fmaf(__fsub_rn(t, mu[j]), gs[j], be[j]);
+                v[4 * h4 + j] = p.post_relu ? fmaxf(t, 0.f) : t;
+              }
+            }
+            if (p.post_sg > 1) {   // consecutive channels land in different consumer units: one element at a time
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const int oc = sh.epi_dst[n0 + 8 * o + j];
+                __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.post_out) + (prow + (int64_t)(oc >> 3) * oct_stride) * 8 + (oc & 7);
+                float t = v[j];
+                for (int tm = 0; tm < p.post_terms; ++tm) {
+                  const uint32_t w = pack2(t, 0.f);
+                  dst[(int64_t)tm * term_vecs * 8] = __ushort_as_bfloat16((unsigned short)(w & 0xffffu));
+                  t -= __uint_as_float(w << 16);
+                }
+              }
+            } else {
+              store_terms8(v, p.post_terms, p.post_out + prow + (int64_t)(((n_base + n0) >> 3) + o) * oct_stride, term_vecs);
+            }
+          }
           return;
         }
         if constexpr (XPOST) {
@@ -2503,6 +2644,45 @@ extern "C" int mnb_pk_plane_maxpool_requant(const void* in_pk, int32_t batch, in
   return plane_maxpool(in_pk, batch, channels, h, w, k, s, p, int8, q_in, q_out, out_pk, stream);
 }
 
+extern "C" int mnb_pk_plane_maxpool_terms(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
+                                          int32_t s, int32_t p, int32_t terms, void* out_pk, mnb_stream_t stream) {
+  MNB_REQUIRE(in_pk && out_pk && in_pk != out_pk, "NULL or aliased pk_plane_maxpool_terms pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0 && terms >= 1 && terms <= 3, "bad pk_plane_maxpool_terms arguments");
+  MNB_REQUIRE(((reinterpret_cast<uintptr_t>(in_pk) | reinterpret_cast<uintptr_t>(out_pk)) & 15) == 0,
+              "packed tensors must be 16-byte aligned");
+  if (k < 1 || s < 1 || p < 0 || 2 * p > k || h + 2 * p < k || w + 2 * p < k)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool_terms: kernel %d, stride %d, padding %d on %d x %d (needs 2 * p <= k)",
+                    k, s, p, h, w);
+  const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
+  const int64_t planes = (int64_t)batch * ((channels + 7) / 8);
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(planes * oh * ow, 256), (int64_t)MNB_NUM_SMS * 16);
+  pk::plane_maxpool_terms_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint4*>(in_pk), planes, h, w, k,
+                                                                            s, p, oh, ow, terms, reinterpret_cast<uint4*>(out_pk));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int mnb_bn_relu_pack_terms_fwd(const float* x, int32_t batch, int32_t channels, int32_t hw, const float* mean,
+                                          const float* invstd, const float* gamma, const float* beta, int32_t relu,
+                                          int32_t out_shuffle_groups, int32_t terms, void* x_packed, mnb_stream_t stream) {
+  MNB_REQUIRE(x && x_packed, "NULL bn_relu_pack_terms pointer");
+  MNB_REQUIRE(batch > 0 && channels > 0 && hw > 0 && terms >= 1 && terms <= 3, "bad bn_relu_pack_terms arguments");
+  const int nbn = (mean != nullptr) + (invstd != nullptr) + (gamma != nullptr) + (beta != nullptr);
+  MNB_REQUIRE(nbn == 0 || nbn == 4, "bn_relu_pack_terms: the BatchNorm needs all four of mean, invstd, gamma, beta");
+  MNB_REQUIRE((reinterpret_cast<uintptr_t>(x_packed) & 15) == 0, "packed tensor must be 16-byte aligned");
+  MNB_REQUIRE(out_shuffle_groups >= 1, "bn_relu_pack_terms: shuffle groups %d", out_shuffle_groups);
+  if (channels % 8 || channels % out_shuffle_groups)
+    return mnb_fail(MNB_E_UNSUPPORTED, "bn_relu_pack_terms: needs channels %% 8 == 0 and shuffle groups %d dividing %d channels",
+                    out_shuffle_groups, channels);
+  const int64_t total = (int64_t)batch * (channels / 8) * hw;
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 16);
+  pk::bn_relu_pack_terms_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, batch, channels, hw, out_shuffle_groups, mean, invstd,
+                                                                           gamma, beta, relu, terms,
+                                                                           reinterpret_cast<uint4*>(x_packed));
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
 // host only: out[0..15] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator
 //                          columns MT * Nt, TH, TB, BW, n_mtiles, n_items, ny},
 //            out[16..20] = {segmented, seg_len, npairs, col_tiles, n_mgroups}; the first min(n, 21) are written
@@ -2575,11 +2755,19 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     if (!i8_quantizer(post->q)) return unsupported(kI8QuantizerRule);
     if (pl.G > 1 && (pl.ng % 16)) return unsupported("int8 consumer plane of a grouped conv needs channels per group % 16 == 0");
   }
+  const bool terms_out = post && !post->q && post->terms_out > 0;    // consumer term planes (no quantizer)
   if (post) {
     MNB_REQUIRE(mode == 0 && !bits8, "pk conv: a fused consumer is a forward-only (inference) option");
-    MNB_REQUIRE(post->q && post->out_pk && (reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "pk conv: consumer plane / quantizer");
-    MNB_REQUIRE(post->q->mode == MNB_ACT_DOREFA || post->q->mode == MNB_ACT_IAO, "pk conv: consumer quantizer must be DoReFa or IAO");
-    MNB_REQUIRE(post->q->bits >= 2 && post->q->bits <= 8, "pk conv: consumer levels must fit one bf16 piece (2..8 bits)");
+    MNB_REQUIRE(post->out_pk && (reinterpret_cast<uintptr_t>(post->out_pk) & 15) == 0, "pk conv: consumer plane");
+    if (terms_out) {
+      MNB_REQUIRE(post->terms_out <= 3, "pk conv: %d consumer term planes (1..3)", post->terms_out);
+      // the XTERMS epilogue stores whole 8-channel units without a per-channel tail (grouped or not)
+      if (pl.ng % 8) return unsupported("consumer term planes need output channels per group % 8 == 0");
+    } else {
+      MNB_REQUIRE(post->q && post->terms_out == 0, "pk conv: a consumer quantizer, or terms_out without one");
+      MNB_REQUIRE(post->q->mode == MNB_ACT_DOREFA || post->q->mode == MNB_ACT_IAO, "pk conv: consumer quantizer must be DoReFa or IAO");
+      MNB_REQUIRE(post->q->bits >= 2 && post->q->bits <= 8, "pk conv: consumer levels must fit one bf16 piece (2..8 bits)");
+    }
     if (pl.G > 1 && (pl.ng % 8)) return unsupported("fused consumer of a grouped conv needs channels per group % 8 == 0");
     if (post->phase_split && ((pl.OH | pl.OW) & 1)) return unsupported("stride-2 consumer of an odd-sized plane");
     // the consumer epilogue is compiled into the single-product kernels only: in the segmented ones (several piece
@@ -2631,9 +2819,11 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   p.n_scale = n_scale; p.a_scale = a_scale; p.a_scale_const = a_scale_const; p.bias = bias; p.bits8 = bits8; p.gain = gain;
   p.out = out; p.err = err_flag; p.codes = codes; p.dec = dec;
   if (post) {
-    p.post_out = reinterpret_cast<uint4*>(post->out_pk); p.post_q = *post->q; p.post_relu = post->relu; p.post_split = post->phase_split;
+    p.post_out = reinterpret_cast<uint4*>(post->out_pk); p.post_relu = post->relu; p.post_split = post->phase_split;
+    if (!terms_out) p.post_q = *post->q;
     p.post_mean = post->bn_mean; p.post_invstd = post->bn_invstd; p.post_gamma = post->bn_gamma; p.post_beta = post->bn_beta;
     p.post_sg = post->shuffle_groups;
+    p.post_terms = terms_out ? post->terms_out : 0;
   }
   { static const int dbg = [] { const char* e = getenv("MNB_PK_DEBUG"); return e ? atoi(e) : 0; }(); p.dbg = dbg; }
   CUtensorMap tm[3];
@@ -2647,17 +2837,18 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
   const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
   using ConvFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
-#define MNB_PK_CONV_FNS(SEG, I8, X) {pk_conv_kernel<SEG, 16, I8, X>, pk_conv_kernel<SEG, 32, I8, X>, pk_conv_kernel<SEG, 48, I8, X>, \
-                                     pk_conv_kernel<SEG, 64, I8, X>, pk_conv_kernel<SEG, 96, I8, X>, pk_conv_kernel<SEG, 128, I8, X>}
-  static const ConvFn fns[5][6] = {MNB_PK_CONV_FNS(false, false, false), MNB_PK_CONV_FNS(true, false, false),
-                                   MNB_PK_CONV_FNS(false, true, false), MNB_PK_CONV_FNS(false, false, true),
-                                   MNB_PK_CONV_FNS(false, true, true)};
+#define MNB_PK_CONV_FNS(SEG, I8, X, T) {pk_conv_kernel<SEG, 16, I8, X, T>, pk_conv_kernel<SEG, 32, I8, X, T>,                       \
+                                        pk_conv_kernel<SEG, 48, I8, X, T>, pk_conv_kernel<SEG, 64, I8, X, T>,                       \
+                                        pk_conv_kernel<SEG, 96, I8, X, T>, pk_conv_kernel<SEG, 128, I8, X, T>}
+  static const ConvFn fns[6][6] = {MNB_PK_CONV_FNS(false, false, false, false), MNB_PK_CONV_FNS(true, false, false, false),
+                                   MNB_PK_CONV_FNS(false, true, false, false), MNB_PK_CONV_FNS(false, false, true, false),
+                                   MNB_PK_CONV_FNS(false, true, true, false), MNB_PK_CONV_FNS(false, false, false, true)};
 #undef MNB_PK_CONV_FNS
   int ki = -1;
   for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
   if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
   const bool xpost = post && (post->bn_mean || post->shuffle_groups > 1);   // (segmented plans refuse a post above)
-  const ConvFn fn = fns[cpu == 16 ? (xpost ? 4 : 2) : (pl.segmented ? 1 : (xpost ? 3 : 0))][ki];
+  const ConvFn fn = fns[terms_out ? 5 : cpu == 16 ? (xpost ? 4 : 2) : (pl.segmented ? 1 : (xpost ? 3 : 0))][ki];
   if (int e = set_max_smem(fn, kSmemBudget)) return e;
   fn<<<dim3(gx, pl.ny), kConvThreads, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
   MNB_LAUNCHED(1);

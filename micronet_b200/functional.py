@@ -285,8 +285,8 @@ def materialized(t):
     storage was never written) - the +-1 tensor rebuilt from the bf16 operand plane [b][c/8][h][w][8], or - for a wbwtab conv
     that handed its output to its BatchNorm as int16 codes (``codes_out``) - that output decoded with the conv epilogue's own
     fmaf, or - for the output of a frozen wbwtab layer (wbwtab.freeze_inference) - the +-1 tensor its consumer's bit plane
-    encodes (bit plane or b1 plane).  Plumbing for tests, hooks and readers outside the fused producers; the training step
-    never calls it."""
+    encodes (bit plane or b1 plane), or the fp32 tensor whose exact pieces a frozen A=32 producer wrote (term planes).
+    Plumbing for tests, hooks and readers outside the fused producers; the training step never calls it."""
     xbits = getattr(t, "_mnb_xbits", None)
     if xbits is not None:
         from . import xnor as XN
@@ -295,6 +295,10 @@ def materialized(t):
     if b1p is not None:
         from . import b1 as B1
         return B1.unpack(b1p[1], t.shape, b1p[3])
+    terms = getattr(t, "_mnb_terms", None)
+    if terms is not None:        # term planes of a frozen A=32 wbwtab producer (wbwtab.freeze_inference)
+        from . import pk as PK
+        return PK.unpack_terms(terms[1], t.shape, terms[4], split=terms[3])
     codes = getattr(t, "_mnb_codes", None)
     if codes is not None:
         b, c = t.shape[0], t.shape[1]

@@ -170,6 +170,55 @@ def conv_post(sh, a_pk, terms_a, w_img, terms_w, out, post_qp, post_plane, post_
                                 L.tc_err_flag(a_pk.device).data_ptr(), L.stream())
 
 
+# ---- term planes as a hand-off (frozen wbwtab graphs with fp32 activations): the consumer reads an fp32 value as T exact pieces
+def terms_plane(b, c, h, w, terms, device):
+    """empty term planes (``terms`` bf16 pieces) of a conv that reads a [b, c, h, w] fp32 activation"""
+    return torch.empty(terms * int(L.load().mnb_pk_act_bytes(b, c, h, w, 1)), dtype=torch.uint8, device=device)
+
+
+def unpack_terms(plane, shape, terms, split=False):
+    """the fp32 [b, c, h, w] tensor a term plane holds (p0 + p1 + p2, exact); ``split``: phase-split layout"""
+    b, c, h, w = shape
+    c8 = (c + 7) // 8
+    pl = plane.view(torch.bfloat16).float()
+    if split:
+        pl = pl.view(terms, b, 2, 2, c8, h // 2, w // 2, 8).permute(0, 1, 4, 7, 5, 2, 6, 3).reshape(terms, b, c8 * 8, h, w)
+    else:
+        pl = pl.view(terms, b, c8, h, w, 8).permute(0, 1, 2, 5, 3, 4).reshape(terms, b, c8 * 8, h, w)
+    out = pl[0].clone()
+    for t in range(1, terms):
+        out += pl[t]
+    return out[:, :c].contiguous()
+
+
+def conv_post_terms(sh, a_pk, w_img, out, plane, terms, relu=True, split=False, n_scale=None, bias=None, bn=None,
+                    shuffle_groups=1):
+    """forward conv (activation ``terms``-piece plane, one piece of integer weight levels) whose epilogue writes the
+    consumer's ``terms`` term planes of [BatchNorm] [ReLU] [shuffle] of its output; out may be None.  Returns the C status."""
+    post = L.PkPost(None, 1 if relu else 0, 1 if split else 0, plane.data_ptr())
+    if bn is not None:
+        post.bn_mean, post.bn_invstd, post.bn_gamma, post.bn_beta = (t.data_ptr() for t in bn)
+    post.shuffle_groups, post.terms_out = int(shuffle_groups), int(terms)
+    return L.load().mnb_pk_conv_post(C.byref(sh), a_pk.data_ptr(), terms, w_img.data_ptr(), 1, L.ptr(n_scale), None, 1.0,
+                                     L.ptr(bias), L.ptr(out), C.byref(post), L.tc_err_flag(a_pk.device).data_ptr(), L.stream())
+
+
+def bn_relu_pack_terms(x, bn, relu, shuffle_groups, terms, plane):
+    """mnb_bn_relu_pack_terms_fwd of a contiguous fp32 [b, c, h, w] x into ``plane``; bn = (mean, invstd, gamma, beta) or None.
+    Returns the C status."""
+    b, c, h, w = x.shape
+    mean, invstd, gamma, beta = (None,) * 4 if bn is None else (t.data_ptr() for t in bn)
+    return L.load().mnb_bn_relu_pack_terms_fwd(x.data_ptr(), b, c, h * w, mean, invstd, gamma, beta, 1 if relu else 0,
+                                               int(shuffle_groups), terms, plane.data_ptr(), L.stream())
+
+
+def plane_maxpool_terms(plane, b, c, h, w, k, s, p, terms):
+    """(C status, pooled term planes) of max_pool2d(k, s, p) of the fp32 tensor a term plane holds (mnb_pk_plane_maxpool_terms)"""
+    oh, ow = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    out = terms_plane(b, c, oh, ow, terms, plane.device)
+    return L.load().mnb_pk_plane_maxpool_terms(plane.data_ptr(), b, c, h, w, k, s, p, terms, out.data_ptr(), L.stream()), out
+
+
 # ---- int8 operands (frozen inference graphs, symmetric IAO): planes [b][c/16][h][w][16] s8, s8 x s8 -> s32 wgmma
 def i8_plan(sh):
     """plan of mnb_pk_i8_conv as a list of the 21 mnb_pk_conv_plan_ex fields, None outside the int8 cover (host only)"""

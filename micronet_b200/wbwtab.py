@@ -430,6 +430,280 @@ def _undo(model):
             obj.__dict__.pop(key, None)
 
 
+# --------------------------------------------------------------------------
+# frozen inference graphs with fp32 activations (A = 32): term-plane hand-offs (DESIGN.md 4.20)
+# --------------------------------------------------------------------------
+A32_TERMS = 3       # exact bf16 pieces of an fp32 activation (the packed-operand family's split, pk.pack_act with qp None)
+A32_PLANE = "terms3"
+
+
+def _a32_block(blk):
+    """(conv, BatchNorm, ReLU) of a conv-bn-act block of an A=32 model (the act: ActivationQuantizer(A=32), WB:79-94, or the
+    nn.ReLU behind the head), else None"""
+    parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
+    if len(parts) != 3 or not isinstance(parts[0], nn.Conv2d):
+        return None
+    conv, bn, act = parts
+    if type(bn) is not nn.BatchNorm2d or not (bn.affine and bn.track_running_stats):
+        return None
+    if not ((type(act) is ActivationQuantizer and act.A == 32) or type(act) is nn.ReLU):
+        return None
+    return conv, bn, act
+
+
+def _a32_freezable(conv):
+    """does this QuantConv2d run frozen on term planes: binary / ternary weights whose levels freeze (frozen_levels: a finite
+    alpha), zero padding, and a packed-operand forward at terms (3, 1) on a nominal shape (batch 1, 32 x 32)"""
+    from . import pk as PK
+    if (type(conv) is not QuantConv2d or conv.training or conv.padding_mode != "zeros" or isinstance(conv.padding, str)
+            or conv.weight_quantizer.W not in (2, 3)):
+        return False
+    # (as _frozen_kernel: the QAT weight quantizer is not run here, W = 2 would centre the parameter in place)
+    if conv.quant_inference:
+        if frozen_levels(conv) is None:
+            return False
+    elif conv.weight_quantizer.W == 3 and not bool((conv.weight.detach().abs().amax(dim=(1, 2, 3)) > 0).all()):
+        return False
+    sh = L.ConvShape(1, conv.in_channels, 32, 32, conv.out_channels, conv.kernel_size[0], conv.kernel_size[1], conv.stride[0],
+                     conv.stride[1], conv.padding[0], conv.padding[1], conv.dilation[0], conv.dilation[1], conv.groups)
+    return L.PK_MODE != "off" and PK.supported(sh, 0, A32_TERMS, 1)
+
+
+class _TermLink:
+    """a producer -> consumer hand-off of an A=32 graph: the consumer conv, the eval BatchNorm the producer applies before the
+    ReLU, the consumer block's channel shuffle and the max-pool (module, k, s, p) in between, which runs on the term plane"""
+
+    def __init__(self, cconv, bn, sg, pool):
+        self.cconv, self.bn, self.sg, self.pool = cconv, bn, int(sg), pool
+        self.target = pool[0] if pool is not None else cconv
+        self._invstd = None
+
+    @property
+    def split(self):
+        return self.cconv.stride[0] == 2 and self.pool is None
+
+    def read_shape(self, out_shape):
+        if self.pool is None:
+            return tuple(out_shape)
+        _, k, s, p = self.pool
+        b, c, h, w = out_shape
+        return (b, c, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1)
+
+    def accepts(self, out_shape):
+        """will the consumer read the term plane of a producer output of this shape (the pk forward at terms (3, 1) on its
+        plain, unsplit or phase-split plane)?"""
+        from . import pk as PK
+        c = self.cconv
+        b, ch, h, w = self.read_shape(out_shape)
+        if ch != c.in_channels or PK.padded(ch, c.groups) or ch % 8:
+            return False
+        if self.sg > 1 and (ch % self.sg or self.split):
+            return False
+        if self.split and (h | w) & 1:
+            return False
+        sh = F_._shape_struct((b, ch, h, w), c.weight.shape, c.stride, c.padding, c.dilation, c.groups)
+        return L.PK_MODE != "off" and PK.supported(sh, 0, A32_TERMS, 1)
+
+    def bn_tensors(self):
+        """(mean, invstd, gamma, beta) of the eval BatchNorm (running statistics); invstd re-computed when running_var changes"""
+        import torch
+        bn = self.bn
+        rv = bn.running_var
+        key = (rv.data_ptr(), rv._version, float(bn.eps))
+        if self._invstd is None or self._invstd[0] != key:
+            self._invstd = (key, torch.rsqrt(rv + bn.eps))
+        return bn.running_mean, self._invstd[1], bn.weight.detach(), bn.bias.detach()
+
+    def tag(self, plane, shape):
+        import torch
+        y = torch.empty(shape, dtype=torch.float32, device="meta")   # shape only: the data lives in the term plane
+        y._mnb_terms = (self.target, plane, y._version, self.split, A32_TERMS)
+        return y
+
+
+def _handed_terms(module, x):
+    """the term plane a frozen producer (or a term-plane pool) wrote for ``module``, if ``x`` is that unmodified output"""
+    pre = getattr(x, "_mnb_terms", None)
+    if pre is not None and pre[0] is module and x._version == pre[2]:
+        return pre[1]
+    return None
+
+
+def _a32_passthrough(m, link, x):
+    """the BatchNorm / ReLU of a block whose producer wrote its consumer's term plane: the tagged output passes through;
+    anything else (a producer that wrote fp32) runs the module as usual"""
+    _check_eval(m)
+    if _handed_terms(link.target, x) is not None:
+        return x
+    return type(m).forward(m, x)
+
+
+def _a32_pool_forward(pool, link, x):
+    """the max-pool between a frozen producer and its consumer, on the producer's term plane (mnb_pk_plane_maxpool_terms)"""
+    from . import pk as PK
+    _check_eval(pool)
+    plane = _handed_terms(pool, x)
+    if plane is not None:
+        _, k, s, p = link.pool
+        b, c, h, w = x.shape
+        rc, out = F_._timed("plane_pool", L.ConvShape(b, c, h, w, c, k, k, s, s, p, p, 1, 1, 1),
+                            lambda: PK.plane_maxpool_terms(plane, b, c, h, w, k, s, p, A32_TERMS))
+        if rc == 0:
+            y = link.tag(out, link.read_shape(x.shape))
+            y._mnb_terms = (link.cconv,) + y._mnb_terms[1:]
+            return y
+        if rc != L.E_UNSUPPORTED:
+            L.check(rc, "pk_plane_maxpool_terms")
+        # the pool as usual on the decoded tensor, in the producer's channel order: the plane holds the consumer's (shuffled)
+        # order, and the consumer applies its block's shuffle itself when no plane arrives (shuffle with C / sg groups is the
+        # inverse of the shuffle with sg)
+        y = F_.materialized(x)
+        if link.sg > 1:
+            from .frozen_graph import shuffle
+            y = shuffle(y, y.shape[1] // link.sg)
+        return type(pool).forward(pool, y)
+    return type(pool).forward(pool, F_.materialized(x))
+
+
+def _a32_produce(link, y):
+    """eval BatchNorm + ReLU of the fp32 tensor y written as its consumer's term planes with the consumer block's shuffle
+    (mnb_bn_relu_pack_terms_fwd): the tagged placeholder, or None when the producer does not take y (y is left as it is)"""
+    import torch
+    from . import pk as PK
+    if not (y.dim() == 4 and y.is_cuda and y.dtype == torch.float32 and not link.split and link.accepts(y.shape)):
+        return None
+    b, c, h, w = y.shape
+    y = y.contiguous()
+    plane = PK.terms_plane(b, c, h, w, A32_TERMS, y.device)
+    rc = PK.bn_relu_pack_terms(y, link.bn_tensors(), True, link.sg, A32_TERMS, plane)
+    if rc == 0:
+        return link.tag(plane, y.shape)
+    if rc != L.E_UNSUPPORTED:
+        L.check(rc, "bn_relu_pack_terms")
+    return None
+
+
+def _a32_stem_forward(bn, link, x):
+    """the BatchNorm behind the fp32 stem conv: with the ReLU and the consumer block's shuffle, written straight as the first
+    quantized conv's term plane (_a32_produce); the BatchNorm as usual where the producer does not take the tensor"""
+    _check_eval(bn)
+    x = F_.materialized(x)
+    out = _a32_produce(link, x)
+    return out if out is not None else type(bn).forward(bn, x)
+
+
+def _epilogue_hand_off(link, sh):
+    """does the conv's epilogue write its consumer's term planes?  Else it writes fp32 and the stem producer writes the planes
+    from it.  Not for a segmented plan (mnb_pk_conv_post refuses it), nor for a shuffled link: its epilogue stores each
+    element as three scattered 2-byte pieces, several times slower than the fp32 output plus the producer's whole-unit stores
+    (harness/wbwtab_a32_infer_probe.py compares both per layer, DESIGN.md 4.20)"""
+    from . import pk as PK
+    return link.sg == 1 and not PK.segmented(sh, 0, A32_TERMS, 1)
+
+
+def _a32_conv_forward(conv, link, x):
+    """eval forward of a frozen A=32 conv: its cached weight levels and (3, 1) weight image, the term plane its producer wrote
+    (else its own pack of x) and, with a link, its consumer's term plane written by the epilogue (BatchNorm, ReLU, shuffle)"""
+    import torch
+    from . import pk as PK
+    _check_eval(conv)
+    w_int, alpha, bias, images = _frozen_conv_operands(conv)
+    plane = _handed_terms(conv, x)
+    if plane is None:
+        x = F_.materialized(x)
+        sg = conv.__dict__.get("_mnb_in_shuffle", 1)
+        if sg > 1:
+            from .frozen_graph import shuffle
+            x = shuffle(x, sg)      # the block's channel shuffle that freeze_inference moved into the producer
+    sh = F_._shape_struct(x.shape, conv.weight.shape, conv.stride, conv.padding, conv.dilation, conv.groups)
+    p, q = F_._out_hw(sh)
+    out_shape = (x.shape[0], conv.out_channels, p, q)
+    if L.PK_MODE == "off" or not PK.supported(sh, 0, A32_TERMS, 1) or (plane is None and x.dtype != torch.float32):
+        # outside the cover: the un-frozen layer on the decoded input
+        wq = w_int.float() * alpha.view(-1, 1, 1, 1)
+        return F_.quant_conv2d(F_.materialized(x), wq, bias, w_int, alpha, None, conv.stride, conv.padding, conv.dilation,
+                               conv.groups)
+    dev = alpha.device
+    if plane is None:
+        L.require_cuda(x, conv.weight)
+        plane, _ = PK.pack_act(x.contiguous(), None, A32_TERMS, phase_split=sh.stride_h == 2, groups=conv.groups)
+    key = ("terms", PK._key(sh))
+    if key not in images:
+        images[key] = PK.pack_weight(sh, 0, A32_TERMS, 1, w_int=w_int)
+    w_img = images[key]
+    hand = link is not None and link.accepts(out_shape) and not PK.padded(conv.out_channels, conv.groups)
+    if hand and _epilogue_hand_off(link, sh):
+        cplane = PK.terms_plane(*out_shape, A32_TERMS, dev)
+        rc = F_._timed("fwd_pk_terms", sh, lambda: PK.conv_post_terms(sh, plane, w_img, None, cplane, A32_TERMS, True,
+                                                                       link.split, n_scale=alpha, bias=bias,
+                                                                       bn=link.bn_tensors(), shuffle_groups=link.sg))
+        if rc == 0:
+            return link.tag(cplane, out_shape)
+        if rc != L.E_UNSUPPORTED:
+            L.check(rc, "pk_conv_post (term planes)")
+    y = torch.empty(out_shape, dtype=torch.float32, device=dev)
+    L.check(F_._timed("fwd_pk", sh, lambda: PK.conv(sh, 0, plane, A32_TERMS, w_img, 1, y, n_scale=alpha, bias=bias)),
+            "pk_conv fwd")
+    if hand:
+        # no consumer epilogue: the stem producer writes the plane from the fp32 output, the same op sequence
+        out = _a32_produce(link, y)
+        if out is not None:
+            return out
+    # no consumer plane: fp32 output; the absorbed modules (BatchNorm, ReLU, pool) run as usual on it
+    return y
+
+
+def _freeze_a32(seq, undo):
+    """link the A=32 conv-bn-act blocks of one nn.Sequential (DESIGN.md 4.20); returns the number of frozen convs"""
+    from .fused import EngineFloatConv2d, EngineMaxPool2d, _pool_cfg
+    kids = [(n, k) for n, k in seq.named_children() if not isinstance(k, nn.Identity)]
+    parsed = [_a32_block(k) for _, k in kids]
+    frozen = set()
+    for p in parsed:
+        if p is not None and _a32_freezable(p[0]):
+            frozen.add(p[0])
+    for conv in frozen:
+        conv.__dict__["_mnb_xnor"] = lambda m, x: _a32_conv_forward(m, m.__dict__.get("_mnb_a32_link"), x)
+        conv.__dict__["_mnb_frozen_plan"] = ("pk", "fp32")
+        for key in ("_mnb_xnor", "_mnb_frozen_plan", "_mnb_xnor_ops", "_mnb_a32_link", "_mnb_in_shuffle"):
+            undo.append(("dict", conv, key, None))
+    for i, p in enumerate(parsed):
+        if p is None:
+            continue
+        conv, bn, act = p
+        j, pool = i + 1, None
+        if j < len(kids) and type(kids[j][1]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j][1]) is not None:
+            pool, j = (kids[j][1],) + _pool_cfg(kids[j][1]), j + 1
+        if j >= len(kids) or parsed[j] is None or parsed[j][0] not in frozen:
+            continue
+        nxt, cconv = kids[j][1], parsed[j][0]
+        if bn.training or (pool is not None and tuple(cconv.stride) != (1, 1)):
+            continue
+        if pool is not None and int(getattr(pool[0], "out_shuffle_groups", 1)) != 1:
+            continue
+        stem = type(conv) in (nn.Conv2d, EngineFloatConv2d)
+        if not (conv in frozen or stem):
+            continue
+        sg = int(getattr(nxt, "shuffle_groups", 1)) if getattr(nxt, "channel_shuffle_flag", 0) else 1
+        link = _TermLink(cconv, bn, sg, pool)
+        if stem:
+            bn.__dict__["forward"] = lambda x, m=bn, link=link: _a32_stem_forward(m, link, x)
+        else:
+            conv.__dict__["_mnb_a32_link"] = link
+            conv.__dict__["_mnb_frozen_plan"] = ("pk", A32_PLANE)
+            bn.__dict__["forward"] = lambda x, m=bn, link=link: _a32_passthrough(m, link, x)
+        act.__dict__["forward"] = lambda x, m=act, link=link: _a32_passthrough(m, link, x)
+        undo += [("dict", bn, "forward", None), ("dict", act, "forward", None)]
+        if pool is not None:
+            pool[0].__dict__["forward"] = lambda x, m=pool[0], link=link: _a32_pool_forward(m, link, x)
+            undo.append(("dict", pool[0], "forward", None))
+        if sg > 1:
+            undo.append(("attr", nxt, "channel_shuffle_flag", nxt.channel_shuffle_flag))
+            nxt.channel_shuffle_flag = 0
+            cconv.__dict__["_mnb_in_shuffle"] = sg      # applied by the consumer itself when no plane arrives
+    return len(frozen)
+
+
 def freeze_inference(model, enable=True):
     """Inference on bit planes for a wbwtab model in eval mode (NIN-GC-style ``nn.Sequential`` of conv-bn-act blocks):
     every binary / ternary conv whose output is binarized for a consumer runs the XNOR-popcount kernel (outside its cover,
@@ -448,6 +722,16 @@ def freeze_inference(model, enable=True):
     ternary channel) stays un-frozen, and so does every producer without a frozen consumer.  A consumer takes a plane only
     from the unmodified tagged producer output; anything else reads ``functional.materialized`` of what it receives.  The
     logits equal the un-frozen eval forward's bit for bit (same integer sums, same fmaf, same BatchNorm op sequence).
+    Models with fp32 activations (``prepare(A=32, W=2|3)``: conv -> nn.BatchNorm2d -> ActivationQuantizer(A=32), a ReLU) hand
+    their activations over as term planes instead (DESIGN.md 4.20): every eval-mode binary / ternary QuantConv2d whose levels
+    freeze and whose shape the packed-operand forward covers at terms (3, 1) runs on its weight levels, quantized and packed
+    once; a block linked to the next block's frozen conv (across a max-pool with 2 p <= k in front of a stride-1 conv) writes
+    that conv's three exact bf16 pieces of ReLU(BatchNorm(y)) in the next block's channel order from its epilogue
+    (mnb_pk_conv_post with terms_out), the pool runs on the plane (mnb_pk_plane_maxpool_terms), and the fp32 stem conv's
+    BatchNorm + ReLU write the first plane (mnb_bn_relu_pack_terms_fwd).  The last quantized conv writes fp32 for the head.
+    ``_mnb_frozen_plan`` is ("pk", "terms3") for a conv writing term planes, ("pk", "fp32") for one writing fp32.  The logits
+    equal a block-by-block composition of those kernels bit for bit; against the un-frozen forward (another conv kernel,
+    ATen's BatchNorm) they agree to the fp32 contract.
     Parameters, buffers and state_dict keys are unchanged; ``enable=False`` restores the modules (needed before training)."""
     from .fused import BatchNormBinarize2d, EngineMaxPool2d, EnginePmConv2d, _pool_cfg
     _undo(model)
@@ -535,4 +819,5 @@ def freeze_inference(model, enable=True):
                     if k is h:
                         undo.append(("child", nxt, n, h))
                         nxt._modules[n] = pm
+        _freeze_a32(seq, undo)
     return model
