@@ -210,6 +210,14 @@ int mnb_fq_conv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const mnb_act_
 int mnb_conv2d_dgrad_tc(const mnb_conv_shape* s, const float* dy, const int16_t* w_int, const float* w_scale,
                         const uint32_t* pass_bits, const mnb_act_qparams* qp, float* dx, void* wpack_scratch,
                         int32_t* err_flag, mnb_stream_t stream);
+/* host only, the plan mnb_fq_conv2d_fwd_tc (dgrad = 0; quant_mode 0 = raw fp32 input, else the quantizer's mode) or
+ * mnb_conv2d_dgrad_tc (dgrad != 0; quant_mode ignored) runs, from the function its launcher uses: the first min(n, 17) of
+ * {NG (output channels per group: the kernel instance), TB (images per tile), TH (rows per tile), row_tiles, n_tiles, CC
+ * (channels per chunk), nchunk, nst (staging slots), nop (operand buffers), slab_groups, n_slabs, collapsed (1: the
+ * (H*W, C, B) tensor map of a 1x1 filter), smem_bytes, BW (padded row), npos_in (operand positions), grid (CTAs),
+ * n_mma_off (entries of the per-(tap, k-step) offset table)}.  Refusals as for the launchers (MNB_E_UNSUPPORTED, the
+ * reason in mnb_last_error). */
+int mnb_tc_conv_plan(const mnb_conv_shape* s, int32_t dgrad, int32_t quant_mode, int32_t* out, int32_t n);
 
 /* Weight gradient on the tensor-core path: dWq = s_a * corr(e_a, dy) with e_a re-quantized from the
  * fp32 input x on the fly (qp as in the forward; NULL = raw x, which must be bf16-exact such as the
@@ -217,6 +225,11 @@ int mnb_conv2d_dgrad_tc(const mnb_conv_shape* s, const float* dy, const int16_t*
  * replaced by mnb_conv2d_wgrad_cond(..., inexact_flag), which runs only when the flag is non-zero,
  * so no host synchronisation is needed).  scratch >= mnb_wgrad_tc_scratch_bytes(s) (-1: unsupported). */
 int64_t mnb_wgrad_tc_scratch_bytes(const mnb_conv_shape* s);
+/* host only, the plan mnb_conv2d_wgrad_tc runs, from the function its launcher uses: the first min(n, 16) of {Gb (groups
+ * per channel block), nsplit (128-channel slices of one group), tap_groups, tpc (taps per CTA), n_block (activation
+ * channels per CTA), CC (channels per chunk), TH, TB, nbuf (operand buffers), nst (staging slots), ranks (CTAs per
+ * block), n_slabs (channel blocks x tap groups), smem_bytes, npos_d, npos_x, n_tiles}.  Refusals as for the launcher. */
+int mnb_wgrad_tc_plan(const mnb_conv_shape* s, int32_t quant_mode, int32_t* out, int32_t n);
 int mnb_conv2d_wgrad_tc(const mnb_conv_shape* s, const float* dy, const float* x, const mnb_act_qparams* qp,
                         float* dwq, void* scratch, int32_t* inexact_flag, int32_t* err_flag, mnb_stream_t stream);
 int mnb_conv2d_wgrad_cond(const mnb_conv_shape* s, const float* dy, const mnb_conv_operands* op, float* dwq,

@@ -82,7 +82,9 @@ PROTOTYPES = {
     "mnb_channel_stats_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "mnb_fq_conv2d_fwd_tc": (C.c_int, [_SHAPE, _P, _ACTQ, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "mnb_conv2d_dgrad_tc": (C.c_int, [_SHAPE, _P, _P, _P, _P, _ACTQ, _P, _P, _P, _P]),
+    "mnb_tc_conv_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),
     "mnb_wgrad_tc_scratch_bytes": (_L, [_SHAPE]),
+    "mnb_wgrad_tc_plan": (C.c_int, [_SHAPE, _I, _P, _I]),
     "mnb_conv2d_wgrad_tc": (C.c_int, [_SHAPE, _P, _P, _ACTQ, _P, _P, _P, _P, _P]),
     "mnb_conv2d_wgrad_cond": (C.c_int, [_SHAPE, _P, _OPS, _P, _P, _P, _P]),
     "mnb_bn_batch_stats": (C.c_int, [_P, _I, _I, _I, _D, _D, _P, _P, _P, _P, _P, _P]),

@@ -586,6 +586,12 @@ static int plan(const mnb_conv_shape* s, bool dgrad, int quant_mode, Params& p, 
   return 0;
 }
 
+// persistent CTAs: one per SM, at least one per slab
+static int grid_size(const Params& p) {
+  const int64_t items = (int64_t)p.n_tiles * p.n_slabs;
+  return std::max((int)std::min<int64_t>(items, MNB_NUM_SMS), p.n_slabs);
+}
+
 static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t st) {
   {
     const int total = p.G * p.b_group_bytes / 2;
@@ -616,9 +622,7 @@ static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t 
     if (ce != cudaSuccess) return mnb_fail((int)ce, "cudaFuncSetAttribute: %s", cudaGetErrorString(ce));
     attr_set[ki] = true;
   }
-  const int64_t items = (int64_t)p.n_tiles * p.n_slabs;
-  int grid = (int)std::min<int64_t>(items, MNB_NUM_SMS);
-  grid = std::max(grid, p.n_slabs);
+  const int grid = grid_size(p);
   Params pp = p;
   pp.prof = g_prof_buffer;
   {
@@ -643,6 +647,18 @@ static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t 
 
 // debug hook: device buffer of 16 int64 cycle counters (NULL disables); see PROF_WAIT above
 extern "C" void mnb_set_tc_profile_buffer(void* dev_ptr) { tcconv::g_prof_buffer = reinterpret_cast<long long*>(dev_ptr); }
+
+extern "C" int mnb_tc_conv_plan(const mnb_conv_shape* s, int32_t dgrad, int32_t quant_mode, int32_t* out, int32_t n) {
+  tcconv::Params p{};
+  int smem_bytes = 0;
+  // the data gradient always splits fp32 dy: its launcher plans with quant_mode 0
+  if (int e = tcconv::plan(s, dgrad != 0, dgrad ? 0 : quant_mode, p, smem_bytes)) return e;
+  const int v[17] = {p.cout_g, p.TB, p.TH, p.row_tiles, p.n_tiles, p.CC, p.nchunk, p.nst, p.nop, p.slab_groups,
+                     p.n_slabs, p.pad == 0, smem_bytes, p.BW, p.npos_in, tcconv::grid_size(p), p.R * p.S * (p.CC / 16)};
+  if (out)
+    for (int i = 0; i < std::min(n, 17); ++i) out[i] = v[i];
+  return 0;
+}
 
 extern "C" int mnb_fq_conv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const mnb_act_qparams* qp,
                                     const int16_t* w_int, const float* w_scale, const float* bias, float* y,

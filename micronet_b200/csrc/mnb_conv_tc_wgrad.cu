@@ -426,6 +426,17 @@ static int plan(const mnb_conv_shape* s, int quant_mode, Params& p, int& smem_by
 
 }  // namespace tcwgrad
 
+extern "C" int mnb_wgrad_tc_plan(const mnb_conv_shape* s, int32_t quant_mode, int32_t* out, int32_t n) {
+  tcwgrad::Params p{};
+  int smem_bytes = 0;
+  if (int e = tcwgrad::plan(s, quant_mode, p, smem_bytes)) return e;
+  const int v[16] = {p.Gb, p.nsplit, p.tap_groups, p.tpc, p.n_block, p.CC, p.TH, p.TB, p.nbuf, p.nst, p.ranks,
+                     p.n_slabs, smem_bytes, p.npos_d, p.npos_x, p.n_tiles};
+  if (out)
+    for (int i = 0; i < std::min(n, 16); ++i) out[i] = v[i];
+  return 0;
+}
+
 extern "C" int64_t mnb_wgrad_tc_scratch_bytes(const mnb_conv_shape* s) {
   tcwgrad::Params p{};
   int smem = 0;
