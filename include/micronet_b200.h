@@ -485,6 +485,14 @@ int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a,
                      const mnb_pk_post* post, int32_t* err_flag, mnb_stream_t stream);
 int mnb_quant_add_pack_fwd(const float* a, const float* b, int32_t batch, int32_t channels, int32_t h, int32_t w,
                            const mnb_act_qparams* qp, int32_t relu, float* out, const mnb_pk_post* post, mnb_stream_t stream);
+/* Host only: the route of a forward conv of the family with consumer `post` (NULL: none) - the checks mnb_pk_conv_post
+ * (cpu 8) or mnb_pk_i8_conv (cpu 16, terms 1 x 1) make before launching, with the same return code and mnb_last_error
+ * text on a refusal.  The pointers of post are compared and checked for alignment, never dereferenced (post->q is read).
+ * out = {epilogue path, Nt, MT, n_mtiles, n_items, ny, col_tiles, n_ntiles, CTAs per output phase, segmented}, the first
+ * min(n, 10) written; path 0 plain bf16 levels (or no consumer), 1 segmented (no consumer), 2 int8 (levels or none),
+ * 3 bf16 levels behind BatchNorm / shuffle, 4 the same into an int8 plane, 5 term planes. */
+int mnb_pk_conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, int32_t cpu, const mnb_pk_post* post,
+                          int32_t* out, int32_t n);
 /* int8 operands for frozen inference graphs (symmetric IAO, IAO:214-240 with q_type 0): the forward conv of the family on
  * s8 x s8 -> s32 wgmma (K32 MMAs, exact integer sums).  The result is  y = fmaf(float(sum), a_scale * n_scale[n], bias[n]),
  * bit-identical to mnb_pk_conv on the same levels whenever its fp32 partial sums stay below 2^24, and exact (one rounding of

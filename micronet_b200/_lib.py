@@ -119,6 +119,7 @@ PROTOTYPES = {
     "mnb_bn_sign_bwd_pack": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P, _P]),
     "mnb_bn_sign_pool_bwd_pack": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P]),
     "mnb_pk_conv_post": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P]),
+    "mnb_pk_conv_post_plan": (C.c_int, [_SHAPE, _I, _I, _I, C.POINTER(PkPost), _P, _I]),
     "mnb_pk_conv_codes": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _I, _P, _P, _P, _P]),
     "mnb_codes_decode": (C.c_int, [_P, _P, _I, _I, _I, _P, _P]),
     "mnb_bn_batch_stats_codes": (C.c_int, [_P, _P, _I, _I, _I, _D, _D, _P, _P, _P, _P, _P, _P]),

@@ -2720,20 +2720,12 @@ extern "C" int mnb_pk_pack_weight(const mnb_conv_shape* s, int32_t mode, int32_t
   return 0;
 }
 
-static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
-                        int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
-                        const float* bias, const uint8_t* bits8, float gain, float* out, const mnb_pk_post* post,
-                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8, int16_t* codes = nullptr, float* dec = nullptr) {
+// The epilogue route of a conv launch: the consumer checks of mnb_pk_conv_post / mnb_pk_i8_conv (before anything is
+// launched) and the pk_conv_kernel instance row that runs it - 0 plain, 1 segmented (no consumer), 2 int8, 3 XPOST,
+// 4 XPOST int8, 5 XTERMS - together with the index range of the kernel's work-item arithmetic.  Host only: the launcher and
+// mnb_pk_conv_post_plan share it, so the query refuses what a launch refuses, with the same code and error text.
+static int conv_route(const pk::Plan& pl, int32_t mode, const uint8_t* bits8, const mnb_pk_post* post, int cpu, int& row) {
   using namespace pk;
-  MNB_REQUIRE(s && a_pk && w_img && (out || post || codes) && err_flag, "NULL pk_conv pointer");
-  Plan pl;
-  if (int e = make_plan(s, mode, terms_a, terms_w, pl, cpu)) return e;
-  if (codes) {
-    MNB_REQUIRE(mode == 0 && cpu == 8 && !out && !post && !bits8 && dec, "pk conv: int16 codes are a plain forward output");
-    // the int16 store is compiled into the single-product kernels only; one piece per operand keeps the sums exact integers
-    if (pl.segmented || terms_a != 1 || terms_w != 1)
-      return unsupported("int16 codes need one activation piece, one weight piece and a non-segmented plan");
-  }
   if (post) {   // BatchNorm and channel shuffle in front of the consumer's quantizer
     const int nbn = (post->bn_mean != nullptr) + (post->bn_invstd != nullptr) + (post->bn_gamma != nullptr) + (post->bn_beta != nullptr);
     MNB_REQUIRE(nbn == 0 || nbn == 4, "pk conv: the consumer's BatchNorm needs all four of mean, invstd, gamma, beta");
@@ -2774,6 +2766,33 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     // products, e.g. an asymmetric-IAO producer whose levels take two pieces) it costs register spills on every launch
     if (pl.segmented) return unsupported("fused consumer of a segmented (multi-piece) plan");
   }
+  int ki = -1;
+  for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
+  if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
+  if (pl.n_items >= (1 << 22) || pl.n_mtiles >= (1 << 22))     // FastDiv's exact range (fp32 reciprocal + one correction step)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
+  const bool xpost = post && (post->bn_mean || post->shuffle_groups > 1);   // (segmented plans refuse a post above)
+  row = terms_out ? 5 : cpu == 16 ? (xpost ? 4 : 2) : (pl.segmented ? 1 : (xpost ? 3 : 0));
+  return 0;
+}
+
+static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
+                        int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
+                        const float* bias, const uint8_t* bits8, float gain, float* out, const mnb_pk_post* post,
+                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8, int16_t* codes = nullptr, float* dec = nullptr) {
+  using namespace pk;
+  MNB_REQUIRE(s && a_pk && w_img && (out || post || codes) && err_flag, "NULL pk_conv pointer");
+  Plan pl;
+  if (int e = make_plan(s, mode, terms_a, terms_w, pl, cpu)) return e;
+  if (codes) {
+    MNB_REQUIRE(mode == 0 && cpu == 8 && !out && !post && !bits8 && dec, "pk conv: int16 codes are a plain forward output");
+    // the int16 store is compiled into the single-product kernels only; one piece per operand keeps the sums exact integers
+    if (pl.segmented || terms_a != 1 || terms_w != 1)
+      return unsupported("int16 codes need one activation piece, one weight piece and a non-segmented plan");
+  }
+  int row = 0;
+  if (int e = conv_route(pl, mode, bits8, post, cpu, row)) return e;
+  const bool terms_out = row == 5;
   static ConvParams p;   // large POD: filled per call (single host thread per process)
   memset(&p, 0, sizeof(p));
   ConvParams::Mma& m = p.m;
@@ -2833,8 +2852,6 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     const int tt = t < pl.TA ? t : 0;
     if (int e = make_pk_tmap(&tm[t], a_pk, plane_bytes, tt, pl.B, C8tot, pl.HA, pl.WA, pl.BW, pl.THH, pl.TB, pl.CC / cpu)) return e;
   }
-  if (pl.n_items >= (1 << 22) || pl.n_mtiles >= (1 << 22))     // FastDiv's exact range (fp32 reciprocal + one correction step)
-    return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
   const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
   using ConvFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
 #define MNB_PK_CONV_FNS(SEG, I8, X, T) {pk_conv_kernel<SEG, 16, I8, X, T>, pk_conv_kernel<SEG, 32, I8, X, T>,                       \
@@ -2844,11 +2861,9 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
                                    MNB_PK_CONV_FNS(false, true, false, false), MNB_PK_CONV_FNS(false, false, true, false),
                                    MNB_PK_CONV_FNS(false, true, true, false), MNB_PK_CONV_FNS(false, false, false, true)};
 #undef MNB_PK_CONV_FNS
-  int ki = -1;
-  for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
-  if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
-  const bool xpost = post && (post->bn_mean || post->shuffle_groups > 1);   // (segmented plans refuse a post above)
-  const ConvFn fn = fns[terms_out ? 5 : cpu == 16 ? (xpost ? 4 : 2) : (pl.segmented ? 1 : (xpost ? 3 : 0))][ki];
+  int ki = 0;
+  while (kNtSizes[ki] != pl.Nt) ++ki;     // (conv_route refuses any other N tile)
+  const ConvFn fn = fns[row][ki];
   if (int e = set_max_smem(fn, kSmemBudget)) return e;
   fn<<<dim3(gx, pl.ny), kConvThreads, pl.smem_bytes, (cudaStream_t)stream>>>(tm[0], tm[1], tm[2], p);
   MNB_LAUNCHED(1);
@@ -2870,6 +2885,23 @@ extern "C" int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32
   MNB_REQUIRE(post, "NULL consumer description");
   return pk_conv_impl(s, 0, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, out, post,
                       err_flag, stream);
+}
+
+// host only: out = {epilogue path (conv_route's instance row), Nt, MT, n_mtiles, n_items, ny, col_tiles, n_ntiles, CTAs per
+//            output phase, segmented}; the first min(n, 10) are written
+extern "C" int mnb_pk_conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, int32_t cpu,
+                                     const mnb_pk_post* post, int32_t* out, int32_t n) {
+  MNB_REQUIRE(s && (cpu == 8 || cpu == 16), "pk conv post plan: shape, 8 or 16 channels per unit");
+  pk::Plan pl;
+  if (int e = pk::make_plan(s, 0, terms_a, terms_w, pl, cpu)) return e;
+  int row = 0;
+  if (int e = conv_route(pl, 0, nullptr, post, cpu, row)) return e;
+  if (out) {
+    const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
+    const int v[10] = {row, pl.Nt, pl.MT, pl.n_mtiles, pl.n_items, pl.ny, pl.col_tiles, pl.n_ntiles, gx, pl.segmented};
+    for (int i = 0; i < std::min(n, 10); ++i) out[i] = v[i];
+  }
+  return 0;
 }
 
 extern "C" int mnb_pk_conv_codes(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,

@@ -215,13 +215,15 @@ def _graph_logits(m, x):
     return out.clone()
 
 
-@pytest.mark.parametrize("kind,a,w,i8", [("nin", 8, 8, False), ("gc", 4, 4, False), ("gc", 4, 4, True)],
-                         ids=["nin_w8a8", "gc_w4a4", "gc_w4a4_int8"])
-def test_frozen_logits_equal_the_block_composition(kind, a, w, i8):
+# batch 256: the batch the benchmark runs the NIN models at
+@pytest.mark.parametrize("kind,a,w,i8,batch", [("nin", 8, 8, False, 8), ("gc", 4, 4, False, 8), ("gc", 4, 4, True, 8),
+                                               ("nin", 8, 8, False, 256), ("gc", 4, 4, False, 256), ("gc", 4, 4, True, 256)],
+                         ids=["nin_w8a8", "gc_w4a4", "gc_w4a4_int8", "nin_w8a8_b256", "gc_w4a4_b256", "gc_w4a4_int8_b256"])
+def test_frozen_logits_equal_the_block_composition(kind, a, w, i8, batch):
     from harness import train as H
     from micronet_b200 import dorefa as DF
     m = _model(kind, a, w)
-    x, _ = H.synthetic_batch(8, 32, seed=4, device=DEV)
+    x, _ = H.synthetic_batch(batch, 32, seed=4, device=DEV)
     ref = _reference_logits(m, x, a, i8)
     DF.freeze_inference(m, int8=i8)
     with torch.no_grad():

@@ -127,11 +127,13 @@ def _pool_outputs(m):
 
 @pytest.mark.parametrize("arch", ["nin", "nin_gc"])
 @pytest.mark.parametrize("q_level,ptq", [(0, False), (1, False), (0, True)], ids=["per_channel", "per_layer", "ptq"])
-@pytest.mark.parametrize("i8", [False, True], ids=["bf16", "int8"])
-def test_handoff_logits_bitwise(arch, q_level, ptq, i8):
+# batch 256: the batch the benchmark runs the NIN models at
+@pytest.mark.parametrize("i8,batch", [(False, 32), (True, 32), (False, 256), (True, 256)],
+                         ids=["bf16", "int8", "bf16_b256", "int8_b256"])
+def test_handoff_logits_bitwise(arch, q_level, ptq, i8, batch):
     from micronet_b200 import iao
     m = _calibrated(arch, q_level, ptq)
-    x = H.synthetic_batch(32, 32, seed=5, device=DEV)[0]
+    x = H.synthetic_batch(batch, 32, seed=5, device=DEV)[0]
     with torch.no_grad():
         plain = m(x)
     off = copy.deepcopy(m)

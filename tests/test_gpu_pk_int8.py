@@ -322,6 +322,14 @@ def test_frozen_int8_resnet18_at_224_is_bit_identical():
     _compare(eng, calib, x)
 
 
+def test_frozen_int8_resnet18_at_224_bench_batch_is_bit_identical():
+    """the ResNet-18 PTQ graph at 224 x 64, the batch of the benchmark's inference metric: bf16 and int8 frozen logits equal
+    the un-frozen eval forward bit for bit"""
+    eng, calib, _ = _resnet((64, 128, 256, 512), 224)
+    x = torch.randn(64, 3, 224, 224, generator=torch.Generator().manual_seed(64))
+    _compare(eng, calib, x)
+
+
 def test_frozen_int8_ningc_is_bit_identical():
     eng, calib, x = _ningc()
     _compare(eng, calib, x)

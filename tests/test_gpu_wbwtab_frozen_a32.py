@@ -236,11 +236,13 @@ WORST = {}
 
 
 @pytest.mark.parametrize("W", [2, 3])
-@pytest.mark.parametrize("name", ["nin", "nin_gc", "ref_nin"])
+@pytest.mark.parametrize("name", ["nin", "nin_gc", "ref_nin", "nin_b256", "nin_gc_b256"])
 def test_frozen_logits_equal_the_composition(name, W):
     from micronet_b200 import functional as F_, wbwtab
+    name, _, batch = name.partition("_b")     # "_b256": the batch the benchmark runs the NIN models at
+    batch = int(batch) if batch else 32
     ref_m, fz = _model(name, W), _model(name, W)
-    x, _ = H.synthetic_batch(32, 32, seed=5, device=DEV)
+    x, _ = H.synthetic_batch(batch, 32, seed=5, device=DEV)
     with torch.no_grad():
         ref, reads = _composed(ref_m, x)
         unfrozen = ref_m(x)
@@ -261,7 +263,7 @@ def test_frozen_logits_equal_the_composition(name, W):
         scale = ref64.abs().max().item()
         err_f = (got.double().cpu() - ref64).abs().max().item() / scale
         err_u = (unfrozen.double().cpu() - ref64).abs().max().item() / scale
-        WORST[(name, W)] = (err_f, err_u)
+        WORST[(name, W, batch)] = (err_f, err_u)
         print(f"\n{name} W{W}: max |logit - fp64| / max |fp64|: frozen {err_f:.3e}, un-frozen {err_u:.3e}")
         assert err_f <= 1e-5 and err_u <= 1e-5
 
