@@ -61,7 +61,8 @@ def layer_routes(fz, x, rounds, reps):
         h.remove()
     rows = []
     for i, c in enumerate(convs):
-        link = c.__dict__.get("_mnb_a32_link")
+        rec = c.__dict__.get("_mnb_frozen")
+        link = None if rec is None or rec["fmt"] != wbwtab.A32_PLANE else rec["link"]
         sh = F_._shape_struct(shapes[c], c.weight.shape, c.stride, c.padding, c.dilation, c.groups)
         if link is None or link.split or PK.segmented(sh, 0, wbwtab.A32_TERMS, 1):
             continue

@@ -7,6 +7,7 @@ same class names, constructor signatures (DF:77-91, DF:178-186), attribute names
 from __future__ import annotations
 
 import copy
+import functools
 
 import torch.nn as nn
 
@@ -199,46 +200,30 @@ def _freezable(conv):
     return not conv.quant_inference or frozen_levels(conv) is not None
 
 
-def _check_eval(m):
-    if m.training:
-        raise RuntimeError("micronet_b200: this module is frozen for inference (dorefa.freeze_inference); call "
-                           "freeze_inference(model, enable=False) before training it")
+_check_eval = functools.partial(FG.check_eval, "dorefa")
 
 
 def _frozen_operands(conv):
     """(wq, w_int, w_scale, bias) computed once; re-done when a parameter or buffer is written in place"""
-    key = tuple(t._version for t in list(conv.parameters()) + list(conv.buffers()))
-    fr = conv.__dict__.get("_mnb_ops")
-    if fr is None or fr[0] != key:
+    def make():
         lv = frozen_levels(conv)
         if lv is None:
             raise RuntimeError("micronet_b200: the weights of a frozen DoReFa layer changed to values that are not weight "
                                "quantizer levels; call dorefa.freeze_inference(model) again")
         lv[1]._mnb_pk_cache = {}          # the packed weight images are built once per shape (functional.frozen_conv)
-        fr = (key,) + tuple(lv) + (None if conv.bias is None else conv.bias.detach(),)
-        conv.__dict__["_mnb_ops"] = fr
-    return fr[1:]
+        return tuple(lv) + (None if conv.bias is None else conv.bias.detach(),)
+    return FG.cached_operands(conv, "_mnb_ops", make)
 
 
 class _Link(FG.Link):
     """frozen_graph.Link whose producer applies the eval BatchNorm (running statistics) before the ReLU and the consumer's
     DoReFa quantizer; a max-pool in between runs as mnb_pk_plane_maxpool"""
 
-    def __init__(self, cconv, bn, relu, sg, pool):
-        super().__init__(cconv, bn, relu, sg, pool)
-        self._invstd = None
-
     def consumer(self):
-        import torch
-        bn, c = self.bn, self.cconv
-        rv = bn.running_var
-        key = (rv.data_ptr(), rv._version, float(bn.eps))
-        if self._invstd is None or self._invstd[0] != key:
-            self._invstd = (key, torch.rsqrt(rv + bn.eps))     # as the un-frozen eval BatchNormReluQuant2d computes it
-        stats = (bn.running_mean, self._invstd[1], bn.weight.detach(), bn.bias.detach())
+        c = self.cconv
         return F_.Consumer(c, c.activation_quantizer.spec(), self.relu, True, tuple(c.weight.shape), tuple(c.stride),
                            tuple(c.padding), tuple(c.dilation), c.groups, True, int8=c.__dict__["_mnb_frozen"]["int8"],
-                           bn=stats, shuffle_groups=self.sg, pool=self.pool)
+                           bn=self.bn_tensors(), shuffle_groups=self.sg, pool=self.pool)
 
 
 def _frozen_conv_forward(conv, x):
@@ -261,9 +246,9 @@ def _frozen_conv_forward(conv, x):
                           consumer=link.consumer() if link is not None else None, int8=info["int8"])
 
 
-def _plane_pool(plane, b, c, h, w, k, s, p, int8):
+def _plane_pool(plane, x, k, s, p):
     from . import pk as PK
-    return PK.plane_maxpool(plane, b, c, h, w, k, s, p, int8=int8)
+    return PK.plane_maxpool(plane, *x.shape, k, s, p, int8=x._mnb_pk_pre[3] == "i8")
 
 
 def _stem_forward(bn, link, x):
@@ -293,7 +278,7 @@ def _stem_forward(bn, link, x):
                 rc = lib.mnb_bn_relu_quant_pack_fwd(x.data_ptr(), b, c, h * w, mean, invstd, gamma, beta, C.byref(qp),
                                                     consumer.sg, plane.data_ptr(), bits.data_ptr(), L.stream())
             if rc == 0:
-                return F_._tag(torch.empty(x.shape, dtype=torch.float32, device="meta"), consumer, plane, fmt)
+                return F_.tag(torch.empty(x.shape, dtype=torch.float32, device="meta"), consumer.target, plane, fmt)
             if rc != L.E_UNSUPPORTED:
                 L.check(rc, "bn_relu_quant_pack (stem)")
     return type(bn).forward(bn, x)
@@ -302,7 +287,7 @@ def _stem_forward(bn, link, x):
 def _conv_bn_act(blk):
     """(conv, BatchNorm, nn.ReLU or None, relu applied?) of one of the reference's conv-bn-relu blocks, else None"""
     from .fused import BatchNormReluQuant2d
-    bp = FG.block_parts(blk)
+    bp = FG.block_parts(blk) if hasattr(blk, "channel_shuffle_flag") else None
     if bp is None or len(bp[1]) not in (1, 2):
         return None
     bn, act = bp[1][0], (bp[1][1] if len(bp[1]) == 2 else None)
@@ -337,7 +322,7 @@ def freeze_inference(model, enable=True, int8=False):
     absorbed modules run as usual.  Numerics (DESIGN.md 4.15): the levels equal the fused BatchNormReluQuant2d's bit for bit;
     where the un-frozen graph ran ATen's BatchNorm a level on a rounding boundary may differ by one.  Parameters, buffers
     and state_dict keys are unchanged; ``enable=False`` restores the modules (needed before training)."""
-    from .fused import EngineFloatConv2d, EngineMaxPool2d, _pool_cfg
+    from .fused import EngineFloatConv2d
     FG.undo(model, _UNDO)
     if not enable:
         return model
@@ -349,12 +334,8 @@ def freeze_inference(model, enable=True, int8=False):
             m.__dict__["_mnb_frozen"] = {"int8": bool(int8) and small, "link": None}
             rw.forget(m, "_mnb_frozen", "_mnb_ops")
             frozen.add(m)
-
-    def pool_cfg(k):
-        return _pool_cfg(k) if type(k) in (nn.MaxPool2d, EngineMaxPool2d) else None
-
-    for (conv, bn, act, relu), pool, cfg, nxt, cconv in FG.block_pairs(model, _conv_bn_act, pool_cfg):
-        if cconv not in frozen or (pool is not None and tuple(cconv.stride) != (1, 1)):
+    for (conv, bn, act, relu), pool, cfg, nxt, cconv, _ in FG.block_pairs(model, _conv_bn_act, FG.max_pool_cfg):
+        if cconv not in frozen or not hasattr(nxt, "channel_shuffle_flag") or (pool is not None and tuple(cconv.stride) != (1, 1)):
             continue
         flag_sg = FG.block_shuffle(nxt)
         fold_sg = int(getattr(pool if pool is not None else bn, "out_shuffle_groups", 1))   # folded by fuse=True
@@ -371,7 +352,7 @@ def freeze_inference(model, enable=True, int8=False):
         if act is not None:
             rw.override(act, FG.absorbed_forward, _check_eval, act, target)
         if pool is not None:
-            rw.override(pool, FG.pool_forward, _check_eval, _plane_pool, pool, link)
+            rw.override(pool, FG.pool_forward, _check_eval, _plane_pool, FG.pool_as_usual, pool, link)
         if flag_sg > 1:
             rw.move_shuffle(nxt, cconv, flag_sg)
     return model

@@ -284,21 +284,24 @@ def materialized(t):
     """the values of a producer output: ``t`` itself, or - for a plane-only output of a fused BatchNorm + binarizer (its fp32
     storage was never written) - the +-1 tensor rebuilt from the bf16 operand plane [b][c/8][h][w][8], or - for a wbwtab conv
     that handed its output to its BatchNorm as int16 codes (``codes_out``) - that output decoded with the conv epilogue's own
-    fmaf, or - for the output of a frozen wbwtab layer (wbwtab.freeze_inference) - the +-1 tensor its consumer's bit plane
-    encodes (bit plane or b1 plane), or the fp32 tensor whose exact pieces a frozen A=32 producer wrote (term planes).
+    fmaf, or - for the output of a frozen wbwtab layer (wbwtab.freeze_inference) - the +-1 tensor its consumer's bit plane or
+    b1 plane encodes, or the fp32 tensor whose exact pieces a frozen A=32 producer wrote (term planes).  A meta-shaped
+    output with a level plane (bf16 / i8) cannot be decoded and raises.
     Plumbing for tests, hooks and readers outside the fused producers; the training step never calls it."""
-    xbits = getattr(t, "_mnb_xbits", None)
-    if xbits is not None:
-        from . import xnor as XN
-        return XN.unpack(xbits[1], t.shape, xbits[3])
-    b1p = getattr(t, "_mnb_b1", None)
-    if b1p is not None:
-        from . import b1 as B1
-        return B1.unpack(b1p[1], t.shape, b1p[3])
-    terms = getattr(t, "_mnb_terms", None)
-    if terms is not None:        # term planes of a frozen A=32 wbwtab producer (wbwtab.freeze_inference)
-        from . import pk as PK
-        return PK.unpack_terms(terms[1], t.shape, terms[4], split=terms[3])
+    pre = getattr(t, "_mnb_pk_pre", None)
+    if pre is not None:
+        _, plane, _, fmt, info = pre
+        if fmt == "bits":
+            from . import xnor as XN
+            return XN.unpack(plane, t.shape, info["groups"])
+        if fmt == "b1":
+            from . import b1 as B1
+            return B1.unpack(plane, t.shape, info["groups"])
+        if fmt == "terms":
+            from . import pk as PK
+            return PK.unpack_terms(plane, t.shape, info["terms"], split=info["split"])
+        if t.device.type == "meta":
+            raise RuntimeError(f"micronet_b200: a {fmt} operand plane cannot be decoded")
     codes = getattr(t, "_mnb_codes", None)
     if codes is not None:
         b, c = t.shape[0], t.shape[1]
@@ -883,19 +886,32 @@ class Consumer:
         return self.stride[0] == 2 and self.pool is None
 
 
+DECODABLE = ("bits", "b1", "terms")     # plane formats materialized decodes; level planes ("bf16", "i8") it cannot
+
+
+def tag(y, target, plane, fmt, **meta):
+    """tag producer output ``y`` with the plane it wrote for module ``target``, in format ``fmt`` ("bf16" / "i8" level
+    planes, "bits" / "b1" planes with their ``groups``, "terms" planes with ``split`` and ``terms``)"""
+    y._mnb_pk_pre = (target, plane, y._version, fmt, meta)
+    return y
+
+
 def handed_plane(module, x):
-    """the operand plane a producer wrote for ``module`` (None if ``x`` does not carry one that is still valid)"""
+    """the plane a frozen producer wrote for ``module`` when ``x`` is that producer's output, else None.  The plane goes
+    to its target only, at the groups it was packed for (bit / b1 planes), and, for an output that also holds values (a
+    tagged fp32 tensor), only while ``x._version`` is the one it was tagged at.  A meta-shaped output holds nothing but its
+    plane, so no in-place write can make the two disagree: its version is not checked.  A meta-shaped output that
+    reaches another module raises unless its plane decodes (functional.materialized: bit, b1 and term planes)."""
     pre = getattr(x, "_mnb_pk_pre", None)
-    if pre is not None and pre[0] is module and (x.device.type == "meta" or x._version == pre[2]):
-        return pre[1]
-    if x.device.type == "meta":
+    meta = x.device.type == "meta"
+    if pre is not None:
+        target, plane, version, fmt, info = pre
+        g = info.get("groups")
+        if target is module and (meta or x._version == version) and (g is None or getattr(module, "groups", g) == g):
+            return plane
+    if meta and (pre is None or pre[3] not in DECODABLE):
         raise RuntimeError("micronet_b200: a plane-only producer output reached a module it was not produced for")
     return None
-
-
-def _tag(y, consumer, plane, fmt="bf16"):
-    y._mnb_pk_pre = (consumer.target, plane, y._version, fmt)
-    return y
 
 
 def _i8_route(spec, w_int, sh):
@@ -967,7 +983,7 @@ def frozen_conv(x, plane, wq, bias, w_int, w_scale, spec, stride, padding, dilat
             "pk_conv_post")
     if y is None:
         y = torch.empty(out_shape, dtype=torch.float32, device="meta")   # shape only: the data lives in the consumer's plane
-    return _tag(y, consumer, cplane)
+    return tag(y, consumer.target, cplane, "bf16")
 
 
 def _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_relu, consumer):
@@ -991,7 +1007,7 @@ def _frozen_conv_i8(x, plane, bias, w_int, w_scale, spec, sh, out_shape, pre_rel
                                                        a_scale_const=a_const, bias=bias, post=post)), "pk_i8_conv")
     if y is None:
         y = torch.empty(out_shape, dtype=torch.float32, device="meta")
-    return _tag(y, consumer, cplane, "i8")
+    return tag(y, consumer.target, cplane, "i8")
 
 
 @torch.no_grad()
@@ -1014,7 +1030,7 @@ def frozen_quant_add(a, b, spec, relu, consumer=None):
     fn = lib.mnb_quant_add_pack_i8_fwd if i8 else lib.mnb_quant_add_pack_fwd
     L.check(fn(a.data_ptr(), b.data_ptr(), a.shape[0], a.shape[1], a.shape[2], a.shape[3], C.byref(qp), 1 if relu else 0,
                out.data_ptr(), C.byref(post), L.stream()), "quant_add_pack_i8_fwd" if i8 else "quant_add_pack_fwd")
-    return _tag(out, consumer, cplane, cfmt)
+    return tag(out, consumer.target, cplane, cfmt)
 
 
 def quant_linear(x, wq, bias, w_int, w_scale, spec):

@@ -165,12 +165,6 @@ class BatchNormBinarize2d(nn.BatchNorm2d):
     plane_only = False     # set by fuse_wbwtab_blocks: the only reader of the output is a conv that takes the bf16 plane
 
     def forward(self, input):
-        frozen = self.__dict__.get("_mnb_xnor")     # set by wbwtab.freeze_inference: a bit-plane producer took this layer over
-        if frozen is not None:
-            return frozen(self, input)
-        return self._forward(input)
-
-    def _forward(self, input):
         L.require_cuda(input, self.weight)
         L.require_f32(input, self.weight)
         assert self.affine and self.track_running_stats and self.momentum is not None, \

@@ -338,9 +338,7 @@ class QuantConv2d(nn.Conv2d):
     def _frozen_operands(self, make):
         """inference fast path (freeze_inference): the quantized weights of an eval-mode module are computed once;
         ``make`` returns (weight to quantize, bias).  Invalidated when any parameter / buffer is written in place."""
-        key = tuple(t._version for t in list(self.parameters()) + list(self.buffers()))
-        fr = self.__dict__.get("_frozen")
-        if fr is None or fr[0] != key:
+        def ops():
             weight, bias = make()
             if not self.quant_inference:
                 wq, w_int, w_scale = self.weight_quantizer.quantize_weight(weight)
@@ -350,9 +348,8 @@ class QuantConv2d(nn.Conv2d):
                 wq, w_int, w_scale = weight, None, None
             wq = wq.detach()
             (w_int if w_int is not None else wq)._mnb_pk_cache = {}
-            fr = (key, wq, w_int, w_scale, None if bias is None else bias.detach())
-            self.__dict__["_frozen"] = fr
-        return fr[1:]
+            return wq, w_int, w_scale, None if bias is None else bias.detach()
+        return FG.cached_operands(self, "_frozen", ops)
 
     def _stored_levels(self, weight):
         """(wq, w_int, w_scale) of a ``quant_inference`` conv whose stored weight freeze_inference accepted as levels: the
@@ -726,39 +723,30 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
     Outputs are bit-identical to the un-frozen eval forward (a deployment graph's: to the frozen QAT graph's);
     ``enable=False`` restores the modules."""
     FG.undo(model, _UNDO)
+    if not enable:
+        return model
+    rw = FG.Rewrite(model, _UNDO)
     for name, m in model.named_modules():
         if isinstance(m, (QuantConv2d, QuantLinear, QuantAdd)):
-            m.__dict__["_frozen_inference"] = bool(enable)
-            m.__dict__["_int8"] = bool(enable and int8)
-            m.__dict__.pop("_frozen", None)
-            m.__dict__.pop("_pre_relu", None)
-            m.__dict__.pop("_fuse_relu", None)
-            m.__dict__.pop("_post_consumer", None)
-            m.__dict__.pop("_int_levels", None)
-            if enable and isinstance(m, QuantConv2d) and not m.training and _holds_levels(m):
-                m.__dict__["_int_levels"] = name or type(m).__name__    # named in the error of a later mismatch
+            rw.set_dict(m, "_frozen_inference", True)
+            rw.set_dict(m, "_int8", bool(int8))
+            rw.forget(m, "_frozen")
+            if isinstance(m, QuantConv2d) and not m.training and _holds_levels(m):
+                rw.set_dict(m, "_int_levels", name or type(m).__name__)    # named in the error of a later mismatch
     for m in model.modules():
-        saved = m.__dict__.setdefault("_mnb_saved_relus", {})
-        for name, relu in list(saved.items()):       # undo an earlier rewrite first
-            m._modules[name] = relu
-        saved.clear()
-        if not enable:
-            continue
         if isinstance(m, nn.Sequential):
             kids = [(n, k) for n, k in m.named_children() if not isinstance(k, nn.Identity)]
             for (n0, k0), (n1, k1) in zip(kids, kids[1:]):
                 if type(k0) is nn.ReLU and isinstance(k1, QuantConv2d) and _int_weights(k1):
-                    k1.__dict__["_pre_relu"] = True
-                    saved[n0] = k0
-                    m._modules[n0] = nn.Identity()
+                    rw.set_dict(k1, "_pre_relu", True)
+                    rw.set_child(m, n0, nn.Identity())
         add, act = m._modules.get("add"), m._modules.get("act")
         if isinstance(add, QuantAdd) and type(act) is nn.ReLU:
-            add.__dict__["_fuse_relu"] = True
-            saved["act"] = act
-            m._modules["act"] = nn.Identity()
-    if enable and handoff:
-        _link_consumers(model)
-        _link_blocks(model)
+            rw.set_dict(add, "_fuse_relu", True)
+            rw.set_child(m, "act", nn.Identity())
+    if handoff:
+        _link_consumers(model, rw)
+        _link_blocks(model, rw)
     return model
 
 
@@ -802,7 +790,7 @@ def _block_conv(conv):
 
 def _conv_relu(blk):
     """(conv, nn.ReLU) of a conv-bn-relu block whose BatchNorm prepare(bn_fuse=True) folded into the conv, else None"""
-    bp = FG.block_parts(blk)
+    bp = FG.block_parts(blk) if hasattr(blk, "channel_shuffle_flag") else None
     if bp is None or len(bp[1]) != 1 or type(bp[1][0]) is not nn.ReLU:
         return None
     return bp[0], bp[1][0]
@@ -816,23 +804,23 @@ def _pool_cover(m):
     return _pool_cfg(m)
 
 
-def _requant_pool(link, plane, b, c, h, w, k, s, p, int8):
+def _requant_pool(link, plane, x, k, s, p):
     from . import pk as PK
     q_in = link.pool[0].activation_quantizer.act_spec().struct()
     q_out = link.cconv.activation_quantizer.act_spec().struct()
-    return PK.plane_maxpool_requant(plane, b, c, h, w, k, s, p, q_in, q_out, int8=int8)
+    return PK.plane_maxpool_requant(plane, *x.shape, k, s, p, q_in, q_out, int8=x._mnb_pk_pre[3] == "i8")
 
 
 def _no_check(m):
     """absorbed IAO modules run un-frozen in training mode: a producer tags its output only on the frozen eval path"""
 
 
-def _link_blocks(model):
-    """block -> block links of NIN / NIN-GC-style graphs (see freeze_inference); recorded for ``enable=False``"""
+def _link_blocks(model, rw):
+    """block -> block links of NIN / NIN-GC-style graphs (see freeze_inference)"""
     import functools
-    rw = FG.Rewrite(model, _UNDO)
-    for (conv, relu), pool, cfg, nxt, cconv in FG.block_pairs(model, _conv_relu, _pool_cover):
-        if not (_block_conv(conv) and _block_conv(cconv)) or (pool is not None and tuple(cconv.stride) != (1, 1)):
+    for (conv, relu), pool, cfg, nxt, cconv, _ in FG.block_pairs(model, _conv_relu, _pool_cover):
+        if (not (_block_conv(conv) and _block_conv(cconv)) or not hasattr(nxt, "channel_shuffle_flag")
+                or (pool is not None and tuple(cconv.stride) != (1, 1))):
             continue
         sg = FG.block_shuffle(nxt)
         if sg > 1 and not _shuffled_link_pays(pool, cconv):
@@ -841,7 +829,7 @@ def _link_blocks(model):
         rw.set_dict(conv, "_post_consumer", link)
         rw.override(relu, FG.absorbed_forward, _no_check, relu, link.target)
         if pool is not None:
-            rw.override(pool, FG.pool_forward, _no_check, functools.partial(_requant_pool, link), pool, link)
+            rw.override(pool, FG.pool_forward, _no_check, functools.partial(_requant_pool, link), FG.pool_as_usual, pool, link)
         if sg > 1:
             rw.move_shuffle(nxt, cconv, sg)
 
@@ -851,7 +839,7 @@ def _first_quant_conv(seq):
     return kids[0] if kids and isinstance(kids[0], QuantConv2d) else None
 
 
-def _link_consumers(model):
+def _link_consumers(model, rw):
     """producer -> consumer links of the frozen graph (the consumer's operand plane is then written by the producer):
     * two quant convs that are adjacent in an nn.Sequential (the nn.ReLU between them already folded away): the first
       one's epilogue writes the second one's plane and no fp32 tensor at all - nobody else can read a Sequential's
@@ -865,12 +853,12 @@ def _link_consumers(model):
             kids = [k for k in m.children() if not isinstance(k, nn.Identity)]
             for k0, k1 in zip(kids, kids[1:]):
                 if isinstance(k0, QuantConv2d) and isinstance(k1, QuantConv2d):
-                    k0.__dict__["_post_consumer"] = (k1, True)
+                    rw.set_dict(k0, "_post_consumer", (k1, True))
     blocks = [m for m in model.modules() if isinstance(m._modules.get("add"), QuantAdd)
               and _first_quant_conv(m._modules.get("residual_function")) is not None]
     for b0, b1 in zip(blocks, blocks[1:]):
         if b0._modules["add"].__dict__.get("_fuse_relu", False):
-            b0._modules["add"].__dict__["_post_consumer"] = (_first_quant_conv(b1._modules["residual_function"]), False)
+            rw.set_dict(b0._modules["add"], "_post_consumer", (_first_quant_conv(b1._modules["residual_function"]), False))
 
 
 def prepare(model, inplace=False, a_bits=8, w_bits=8, q_type=0, q_level=0, weight_observer=0, bn_fuse=False,

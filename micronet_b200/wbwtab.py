@@ -5,10 +5,12 @@ Drop-in for the reference's ``micronet/compression/quantization/wbwtab/quantize.
 from __future__ import annotations
 
 import copy
+import functools
 
 import torch.nn as nn
 
 from . import _lib as L
+from . import frozen_graph as FG
 from . import functional as F_
 
 
@@ -26,9 +28,6 @@ class ActivationQuantizer(nn.Module):
         return y
 
     def forward(self, input):
-        frozen = self.__dict__.get("_mnb_xnor")     # set by freeze_inference: this binarizer writes its consumer's bit plane
-        if frozen is not None:
-            return frozen(self, input)
         return self.binary(input) if self.A == 2 else self.relu(input)
 
 
@@ -60,9 +59,6 @@ class QuantConv2d(nn.Conv2d):
         self.weight_quantizer = WeightQuantizer(W=W)
 
     def forward(self, input):
-        frozen = self.__dict__.get("_mnb_xnor")     # set by freeze_inference: XNOR conv writing its consumer's operand
-        if frozen is not None:
-            return frozen(self, input)
         if not self.quant_inference:
             wq, w_int, w_scale = self.weight_quantizer.quantize(self.weight)
         else:
@@ -147,6 +143,10 @@ def prepare(model, inplace=False, A=2, W=2, quant_inference=False, fuse_bn=False
 # --------------------------------------------------------------------------
 # frozen inference graphs on bit planes
 # --------------------------------------------------------------------------
+_UNDO = "_mnb_xnor_undo"
+_check_eval = functools.partial(FG.check_eval, "wbwtab")
+
+
 def frozen_levels(conv):
     """(w_int i16 [K, C/g, R, S], alpha f32 [K]) of a wbwtab conv for the XNOR kernels, or None when its weights cannot be
     frozen.  A ``quant_inference`` layer holds alpha_k * {-1, 0, +1} (bn_fuse.wbwtab_quantize_inference_weights): the levels
@@ -194,10 +194,6 @@ def _frozen_kernel(conv):
     return kind if ok else None
 
 
-def _freezable(conv):
-    return _frozen_kernel(conv) is not None
-
-
 class _Link:
     """what a frozen producer writes for its consumer: format (bit plane for a frozen XNOR conv, bf16 +-1 plane for the
     un-quantized head), the consumer's groups, and the modules the epilogue stands for (the eval BatchNorm of a
@@ -230,30 +226,24 @@ class _Link:
         """the absorbed modules, run as they would run un-frozen (planes the kernels refuse at run time)"""
         from .fused import BatchNormBinarize2d
         if isinstance(self.act, BatchNormBinarize2d):
-            y = self.act._forward(y)             # BatchNorm + sign [+ pool] [+ shuffle]
+            y = type(self.act).forward(self.act, y)     # BatchNorm + sign [+ pool] [+ shuffle]
         else:
             y = self.act.binary(y)
             if self.pool is not None:
                 y = self.pool(y)
             if self.sg > 1:
-                b, c = y.shape[0], y.shape[1]
-                y = y.view(b, self.sg, c // self.sg, *y.shape[2:]).transpose(1, 2).contiguous().view(y.shape)
+                y = FG.shuffle(y, self.sg)
                 y._mnb_pm1 = True
         return y
 
     def tag(self, plane, shape, device):
         import torch
-        if self.fmt == L.XNOR_B1_PLANE:
-            y = torch.empty(shape, dtype=torch.float32, device="meta")     # shape only: the data lives in the b1 plane
-            y._mnb_b1 = (self.consumer, plane, y._version, self.out_groups)
+        if self.fmt == L.XNOR_PM1_BF16:
+            y = torch.empty(shape, dtype=torch.float32, device=device)      # the placeholder of a plane-only producer
+            y._mnb_pk_pm1, y._mnb_plane_only, y._mnb_pm1 = plane, True, True
             return y
-        if self.fmt == L.XNOR_BITS:
-            y = torch.empty(shape, dtype=torch.float32, device="meta")     # shape only: the data lives in the bit plane
-            y._mnb_xbits = (self.consumer, plane, y._version, self.out_groups)
-            return y
-        y = torch.empty(shape, dtype=torch.float32, device=device)          # the placeholder of a plane-only producer
-        y._mnb_pk_pm1, y._mnb_plane_only, y._mnb_pm1 = plane, True, True
-        return y
+        y = torch.empty(shape, dtype=torch.float32, device="meta")         # shape only: the data lives in the plane
+        return F_.tag(y, self.consumer, plane, "b1" if self.fmt == L.XNOR_B1_PLANE else "bits", groups=self.out_groups)
 
 
 def _out_buffer(nbytes, fmt, device):
@@ -263,79 +253,59 @@ def _out_buffer(nbytes, fmt, device):
     return torch.empty(nbytes, dtype=torch.uint8, device=device)
 
 
-def _handed_bits(module, x):
-    """the bit plane a frozen producer wrote for ``module``, if ``x`` is that producer's unmodified output"""
-    pre = getattr(x, "_mnb_xbits", None)
-    if pre is not None and pre[0] is module and x._version == pre[2] and pre[3] == module.groups:
-        return pre[1]
-    return None
-
-
-def _handed_b1(module, x):
-    """the b1 plane a frozen producer (or a plane pool) wrote for ``module``, if ``x`` is that unmodified output"""
-    pre = getattr(x, "_mnb_b1", None)
-    if pre is not None and pre[0] is module and x._version == pre[2] and pre[3] == module.groups:
-        return pre[1]
-    return None
-
-
 class _PlanePool(nn.Module):
     """a MaxPool2d(k, s, p) between a frozen producer and a frozen b1 consumer: the pool of the +-1 tensor taken on its b1
     plane (mnb_b1_plane_maxpool); any other input runs the original pool"""
 
-    def __init__(self, pool, consumer):
+    def __init__(self, pool, cfg, consumer):
         super().__init__()
-        self.__dict__["pool"], self.__dict__["consumer"] = pool, consumer      # not sub-modules: state_dict unchanged
-        self.k, self.s, self.p = _pool_cfg_b1(pool)
+        self.__dict__["pool"] = pool        # not a sub-module: state_dict unchanged
+        self.k, self.s, self.p = cfg
+        self.link = FG.Link(consumer, None, None, 1, (self,) + tuple(cfg))
+        self.train(pool.training)
 
     def forward(self, x):
-        import torch
-        from . import b1 as B1
-        _check_eval(self)
-        pre = getattr(x, "_mnb_b1", None)
-        if pre is not None and pre[0] is self and x._version == pre[2]:
-            rc, out, shape = B1.plane_maxpool(pre[1], x.shape, pre[3], self.k, self.s, self.p)
-            if rc == 0:
-                y = torch.empty(shape, dtype=torch.float32, device="meta")
-                y._mnb_b1 = (self.consumer, out, y._version, pre[3])
-                return y
-            if rc != L.E_UNSUPPORTED:
-                L.check(rc, "b1_plane_maxpool")
-        return self.pool(F_.materialized(x))
+        return FG.pool_forward(_check_eval, _b1_pool, _b1_pool_fallback, self, self.link, x, timed=False)
 
 
-def _pool_cfg_b1(pool):
-    from .fused import EngineMaxPool2d, _pool_cfg
-    if type(pool) not in (nn.MaxPool2d, EngineMaxPool2d) or int(getattr(pool, "out_shuffle_groups", 1)) != 1:
-        return None
-    return _pool_cfg(pool)
+def _b1_pool(plane, x, k, s, p):
+    from . import b1 as B1
+    rc, out, _ = B1.plane_maxpool(plane, x.shape, x._mnb_pk_pre[4]["groups"], k, s, p)
+    if rc == 0:
+        return out
+    if rc != L.E_UNSUPPORTED:
+        L.check(rc, "b1_plane_maxpool")
+    return None
 
 
-def _check_eval(m):
-    if m.training:
-        raise RuntimeError("micronet_b200: this module is frozen for inference (wbwtab.freeze_inference); call "
-                           "freeze_inference(model, enable=False) before training it")
+def _b1_pool_fallback(pp, link, x, plane):
+    return pp.pool(F_.materialized(x))
 
 
 def _frozen_conv_operands(conv):
     """(w_int, alpha, bias, XNOR weight image) computed once; re-done when a parameter or buffer is written in place"""
-    key = tuple(t._version for t in list(conv.parameters()) + list(conv.buffers()))
-    fr = conv.__dict__.get("_mnb_xnor_ops")
-    if fr is None or fr[0] != key:
+    def make():
         lv = frozen_levels(conv)
         if lv is None:
             raise RuntimeError("micronet_b200: the weights of a frozen wbwtab layer changed to values the XNOR kernel cannot "
                                "hold (NaN alpha or not alpha * {-1, 0, 1}); call wbwtab.freeze_inference(model) again")
-        key = tuple(t._version for t in list(conv.parameters()) + list(conv.buffers()))   # W = 2 centres in place
-        fr = (key, lv[0], lv[1], None if conv.bias is None else conv.bias.detach(), {})
-        conv.__dict__["_mnb_xnor_ops"] = fr
-    return fr[1:]
+        return lv[0], lv[1], None if conv.bias is None else conv.bias.detach(), {}
+    return FG.cached_operands(conv, "_mnb_ops", make)
 
 
-def _frozen_conv_forward(link, conv, x, kind="xnor"):
+def _record(rw, conv, kernel, fmt, link):
+    """the record of a frozen conv (or stem binarizer), read by its forward: the kernel it runs, the format it hands over,
+    its link"""
+    rw.set_dict(conv, "_mnb_frozen", {"kernel": kernel, "fmt": fmt, "link": link})
+    rw.set_dict(conv, "_mnb_frozen_plan", (kernel, fmt))
+
+
+def _frozen_conv_forward(conv, x):
     """XNOR (or, outside its cover, binary tensor-core) conv whose epilogue applies the absorbed BatchNorm / binarizer /
     pool / shuffle and writes the consumer's operand"""
     from . import b1 as B1, xnor as XN
+    rec = conv.__dict__["_mnb_frozen"]
+    kind, link = rec["kernel"], rec["link"]
     K = B1 if kind == "b1" else XN
     _check_eval(conv)
     w_int, alpha, bias, images = _frozen_conv_operands(conv)
@@ -343,7 +313,7 @@ def _frozen_conv_forward(link, conv, x, kind="xnor"):
     post, keep = link.post()
     nbytes = K.post_bytes(sh, post)
     if nbytes >= 0:
-        plane = _handed_b1(conv, x) if kind == "b1" else _handed_bits(conv, x)
+        plane = F_.handed_plane(conv, x)
         if plane is None:
             plane = K.pack_act(F_.materialized(x).contiguous(), conv.groups)
         if "w_img" not in images:
@@ -362,11 +332,12 @@ def _frozen_conv_forward(link, conv, x, kind="xnor"):
     return link.tail(y)
 
 
-def _frozen_stem_forward(link, act, x):
+def _frozen_stem_forward(act, x):
     """the binarizer behind the un-quantized stem conv: [eval BatchNorm] + sign [+ pool] [+ shuffle] straight into the
     first XNOR layer's bit plane"""
     import torch
     from . import b1 as B1, xnor as XN
+    link = act.__dict__["_mnb_frozen"]["link"]
     K = B1 if link.fmt == L.XNOR_B1_PLANE else XN
     _check_eval(act)
     x = F_.materialized(x)
@@ -387,31 +358,17 @@ def _frozen_stem_forward(link, act, x):
     return link.tail(x)
 
 
-def _absorbed(m, x):
-    _check_eval(m)
-    return x
-
-
-def _block_parts(blk):
-    """[conv, act] of a conv-bn-act block: NIN-GC's (with channel_shuffle_flag) or the reference nin.py one (without)"""
-    parts = [k for k in blk.children() if not isinstance(k, nn.Identity)]
-    return parts if len(parts) == 2 and isinstance(parts[0], nn.Conv2d) else None
-
-
-def _blocks(seq):
-    """[(index in kids, name, block, conv, binarizer)] of the conv-bn-act blocks of an nn.Sequential that end in a binarizer
-    (BatchNormBinarize2d, or a BatchNorm-fused conv followed by ActivationQuantizer(A=2))"""
+def _bit_block(blk):
+    """(conv, binarizer) of a conv-bn-act block that ends in a binarizer (BatchNormBinarize2d, or a BatchNorm-fused conv
+    followed by ActivationQuantizer(A=2)), else None"""
     from .fused import BatchNormBinarize2d
-    out = []
-    kids = [(n, k) for n, k in seq.named_children() if not isinstance(k, nn.Identity)]
-    for i, (name, blk) in enumerate(kids):
-        parts = _block_parts(blk)
-        if parts is None:
-            continue
-        act = parts[1]
-        if isinstance(act, BatchNormBinarize2d) or (type(act) is ActivationQuantizer and act.A == 2):
-            out.append((i, name, blk, parts[0], act))
-    return kids, out
+    bp = FG.block_parts(blk)
+    if bp is None or len(bp[1]) != 1:
+        return None
+    act = bp[1][0]
+    if isinstance(act, BatchNormBinarize2d) or (type(act) is ActivationQuantizer and act.A == 2):
+        return bp[0], act
+    return None
 
 
 def _head_conv(conv):
@@ -420,14 +377,73 @@ def _head_conv(conv):
             and not isinstance(conv.padding, str))
 
 
-def _undo(model):
-    for kind, obj, key, val in reversed(model.__dict__.pop("_mnb_xnor_undo", [])):
-        if kind == "child":
-            obj._modules[key] = val
-        elif kind == "attr":
-            setattr(obj, key, val)
+def _freeze_bits(model, rw):
+    """link the conv-bn-act blocks that end in a binarizer (see freeze_inference)"""
+    from .fused import BatchNormBinarize2d, EnginePmConv2d
+    frozen = {}             # conv -> the kernel it runs frozen ("xnor" / "b1")
+    links = []
+    # from the last block back: a producer is frozen only when its consumer reads what it writes
+    for (conv, act), pool, cfg, nxt, cconv, slot in reversed(list(FG.block_pairs(model, _bit_block, FG.max_pool_cfg))):
+        bnb = isinstance(act, BatchNormBinarize2d)
+        fold = ppool = None
+        if pool is not None:
+            if cfg == (2, 2, 0) and not bnb:
+                fold = pool         # the 2x2 pool moves into the epilogue
+            elif cfg != (2, 2, 0) and int(getattr(pool, "out_shuffle_groups", 1)) == 1:
+                ppool = pool        # taken on the consumer's b1 plane (mnb_b1_plane_maxpool), if it has one
+            else:
+                continue
+        shuffled = FG.block_shuffle(nxt) > 1
+        if bnb and shuffled:
+            continue        # a shuffle the fused producer did not take (not a graph prepare(fuse_bn=True) builds)
+        sg = FG.block_shuffle(nxt) if shuffled else (int(act.out_shuffle_groups) if bnb else 1)
+        ckind = frozen.get(cconv)
+        if ppool is not None and ckind != "b1":
+            continue        # a pool the epilogue cannot take and no b1 plane to take it on
+        if ckind is not None:
+            link = _Link(cconv, L.XNOR_B1_PLANE if ckind == "b1" else L.XNOR_BITS, cconv.groups, act, fold, sg)
+        elif (_head_conv(cconv) and not isinstance(cconv, QuantConv2d) and sg == 1 and pool is None
+              and not (bnb and act.pool2)):
+            link = _Link(cconv, L.XNOR_PM1_BF16, 1, act, None, 1)
         else:
-            obj.__dict__.pop(key, None)
+            continue
+        kind = None
+        if isinstance(conv, QuantConv2d):
+            kind = _frozen_kernel(conv)
+            # an XNOR producer has no b1-plane epilogue: in front of a b1 consumer it runs un-frozen
+            if kind is None or (kind == "xnor" and link.fmt == L.XNOR_B1_PLANE):
+                continue
+            frozen[conv] = kind
+        elif link.fmt == L.XNOR_PM1_BF16:
+            continue
+        links.append((conv, kind, link, cfg, slot, ppool, nxt, shuffled))
+    for conv, kind, link, cfg, slot, ppool, nxt, shuffled in links:
+        if ppool is not None:
+            # the pool reads what the producer writes and hands its pooled plane to the consumer
+            link.consumer = _PlanePool(ppool, cfg, link.consumer)
+            rw.set_child(*slot, link.consumer)
+        if kind is not None:
+            _record(rw, conv, kind, link.fmt, link)
+            rw.forget(conv, "_mnb_ops")
+            rw.override(conv, _frozen_conv_forward, conv)
+            rw.override(link.act, FG.absorbed_forward, _check_eval, link.act, None)    # done in the conv's epilogue
+        else:
+            _record(rw, link.act, "b1" if link.fmt == L.XNOR_B1_PLANE else "xnor", link.fmt, link)
+            rw.override(link.act, _frozen_stem_forward, link.act)
+        if link.pool is not None:
+            rw.set_child(*slot, nn.Identity())
+        if shuffled:
+            rw.set_attr(nxt, "channel_shuffle_flag", 0)
+        if link.fmt == L.XNOR_PM1_BF16 and type(link.consumer) is nn.Conv2d:
+            # the BatchNorm-fused head reads the +-1 plane on the packed-operand family (same parameters)
+            h = link.consumer
+            pm = EnginePmConv2d(h.in_channels, h.out_channels, h.kernel_size, h.stride, h.padding, h.dilation, h.groups,
+                                h.bias is not None, h.padding_mode)
+            pm.weight, pm.bias = h.weight, h.bias
+            pm.train(h.training)
+            for n, k in list(nxt.named_children()):
+                if k is h:
+                    rw.set_child(nxt, n, pm)
 
 
 # --------------------------------------------------------------------------
@@ -469,14 +485,12 @@ def _a32_freezable(conv):
     return L.PK_MODE != "off" and PK.supported(sh, 0, A32_TERMS, 1)
 
 
-class _TermLink:
-    """a producer -> consumer hand-off of an A=32 graph: the consumer conv, the eval BatchNorm the producer applies before the
-    ReLU, the consumer block's channel shuffle and the max-pool (module, k, s, p) in between, which runs on the term plane"""
+class _TermLink(FG.Link):
+    """frozen_graph.Link of an A=32 graph: the producer applies the eval BatchNorm before the ReLU and the consumer block's
+    channel shuffle and writes the consumer's term planes; the max-pool in between runs on them"""
 
     def __init__(self, cconv, bn, sg, pool):
-        self.cconv, self.bn, self.sg, self.pool = cconv, bn, int(sg), pool
-        self.target = pool[0] if pool is not None else cconv
-        self._invstd = None
+        super().__init__(cconv, bn, None, sg, pool)
 
     @property
     def split(self):
@@ -504,65 +518,34 @@ class _TermLink:
         sh = F_._shape_struct((b, ch, h, w), c.weight.shape, c.stride, c.padding, c.dilation, c.groups)
         return L.PK_MODE != "off" and PK.supported(sh, 0, A32_TERMS, 1)
 
-    def bn_tensors(self):
-        """(mean, invstd, gamma, beta) of the eval BatchNorm (running statistics); invstd re-computed when running_var changes"""
-        import torch
-        bn = self.bn
-        rv = bn.running_var
-        key = (rv.data_ptr(), rv._version, float(bn.eps))
-        if self._invstd is None or self._invstd[0] != key:
-            self._invstd = (key, torch.rsqrt(rv + bn.eps))
-        return bn.running_mean, self._invstd[1], bn.weight.detach(), bn.bias.detach()
-
     def tag(self, plane, shape):
         import torch
         y = torch.empty(shape, dtype=torch.float32, device="meta")   # shape only: the data lives in the term plane
-        y._mnb_terms = (self.target, plane, y._version, self.split, A32_TERMS)
-        return y
+        return F_.tag(y, self.target, plane, "terms", split=self.split, terms=A32_TERMS)
 
 
-def _handed_terms(module, x):
-    """the term plane a frozen producer (or a term-plane pool) wrote for ``module``, if ``x`` is that unmodified output"""
-    pre = getattr(x, "_mnb_terms", None)
-    if pre is not None and pre[0] is module and x._version == pre[2]:
-        return pre[1]
+def _terms_pool(plane, x, k, s, p):
+    from . import pk as PK
+    rc, out = PK.plane_maxpool_terms(plane, *x.shape, k, s, p, A32_TERMS)
+    if rc == 0:
+        return out
+    if rc != L.E_UNSUPPORTED:
+        L.check(rc, "pk_plane_maxpool_terms")
     return None
 
 
-def _a32_passthrough(m, link, x):
-    """the BatchNorm / ReLU of a block whose producer wrote its consumer's term plane: the tagged output passes through;
-    anything else (a producer that wrote fp32) runs the module as usual"""
-    _check_eval(m)
-    if _handed_terms(link.target, x) is not None:
-        return x
-    return type(m).forward(m, x)
+def _terms_pool_fallback(pool, link, x, plane):
+    """the pool as usual on the decoded tensor, in the producer's channel order: a refused plane holds the consumer's
+    (shuffled) order, and the consumer applies its block's shuffle itself when no plane arrives (shuffle with C / sg groups
+    is the inverse of the shuffle with sg)"""
+    y = F_.materialized(x)
+    if plane is not None and link.sg > 1:
+        y = FG.shuffle(y, y.shape[1] // link.sg)
+    return type(pool).forward(pool, y)
 
 
-def _a32_pool_forward(pool, link, x):
-    """the max-pool between a frozen producer and its consumer, on the producer's term plane (mnb_pk_plane_maxpool_terms)"""
-    from . import pk as PK
-    _check_eval(pool)
-    plane = _handed_terms(pool, x)
-    if plane is not None:
-        _, k, s, p = link.pool
-        b, c, h, w = x.shape
-        rc, out = F_._timed("plane_pool", L.ConvShape(b, c, h, w, c, k, k, s, s, p, p, 1, 1, 1),
-                            lambda: PK.plane_maxpool_terms(plane, b, c, h, w, k, s, p, A32_TERMS))
-        if rc == 0:
-            y = link.tag(out, link.read_shape(x.shape))
-            y._mnb_terms = (link.cconv,) + y._mnb_terms[1:]
-            return y
-        if rc != L.E_UNSUPPORTED:
-            L.check(rc, "pk_plane_maxpool_terms")
-        # the pool as usual on the decoded tensor, in the producer's channel order: the plane holds the consumer's (shuffled)
-        # order, and the consumer applies its block's shuffle itself when no plane arrives (shuffle with C / sg groups is the
-        # inverse of the shuffle with sg)
-        y = F_.materialized(x)
-        if link.sg > 1:
-            from .frozen_graph import shuffle
-            y = shuffle(y, y.shape[1] // link.sg)
-        return type(pool).forward(pool, y)
-    return type(pool).forward(pool, F_.materialized(x))
+# the max-pool between a frozen producer and its consumer, on the producer's term plane (mnb_pk_plane_maxpool_terms)
+_a32_pool_forward = functools.partial(FG.pool_forward, _check_eval, _terms_pool, _terms_pool_fallback)
 
 
 def _a32_produce(link, y):
@@ -601,20 +584,20 @@ def _epilogue_hand_off(link, sh):
     return link.sg == 1 and not PK.segmented(sh, 0, A32_TERMS, 1)
 
 
-def _a32_conv_forward(conv, link, x):
+def _a32_conv_forward(conv, x):
     """eval forward of a frozen A=32 conv: its cached weight levels and (3, 1) weight image, the term plane its producer wrote
     (else its own pack of x) and, with a link, its consumer's term plane written by the epilogue (BatchNorm, ReLU, shuffle)"""
     import torch
     from . import pk as PK
     _check_eval(conv)
+    link = conv.__dict__["_mnb_frozen"]["link"]
     w_int, alpha, bias, images = _frozen_conv_operands(conv)
-    plane = _handed_terms(conv, x)
+    plane = F_.handed_plane(conv, x)
     if plane is None:
         x = F_.materialized(x)
         sg = conv.__dict__.get("_mnb_in_shuffle", 1)
         if sg > 1:
-            from .frozen_graph import shuffle
-            x = shuffle(x, sg)      # the block's channel shuffle that freeze_inference moved into the producer
+            x = FG.shuffle(x, sg)      # the block's channel shuffle that freeze_inference moved into the producer
     sh = F_._shape_struct(x.shape, conv.weight.shape, conv.stride, conv.padding, conv.dilation, conv.groups)
     p, q = F_._out_hw(sh)
     out_shape = (x.shape[0], conv.out_channels, p, q)
@@ -653,55 +636,34 @@ def _a32_conv_forward(conv, link, x):
     return y
 
 
-def _freeze_a32(seq, undo):
-    """link the A=32 conv-bn-act blocks of one nn.Sequential (DESIGN.md 4.20); returns the number of frozen convs"""
-    from .fused import EngineFloatConv2d, EngineMaxPool2d, _pool_cfg
-    kids = [(n, k) for n, k in seq.named_children() if not isinstance(k, nn.Identity)]
-    parsed = [_a32_block(k) for _, k in kids]
-    frozen = set()
-    for p in parsed:
-        if p is not None and _a32_freezable(p[0]):
-            frozen.add(p[0])
+def _freeze_a32(model, rw):
+    """link the A=32 conv-bn-act blocks (DESIGN.md 4.20)"""
+    from .fused import EngineFloatConv2d
+    frozen = {p[0] for p in FG.blocks(model, _a32_block) if _a32_freezable(p[0])}
     for conv in frozen:
-        conv.__dict__["_mnb_xnor"] = lambda m, x: _a32_conv_forward(m, m.__dict__.get("_mnb_a32_link"), x)
-        conv.__dict__["_mnb_frozen_plan"] = ("pk", "fp32")
-        for key in ("_mnb_xnor", "_mnb_frozen_plan", "_mnb_xnor_ops", "_mnb_a32_link", "_mnb_in_shuffle"):
-            undo.append(("dict", conv, key, None))
-    for i, p in enumerate(parsed):
-        if p is None:
+        _record(rw, conv, "pk", "fp32", None)
+        rw.forget(conv, "_mnb_ops")
+        rw.override(conv, _a32_conv_forward, conv)
+    for (conv, bn, act), pool, cfg, nxt, cconv, _ in FG.block_pairs(model, _a32_block, FG.max_pool_cfg):
+        if cconv not in frozen or bn.training or (pool is not None and tuple(cconv.stride) != (1, 1)):
             continue
-        conv, bn, act = p
-        j, pool = i + 1, None
-        if j < len(kids) and type(kids[j][1]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j][1]) is not None:
-            pool, j = (kids[j][1],) + _pool_cfg(kids[j][1]), j + 1
-        if j >= len(kids) or parsed[j] is None or parsed[j][0] not in frozen:
-            continue
-        nxt, cconv = kids[j][1], parsed[j][0]
-        if bn.training or (pool is not None and tuple(cconv.stride) != (1, 1)):
-            continue
-        if pool is not None and int(getattr(pool[0], "out_shuffle_groups", 1)) != 1:
+        if pool is not None and int(getattr(pool, "out_shuffle_groups", 1)) != 1:
             continue
         stem = type(conv) in (nn.Conv2d, EngineFloatConv2d)
         if not (conv in frozen or stem):
             continue
-        sg = int(getattr(nxt, "shuffle_groups", 1)) if getattr(nxt, "channel_shuffle_flag", 0) else 1
-        link = _TermLink(cconv, bn, sg, pool)
+        sg = FG.block_shuffle(nxt)
+        link = _TermLink(cconv, bn, sg, None if pool is None else (pool,) + cfg)
         if stem:
-            bn.__dict__["forward"] = lambda x, m=bn, link=link: _a32_stem_forward(m, link, x)
+            rw.override(bn, _a32_stem_forward, bn, link)
         else:
-            conv.__dict__["_mnb_a32_link"] = link
-            conv.__dict__["_mnb_frozen_plan"] = ("pk", A32_PLANE)
-            bn.__dict__["forward"] = lambda x, m=bn, link=link: _a32_passthrough(m, link, x)
-        act.__dict__["forward"] = lambda x, m=act, link=link: _a32_passthrough(m, link, x)
-        undo += [("dict", bn, "forward", None), ("dict", act, "forward", None)]
+            _record(rw, conv, "pk", A32_PLANE, link)
+            rw.override(bn, FG.absorbed_forward, _check_eval, bn, link.target)
+        rw.override(act, FG.absorbed_forward, _check_eval, act, link.target)
         if pool is not None:
-            pool[0].__dict__["forward"] = lambda x, m=pool[0], link=link: _a32_pool_forward(m, link, x)
-            undo.append(("dict", pool[0], "forward", None))
+            rw.override(pool, _a32_pool_forward, pool, link)
         if sg > 1:
-            undo.append(("attr", nxt, "channel_shuffle_flag", nxt.channel_shuffle_flag))
-            nxt.channel_shuffle_flag = 0
-            cconv.__dict__["_mnb_in_shuffle"] = sg      # applied by the consumer itself when no plane arrives
-    return len(frozen)
+            rw.move_shuffle(nxt, cconv, sg)
 
 
 def freeze_inference(model, enable=True):
@@ -729,95 +691,16 @@ def freeze_inference(model, enable=True):
     that conv's three exact bf16 pieces of ReLU(BatchNorm(y)) in the next block's channel order from its epilogue
     (mnb_pk_conv_post with terms_out), the pool runs on the plane (mnb_pk_plane_maxpool_terms), and the fp32 stem conv's
     BatchNorm + ReLU write the first plane (mnb_bn_relu_pack_terms_fwd).  The last quantized conv writes fp32 for the head.
-    ``_mnb_frozen_plan`` is ("pk", "terms3") for a conv writing term planes, ("pk", "fp32") for one writing fp32.  The logits
+    Each frozen conv holds its record ``_mnb_frozen``: the kernel it runs, the format it hands over and its link;
+    ``_mnb_frozen_plan`` is (kernel, format): ("xnor" or "b1", the XNOR post format) on bit planes, ("pk", "terms3") for an
+    A=32 conv writing term planes and ("pk", "fp32") for one writing fp32.  The logits
     equal a block-by-block composition of those kernels bit for bit; against the un-frozen forward (another conv kernel,
     ATen's BatchNorm) they agree to the fp32 contract.
     Parameters, buffers and state_dict keys are unchanged; ``enable=False`` restores the modules (needed before training)."""
-    from .fused import BatchNormBinarize2d, EngineMaxPool2d, EnginePmConv2d, _pool_cfg
-    _undo(model)
+    FG.undo(model, _UNDO)
     if not enable:
         return model
-    undo = model.__dict__.setdefault("_mnb_xnor_undo", [])
-    for seq in [m for m in model.modules() if isinstance(m, nn.Sequential)]:
-        kids, blocks = _blocks(seq)
-        frozen = {}             # conv -> the kernel it runs frozen ("xnor" / "b1")
-        links = []
-        # from the last block back: a producer is frozen only when its consumer reads what it writes
-        for i, name, blk, conv, act in reversed(blocks):
-            j, pool, ppool = i + 1, None, None
-            if (j < len(kids) and type(kids[j][1]) in (nn.MaxPool2d, EngineMaxPool2d) and _pool_cfg(kids[j][1]) == (2, 2, 0)
-                    and not isinstance(act, BatchNormBinarize2d)):
-                pool, j = kids[j], j + 1
-            elif j < len(kids) and _pool_cfg_b1(kids[j][1]) is not None and _pool_cfg_b1(kids[j][1]) != (2, 2, 0):
-                ppool, j = kids[j], j + 1     # taken on the consumer's b1 plane (mnb_b1_plane_maxpool), if it has one
-            if j >= len(kids):
-                continue
-            nxt = kids[j][1]
-            shuffled = bool(getattr(nxt, "channel_shuffle_flag", 0)) and int(getattr(nxt, "shuffle_groups", 1)) > 1
-            if isinstance(act, BatchNormBinarize2d) and shuffled:
-                continue        # a shuffle the fused producer did not take (not a graph prepare(fuse_bn=True) builds)
-            nparts = [k for k in nxt.children() if not isinstance(k, nn.Identity)]
-            cconv = nparts[0] if nparts and isinstance(nparts[0], nn.Conv2d) else None
-            if cconv is None:
-                continue
-            sg = int(nxt.shuffle_groups) if shuffled else (int(act.out_shuffle_groups) if isinstance(act, BatchNormBinarize2d) else 1)
-            ckind = frozen.get(cconv)
-            if ppool is not None and ckind != "b1":
-                continue        # a pool the epilogue cannot take and no b1 plane to take it on
-            link = None
-            if ckind == "b1":
-                link = _Link(cconv, L.XNOR_B1_PLANE, cconv.groups, act, pool[1] if pool else None, sg)
-            elif ckind == "xnor":
-                link = _Link(cconv, L.XNOR_BITS, cconv.groups, act, pool[1] if pool else None, sg)
-            elif _head_conv(cconv) and not isinstance(cconv, QuantConv2d) and sg == 1 and pool is None and not (
-                    isinstance(act, BatchNormBinarize2d) and act.pool2):
-                link = _Link(cconv, L.XNOR_PM1_BF16, 1, act, None, 1)
-            if link is None:
-                continue
-            if isinstance(conv, QuantConv2d):
-                kind = _frozen_kernel(conv)
-                # an XNOR producer has no b1-plane epilogue: in front of a b1 consumer it runs un-frozen
-                if kind is None or (kind == "xnor" and link.fmt == L.XNOR_B1_PLANE):
-                    continue
-                frozen[conv] = kind
-                links.append(("conv", conv, link, pool, nxt, shuffled, ppool, kind))
-            elif link.fmt in (L.XNOR_BITS, L.XNOR_B1_PLANE) and type(conv) is not QuantConv2d:
-                links.append(("stem", act, link, pool, nxt, shuffled, ppool, None))
-        for kind, mod, link, pool, nxt, shuffled, ppool, ckind in links:
-            if ppool is not None:
-                # the pool reads what the producer writes and hands its pooled plane to the consumer
-                pp = _PlanePool(ppool[1], link.consumer)
-                pp.train(ppool[1].training)
-                link.consumer = pp
-                undo.append(("child", seq, ppool[0], ppool[1]))
-                seq._modules[ppool[0]] = pp
-            if kind == "conv":
-                mod.__dict__["_mnb_xnor"] = lambda m, x, link=link, k=ckind: _frozen_conv_forward(link, m, x, k)
-                mod.__dict__["_mnb_frozen_plan"] = (ckind, link.fmt)     # the kernel and hand-off format (introspection)
-                undo.append(("dict", mod, "_mnb_frozen_plan", None))
-                undo.append(("dict", mod, "_mnb_xnor", None))
-                undo.append(("dict", mod, "_mnb_xnor_ops", None))
-                link.act.__dict__["_mnb_xnor"] = _absorbed       # its work is done in the conv's epilogue
-                undo.append(("dict", link.act, "_mnb_xnor", None))
-            else:
-                mod.__dict__["_mnb_xnor"] = lambda m, x, link=link: _frozen_stem_forward(link, m, x)
-                undo.append(("dict", mod, "_mnb_xnor", None))
-            if pool is not None:
-                undo.append(("child", seq, pool[0], pool[1]))
-                seq._modules[pool[0]] = nn.Identity()
-            if shuffled:
-                undo.append(("attr", nxt, "channel_shuffle_flag", nxt.channel_shuffle_flag))
-                nxt.channel_shuffle_flag = 0
-            if link.fmt == L.XNOR_PM1_BF16 and type(link.consumer) is nn.Conv2d:
-                # the BatchNorm-fused head reads the +-1 plane on the packed-operand family (same parameters)
-                h = link.consumer
-                pm = EnginePmConv2d(h.in_channels, h.out_channels, h.kernel_size, h.stride, h.padding, h.dilation, h.groups,
-                                    h.bias is not None, h.padding_mode)
-                pm.weight, pm.bias = h.weight, h.bias
-                pm.train(h.training)
-                for n, k in nxt.named_children():
-                    if k is h:
-                        undo.append(("child", nxt, n, h))
-                        nxt._modules[n] = pm
-        _freeze_a32(seq, undo)
+    rw = FG.Rewrite(model, _UNDO)
+    _freeze_bits(model, rw)
+    _freeze_a32(model, rw)
     return model

@@ -118,7 +118,8 @@ def _a32(base_fn, name, batch):
     wbwtab.freeze_inference(m)
     out = {}
     for n, c in m.named_modules():
-        link = c.__dict__.get("_mnb_a32_link")
+        rec = c.__dict__.get("_mnb_frozen")
+        link = None if rec is None or rec["fmt"] != wbwtab.A32_PLANE else rec["link"]
         if link is None:
             continue
         shape = _shape(shapes[n], c)

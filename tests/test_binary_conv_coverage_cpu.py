@@ -94,9 +94,9 @@ def _conv_inputs(m, hw=32):
 
 
 def _link(conv):
-    """the (_Link, kernel) freeze_inference bound to a frozen conv's forward, or None when the conv stayed un-frozen"""
-    fn = conv.__dict__.get("_mnb_xnor")
-    return None if fn is None else fn.__defaults__
+    """the (_Link, kernel) of a frozen conv's record, or None when the conv stayed un-frozen"""
+    rec = conv.__dict__.get("_mnb_frozen")
+    return None if rec is None else (rec["link"], rec["kernel"])
 
 
 def _post_of(link):
@@ -126,7 +126,7 @@ def frozen():
     return {name: _frozen_layers(name) for name in ("nin", "nin_gc", "pruned")}
 
 
-def test_frozen_graph_convs_are_covered_by_cases(frozen):
+def test_frozen_records_are_covered_by_cases(frozen):
     tested = {(k, BC.plan_tuple(k, p)) for _, k, p in _launches()}
     missing, n = [], 0
     for name, (_, layers) in frozen.items():
@@ -143,7 +143,7 @@ def test_frozen_graph_convs_are_covered_by_cases(frozen):
     assert not missing, f"plans of frozen-graph convs no case runs: {missing}"
 
 
-def test_model_cases_are_the_frozen_links(frozen):
+def test_model_cases_are_the_frozen_records(frozen):
     """MODEL_LAYERS is what freeze_inference links today: same kernel, geometry and hand-off for every layer"""
     want = [(m, layer, BC.MODEL_KERNEL[m], geo, post) for m, layer, geo, post in BC.MODEL_LAYERS]
     got = []
@@ -154,7 +154,7 @@ def test_model_cases_are_the_frozen_links(frozen):
     assert got == want
 
 
-def test_pruned_nin_gc_link_plan(frozen):
+def test_pruned_nin_gc_frozen_records(frozen):
     """README-cfg pruned NIN-GC (154 162 144 304 320 320 608 584): all seven binarized convs freeze on the XNOR kernel
     (76 - 81 channels per group on the 1x1 layers: three words, the third partial), each epilogue writes its consumer's bit
     plane at the consumer's groups with the consumer block's shuffle and the folded 2x2 pools, the last one the head's bf16
@@ -176,9 +176,9 @@ def test_pruned_nin_gc_link_plan(frozen):
     assert nws == [3, 3, 1, 3, 3, 1, 3]
     # the stem's binarizer: a producer of L1's bit plane (2 groups of 77 channels)
     acts = [k for k in m.modules() if isinstance(k, fused.BatchNormBinarize2d)]
-    stem = acts[0].__dict__.get("_mnb_xnor")
-    assert stem is not None and stem.__defaults__[0].fmt == L.XNOR_BITS and stem.__defaults__[0].out_groups == 2
-    assert all(k.__dict__.get("_mnb_xnor") is not None for k in acts[1:])     # absorbed into the conv epilogues
+    stem = acts[0].__dict__.get("_mnb_frozen")
+    assert stem is not None and stem["link"].fmt == L.XNOR_BITS and stem["link"].out_groups == 2
+    assert all("forward" in k.__dict__ for k in acts[1:])     # absorbed into the conv epilogues
     assert not any(type(k).__name__ == "_PlanePool" for k in m.modules())
 
 

@@ -249,7 +249,7 @@ def _all_links(m):
     return out
 
 
-def test_resnet18_links_unchanged():
+def test_resnet18_links_and_undo_record():
     """ResNet-18 keeps exactly the links of its two rules: adjacent convs of a residual_function, QuantAdd -> first conv of
     the next block; no block link, no override"""
     from micronet_b200 import iao
@@ -260,6 +260,9 @@ def test_resnet18_links_unchanged():
     want |= {(f"{b0}.add", f"{b1}.residual_function.0", False) for b0, b1 in zip(blocks, blocks[1:])}
     assert _all_links(m) == want
     assert not any("forward" in c.__dict__ or "_mnb_in_shuffle" in c.__dict__ for c in m.modules())
-    assert "_mnb_iao_undo" not in m.__dict__ or m.__dict__["_mnb_iao_undo"] == []
+    # the undo record holds the flags, the folded ReLUs and the links above: no block link moved a shuffle or a pool
+    flags = {"_frozen_inference", "_int8", "_frozen", "_int_levels", "_pre_relu", "_fuse_relu", "_post_consumer"}
+    for rec in m.__dict__["_mnb_iao_undo"]:
+        assert (rec[0] == "dict" and rec[2] in flags) or (rec[0] == "child" and type(rec[3]) is nn.ReLU), rec
     iao.freeze_inference(m, enable=False)
     assert _all_links(m) == set()

@@ -214,7 +214,7 @@ def links():
     return K.linked_convs()
 
 
-def test_every_linked_model_conv_is_a_case(links, plans):
+def test_every_recorded_link_is_a_case(links, plans):
     """every conv that freeze_inference links to its consumer, at the graph's bench batch, is a case with the same shape,
     epilogue path and consumer options (shuffle, BatchNorm, phase split, ReLU, quantizer, term planes), and the case lists it"""
     from tests import pk_post_links as K

@@ -35,7 +35,9 @@ def _plan(m):
 
 
 def _links(m):
-    return [c.__dict__.get("_mnb_a32_link") for c in _quant_convs(m)]
+    """the link of each quantized conv that writes term planes (None for the others)"""
+    recs = [c.__dict__.get("_mnb_frozen") for c in _quant_convs(m)]
+    return [r["link"] if r is not None and r["fmt"] == "terms3" else None for r in recs]
 
 
 def _overridden(m, cls):
@@ -47,7 +49,7 @@ TERMS, FP32 = ("pk", "terms3"), ("pk", "fp32")
 
 @pytest.mark.parametrize("W", [2, 3])
 @pytest.mark.parametrize("name", ["nin", "ref_nin"])
-def test_nin_link_plan(name, W):
+def test_nin_frozen_records(name, W):
     import micronet_b200 as E
     m = _model(name, W)
     tree = [type(k) for k in m.modules()]
@@ -72,7 +74,7 @@ def test_nin_link_plan(name, W):
 
 
 @pytest.mark.parametrize("W", [2, 3])
-def test_nin_gc_link_plan(W):
+def test_nin_gc_frozen_records(W):
     import micronet_b200 as E
     m = _model("nin_gc", W)
     flags = [getattr(b, "channel_shuffle_flag", None) for b in m.model.children()]
@@ -111,7 +113,7 @@ SEGMENTED = {"nin": {3, 6}, "nin_gc": set()}
 
 
 @pytest.mark.parametrize("name", ["nin", "nin_gc"])
-def test_plan_table_at_terms_3_1(name):
+def test_record_table_at_terms_3_1(name):
     """mnb_pk_conv_plan_ex of every quantized layer at batch 256 and how its output reaches its consumer"""
     from micronet_b200 import _lib as L
     shapes = _layer_shapes(name)

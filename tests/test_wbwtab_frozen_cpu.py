@@ -142,7 +142,7 @@ def _g1(raw=None, nan=None):
 
 def _frozen_convs(m):
     import micronet_b200 as E
-    return [i for i, c in enumerate(c for c in m.modules() if isinstance(c, E.wbwtab.QuantConv2d)) if "_mnb_xnor" in c.__dict__]
+    return [i for i, c in enumerate(c for c in m.modules() if isinstance(c, E.wbwtab.QuantConv2d)) if "_mnb_frozen" in c.__dict__]
 
 
 def _snapshot(m):
@@ -155,7 +155,7 @@ def _same(a, b):
     assert a[1].keys() == b[1].keys() and all(torch.equal(a[1][k], b[1][k]) for k in a[1])
 
 
-def test_g2_recognition_and_restore():
+def test_g2_records_and_restore():
     import micronet_b200 as E
     from micronet_b200.fused import BatchNormBinarize2d
     m = _g2()
@@ -163,15 +163,15 @@ def test_g2_recognition_and_restore():
     E.wbwtab.freeze_inference(m)
     assert _frozen_convs(m) == list(range(7))                          # L1 .. L7
     bnb = [k for k in m.modules() if isinstance(k, BatchNormBinarize2d)]
-    assert len(bnb) == 8 and all("_mnb_xnor" in k.__dict__ for k in bnb)   # stem producer + seven absorbed
+    assert len(bnb) == 8 and all("forward" in k.__dict__ for k in bnb)     # stem producer + seven absorbed
     # nothing structural moved: the fused graph already folded pools and shuffles
     _same(before, _snapshot(m))
     E.wbwtab.freeze_inference(m, enable=False)
-    assert _frozen_convs(m) == [] and not any("_mnb_xnor" in k.__dict__ for k in m.modules())
+    assert _frozen_convs(m) == [] and not any("forward" in k.__dict__ for k in m.modules())
     _same(before, _snapshot(m))
 
 
-def test_g2_all_zero_ternary_channel_is_not_frozen():
+def test_g2_all_zero_ternary_channel_has_no_record():
     import micronet_b200 as E
     m = _g2()
     convs = [c for c in m.modules() if isinstance(c, E.wbwtab.QuantConv2d)]
@@ -182,7 +182,7 @@ def test_g2_all_zero_ternary_channel_is_not_frozen():
     assert _frozen_convs(m) == [4, 5, 6]
 
 
-def test_g1_recognition_and_restore():
+def test_g1_records_and_restore():
     import micronet_b200 as E
     from micronet_b200.fused import EnginePmConv2d
     m = _g1()
@@ -194,7 +194,7 @@ def test_g1_recognition_and_restore():
     assert all(getattr(b, "channel_shuffle_flag", 0) == 0 for b in seq.children())     # every shuffle folded
     assert isinstance(seq._modules["10"].conv, EnginePmConv2d)                        # the head reads the bf16 plane
     aqs = [k for k in m.modules() if isinstance(k, E.wbwtab.ActivationQuantizer)]
-    assert len(aqs) == 8 and all("_mnb_xnor" in k.__dict__ for k in aqs)
+    assert len(aqs) == 8 and all("forward" in k.__dict__ for k in aqs)
     assert m.state_dict().keys() == before[1].keys()
     E.wbwtab.freeze_inference(m, enable=False)
     _same(before, _snapshot(m))
@@ -202,7 +202,7 @@ def test_g1_recognition_and_restore():
 
 
 @pytest.mark.parametrize("what", ["raw", "nan"])
-def test_g1_refuses_weights_that_are_not_ternary_levels(what):
+def test_g1_records_no_weights_that_are_not_ternary_levels(what):
     import micronet_b200 as E
     from micronet_b200.fused import EnginePmConv2d
     m = _g1(**{what: 3})                                               # L4: raw fp32 weights, or a NaN channel
