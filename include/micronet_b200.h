@@ -430,12 +430,16 @@ int mnb_pk_pack_act_grouped(const float* x, int32_t batch, int32_t channels, int
                             int32_t terms, const float* ch_scale, int32_t phase_split, int32_t relu, void* out_pk,
                             uint8_t* bits8, int32_t groups, mnb_stream_t stream);
 int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out16); /* host only */
-/* host only, the plan mnb_pk_conv / mnb_pk_wgrad will run (same MNB_PK_* environment knobs); the first min(n, 21) resp.
- * min(n, 10) fields are written:
+/* host only, the plan mnb_pk_conv / mnb_pk_wgrad will run (same MNB_PK_* environment knobs); the first min(n, 31) resp.
+ * min(n, 16) fields are written.  Each query (and mnb_pk_conv_plan, mnb_pk_wimage_bytes, mnb_pk_wgrad_scratch_bytes)
+ * refuses exactly what its launch refuses on the host, with the same code and error text:
  *   mnb_pk_conv_plan_ex: the 16 fields of mnb_pk_conv_plan, then segmented, seg_len (stages per segment, 0 when not
- *                        segmented), npairs (piece products per K-step), col_tiles, n_mgroups
+ *                        segmented), npairs (piece products per K-step), col_tiles, n_mgroups, stage templates (tap groups)
+ *                        of output phases 0..3, filter taps of output phases 0..3, MMA program words, stages of the last
+ *                        accumulation segment of a phase-0 item (0 when not segmented)
  *   mnb_pk_wgrad_plan  : Nc, n_ctiles, tpg (taps per CTA), n_tg (tap groups), gm (merged groups), splits (batch splits),
- *                        NI (sub-blocks per stage), nstage, BW, TH */
+ *                        NI (sub-blocks per stage), nstage, BW, TH, n_ktiles, nkph_used (k-phase planes read),
+ *                        stg_per_split, nsub (row-tile sub-blocks), issue-program entries, nstg_total */
 int mnb_pk_conv_plan_ex(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out, int32_t n);
 int mnb_pk_wgrad_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n);
 int64_t mnb_pk_wimage_bytes(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w);

@@ -1551,6 +1551,8 @@ struct WgPlan {
   int64_t partial_floats;
 };
 
+constexpr int kWgProg4 = MAXPAIR * MAXTAP / 4 + MAXPAIR * 16;   // uint4 entries of the wgrad issue program (WgParams)
+
 static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, int nc_cap) {
   MNB_REQUIRE(s != nullptr, "conv shape is NULL");
   memset(&p, 0, sizeof(p));
@@ -1609,6 +1611,10 @@ static int make_wg_plan_nc(const mnb_conv_shape* s, int TA, int TX, WgPlan& p, i
   p.n_tg = ceil_div(p.ntap, p.tpg);
   p.tpg = ceil_div(p.ntap, p.n_tg);                        // balance the groups
   if (p.tpg * p.Nc > 128) return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: accumulators exceed the register budget");
+  // the issue program holds ceil(tpg / 4) groups of four x-offsets per (piece pair, tap group): many tap groups of a wide N
+  // tile (7x7 filters at Nc > 64: one tap per CTA) with several piece pairs overflow it; make_wg_plan then tries a narrower tile
+  if ((int64_t)p.npairs * p.n_tg * ceil_div(p.tpg, 4) > kWgProg4)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk wgrad: issue program too long (%d piece pairs x %d tap groups)", p.npairs, p.n_tg);
   // stage = NI sub-blocks (one image row-tile each): dy [TA][16 octets][rows_dy], x [TX][k-phase][Nc/8][rows_x].
   // Pick the raster (BW, TH) with the best useful fraction whose sub-block fits four times (else twice).
   auto sub_bytes_of = [&](int bw, int th) {
@@ -1681,7 +1687,7 @@ struct WgParams {
     uint32_t pair_a16[MAXPAIR], pair_b16[MAXPAIR];   // piece-plane offsets of the pairs (16-byte units)
     // per (piece pair, tap group, tap): x-operand offsets = pair plane + k-phase slot + tap row offset, in groups of four
     // (0xffffffff behind the last tap of a group)
-    alignas(16) uint4 progb4[MAXPAIR * MAXTAP / 4 + MAXPAIR * 16];
+    alignas(16) uint4 progb4[kWgProg4];
     uint32_t g4;                        // uint4 entries per (pair, tap group) = ceil(tpg / 4)
   } m;
   int G, n_ktiles, n_ctiles, n_tg, tpg, splits, stg_per_split, nstg_total, NI, nsub, row_tiles, TA, TX, nkph_used, kph_used[4];
@@ -2370,12 +2376,15 @@ static int quant_add_pack(const float* a, const float* b, int32_t batch, int32_t
   return 0;
 }
 
-// the first min(n, 21) fields of mnb_pk_conv_plan_ex / mnb_pk_i8_conv_plan
-static void plan_fields(const pk::Plan& p, int32_t* out, int32_t n) {
-  const int v[21] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
+// the first min(n, 31) fields of mnb_pk_conv_plan_ex / mnb_pk_i8_conv_plan (words: MMA program words of the plan)
+static void plan_fields(const pk::Plan& p, int words, int32_t* out, int32_t n) {
+  // stages of the last accumulation segment of an output-phase-0 item (segmented plans; 0 otherwise)
+  const int last_seg = p.segmented ? (p.ntmpl[0] * p.chunks - 1) % p.seg_len + 1 : 0;
+  const int v[31] = {(int)(p.wimg_bytes & 0x7fffffff), (int)(p.wimg_bytes >> 31), p.Nt, p.n_ntiles, p.MT, p.CC, p.chunks, p.nstage,
                      p.smem_bytes, p.MT * p.Nt, p.TH, p.TB, p.BW, p.n_mtiles, p.n_items, p.ny,
-                     p.segmented, p.segmented ? p.seg_len : 0, p.npairs, p.col_tiles, p.n_mgroups};
-  for (int i = 0; i < std::min(n, 21); ++i) out[i] = v[i];
+                     p.segmented, p.segmented ? p.seg_len : 0, p.npairs, p.col_tiles, p.n_mgroups,
+                     p.ntmpl[0], p.ntmpl[1], p.ntmpl[2], p.ntmpl[3], p.ntap[0], p.ntap[1], p.ntap[2], p.ntap[3], words, last_seg};
+  for (int i = 0; i < std::min(n, 31); ++i) out[i] = v[i];
 }
 
 extern "C" int64_t mnb_pk_act_bytes(int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t terms) {
@@ -2685,12 +2694,18 @@ extern "C" int mnb_bn_relu_pack_terms_fwd(const float* x, int32_t batch, int32_t
 
 // host only: out[0..15] = {wimg_bytes(lo), wimg_bytes(hi), Nt, n_ntiles, MT, CC, chunks, nstage, smem_bytes, accumulator
 //                          columns MT * Nt, TH, TB, BW, n_mtiles, n_items, ny},
-//            out[16..20] = {segmented, seg_len, npairs, col_tiles, n_mgroups}; the first min(n, 21) are written
+//            out[16..20] = {segmented, seg_len, npairs, col_tiles, n_mgroups},
+//            out[21..30] = {stage templates (tap groups) of output phases 0..3, filter taps of output phases 0..3, MMA program
+//                           words, stages of the last accumulation segment of a phase-0 item (0: not segmented)};
+//            the first min(n, 31) are written.  Refuses what mnb_pk_conv refuses on the host, with its code and error text.
+static int conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int cpu, pk::Plan& pl, int& words);
+
 extern "C" int mnb_pk_conv_plan_ex(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int32_t* out,
                                    int32_t n) {
   pk::Plan p;
-  if (int e = pk::make_plan(s, mode, terms_a, terms_w, p)) return e;
-  if (out) plan_fields(p, out, n);
+  int words = 0;
+  if (int e = conv_plan(s, mode, terms_a, terms_w, 8, p, words)) return e;
+  if (out) plan_fields(p, words, out, n);
   return 0;
 }
 
@@ -2698,9 +2713,11 @@ extern "C" int mnb_pk_conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t t
   return mnb_pk_conv_plan_ex(s, mode, terms_a, terms_w, out16, 16);
 }
 
+// -1 where mnb_pk_conv_plan_ex refuses
 extern "C" int64_t mnb_pk_wimage_bytes(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w) {
   pk::Plan p;
-  if (pk::make_plan(s, mode, terms_a, terms_w, p)) return -1;
+  int words = 0;
+  if (conv_plan(s, mode, terms_a, terms_w, 8, p, words)) return -1;
   return p.wimg_bytes;
 }
 
@@ -2776,6 +2793,54 @@ static int conv_route(const pk::Plan& pl, int32_t mode, const uint8_t* bits8, co
   return 0;
 }
 
+// The MMA warpgroups' parameter block of a plan, with its program: one word per (piece pair, tap, K-step) of every stage
+// template.  Host only: the launcher writes it into the kernel's parameters and the plan queries build it too, so that a
+// program that does not fit (length or 16-bit offsets) is refused by the query with the launch's code and error text.
+// words: program words used (each template padded to a group of four).
+static int conv_mma(const pk::Plan& pl, int cpu, pk::ConvParams::Mma& m, int& words) {
+  using namespace pk;
+  memset(&m, 0, sizeof(m));
+  m.n_items = pl.n_items; m.chunks = pl.chunks; m.ksteps = pl.ksteps; m.MT = pl.MT; m.Nt = pl.Nt; m.npairs = pl.npairs;
+  m.st_mask = pl.nstage - 1; m.st_log2 = pl.st_log2; m.stage16 = pl.stage_bytes >> 4;
+  m.a_term16 = pl.a_bytes >> 4; m.a_mt16 = (pl.TA * pl.a_bytes) >> 4; m.a_k16 = 2 * pl.npos;
+  m.b_off16 = pl.b_off >> 4; m.b_tap16 = (pl.CC / cpu) * pl.Nt; m.b_k16 = 2 * pl.Nt;
+  m.a_lbo = (uint32_t)pl.npos * 16u; m.b_lbo = (uint32_t)pl.Nt * 16u;
+  m.seg_len = (uint32_t)pl.seg_len;
+  int nprog = 0;
+  uint32_t* prog = reinterpret_cast<uint32_t*>(m.prog4);
+  for (int i = 0; i < MAXPROG; ++i) prog[i] = 0xffffffffu;    // padding words: no MMA
+  for (int y = 0; y < pl.ny; ++y) {
+    m.ntmpl[y] = pl.ntmpl[y];
+    for (int t = 0; t < pl.ntmpl[y]; ++t) {
+      const Tmpl& tp = pl.tmpl[y][t];
+      const int cnt = tp.ntap * pl.npairs * pl.ksteps;
+      nprog = (nprog + 3) & ~3;                       // every template starts on a group of four words
+      m.tmpl_begin[y][t] = (uint16_t)(nprog / 4); m.tmpl_cnt[y][t] = (uint16_t)((cnt + 3) / 4);
+      if (nprog + ((cnt + 3) & ~3) > MAXPROG) return unsupported("MMA program longer than 512 entries");
+      for (int pr = 0; pr < pl.npairs; ++pr)          // piece pairs outermost: small products first
+        for (int i = 0; i < tp.ntap; ++i)
+          for (int j = 0; j < pl.ksteps; ++j) {
+            const uint32_t a16 = (uint32_t)pl.tap_aoff[y][tp.tap0 + i] + (uint32_t)pl.pair_a[pr] * m.a_term16 + (uint32_t)j * m.a_k16;
+            const uint32_t b16 = (uint32_t)i * m.b_tap16 + (uint32_t)pl.pair_b[pr] * (uint32_t)tp.ntap * m.b_tap16 + (uint32_t)j * m.b_k16;
+            if (a16 > 0xffffu || b16 > 0xffffu) return mnb_fail(MNB_E_ARG, "pk conv: MMA program offset overflow");
+            prog[nprog++] = a16 | (b16 << 16);
+          }
+    }
+  }
+  words = (nprog + 3) & ~3;
+  return 0;
+}
+
+// The plan of a plain (no consumer) pk_conv_kernel launch and everything that launch refuses on the host: make_plan,
+// conv_route and the MMA program.  The plan queries and the weight-image size use it.  words: as conv_mma.
+static int conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int32_t terms_w, int cpu, pk::Plan& pl, int& words) {
+  if (int e = pk::make_plan(s, mode, terms_a, terms_w, pl, cpu)) return e;
+  int row = 0;
+  if (int e = conv_route(pl, mode, nullptr, nullptr, cpu, row)) return e;
+  pk::ConvParams::Mma m;   // the program itself is not kept (2.4 KB on the stack: queries may run on any host thread)
+  return conv_mma(pl, cpu, m, words);
+}
+
 static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
                         int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
                         const float* bias, const uint8_t* bits8, float gain, float* out, const mnb_pk_post* post,
@@ -2795,33 +2860,13 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
   const bool terms_out = row == 5;
   static ConvParams p;   // large POD: filled per call (single host thread per process)
   memset(&p, 0, sizeof(p));
-  ConvParams::Mma& m = p.m;
-  m.n_items = pl.n_items; m.chunks = pl.chunks; m.ksteps = pl.ksteps; m.MT = pl.MT; m.Nt = pl.Nt; m.npairs = pl.npairs;
-  m.st_mask = pl.nstage - 1; m.st_log2 = pl.st_log2; m.stage16 = pl.stage_bytes >> 4;
-  m.a_term16 = pl.a_bytes >> 4; m.a_mt16 = (pl.TA * pl.a_bytes) >> 4; m.a_k16 = 2 * pl.npos;
-  m.b_off16 = pl.b_off >> 4; m.b_tap16 = (pl.CC / cpu) * pl.Nt; m.b_k16 = 2 * pl.Nt;
-  m.a_lbo = (uint32_t)pl.npos * 16u; m.b_lbo = (uint32_t)pl.Nt * 16u;
-  m.seg_len = (uint32_t)pl.seg_len;
   int nprog = 0;
-  uint32_t* prog = reinterpret_cast<uint32_t*>(m.prog4);
-  for (int i = 0; i < MAXPROG; ++i) prog[i] = 0xffffffffu;    // padding words: no MMA
+  if (int e = conv_mma(pl, cpu, p.m, nprog)) return e;
   for (int y = 0; y < pl.ny; ++y) {
-    m.ntmpl[y] = pl.ntmpl[y]; p.ntmpl[y] = pl.ntmpl[y];
+    p.ntmpl[y] = pl.ntmpl[y];
     for (int t = 0; t < pl.ntmpl[y]; ++t) {
       const Tmpl& tp = pl.tmpl[y][t];
       p.tmpl_kph[y][t] = tp.kph; p.tmpl_blk_off[y][t] = tp.blk_off; p.tmpl_blk_bytes[y][t] = tp.blk_bytes;
-      const int cnt = tp.ntap * pl.npairs * pl.ksteps;
-      nprog = (nprog + 3) & ~3;                       // every template starts on a group of four words
-      m.tmpl_begin[y][t] = (uint16_t)(nprog / 4); m.tmpl_cnt[y][t] = (uint16_t)((cnt + 3) / 4);
-      if (nprog + ((cnt + 3) & ~3) > MAXPROG) return unsupported("MMA program longer than 512 entries");
-      for (int pr = 0; pr < pl.npairs; ++pr)          // piece pairs outermost: small products first
-        for (int i = 0; i < tp.ntap; ++i)
-          for (int j = 0; j < pl.ksteps; ++j) {
-            const uint32_t a16 = (uint32_t)pl.tap_aoff[y][tp.tap0 + i] + (uint32_t)pl.pair_a[pr] * m.a_term16 + (uint32_t)j * m.a_k16;
-            const uint32_t b16 = (uint32_t)i * m.b_tap16 + (uint32_t)pl.pair_b[pr] * (uint32_t)tp.ntap * m.b_tap16 + (uint32_t)j * m.b_k16;
-            if (a16 > 0xffffu || b16 > 0xffffu) return mnb_fail(MNB_E_ARG, "pk conv: MMA program offset overflow");
-            prog[nprog++] = a16 | (b16 << 16);
-          }
     }
     p.img_bytes[y] = pl.img_bytes[y]; p.y_off[y] = pl.y_off[y];
   }
@@ -2896,6 +2941,9 @@ extern "C" int mnb_pk_conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, i
   if (int e = pk::make_plan(s, 0, terms_a, terms_w, pl, cpu)) return e;
   int row = 0;
   if (int e = conv_route(pl, 0, nullptr, post, cpu, row)) return e;
+  pk::ConvParams::Mma m;   // (not kept: see conv_plan)
+  int words = 0;
+  if (int e = conv_mma(pl, cpu, m, words)) return e;
   if (out) {
     const int gx = std::max(1, std::min(pl.n_items, MNB_NUM_SMS / pl.ny));
     const int v[10] = {row, pl.Nt, pl.MT, pl.n_mtiles, pl.n_items, pl.ny, pl.col_tiles, pl.n_ntiles, gx, pl.segmented};
@@ -2941,16 +2989,19 @@ extern "C" int mnb_pk_i8_pack_act(const float* x, int32_t batch, int32_t channel
   return 0;
 }
 
+// host only: the fields of mnb_pk_conv_plan_ex for the int8 forward; refuses what mnb_pk_i8_conv refuses without a consumer
 extern "C" int mnb_pk_i8_conv_plan(const mnb_conv_shape* s, int32_t* out, int32_t n) {
   pk::Plan p;
-  if (int e = pk::make_plan(s, 0, 1, 1, p, 16)) return e;
-  if (out) plan_fields(p, out, n);
+  int words = 0;
+  if (int e = conv_plan(s, 0, 1, 1, 16, p, words)) return e;
+  if (out) plan_fields(p, words, out, n);
   return 0;
 }
 
 extern "C" int64_t mnb_pk_i8_wimage_bytes(const mnb_conv_shape* s) {
   pk::Plan p;
-  if (pk::make_plan(s, 0, 1, 1, p, 16)) return -1;
+  int words = 0;
+  if (conv_plan(s, 0, 1, 1, 16, p, words)) return -1;
   return p.wimg_bytes;
 }
 
@@ -2987,13 +3038,16 @@ extern "C" int64_t mnb_pk_wgrad_scratch_bytes(const mnb_conv_shape* s, int32_t t
   return p.partial_floats * 4;
 }
 
-// host only: out = {Nc, n_ctiles, tpg, n_tg, gm, splits, NI, nstage, BW, TH}; the first min(n, 10) are written
+// host only: out = {Nc, n_ctiles, tpg, n_tg, gm, splits, NI, nstage, BW, TH, n_ktiles, nkph_used, stg_per_split, nsub,
+//                   issue-program entries (uint4: piece pairs x tap groups x ceil(tpg / 4)), nstg_total};
+//            the first min(n, 16) are written.  Refuses what mnb_pk_wgrad refuses on the host, with its code and error text.
 extern "C" int mnb_pk_wgrad_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n) {
   pk::WgPlan p;
   if (int e = pk::make_wg_plan(s, terms_dy, terms_x, p)) return e;
   if (out) {
-    const int v[10] = {p.Nc, p.n_ctiles, p.tpg, p.n_tg, p.gm, p.splits, p.NI, p.nstage, p.BW, p.TH};
-    for (int i = 0; i < std::min(n, 10); ++i) out[i] = v[i];
+    const int v[16] = {p.Nc, p.n_ctiles, p.tpg, p.n_tg, p.gm, p.splits, p.NI, p.nstage, p.BW, p.TH, p.n_ktiles, p.nkph_used,
+                       p.stg_per_split, p.nsub, p.npairs * p.n_tg * ((p.tpg + 3) / 4), p.nstg_total};
+    for (int i = 0; i < std::min(n, 16); ++i) out[i] = v[i];
   }
   return 0;
 }
@@ -3017,8 +3071,7 @@ extern "C" int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t 
   m.dy_sbo = (uint32_t)pl.rows_dy * 16u; m.x_sbo = (uint32_t)pl.rows_x * 16u; m.nsub = pl.nsub;
   for (int i = 0; i < pl.npairs; ++i) { m.pair_a16[i] = pl.pair_a[i] * m.dy_term16; m.pair_b16[i] = pl.pair_b[i] * m.x_term16; }
   {
-    m.g4 = (uint32_t)ceil_div(pl.tpg, 4);
-    if ((size_t)pl.npairs * pl.n_tg * m.g4 > sizeof(m.progb4) / sizeof(uint4)) return unsupported("wgrad issue program too long");
+    m.g4 = (uint32_t)ceil_div(pl.tpg, 4);      // (make_wg_plan_nc refuses programs longer than progb4)
     uint32_t* prog = reinterpret_cast<uint32_t*>(m.progb4);
     for (size_t i = 0; i < sizeof(m.progb4) / 4; ++i) prog[i] = 0xffffffffu;
     for (int i = 0; i < pl.npairs; ++i)
