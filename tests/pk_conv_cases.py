@@ -10,7 +10,8 @@ Case fields:
   terms   (streamed operand, weight / x operand) pieces
   ops     "int": integer levels, one piece per operand (dgrad / wgrad: dy packed with the case's pieces, the later ones zero);
           "asym": streamed operand holds two-piece integer levels (|level| up to 383, as asymmetric IAO levels);
-          "f32": split fp32 streamed operand (and fp32 weights / x where that side has more than one piece);
+          "f32": split fp32 streamed operand (and fp32 weights / x where that side has more than one piece, integer levels
+                 where it has one);
           "pm1": +-1 streamed operand (one exact piece) against split fp32 weights
   epi     forward: n_scale (bool), a_scale ("dev" device scalar / "const"), bias (bool);
           dgrad: gain (STE mask with this gain) or None (no mask, a_scale_const = const);
@@ -19,15 +20,20 @@ Case fields:
   env     MNB_PK_* knobs set around the plan query and the launch
   bench   the bench launch the case stands for ("" for none)
   refuse  substring of the refusal text, for a case whose launch must be refused
+  maxnorm split fp32 cases: also |err| <= maxnorm * max |ref| (0: the element-wise bound alone)
 """
 from collections import namedtuple
 
-Case = namedtuple("Case", "id mode shape terms ops epi pin env bench refuse", defaults=({}, {}, {}, "", ""))
+Case = namedtuple("Case", "id mode shape terms ops epi pin env bench refuse maxnorm", defaults=({}, {}, {}, "", "", 0.0))
 
 E_FULL = dict(n_scale=True, a_scale="dev", bias=True)
 E_NONE = dict(n_scale=False, a_scale="const", bias=False)
 E_SCALE = dict(n_scale=True, a_scale="const", bias=False)
 E_BIAS = dict(n_scale=False, a_scale="dev", bias=True)
+D_STE = dict(gain=0.1)
+D_CONST = dict(gain=None, const=1.0)
+W_ALL = dict(a_scale=True, kdiv=True)
+W_NONE = dict(a_scale=False, kdiv=False)
 
 CASES = [
     # ---- plain bf16 forward (row 0): every N tile; R != S, pad_h != pad_w, kg % 16 != 0, ng % 16 != 0
@@ -114,6 +120,174 @@ CASES = [
     Case("wg_raster_pass2", "wgrad", (1, 32, 2, 126, 16, 3, 3, 1, 1, 1, 1), (2, 1), "int", dict(a_scale=True, kdiv=True), dict()),
     Case("wg_7x7_33_f32", "wgrad", (1, 96, 6, 2, 32, 7, 7, 1, 5, 5, 1), (3, 3), "f32", dict(a_scale=False, kdiv=False), dict(Nc=48)),
     Case("wg_22_f32", "wgrad", (2, 64, 8, 8, 64, 3, 3, 1, 1, 1, 1), (2, 2), "f32", dict(a_scale=False, kdiv=False), dict()),
+    # ---- plans the older packed-operand tests reached and the cases above do not: three-piece dy (the exact split), the
+    # bench models' multi-tile and phase-split plans, fp32 dy against integer weights with the STE mask; the fp32 backward
+    # with three dy pieces also keeps its max-norm bound
+    Case("pk_fwd11_3x64x32x32_64_3x3s1g1", "fwd", (3, 64, 32, 32, 64, 3, 3, 1, 1, 1, 1), (1, 1), "int", E_FULL,
+         dict(segmented=0, Nt=64, MT=1, ny=1)),
+    Case("pk_fwd33_2x3x32x32_64_3x3s1g1", "fwd", (2, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=0, Nt=64, MT=1, ny=1)),
+    Case("pk_fwd33_2x96x16x16_192_5x5s1g1", "fwd", (2, 96, 16, 16, 192, 5, 5, 1, 2, 2, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=1, Nt=96, MT=1, ny=1)),
+    Case("pk_fwd33_2x160x32x32_96_1x1s1g1", "fwd", (2, 160, 32, 32, 96, 1, 1, 1, 0, 0, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=0, Nt=96, MT=1, ny=1)),
+    Case("pk_fwd33_2x192x8x8_10_1x1s1g1", "fwd", (2, 192, 8, 8, 10, 1, 1, 1, 0, 0, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=1, Nt=16, MT=1, ny=1)),
+    Case("pk_fwd33_2x256x16x16_512_3x3s1g16", "fwd", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (3, 3), "f32", E_FULL,
+         dict(segmented=0, Nt=32, MT=1, ny=1)),
+    Case("pk_fwd33_2x32x9x9_48_3x3s1g1", "fwd", (2, 32, 9, 9, 48, 3, 3, 1, 0, 0, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=1, Nt=48, MT=1, ny=1)),
+    Case("gc3x3g32_fwd", "fwd", (8, 512, 8, 8, 1024, 3, 3, 1, 1, 1, 32), (1, 1), "int", E_FULL,
+         dict(segmented=0, Nt=32, MT=2, ny=1)),
+    Case("mt4_partial_seg", "fwd", (3, 64, 32, 32, 32, 3, 3, 1, 1, 1, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=1, Nt=32, MT=4, ny=1, n_mtiles=33, n_mgroups=9), {"MNB_PK_MT": "4"}),
+    Case("mt2_partial_seg48", "fwd", (3, 64, 32, 32, 48, 3, 3, 1, 1, 1, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=1, Nt=48, MT=2, ny=1, n_mtiles=33, n_mgroups=17), {"MNB_PK_MT": "2"}),
+    Case("seg32_fwd", "fwd", (2, 64, 16, 16, 32, 3, 3, 1, 1, 1, 1), (3, 3), "f32", E_FULL,
+         dict(segmented=1, Nt=32, MT=1, ny=1)),
+    Case("pk_dgrad31_3x64x32x32_64_3x3s1g1", "dgrad", (3, 64, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=64, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad21_3x64x32x32_128_3x3s2g1", "dgrad", (3, 64, 32, 32, 128, 3, 3, 2, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=64, MT=1, ny=4)),
+    Case("pk_dgrad31_3x64x32x32_128_3x3s2g1", "dgrad", (3, 64, 32, 32, 128, 3, 3, 2, 1, 1, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=64, MT=1, ny=4), maxnorm=3e-06),
+    Case("pk_dgrad31_3x64x32x32_128_1x1s2g1", "dgrad", (3, 64, 32, 32, 128, 1, 1, 2, 0, 0, 1), (3, 1), "f32", D_STE,
+         dict(segmented=0, Nt=64, MT=1, ny=4), maxnorm=3e-06),
+    Case("pk_dgrad31_5x128x16x16_128_3x3s1g1", "dgrad", (5, 128, 16, 16, 128, 3, 3, 1, 1, 1, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=128, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad31_4x256x8x8_512_3x3s2g1", "dgrad", (4, 256, 8, 8, 512, 3, 3, 2, 1, 1, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=128, MT=1, ny=4), maxnorm=3e-06),
+    Case("pk_dgrad31_2x3x32x32_64_3x3s1g1", "dgrad", (2, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=16, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad31_2x96x16x16_192_5x5s1g1", "dgrad", (2, 96, 16, 16, 192, 5, 5, 1, 2, 2, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=96, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad31_2x192x32x32_160_1x1s1g1", "dgrad", (2, 192, 32, 32, 160, 1, 1, 1, 0, 0, 1), (3, 1), "f32", D_STE,
+         dict(segmented=0, Nt=96, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad31_2x256x16x16_512_3x3s1g16", "dgrad", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (3, 1), "f32", D_STE,
+         dict(segmented=0, Nt=16, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad31_2x256x32x32_256_1x1s1g2", "dgrad", (2, 256, 32, 32, 256, 1, 1, 1, 0, 0, 2), (3, 1), "f32", D_STE,
+         dict(segmented=0, Nt=128, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad21_1x3x64x64_16_7x7s2g1", "dgrad", (1, 3, 64, 64, 16, 7, 7, 2, 3, 3, 1), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=16, MT=1, ny=4)),
+    Case("pk_dgrad31_1x3x64x64_16_7x7s2g1", "dgrad", (1, 3, 64, 64, 16, 7, 7, 2, 3, 3, 1), (3, 1), "f32", D_STE,
+         dict(segmented=0, Nt=16, MT=1, ny=4), maxnorm=3e-06),
+    Case("pk_dgrad31_2x32x9x9_48_3x3s1g1", "dgrad", (2, 32, 9, 9, 48, 3, 3, 1, 0, 0, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=32, MT=1, ny=1), maxnorm=3e-06),
+    Case("pk_dgrad31_2x48x16x16_64_3x3s1g1", "dgrad", (2, 48, 16, 16, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", D_STE,
+         dict(segmented=1, Nt=48, MT=1, ny=1), maxnorm=3e-06),
+    Case("gc3x3g16_dgrad21_ste", "dgrad", (32, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=16, MT=4, ny=1)),
+    Case("gc3x3g32_dgrad21_ste", "dgrad", (8, 512, 8, 8, 1024, 3, 3, 1, 1, 1, 32), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=16, MT=2, ny=1)),
+    Case("stem_dgrad21", "dgrad", (64, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_CONST,
+         dict(segmented=1, Nt=16, MT=2, ny=1)),
+    Case("mt2_dgrad21_ste", "dgrad", (3, 64, 28, 28, 48, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=64, MT=2, ny=1, n_mtiles=21, n_mgroups=11), {"MNB_PK_MT": "2"}),
+    Case("i8_stem_224", "i8", (1, 3, 224, 224, 64, 3, 3, 1, 1, 1, 1), (1, 1), "int", E_FULL, dict(Nt=64, MT=2)),
+    Case("i8_sc_1x1_s2", "i8", (4, 64, 16, 16, 128, 1, 1, 2, 0, 0, 1), (1, 1), "int", E_FULL, dict(Nt=128, MT=1)),
+    Case("i8_nt48_s1", "i8", (4, 48, 16, 16, 48, 3, 3, 1, 1, 1, 1), (1, 1), "int", E_FULL, dict(Nt=48, MT=1)),
+    Case("i8_mt4_nt32", "i8", (8, 64, 16, 16, 32, 3, 3, 1, 1, 1, 1), (1, 1), "int", E_FULL,
+         dict(Nt=32, MT=4), {"MNB_PK_MT": "4"}),
+    Case("pk_wgrad31_3x64x32x32_64_3x3s1g1", "wgrad", (3, 64, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=64, tpg=2, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_3x64x32x32_64_3x3s1g1", "wgrad", (3, 64, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=64, tpg=2, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_3x64x32x32_128_3x3s2g1", "wgrad", (3, 64, 32, 32, 128, 3, 3, 2, 1, 1, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=32, tpg=3, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad31_3x64x32x32_128_1x1s2g1", "wgrad", (3, 64, 32, 32, 128, 1, 1, 2, 0, 0, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=64, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_3x64x32x32_128_1x1s2g1", "wgrad", (3, 64, 32, 32, 128, 1, 1, 2, 0, 0, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=64, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad31_5x128x16x16_128_3x3s1g1", "wgrad", (5, 128, 16, 16, 128, 3, 3, 1, 1, 1, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=128, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_5x128x16x16_128_3x3s1g1", "wgrad", (5, 128, 16, 16, 128, 3, 3, 1, 1, 1, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=128, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad22_2x3x32x32_64_3x3s1g1", "wgrad", (2, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (2, 2), "f32", W_NONE,
+         dict(Nc=16, tpg=5, gm=1)),
+    Case("pk_wgrad31_2x3x32x32_64_3x3s1g1", "wgrad", (2, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=16, tpg=5, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_2x3x32x32_64_3x3s1g1", "wgrad", (2, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=16, tpg=5, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad22_2x96x16x16_192_5x5s1g1", "wgrad", (2, 96, 16, 16, 192, 5, 5, 1, 2, 2, 1), (2, 2), "f32", W_NONE,
+         dict(Nc=96, tpg=1, gm=1)),
+    Case("pk_wgrad31_2x96x16x16_192_5x5s1g1", "wgrad", (2, 96, 16, 16, 192, 5, 5, 1, 2, 2, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=96, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_2x192x8x8_192_3x3s1g1", "wgrad", (2, 192, 8, 8, 192, 3, 3, 1, 1, 1, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=96, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad22_2x160x32x32_96_1x1s1g1", "wgrad", (2, 160, 32, 32, 96, 1, 1, 1, 0, 0, 1), (2, 2), "f32", W_NONE,
+         dict(Nc=80, tpg=1, gm=1)),
+    Case("pk_wgrad31_2x160x32x32_96_1x1s1g1", "wgrad", (2, 160, 32, 32, 96, 1, 1, 1, 0, 0, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=80, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_2x160x32x32_96_1x1s1g1", "wgrad", (2, 160, 32, 32, 96, 1, 1, 1, 0, 0, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=80, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad22_2x256x16x16_512_3x3s1g16", "wgrad", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (2, 2), "f32", W_NONE,
+         dict(Nc=64, tpg=2, gm=4)),
+    Case("pk_wgrad31_2x256x16x16_512_3x3s1g16", "wgrad", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (3, 1), "f32", W_ALL,
+         dict(Nc=64, tpg=2, gm=4), maxnorm=3e-06),
+    Case("pk_wgrad33_2x256x16x16_512_3x3s1g16", "wgrad", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (3, 3), "f32", W_NONE,
+         dict(Nc=64, tpg=2, gm=4), maxnorm=3e-06),
+    Case("pk_wgrad22_2x32x9x9_48_3x3s1g1", "wgrad", (2, 32, 9, 9, 48, 3, 3, 1, 0, 0, 1), (2, 2), "f32", W_NONE,
+         dict(Nc=32, tpg=3, gm=1)),
+    Case("pk_wgrad31_2x32x9x9_48_3x3s1g1", "wgrad", (2, 32, 9, 9, 48, 3, 3, 1, 0, 0, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=32, tpg=3, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad22_2x48x16x16_64_3x3s1g1", "wgrad", (2, 48, 16, 16, 64, 3, 3, 1, 1, 1, 1), (2, 2), "f32", W_NONE,
+         dict(Nc=48, tpg=2, gm=1)),
+    Case("pk_wgrad31_2x48x16x16_64_3x3s1g1", "wgrad", (2, 48, 16, 16, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=48, tpg=2, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad22_2x112x16x16_64_3x3s1g1", "wgrad", (2, 112, 16, 16, 64, 3, 3, 1, 1, 1, 1), (2, 2), "f32", W_NONE,
+         dict(Nc=112, tpg=1, gm=1)),
+    Case("pk_wgrad31_2x112x16x16_64_3x3s1g1", "wgrad", (2, 112, 16, 16, 64, 3, 3, 1, 1, 1, 1), (3, 1), "f32", W_ALL,
+         dict(Nc=112, tpg=1, gm=1), maxnorm=3e-06),
+    Case("pk_wgrad33_2x112x16x16_64_3x3s1g1", "wgrad", (2, 112, 16, 16, 64, 3, 3, 1, 1, 1, 1), (3, 3), "f32", W_NONE,
+         dict(Nc=112, tpg=1, gm=1), maxnorm=3e-06),
+    Case("wg_chain16", "wgrad", (8, 64, 16, 16, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=64, splits=32), {"MNB_PK_WG_CHAIN": "16"}),
+    Case("wg_merge0", "wgrad", (4, 256, 8, 8, 512, 3, 3, 1, 1, 1, 16), (2, 1), "f32", W_ALL,
+         dict(Nc=16, gm=1), {"MNB_PK_WG_MERGE": "0"}),
+    Case("wg_nc48_forced", "wgrad", (2, 96, 16, 16, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=48, n_ctiles=2), {"MNB_PK_WG_NC": "48"}),
+    # ---- fp32 dy (two nonzero pieces) at the (2, 1) plans the older tests ran so and the integer cases above reach with
+    # the second dy piece zero
+    Case("res64_dgrad21", "dgrad", (64, 64, 32, 32, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_CONST,
+         dict(segmented=1, Nt=64, MT=2, ny=1)),
+    Case("res128s2_dgrad21_ste", "dgrad", (64, 64, 32, 32, 128, 3, 3, 2, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=64, MT=2, ny=4)),
+    Case("res256s2_dgrad21", "dgrad", (16, 128, 16, 16, 256, 3, 3, 2, 1, 1, 1), (2, 1), "f32", D_CONST,
+         dict(segmented=1, Nt=128, MT=1, ny=4)),
+    Case("res256sc_dgrad21_ste", "dgrad", (16, 128, 16, 16, 256, 1, 1, 2, 0, 0, 1), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=128, MT=1, ny=4)),
+    Case("coltiles2_dgrad21", "dgrad", (2, 32, 16, 16, 48, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_CONST,
+         dict(segmented=0, Nt=32, MT=1, ny=1, col_tiles=2), {"MNB_PK_COLTILES": "2"}),
+    Case("pk_dgrad21_f32_3x64x32x32_64_3x3s1g1", "dgrad", (3, 64, 32, 32, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=1, Nt=64, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_5x128x16x16_128_3x3s1g1", "dgrad", (5, 128, 16, 16, 128, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=1, Nt=128, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_2x3x32x32_64_3x3s1g1", "dgrad", (2, 3, 32, 32, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=1, Nt=16, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_2x96x16x16_192_5x5s1g1", "dgrad", (2, 96, 16, 16, 192, 5, 5, 1, 2, 2, 1), (2, 1), "f32", D_STE,
+         dict(segmented=1, Nt=96, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_2x192x32x32_160_1x1s1g1", "dgrad", (2, 192, 32, 32, 160, 1, 1, 1, 0, 0, 1), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=96, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_2x256x16x16_512_3x3s1g16", "dgrad", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=16, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_2x256x32x32_256_1x1s1g2", "dgrad", (2, 256, 32, 32, 256, 1, 1, 1, 0, 0, 2), (2, 1), "f32", D_STE,
+         dict(segmented=0, Nt=128, MT=1, ny=1)),
+    Case("pk_dgrad21_f32_2x48x16x16_64_3x3s1g1", "dgrad", (2, 48, 16, 16, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", D_STE,
+         dict(segmented=1, Nt=48, MT=1, ny=1)),
+    Case("wg_nc112_f32", "wgrad", (2, 112, 16, 16, 64, 3, 3, 1, 1, 1, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=112, tpg=1, gm=1)),
+    Case("pk_wgrad21_f32_3x64x32x32_128_1x1s2g1", "wgrad", (3, 64, 32, 32, 128, 1, 1, 2, 0, 0, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=64, tpg=1, gm=1)),
+    Case("pk_wgrad21_f32_5x128x16x16_128_3x3s1g1", "wgrad", (5, 128, 16, 16, 128, 3, 3, 1, 1, 1, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=128, tpg=1, gm=1)),
+    Case("pk_wgrad21_f32_2x96x16x16_192_5x5s1g1", "wgrad", (2, 96, 16, 16, 192, 5, 5, 1, 2, 2, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=96, tpg=1, gm=1)),
+    Case("pk_wgrad21_f32_2x160x32x32_96_1x1s1g1", "wgrad", (2, 160, 32, 32, 96, 1, 1, 1, 0, 0, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=80, tpg=1, gm=1)),
+    Case("pk_wgrad21_f32_2x256x16x16_512_3x3s1g16", "wgrad", (2, 256, 16, 16, 512, 3, 3, 1, 1, 1, 16), (2, 1), "f32", W_ALL,
+         dict(Nc=64, tpg=2, gm=4)),
+    Case("pk_wgrad21_f32_2x32x9x9_48_3x3s1g1", "wgrad", (2, 32, 9, 9, 48, 3, 3, 1, 0, 0, 1), (2, 1), "f32", W_ALL,
+         dict(Nc=32, tpg=3, gm=1)),
     # ---- refusals (launch refuses with the query's code and text, writes nothing)
     Case("no_fwd_dilation", "fwd", (1, 16, 8, 8, 16, 3, 3, 1, 1, 1, 1, 2), (1, 1), "int", E_FULL, refuse="dilation != 1"),
     Case("no_fwd_stride3", "fwd", (1, 16, 9, 9, 16, 3, 3, 3, 1, 1, 1), (1, 1), "int", E_FULL, refuse="stride must be 1 or 2"),

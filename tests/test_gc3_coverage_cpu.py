@@ -22,30 +22,10 @@ import types
 import pytest
 
 from tests import gc3_cases as P
+from tests import pk_plan_util as PU
 
 CODES = {"E_ARG": -1, "E_UNSUPPORTED": -2}
 SRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "micronet_b200", "csrc", "mnb_pk.cu")
-
-
-class _env:
-    def __init__(self, env):
-        self.env, self.old = env, {}
-
-    def __enter__(self):
-        from micronet_b200 import pk as PK
-        for k, v in self.env.items():
-            self.old[k] = os.environ.get(k)
-            os.environ[k] = v
-        PK._plan_cache.clear()        # keyed by shape only
-
-    def __exit__(self, *exc):
-        from micronet_b200 import pk as PK
-        for k, v in self.old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-        PK._plan_cache.clear()
 
 
 @pytest.fixture(scope="module")
@@ -192,7 +172,7 @@ def test_every_refusal_reason_is_listed_and_agrees_with_the_query():
     from micronet_b200 import _lib as L
     bad = {}
     for r in P.REFUSALS:
-        with _env(r.env):
+        with PU.env(r.env):
             got = P.query(P.refusal_shape(r), r.mode, r.terms)
         if r.launch:
             # the plan accepts; the launcher refuses (alignment, the codes bound)
@@ -256,10 +236,9 @@ def _bench_launches():
     """(workload, layer, mode, shape, pieces) of every gc3 launch of a bench step at batch 256: the forward and the data
     gradient of the grouped 3x3 layers, at the piece counts the engine gives them"""
     from micronet_b200 import _lib as L, functional as F_
-    from tests.test_pk_plan_cpu import _model_convs
     Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
     out = []
-    for name, B, Cc, H, W, K, R, st, pad, G in _model_convs():
+    for name, B, Cc, H, W, K, R, st, pad, G in PU.model_convs():
         if not name.startswith("gc") or R != 3:
             continue
         shape = (B, Cc, H, W, K, pad, pad, G)
@@ -315,9 +294,8 @@ def test_make_plan_knobs_keep_the_chain_of_mnb_pk_conv(env):
     mnb_pk_conv_plan_ex's plan (chunks, K-steps, piece pairs); the weight image is packed by that plan, so this is the one
     way the image could disagree with the kernel's program"""
     from micronet_b200 import pk as PK
-    from tests import pk_plan_util as PU
     seen = 0
-    with _env(env):
+    with PU.env(env):
         for c in P.CASES:
             if not c.model:
                 continue

@@ -8,7 +8,7 @@ with bitwise-identical results, and the tensor-core error flag must stay clean.
 
 * Forward on integer levels (+-1 x ternary, DoReFa 4-bit, int8 range): the exact sum S (fp64, exact below 2^24).  codes
   = S; the decode pair = (fl(a_scale * n_scale[k]), bias[k]) bit for bit; the fp32 output = fmaf(S, fl(a_scale * n_scale[k]),
-  bias[k]) bit for bit (fmaf emulated in fp64, double-rounding midpoints redone with Fraction).
+  bias[k]) bit for bit (fmaf emulated in fp64, double-rounding midpoints settled by the TwoSum error).
 * Data gradient on integer dy (|dy| <= 255 is bf16-exact, so the second piece is 0): exact, so dx = fl(S * a_scale_const)
   or, under the STE mask, fl(S * gain), masked-out positions +0.0, bit for bit.
 * Data gradient on real dy (two pieces, w_scale folded into dy, kzero channels): element-wise within 2^-15 R, R the same
@@ -22,7 +22,7 @@ import torch
 import torch.nn.functional as TF
 
 from tests import gc3_cases as P
-from tests.test_gpu_pk_post import fma32
+from tests.pk_plan_util import fmaf32
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -148,13 +148,13 @@ def test_forward_matches_the_exact_sum(case):
                                         a_const, L.ptr(bias), None, 1.0, out.data_ptr(), err, L.stream()),
             [(out, out_buf, float("nan"), F_SENT, n)], case.id)
         stats = {}
-        want = fma32(S.float(), scv.view(1, -1, 1, 1), bsv.view(1, -1, 1, 1), stats)
+        want = fmaf32(S.float(), scv.view(1, -1, 1, 1), bsv.view(1, -1, 1, 1), stats)
         got = got.view(B, K, OH, OW)
         assert not torch.isnan(got).any(), f"{case.id}: output elements never written"
         bad = (_bits(got) != _bits(want)).sum().item()
         assert bad == 0, f"{case.id}: {bad} of {n} outputs differ from fmaf(S, fl(a_scale * n_scale), bias)"
         got_dec = None          # (the decode pair belongs to the codes entry point)
-        print(f"{case.id}: fma midpoints redone exactly: {stats.get('midpoints', 0)}")
+        print(f"{case.id}: fma midpoints settled: {stats.get('midpoints', 0)}")
     if got_dec is not None:
         want_dec = torch.cat([scv, bsv])
         assert torch.equal(_bits(got_dec), _bits(want_dec)), \

@@ -8,6 +8,7 @@ convolutions of the same operands (computed on the GPU in float64).
   that kg x taps x |a| x |w| < 2^24; two-piece asymmetric levels up to 383 on the segmented plans), so the conv sum S is
   the fp64 one and the epilogue is checked bit for bit:
     forward / int8      y  = fmaf(S, sc, bias),   sc = fl(a_scale * n_scale[k]) (or a_scale alone), bias 0 when absent;
+                        the int8 result also equals mnb_pk_conv's on the same levels bit for bit;
     data gradient       dx = fl(S * gain) where the STE mask passes, +0.0 where it does not; without a mask
                         fmaf(S, a_scale_const, 0);
     weight gradient     dw = fl(S * fl(a_scale / kdiv[k])), fl(S * a_scale), fl(S * fl(1 / kdiv[k])) or S.
@@ -20,9 +21,12 @@ convolutions of the same operands (computed on the GPU in float64).
       c = 2^-20.  A dropped kept product or a lost segment is caught when its magnitude exceeds 2^-20 R: every product of
       the leading pieces, the second-piece products of (3, 1) / (3, 3) on these operands, and any lost segment of the
       plans here; the smallest kept products (2^-16 of the operand magnitudes, times a sum of mixed signs) can be smaller.
-    data gradient (2, 2), weight gradient (2, 2), (3, 3): dy keeps two pieces (2^-16 relative truncation of dy), the
-      weight / x side two pieces as well, and wgrad chains reach 256 MMAs before their RN split adds: c = 2^-14.
-  The worst err / R of every configuration is printed.
+      Each is also held to max |err| <= 3e-6 max |ref|, which R does not imply under cancellation.
+    data gradient: dy keeps two pieces (2^-16 relative truncation of dy) over chains of <= 64 MMAs: c = 2^-15.
+    weight gradient: dy keeps two pieces, and the chains reach 256 MMAs before their RN split adds: c = 2^-14.
+  A case with ``maxnorm`` is held to max |err| <= maxnorm * max |ref| as well.  With an fp32 dy against integer weights
+  the weights' per-channel scale is folded into dy (one channel's scale 0), as the models' data gradient does.  The worst
+  err / R of every configuration is printed.
 * Refusal cases return the query's code and text, launch nothing, and leave outputs and guards untouched."""
 import ctypes as C
 
@@ -31,36 +35,18 @@ import torch
 import torch.nn.functional as TF
 
 from tests import pk_conv_cases as PC
-from tests.test_pk_conv_coverage_cpu import _env, query, shape
+from tests.pk_plan_util import case_shape as shape, env, fmaf32, query
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 GUARD = 64
-C_FWD, C_BWD = 2.0 ** -20, 2.0 ** -14
+C_FWD, C_DGRAD, C_WGRAD = 2.0 ** -20, 2.0 ** -15, 2.0 ** -14
+MAX_FWD = 3e-6
 WORST = {}
 
 
 def _nan(n):
     return torch.full((n + GUARD,), float("nan"), dtype=torch.float32, device=DEV)
-
-
-def _fmaf(a, b, c):
-    """fp32 fmaf(a, b, c) of float32 device tensors, correctly rounded: t = a * b is exact in fp64, s = fl64(t + c) with its
-    exact error e (TwoSum), and s rounded to fp32 - wrong only where s lies on an fp32 midpoint and e != 0, where the
-    neighbour on e's side is the answer"""
-    t = a.double() * b.double()                # exact: 24 x 24 significant bits
-    c = c.double()
-    s = t + c
-    bb = s - t
-    e = (t - (s - bb)) + (c - bb)
-    r = s.float()
-    r64 = r.double()
-    toward = torch.where(s > r64, torch.full_like(r, float("inf")), torch.full_like(r, float("-inf")))
-    nb = torch.nextafter(r, toward)
-    mid = (s != r64) & ((s - r64).abs() * 2 == (nb.double() - r64).abs())
-    # at a midpoint RN picked r (ties to even) from s alone; the exact value s + e lies on nb's side iff e points away from r
-    up = mid & (e != 0) & ((e > 0) == (nb.double() > r64))
-    return torch.where(up, nb, r)
 
 
 def _rand_int(shape, bound, g):
@@ -121,13 +107,19 @@ def _bits_equal(got, want, what):
                              f"want {want.reshape(-1)[i].tolist()}")
 
 
-def _bound(got, ref, R, c, key):
+def _bound(got, ref, R, c, key, maxnorm=0.0):
+    """|got - ref| <= c * R element-wise and, where maxnorm is given, max |got - ref| <= maxnorm * max |ref|"""
     err = (got.double() - ref).abs()
     ratio = float((err / R.clamp_min(1e-30)).max())
     WORST[key] = max(WORST.get(key, 0.0), ratio)
     print(f"worst err/R {key}: {WORST[key]:.3e}")
     assert torch.isfinite(got).all()
     assert bool((err <= c * R).all()), f"{key}: err/R {ratio:.3e} > {c:.3e}"
+    if maxnorm:
+        rel = float(err.max()) / float(ref.abs().max())
+        WORST[key + " max-norm"] = max(WORST.get(key + " max-norm", 0.0), rel)
+        print(f"worst max|err|/max|ref| {key}: {WORST[key + ' max-norm']:.3e}")
+        assert rel <= maxnorm, f"{key}: max|err| / max|ref| {rel:.3e} > {maxnorm:.1e}"
 
 
 def _iao_spec(scale=1.0, bits=8):
@@ -164,12 +156,20 @@ def _fwd(case, g):
         a_pk = PK.pack_act_i8(x, _iao_spec().struct(), phase_split=st == 2)
         w_img = PK.pack_weight_i8(sh, w_int.to(torch.int16))
         fn = lambda: PK.conv_i8(sh, a_pk, w_img, out, n_scale=n_scale, a_scale=a_dev, a_scale_const=a_const, bias=bias)
+        # the bf16 kernel on the same levels, which the int8 result must equal bit for bit
+        b_pk, _ = PK.pack_act(x, None, 1, phase_split=st == 2)
+        b_img = PK.pack_weight(sh, 0, 1, 1, w_int=w_int.to(torch.int16))
+        b_out = _nan(n)
+        fn_bf16 = lambda: PK.conv(sh, 0, b_pk, 1, b_img, 1, b_out, n_scale=n_scale, a_scale=a_dev, a_scale_const=a_const,
+                                  bias=bias)
     else:
         a_pk, _ = PK.pack_act(x, None, ta, phase_split=st == 2, groups=G)
         w_img = PK.pack_weight(sh, 0, ta, tw, w_f32=w_f32) if w_f32 is not None else \
             PK.pack_weight(sh, 0, ta, tw, w_int=w_int.to(torch.int16))
         fn = lambda: PK.conv(sh, 0, a_pk, ta, w_img, tw, out, n_scale=n_scale, a_scale=a_dev, a_scale_const=a_const, bias=bias)
     got = _launch_twice(fn, out, n).view(B, K, P, Q)
+    if case.mode == "i8":
+        _bits_equal(got, _launch_twice(fn_bf16, b_out, n).view(B, K, P, Q), f"{case.id}: int8 against bf16")
     w = w_f32 if w_f32 is not None else w_int
     Ssum = _ref_conv(x, w, case)
     a = torch.tensor(0.37 if a_dev is not None else a_const, dtype=torch.float32, device=DEV)
@@ -179,11 +179,11 @@ def _fwd(case, g):
     if case.ops in ("f32", "pm1"):
         ref = Ssum * sc4.double() + bs4.double()
         Rm = _ref_conv(x.abs(), w.abs(), case) * sc4.double().abs() + bs4.double().abs()
-        _bound(got, ref, Rm, C_FWD, f"fwd {case.terms}")
+        _bound(got, ref, Rm, C_FWD, f"fwd {case.terms}", MAX_FWD)
     else:
         assert float(Ssum.abs().max()) < 2 ** 24
         S32 = Ssum.float()
-        _bits_equal(got, _fmaf(S32, sc4.expand_as(S32), bs4.expand_as(S32)), case.id)
+        _bits_equal(got, fmaf32(S32, sc4.expand_as(S32), bs4.expand_as(S32)), case.id)
 
 
 def _dgrad(case, g):
@@ -195,31 +195,47 @@ def _dgrad(case, g):
     f32 = case.ops == "f32"
     db, wb = _bounds(K // G, R * S, 8, 7)
     dy = torch.randn(B, K, P, Q, generator=g, device=DEV) if f32 else _rand_int((B, K, P, Q), db, g)
-    w = torch.randn(K, Cc // G, R, S, generator=g, device=DEV) if f32 else _rand_int((K, Cc // G, R, S), wb, g)
+    w_scale = None
+    if f32 and tw > 1:
+        w = torch.randn(K, Cc // G, R, S, generator=g, device=DEV)
+        w_img = PK.pack_weight(sh, 1, ta, tw, w_f32=w)
+    else:
+        w = _rand_int((K, Cc // G, R, S), 127 if f32 else wb, g)
+        if f32:     # integer weight levels with their per-channel scale folded into dy, one channel's scale 0 (kzero)
+            w_scale = torch.rand(K, generator=g, device=DEV) * 0.02 + 0.001
+            w_scale[0] = 0.0
+        w_img = PK.pack_weight(sh, 1, ta, tw, w_int=w.to(torch.int16), kzero=w_scale)
+    dy_pk, _ = PK.pack_act(dy, None, ta, ch_scale=w_scale, groups=G)
+    if w_scale is not None:
+        dy = dy * w_scale.view(1, -1, 1, 1)      # the fp32 product is the operand the kernel splits
     gain, const = case.epi["gain"], case.epi.get("const", 1.0)
     c8o = G * (-(-(Cc // G) // 8))
     bits = torch.randint(0, 256, (B, c8o, H, W), generator=g, device=DEV, dtype=torch.uint8) if gain is not None else None
     n = B * Cc * H * W
     out = _nan(n)
-    dy_pk, _ = PK.pack_act(dy, None, ta, groups=G)
-    w_img = PK.pack_weight(sh, 1, ta, tw, w_f32=w) if tw > 1 else PK.pack_weight(sh, 1, ta, tw, w_int=w.to(torch.int16))
     fn = lambda: PK.conv(sh, 1, dy_pk, ta, w_img, tw, out, bits8=bits, gain=gain if gain is not None else 1.0,
                          a_scale_const=const)
     got = _launch_twice(fn, out, n).view(B, Cc, H, W)
     Ssum = _ref_dgrad(dy, w, case)
-    if f32:
-        _bound(got, Ssum * const, _ref_dgrad(dy.abs(), w.abs(), case) * abs(const), C_BWD, f"dgrad {case.terms}")
-        return
-    assert float(Ssum.abs().max()) < 2 ** 24
-    S32 = Ssum.float()
-    if bits is None:
-        want = _fmaf(S32, torch.full_like(S32, const), torch.zeros_like(S32))
-    else:
+    mask = None
+    if bits is not None:
         cg = Cc // G
         ch = torch.arange(Cc, device=DEV)
         octet = (ch // cg) * (-(-cg // 8)) + (ch % cg) // 8
         bitno = ((ch % cg) % 8).view(1, Cc, 1, 1)
         mask = ((bits.index_select(1, octet).int() >> bitno) & 1).bool()
+    if f32:
+        mul = gain if mask is not None else const
+        ref, Rm = Ssum * mul, _ref_dgrad(dy.abs(), w.abs(), case) * abs(mul)
+        if mask is not None:
+            ref, Rm = torch.where(mask, ref, torch.zeros_like(ref)), torch.where(mask, Rm, torch.zeros_like(Rm))
+        _bound(got, ref, Rm, C_DGRAD, f"dgrad {case.terms}", case.maxnorm)
+        return
+    assert float(Ssum.abs().max()) < 2 ** 24
+    S32 = Ssum.float()
+    if mask is None:
+        want = fmaf32(S32, torch.full_like(S32, const), torch.zeros_like(S32))
+    else:
         want = torch.where(mask, S32 * torch.tensor(gain, dtype=torch.float32, device=DEV), torch.zeros_like(S32))
     _bits_equal(got, want, case.id)
 
@@ -233,7 +249,7 @@ def _wgrad(case, g):
     f32 = case.ops == "f32"
     db, xb = _bounds(B * P * Q, 1, 8, 8)
     dy = torch.randn(B, K, P, Q, generator=g, device=DEV) if f32 else _rand_int((B, K, P, Q), db, g)
-    x = torch.randn(B, Cc, H, W, generator=g, device=DEV) if f32 else _rand_int((B, Cc, H, W), xb, g)
+    x = torch.randn(B, Cc, H, W, generator=g, device=DEV) if f32 and tx > 1 else _rand_int((B, Cc, H, W), 127 if f32 else xb, g)
     a = torch.tensor([0.37], device=DEV) if case.epi["a_scale"] else None
     kdiv = (torch.rand(K, generator=g, device=DEV) + 0.5) if case.epi["kdiv"] else None
     n = K * (Cc // G) * R * S
@@ -249,18 +265,18 @@ def _wgrad(case, g):
                                   scratch.data_ptr(), flag.data_ptr(), L.stream())
     got = _launch_twice(fn, out, n, scratch).view(K, Cc // G, R, S)
     Ssum = _ref_wgrad(x, dy, case)
+    mul = torch.ones(K, device=DEV)
+    if a is not None or kdiv is not None:
+        av = a if a is not None else torch.ones(1, device=DEV)
+        mul = (av / kdiv) if kdiv is not None else av.expand(K)      # fp32 division: RN, as __fdiv_rn
+    mul = mul.view(K, 1, 1, 1)
     if f32:
-        _bound(got, Ssum, _ref_wgrad(x.abs(), dy.abs(), case), C_BWD, f"wgrad {case.terms}")
+        Rm = _ref_wgrad(x.abs(), dy.abs(), case) * mul.double().abs()
+        _bound(got, Ssum * mul.double(), Rm, C_WGRAD, f"wgrad {case.terms}", case.maxnorm)
         return
     assert float(Ssum.abs().max()) < 2 ** 24
     S32 = Ssum.float()
-    if a is None and kdiv is None:
-        want = S32
-    else:
-        av = a if a is not None else torch.ones(1, device=DEV)
-        mul = (av / kdiv) if kdiv is not None else av.expand(K)      # fp32 division: RN, as __fdiv_rn
-        want = S32 * mul.view(K, 1, 1, 1)
-    _bits_equal(got, want, case.id)
+    _bits_equal(got, S32 if a is None and kdiv is None else S32 * mul, case.id)
 
 
 def _refusal(case):
@@ -291,7 +307,7 @@ def _refusal(case):
 @pytest.mark.parametrize("case", PC.CASES, ids=lambda c: c.id)
 def test_case_against_fp64(case):
     g = torch.Generator(device=DEV).manual_seed(sum(map(ord, case.id)))
-    with _env(case.env):            # the knobs change the plan, hence the weight image as well as the launch
+    with env(case.env):            # the knobs change the plan, hence the weight image as well as the launch
         if case.refuse:
             _refusal(case)
         elif case.mode in ("fwd", "i8"):

@@ -1,77 +1,19 @@
 """int8 operands of the packed-operand family (mnb_pk_i8_*, iao.freeze_inference(int8=True)) on the H100.
 
-* kernel cases: the int8 conv of random s8 levels is bitwise equal to mnb_pk_conv (bf16 wgmma) on the same levels, and to
-  the fp64 convolution of the levels rounded as fmaf(float(sum), scale, bias); outputs start as NaN and every case runs twice
-  with bitwise-identical results.  CASES (read by test_pk_int8_cpu.py) reach every int8 plan signature of the ResNet models
-  and every pk_conv_kernel<false, Nt, true> instance;
+* the kernel at every plan it can take: the "i8" cases of tests/pk_conv_cases.py in test_gpu_pk_conv_fp64.py (bit for bit
+  the fp64 sum's fmaf(S, scale, bias) and mnb_pk_conv's result on the same levels);
 * above 2^24: the s32 sum is exact and rounded once;
 * packers and hand-offs: pack_act_i8 holds the levels of the bf16 plane, the consumer-plane epilogue and
   mnb_quant_add_pack_i8_fwd write exactly pack_act_i8 of their fp32 result;
 * models: freeze_inference(int8=True) logits are bitwise equal to freeze_inference() and to the plain eval forward."""
 import collections
 import ctypes as C
-import os
 
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-Case = collections.namedtuple("Case", "id shape env")   # shape = (B, C, H, W, K, R, stride, pad, groups)
-
-CASES = [
-    Case("stem_c3", (4, 3, 32, 32, 64, 3, 1, 1, 1), {}),
-    Case("stem_224", (1, 3, 224, 224, 64, 3, 1, 1, 1), {}),
-    Case("sc_1x1_s2", (4, 64, 16, 16, 128, 1, 2, 0, 1), {}),
-    Case("s2_3x3", (4, 64, 16, 16, 128, 3, 2, 1, 1), {}),
-    Case("s2_3x3_224", (1, 64, 224, 224, 128, 3, 2, 1, 1), {}),
-    Case("w224", (1, 64, 224, 224, 64, 3, 1, 1, 1), {}),
-    Case("grouped_kg16", (4, 64, 8, 8, 64, 3, 1, 1, 4), {}),
-    Case("grouped_kg32", (4, 128, 8, 8, 128, 3, 1, 1, 4), {}),
-    Case("res32_256", (8, 256, 8, 8, 256, 3, 1, 1, 1), {}),
-    Case("res32_512", (16, 512, 4, 4, 512, 3, 1, 1, 1), {}),
-    Case("res32_512_s2", (16, 256, 8, 8, 512, 3, 2, 1, 1), {}),
-    Case("res224_128", (8, 128, 28, 28, 128, 3, 1, 1, 1), {}),
-    Case("res224_512_sc", (8, 256, 14, 14, 512, 1, 2, 0, 1), {}),
-    Case("nt16", (4, 32, 16, 16, 16, 3, 1, 1, 1), {}),
-    Case("nt32", (4, 32, 16, 16, 32, 3, 1, 1, 1), {}),
-    Case("nt48", (4, 48, 16, 16, 48, 3, 1, 1, 1), {}),
-    Case("nt96_k10", (4, 40, 12, 12, 90, 3, 1, 1, 1), {}),
-    Case("mt4_nt32", (8, 64, 16, 16, 32, 3, 1, 1, 1), {"MNB_PK_MT": "4"}),
-    Case("mt2_nt64", (8, 64, 16, 16, 64, 3, 1, 1, 1), {"MNB_PK_MT": "2"}),
-    Case("mt1_nt128", (8, 128, 16, 16, 128, 3, 1, 1, 1), {"MNB_PK_MT": "1"}),
-    Case("stages2", (4, 128, 16, 16, 128, 3, 1, 1, 1), {"MNB_PK_STAGES": "2"}),
-    Case("stages4", (4, 256, 8, 8, 128, 3, 1, 1, 1), {"MNB_PK_STAGES": "4"}),
-    Case("coltiles3", (2, 64, 56, 56, 64, 3, 1, 1, 1), {"MNB_PK_COLTILES": "3"}),
-]
-
-
-class _env:
-    def __init__(self, env):
-        self.env, self.old = env, {}
-
-    def __enter__(self):
-        for k, v in self.env.items():
-            self.old[k] = os.environ.get(k)
-            os.environ[k] = v
-
-    def __exit__(self, *exc):
-        for k, v in self.old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-
-
-def plan_of(case):
-    """the int8 plan of a case under its environment (host only)"""
-    from micronet_b200 import pk as PK
-    from tests import pk_plan_util as PU
-    with _env(case.env):
-        p = PK.i8_plan(PU.shape(*case.shape))
-    return None if p is None else dict(zip(PU.CONV_FIELDS, p))
-
 
 def _iao_spec(scale, bits=8):
     from micronet_b200 import _lib as L, functional as F_
@@ -98,17 +40,6 @@ def _levels_bf16(plane, B, Cc, H, W, split=False):
     return v.view(B, o, H, W, 8).permute(0, 1, 4, 2, 3).reshape(B, o * 8, H, W)[:, :Cc]
 
 
-def _fmaf_ref(sum64, scale, bias):
-    """float32(fmaf(float32(sum), scale, bias)) per element, from the exact fp64 sum; also the mask of elements where the
-    fp64 evaluation could round differently (exact fp32 midpoint after the fp64 add: never seen, excluded)"""
-    a = sum64.float().double()
-    r = a * scale.double().view(1, -1, 1, 1) + bias.double().view(1, -1, 1, 1)
-    y = r.float()
-    lo, hi = torch.nextafter(y, torch.full_like(y, -float("inf"))), torch.nextafter(y, torch.full_like(y, float("inf")))
-    mid = ((r - (y.double() + lo.double()) / 2).abs() == 0) | ((r - (y.double() + hi.double()) / 2).abs() == 0)
-    return y, mid
-
-
 def _case_operands(B, Cc, H, W, K, R, st, pad, G, seed, extreme=False):
     from micronet_b200 import _lib as L
     g = torch.Generator(device=DEV).manual_seed(seed)
@@ -125,49 +56,37 @@ def _case_operands(B, Cc, H, W, K, R, st, pad, G, seed, extreme=False):
     return sh, xl, w_int, w_scale, bias
 
 
-def _run_case(case, seed=11, extreme=False):
-    """(int8 result, bf16 result, exact fp64 sum) of one case; asserts the repeat is bitwise identical"""
+def _run_case(shape, seed=11, extreme=False):
+    """(int8 result, bf16 result, exact fp64 sum) of one shape (B, C, H, W, K, R, stride, pad, groups); asserts the repeat
+    is bitwise identical"""
     from micronet_b200 import _lib as L, pk as PK
-    B, Cc, H, W, K, R, st, pad, G = case.shape
+    B, Cc, H, W, K, R, st, pad, G = shape
     sh, xl, w_int, w_scale, bias = _case_operands(B, Cc, H, W, K, R, st, pad, G, seed, extreme)
     spec = _iao_spec(1.0)                    # scale 1: the levels are the input values themselves
     a_scale = torch.ones(1, device=DEV)
     P, Q = (H + 2 * pad - R) // st + 1, (W + 2 * pad - R) // st + 1
-    with _env(case.env):
-        x8 = PK.pack_act_i8(xl, spec.struct(), phase_split=st == 2)
-        w8 = PK.pack_weight_i8(sh, w_int)
-        outs = []
-        for _ in range(2):
-            y = torch.full((B, K, P, Q), float("nan"), device=DEV)
-            L.check(PK.conv_i8(sh, x8, w8, y, n_scale=w_scale, a_scale=a_scale, bias=bias), "pk_i8_conv")
-            outs.append(y)
-        xb, _ = PK.pack_act(xl, spec.struct(), 1, phase_split=st == 2)
-        wb = PK.pack_weight(sh, 0, 1, 1, w_int=w_int)
-        yb = torch.full((B, K, P, Q), float("nan"), device=DEV)
-        L.check(PK.conv(sh, 0, xb, 1, wb, 1, yb, n_scale=w_scale, a_scale=a_scale, bias=bias), "pk_conv")
+    x8 = PK.pack_act_i8(xl, spec.struct(), phase_split=st == 2)
+    w8 = PK.pack_weight_i8(sh, w_int)
+    outs = []
+    for _ in range(2):
+        y = torch.full((B, K, P, Q), float("nan"), device=DEV)
+        L.check(PK.conv_i8(sh, x8, w8, y, n_scale=w_scale, a_scale=a_scale, bias=bias), "pk_i8_conv")
+        outs.append(y)
+    xb, _ = PK.pack_act(xl, spec.struct(), 1, phase_split=st == 2)
+    wb = PK.pack_weight(sh, 0, 1, 1, w_int=w_int)
+    yb = torch.full((B, K, P, Q), float("nan"), device=DEV)
+    L.check(PK.conv(sh, 0, xb, 1, wb, 1, yb, n_scale=w_scale, a_scale=a_scale, bias=bias), "pk_conv")
     torch.cuda.synchronize()
     L.tc_check()
-    assert torch.equal(outs[0], outs[1]), f"{case.id}: the repeat differs"
+    assert torch.equal(outs[0], outs[1]), "the repeat differs"
     s64 = torch.nn.functional.conv2d(xl.double(), w_int.double(), stride=st, padding=pad, groups=G)
     return outs[0], yb, s64, w_scale, bias
-
-
-@pytest.mark.parametrize("case", CASES, ids=lambda c: c.id)
-def test_int8_conv_matches_bf16_and_fp64(case):
-    y8, yb, s64, w_scale, bias = _run_case(case)
-    assert not torch.isnan(y8).any(), f"{case.id}: outputs left unwritten"
-    assert s64.abs().max().item() < 2 ** 24
-    assert torch.equal(y8, yb), f"{case.id}: int8 and bf16 results differ at {(y8 != yb).sum().item()} elements"
-    ref, mid = _fmaf_ref(s64, w_scale, bias)
-    bad = (y8 != ref) & ~mid
-    assert not bad.any(), f"{case.id}: {bad.sum().item()} elements differ from the fp64 reference"
 
 
 def test_sums_above_2_24_are_exact_and_rounded_once():
     """sums of ~7.4e7 that fp32 cannot hold: the s32 accumulators keep them exact, so the result is the exact sum rounded
     once (scale 1, bias 0), where an fp32 accumulation (the bf16 kernel's) rounds its partial sums on the way"""
-    case = Case("extreme", (1, 512, 8, 8, 64, 3, 1, 1, 1), {})
-    y8, yb, s64, _, _ = _run_case(case, extreme=True)
+    y8, yb, s64, _, _ = _run_case((1, 512, 8, 8, 64, 3, 1, 1, 1), extreme=True)
     assert s64.abs().min().item() > 2 ** 24                         # >= 512 x 4 x 126^2 even in the corners
     want = s64.float()                                              # the exact integer sum rounded once to fp32
     assert (want.double() != s64).float().mean().item() > 0.5       # most exact sums are not fp32 numbers

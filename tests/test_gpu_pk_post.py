@@ -1,6 +1,8 @@
 """Consumer-plane epilogues of the packed-operand convolutions (mnb_pk_conv_post, mnb_pk_i8_conv with a consumer) against a
 host reference, at every case of tests/pk_post_cases.py: every (epilogue path, N tile) instance, the plan features, several
-work items per CTA, and every linked conv of the frozen graphs at the batch the benchmark runs them.
+work items per CTA, and every linked conv of the frozen graphs at the batch the benchmark runs them.  Behind a segmented
+producer plan (asymmetric levels), mnb_pk_conv_post refuses before launching or writes what the unfused pair writes, and
+functional.frozen_conv hands the consumer the plane its own quantizer makes of y.
 
 Operands are integer levels, so the conv sum S is exact (|S| < 2^24, asserted; S is computed on the device in fp64 and
 must be integral).  Each launch writes into an fp32 ``out`` filled with NaN and a plane filled with 0x5A followed by guard
@@ -10,7 +12,7 @@ Bit-exact check: the epilogue's documented fp32 op sequence, evaluated from S:
     scv = fl(a_scale * n_scale);  y = fmaf(S, scv, bias);  [BatchNorm: fmaf(fl(y - mean), fl(gamma * invstd), beta)];
     [ReLU];  the oracle's quantizer (levels + zero point), or the sequential round-to-nearest bf16 split into pieces.
 fmaf is emulated as an fp64 sum rounded to fp32; the only elements that double rounding can flip are those whose fp64 sum
-is exactly halfway between two fp32 values, and those are recomputed exactly with fractions.Fraction.  Every plane byte
+is exactly halfway between two fp32 values, and those are settled by the sign of the sum's exact TwoSum error.  Every plane byte
 (levels, zeroed channel padding, every phase, the shuffled destination) and the guard bytes must match; ``out`` too.
 
 fp64 check (against a reference that copies a wrong op order): the chain in fp64 without intermediate rounding, quantized
@@ -22,13 +24,13 @@ the bias, set to a boundary or one ulp beside it), others a power-of-two scale o
 +-1 weight tap, so y steps through the consecutive fp32 values around that boundary."""
 import ctypes as C
 import math
-from fractions import Fraction
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as TF
 
+from tests import pk_plan_util as PU
 from tests import pk_post_cases as P
 
 pytestmark = pytest.mark.gpu
@@ -38,38 +40,6 @@ EPS = 2.0 ** -24
 
 
 # ---- fp32 arithmetic of the reference
-def _f32_of_fraction(q):
-    """the fp32 value nearest to the rational q (ties to even)"""
-    f = np.float32(float(q))
-    best = None
-    for c in (np.nextafter(f, np.float32(-np.inf)), f, np.nextafter(f, np.float32(np.inf))):
-        d = abs(Fraction(float(c)) - q)
-        even = (int(np.array(c, dtype=np.float32).view(np.int32)) & 1) == 0
-        if best is None or d < best[0] or (d == best[0] and even):
-            best = (d, c)
-    return float(best[1])
-
-
-def fma32(a, b, c, stats=None):
-    """fl32(a * b + c) of float32 tensors (broadcasting): the product is exact in fp64, the fp64 sum rounds once, and the
-    elements whose fp64 sum lies exactly halfway between two fp32 values are recomputed with Fraction"""
-    a, b, c = torch.broadcast_tensors(a, b, c)
-    s = a.double() * b.double() + c.double()
-    f = s.float()
-    d = s - f.double()
-    g = torch.nextafter(f, torch.where(d > 0, torch.full_like(f, math.inf), torch.full_like(f, -math.inf)))
-    mid = (d != 0) & (s == (f.double() + g.double()) * 0.5)
-    idx = mid.nonzero(as_tuple=True)
-    if idx[0].numel():
-        av, bv, cv = a[idx].tolist(), b[idx].tolist(), c[idx].tolist()
-        exact = [_f32_of_fraction(Fraction(x) * Fraction(y) + Fraction(z)) for x, y, z in zip(av, bv, cv)]
-        f = f.clone()
-        f[idx] = torch.tensor(exact, dtype=torch.float32, device=f.device)
-    if stats is not None:
-        stats["midpoints"] = stats.get("midpoints", 0) + int(idx[0].numel())
-    return f
-
-
 def round_half_away(v):
     return torch.sign(v) * torch.floor(torch.abs(v) + 0.5)
 
@@ -285,7 +255,7 @@ def run_case(case, monkeypatch):
     # ---- bit-exact reference of the fp32 op sequence
     stats = {}
     scv = n_scale.view(1, -1, 1, 1)                  # a_scale = 1: scv = fl(1 * n_scale) = n_scale
-    y = fma32(S.float(), scv, bias.view(1, -1, 1, 1), stats)
+    y = PU.fmaf32(S.float(), scv, bias.view(1, -1, 1, 1), stats)
     if out is not None:
         assert not torch.isnan(yout).any(), "out positions the epilogue never wrote"
         assert torch.equal(yout.view(torch.int32), y.view(torch.int32)), \
@@ -293,7 +263,7 @@ def run_case(case, monkeypatch):
     v = y
     if bn is not None:
         mean, invstd, gamma, beta = (t.view(1, -1, 1, 1) for t in bn)
-        v = fma32(v - mean, gamma * invstd, beta.expand_as(v), stats)
+        v = PU.fmaf32(v - mean, gamma * invstd, beta.expand_as(v), stats)
     if case.relu:
         v = torch.clamp_min(v, 0.0)
     # fp64 chain, no intermediate rounding
@@ -329,7 +299,7 @@ def run_case(case, monkeypatch):
             assert (err <= ex).all(), f"{case.id}: term planes off the fp64 chain by more than 4 * 2^-24 * M"
             ratio = (err / ex.clamp_min(1e-300)).max().item()
         print(f"{case.id}: terms {terms}, worst |pieces - fp64 chain| / bound = {ratio}, "
-              f"fma midpoints redone exactly: {stats.get('midpoints', 0)}")
+              f"fma midpoints settled: {stats.get('midpoints', 0)}")
         return ratio
     lev = quant_levels(v, qd)
     want = encode(lev, K, cpu, case.split, case.sg)
@@ -352,7 +322,7 @@ def run_case(case, monkeypatch):
     placed = (role > 0).to(DEV).view(1, -1, 1, 1).expand_as(near)
     print(f"{case.id}: one level off the fp64 chain near a boundary: {int((near & ~placed).sum())} elements of the random "
           f"channels, {int((near & placed).sum())} of the boundary channels ({int((dist <= du).sum())} within the bound of a "
-          f"boundary); fma midpoints redone exactly: {stats.get('midpoints', 0)}")
+          f"boundary); fma midpoints settled: {stats.get('midpoints', 0)}")
     return None
 
 
@@ -518,3 +488,97 @@ def test_plane_maxpool_requant_matches_the_reference(plane, i8):
     assert (got[nbytes:] == 0x5A).all(), "guard bytes behind the plane were written"
     bad = (got[:nbytes] != want).sum().item()
     assert bad == 0, f"{bad} of {nbytes} plane bytes differ"
+
+
+# ---- fused consumer behind a segmented producer plan (frozen inference graphs)
+# asymmetric IAO producer: its levels (code + zero point) take two bf16 pieces, so with 3x3 x 64 channels the K loop is
+# segmented; the consumer is a symmetric IAO conv (one-piece plane)
+POST_SHAPE = (4, 64, 16, 16, 128, 3, 1, 1, 1)
+POST_PLAN = dict(segmented=1, npairs=2, Nt=128)
+
+
+def _iao(scale, sym, dev=DEV):
+    from micronet_b200 import _lib as L, functional as F_
+    zp = 0.0 if sym else -101.0
+    lo, hi = (-127.5 * scale, 127.5 * scale) if sym else ((0 + zp) * scale, (255 + zp) * scale)
+    bufs = dict(scale=torch.tensor([scale]), zero_point=torch.tensor([zp]), obs_min=torch.tensor([lo]), obs_max=torch.tensor([hi]))
+    return F_.ActSpec(L.ACT_IAO, qmin=-128 if sym else 0, qmax=127 if sym else 255, q_type=0 if sym else 1,
+                      **{k: v.to(dev) for k, v in bufs.items()})
+
+
+def _post_operands():
+    from micronet_b200 import pk as PK
+    B, Cc, H, W, K, R, st, pad, G = POST_SHAPE
+    g = torch.Generator().manual_seed(21)
+    x = (torch.randn(B, Cc, H, W, generator=g) * 3).to(DEV)
+    w_int = torch.randint(-127, 128, (K, Cc, R, R), generator=g, dtype=torch.int16).to(DEV)
+    w_scale = (torch.rand(K, generator=g) * 0.01 + 0.001).to(DEV)
+    bias = torch.randn(K, generator=g).to(DEV)
+    spec, nxt = _iao(0.05, False), _iao(0.11, True)
+    sh = PU.shape(*POST_SHAPE)
+    x_pk, _ = PK.pack_act(x, spec.struct(), 2)
+    w_img = PK.pack_weight(sh, 0, 2, 1, w_int=w_int)
+    y_ref = torch.empty(B, K, H, W, device=DEV)
+    from micronet_b200 import _lib as L
+    L.check(PK.conv(sh, 0, x_pk, 2, w_img, 1, y_ref, n_scale=w_scale, a_scale=spec.scale, bias=bias), "conv")
+    return sh, x, x_pk, w_int, w_img, w_scale, bias, spec, nxt, y_ref
+
+
+def _check_post(with_out):
+    """mnb_pk_conv_post on the segmented plan either refuses it before launching or writes exactly what the unfused pair
+    writes; it must never return success with the consumer plane (or y) left unwritten"""
+    from micronet_b200 import _lib as L, pk as PK
+    plan = PU.conv_plan(PU.shape(*POST_SHAPE), 0, 2, 1)
+    assert {k: plan[k] for k in POST_PLAN} == POST_PLAN, plan
+    sh, x, x_pk, w_int, w_img, w_scale, bias, spec, nxt, y_ref = _post_operands()
+    B, Cc, H, W, K = POST_SHAPE[:5]
+    for relu in (False, True):
+        for split in (False, True):
+            want, _ = PK.pack_act(y_ref, nxt.struct(), 1, phase_split=split, relu=relu)
+            plane = PK.consumer_plane(B, K, H, W, DEV).fill_(0xFF)
+            y = torch.full_like(y_ref, float("nan")) if with_out else None
+            rc = PK.conv_post(sh, x_pk, 2, w_img, 1, y, nxt.struct(), plane, relu, split, n_scale=w_scale,
+                              a_scale=spec.scale, bias=bias)
+            torch.cuda.synchronize()
+            if rc == L.E_UNSUPPORTED:
+                assert (plane == 0xFF).all() and (y is None or torch.isnan(y).all()), "refused, yet something was written"
+                continue
+            L.check(rc, "conv_post")
+            assert torch.equal(plane, want), ("consumer plane", relu, split)
+            if with_out:
+                assert torch.equal(y, y_ref), ("y", relu, split)
+    L.tc_check()
+
+
+def test_conv_post_on_a_segmented_producer_plan_with_out():
+    _check_post(True)
+
+
+def test_conv_post_on_a_segmented_producer_plan_plane_only():
+    _check_post(False)
+
+
+@pytest.mark.parametrize("only", [False, True], ids=["y_kept", "plane_only"])
+def test_frozen_conv_behind_an_asymmetric_producer_hands_the_right_plane(only):
+    """functional.frozen_conv with a consumer: whatever path it takes, y equals the plain conv and the plane the consumer
+    reads equals the consumer's own quantizer applied to y"""
+    from micronet_b200 import functional as F_, pk as PK
+    sh, x, x_pk, w_int, w_img, w_scale, bias, spec, nxt, y_ref = _post_operands()
+    B, Cc, H, W, K, R, st, pad, G = POST_SHAPE
+    wq = w_int.float() * w_scale.view(-1, 1, 1, 1)
+    consumer_mod = torch.nn.Identity()
+    for relu in (False, True):
+        cons = F_.Consumer(consumer_mod, nxt, relu, only, (K, K, 3, 3), (1, 1), (1, 1), (1, 1), 1, True)
+        assert cons.accepts((B, K, H, W))
+        y = F_.frozen_conv(x, None, wq, bias, w_int, w_scale, spec, (1, 1), (1, 1), (1, 1), 1, consumer=cons)
+        torch.cuda.synchronize()
+        plane = F_.handed_plane(consumer_mod, y)
+        want, _ = PK.pack_act(y_ref, nxt.struct(), 1, relu=relu)
+        if plane is None:            # not fused: y holds the data, the consumer packs it itself
+            assert torch.equal(y, y_ref)
+            got, _ = PK.pack_act(y, nxt.struct(), 1, relu=relu)
+            assert torch.equal(got, want)
+        else:
+            assert torch.equal(plane, want), relu
+            if y.device.type != "meta":
+                assert torch.equal(y, y_ref)

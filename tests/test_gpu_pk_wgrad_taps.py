@@ -3,8 +3,8 @@ registers, against an fp64 convolution of the same operands and against mnb_pk_w
 for bit (same accumulation chains, batch splits and reduction order).
 
 Bound: element-wise |dw - ref| <= 2^-14 * R, R = the same weight gradient of |dy| and |x| in fp64 (chains of <= 256 MMAs
-between round-to-nearest adds, two bf16 pieces of dy), the bound test_gpu_pk.py holds mnb_pk_wgrad to.  Results start as
-NaN, so an element the kernels never write fails."""
+between round-to-nearest adds, two bf16 pieces of dy), the bound test_gpu_pk_conv_fp64.py holds mnb_pk_wgrad to.
+Results start as NaN, so an element the kernels never write fails."""
 import copy
 
 import pytest

@@ -353,16 +353,9 @@ def _ulp(v):
 
 
 def _fmaf_exact(sum64, scale, bias):
-    """float32(fmaf(float32(sum), scale, bias)) per element from the exact fp64 sum, and the mask of elements where that
-    is not certain: the fp64 add rounded (its two-sum error is non-zero) and landed on an fp32 midpoint"""
-    from tests.test_gpu_pk_int8 import _fmaf_ref
-    y, mid = _fmaf_ref(sum64, scale, bias)
-    p = sum64.float().double() * scale.double().view(1, -1, 1, 1)       # exact: 24 x 24 significand bits
-    b = bias.double().view(1, -1, 1, 1)
-    s = p + b
-    bb = s - p
-    rounded = ((p - (s - bb)) + (b - bb)) != 0
-    return y, mid & rounded
+    """float32(fmaf(float32(sum), scale, bias)) per element from the exact fp64 sum, correctly rounded"""
+    from tests.pk_plan_util import fmaf32
+    return fmaf32(sum64.float(), scale.view(1, -1, 1, 1), bias.view(1, -1, 1, 1))
 
 
 def _check_bound(got, ref, absref, n, scale=1.0, what=""):
@@ -450,7 +443,7 @@ def _levels(x, spec, codes, offset):
 @pytest.mark.parametrize("case", FWD_CASES, ids=lambda c: c.id)
 def test_forward_integer_operands_equal_the_exact_epilogue(case, mode):
     """integer operands with every partial sum below 2^24: y is bitwise fmaf(sum, a_scale * w_scale, bias) of the exact
-    sum (the fp32 accumulation is exact), except where the fp64 evaluation sits on an fp32 midpoint"""
+    sum (the fp32 accumulation is exact), at every element"""
     if case.id in T.MODEL_CASES and mode not in ("pm1", "dorefa4"):
         pytest.skip("model shapes: the wbwtab operands and one quantizer")
     _pinned(case)
@@ -467,10 +460,8 @@ def test_forward_integer_operands_equal_the_exact_epilogue(case, mode):
     s64 = TF.conv2d(e, w_int.double(), None, 1, R // 2, 1, G)
     assert s64.abs().max().item() < 2 ** 24
     sc = (a_scale * w_scale).float()                     # __fmul_rn(a_scale, w_scale[n]) of the kernel's constants
-    want, unsure = _fmaf_exact(s64, sc, bias)
-    bad = (out[0] != want) & ~unsure
+    bad = out[0] != _fmaf_exact(s64, sc, bias)
     assert not bad.any(), f"{int(bad.sum())} elements differ from the exact epilogue, first at {bad.nonzero()[0].tolist()}"
-    assert unsure.float().mean().item() < 1e-4
 
 
 def test_forward_sums_past_2_24_keep_the_fp32_bound():
@@ -581,8 +572,7 @@ def test_forward_mixed_exactness_is_exact():
     (y,) = _fwd(case, x, None, w_int, w_scale, bias)
     s64 = TF.conv2d(x.double(), w_int.double(), None, 1, R // 2, 1, G)
     assert torch.equal(s64.float().double(), s64)
-    want, unsure = _fmaf_exact(s64, w_scale, bias)
-    bad = (y != want) & ~unsure
+    bad = y != _fmaf_exact(s64, w_scale, bias)
     assert not bad.any(), f"{int(bad.sum())} elements differ, first at {bad.nonzero()[0].tolist()}"
 
 

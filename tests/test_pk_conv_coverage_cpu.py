@@ -4,6 +4,9 @@
 * the cases reach every pk_conv_kernel instance of rows 0 / 1 (forward and data gradient) and row 2 (int8), every
   pk_wgrad_kernel<Nc>, every plan feature and epilogue form listed below, and every refusal reason of the source that a
   shape can reach (the others are listed in pk_conv_cases.UNREACHABLE with the reason);
+* the cases reach every plan signature of the bench models' convs at every terms configuration the models use (forward,
+  data gradient, weight gradient, and int8 for the ResNet convs), and every (mode, terms, signature) the older
+  packed-operand tests launched (RETIRED_LAUNCHES), and set every MNB_PK_* knob those launches set;
 * a seeded sweep of random shapes at the term counts the models use meets no refusal reason outside that list, and for
   every shape the plan query and the launch agree: the launch, given a misaligned operand pointer, returns the query's code
   and text where the query refuses, and fails at the operand's tensor map (before any kernel launch) where it accepts;
@@ -18,55 +21,13 @@ import pytest
 
 from tests import pk_conv_cases as PC
 from tests import pk_plan_util as PU
+from tests.pk_plan_util import case_shape as shape, query
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CONV_FIELDS = PU.CONV_FIELDS + ("ntmpl0 ntmpl1 ntmpl2 ntmpl3 ntap0 ntap1 ntap2 ntap3 words last_seg").split()
-WGRAD_FIELDS = PU.WGRAD_FIELDS + "n_ktiles nkph_used stg_per_split nsub prog nstg_total".split()
+ROOT = PU.ROOT
+FWD_TERMS = [(1, 1), (2, 1), (3, 3), (1, 3)]     # integer levels, asymmetric levels, fp32 x fp32, fp32 x levels
+BWD_TERMS = [(2, 1), (2, 2)]                     # two dy pieces (PK_TERMS_BWD) x integer / fp32 second operand
 MISALIGNED = 4096 + 8        # never dereferenced: the first tensor map refuses a base that is not 16-byte aligned
 SMEM_BUDGET = 227 * 1024 - 3072
-
-
-class _env:
-    def __init__(self, env):
-        self.env, self.old = env, {}
-
-    def __enter__(self):
-        for k, v in self.env.items():
-            self.old[k] = os.environ.get(k)
-            os.environ[k] = v
-
-    def __exit__(self, *exc):
-        for k, v in self.old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-
-
-def shape(s):
-    from micronet_b200 import _lib as L
-    B, Cc, H, W, K, R, S, st, ph, pw, G = s[:11]
-    dil = s[11] if len(s) > 11 else 1
-    return L.ConvShape(B, Cc, H, W, K, R, S, st, st, ph, pw, dil, dil, G)
-
-
-def query(mode, sh, terms):
-    """(code, error text, plan dict) of the host-only query of a launch mode"""
-    from micronet_b200 import _lib as L
-    lib = L.load()
-    if mode == "wgrad":
-        out = (C.c_int32 * len(WGRAD_FIELDS))()
-        rc = lib.mnb_pk_wgrad_plan(C.byref(sh), terms[0], terms[1], out, len(out))
-        names = WGRAD_FIELDS
-    else:
-        out = (C.c_int32 * len(CONV_FIELDS))()
-        if mode == "i8":
-            rc = lib.mnb_pk_i8_conv_plan(C.byref(sh), out, len(out))
-        else:
-            rc = lib.mnb_pk_conv_plan_ex(C.byref(sh), 0 if mode == "fwd" else 1, terms[0], terms[1], out, len(out))
-        names = CONV_FIELDS
-    text = lib.mnb_last_error() if rc else b""
-    return rc, text, (dict(zip(names, list(out))) if rc == 0 else None)
 
 
 def fake_launch(mode, sh, terms):
@@ -85,7 +46,7 @@ def fake_launch(mode, sh, terms):
 
 
 def case_plan(case):
-    with _env(case.env):
+    with PU.env(case.env):
         return query(case.mode, shape(case.shape), case.terms)
 
 
@@ -158,7 +119,8 @@ def epilogue_forms(case):
 
 
 WANT_FEATURES = (
-    {f"{m} MT{t} partial last M group" for m in ("fwd",) for t in (2, 4)} | {"fwd MT1", "dgrad MT1"} |
+    {f"{m} MT{t} partial last M group" for m in ("fwd",) for t in (2, 4)} | {"dgrad MT2 partial last M group"} |
+    {"fwd MT1", "dgrad MT1"} |
     {f"{m} {f}" for m in ("fwd", "dgrad") for f in ("TB > 1", "partial last row tile", "kg % 16 != 0", "partial last N tile",
                                                    "ng % 16 != 0", "group-padded planes")} |
     {"fwd partial last column tile", "fwd ragged last K chunk", "fwd several tap groups in a k-phase", "fwd stride 2 (4 k-phases)",
@@ -255,7 +217,7 @@ def test_every_refusal_reason_is_cased_or_listed(plans):
 
 @pytest.mark.parametrize("case", [c for c in PC.CASES if c.refuse], ids=lambda c: c.id)
 def test_refusal_launch_returns_the_query_code_and_text(case):
-    with _env(case.env):
+    with PU.env(case.env):
         sh = shape(case.shape)
         q = query(case.mode, sh, case.terms)
         f = fake_launch(case.mode, sh, case.terms)
@@ -309,6 +271,161 @@ def test_sweep_query_and_launch_agree():
     assert any("MMA program longer" in r for r in reasons), sorted(reasons)
 
 
+# ---- plan signatures: the bench models' and the retired tests'
+# (mode, terms, plan signature, operand kind, MNB_PK_* knobs) of every launch of the packed-operand tests the case list
+# replaced: 20 ResNet / NIN / NIN-GC shapes at forward (1, 1) / (3, 3), data gradient (2, 1) / (3, 1) and weight gradient
+# (2, 1) / (2, 2) / (3, 1) / (3, 3), the bench models' multi-tile plans at reduced batch, the plans forced through the
+# knobs, and the int8 cases (signature (Nt, MT, phase split)).  Their backward ran on fp32 dy (every dy piece nonzero), so a
+# case of the same kind must reach each one.
+RETIRED_LAUNCHES = [
+    ("dgrad", (2, 1), (False, 128, 1, 1), "f32", ()), ("dgrad", (2, 1), (False, 128, 1, 4), "f32", ()),
+    ("dgrad", (2, 1), (False, 16, 1, 1), "f32", ()), ("dgrad", (2, 1), (False, 16, 1, 4), "f32", ()),
+    ("dgrad", (2, 1), (False, 16, 2, 1), "f32", ()), ("dgrad", (2, 1), (False, 16, 4, 1), "f32", ()),
+    ("dgrad", (2, 1), (False, 32, 1, 1), "f32", (("MNB_PK_COLTILES", "2"),)), ("dgrad", (2, 1), (False, 32, 1, 1), "f32", ()),
+    ("dgrad", (2, 1), (False, 64, 1, 4), "f32", ()), ("dgrad", (2, 1), (False, 64, 2, 1), "f32", (("MNB_PK_MT", "2"),)),
+    ("dgrad", (2, 1), (False, 64, 2, 4), "f32", ()), ("dgrad", (2, 1), (False, 96, 1, 1), "f32", ()),
+    ("dgrad", (2, 1), (True, 128, 1, 1), "f32", ()), ("dgrad", (2, 1), (True, 128, 1, 4), "f32", ()),
+    ("dgrad", (2, 1), (True, 16, 1, 1), "f32", ()), ("dgrad", (2, 1), (True, 16, 2, 1), "f32", ()),
+    ("dgrad", (2, 1), (True, 48, 1, 1), "f32", ()), ("dgrad", (2, 1), (True, 64, 1, 1), "f32", ()),
+    ("dgrad", (2, 1), (True, 64, 2, 1), "f32", ()), ("dgrad", (2, 1), (True, 96, 1, 1), "f32", ()),
+    ("dgrad", (2, 2), (True, 64, 1, 1), "f32", (("MNB_PK_SEG_MMAS", "8"),)), ("dgrad", (2, 2), (True, 64, 2, 1), "f32", ()),
+    ("dgrad", (2, 2), (True, 64, 2, 4), "f32", ()), ("dgrad", (3, 1), (False, 128, 1, 1), "f32", ()),
+    ("dgrad", (3, 1), (False, 16, 1, 1), "f32", ()), ("dgrad", (3, 1), (False, 16, 1, 4), "f32", ()),
+    ("dgrad", (3, 1), (False, 64, 1, 4), "f32", ()), ("dgrad", (3, 1), (False, 96, 1, 1), "f32", ()),
+    ("dgrad", (3, 1), (True, 128, 1, 1), "f32", ()), ("dgrad", (3, 1), (True, 128, 1, 4), "f32", ()),
+    ("dgrad", (3, 1), (True, 16, 1, 1), "f32", ()), ("dgrad", (3, 1), (True, 32, 1, 1), "f32", ()),
+    ("dgrad", (3, 1), (True, 48, 1, 1), "f32", ()), ("dgrad", (3, 1), (True, 64, 1, 1), "f32", ()),
+    ("dgrad", (3, 1), (True, 64, 1, 4), "f32", ()), ("dgrad", (3, 1), (True, 96, 1, 1), "f32", ()),
+    ("fwd", (1, 1), (False, 128, 1, 1), "int", ()), ("fwd", (1, 1), (False, 16, 1, 1), "int", ()),
+    ("fwd", (1, 1), (False, 32, 1, 1), "int", (("MNB_PK_COLTILES", "3"),)),
+    ("fwd", (1, 1), (False, 32, 1, 1), "int", (("MNB_PK_STAGES", "2"),)),
+    ("fwd", (1, 1), (False, 32, 1, 1), "int", (("MNB_PK_STAGES", "4"),)),
+    ("fwd", (1, 1), (False, 32, 1, 1), "int", (("MNB_PK_STAGES", "8"),)), ("fwd", (1, 1), (False, 32, 1, 1), "int", ()),
+    ("fwd", (1, 1), (False, 32, 2, 1), "int", ()), ("fwd", (1, 1), (False, 32, 4, 1), "int", (("MNB_PK_MT", "4"),)),
+    ("fwd", (1, 1), (False, 32, 4, 1), "int", ()), ("fwd", (1, 1), (False, 48, 1, 1), "int", ()),
+    ("fwd", (1, 1), (False, 64, 1, 1), "int", ()), ("fwd", (1, 1), (False, 64, 2, 1), "int", (("MNB_PK_MT", "2"),)),
+    ("fwd", (1, 1), (False, 96, 1, 1), "int", ()), ("fwd", (3, 3), (False, 128, 1, 1), "f32", ()),
+    ("fwd", (3, 3), (False, 32, 1, 1), "f32", ()), ("fwd", (3, 3), (False, 64, 1, 1), "f32", ()),
+    ("fwd", (3, 3), (False, 96, 1, 1), "f32", ()), ("fwd", (3, 3), (True, 128, 1, 1), "f32", ()),
+    ("fwd", (3, 3), (True, 16, 1, 1), "f32", ()), ("fwd", (3, 3), (True, 32, 1, 1), "f32", ()),
+    ("fwd", (3, 3), (True, 32, 4, 1), "f32", (("MNB_PK_MT", "4"),)), ("fwd", (3, 3), (True, 48, 1, 1), "f32", ()),
+    ("fwd", (3, 3), (True, 48, 2, 1), "f32", (("MNB_PK_MT", "2"),)),
+    ("fwd", (3, 3), (True, 64, 1, 1), "f32", (("MNB_PK_SEG_MMAS", "8"),)),
+    ("fwd", (3, 3), (True, 64, 1, 1), "f32", (("MNB_PK_STAGES", "2"),)), ("fwd", (3, 3), (True, 64, 1, 1), "f32", ()),
+    ("fwd", (3, 3), (True, 64, 2, 1), "f32", ()), ("fwd", (3, 3), (True, 96, 1, 1), "f32", ()),
+    ("i8", (1, 1), (128, 1, False), "int", (("MNB_PK_MT", "1"),)),
+    ("i8", (1, 1), (128, 1, False), "int", (("MNB_PK_STAGES", "2"),)),
+    ("i8", (1, 1), (128, 1, False), "int", (("MNB_PK_STAGES", "4"),)), ("i8", (1, 1), (128, 1, False), "int", ()),
+    ("i8", (1, 1), (128, 1, True), "int", ()), ("i8", (1, 1), (16, 1, False), "int", ()),
+    ("i8", (1, 1), (32, 1, False), "int", ()), ("i8", (1, 1), (32, 4, False), "int", (("MNB_PK_MT", "4"),)),
+    ("i8", (1, 1), (48, 1, False), "int", ()), ("i8", (1, 1), (64, 1, False), "int", (("MNB_PK_COLTILES", "3"),)),
+    ("i8", (1, 1), (64, 1, False), "int", ()), ("i8", (1, 1), (64, 2, False), "int", (("MNB_PK_MT", "2"),)),
+    ("i8", (1, 1), (64, 2, False), "int", ()), ("i8", (1, 1), (96, 1, False), "int", ()),
+    ("wgrad", (2, 1), (112, False, False), "f32", ()), ("wgrad", (2, 1), (128, False, False), "f32", ()),
+    ("wgrad", (2, 1), (16, True, False), "f32", (("MNB_PK_WG_MERGE", "0"),)), ("wgrad", (2, 1), (16, True, False), "f32", ()),
+    ("wgrad", (2, 1), (32, True, False), "f32", ()), ("wgrad", (2, 1), (48, True, False), "f32", (("MNB_PK_WG_NC", "48"),)),
+    ("wgrad", (2, 1), (48, True, False), "f32", ()), ("wgrad", (2, 1), (64, False, False), "f32", ()),
+    ("wgrad", (2, 1), (64, True, False), "f32", (("MNB_PK_WG_CHAIN", "16"),)), ("wgrad", (2, 1), (64, True, False), "f32", ()),
+    ("wgrad", (2, 1), (64, True, True), "f32", ()), ("wgrad", (2, 1), (80, False, False), "f32", ()),
+    ("wgrad", (2, 1), (96, False, False), "f32", ()), ("wgrad", (2, 2), (112, False, False), "f32", ()),
+    ("wgrad", (2, 2), (128, False, False), "f32", ()), ("wgrad", (2, 2), (16, True, False), "f32", ()),
+    ("wgrad", (2, 2), (32, True, False), "f32", ()), ("wgrad", (2, 2), (48, True, False), "f32", ()),
+    ("wgrad", (2, 2), (64, False, False), "f32", ()), ("wgrad", (2, 2), (64, True, False), "f32", ()),
+    ("wgrad", (2, 2), (64, True, True), "f32", ()), ("wgrad", (2, 2), (80, False, False), "f32", ()),
+    ("wgrad", (2, 2), (96, False, False), "f32", ()), ("wgrad", (3, 1), (112, False, False), "f32", ()),
+    ("wgrad", (3, 1), (128, False, False), "f32", ()), ("wgrad", (3, 1), (16, True, False), "f32", ()),
+    ("wgrad", (3, 1), (32, True, False), "f32", ()), ("wgrad", (3, 1), (48, True, False), "f32", ()),
+    ("wgrad", (3, 1), (64, False, False), "f32", ()), ("wgrad", (3, 1), (64, True, False), "f32", ()),
+    ("wgrad", (3, 1), (64, True, True), "f32", ()), ("wgrad", (3, 1), (80, False, False), "f32", ()),
+    ("wgrad", (3, 1), (96, False, False), "f32", ()), ("wgrad", (3, 3), (112, False, False), "f32", ()),
+    ("wgrad", (3, 3), (128, False, False), "f32", ()), ("wgrad", (3, 3), (16, True, False), "f32", ()),
+    ("wgrad", (3, 3), (32, True, False), "f32", ()), ("wgrad", (3, 3), (48, True, False), "f32", ()),
+    ("wgrad", (3, 3), (64, False, False), "f32", ()), ("wgrad", (3, 3), (64, True, False), "f32", ()),
+    ("wgrad", (3, 3), (64, True, True), "f32", ()), ("wgrad", (3, 3), (80, False, False), "f32", ()),
+    ("wgrad", (3, 3), (96, False, False), "f32", ()),
+]
+
+
+def signature(case, p):
+    if case.mode == "wgrad":
+        return PU.wgrad_signature(p)
+    if case.mode == "i8":
+        return PU.i8_signature(p, case.shape[7])
+    return PU.conv_signature(p)
+
+
+def case_signatures(plans):
+    """{(mode, terms, plan signature, operand kind)} of the cases"""
+    return {(c.mode, c.terms, signature(c, plans[c.id][2]), c.ops) for c in PC.CASES if not c.refuse}
+
+
+def test_every_retired_launch_is_reached(plans):
+    held = case_signatures(plans)
+    missing = [r for r in RETIRED_LAUNCHES if r[:4] not in held]
+    assert not missing, f"(mode, terms, plan signature, operand kind, knobs) of retired launches no case reaches: {missing}"
+
+
+def test_every_knob_of_the_retired_launches_is_set_by_a_case():
+    want = {k for r in RETIRED_LAUNCHES for k, _ in r[4]}
+    missing = sorted(want - {k for c in PC.CASES for k in c.env})
+    assert not missing, f"MNB_PK_* knobs no case sets: {missing}"
+
+
+def _model_signatures():
+    """{conv signature: [where]}, {wgrad signature: [where]}, {int8 signature: [where]} of the bench models"""
+    conv, wgrad, i8 = {}, {}, {}
+    for name, B, Cc, H, W, K, R, st, pad, G in PU.model_convs():
+        sh = PU.shape(B, Cc, H, W, K, R, st, pad, G)
+        train = not name.startswith("res224")      # the 224 x 224 workload is inference only
+        cfgs = [(0, t) for t in FWD_TERMS] + ([(1, t) for t in BWD_TERMS] if train else [])
+        for mode, terms in cfgs:
+            p = PU.conv_plan(sh, mode, *terms)
+            if p is not None:
+                conv.setdefault(PU.conv_signature(p), []).append(f"{name} mode {mode} terms {terms}")
+        if train:
+            for terms in BWD_TERMS:
+                p = PU.wgrad_plan(sh, *terms)
+                if p is not None:
+                    wgrad.setdefault(PU.wgrad_signature(p), []).append(f"{name} wgrad terms {terms}")
+        if name.startswith(("res32_", "res224_")):
+            p = PU.i8_plan(sh)
+            assert p is not None, name
+            i8.setdefault(PU.i8_signature(p, st), []).append(name)
+    return conv, wgrad, i8
+
+
+def test_model_signatures_are_reached(plans):
+    model = dict(zip(("conv", "wgrad", "i8"), _model_signatures()))
+    assert len(model["conv"]) >= 10 and len(model["wgrad"]) >= 5 and len(model["i8"]) >= 3, model
+    held = {}
+    for mode, terms, sig, _ in case_signatures(plans):
+        held.setdefault({"fwd": "conv", "dgrad": "conv"}.get(mode, mode), set()).add(sig)
+    missing = {(kind, sig): where[:3] for kind, sigs in model.items()
+               for sig, where in sigs.items() if sig not in held[kind]}
+    assert not missing, f"plan signatures of the bench models no case reaches (conv: segmented, Nt, MT, ny; wgrad: Nc, " \
+                        f"tpg > 1, gm > 1; i8: Nt, MT, phase split): {missing}"
+
+
+def test_plan_query_agrees_with_the_16_field_query():
+    """mnb_pk_conv_plan is mnb_pk_conv_plan_ex's first 16 fields; the wgrad query agrees with the scratch size"""
+    from micronet_b200 import _lib as L
+    lib = L.load()
+    for name, B, Cc, H, W, K, R, st, pad, G in PU.model_convs()[::3]:
+        sh = PU.shape(B, Cc, H, W, K, R, st, pad, G)
+        old = (C.c_int32 * 16)()
+        assert lib.mnb_pk_conv_plan(C.byref(sh), 0, 1, 1, old) == 0
+        p = PU.conv_plan(sh, 0, 1, 1)
+        assert list(old) == [p[f] for f in PU.CONV_FIELDS[:16]], name
+        assert p["acc"] == p["MT"] * p["Nt"] and p["n_mgroups"] == -(-p["n_mtiles"] // p["MT"]), name
+        assert p["n_items"] % p["n_mgroups"] == 0 and p["npairs"] == 1 and p["segmented"] == 0, name
+        short = (C.c_int32 * 3)(-7, -7, -7)
+        assert lib.mnb_pk_conv_plan_ex(C.byref(sh), 0, 1, 1, short, 2) == 0 and list(short)[2] == -7   # writes n fields only
+        w = PU.wgrad_plan(sh, 2, 1)
+        assert (w is None) == (lib.mnb_pk_wgrad_scratch_bytes(C.byref(sh), 2, 1) < 0), name
+        if w is not None:
+            assert w["tpg"] * w["Nc"] <= 128 and w["Nc"] in PU.WGRAD_NC, (name, w)
+
+
 def test_7x7_stride2_dgrad_is_refused_and_routed_to_the_generic_kernels():
     """the data gradient at (2, 1) of this shape needs an MMA program over 512 words: the query refuses it, so the layer's
     forward never commits it to the packed family (the launch in its backward would refuse)"""
@@ -335,7 +452,6 @@ def test_every_bench_launch_is_a_case():
     or a recorded consumer-plane launch, or is taken by gc3 (pk.gc3_plan), or runs on another family (the fp32 stems)"""
     from micronet_b200 import pk as PK
     from tests.pk_conv_bench_launches import BENCH_LAUNCHES, POST_LAUNCHES
-    from tests.test_pk_plan_cpu import _model_convs
     held = {(c.shape, {"fwd": 0, "dgrad": 1, "wgrad": 2}[c.mode], c.terms) for c in PC.CASES if c.bench}
     missing = []
     for wl, fn, sh, mode, ta, tw in BENCH_LAUNCHES:
@@ -345,7 +461,7 @@ def test_every_bench_launch_is_a_case():
     assert not missing, f"bench launches no case holds: {missing}"
     fwd_shapes = {tuple(sh) for wl, fn, sh, mode, ta, tw in BENCH_LAUNCHES + POST_LAUNCHES if mode == 0}
     unaccounted = []
-    for name, B, Cc, H, W, K, R, st, pad, G in _model_convs():
+    for name, B, Cc, H, W, K, R, st, pad, G in PU.model_convs():
         sh = PU.shape(B, Cc, H, W, K, R, st, pad, G)
         if PK._key(sh) in fwd_shapes or PK.gc3_plan(sh, 0, 1, 1) is not None or Cc == 3:
             continue

@@ -8,7 +8,7 @@ import subprocess
 
 import pytest
 
-from tests.test_pk_plan_cpu import LIMIT, RESERVED, _budget, _model_convs
+from tests.pk_plan_util import LIMIT, RESERVED, budget, model_convs
 
 GC3_LAYERS = {"gc3x3g16", "gc3x3g32"}
 E_ARG = -1   # MNB_E_ARG
@@ -26,7 +26,7 @@ def _plan(sh, mode, ta, tw):
     return rc, list(out)
 
 
-@pytest.mark.parametrize("conv", _model_convs(), ids=lambda c: c[0])
+@pytest.mark.parametrize("conv", model_convs(), ids=lambda c: c[0])
 def test_cover_is_exactly_the_grouped_3x3_layers(conv):
     from micronet_b200 import _lib as L
     name, B, Cc, H, W, K, R, st, pad, G = conv
@@ -78,7 +78,7 @@ def test_plan_limits(layer, B):
         assert nmb * 64 >= (tb - 1) * (H + 2) ** 2 + (H - 1) * (H + 2) + H, "M tile shorter than the image raster"
         assert nmb * nt // 2 <= 96, "accumulators over the register budget"
         # every ring slot belongs to one MMA warpgroup (stage k: slot k % nstage, warpgroup k % ncons)
-        assert ncons == 3 and nstage % ncons == 0 and ncons <= nstage <= 8 and 0 < smem <= _budget("mnb_pk.cu", "kGc3SmemBudget")
+        assert ncons == 3 and nstage % ncons == 0 and ncons <= nstage <= 8 and 0 < smem <= budget("mnb_pk.cu", "kGc3SmemBudget")
         assert ctas <= 132 and ctas % (G // gb) == 0
 
 
@@ -134,7 +134,7 @@ def test_kernels_have_no_spills_and_fit_shared_memory():
     for n, usage in funcs:
         assert re.search(r"STACK:0\b", usage) and re.search(r"LOCAL:0\b", usage), (n, usage)
         static = int(re.search(r"SHARED:(\d+)", usage).group(1)) - RESERVED
-        assert static + _budget("mnb_pk.cu", "kGc3SmemBudget") + RESERVED <= LIMIT, (n, usage)
+        assert static + budget("mnb_pk.cu", "kGc3SmemBudget") + RESERVED <= LIMIT, (n, usage)
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")

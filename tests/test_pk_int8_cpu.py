@@ -2,10 +2,6 @@
 
 * the int8 plan (mnb_pk_i8_conv_plan) covers every conv of the ResNet-18 bench models (32 x 32 and 224 x 224) inside shared
   memory and the register budget of the accumulators, and the int8 plane holds 16 channels per 16 bytes;
-* adding the element size to the plan left every bf16 plan as it was: mnb_pk_conv_plan_ex of every model conv at every
-  terms configuration of test_pk_plan_coverage_cpu.py equals the values recorded before int8 operands existed (BF16_PLANS);
-* the GPU cases of test_gpu_pk_int8.py reach every int8 plan signature (Nt, MT, phase split) of the ResNet models and launch
-  all six pk_conv_kernel<false, Nt, true> instances;
 * the int8 entry points refuse requests outside their cover on the host, before launching (the pointers are fakes that
   are never dereferenced)."""
 import ctypes as C
@@ -13,231 +9,10 @@ import ctypes as C
 import pytest
 
 from tests import pk_plan_util as PU
-from tests.test_pk_plan_cpu import _budget, _model_convs
-
-# (conv, mode, terms_a, terms_w, the 21 fields of mnb_pk_conv_plan_ex or None), recorded with the bf16-only plan
-BF16_PLANS = [
-    ('gc1x1g2', 0, 1, 1, (65536, 0, 128, 1, 1, 64, 2, 4, 151040, 128, 4, 1, 32, 2048, 4096, 1, 0, 0, 1, 1, 2048)),
-    ('gc1x1g2', 0, 2, 1, (65536, 0, 128, 1, 1, 64, 2, 4, 216576, 128, 4, 1, 32, 2048, 4096, 1, 0, 0, 2, 1, 2048)),
-    ('gc1x1g2', 0, 3, 3, (196608, 0, 128, 1, 1, 32, 4, 4, 216576, 128, 4, 1, 32, 2048, 4096, 1, 0, 0, 6, 1, 2048)),
-    ('gc1x1g2', 0, 1, 3, (221184, 0, 128, 1, 1, 48, 3, 4, 216576, 128, 4, 1, 32, 2048, 4096, 1, 0, 0, 3, 1, 2048)),
-    ('gc1x1g2', 1, 2, 1, (65536, 0, 128, 1, 1, 64, 2, 4, 216576, 128, 4, 1, 32, 2048, 4096, 1, 0, 0, 2, 1, 2048)),
-    ('gc1x1g2', 1, 2, 2, (147456, 0, 128, 1, 1, 48, 3, 4, 216576, 128, 4, 1, 32, 2048, 4096, 1, 0, 0, 3, 1, 2048)),
-    ('gc3x3g16', 0, 1, 1, (147456, 0, 32, 1, 4, 16, 1, 4, 142848, 128, 7, 1, 18, 768, 3072, 1, 0, 0, 1, 1, 192)),
-    ('gc3x3g16', 0, 2, 1, (147456, 0, 32, 1, 4, 16, 1, 4, 224768, 128, 7, 1, 18, 768, 3072, 1, 0, 0, 2, 1, 192)),
-    ('gc3x3g16', 0, 3, 3, (442368, 0, 32, 1, 4, 16, 1, 2, 153088, 128, 7, 1, 18, 768, 3072, 1, 0, 0, 6, 1, 192)),
-    ('gc3x3g16', 0, 1, 3, (442368, 0, 32, 1, 4, 16, 1, 4, 216576, 128, 7, 1, 18, 768, 3072, 1, 0, 0, 3, 1, 192)),
-    ('gc3x3g16', 1, 2, 1, (147456, 0, 16, 1, 4, 16, 2, 4, 208384, 64, 7, 1, 18, 768, 3072, 1, 0, 0, 2, 1, 192)),
-    ('gc3x3g16', 1, 2, 2, (294912, 0, 16, 1, 4, 16, 2, 4, 224768, 64, 7, 1, 18, 768, 3072, 1, 0, 0, 3, 1, 192)),
-    ('gc1x1g4', 0, 1, 1, (131072, 0, 128, 1, 1, 64, 2, 4, 151040, 128, 8, 1, 16, 512, 2048, 1, 0, 0, 1, 1, 512)),
-    ('gc1x1g4', 0, 2, 1, (131072, 0, 128, 1, 1, 64, 2, 4, 216576, 128, 8, 1, 16, 512, 2048, 1, 0, 0, 2, 1, 512)),
-    ('gc1x1g4', 0, 3, 3, (393216, 0, 128, 1, 1, 32, 4, 4, 216576, 128, 8, 1, 16, 512, 2048, 1, 0, 0, 6, 1, 512)),
-    ('gc1x1g4', 0, 1, 3, (442368, 0, 128, 1, 1, 48, 3, 4, 216576, 128, 8, 1, 16, 512, 2048, 1, 0, 0, 3, 1, 512)),
-    ('gc1x1g4', 1, 2, 1, (131072, 0, 128, 1, 1, 64, 2, 4, 216576, 128, 8, 1, 16, 512, 2048, 1, 0, 0, 2, 1, 512)),
-    ('gc1x1g4', 1, 2, 2, (294912, 0, 128, 1, 1, 48, 3, 4, 216576, 128, 8, 1, 16, 512, 2048, 1, 0, 0, 3, 1, 512)),
-    ('gc3x3g32', 0, 1, 1, (294912, 0, 32, 1, 4, 16, 1, 8, 200192, 128, 8, 1, 10, 256, 2048, 1, 0, 0, 1, 1, 64)),
-    ('gc3x3g32', 0, 2, 1, (294912, 0, 32, 1, 4, 16, 1, 4, 159232, 128, 8, 1, 10, 256, 2048, 1, 0, 0, 2, 1, 64)),
-    ('gc3x3g32', 0, 3, 3, (884736, 0, 32, 1, 4, 16, 1, 2, 134656, 128, 8, 1, 10, 256, 2048, 1, 0, 0, 6, 1, 64)),
-    ('gc3x3g32', 0, 1, 3, (884736, 0, 32, 1, 4, 16, 1, 4, 183808, 128, 8, 1, 10, 256, 2048, 1, 0, 0, 3, 1, 64)),
-    ('gc3x3g32', 1, 2, 1, (294912, 0, 16, 1, 4, 16, 2, 4, 142848, 64, 8, 1, 10, 256, 2048, 1, 0, 0, 2, 1, 64)),
-    ('gc3x3g32', 1, 2, 2, (589824, 0, 16, 1, 4, 16, 2, 4, 159232, 64, 8, 1, 10, 256, 2048, 1, 0, 0, 3, 1, 64)),
-    ('gc1x1g8', 0, 1, 1, (262144, 0, 128, 1, 1, 64, 2, 4, 151040, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 1, 1, 128)),
-    ('gc1x1g8', 0, 2, 1, (262144, 0, 128, 1, 1, 64, 2, 4, 216576, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 2, 1, 128)),
-    ('gc1x1g8', 0, 3, 3, (786432, 0, 128, 1, 1, 32, 4, 4, 216576, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 6, 1, 128)),
-    ('gc1x1g8', 0, 1, 3, (884736, 0, 128, 1, 1, 48, 3, 4, 216576, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 3, 1, 128)),
-    ('gc1x1g8', 1, 2, 1, (262144, 0, 128, 1, 1, 64, 2, 4, 216576, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 2, 1, 128)),
-    ('gc1x1g8', 1, 2, 2, (589824, 0, 128, 1, 1, 48, 3, 4, 216576, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 3, 1, 128)),
-    ('gc_head', 0, 1, 1, (33792, 0, 16, 1, 1, 176, 6, 4, 224768, 16, 8, 2, 8, 128, 128, 1, 0, 0, 1, 1, 128)),
-    ('gc_head', 0, 2, 1, (33792, 0, 16, 1, 1, 96, 11, 4, 228864, 16, 8, 2, 8, 128, 128, 1, 1, 5, 2, 1, 128)),
-    ('gc_head', 0, 3, 3, (98304, 0, 16, 1, 1, 64, 16, 2, 130560, 16, 8, 2, 8, 128, 128, 1, 1, 2, 6, 1, 128)),
-    ('gc_head', 0, 1, 3, (107520, 0, 16, 1, 1, 160, 7, 2, 132608, 16, 8, 2, 8, 128, 128, 1, 1, 2, 3, 1, 128)),
-    ('gc_head', 1, 2, 1, (32768, 0, 128, 8, 1, 16, 1, 8, 118272, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 2, 1, 128)),
-    ('gc_head', 1, 2, 2, (65536, 0, 128, 8, 1, 16, 1, 8, 151040, 128, 8, 2, 8, 128, 1024, 1, 0, 0, 3, 1, 128)),
-    ('nin1x1a', 0, 1, 1, (73728, 0, 96, 2, 1, 96, 2, 4, 192000, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 1, 1, 2048)),
-    ('nin1x1a', 0, 2, 1, (73728, 0, 96, 2, 1, 64, 3, 4, 200192, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 2, 1, 2048)),
-    ('nin1x1a', 0, 3, 3, (221184, 0, 96, 2, 1, 32, 6, 4, 192000, 96, 4, 1, 32, 2048, 4096, 1, 1, 5, 6, 1, 2048)),
-    ('nin1x1a', 0, 1, 3, (221184, 0, 96, 2, 1, 64, 3, 2, 126464, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 3, 1, 2048)),
-    ('nin1x1a', 1, 2, 1, (61440, 0, 96, 2, 1, 80, 2, 2, 132608, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 2, 1, 2048)),
-    ('nin1x1a', 1, 2, 2, (147456, 0, 96, 2, 1, 64, 3, 2, 134656, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 3, 1, 2048)),
-    ('nin1x1b', 0, 1, 1, (30720, 0, 96, 1, 1, 80, 2, 4, 163328, 96, 4, 1, 32, 2048, 2048, 1, 0, 0, 1, 1, 2048)),
-    ('nin1x1b', 0, 2, 1, (30720, 0, 96, 1, 1, 80, 2, 2, 132608, 96, 4, 1, 32, 2048, 2048, 1, 0, 0, 2, 1, 2048)),
-    ('nin1x1b', 0, 3, 3, (92160, 0, 96, 1, 1, 32, 5, 4, 192000, 96, 4, 1, 32, 2048, 2048, 1, 0, 0, 6, 1, 2048)),
-    ('nin1x1b', 0, 1, 3, (110592, 0, 96, 1, 1, 64, 3, 2, 126464, 96, 4, 1, 32, 2048, 2048, 1, 0, 0, 3, 1, 2048)),
-    ('nin1x1b', 1, 2, 1, (36864, 0, 96, 2, 1, 48, 2, 4, 155136, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 2, 1, 2048)),
-    ('nin1x1b', 1, 2, 2, (73728, 0, 96, 2, 1, 48, 2, 4, 192000, 96, 4, 1, 32, 2048, 4096, 1, 0, 0, 3, 1, 2048)),
-    ('nin5x5', 0, 1, 1, (921600, 0, 96, 2, 1, 16, 6, 2, 133632, 96, 6, 1, 20, 768, 1536, 1, 0, 0, 1, 1, 768)),
-    ('nin5x5', 0, 2, 1, (921600, 0, 96, 2, 1, 16, 6, 2, 133632, 96, 6, 1, 20, 768, 1536, 1, 1, 2, 2, 1, 768)),
-    ('nin5x5', 0, 3, 3, (2764800, 0, 96, 2, 1, 16, 6, 2, 133632, 96, 6, 1, 20, 768, 1536, 1, 1, 2, 6, 1, 768)),
-    ('nin5x5', 0, 1, 3, (2764800, 0, 96, 2, 1, 16, 6, 2, 127488, 96, 6, 1, 20, 768, 1536, 1, 1, 4, 3, 1, 768)),
-    ('nin5x5', 1, 2, 1, (921600, 0, 96, 1, 1, 16, 12, 2, 133632, 96, 6, 1, 20, 768, 768, 1, 1, 2, 2, 1, 768)),
-    ('nin5x5', 1, 2, 2, (1843200, 0, 96, 1, 1, 16, 12, 2, 133632, 96, 6, 1, 20, 768, 768, 1, 1, 3, 3, 1, 768)),
-    ('nin1x1c', 0, 1, 1, (73728, 0, 96, 2, 1, 96, 2, 4, 192000, 96, 8, 1, 16, 512, 1024, 1, 0, 0, 1, 1, 512)),
-    ('nin1x1c', 0, 2, 1, (73728, 0, 96, 2, 1, 64, 3, 4, 200192, 96, 8, 1, 16, 512, 1024, 1, 0, 0, 2, 1, 512)),
-    ('nin1x1c', 0, 3, 3, (221184, 0, 96, 2, 1, 32, 6, 4, 192000, 96, 8, 1, 16, 512, 1024, 1, 1, 5, 6, 1, 512)),
-    ('nin1x1c', 0, 1, 3, (221184, 0, 96, 2, 1, 64, 3, 2, 126464, 96, 8, 1, 16, 512, 1024, 1, 0, 0, 3, 1, 512)),
-    ('nin1x1c', 1, 2, 1, (73728, 0, 96, 2, 1, 64, 3, 4, 200192, 96, 8, 1, 16, 512, 1024, 1, 0, 0, 2, 1, 512)),
-    ('nin1x1c', 1, 2, 2, (147456, 0, 96, 2, 1, 64, 3, 2, 134656, 96, 8, 1, 16, 512, 1024, 1, 0, 0, 3, 1, 512)),
-    ('nin3x3', 0, 1, 1, (663552, 0, 96, 2, 1, 16, 12, 4, 146944, 96, 8, 1, 10, 256, 512, 1, 0, 0, 1, 1, 256)),
-    ('nin3x3', 0, 2, 1, (663552, 0, 96, 2, 1, 16, 12, 4, 159232, 96, 8, 1, 10, 256, 512, 1, 1, 3, 2, 1, 256)),
-    ('nin3x3', 0, 3, 3, (1990656, 0, 96, 2, 1, 16, 12, 2, 132608, 96, 8, 1, 10, 256, 512, 1, 1, 2, 6, 1, 256)),
-    ('nin3x3', 0, 1, 3, (1990656, 0, 96, 2, 1, 16, 12, 4, 220672, 96, 8, 1, 10, 256, 512, 1, 1, 4, 3, 1, 256)),
-    ('nin3x3', 1, 2, 1, (663552, 0, 96, 2, 1, 16, 12, 4, 159232, 96, 8, 1, 10, 256, 512, 1, 1, 3, 2, 1, 256)),
-    ('nin3x3', 1, 2, 2, (1327104, 0, 96, 2, 1, 16, 12, 2, 132608, 96, 8, 1, 10, 256, 512, 1, 1, 2, 3, 1, 256)),
-    ('nin1x1d', 0, 1, 1, (73728, 0, 96, 2, 1, 96, 2, 4, 192000, 96, 8, 2, 8, 128, 256, 1, 0, 0, 1, 1, 128)),
-    ('nin1x1d', 0, 2, 1, (73728, 0, 96, 2, 1, 64, 3, 4, 200192, 96, 8, 2, 8, 128, 256, 1, 0, 0, 2, 1, 128)),
-    ('nin1x1d', 0, 3, 3, (221184, 0, 96, 2, 1, 32, 6, 4, 192000, 96, 8, 2, 8, 128, 256, 1, 1, 5, 6, 1, 128)),
-    ('nin1x1d', 0, 1, 3, (221184, 0, 96, 2, 1, 64, 3, 2, 126464, 96, 8, 2, 8, 128, 256, 1, 0, 0, 3, 1, 128)),
-    ('nin1x1d', 1, 2, 1, (73728, 0, 96, 2, 1, 64, 3, 4, 200192, 96, 8, 2, 8, 128, 256, 1, 0, 0, 2, 1, 128)),
-    ('nin1x1d', 1, 2, 2, (147456, 0, 96, 2, 1, 64, 3, 2, 134656, 96, 8, 2, 8, 128, 256, 1, 0, 0, 3, 1, 128)),
-    ('nin_head', 0, 1, 1, (6144, 0, 16, 1, 1, 192, 1, 2, 130560, 16, 8, 2, 8, 128, 128, 1, 0, 0, 1, 1, 128)),
-    ('nin_head', 0, 2, 1, (6144, 0, 16, 1, 1, 96, 2, 4, 228864, 16, 8, 2, 8, 128, 128, 1, 0, 0, 2, 1, 128)),
-    ('nin_head', 0, 3, 3, (18432, 0, 16, 1, 1, 64, 3, 2, 130560, 16, 8, 2, 8, 128, 128, 1, 1, 2, 6, 1, 128)),
-    ('nin_head', 0, 1, 3, (18432, 0, 16, 1, 1, 96, 2, 4, 155136, 16, 8, 2, 8, 128, 128, 1, 0, 0, 3, 1, 128)),
-    ('nin_head', 1, 2, 1, (6144, 0, 96, 2, 1, 16, 1, 8, 110080, 96, 8, 2, 8, 128, 256, 1, 0, 0, 2, 1, 128)),
-    ('nin_head', 1, 2, 2, (12288, 0, 96, 2, 1, 16, 1, 8, 134656, 96, 8, 2, 8, 128, 256, 1, 0, 0, 3, 1, 128)),
-    ('res32_stem', 0, 1, 1, (18432, 0, 64, 1, 2, 16, 1, 4, 138752, 128, 7, 1, 18, 2560, 1280, 1, 0, 0, 1, 2, 1280)),
-    ('res32_stem', 0, 2, 1, (18432, 0, 64, 1, 2, 16, 1, 4, 184832, 128, 3, 1, 34, 2816, 1408, 1, 0, 0, 2, 1, 1408)),
-    ('res32_stem', 0, 3, 3, (55296, 0, 64, 1, 2, 16, 1, 2, 125440, 128, 3, 1, 34, 2816, 1408, 1, 0, 0, 6, 1, 1408)),
-    ('res32_stem', 0, 1, 3, (55296, 0, 64, 1, 2, 16, 1, 2, 129536, 128, 3, 1, 34, 2816, 1408, 1, 0, 0, 3, 1, 1408)),
-    ('res32_stem', 1, 2, 1, (18432, 0, 16, 1, 2, 32, 2, 2, 127488, 32, 3, 1, 34, 2816, 1408, 1, 1, 1, 2, 1, 1408)),
-    ('res32_stem', 1, 2, 2, (36864, 0, 16, 1, 2, 16, 4, 4, 147968, 32, 3, 1, 34, 2816, 1408, 1, 1, 2, 3, 1, 1408)),
-    ('res32_64', 0, 1, 1, (73728, 0, 64, 1, 2, 16, 4, 4, 138752, 128, 7, 1, 18, 2560, 1280, 1, 0, 0, 1, 2, 1280)),
-    ('res32_64', 0, 2, 1, (73728, 0, 64, 1, 2, 16, 4, 4, 184832, 128, 3, 1, 34, 2816, 1408, 1, 1, 3, 2, 1, 1408)),
-    ('res32_64', 0, 3, 3, (221184, 0, 64, 1, 2, 16, 4, 2, 125440, 128, 3, 1, 34, 2816, 1408, 1, 1, 3, 6, 1, 1408)),
-    ('res32_64', 0, 1, 3, (221184, 0, 64, 1, 2, 16, 4, 2, 129536, 128, 3, 1, 34, 2816, 1408, 1, 1, 3, 3, 1, 1408)),
-    ('res32_64', 1, 2, 1, (73728, 0, 64, 1, 2, 16, 4, 4, 184832, 128, 3, 1, 34, 2816, 1408, 1, 1, 3, 2, 1, 1408)),
-    ('res32_64', 1, 2, 2, (147456, 0, 64, 1, 2, 16, 4, 2, 131584, 128, 3, 1, 34, 2816, 1408, 1, 1, 2, 3, 1, 1408)),
-    ('res32_128_s2', 0, 1, 1, (147456, 0, 128, 1, 1, 32, 2, 4, 187904, 128, 7, 1, 17, 768, 768, 1, 0, 0, 1, 1, 768)),
-    ('res32_128_s2', 0, 2, 1, (147456, 0, 128, 1, 1, 32, 2, 4, 220672, 128, 7, 1, 17, 768, 768, 1, 1, 4, 2, 1, 768)),
-    ('res32_128_s2', 0, 3, 3, (442368, 0, 128, 1, 1, 16, 4, 4, 220672, 128, 7, 1, 17, 768, 768, 1, 1, 3, 6, 1, 768)),
-    ('res32_128_s2', 0, 1, 3, (442368, 0, 128, 1, 1, 16, 4, 2, 128512, 128, 7, 1, 17, 768, 768, 1, 1, 5, 3, 1, 768)),
-    ('res32_128_s2', 1, 2, 1, (147456, 0, 64, 1, 2, 32, 4, 4, 224768, 128, 7, 1, 17, 768, 384, 4, 0, 0, 2, 1, 384)),
-    ('res32_128_s2', 1, 2, 2, (294912, 0, 64, 1, 2, 16, 8, 4, 155136, 128, 7, 1, 17, 768, 384, 4, 1, 5, 3, 1, 384)),
-    ('res32_128_sc', 0, 1, 1, (16384, 0, 128, 1, 1, 64, 1, 4, 151040, 128, 8, 1, 16, 512, 512, 1, 0, 0, 1, 1, 512)),
-    ('res32_128_sc', 0, 2, 1, (16384, 0, 128, 1, 1, 64, 1, 4, 216576, 128, 8, 1, 16, 512, 512, 1, 0, 0, 2, 1, 512)),
-    ('res32_128_sc', 0, 3, 3, (49152, 0, 128, 1, 1, 32, 2, 4, 216576, 128, 8, 1, 16, 512, 512, 1, 0, 0, 6, 1, 512)),
-    ('res32_128_sc', 0, 1, 3, (49152, 0, 128, 1, 1, 32, 2, 4, 151040, 128, 8, 1, 16, 512, 512, 1, 0, 0, 3, 1, 512)),
-    ('res32_128_sc', 1, 2, 1, (18432, 0, 64, 1, 2, 48, 3, 2, 130560, 128, 8, 1, 16, 512, 256, 4, 0, 0, 2, 1, 256)),
-    ('res32_128_sc', 1, 2, 2, (32768, 0, 64, 1, 2, 32, 4, 4, 183808, 128, 8, 1, 16, 512, 256, 4, 0, 0, 3, 1, 256)),
-    ('res32_128', 0, 1, 1, (294912, 0, 128, 1, 1, 16, 8, 4, 192000, 128, 7, 1, 18, 768, 768, 1, 0, 0, 1, 1, 768)),
-    ('res32_128', 0, 2, 1, (294912, 0, 128, 1, 1, 16, 8, 4, 212480, 128, 7, 1, 18, 768, 768, 1, 1, 3, 2, 1, 768)),
-    ('res32_128', 0, 3, 3, (884736, 0, 128, 1, 1, 16, 8, 2, 126464, 128, 7, 1, 18, 768, 768, 1, 1, 3, 6, 1, 768)),
-    ('res32_128', 0, 1, 3, (884736, 0, 128, 1, 1, 16, 8, 2, 130560, 128, 7, 1, 18, 768, 768, 1, 1, 5, 3, 1, 768)),
-    ('res32_128', 1, 2, 1, (294912, 0, 128, 1, 1, 16, 8, 4, 212480, 128, 7, 1, 18, 768, 768, 1, 1, 3, 2, 1, 768)),
-    ('res32_128', 1, 2, 2, (589824, 0, 128, 1, 1, 16, 8, 4, 228864, 128, 7, 1, 18, 768, 768, 1, 1, 4, 3, 1, 768)),
-    ('res32_256_s2', 0, 1, 1, (663552, 0, 128, 2, 1, 48, 3, 2, 134656, 128, 8, 1, 9, 256, 512, 1, 0, 0, 1, 1, 256)),
-    ('res32_256_s2', 0, 2, 1, (589824, 0, 128, 2, 1, 32, 4, 4, 196096, 128, 8, 1, 9, 256, 512, 1, 1, 4, 2, 1, 256)),
-    ('res32_256_s2', 0, 3, 3, (1769472, 0, 128, 2, 1, 16, 8, 2, 134656, 128, 8, 1, 9, 256, 512, 1, 1, 2, 6, 1, 256)),
-    ('res32_256_s2', 0, 1, 3, (1769472, 0, 128, 2, 1, 16, 8, 4, 228864, 128, 8, 1, 9, 256, 512, 1, 1, 5, 3, 1, 256)),
-    ('res32_256_s2', 1, 2, 1, (589824, 0, 128, 1, 1, 32, 8, 4, 196096, 128, 8, 1, 9, 256, 256, 4, 1, 4, 2, 1, 256)),
-    ('res32_256_s2', 1, 2, 2, (1179648, 0, 128, 1, 1, 16, 16, 4, 175616, 128, 8, 1, 9, 256, 256, 4, 1, 5, 3, 1, 256)),
-    ('res32_256_sc', 0, 1, 1, (65536, 0, 128, 2, 1, 64, 2, 4, 151040, 128, 8, 2, 8, 128, 256, 1, 0, 0, 1, 1, 128)),
-    ('res32_256_sc', 0, 2, 1, (65536, 0, 128, 2, 1, 64, 2, 4, 216576, 128, 8, 2, 8, 128, 256, 1, 0, 0, 2, 1, 128)),
-    ('res32_256_sc', 0, 3, 3, (196608, 0, 128, 2, 1, 32, 4, 4, 216576, 128, 8, 2, 8, 128, 256, 1, 0, 0, 6, 1, 128)),
-    ('res32_256_sc', 0, 1, 3, (221184, 0, 128, 2, 1, 48, 3, 4, 216576, 128, 8, 2, 8, 128, 256, 1, 0, 0, 3, 1, 128)),
-    ('res32_256_sc', 1, 2, 1, (65536, 0, 128, 1, 1, 64, 4, 4, 216576, 128, 8, 2, 8, 128, 128, 4, 0, 0, 2, 1, 128)),
-    ('res32_256_sc', 1, 2, 2, (147456, 0, 128, 1, 1, 48, 6, 4, 216576, 128, 8, 2, 8, 128, 128, 4, 0, 0, 3, 1, 128)),
-    ('res32_256', 0, 1, 1, (1179648, 0, 128, 2, 1, 16, 16, 4, 183808, 128, 8, 1, 10, 256, 512, 1, 0, 0, 1, 1, 256)),
-    ('res32_256', 0, 2, 1, (1179648, 0, 128, 2, 1, 16, 16, 4, 196096, 128, 8, 1, 10, 256, 512, 1, 1, 3, 2, 1, 256)),
-    ('res32_256', 0, 3, 3, (3538944, 0, 128, 2, 1, 16, 16, 4, 208384, 128, 8, 1, 10, 256, 512, 1, 1, 3, 6, 1, 256)),
-    ('res32_256', 0, 1, 3, (3538944, 0, 128, 2, 1, 16, 16, 2, 126464, 128, 8, 1, 10, 256, 512, 1, 1, 5, 3, 1, 256)),
-    ('res32_256', 1, 2, 1, (1179648, 0, 128, 2, 1, 16, 16, 4, 196096, 128, 8, 1, 10, 256, 512, 1, 1, 3, 2, 1, 256)),
-    ('res32_256', 1, 2, 2, (2359296, 0, 128, 2, 1, 16, 16, 2, 132608, 128, 8, 1, 10, 256, 512, 1, 1, 3, 3, 1, 256)),
-    ('res32_512_s2', 0, 1, 1, (2359296, 0, 128, 4, 1, 32, 8, 4, 183808, 128, 4, 5, 5, 52, 208, 1, 0, 0, 1, 1, 52)),
-    ('res32_512_s2', 0, 2, 1, (2359296, 0, 128, 4, 1, 32, 8, 4, 216576, 128, 4, 5, 5, 52, 208, 1, 1, 4, 2, 1, 52)),
-    ('res32_512_s2', 0, 3, 3, (7077888, 0, 128, 4, 1, 16, 16, 4, 216576, 128, 4, 5, 5, 52, 208, 1, 1, 3, 6, 1, 52)),
-    ('res32_512_s2', 0, 1, 3, (7077888, 0, 128, 4, 1, 16, 16, 2, 126464, 128, 4, 5, 5, 52, 208, 1, 1, 5, 3, 1, 52)),
-    ('res32_512_s2', 1, 2, 1, (2359296, 0, 128, 2, 1, 32, 16, 4, 216576, 128, 4, 5, 5, 52, 104, 4, 1, 4, 2, 1, 52)),
-    ('res32_512_s2', 1, 2, 2, (4718592, 0, 128, 2, 1, 16, 32, 4, 183808, 128, 4, 5, 5, 52, 104, 4, 1, 5, 3, 1, 52)),
-    ('res32_512_sc', 0, 1, 1, (294912, 0, 128, 4, 1, 96, 3, 4, 216576, 128, 4, 8, 4, 32, 128, 1, 0, 0, 1, 1, 32)),
-    ('res32_512_sc', 0, 2, 1, (262144, 0, 128, 4, 1, 64, 4, 4, 216576, 128, 4, 8, 4, 32, 128, 1, 0, 0, 2, 1, 32)),
-    ('res32_512_sc', 0, 3, 3, (786432, 0, 128, 4, 1, 32, 8, 4, 216576, 128, 4, 8, 4, 32, 128, 1, 1, 5, 6, 1, 32)),
-    ('res32_512_sc', 0, 1, 3, (884736, 0, 128, 4, 1, 48, 6, 4, 216576, 128, 4, 8, 4, 32, 128, 1, 0, 0, 3, 1, 32)),
-    ('res32_512_sc', 1, 2, 1, (262144, 0, 128, 2, 1, 64, 8, 4, 216576, 128, 4, 8, 4, 32, 64, 4, 0, 0, 2, 1, 32)),
-    ('res32_512_sc', 1, 2, 2, (540672, 0, 128, 2, 1, 48, 11, 4, 216576, 128, 4, 8, 4, 32, 64, 4, 1, 7, 3, 1, 32)),
-    ('res32_512', 0, 1, 1, (4718592, 0, 128, 4, 1, 16, 32, 4, 183808, 128, 4, 3, 6, 86, 344, 1, 0, 0, 1, 1, 86)),
-    ('res32_512', 0, 2, 1, (4718592, 0, 128, 4, 1, 16, 32, 4, 196096, 128, 4, 3, 6, 86, 344, 1, 1, 3, 2, 1, 86)),
-    ('res32_512', 0, 3, 3, (14155776, 0, 128, 4, 1, 16, 32, 4, 212480, 128, 4, 3, 6, 86, 344, 1, 1, 3, 6, 1, 86)),
-    ('res32_512', 0, 1, 3, (14155776, 0, 128, 4, 1, 16, 32, 2, 126464, 128, 4, 3, 6, 86, 344, 1, 1, 5, 3, 1, 86)),
-    ('res32_512', 1, 2, 1, (4718592, 0, 128, 4, 1, 16, 32, 4, 196096, 128, 4, 3, 6, 86, 344, 1, 1, 3, 2, 1, 86)),
-    ('res32_512', 1, 2, 2, (9437184, 0, 128, 4, 1, 16, 32, 2, 132608, 128, 4, 3, 6, 86, 344, 1, 1, 3, 3, 1, 86)),
-    ('res224_stem', 0, 1, 1, (18432, 0, 64, 1, 2, 16, 1, 4, 143872, 128, 4, 1, 30, 28672, 14336, 1, 0, 0, 1, 8, 14336)),
-    ('res224_stem', 0, 2, 1, (18432, 0, 64, 1, 2, 16, 1, 4, 188928, 128, 4, 1, 30, 28672, 14336, 1, 0, 0, 2, 8, 14336)),
-    ('res224_stem', 0, 3, 3, (55296, 0, 64, 1, 2, 16, 1, 2, 127488, 128, 4, 1, 30, 28672, 14336, 1, 0, 0, 6, 8, 14336)),
-    ('res224_stem', 0, 1, 3, (55296, 0, 64, 1, 2, 16, 1, 2, 131584, 128, 4, 1, 30, 28672, 14336, 1, 0, 0, 3, 8, 14336)),
-    ('res224_stem', 1, 2, 1, (18432, 0, 16, 1, 4, 16, 4, 4, 225792, 64, 4, 1, 30, 28672, 7168, 1, 1, 3, 2, 8, 7168)),
-    ('res224_stem', 1, 2, 2, (36864, 0, 16, 1, 4, 16, 4, 2, 131584, 64, 4, 1, 30, 28672, 7168, 1, 1, 2, 3, 8, 7168)),
-    ('res224_64', 0, 1, 1, (73728, 0, 64, 1, 2, 16, 4, 4, 143872, 128, 4, 1, 30, 28672, 14336, 1, 0, 0, 1, 8, 14336)),
-    ('res224_64', 0, 2, 1, (73728, 0, 64, 1, 2, 16, 4, 4, 188928, 128, 4, 1, 30, 28672, 14336, 1, 1, 3, 2, 8, 14336)),
-    ('res224_64', 0, 3, 3, (221184, 0, 64, 1, 2, 16, 4, 2, 127488, 128, 4, 1, 30, 28672, 14336, 1, 1, 3, 6, 8, 14336)),
-    ('res224_64', 0, 1, 3, (221184, 0, 64, 1, 2, 16, 4, 2, 131584, 128, 4, 1, 30, 28672, 14336, 1, 1, 3, 3, 8, 14336)),
-    ('res224_64', 1, 2, 1, (73728, 0, 64, 1, 2, 16, 4, 4, 188928, 128, 4, 1, 30, 28672, 14336, 1, 1, 3, 2, 8, 14336)),
-    ('res224_64', 1, 2, 2, (147456, 0, 64, 1, 2, 16, 4, 2, 133632, 128, 4, 1, 30, 28672, 14336, 1, 1, 2, 3, 8, 14336)),
-    ('res224_128_s2', 0, 1, 1, (147456, 0, 128, 1, 1, 32, 2, 4, 197120, 128, 2, 1, 57, 7168, 7168, 1, 0, 0, 1, 2, 7168)),
-    ('res224_128_s2', 0, 2, 1, (147456, 0, 128, 1, 1, 16, 4, 4, 147968, 128, 1, 1, 113, 7168, 7168, 1, 1, 8, 2, 1, 7168)),
-    ('res224_128_s2', 0, 3, 3, (442368, 0, 128, 1, 1, 16, 4, 4, 209408, 128, 1, 1, 113, 7168, 7168, 1, 1, 5, 6, 1, 7168)),
-    ('res224_128_s2', 0, 1, 3, (442368, 0, 128, 1, 1, 16, 4, 2, 135680, 128, 1, 1, 113, 7168, 7168, 1, 1, 5, 3, 1, 7168)),
-    ('res224_128_s2', 1, 2, 1, (147456, 0, 64, 1, 2, 16, 8, 4, 172544, 128, 1, 1, 113, 7168, 3584, 4, 0, 0, 2, 1, 3584)),
-    ('res224_128_s2', 1, 2, 2, (294912, 0, 64, 1, 2, 16, 8, 4, 205312, 128, 1, 1, 113, 7168, 3584, 4, 1, 5, 3, 1, 3584)),
-    ('res224_128_sc', 0, 1, 1, (16384, 0, 128, 1, 1, 64, 1, 4, 142848, 128, 1, 1, 112, 7168, 7168, 1, 0, 0, 1, 1, 7168)),
-    ('res224_128_sc', 0, 2, 1, (16384, 0, 128, 1, 1, 64, 1, 4, 200192, 128, 1, 1, 112, 7168, 7168, 1, 0, 0, 2, 1, 7168)),
-    ('res224_128_sc', 0, 3, 3, (49152, 0, 128, 1, 1, 32, 2, 4, 204288, 128, 1, 1, 112, 7168, 7168, 1, 0, 0, 6, 1, 7168)),
-    ('res224_128_sc', 0, 1, 3, (49152, 0, 128, 1, 1, 32, 2, 4, 146944, 128, 1, 1, 112, 7168, 7168, 1, 0, 0, 3, 1, 7168)),
-    ('res224_128_sc', 1, 2, 1, (18432, 0, 64, 1, 2, 48, 3, 4, 216576, 128, 1, 1, 112, 7168, 3584, 4, 0, 0, 2, 1, 3584)),
-    ('res224_128_sc', 1, 2, 2, (36864, 0, 64, 1, 2, 48, 3, 2, 130560, 128, 1, 1, 112, 7168, 3584, 4, 0, 0, 3, 1, 3584)),
-    ('res224_128', 0, 1, 1, (294912, 0, 128, 1, 1, 16, 8, 4, 193024, 128, 4, 1, 30, 7168, 7168, 1, 0, 0, 1, 4, 7168)),
-    ('res224_128', 0, 2, 1, (294912, 0, 128, 1, 1, 16, 8, 4, 217600, 128, 4, 1, 30, 7168, 7168, 1, 1, 3, 2, 4, 7168)),
-    ('res224_128', 0, 3, 3, (884736, 0, 128, 1, 1, 16, 8, 2, 129536, 128, 4, 1, 30, 7168, 7168, 1, 1, 3, 6, 4, 7168)),
-    ('res224_128', 0, 1, 3, (884736, 0, 128, 1, 1, 16, 8, 2, 131584, 128, 4, 1, 30, 7168, 7168, 1, 1, 5, 3, 4, 7168)),
-    ('res224_128', 1, 2, 1, (294912, 0, 128, 1, 1, 16, 8, 4, 217600, 128, 4, 1, 30, 7168, 7168, 1, 1, 3, 2, 4, 7168)),
-    ('res224_128', 1, 2, 2, (589824, 0, 128, 1, 1, 16, 8, 2, 127488, 128, 4, 1, 30, 7168, 7168, 1, 1, 4, 3, 4, 7168)),
-    ('res224_256_s2', 0, 1, 1, (589824, 0, 128, 2, 1, 32, 4, 4, 197120, 128, 2, 1, 57, 1792, 3584, 1, 0, 0, 1, 1, 1792)),
-    ('res224_256_s2', 0, 2, 1, (589824, 0, 128, 2, 1, 32, 4, 2, 131584, 128, 2, 1, 57, 1792, 3584, 1, 1, 4, 2, 1, 1792)),
-    ('res224_256_s2', 0, 3, 3, (1769472, 0, 128, 2, 1, 16, 8, 2, 129536, 128, 2, 1, 57, 1792, 3584, 1, 1, 3, 6, 1, 1792)),
-    ('res224_256_s2', 0, 1, 3, (1769472, 0, 128, 2, 1, 16, 8, 2, 131584, 128, 2, 1, 57, 1792, 3584, 1, 1, 5, 3, 1, 1792)),
-    ('res224_256_s2', 1, 2, 1, (589824, 0, 128, 1, 1, 32, 8, 2, 131584, 128, 2, 1, 57, 1792, 1792, 4, 1, 4, 2, 1, 1792)),
-    ('res224_256_s2', 1, 2, 2, (1179648, 0, 128, 1, 1, 16, 16, 4, 197120, 128, 2, 1, 57, 1792, 1792, 4, 1, 5, 3, 1, 1792)),
-    ('res224_256_sc', 0, 1, 1, (65536, 0, 128, 2, 1, 64, 2, 4, 142848, 128, 2, 1, 56, 1792, 3584, 1, 0, 0, 1, 1, 1792)),
-    ('res224_256_sc', 0, 2, 1, (65536, 0, 128, 2, 1, 64, 2, 4, 200192, 128, 2, 1, 56, 1792, 3584, 1, 0, 0, 2, 1, 1792)),
-    ('res224_256_sc', 0, 3, 3, (196608, 0, 128, 2, 1, 32, 4, 4, 204288, 128, 2, 1, 56, 1792, 3584, 1, 0, 0, 6, 1, 1792)),
-    ('res224_256_sc', 0, 1, 3, (221184, 0, 128, 2, 1, 48, 3, 4, 212480, 128, 2, 1, 56, 1792, 3584, 1, 0, 0, 3, 1, 1792)),
-    ('res224_256_sc', 1, 2, 1, (65536, 0, 128, 1, 1, 64, 4, 4, 200192, 128, 2, 1, 56, 1792, 1792, 4, 0, 0, 2, 1, 1792)),
-    ('res224_256_sc', 1, 2, 2, (147456, 0, 128, 1, 1, 48, 6, 4, 204288, 128, 2, 1, 56, 1792, 1792, 4, 0, 0, 3, 1, 1792)),
-    ('res224_256', 0, 1, 1, (1179648, 0, 128, 2, 1, 16, 16, 4, 193024, 128, 4, 1, 30, 1792, 3584, 1, 0, 0, 1, 2, 1792)),
-    ('res224_256', 0, 2, 1, (1179648, 0, 128, 2, 1, 16, 16, 2, 125440, 128, 2, 1, 58, 1792, 3584, 1, 1, 3, 2, 1, 1792)),
-    ('res224_256', 0, 3, 3, (3538944, 0, 128, 2, 1, 16, 16, 4, 209408, 128, 2, 1, 58, 1792, 3584, 1, 1, 5, 6, 1, 1792)),
-    ('res224_256', 0, 1, 3, (3538944, 0, 128, 2, 1, 16, 16, 2, 135680, 128, 2, 1, 58, 1792, 3584, 1, 1, 5, 3, 1, 1792)),
-    ('res224_256', 1, 2, 1, (1179648, 0, 128, 2, 1, 16, 16, 2, 125440, 128, 2, 1, 58, 1792, 3584, 1, 1, 3, 2, 1, 1792)),
-    ('res224_256', 1, 2, 2, (2359296, 0, 128, 2, 1, 16, 16, 2, 133632, 128, 2, 1, 58, 1792, 3584, 1, 1, 4, 3, 1, 1792)),
-    ('res224_512_s2', 0, 1, 1, (2359296, 0, 128, 4, 1, 32, 8, 4, 192000, 128, 4, 1, 29, 448, 1792, 1, 0, 0, 1, 1, 448)),
-    ('res224_512_s2', 0, 2, 1, (2359296, 0, 128, 4, 1, 32, 8, 4, 228864, 128, 4, 1, 29, 448, 1792, 1, 1, 4, 2, 1, 448)),
-    ('res224_512_s2', 0, 3, 3, (7077888, 0, 128, 4, 1, 16, 16, 4, 224768, 128, 4, 1, 29, 448, 1792, 1, 1, 3, 6, 1, 448)),
-    ('res224_512_s2', 0, 1, 3, (7077888, 0, 128, 4, 1, 16, 16, 2, 128512, 128, 4, 1, 29, 448, 1792, 1, 1, 5, 3, 1, 448)),
-    ('res224_512_s2', 1, 2, 1, (2359296, 0, 128, 2, 1, 32, 16, 4, 228864, 128, 4, 1, 29, 448, 896, 4, 1, 4, 2, 1, 448)),
-    ('res224_512_s2', 1, 2, 2, (4718592, 0, 128, 2, 1, 16, 32, 4, 192000, 128, 4, 1, 29, 448, 896, 4, 1, 5, 3, 1, 448)),
-    ('res224_512_sc', 0, 1, 1, (294912, 0, 128, 4, 1, 96, 3, 4, 204288, 128, 4, 1, 28, 448, 1792, 1, 0, 0, 1, 1, 448)),
-    ('res224_512_sc', 0, 2, 1, (262144, 0, 128, 4, 1, 64, 4, 4, 200192, 128, 4, 1, 28, 448, 1792, 1, 0, 0, 2, 1, 448)),
-    ('res224_512_sc', 0, 3, 3, (786432, 0, 128, 4, 1, 32, 8, 4, 204288, 128, 4, 1, 28, 448, 1792, 1, 1, 5, 6, 1, 448)),
-    ('res224_512_sc', 0, 1, 3, (884736, 0, 128, 4, 1, 48, 6, 4, 212480, 128, 4, 1, 28, 448, 1792, 1, 0, 0, 3, 1, 448)),
-    ('res224_512_sc', 1, 2, 1, (286720, 0, 128, 2, 1, 80, 7, 2, 132608, 128, 4, 1, 28, 448, 896, 4, 0, 0, 2, 1, 448)),
-    ('res224_512_sc', 1, 2, 2, (540672, 0, 128, 2, 1, 48, 11, 4, 204288, 128, 4, 1, 28, 448, 896, 4, 1, 7, 3, 1, 448)),
-    ('res224_512', 0, 1, 1, (4718592, 0, 128, 4, 1, 16, 32, 4, 193024, 128, 4, 1, 30, 448, 1792, 1, 0, 0, 1, 1, 448)),
-    ('res224_512', 0, 2, 1, (4718592, 0, 128, 4, 1, 16, 32, 4, 217600, 128, 4, 1, 30, 448, 1792, 1, 1, 3, 2, 1, 448)),
-    ('res224_512', 0, 3, 3, (14155776, 0, 128, 4, 1, 16, 32, 2, 129536, 128, 4, 1, 30, 448, 1792, 1, 1, 3, 6, 1, 448)),
-    ('res224_512', 0, 1, 3, (14155776, 0, 128, 4, 1, 16, 32, 2, 131584, 128, 4, 1, 30, 448, 1792, 1, 1, 5, 3, 1, 448)),
-    ('res224_512', 1, 2, 1, (4718592, 0, 128, 4, 1, 16, 32, 4, 217600, 128, 4, 1, 30, 448, 1792, 1, 1, 3, 2, 1, 448)),
-    ('res224_512', 1, 2, 2, (9437184, 0, 128, 4, 1, 16, 32, 2, 127488, 128, 4, 1, 30, 448, 1792, 1, 1, 4, 3, 1, 448)),
-]
-
-
-def _i8_plan(sh):
-    from micronet_b200 import pk as PK
-    p = PK.i8_plan(sh)
-    return None if p is None else dict(zip(PU.CONV_FIELDS, p))
 
 
 def _resnet_convs():
-    return [c for c in _model_convs() if c[0].startswith(("res32_", "res224_"))]
+    return [c for c in PU.model_convs() if c[0].startswith(("res32_", "res224_"))]
 
 
 @pytest.mark.parametrize("conv", _resnet_convs(), ids=lambda c: c[0])
@@ -246,9 +21,9 @@ def test_int8_plan_covers_the_resnet_convs(conv):
     lib = L.load()
     name, B, Cc, H, W, K, R, st, pad, G = conv
     sh = PU.shape(B, Cc, H, W, K, R, st, pad, G)
-    p = _i8_plan(sh)
+    p = PU.i8_plan(sh)
     assert p is not None, (name, lib.mnb_last_error())
-    assert 0 < p["smem"] <= _budget("mnb_pk.cu", "kSmemBudget"), (name, p)
+    assert 0 < p["smem"] <= PU.budget("mnb_pk.cu", "kSmemBudget"), (name, p)
     assert p["acc"] == p["MT"] * p["Nt"] and p["acc"] <= 128 and p["Nt"] in PU.CONV_NT, (name, p)
     assert p["segmented"] == 0 and p["npairs"] == 1 and p["ny"] == 1 and p["CC"] % 32 == 0, (name, p)
     assert 1 <= p["n_items"] < (1 << 22) and p["n_mtiles"] < (1 << 22), (name, p)
@@ -258,40 +33,6 @@ def test_int8_plan_covers_the_resnet_convs(conv):
     assert int(lib.mnb_pk_i8_act_bytes(B, Cc, H, W)) == B * ((Cc + 15) // 16) * H * W * 16
     if Cc % 16 == 0:
         assert 2 * int(lib.mnb_pk_i8_act_bytes(B, Cc, H, W)) == int(lib.mnb_pk_act_bytes(B, Cc, H, W, 1))
-
-
-def test_bf16_plans_are_unchanged():
-    convs = {c[0]: c for c in _model_convs()}
-    assert len(BF16_PLANS) == 6 * len(convs)
-    changed = []
-    for name, mode, ta, tw, want in BF16_PLANS:
-        _, B, Cc, H, W, K, R, st, pad, G = convs[name]
-        p = PU.conv_plan(PU.shape(B, Cc, H, W, K, R, st, pad, G), mode, ta, tw)
-        got = None if p is None else tuple(p[f] for f in PU.CONV_FIELDS)
-        if got != want:
-            changed.append((name, mode, ta, tw, want, got))
-    assert not changed, changed[:4]
-
-
-def _i8_signature(p, stride):
-    return (p["Nt"], p["MT"], stride == 2)
-
-
-def test_gpu_cases_cover_the_int8_plans_of_the_models():
-    from tests import test_gpu_pk_int8 as T
-    model = {}
-    for name, B, Cc, H, W, K, R, st, pad, G in _resnet_convs():
-        p = _i8_plan(PU.shape(B, Cc, H, W, K, R, st, pad, G))
-        model.setdefault(_i8_signature(p, st), []).append(name)
-    tested, nts = set(), set()
-    for case in T.CASES:
-        p = T.plan_of(case)
-        assert p is not None, case.id
-        tested.add(_i8_signature(p, case.shape[6]))
-        nts.add(p["Nt"])
-    missing = {sig: model[sig] for sig in model if sig not in tested}
-    assert not missing, f"int8 plans (Nt, MT, phase split) of the ResNet models no GPU case runs: {missing}"
-    assert nts == set(PU.CONV_NT), f"pk_conv_kernel<false, Nt, true> instances no GPU case launches: {set(PU.CONV_NT) - nts}"
 
 
 def test_int8_entry_points_refuse_before_launching():
@@ -311,7 +52,7 @@ def test_int8_entry_points_refuse_before_launching():
         assert rc == L.E_UNSUPPORTED and b"symmetric" in lib.mnb_last_error(), rc
     # grouped convs: GEMM-K channels per group must be a multiple of 16 (one 16-byte unit)
     g8 = PU.shape(2, 32, 8, 8, 32, 3, 1, 1, 4)
-    assert PU.conv_plan(g8, 0, 1, 1) is not None and _i8_plan(g8) is None
+    assert PU.conv_plan(g8, 0, 1, 1) is not None and PU.i8_plan(g8) is None
     assert lib.mnb_pk_i8_wimage_bytes(C.byref(g8)) == -1
     rc = lib.mnb_pk_i8_conv(C.byref(g8), fake, fake, None, None, 1.0, None, fake, None, fake, None)
     assert rc == L.E_UNSUPPORTED and b"% 16" in lib.mnb_last_error()

@@ -7,16 +7,13 @@
   `mnb_pk_act_bytes`) covers every convolution of the BASELINE.json models at their bench shapes, inside shared memory and the
   register budget of the accumulators."""
 import ctypes as C
-import os
 import re
 import shutil
 import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIMIT = 227 * 1024          # opt-in shared memory per block on sm_90 (H100)
-RESERVED = 1024             # per-block reservation that cuobjdump's SHARED figure includes
+from tests.pk_plan_util import LIMIT, RESERVED, budget, model_convs
 
 # kernel (mangled-name fragment) -> (source file, name of its dynamic shared-memory budget constant)
 BUDGETS = {
@@ -27,13 +24,6 @@ BUDGETS = {
     "tcfp3210fwd_kernel": ("mnb_conv_fp32_tc.cu", "kMaxDynSmem"),
     "tcfp3212wgrad_kernel": ("mnb_conv_fp32_tc.cu", "kMaxDynSmem"),
 }
-
-
-def _budget(src, name):
-    text = open(os.path.join(ROOT, "micronet_b200", "csrc", src)).read()
-    m = re.search(r"constexpr int %s = ([0-9*+\- ]+);" % name, text)
-    assert m, (src, name)
-    return int(eval(m.group(1)))      # e.g. "227 * 1024 - 3072"
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
@@ -49,38 +39,14 @@ def test_static_plus_dynamic_shared_memory_fits_the_block_limit():
         for frag, (src, const) in BUDGETS.items():
             if frag in name:
                 seen.add(frag)
-                dyn = _budget(src, const)
+                dyn = budget(src, const)
                 assert static + dyn <= LIMIT, f"{name}: static {static} + dynamic budget {dyn} > {LIMIT}"
         regs = re.search(r"REG:(\d+)", usage)
         assert regs and int(regs.group(1)) <= 255
     assert seen == set(BUDGETS), f"kernels not found in the library: {set(BUDGETS) - seen}"
 
 
-def _model_convs():
-    """(name, B, C, H, W, K, R, stride, pad, groups) of every conv of the bench models (harness/models.py)"""
-    out = []
-    B = 256
-    gc = [("gc1x1g2", 256, 32, 256, 1, 1, 0, 2), ("gc3x3g16", 256, 16, 512, 3, 1, 1, 16), ("gc1x1g4", 512, 16, 512, 1, 1, 0, 4),
-          ("gc3x3g32", 512, 8, 1024, 3, 1, 1, 32), ("gc1x1g8", 1024, 8, 1024, 1, 1, 0, 8), ("gc_head", 1024, 8, 10, 1, 1, 0, 1)]
-    nin = [("nin1x1a", 192, 32, 160, 1, 1, 0, 1), ("nin1x1b", 160, 32, 96, 1, 1, 0, 1), ("nin5x5", 96, 16, 192, 5, 1, 2, 1),
-           ("nin1x1c", 192, 16, 192, 1, 1, 0, 1), ("nin3x3", 192, 8, 192, 3, 1, 1, 1), ("nin1x1d", 192, 8, 192, 1, 1, 0, 1),
-           ("nin_head", 192, 8, 10, 1, 1, 0, 1)]
-    for n, c, h, k, r, st, p, g in gc + nin:
-        out.append((n, B, c, h, h, k, r, st, p, g))
-    for hw, b, tag in ((32, 256, "res32"), (224, 64, "res224")):
-        c, h = 64, hw
-        out.append((f"{tag}_stem", b, 3, h, h, 64, 3, 1, 1, 1))
-        for width in (64, 128, 256, 512):
-            if width != 64:
-                out.append((f"{tag}_{width}_s2", b, c, h, h, width, 3, 2, 1, 1))
-                out.append((f"{tag}_{width}_sc", b, c, h, h, width, 1, 2, 0, 1))
-                h //= 2
-            out.append((f"{tag}_{width}", b, width, h, h, width, 3, 1, 1, 1))
-            c = width
-    return out
-
-
-@pytest.mark.parametrize("conv", _model_convs(), ids=lambda c: c[0])
+@pytest.mark.parametrize("conv", model_convs(), ids=lambda c: c[0])
 def test_packed_operand_plan_covers_the_bench_models(conv):
     from micronet_b200 import _lib as L
     lib = L.load()
@@ -95,7 +61,7 @@ def test_packed_operand_plan_covers_the_bench_models(conv):
         plan = (C.c_int32 * 16)()
         assert lib.mnb_pk_conv_plan(C.byref(sh), mode, ta, tw, plan) == 0, (name, mode, ta, tw, lib.mnb_last_error())
         p = dict(zip(names, list(plan)[2:]))
-        assert 0 < p["smem"] <= _budget("mnb_pk.cu", "kSmemBudget"), (name, p)
+        assert 0 < p["smem"] <= budget("mnb_pk.cu", "kSmemBudget"), (name, p)
         # accumulators of one thread: MT x Nt / 2 registers (two warpgroups of 64 rows each)
         assert p["acc"] == p["MT"] * p["Nt"] and p["acc"] <= 128, (name, p)
         assert p["nstage"] in (2, 4, 8) and p["Nt"] % 16 == 0 and p["Nt"] <= 128 and p["CC"] % 16 == 0, (name, p)

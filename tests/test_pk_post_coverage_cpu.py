@@ -9,38 +9,21 @@ of pk_conv_kernel - and the plan.  This test requires
 * every refusal reason the host can reach to be listed, with the code and text of the query;
 * every linked conv of the frozen graphs at the batch the benchmark runs them to be a case,
 
-so deleting a case, or a change of the plan heuristics that moves a case elsewhere, fails here naming what lost its cover."""
-import os
-
+so deleting a case, or a change of the plan heuristics that moves a case elsewhere, fails here naming what lost its cover.
+mnb_pk_conv_post also refuses a segmented producer plan on the host, before launching."""
 import pytest
 
 from tests import pk_post_cases as P
+from tests import pk_plan_util as PU
 
 E_ARG = -1
-
-
-class _env:
-    def __init__(self, env):
-        self.env, self.old = env, {}
-
-    def __enter__(self):
-        for k, v in self.env.items():
-            self.old[k] = os.environ.get(k)
-            os.environ[k] = v
-
-    def __exit__(self, *exc):
-        for k, v in self.old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
 
 
 @pytest.fixture(scope="module")
 def plans():
     out = {}
     for c in P.ALL_CASES:
-        with _env(c.env):
+        with PU.env(c.env):
             out[c.id] = P.plan_of(c)
     return out
 
@@ -235,3 +218,20 @@ def test_every_recorded_link_is_a_case(links, plans):
     stale = sorted(set(by_link) - set(links))
     assert not missing and not wrong and not stale, \
         f"links no case runs: {missing}; cases that differ from their link: {wrong}; cases of links that no longer exist: {stale}"
+
+
+def test_conv_post_refuses_a_segmented_plan_before_launching():
+    """a fused consumer epilogue exists only in the single-product kernels: mnb_pk_conv_post must refuse a segmented
+    producer plan on the host (the pointers below are never dereferenced), not launch and leave the plane unwritten"""
+    import ctypes as C
+    from micronet_b200 import _lib as L
+    lib = L.load()
+    fake = 4096
+    qp = L.ActQParams(L.ACT_IAO, 8, -128, 127, 0, fake, fake, fake, fake)
+    post = L.PkPost(C.pointer(qp), 0, 0, fake)
+    sh = PU.shape(4, 64, 16, 16, 128, 3, 1, 1, 1)
+    assert PU.conv_plan(sh, 0, 2, 1)["segmented"] == 1
+    rc = lib.mnb_pk_conv_post(C.byref(sh), fake, 2, fake, 1, None, None, 1.0, None, None, C.byref(post), fake, None)
+    assert rc == L.E_UNSUPPORTED and b"segmented" in lib.mnb_last_error()
+    from micronet_b200 import pk as PK
+    assert PK.segmented(sh, 0, 2, 1) and not PK.segmented(sh, 0, 1, 1)

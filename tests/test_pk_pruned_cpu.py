@@ -3,7 +3,8 @@
 * the plans of the packed-operand family cover every conv of a channel-pruned NIN-GC (the reference README's
   group + prune cfg 154 162 144 304 320 320 608 584): forward at the piece counts the three schemes use, data gradient and
   weight gradient;
-* the plans of every conv of the bench models are those recorded before group-padded planes existed (BENCH_PLANS);
+* the plans of every conv of the bench models at every terms configuration are those recorded in
+  tests/pk_plan_bench_table.py (BENCH_PLANS): a change to any of them must be deliberate and recorded there;
 * the specialised kernels (pk_gc3, pk_wgrad_taps, int8) refuse padded shapes, so the engine runs them on mnb_pk_conv /
   mnb_pk_wgrad;
 * the Python hand-off decisions never hand a plain plane to a conv that reads a group-padded one."""
@@ -12,8 +13,7 @@ import ctypes as C
 import pytest
 
 from tests import pk_plan_util as PU
-from tests.test_pk_plan_cpu import _model_convs
-from tests.pk_plan_bench_table import BENCH_PLANS
+from tests.pk_plan_bench_table import BENCH_PLANS, CONFIGS
 
 README_CFG = [154, 162, 144, 304, 320, 320, 608, 584]
 
@@ -69,8 +69,12 @@ def test_plans_cover_edge_channel_counts(cg, kg):
 
 
 def _bench_rows():
-    convs = {c[0]: c for c in _model_convs()}
-    return [(convs[r[1]],) + r for r in BENCH_PLANS]
+    """(conv, kind, name, mode / terms..., recorded plan) of every bench-model conv at every configuration of the table"""
+    table = {r[:5]: r[5] for r in BENCH_PLANS}
+    rows = [(conv, kind, conv[0], a, b, c, table.pop((kind, conv[0], a, b, c), "not recorded"))
+            for conv in PU.model_convs() for kind, a, b, c in CONFIGS]
+    assert not table, f"recorded plans of convs or configurations the bench models do not have: {sorted(table)}"
+    return rows
 
 
 @pytest.mark.parametrize("row", _bench_rows(), ids=lambda r: f"{r[1]}-{r[2]}-{r[3]}-{r[4]}-{r[5]}")

@@ -9,7 +9,7 @@ import subprocess
 
 import pytest
 
-from tests.test_pk_plan_cpu import LIMIT, RESERVED, _budget, _model_convs
+from tests.pk_plan_util import LIMIT, RESERVED, budget, model_convs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TAPS_LAYERS = {"gc3x3g16", "gc3x3g32"}
@@ -28,7 +28,7 @@ def _plan(sh, t_dy, t_x):
     return rc, list(out)
 
 
-@pytest.mark.parametrize("conv", _model_convs(), ids=lambda c: c[0])
+@pytest.mark.parametrize("conv", model_convs(), ids=lambda c: c[0])
 def test_cover_is_exactly_the_grouped_3x3_layers(conv):
     from micronet_b200 import _lib as L
     name, B, Cc, H, W, K, R, st, pad, G = conv
@@ -51,7 +51,7 @@ def test_plan_limits(layer, B, terms):
     assert blocks == G // 4 and acc == 9 * 16
     # registers: 144 accumulators within the 232 the MMA warpgroups raise to (128 * 40 + 256 * 232 = 384 * 168)
     assert 128 * 40 + 256 * 232 <= 384 * 168
-    assert 2 <= nstage <= 8 and 0 < smem <= _budget("mnb_pk.cu", "kSmemBudget") and smem + RESERVED <= LIMIT
+    assert 2 <= nstage <= 8 and 0 < smem <= budget("mnb_pk.cu", "kSmemBudget") and smem + RESERVED <= LIMIT
     assert BW >= H + 2 and (BW * TH) % 16 == 0
     nstg = -(-B * -(-H // TH) // NI)
     assert splits == -(-nstg // spp) and (splits - 1) * spp < nstg
@@ -103,7 +103,7 @@ def test_kernel_has_no_spills():
     usage = funcs[0][1]
     assert re.search(r"STACK:0\b", usage) and re.search(r"LOCAL:0\b", usage), usage
     static = int(re.search(r"SHARED:(\d+)", usage).group(1)) - RESERVED
-    assert static + _budget("mnb_pk.cu", "kSmemBudget") <= LIMIT
+    assert static + budget("mnb_pk.cu", "kSmemBudget") <= LIMIT
 
 
 def test_gpu_cases_cover_the_bench_layers_and_the_edges():

@@ -87,7 +87,7 @@ def test_unreachable_refusals_stay_unreachable():
 
 
 def _model_convs():
-    from tests.test_pk_plan_cpu import _model_convs as convs
+    from tests.pk_plan_util import model_convs as convs
     out = []
     for name, B, Cc, H, W, K, R, st, pad, G in convs():
         if name.startswith(("gc", "nin")) and not name.endswith("head"):
