@@ -589,6 +589,19 @@ int mnb_pk_wgrad(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, c
 int mnb_pk_wgrad_taps_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t* out, int32_t n);
 int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
                       const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);
+/* Data gradient (mnb_pk_conv mode 1) and weight gradient (mnb_pk_wgrad) of a 1x1 convolution in one pass over dy: stride
+ * 1, no padding, <= 128 input and output channels per group, not group-padded, on the weight gradient's own raster, stages
+ * and batch splits.  w_img: the data-gradient weight image of mnb_pk_pack_weight (mode 1, terms_dy, terms_w).  dx is
+ * mnb_pk_conv's result without n_scale, a_scale or bias (dx = acc * a_scale_const; with the STE mask bits8,
+ * dx = pass ? acc * gain : 0) and dw mnb_pk_wgrad's (a_scale, kdiv), both bit for bit.  MNB_E_UNSUPPORTED (nothing launched)
+ * outside that cover.
+ * mnb_pk_bwd1x1_plan (host only): out = {groups, splits, NI, nstage, BW, TH, stages per split, smem bytes, sub-blocks,
+ * stages, data-gradient MMAs per chain, scratch bytes (lo 31 bits), scratch bytes (hi), npairs, N tile}; the first
+ * min(n, 15) are written. */
+int mnb_pk_bwd1x1_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t terms_w, int32_t* out, int32_t n);
+int mnb_pk_bwd1x1(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
+                  const void* w_img, int32_t terms_w, float a_scale_const, const uint8_t* bits8, float gain, float* dx,
+                  const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag, mnb_stream_t stream);
 /* Forward and data gradient of the same narrow grouped 3x3 layers (stride 1, padding 0..2, 16 input / 32 output channels per
  * group, groups % 4 == 0) with whole images as M tiles and a CTA per block of groups whose weights stay in shared memory.
  * Forward: one activation piece and one weight piece (mnb_pk_gc3_conv mode 0 = mnb_pk_conv mode 0, mnb_pk_gc3_conv_codes =

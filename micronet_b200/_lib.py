@@ -147,6 +147,8 @@ PROTOTYPES = {
     "mnb_pk_wgrad": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
     "mnb_pk_wgrad_taps_plan": (C.c_int, [_SHAPE, _I, _I, _P, _I]),
     "mnb_pk_wgrad_taps": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "mnb_pk_bwd1x1_plan": (C.c_int, [_SHAPE, _I, _I, _I, _P, _I]),
+    "mnb_pk_bwd1x1": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _I, C.c_float, _P, C.c_float, _P, _P, _P, _P, _P, _P, _P]),
     "mnb_pk_gc3_plan": (C.c_int, [_SHAPE, _I, _I, _I, _P, _I]),
     "mnb_pk_gc3_conv": (C.c_int, [_SHAPE, _I, _P, _I, _P, _I, _P, _P, C.c_float, _P, _P, C.c_float, _P, _P, _P]),
     "mnb_pk_gc3_conv_codes": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _I, _P, _P, _P, _P]),
@@ -274,6 +276,9 @@ PK_WG_TAPS = os.environ.get("MNB_PK_WG_TAPS", "1") != "0"
 # forward and data gradient of the same layers on mnb_pk_gc3_conv / mnb_pk_gc3_conv_codes (whole images as M tiles, the
 # weights of a block of groups resident in shared memory); MNB_PK_GC3=0 keeps them on mnb_pk_conv / mnb_pk_conv_codes
 PK_GC3 = os.environ.get("MNB_PK_GC3", "1") != "0"
+# data and weight gradient of the 1x1 grouped layers in one pass over dy on mnb_pk_bwd1x1; MNB_PK_BWD1X1=0 keeps them on
+# mnb_pk_conv + mnb_pk_wgrad (to compare the two in one process)
+PK_BWD1X1 = os.environ.get("MNB_PK_BWD1X1", "1") != "0"
 
 # bit-packed XNOR-popcount forward for wbwtab inference (mnb_xnor.cu): "auto" = the layers where it is expected to beat the
 # tensor-core forward (functional.xnor_preferred), "all" = wherever it has cover, "off" = never

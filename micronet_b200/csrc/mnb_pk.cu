@@ -2014,6 +2014,217 @@ pk_wgrad_taps_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_const
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// data and weight gradient of a 1x1 grouped convolution in one pass over dy
+// ---------------------------------------------------------------------------------------------------------
+// pk_conv_kernel (data gradient) and pk_wgrad_kernel read the same dy boxes op[c/8][position][8] from HBM, one K-major and
+// one MN-major.  Here one CTA per (group, batch split) of the weight gradient's own plan streams each box once and feeds
+// both MMAs from it: the wgrad MMAs exactly as pk_wgrad_kernel issues them (same split partials, reduced by
+// wg_reduce_kernel), and per sub-block of 64 positions the data-gradient MMAs against the group's weight image, resident
+// in shared memory, in the piece-pair / K-step order of make_plan's data-gradient program for the same shape.  Every
+// accumulator sees the chain of MMAs it sees in the two separate kernels, so dx and dW are theirs bit for bit.
+// The register file is split with setmaxnreg as in pk_wgrad_taps_kernel: wgrad Nc / 2 + dgrad Nc / 4 accumulators per thread.
+constexpr int kBwdThreads = 384;   // warpgroup 0: TMA (warp 0, lane 0), warpgroups 1, 2: MMA + data-gradient epilogue
+constexpr int kBwdRows = 64;       // positions per sub-block: one m64 block of data-gradient rows
+constexpr int kBwdProg = 64;       // data-gradient MMAs per accumulator chain
+constexpr int kBwdTmaRegs = 40, kBwdMmaRegs = 232;
+
+struct BwdPlan {
+  WgPlan wg;          // raster, sub-blocks, stages and splits (make_wg_plan; only the ring depth differs)
+  Plan dg;            // data-gradient plan of the same shape (make_plan mode 1): N tile, K chunks, piece pairs
+  int nprog, off_w, w_bytes, nstage, smem_bytes;
+};
+
+// The cover: stride 1, 1x1, no padding, channels per group <= 128 on either side and not group-padded, one 64-position
+// sub-block raster, and data-gradient / weight-gradient plans that tile a group the same way (one N tile as wide as the
+// wgrad's input-channel tile, one K box).
+static int make_bwd_plan(const mnb_conv_shape* s, int TA, int TX, int TW, BwdPlan& b) {
+  MNB_REQUIRE(s != nullptr, "conv shape is NULL");
+  MNB_REQUIRE(TA >= 1 && TA <= 3 && TX >= 1 && TX <= 3 && TW >= 1 && TW <= 3, "term counts must be 1..3");
+  memset(&b, 0, sizeof(b));
+  const int C = s->in_c, K = s->out_c, G = s->groups;
+  MNB_REQUIRE(s->batch > 0 && C > 0 && K > 0 && s->in_h > 0 && s->in_w > 0 && G > 0 && C % G == 0 && K % G == 0,
+              "bad conv shape");
+  auto no = [](const char* why) { return mnb_fail(MNB_E_UNSUPPORTED, "pk bwd1x1: %s", why); };
+  if (s->ker_h != 1 || s->ker_w != 1) return no("filter is not 1x1");
+  if (s->stride_h != 1 || s->stride_w != 1 || s->dil_h != 1 || s->dil_w != 1) return no("stride or dilation != 1");
+  if (s->pad_h != 0 || s->pad_w != 0) return no("padding != 0");
+  if (C / G > 128 || K / G > 128) return no("more than 128 channels per group");
+  if (G > 1 && ((C / G) % 8 || (K / G) % 8)) return no("group-padded operand planes");
+  if (int e = make_wg_plan(s, TA, TX, b.wg)) return e;
+  if (int e = make_plan(s, 1, TA, TW, b.dg)) return e;
+  const WgPlan& w = b.wg;
+  const Plan& d = b.dg;
+  if (w.gm != 1 || w.n_ktiles != 1 || w.n_ctiles != 1 || w.n_tg != 1) return no("weight-gradient block is not one whole group");
+  if (w.rows_dy != kBwdRows) return no("sub-block raster is not 64 positions");
+  if (d.n_ntiles != 1 || d.Nt != w.Nc || d.Nt % 32) return no("data-gradient N tile differs from the weight-gradient tile");
+  if (d.segmented) return no("segmented data-gradient plan");
+  if (d.chunks * d.ksteps * 16 > 128) return no("data-gradient K-steps beyond the dy box");
+  b.nprog = d.chunks * d.npairs * d.ksteps;
+  // (one filter tap, <= 8 K-steps of at most 6 piece pairs: one stage template and at most 48 MMAs)
+  if (d.ny != 1 || d.ntmpl[0] != 1 || b.nprog > kBwdProg)
+    return mnb_fail(MNB_E_ARG, "pk bwd1x1: data-gradient plan with %d templates, %d MMAs", d.ntmpl[0], b.nprog);
+  b.w_bytes = round_up(d.img_bytes[0], 1024);
+  b.nstage = std::min(MAXST, (kSmemBudget - 1024 - b.w_bytes) / w.stage_bytes);
+  if (b.nstage < 2) return no("fewer than two stages fit next to the weight image");
+  b.off_w = b.nstage * w.stage_bytes + 1024;
+  b.smem_bytes = b.off_w + b.w_bytes;
+  return 0;
+}
+
+struct BwdParams {
+  // weight gradient (pk_wgrad_kernel's quantities for tpg = 1, one tap)
+  uint32_t stg_per_split, nstg_total, NI, nsub, ksteps, npairs, nstage, stage16, sub16, dy_sbo, x_sbo, x_off16;
+  uint32_t pair_a16[MAXPAIR], pair_b16[MAXPAIR];
+  int row_tiles, TA, TX, TH, stage_bytes, sub_bytes, dy_bytes, x_bytes, dy_box_bytes, x_box_bytes, smem_bytes, cout_g8, cin_g8;
+  float* partial;
+  // data gradient: chain of (A offset in the sub-block | B offset in the weight image << 16), 16-byte units
+  uint32_t nprog, dg_lbo, w_lbo, off_w, w_bytes, img_bytes;
+  uint32_t prog[kBwdProg];
+  const uint8_t* w_img;
+  int B, P, Q, BW, C, cin_g, C8O;
+  float a_scale_const, gain;
+  float bias0;              // 0: pk_conv_kernel's epilogue adds its (zero) bias with the same fmaf
+  const uint8_t* bits8;     // STE mask [B][C8O][P][Q] or NULL
+  float* dx;
+  int* err;
+};
+
+// CTA (blockIdx.x = group, blockIdx.y = batch split).  NC: input channels per group rounded up to 16 (wgrad N, dgrad N tile)
+template <int NC>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+pk_bwd1x1_kernel(const __grid_constant__ CUtensorMap dy0, const __grid_constant__ CUtensorMap dy1,
+                 const __grid_constant__ CUtensorMap dy2, const __grid_constant__ CUtensorMap x0,
+                 const __grid_constant__ CUtensorMap x1, const __grid_constant__ CUtensorMap x2,
+                 const __grid_constant__ BwdParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ WgShared sh;
+  __shared__ uint64_t wbar;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int i = 0; i < MAXST; ++i) { tc::mbar_init(&sh.full[i], 1); tc::mbar_init(&sh.empty[i], 8); }
+    tc::mbar_init(&wbar, 1);
+    sh.abort = 0;
+    tc::fence_barrier_init();
+    tc::prefetch_tmap(&dy0); tc::prefetch_tmap(&x0);
+  }
+  // every row an MMA can read must be finite (positions are the wgrad's reduction dimension): zero the ring once
+  for (int i = tid; i < (int)p.off_w / 16; i += kBwdThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+  const int g = blockIdx.x, split = blockIdx.y;
+  const uint32_t stg0 = (uint32_t)split * p.stg_per_split, stg1 = min(p.nstg_total, stg0 + p.stg_per_split);
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kBwdTmaRegs));
+    if (warp == 0 && lane == 0) {
+      // the group's data-gradient weight image (n tile 0, group g), once
+      tc::mbar_arrive_expect_tx(&wbar, p.img_bytes);
+      tc::bulk_load_1d(smem + p.off_w, p.w_img + (size_t)g * p.img_bytes, p.img_bytes, &wbar);
+      uint32_t slot = 0, ph = 0;
+      const int k8 = g * p.cout_g8, c8 = g * p.cin_g8;
+      for (uint32_t stg = stg0; stg < stg1; ++stg) {
+        if (!tc::mbar_wait(&sh.empty[slot], ph ^ 1u, p.err, 731)) break;
+        const int sub0 = (int)(stg * p.NI), nsubs = min((int)p.NI, (int)p.nsub - sub0);
+        tc::mbar_arrive_expect_tx(&sh.full[slot], (uint32_t)(nsubs * (p.TA * p.dy_box_bytes + p.TX * p.x_box_bytes)));
+        for (int si = 0; si < nsubs; ++si) {
+          const int sub = sub0 + si;
+          const int b = sub / p.row_tiles, h0 = (sub - b * p.row_tiles) * p.TH;
+          uint8_t* sb = smem + (size_t)slot * p.stage_bytes + (size_t)si * p.sub_bytes;
+          tc::tma_load_4d(sb, &dy0, &sh.full[slot], 0, h0, b, k8);
+          if (p.TA > 1) tc::tma_load_4d(sb + p.dy_bytes, &dy1, &sh.full[slot], 0, h0, b, k8);
+          if (p.TA > 2) tc::tma_load_4d(sb + 2 * p.dy_bytes, &dy2, &sh.full[slot], 0, h0, b, k8);
+          uint8_t* xb = sb + (size_t)p.TA * p.dy_bytes;
+          tc::tma_load_4d(xb, &x0, &sh.full[slot], 0, h0, b, c8);
+          if (p.TX > 1) tc::tma_load_4d(xb + p.x_bytes, &x1, &sh.full[slot], 0, h0, b, c8);
+          if (p.TX > 2) tc::tma_load_4d(xb + 2 * p.x_bytes, &x2, &sh.full[slot], 0, h0, b, c8);
+        }
+        // sub-blocks of a short last stage keep their previous (finite) contents; the MMA loop skips them
+        if (++slot == p.nstage) { slot = 0; ph ^= 1u; }
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kBwdMmaRegs));
+    constexpr int NR = NC / 2, ND = NC / 2, NRD = ND / 2;
+    const int wg = (warp - 4) >> 2, w4 = (warp - 4) & 3;
+    // wgrad: A = the warpgroup's 64 dy channels (MN-major), B = the x channels (MN-major)
+    const uint64_t a_desc0 = tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.dy_sbo) + (uint64_t)((8u * wg * p.dy_sbo) >> 4);
+    const uint64_t b_desc0 = tc::smem_desc_mnmajor_noswz(tc::smem_u32(smem), 128, p.x_sbo) + (uint64_t)p.x_off16;
+    // dgrad: A = the 64 positions of the sub-block (K-major: dy channels along K), B = the warpgroup's half of the N tile
+    const uint64_t da_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem), p.dg_lbo, 128);
+    const uint64_t db_desc0 = tc::smem_desc_kmajor_noswz(tc::smem_u32(smem + p.off_w), p.w_lbo, 128) + (uint64_t)(ND * wg);
+    const uint32_t a_lo0 = (uint32_t)a_desc0, b_lo0 = (uint32_t)b_desc0, da_lo0 = (uint32_t)da_desc0, db_lo0 = (uint32_t)db_desc0;
+    const uint64_t a_hi = a_desc0 & 0xffffffff00000000ull, b_hi = b_desc0 & 0xffffffff00000000ull;
+    const uint64_t da_hi = da_desc0 & 0xffffffff00000000ull, db_hi = db_desc0 & 0xffffffff00000000ull;
+    // data-gradient epilogue: fragment d[4j + 2i + c] = D[position 16 w4 + lane/4 + 8i][channel ND wg + 8j + 2(lane%4) + c]
+    const int64_t plane = (int64_t)p.P * p.Q;
+    const int n_lo = ND * wg + 2 * (lane & 3);
+    float acc[NR], dacc[NRD];
+    tc::zero_acc(acc);
+    tc::mbar_wait_soft(&wbar, 0, p.err, 733, &sh.abort);
+    uint32_t slot = 0, ph = 0;
+    for (uint32_t stg = stg0; stg < stg1; ++stg) {
+      tc::mbar_wait_soft(&sh.full[slot], ph, p.err, 732, &sh.abort);
+      const uint32_t nsubs = min(p.NI, p.nsub - stg * p.NI);
+      for (uint32_t si = 0; si < nsubs; ++si) {
+        const uint32_t s16 = slot * p.stage16 + si * p.sub16;
+        tc::zero_acc(dacc);
+        tc::wg_fence();
+        tc::fence_acc(acc);
+        tc::fence_acc(dacc);
+        for (uint32_t j = 0; j < p.ksteps; ++j)
+          for (uint32_t pr = 0; pr < p.npairs; ++pr)
+            tc::Mma<NC>::template bf16<1, 1>(acc, a_hi | (uint64_t)(a_lo0 + s16 + 16u * j + p.pair_a16[pr]),
+                                             b_hi | (uint64_t)(b_lo0 + s16 + 16u * j + p.pair_b16[pr]), 1);
+        for (uint32_t e = 0; e < p.nprog; ++e) {
+          const uint32_t w = p.prog[e];
+          tc::Mma<ND>::template bf16<0, 0>(dacc, da_hi | (uint64_t)(da_lo0 + s16 + (w & 0xffffu)),
+                                           db_hi | (uint64_t)(db_lo0 + (w >> 16)), 1);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::fence_acc(acc);
+        tc::fence_acc(dacc);
+        // dx of the sub-block: pk_conv_kernel's data-gradient epilogue (a_scale_const, or the STE mask times gain)
+        const int sub = (int)((stg * p.NI) + si);
+        const int b = sub / p.row_tiles, h0 = (sub - b * p.row_tiles) * p.TH;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int m = 16 * w4 + (lane >> 2) + 8 * i;
+          const int oh = h0 + m / p.BW, ow = m - (m / p.BW) * p.BW;
+          if (oh >= p.P || ow >= p.Q) continue;
+          float* orow = p.dx + ((int64_t)b * p.C + g * p.cin_g) * plane + (int64_t)oh * p.Q + ow;
+          const uint8_t* brow = p.bits8 ? p.bits8 + ((int64_t)b * p.C8O + g * (p.cin_g >> 3)) * plane + (int64_t)oh * p.Q + ow : nullptr;
+#pragma unroll
+          for (int j = 0; j < ND / 8; ++j) {
+            const int n = n_lo + 8 * j;     // channels n, n + 1 (same octet)
+            if (n >= p.cin_g) continue;
+            if (brow) {
+              const uint32_t mk = __ldg(brow + (int64_t)(n >> 3) * plane) >> (n & 7);
+              orow[(int64_t)n * plane] = (mk & 1u) ? dacc[4 * j + 2 * i] * p.gain : 0.f;
+              if (n + 1 < p.cin_g) orow[(int64_t)(n + 1) * plane] = (mk & 2u) ? dacc[4 * j + 2 * i + 1] * p.gain : 0.f;
+            } else {
+              orow[(int64_t)n * plane] = fmaf(dacc[4 * j + 2 * i], p.a_scale_const, p.bias0);
+              if (n + 1 < p.cin_g) orow[(int64_t)(n + 1) * plane] = fmaf(dacc[4 * j + 2 * i + 1], p.a_scale_const, p.bias0);
+            }
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&sh.empty[slot]);
+      if (++slot == p.nstage) { slot = 0; ph ^= 1u; }
+    }
+    // partial[split][g][c][k]: pk_wgrad_kernel's layout for one k tile, one c tile, one tap
+    float* dst = p.partial + ((int64_t)split * gridDim.x + g) * (int64_t)(NC * 128);
+    const int fr = 64 * wg + 16 * w4 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < NR / 4; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) dst[(int64_t)(8 * j + fc + (e & 1)) * 128 + fr + 8 * (e >> 1)] = acc[4 * j + e];
+  }
+  __syncthreads();
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // forward and data gradient of narrow grouped 3x3 convolutions with whole images as M tiles
 // ---------------------------------------------------------------------------------------------------------
 // pk_conv_kernel tiles these layers (16 / 32 channels per group) into 128-row M tiles of a few image rows: a 16 x 16 image
@@ -3167,6 +3378,95 @@ extern "C" int mnb_pk_wgrad_taps(const mnb_conv_shape* s, const void* dy_pk, int
   const dim3 rgrid(kTapsCin * kTapsN, 1, pl.G * kTapsGm);
   wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, kTapsGm, 1, 1, kTapsN, pl.Nc, kTapsCout, kTapsCin, kTapsCout,
                                           kTapsCin, a_scale, kdiv, dw);
+  MNB_LAUNCHED(2);
+  return 0;
+}
+
+// ---- data and weight gradient of 1x1 grouped convolutions in one pass over dy (pk_bwd1x1_kernel)
+
+// host only: out = {groups, splits, NI, nstage, BW, TH, stg_per_split, smem_bytes, nsub, nstg_total, data-gradient MMAs per
+// chain, scratch bytes (lo), scratch bytes (hi), npairs (wgrad), N tile}; the first min(n, 15) are written.  Refuses what
+// mnb_pk_bwd1x1 refuses on the host, with its code and error text.
+extern "C" int mnb_pk_bwd1x1_plan(const mnb_conv_shape* s, int32_t terms_dy, int32_t terms_x, int32_t terms_w, int32_t* out,
+                                  int32_t n) {
+  pk::BwdPlan b;
+  if (int e = pk::make_bwd_plan(s, terms_dy, terms_x, terms_w, b)) return e;
+  if (out) {
+    const pk::WgPlan& w = b.wg;
+    const int64_t sb = w.partial_floats * 4;
+    const int v[15] = {w.G, w.splits, w.NI, b.nstage, w.BW, w.TH, w.stg_per_split, b.smem_bytes, w.nsub, w.nstg_total, b.nprog,
+                       (int)(sb & 0x7fffffff), (int)(sb >> 31), w.npairs, w.Nc};
+    for (int i = 0; i < std::min(n, 15); ++i) out[i] = v[i];
+  }
+  return 0;
+}
+
+// mnb_pk_conv (mode 1, data gradient into dx) followed by mnb_pk_wgrad (into dw) for the shapes of mnb_pk_bwd1x1_plan's cover,
+// with the same operands - w_img: the data-gradient weight image of mnb_pk_pack_weight (mode 1, terms_dy, terms_w) - and the
+// same results bit for bit.  The data-gradient epilogue is the one mnb_pk_conv runs without n_scale, a_scale or bias:
+// dx = acc * a_scale_const, or with bits8 (STE mask) dx = pass ? acc * gain : 0.  scratch: the plan's scratch bytes.
+extern "C" int mnb_pk_bwd1x1(const mnb_conv_shape* s, const void* dy_pk, int32_t terms_dy, const void* x_pk, int32_t terms_x,
+                             const void* w_img, int32_t terms_w, float a_scale_const, const uint8_t* bits8, float gain, float* dx,
+                             const float* a_scale, const float* kdiv, float* dw, void* scratch, int32_t* err_flag,
+                             mnb_stream_t stream) {
+  using namespace pk;
+  MNB_REQUIRE(s && dy_pk && x_pk && w_img && dx && dw && scratch && err_flag, "NULL pk_bwd1x1 pointer");
+  BwdPlan b;
+  if (int e = make_bwd_plan(s, terms_dy, terms_x, terms_w, b)) return e;
+  const WgPlan& pl = b.wg;
+  const Plan& d = b.dg;
+  static BwdParams p;   // filled per call (single host thread per process)
+  memset(&p, 0, sizeof(p));
+  p.stg_per_split = pl.stg_per_split; p.nstg_total = pl.nstg_total; p.NI = pl.NI; p.nsub = pl.nsub; p.ksteps = pl.rows_dy / 16;
+  p.npairs = pl.npairs; p.nstage = b.nstage; p.stage16 = pl.stage_bytes >> 4; p.sub16 = pl.sub_bytes >> 4;
+  p.dy_sbo = (uint32_t)pl.rows_dy * 16u; p.x_sbo = (uint32_t)pl.rows_x * 16u; p.x_off16 = (pl.TA * pl.dy_bytes) >> 4;
+  for (int i = 0; i < pl.npairs; ++i) {
+    p.pair_a16[i] = (uint32_t)(pl.pair_a[i] * pl.dy_bytes) >> 4;
+    p.pair_b16[i] = (uint32_t)(pl.pair_b[i] * pl.x_bytes) >> 4;
+  }
+  p.row_tiles = pl.row_tiles; p.TA = pl.TA; p.TX = pl.TX; p.TH = pl.TH;
+  p.stage_bytes = pl.stage_bytes; p.sub_bytes = pl.sub_bytes; p.dy_bytes = pl.dy_bytes; p.x_bytes = pl.x_bytes;
+  p.dy_box_bytes = pl.dy_box_bytes; p.x_box_bytes = pl.x_box_bytes; p.smem_bytes = b.smem_bytes;
+  p.cout_g8 = pl.cout_g / 8; p.cin_g8 = pl.cin_g / 8;
+  p.partial = reinterpret_cast<float*>(scratch);
+  // the data-gradient chain of make_plan's program (conv_mma: chunk, piece pair, K-step), re-addressed: A in the sub-block's
+  // dy box (octet stride = rows_dy * 16 bytes), B in the resident weight image (chunk blocks of blk_bytes)
+  p.nprog = (uint32_t)b.nprog;
+  {
+    const int b_tap16 = (d.CC / 8) * d.Nt, blk16 = d.tmpl[0][0].blk_bytes >> 4;
+    int e = 0;
+    for (int cc = 0; cc < d.chunks; ++cc)
+      for (int pr = 0; pr < d.npairs; ++pr)
+        for (int j = 0; j < d.ksteps; ++j) {
+          const uint32_t a16 = (uint32_t)(d.pair_a[pr] * pl.dy_bytes / 16 + (cc * d.ksteps + j) * 2 * pl.rows_dy);
+          const uint32_t b16 = (uint32_t)(cc * blk16 + d.pair_b[pr] * b_tap16 + j * 2 * d.Nt);
+          if (a16 > 0xffffu || b16 > 0xffffu) return mnb_fail(MNB_E_ARG, "pk bwd1x1: MMA program offset overflow");
+          p.prog[e++] = a16 | (b16 << 16);
+        }
+  }
+  p.dg_lbo = (uint32_t)pl.rows_dy * 16u; p.w_lbo = (uint32_t)d.Nt * 16u; p.off_w = (uint32_t)b.off_w;
+  p.w_bytes = (uint32_t)b.w_bytes; p.img_bytes = (uint32_t)d.img_bytes[0];
+  p.w_img = reinterpret_cast<const uint8_t*>(w_img);
+  p.B = pl.B; p.P = pl.P; p.Q = pl.Q; p.BW = pl.BW; p.C = s->in_c; p.cin_g = s->in_c / s->groups;
+  p.C8O = s->groups * ceil_div(p.cin_g, 8);
+  p.a_scale_const = a_scale_const; p.gain = gain; p.bias0 = 0.f; p.bits8 = bits8; p.dx = dx; p.err = err_flag;
+  CUtensorMap tdy[3], tx[3];
+  const int64_t dy_plane = (int64_t)pl.B * pl.K8 * pl.P * pl.Q * 16;
+  const int64_t x_plane = (int64_t)pl.B * pl.C8X * pl.HX * pl.WX * 16;
+  for (int t = 0; t < 3; ++t) {
+    if (int e = make_pk_tmap(&tdy[t], dy_pk, dy_plane, t < pl.TA ? t : 0, pl.B, pl.K8, pl.P, pl.Q, pl.BW, pl.TH, 1, 16)) return e;
+    if (int e = make_pk_tmap(&tx[t], x_pk, x_plane, t < pl.TX ? t : 0, pl.B, pl.C8X, pl.HX, pl.WX, pl.BW, pl.THH, 1, pl.Nc / 8)) return e;
+  }
+  using BwdFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                         const CUtensorMap, const BwdParams);
+  static const BwdFn fns[4] = {pk_bwd1x1_kernel<32>, pk_bwd1x1_kernel<64>, pk_bwd1x1_kernel<96>, pk_bwd1x1_kernel<128>};
+  const BwdFn fn = fns[pl.Nc / 32 - 1];     // (make_bwd_plan: Nc % 32 == 0, Nc <= 128)
+  if (int e = set_max_smem(fn, kSmemBudget)) return e;
+  cudaStream_t st = (cudaStream_t)stream;
+  fn<<<dim3(pl.G, pl.splits), kBwdThreads, b.smem_bytes, st>>>(tdy[0], tdy[1], tdy[2], tx[0], tx[1], tx[2], p);
+  const dim3 rgrid(pl.cin_o, 1, pl.G);
+  wg_reduce_kernel<<<rgrid, 128, 0, st>>>(p.partial, pl.splits, pl.G, 1, 1, 1, 1, pl.Nc, pl.cout_o, pl.cin_o, pl.cout_g, pl.cin_g,
+                                          a_scale, kdiv, dw);
   MNB_LAUNCHED(2);
   return 0;
 }

@@ -412,19 +412,28 @@ def _pk_backward(ctx, dy):
     else:
         dy_pk, _ = PK.pack_act(dy, None, T, ch_scale=ctx.w_scale if fold else None, groups=sh.groups)
     dx = dwq = None
+    tw = 1 if int_w else T
+    tx = min(ctx.pk_ta, T)     # a 3-piece saved input contributes its two leading pieces
+    kdiv = ctx.w_scale if fold else None
+    # a fused producer applies the STE mask itself (it owns the mask bits): plain data gradient times the quantizer's gain
+    plain_gain = ctx.pk_gain if ctx.pk_prepacked else 1.0
     if need_dx:
-        tw = 1 if int_w else T
         w_img = PK.pack_weight(sh, 1, T, tw, w_int=ctx.w_int, w_f32=None if int_w else ctx.wq,
                                kzero=ctx.w_scale if int_w else None)
         dx = torch.empty((sh.batch, sh.in_c, sh.in_h, sh.in_w), dtype=torch.float32, device=dy.device)
-        # a fused producer applies the STE mask itself (it owns the mask bits): plain data gradient times the quantizer's gain
-        plain_gain = ctx.pk_gain if ctx.pk_prepacked else 1.0
+    if need_dx and need_dw and pre is not None and PK.bwd1x1_taken(sh, T, tx, tw):
+        # 1x1 layers whose dy a fused BatchNorm + binarizer backward packed (the wbwtab graphs): both gradients in one pass
+        # over dy (mnb_pk_bwd1x1).  The DoReFa graphs keep the two launches, which their span tests time kernel by kernel.
+        dwq = torch.empty_like(ctx.wq)
+        L.check(_timed("bwd1x1_pk", sh, lambda: PK.run_bwd(sh, dy_pk, T, ctx.pk_x, tx, w_img, tw, dx, dwq, bits8=ctx.pk_bits8,
+                                                           gain=ctx.pk_gain, a_scale_const=plain_gain,
+                                                           a_scale=ctx.pk_wg_scale, kdiv=kdiv)), "pk_bwd1x1")
+        return dx, dwq
+    if need_dx:
         L.check(_timed("dgrad_pk", sh, lambda: PK.run_conv(sh, 1, dy_pk, T, w_img, tw, dx, bits8=ctx.pk_bits8, gain=ctx.pk_gain,
                                                            a_scale_const=plain_gain)), "pk_conv dgrad")
     if need_dw:
         dwq = torch.empty_like(ctx.wq)
-        tx = min(ctx.pk_ta, T)     # a 3-piece saved input contributes its two leading pieces
-        kdiv = ctx.w_scale if fold else None
         L.check(_timed("wgrad_pk", sh, lambda: PK.run_wgrad(sh, dy_pk, T, ctx.pk_x, tx, dwq, a_scale=ctx.pk_wg_scale,
                                                             kdiv=kdiv)), "pk_wgrad")
     return dx, dwq

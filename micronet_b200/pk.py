@@ -9,9 +9,10 @@ shared memory, stride 2, 5x5 filters, 4x4 or 224x224 images ...) and every fused
     wgrad       the same boxes read as MN-major operands, split over the batch, deterministic reduction
     wgrad_taps  wgrad of narrow grouped 3x3 layers with all nine taps of a CTA in registers
     gc3_conv    forward / data gradient of the same layers with whole images as M tiles (same result as conv)
+    bwd1x1      data gradient and weight gradient of a 1x1 layer in one pass over dy (same results as conv + wgrad)
 
-The layers of the engine go through run_conv / run_conv_codes / run_wgrad, which pick among those kernels (``PK_GC3``,
-``PK_WG_TAPS``); the single-kernel calls stay for tests and probes that compare the kernels directly.
+The layers of the engine go through run_conv / run_conv_codes / run_wgrad / run_bwd, which pick among those kernels
+(``PK_GC3``, ``PK_WG_TAPS``, ``PK_BWD1X1``); the single-kernel calls stay for tests and probes that compare the kernels directly.
 
 Reference math: F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen's
 convolution_backward."""
@@ -323,6 +324,36 @@ def wgrad_taps(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
                                       L.ptr(kdiv), dw.data_ptr(), ws.data_ptr(), L.tc_err_flag(dw.device).data_ptr(), L.stream())
 
 
+def bwd1x1_plan(sh, terms_dy, terms_x, terms_w):
+    """plan of mnb_pk_bwd1x1 as a dict, None outside its cover (host-only plan query, cached)"""
+    k = ("b1", _key(sh), terms_dy, terms_x, terms_w)
+    if k not in _plan_cache:
+        out = (C.c_int32 * 15)()
+        ok = L.load().mnb_pk_bwd1x1_plan(C.byref(sh), terms_dy, terms_x, terms_w, out, 15) == 0
+        plan = None
+        if ok:
+            names = ("groups", "splits", "NI", "nstage", "BW", "TH", "stg_per_split", "smem_bytes", "nsub", "nstg_total",
+                     "dgrad_chain")
+            plan = dict(zip(names, out[:11]))
+            plan["scratch_bytes"] = out[11] | (out[12] << 31)
+            plan["npairs"], plan["Nc"] = out[13], out[14]
+        _plan_cache[k] = plan
+    return _plan_cache[k]
+
+
+def bwd1x1(sh, dy_pk, terms_dy, x_pk, terms_x, w_img, terms_w, dx, dw, bits8=None, gain=1.0, a_scale_const=1.0, a_scale=None,
+           kdiv=None):
+    """mnb_pk_bwd1x1: conv(sh, 1, dy_pk, terms_dy, w_img, terms_w, dx, bits8=, gain=, a_scale_const=) followed by
+    wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=, kdiv=), the same results bit for bit; returns the C status"""
+    plan = bwd1x1_plan(sh, terms_dy, terms_x, terms_w)
+    if plan is None:
+        return L.E_UNSUPPORTED
+    ws = torch.empty(plan["scratch_bytes"], dtype=torch.uint8, device=dw.device)
+    return L.load().mnb_pk_bwd1x1(C.byref(sh), dy_pk.data_ptr(), terms_dy, x_pk.data_ptr(), terms_x, w_img.data_ptr(), terms_w,
+                                  float(a_scale_const), L.ptr(bits8), float(gain), dx.data_ptr(), L.ptr(a_scale), L.ptr(kdiv),
+                                  dw.data_ptr(), ws.data_ptr(), L.tc_err_flag(dw.device).data_ptr(), L.stream())
+
+
 def gc3_plan(sh, mode, terms_a, terms_w):
     """plan of mnb_pk_gc3_conv as a dict, None outside its cover (host-only plan query, cached).  ``chain``: the MMAs of
     one accumulator in issue order as (filter tap r * 3 + s, streamed-operand piece, weight piece, 16-channel K-step)"""
@@ -380,3 +411,21 @@ def run_wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
     wgrad otherwise.  Returns the C status."""
     fn = wgrad_taps if L.PK_WG_TAPS and wgrad_taps_plan(sh, terms_dy, terms_x) is not None else wgrad
     return fn(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=a_scale, kdiv=kdiv)
+
+
+def bwd1x1_taken(sh, terms_dy, terms_x, terms_w):
+    """does run_bwd take mnb_pk_bwd1x1 for this layer?"""
+    return L.PK_BWD1X1 and bwd1x1_plan(sh, terms_dy, terms_x, terms_w) is not None
+
+
+def run_bwd(sh, dy_pk, terms_dy, x_pk, terms_x, w_img, terms_w, dx, dw, bits8=None, gain=1.0, a_scale_const=1.0, a_scale=None,
+            kdiv=None):
+    """data and weight gradient: on bwd1x1 where its plan covers the shape and PK_BWD1X1 allows, otherwise run_conv
+    (mode 1) followed by run_wgrad.  Returns the C status of the first call that fails, or 0."""
+    if bwd1x1_taken(sh, terms_dy, terms_x, terms_w):
+        return bwd1x1(sh, dy_pk, terms_dy, x_pk, terms_x, w_img, terms_w, dx, dw, bits8=bits8, gain=gain,
+                      a_scale_const=a_scale_const, a_scale=a_scale, kdiv=kdiv)
+    rc = run_conv(sh, 1, dy_pk, terms_dy, w_img, terms_w, dx, bits8=bits8, gain=gain, a_scale_const=a_scale_const)
+    if rc != 0:
+        return rc
+    return run_wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=a_scale, kdiv=kdiv)
