@@ -494,9 +494,21 @@ int mnb_quant_add_pack_fwd(const float* a, const float* b, int32_t batch, int32_
  * text on a refusal.  The pointers of post are compared and checked for alignment, never dereferenced (post->q is read).
  * out = {epilogue path, Nt, MT, n_mtiles, n_items, ny, col_tiles, n_ntiles, CTAs per output phase, segmented}, the first
  * min(n, 10) written; path 0 plain bf16 levels (or no consumer), 1 segmented (no consumer), 2 int8 (levels or none),
- * 3 bf16 levels behind BatchNorm / shuffle, 4 the same into an int8 plane, 5 term planes. */
+ * 3 bf16 levels behind BatchNorm / shuffle or with a consumer STE mask, 4 the same into an int8 plane, 5 term planes. */
 int mnb_pk_conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, int32_t cpu, const mnb_pk_post* post,
                           int32_t* out, int32_t n);
+/* A training consumer (QAFT hand-offs: quantizers frozen).  mnb_pk_conv_post that also writes the STE mask of the levels it
+ * stores, bit = [y > 0 when post->relu] & pass(level), as bits8_out [b][C_out/8][OH][OW] - the layout mnb_pk_pack_act writes,
+ * never phase-split - which the consumer's data gradient (mnb_pk_conv mode 1) reads.  With a pool between producer and
+ * consumer, post->q is the pool's quantizer and the mask is the producer side of the pool's backward
+ * (mnb_pk_plane_maxpool_requant_bwd).  MNB_E_UNSUPPORTED unless post->q is symmetric IAO (q_type 0) and the plane is bf16
+ * without BatchNorm, channel shuffle or term planes; mnb_pk_conv_post_train_plan is its host-only plan query (the fields
+ * and refusals of mnb_pk_conv_post_plan with cpu 8). */
+int mnb_pk_conv_post_train(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img, int32_t terms_w,
+                           const float* n_scale, const float* a_scale, float a_scale_const, const float* bias, float* out,
+                           const mnb_pk_post* post, uint8_t* bits8_out, int32_t* err_flag, mnb_stream_t stream);
+int mnb_pk_conv_post_train_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, const mnb_pk_post* post, int32_t* out,
+                                int32_t n);
 /* int8 operands for frozen inference graphs (symmetric IAO, IAO:214-240 with q_type 0): the forward conv of the family on
  * s8 x s8 -> s32 wgmma (K32 MMAs, exact integer sums).  The result is  y = fmaf(float(sum), a_scale * n_scale[n], bias[n]),
  * bit-identical to mnb_pk_conv on the same levels whenever its fp32 partial sums stay below 2^24, and exact (one rounding of
@@ -559,6 +571,25 @@ int mnb_pk_plane_maxpool(const void* in_pk, int32_t batch, int32_t channels, int
 int mnb_pk_plane_maxpool_requant(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s,
                                  int32_t p, int32_t int8, const mnb_act_qparams* q_in, const mnb_act_qparams* q_out, void* out_pk,
                                  mnb_stream_t stream);
+/* The same pool in a QAFT training step (IAO quantizers frozen, nn.ReLU -> QuantMaxPool2d -> QuantConv2d of NIN / NIN-GC):
+ *   mnb_pk_plane_maxpool_requant_train : the bf16 form of mnb_pk_plane_maxpool_requant that also writes, per channel, the
+ *                                        window index of ATen's max_pool2d (first maximum in row-major order, the byte
+ *                                        r * k + s that mnb_maxpool2d_fwd records) as argmax [b][c/8][OH][OW][8] bytes
+ *                                        (8-byte aligned), and the consumer quantizer's STE mask of the pooled value as bits8
+ *                                        [b][c/8][OH][OW] (the mask mnb_pk_pack_act writes for that value).
+ *   mnb_pk_plane_maxpool_requant_bwd   : g [b][c][OH][OW] (the consumer's data gradient) gathered through argmax in ATen's
+ *                                        max_pool2d backward order, then dx = STE_in(sum) (act_quant_bwd's op sequence) where
+ *                                        bits8 [b][c/8][H][W] (mnb_pk_conv_post_train's bits8_out: relu'(y) & pass) is set,
+ *                                        else 0: the producer's fp32 gradient [b][c][H][W], bit for bit ATen's max_pool2d,
+ *                                        ActQuantFn and ReLU backward.
+ * Both need channels % 8 == 0, square windows k <= 15 with 2 * p <= k and symmetric IAO quantizers (q_type 0, 2..8 bits);
+ * anything else returns MNB_E_UNSUPPORTED before launching. */
+int mnb_pk_plane_maxpool_requant_train(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
+                                       int32_t s, int32_t p, const mnb_act_qparams* q_in, const mnb_act_qparams* q_out,
+                                       void* out_pk, uint8_t* argmax, uint8_t* bits8, mnb_stream_t stream);
+int mnb_pk_plane_maxpool_requant_bwd(const float* g, const uint8_t* argmax, const uint8_t* bits8, int32_t batch, int32_t channels,
+                                     int32_t h, int32_t w, int32_t k, int32_t s, int32_t p, const mnb_act_qparams* q_in, float* dx,
+                                     mnb_stream_t stream);
 /* Frozen wbwtab inference graphs with fp32 activations (prepare(A=32, W=2|3), WB:79-94: the "activation quantizer" is a ReLU):
  * activations cross between layers as term planes (terms exact bf16 pieces, the mnb_pk_pack_act layout with qp == NULL).
  *   mnb_pk_plane_maxpool_terms : max_pool2d(k, s, p) of the fp32 tensor a term plane holds (nin.py:51/56 3x3/2/1, nin_gc.py

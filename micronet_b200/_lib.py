@@ -120,6 +120,8 @@ PROTOTYPES = {
     "mnb_bn_sign_pool_bwd_pack": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P, _P]),
     "mnb_pk_conv_post": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P]),
     "mnb_pk_conv_post_plan": (C.c_int, [_SHAPE, _I, _I, _I, C.POINTER(PkPost), _P, _I]),
+    "mnb_pk_conv_post_train": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _P, C.POINTER(PkPost), _P, _P, _P]),
+    "mnb_pk_conv_post_train_plan": (C.c_int, [_SHAPE, _I, _I, C.POINTER(PkPost), _P, _I]),
     "mnb_pk_conv_codes": (C.c_int, [_SHAPE, _P, _I, _P, _I, _P, _P, C.c_float, _P, _I, _P, _P, _P, _P]),
     "mnb_codes_decode": (C.c_int, [_P, _P, _I, _I, _I, _P, _P]),
     "mnb_bn_batch_stats_codes": (C.c_int, [_P, _P, _I, _I, _I, _D, _D, _P, _P, _P, _P, _P, _P]),
@@ -141,6 +143,8 @@ PROTOTYPES = {
     "mnb_bn_relu_quant_pack_i8_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _ACTQ, _I, _P, _P]),
     "mnb_pk_plane_maxpool": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "mnb_pk_plane_maxpool_requant": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _ACTQ, _ACTQ, _P, _P]),
+    "mnb_pk_plane_maxpool_requant_train": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _ACTQ, _ACTQ, _P, _P, _P, _P]),
+    "mnb_pk_plane_maxpool_requant_bwd": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _ACTQ, _P, _P]),
     "mnb_pk_plane_maxpool_terms": (C.c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "mnb_bn_relu_pack_terms_fwd": (C.c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "mnb_pk_wgrad_scratch_bytes": (_L, [_SHAPE, _I, _I]),

@@ -556,8 +556,10 @@ __global__ void __launch_bounds__(256) bn_relu_quant_pack_i8_kernel(const float*
 // (act_quant_fwd_kernel), requantized by the consumer's quantizer with the exact op sequence of mnb_act_quantize_one
 // (__fdiv_rn, mnb_round_half_away, clamp) and stored as the consumer's plane value fl(level + zp_out): bf16 bits, or the
 // s8 byte in the low 8 bits.  Symmetric quantizers have zero_point 0, so P is the pool quantizer's level itself.
+// ptab (training pools, may be NULL): the consumer quantizer's STE pass flag of the same value.
 template <bool I8>
-__device__ __forceinline__ void build_requant_table(const mnb_act_qparams& qin, const mnb_act_qparams& qout, uint16_t* tab) {
+__device__ __forceinline__ void build_requant_table(const mnb_act_qparams& qin, const mnb_act_qparams& qout, uint16_t* tab,
+                                                    uint8_t* ptab = nullptr) {
   const MnbActQ a = mnb_load_actq(qin), b = mnb_load_actq(qout);
   for (int i = threadIdx.x; i < 256; i += blockDim.x) {
     const float lev = (float)min(max(i - 128, a.qmin), a.qmax);
@@ -567,6 +569,7 @@ __device__ __forceinline__ void build_requant_table(const mnb_act_qparams& qin, 
     const float o = __fadd_rn((float)(mnb_act_quantize_one(b, v, pass, xq) + b.qmin), b.zp);
     if constexpr (I8) tab[i] = (uint16_t)((uint32_t)__float2int_rn(o) & 0xffu);
     else tab[i] = __bfloat16_as_ushort(__float2bfloat16_rn(o));
+    if (ptab) ptab[i] = pass ? 1 : 0;
   }
 }
 
@@ -643,6 +646,97 @@ __global__ void __launch_bounds__(256) plane_maxpool_requant_kernel(const uint4*
   build_requant_table<I8>(qin, qout, tab);
   __syncthreads();
   plane_maxpool_body<I8, true>(in, planes, H, W, k, s, pad, OH, OW, out, tab);
+}
+
+// The same pool in a QAFT training step (mnb_pk_plane_maxpool_requant_train), bf16 planes of whole 8-channel units: per
+// channel the window index of ATen's max_pool2d (row-major scan, the first maximum stays; levels are never NaN) as the byte
+// r * k + s that mnb_maxpool2d_fwd records, arg[unit position][8], and the consumer quantizer's STE mask of the pooled value
+// as bits8 [b][c/8][OH][OW].  The pool quantizer's dequantization is strictly increasing in the level, so the first maximum
+// of the levels is the first maximum of the values ActQuantFn writes.  One thread = one output position of one unit.
+__global__ void __launch_bounds__(256) plane_maxpool_requant_train_kernel(const uint4* __restrict__ in, int64_t planes, int H,
+                                                                          int W, int k, int s, int pad, int OH, int OW,
+                                                                          uint4* __restrict__ out, uint2* __restrict__ arg,
+                                                                          uint8_t* __restrict__ bits, mnb_act_qparams qin,
+                                                                          mnb_act_qparams qout) {
+  __shared__ uint16_t tab[256];
+  __shared__ uint8_t ptab[256];
+  build_requant_table<false>(qin, qout, tab, ptab);
+  __syncthreads();
+  const int64_t total = planes * OH * OW;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int ow = (int)(idx % OW);
+    const int64_t t = idx / OW;
+    const int oh = (int)(t % OH);
+    const uint4* src = in + (t / OH) * H * W;
+    const int h0 = oh * s - pad, w0 = ow * s - pad;
+    float m[8];
+    uint32_t a[8];
+    bool first = true;
+    for (int r = 0; r < k; ++r) {
+      const int i = h0 + r;
+      if (i < 0 || i >= H) continue;
+      for (int c = 0; c < k; ++c) {
+        const int j = w0 + c;
+        if (j < 0 || j >= W) continue;
+        const uint4 u = __ldg(src + (int64_t)i * W + j);
+        const float f[8] = {__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                            __uint_as_float(u.y & 0xffff0000u), __uint_as_float(u.z << 16), __uint_as_float(u.z & 0xffff0000u),
+                            __uint_as_float(u.w << 16), __uint_as_float(u.w & 0xffff0000u)};
+        const uint32_t code = (uint32_t)(r * k + c);
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          if (first || f[e] > m[e]) { m[e] = f[e]; a[e] = code; }
+        first = false;
+      }
+    }
+    uint32_t w[4], pb = 0;
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) {
+      const int lo = min(max(__float2int_rz(m[e]) + 128, 0), 255), hi = min(max(__float2int_rz(m[e + 1]) + 128, 0), 255);
+      w[e >> 1] = (uint32_t)tab[lo] | ((uint32_t)tab[hi] << 16);
+      pb |= ((uint32_t)ptab[lo] << e) | ((uint32_t)ptab[hi] << (e + 1));
+    }
+    out[idx] = make_uint4(w[0], w[1], w[2], w[3]);
+    arg[idx] = make_uint2(a[0] | (a[1] << 8) | (a[2] << 16) | (a[3] << 24), a[4] | (a[5] << 8) | (a[6] << 16) | (a[7] << 24));
+    bits[idx] = (uint8_t)pb;
+  }
+}
+
+// Its backward, the chain max_pool2d -> ActQuantFn -> nn.ReLU of the un-linked graph in one pass: the pooled gradient g
+// [b][C][OH][OW] gathered through the window indices in ATen's max_pool_backward_nchw order (windows in (oh, ow) order, one
+// fp32 sum from 0, as maxpool_bwd_kernel), then the pool quantizer's STE with the producer's mask bit relu'(y) & pass
+// (mnb_act_ste_one, the op sequence of act_quant_bwd_kernel), written as the producer's fp32 gradient [b][C][H][W].
+// One thread = one input position of one 8-channel unit.
+__global__ void __launch_bounds__(256) plane_maxpool_requant_bwd_kernel(const float* __restrict__ g, const uint2* __restrict__ arg,
+                                                                        const uint8_t* __restrict__ bits, int H, int W,
+                                                                        int OH, int OW, int k, int st, int pad, int64_t total,
+                                                                        mnb_act_qparams qin, float* __restrict__ dx) {
+  const MnbActQ q = mnb_load_actq(qin);
+  const int64_t HW = (int64_t)H * W, OHW = (int64_t)OH * OW;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int w = (int)(idx % W);
+    const int64_t t = idx / W;
+    const int h = (int)(t % H);
+    const int64_t plane = t / H;     // b * C8 + c8: channel 8 * plane + e of the NCHW tensors
+    const int oh_lo = (h + pad < k) ? 0 : (h + pad - k) / st + 1, oh_hi = min((h + pad) / st + 1, OH);
+    const int ow_lo = (w + pad < k) ? 0 : (w + pad - k) / st + 1, ow_hi = min((w + pad) / st + 1, OW);
+    float acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+    const float* gp = g + plane * 8 * OHW;
+    for (int oh = oh_lo; oh < oh_hi; ++oh)
+      for (int ow = ow_lo; ow < ow_hi; ++ow) {
+        const uint32_t code = (uint32_t)((h - (oh * st - pad)) * k + (w - (ow * st - pad)));
+        const uint2 av = __ldg(arg + plane * OHW + (int64_t)oh * OW + ow);
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          if ((((e < 4 ? av.x : av.y) >> (8 * (e & 3))) & 0xffu) == code) acc[e] += __ldg(gp + e * OHW + (int64_t)oh * OW + ow);
+      }
+    const uint32_t mb = __ldg(bits + idx);
+    float* dp = dx + plane * 8 * HW + (int64_t)h * W + w;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) dp[e * HW] = mnb_act_ste_one(q, acc[e], (mb >> e) & 1u);
+  }
 }
 
 // the exact split of pack_act_body: piece t of each of 8 values into unit dst[t * term_vecs], residues carried over
@@ -1047,6 +1141,9 @@ struct ConvParams {
   // XTERMS instances (no consumer quantizer): the consumer's fp32 operand as post_terms exact bf16 pieces (after err, so
   // the parameter offsets of every other instance stay as they were)
   int post_terms;
+  // training consumer (QAFT hand-offs): the STE mask of the levels written to post_out, [ReLU'] & pass, as bits8
+  // [b][C8O][OH][OW] (the layout mnb_pk_pack_act writes, never phase-split), or NULL
+  uint8_t* post_bits;
 };
 
 struct alignas(16) ConvShared {
@@ -1273,6 +1370,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
       bool valid = false;
       int64_t orow = 0;      // element offset of this thread's output position in channel n_base of out / codes
       const uint8_t* brow = nullptr;
+      uint8_t* qrow = nullptr;   // this thread's position in octet 0 of the consumer's STE mask (training consumer only)
       int64_t prow = 0;      // vector index of this thread's position in octet 0 of the consumer's operand plane
       // one slot = 16 accumulator columns of one M tile
       auto do_slot = [&](const int mt, const int c16, const float (&r)[16]) {
@@ -1294,6 +1392,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
               prow = (((int64_t)b * 4 * p.C8O + ((oh & 1) * 2 + (ow & 1)) * p.C8O) * (p.OH >> 1) + (oh >> 1)) * (p.OW >> 1) + (ow >> 1);
             else
               prow = ((int64_t)b * p.C8O * p.OH + oh) * p.OW + ow;
+            if (XPOST && !I8 && p.post_bits) qrow = p.post_bits + (int64_t)b * p.C8O * plane + (int64_t)oh * p.OW + ow;
           }
         }
         if (!valid || n0 >= n_cnt || (p.dbg & 1)) return;
@@ -1366,6 +1465,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           // instances free of spills.
           const int64_t oct_stride = p.post_split ? (int64_t)(p.OH >> 1) * (p.OW >> 1) : plane;
           uint32_t pw[4];     // packed words of the current 16-byte unit (bf16: 8 channels, int8: 16 channels)
+          uint32_t mk = 0;    // training consumer: STE mask bits of the current octet
 #pragma unroll
           for (int qc = 0; qc < 4; ++qc) {
             if (!I8 && qc >= 2 && n0 + 8 >= n_cnt) break;
@@ -1398,6 +1498,15 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
             mnb_act_levels<4>(pq, yv, lev, passbits);
 #pragma unroll
             for (int j = 0; j < 4; ++j) lev[j] = n0 + 4 * qc + j < n_cnt ? lev[j] + pzp : 0.f;
+            if (!I8 && qrow) {   // STE mask of the consumer's data gradient: pass & relu'(y) (relu'(0) = 0, as ATen's)
+#pragma unroll
+              for (int j = 0; j < 4; ++j)
+                if (n0 + 4 * qc + j < n_cnt && ((passbits >> j) & 1u) && (!p.post_relu || yv[j] > 0.f)) mk |= 1u << (4 * (qc & 1) + j);
+              if (qc & 1) {
+                qrow[(int64_t)(((n_base + n0) >> 3) + (qc >> 1)) * plane] = (uint8_t)mk;
+                mk = 0;
+              }
+            }
             if (p.post_sg > 1) {   // consecutive channels land in different consumer units: one element at a time
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
@@ -2864,6 +2973,61 @@ extern "C" int mnb_pk_plane_maxpool_requant(const void* in_pk, int32_t batch, in
   return plane_maxpool(in_pk, batch, channels, h, w, k, s, p, int8, q_in, q_out, out_pk, stream);
 }
 
+// the checks of both training pool entry points (before anything is launched)
+static int plane_pool_train_check(int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s, int32_t p,
+                                  const mnb_act_qparams* q_in) {
+  MNB_REQUIRE(batch > 0 && channels > 0 && h > 0 && w > 0, "bad pk_plane_maxpool_requant_train shape");
+  if (k < 1 || k > 15 || s < 1 || p < 0 || 2 * p > k || h + 2 * p < k || w + 2 * p < k)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool_requant_train: kernel %d, stride %d, padding %d on %d x %d (needs "
+                                       "k <= 15, 2 * p <= k)", k, s, p, h, w);
+  if (channels % 8) return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool_requant_train: %d channels (needs a multiple of 8)", channels);
+  MNB_REQUIRE(q_in && q_in->scale && q_in->zero_point && q_in->obs_min && q_in->obs_max, "NULL pool quantizer scalar");
+  if (q_in->mode != MNB_ACT_IAO || q_in->q_type != 0 || q_in->bits < 2 || q_in->bits > 8 || q_in->qmin < -128 || q_in->qmax > 127)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool_requant_train: the pool quantizer must be symmetric IAO (q_type 0) "
+                                       "with 2..8 bits");
+  return 0;
+}
+
+extern "C" int mnb_pk_plane_maxpool_requant_train(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w,
+                                                  int32_t k, int32_t s, int32_t p, const mnb_act_qparams* q_in,
+                                                  const mnb_act_qparams* q_out, void* out_pk, uint8_t* argmax, uint8_t* bits8,
+                                                  mnb_stream_t stream) {
+  MNB_REQUIRE(in_pk && out_pk && argmax && bits8 && in_pk != out_pk, "NULL or aliased pk_plane_maxpool_requant_train pointer");
+  MNB_REQUIRE(((reinterpret_cast<uintptr_t>(in_pk) | reinterpret_cast<uintptr_t>(out_pk)) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(argmax) & 7) == 0,
+              "packed tensors must be 16-byte aligned, window indices 8-byte aligned");
+  if (int e = plane_pool_train_check(batch, channels, h, w, k, s, p, q_in)) return e;
+  MNB_REQUIRE(q_out, "NULL consumer quantizer");
+  if (q_out->mode != MNB_ACT_IAO || q_out->q_type != 0 || q_out->bits < 2 || q_out->bits > 8 || q_out->qmin < -128 ||
+      q_out->qmax > 127)
+    return mnb_fail(MNB_E_UNSUPPORTED, "pk_plane_maxpool_requant_train: the consumer quantizer must be symmetric IAO (q_type 0) "
+                                       "with 2..8 bits");
+  MNB_REQUIRE(q_out->scale && q_out->zero_point && q_out->obs_min && q_out->obs_max, "NULL consumer quantizer scalar");
+  const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
+  const int64_t planes = (int64_t)batch * (channels / 8), total = planes * oh * ow;
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 16);
+  pk::plane_maxpool_requant_train_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const uint4*>(in_pk), planes, h, w, k, s, p, oh, ow, reinterpret_cast<uint4*>(out_pk),
+      reinterpret_cast<uint2*>(argmax), bits8, *q_in, *q_out);
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int mnb_pk_plane_maxpool_requant_bwd(const float* g, const uint8_t* argmax, const uint8_t* bits8, int32_t batch,
+                                                int32_t channels, int32_t h, int32_t w, int32_t k, int32_t s, int32_t p,
+                                                const mnb_act_qparams* q_in, float* dx, mnb_stream_t stream) {
+  MNB_REQUIRE(g && argmax && bits8 && dx, "NULL pk_plane_maxpool_requant_bwd pointer");
+  MNB_REQUIRE((reinterpret_cast<uintptr_t>(argmax) & 7) == 0, "window indices must be 8-byte aligned");
+  if (int e = plane_pool_train_check(batch, channels, h, w, k, s, p, q_in)) return e;
+  const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
+  const int64_t total = (int64_t)batch * (channels / 8) * h * w;
+  const int blocks = (int)std::min<int64_t>(mnb_ceil_div(total, 256), (int64_t)MNB_NUM_SMS * 16);
+  pk::plane_maxpool_requant_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(g, reinterpret_cast<const uint2*>(argmax), bits8, h,
+                                                                                  w, oh, ow, k, s, p, total, *q_in, dx);
+  MNB_LAUNCHED(1);
+  return 0;
+}
+
 extern "C" int mnb_pk_plane_maxpool_terms(const void* in_pk, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t k,
                                           int32_t s, int32_t p, int32_t terms, void* out_pk, mnb_stream_t stream) {
   MNB_REQUIRE(in_pk && out_pk && in_pk != out_pk, "NULL or aliased pk_plane_maxpool_terms pointer");
@@ -2952,7 +3116,8 @@ extern "C" int mnb_pk_pack_weight(const mnb_conv_shape* s, int32_t mode, int32_t
 // launched) and the pk_conv_kernel instance row that runs it - 0 plain, 1 segmented (no consumer), 2 int8, 3 XPOST,
 // 4 XPOST int8, 5 XTERMS - together with the index range of the kernel's work-item arithmetic.  Host only: the launcher and
 // mnb_pk_conv_post_plan share it, so the query refuses what a launch refuses, with the same code and error text.
-static int conv_route(const pk::Plan& pl, int32_t mode, const uint8_t* bits8, const mnb_pk_post* post, int cpu, int& row) {
+static int conv_route(const pk::Plan& pl, int32_t mode, const uint8_t* bits8, const mnb_pk_post* post, int cpu, int& row,
+                      const uint8_t* post_bits = nullptr) {
   using namespace pk;
   if (post) {   // BatchNorm and channel shuffle in front of the consumer's quantizer
     const int nbn = (post->bn_mean != nullptr) + (post->bn_invstd != nullptr) + (post->bn_gamma != nullptr) + (post->bn_beta != nullptr);
@@ -2993,13 +3158,23 @@ static int conv_route(const pk::Plan& pl, int32_t mode, const uint8_t* bits8, co
     // the consumer epilogue is compiled into the single-product kernels only: in the segmented ones (several piece
     // products, e.g. an asymmetric-IAO producer whose levels take two pieces) it costs register spills on every launch
     if (pl.segmented) return unsupported("fused consumer of a segmented (multi-piece) plan");
+    if (post_bits) {   // training consumer: plain bf16 levels of a symmetric IAO quantizer, and their STE mask
+      if (cpu != 8 || terms_out || post->bn_mean || post->shuffle_groups > 1)
+        return unsupported("a consumer STE mask needs a bf16 level plane without BatchNorm or channel shuffle");
+      if (post->q->mode != MNB_ACT_IAO || post->q->q_type != 0)
+        return unsupported("a consumer STE mask needs a symmetric IAO consumer quantizer (q_type 0)");
+      // the mask is stored one byte per 8-channel unit: a partial unit would mix channels of two images or groups
+      if (pl.ng % 8) return unsupported("a consumer STE mask needs output channels (per group) % 8 == 0");
+    }
   }
   int ki = -1;
   for (int i = 0; i < 6; ++i) if (kNtSizes[i] == pl.Nt) ki = i;
   if (ki < 0 || pl.MT * pl.Nt > 128) return mnb_fail(MNB_E_ARG, "pk conv: plan with Nt %d, MT %d", pl.Nt, pl.MT);
   if (pl.n_items >= (1 << 22) || pl.n_mtiles >= (1 << 22))     // FastDiv's exact range (fp32 reciprocal + one correction step)
     return mnb_fail(MNB_E_UNSUPPORTED, "pk conv: %d work items / %d M tiles exceed the index arithmetic of the kernel", pl.n_items, pl.n_mtiles);
-  const bool xpost = post && (post->bn_mean || post->shuffle_groups > 1);   // (segmented plans refuse a post above)
+  // (segmented plans refuse a post above; a training consumer's mask is stored by the chunked XPOST epilogue, which stays
+  // free of spills where the plain instances' 16-channel one would not)
+  const bool xpost = post && (post->bn_mean || post->shuffle_groups > 1 || post_bits);
   row = terms_out ? 5 : cpu == 16 ? (xpost ? 4 : 2) : (pl.segmented ? 1 : (xpost ? 3 : 0));
   return 0;
 }
@@ -3055,7 +3230,8 @@ static int conv_plan(const mnb_conv_shape* s, int32_t mode, int32_t terms_a, int
 static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk, int32_t terms_a, const void* w_img,
                         int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
                         const float* bias, const uint8_t* bits8, float gain, float* out, const mnb_pk_post* post,
-                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8, int16_t* codes = nullptr, float* dec = nullptr) {
+                        int32_t* err_flag, mnb_stream_t stream, int cpu = 8, int16_t* codes = nullptr, float* dec = nullptr,
+                        uint8_t* post_bits = nullptr) {
   using namespace pk;
   MNB_REQUIRE(s && a_pk && w_img && (out || post || codes) && err_flag, "NULL pk_conv pointer");
   Plan pl;
@@ -3067,7 +3243,7 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
       return unsupported("int16 codes need one activation piece, one weight piece and a non-segmented plan");
   }
   int row = 0;
-  if (int e = conv_route(pl, mode, bits8, post, cpu, row)) return e;
+  if (int e = conv_route(pl, mode, bits8, post, cpu, row, post_bits)) return e;
   const bool terms_out = row == 5;
   static ConvParams p;   // large POD: filled per call (single host thread per process)
   memset(&p, 0, sizeof(p));
@@ -3099,6 +3275,7 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     p.post_mean = post->bn_mean; p.post_invstd = post->bn_invstd; p.post_gamma = post->bn_gamma; p.post_beta = post->bn_beta;
     p.post_sg = post->shuffle_groups;
     p.post_terms = terms_out ? post->terms_out : 0;
+    p.post_bits = post_bits;
   }
   { static const int dbg = [] { const char* e = getenv("MNB_PK_DEBUG"); return e ? atoi(e) : 0; }(); p.dbg = dbg; }
   CUtensorMap tm[3];
@@ -3143,15 +3320,39 @@ extern "C" int mnb_pk_conv_post(const mnb_conv_shape* s, const void* a_pk, int32
                       err_flag, stream);
 }
 
+extern "C" int mnb_pk_conv_post_train(const mnb_conv_shape* s, const void* a_pk, int32_t terms_a, const void* w_img,
+                                      int32_t terms_w, const float* n_scale, const float* a_scale, float a_scale_const,
+                                      const float* bias, float* out, const mnb_pk_post* post, uint8_t* bits8_out,
+                                      int32_t* err_flag, mnb_stream_t stream) {
+  MNB_REQUIRE(post && bits8_out, "NULL consumer description or STE mask");
+  return pk_conv_impl(s, 0, a_pk, terms_a, w_img, terms_w, n_scale, a_scale, a_scale_const, bias, nullptr, 1.f, out, post,
+                      err_flag, stream, 8, nullptr, nullptr, bits8_out);
+}
+
+static int conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, int32_t cpu, const mnb_pk_post* post,
+                          const uint8_t* post_bits, int32_t* out, int32_t n);
+
 // host only: out = {epilogue path (conv_route's instance row), Nt, MT, n_mtiles, n_items, ny, col_tiles, n_ntiles, CTAs per
 //            output phase, segmented}; the first min(n, 10) are written
 extern "C" int mnb_pk_conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, int32_t cpu,
                                      const mnb_pk_post* post, int32_t* out, int32_t n) {
+  return conv_post_plan(s, terms_a, terms_w, cpu, post, nullptr, out, n);
+}
+
+extern "C" int mnb_pk_conv_post_train_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, const mnb_pk_post* post,
+                                           int32_t* out, int32_t n) {
+  MNB_REQUIRE(post, "NULL consumer description");
+  static uint8_t mask;   // compared with NULL, never dereferenced
+  return conv_post_plan(s, terms_a, terms_w, 8, post, &mask, out, n);
+}
+
+static int conv_post_plan(const mnb_conv_shape* s, int32_t terms_a, int32_t terms_w, int32_t cpu, const mnb_pk_post* post,
+                          const uint8_t* post_bits, int32_t* out, int32_t n) {
   MNB_REQUIRE(s && (cpu == 8 || cpu == 16), "pk conv post plan: shape, 8 or 16 channels per unit");
   pk::Plan pl;
   if (int e = pk::make_plan(s, 0, terms_a, terms_w, pl, cpu)) return e;
   int row = 0;
-  if (int e = conv_route(pl, 0, nullptr, post, cpu, row)) return e;
+  if (int e = conv_route(pl, 0, nullptr, post, cpu, row, post_bits)) return e;
   pk::ConvParams::Mma m;   // (not kept: see conv_plan)
   int words = 0;
   if (int e = conv_mma(pl, cpu, m, words)) return e;

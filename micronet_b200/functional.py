@@ -340,9 +340,14 @@ def _pk_terms(spec, w_int, pm1=False):
     return ta, (1 if w_int is not None else T)
 
 
-def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, pre_relu=False, pm1=False, codes_out=False):
+def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, pre_relu=False, pm1=False, codes_out=False,
+                prepacked_bits=None, train_post=None):
     """forward on the packed-operand tensor-core family; returns False when the shape is outside its cover.
-    ``prepacked``: the operand plane a fused producer (fused.BNReluQuantFn) already wrote - x itself holds no data then.
+    ``prepacked``: the operand plane a fused producer (fused.BNReluQuantFn) already wrote - x itself holds no data then;
+    ``prepacked_bits``: the STE mask that producer wrote with it for this layer's data gradient (QAFT hand-offs; without it
+    the producer applies the mask in its own backward).
+    ``train_post``: the Consumer of a QAFT hand-off (iao.prepare(fuse=True)): the epilogue writes its plane and STE mask
+    (mnb_pk_conv_post_train) and y is left unwritten, tagged with both; where that epilogue refuses, y as usual.
     ``codes_out`` (wbwtab layer on a +-1 input whose only reader is its fused BatchNorm + binarizer): the exact integer sums
     go out as int16 codes with their decode pair, tagged on y as ``_mnb_codes``; y itself is then not written.  Shapes the
     int16 hand-off does not cover write y as usual."""
@@ -359,7 +364,7 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, p
         return False
     qp = spec.struct() if spec is not None else None
     if prepacked is not None:
-        x_pk, bits8 = prepacked, None      # the producer keeps the STE mask for its own backward
+        x_pk, bits8 = prepacked, prepacked_bits
     else:
         x_pk, bits8 = PK.pack_act(x, qp, ta, phase_split=sh.stride_h == 2, want_bits=need_dx, relu=pre_relu,
                                   groups=sh.groups)
@@ -374,6 +379,14 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, p
                                                             a_scale_const=a_const, bias=bias))
         if rc == 0:
             y._mnb_codes = (codes, dec)
+    if train_post is not None and w_int is not None:
+        cplane, cbits = PK.consumer_plane(*y.shape, y.device), PK.consumer_bits(*y.shape, y.device)
+        cqp = train_post.post_spec.struct()
+        rc = _timed("fwd_pk", sh, lambda: PK.conv_post(sh, x_pk, ta, w_img, tw, None, cqp, cplane, True, train_post.split,
+                                                       n_scale=w_scale, a_scale=a_scale, a_scale_const=a_const, bias=bias,
+                                                       post_bits=cbits))
+        if rc == 0:
+            tag(y, train_post.target, cplane, "bf16", bits=cbits)
     if rc == L.E_UNSUPPORTED:
         rc = _timed("fwd_pk", sh, lambda: PK.run_conv(sh, 0, x_pk, ta, w_img, tw, y,
                                                       n_scale=w_scale if w_int is not None else None, a_scale=a_scale,
@@ -381,7 +394,7 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, p
     if rc == L.E_UNSUPPORTED:
         return False
     L.check(rc, "pk_conv fwd")
-    ctx.pk_x, ctx.pk_ta, ctx.pk_bits8, ctx.pk_prepacked = x_pk, ta, bits8, prepacked is not None
+    ctx.pk_x, ctx.pk_ta, ctx.pk_bits8, ctx.pk_prepacked = x_pk, ta, bits8, prepacked is not None and bits8 is None
     # the quantizer's STE gain on the data gradient, and the scale of the saved activation levels in the weight gradient
     ctx.pk_gain = 0.1 if (spec is not None and spec.mode == L.ACT_DOREFA) else 1.0
     ctx.pk_wg_scale = None
@@ -627,7 +640,7 @@ class QuantConv2dFn(Function):
 
     @staticmethod
     def forward(ctx, x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, no_grad=False,
-                codes_out=False):
+                codes_out=False, handed=None, train_post=None):
         from . import pk as PK
         L.require_cuda(x, wq)
         assert not (pre_relu and any(ctx.needs_input_grad)), "the folded ReLU is an inference-only fusion"
@@ -653,6 +666,13 @@ class QuantConv2dFn(Function):
         if (L.XNOR_MODE != "off" and spec is None and w_int is not None and pm1 and not pre_relu
                 and (no_grad or not any(ctx.needs_input_grad[:3])) and _xnor_forward(x, w_int, w_scale, bias, sh, y, groups)):
             family = "xnor"
+        elif handed is not None:
+            # a QAFT producer's epilogue (or the plane pool behind it) wrote this layer's plane and STE mask; the layer may
+            # in turn write its own consumer's (train_post)
+            if not _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=handed[0], prepacked_bits=handed[1],
+                               train_post=train_post):
+                raise RuntimeError("micronet_b200: handed-over plane in front of a conv outside the packed-operand cover")
+            family = "pk"
         elif pkq is not None:
             if spec is None or spec.mode != L.ACT_DOREFA or spec.bits != pkq[1] or w_int is None:
                 raise RuntimeError("micronet_b200: a fused producer's packed output reached a conv with another quantizer")
@@ -660,7 +680,7 @@ class QuantConv2dFn(Function):
                 raise RuntimeError("micronet_b200: fused producer output in front of a conv outside the packed-operand cover")
             family = "pk"
         elif ((pk_on and x.dtype == torch.float32 and (L.PK_MODE == "all" or spec is not None) and not plane_only
-               and _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, pre_relu=pre_relu))
+               and _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, pre_relu=pre_relu, train_post=train_post))
               # wbwtab layer behind a fused BatchNorm + binarizer: +-1 input (one exact bf16 piece).  With the producer's
               # plane the layer is pure TMA -> MMA; 3x3 layers win on the packed-operand family even when they pack
               # themselves (measured per layer, DESIGN.md 6).  Outside the cover: the round-1 fused kernels below.
@@ -723,14 +743,16 @@ class QuantConv2dFn(Function):
         else:
             dx = _dgrad(ctx, dy, tc=False) if need_dx else None
             dwq = _wgrad(ctx, dy, tc=False) if need_dw else None
-        return dx, dwq, db, None, None, None, None, None, None, None, None, None, None
+        return dx, dwq, db, None, None, None, None, None, None, None, None, None, None, None, None
 
 
-def quant_conv2d(x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, codes_out=False):
+def quant_conv2d(x, wq, bias, w_int, w_scale, spec, stride, padding, dilation, groups, pre_relu=False, codes_out=False,
+                 handed=None, train_post=None):
+    """``handed`` / ``train_post``: the two ends of a QAFT hand-off (QuantConv2dFn, _pk_forward)"""
     # (autograd runs a Function's forward with grad mode off and needs_input_grad ignores torch.no_grad(): whether this call
     # will ever be differentiated is only known out here)
     return QuantConv2dFn.apply(x, wq, bias, w_int, w_scale, spec, tuple(stride), tuple(padding),
-                               tuple(dilation), groups, pre_relu, not torch.is_grad_enabled(), codes_out)
+                               tuple(dilation), groups, pre_relu, not torch.is_grad_enabled(), codes_out, handed, train_post)
 
 
 # --------------------------------------------------------------------------
@@ -893,6 +915,52 @@ class Consumer:
     @property
     def split(self):
         return self.stride[0] == 2 and self.pool is None
+
+
+def train_consumer_ok(consumer, out_shape):
+    """can a QAFT producer writing ``out_shape`` hand ``consumer`` its plane?  The consumer's forward takes a one-piece plane
+    of the activation it reads (Consumer.accepts) and its data and weight gradients stay on the packed-operand family."""
+    from . import pk as PK
+    act = consumer.read_shape(out_shape)
+    if not consumer.accepts(act):
+        return False
+    sh = _shape_struct(act, consumer.w_shape, consumer.stride, consumer.padding, consumer.dilation, consumer.groups)
+    Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    return PK.supported(sh, 1, Tb, 1) and PK.wgrad_supported(sh, Tb, 1)
+
+
+def handed_train(module, x):
+    """(plane, STE mask) a QAFT producer wrote for ``module`` when ``x`` is its tagged output, else None"""
+    plane = handed_plane(module, x)
+    return None if plane is None or "bits" not in x._mnb_pk_pre[4] else (plane, x._mnb_pk_pre[4]["bits"])
+
+
+class PlanePoolFn(Function):
+    """the QuantMaxPool2d between two linked blocks of a QAFT step (iao.prepare(fuse=True)) on the producer's plane of the
+    pool quantizer's levels: max-pool, window indices, requantization to the consumer's levels and their STE mask in one
+    kernel (mnb_pk_plane_maxpool_requant_train); the returned tensor is a shape-carrying placeholder tagged with that plane
+    for ``target``.  Backward: max_pool2d, ActQuantFn and nn.ReLU backward in one kernel (mnb_pk_plane_maxpool_requant_bwd)."""
+
+    @staticmethod
+    def forward(ctx, x, plane, bits, k, s, p, spec_p, spec_c, target):
+        from . import pk as PK
+        b, c, h, w = x.shape
+        q_in = spec_p.frozen()     # the pool's backward sees the forward-time scale, as ActQuantFn's does
+        out, arg, cbits = _timed("plane_pool", L.ConvShape(b, c, h, w, c, k, k, s, s, p, p, 1, 1, 1),
+                                 lambda: PK.plane_maxpool_requant_train(plane, b, c, h, w, k, s, p, q_in.struct(),
+                                                                        spec_c.struct()))
+        y = torch.empty((b, c, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1), dtype=torch.float32, device=x.device)
+        ctx.arg, ctx.bits, ctx.spec, ctx.cfg = arg, bits, q_in, (b, c, h, w, k, s, p)
+        return tag(y, target, out, "bf16", bits=cbits)
+
+    @staticmethod
+    def backward(ctx, g):
+        from . import pk as PK
+        b, c, h, w, k, s, p = ctx.cfg
+        qp = ctx.spec.struct()
+        dx = _timed("plane_pool_bwd", L.ConvShape(b, c, h, w, c, k, k, s, s, p, p, 1, 1, 1),
+                    lambda: PK.plane_maxpool_requant_bwd(g.contiguous(), ctx.arg, ctx.bits, b, c, h, w, k, s, p, qp))
+        return dx, None, None, None, None, None, None, None, None
 
 
 DECODABLE = ("bits", "b1", "terms")     # plane formats materialized decodes; level planes ("bf16", "i8") it cannot

@@ -332,8 +332,23 @@ class QuantConv2d(nn.Conv2d):
             wq, w_int, w_scale = weight, None, None
         if L.KEEP_DEBUG:   # tests: the fake-quantized weight of this call (tie-excuse rule for BN-fused weights)
             self.__dict__["_dbg_wq"] = wq.detach()
+        handed = F_.handed_train(self, input) if self.training else None
         return F_.quant_conv2d(input, wq, bias, w_int, w_scale, spec, self.stride, self.padding,
-                               self.dilation, self.groups)
+                               self.dilation, self.groups, handed=handed, train_post=self._train_post(input, weight))
+
+    def _train_post(self, input, weight):
+        """the Consumer whose plane and STE mask this conv's epilogue writes in a QAFT training step (prepare(fuse=True)
+        linked it, _link_training), or None: not linked, not every module of the link in training mode, frozen, a quantizer
+        no longer frozen (qaft cleared since, e.g. to resume QAT: the consumer would refresh its observer from the unwritten
+        placeholder), or a shape outside the hand-off's cover"""
+        link = self.__dict__.get("_mnb_train_link")
+        if (link is None or not self.training or self.__dict__.get("_frozen_inference", False)
+                or not all(m.training for m in link.modules()) or input.dim() != 4 or not link.frozen_quantizers(self)):
+            return None
+        c = link.consumer()
+        sh = F_._shape_struct(input.shape, weight.shape, self.stride, self.padding, self.dilation, self.groups)
+        out_shape = (input.shape[0], weight.shape[0]) + F_._out_hw(sh)
+        return c if F_.train_consumer_ok(c, out_shape) else None
 
     def _frozen_operands(self, make):
         """inference fast path (freeze_inference): the quantized weights of an eval-mode module are computed once;
@@ -723,6 +738,8 @@ def freeze_inference(model, enable=True, handoff=True, int8=False):
     Outputs are bit-identical to the un-frozen eval forward (a deployment graph's: to the frozen QAT graph's);
     ``enable=False`` restores the modules."""
     FG.undo(model, _UNDO)
+    if model.__dict__.get(_TRAIN_LINKED, False):
+        _link_training(model)     # the undo dropped the training overrides of the modules the freeze had absorbed
     if not enable:
         return model
     rw = FG.Rewrite(model, _UNDO)
@@ -834,6 +851,87 @@ def _link_blocks(model, rw):
             rw.move_shuffle(nxt, cconv, sg)
 
 
+# ********************* QAFT hand-offs (prepare(..., fuse=True)) *********************
+_TRAIN_LINKED = "_mnb_iao_train_linked"
+
+
+class _TrainLink:
+    """a producer -> consumer hand-off of a QAFT training step between two conv-bn-relu blocks of an nn.Sequential: the
+    producer's epilogue applies the nn.ReLU and the quantizer of the QuantMaxPool2d in between (the consumer's without one)
+    and writes its level plane and STE mask; the pool runs on that plane (functional.PlanePoolFn)"""
+
+    def __init__(self, cconv, relu, pool):
+        self.cconv, self.relu, self.pool = cconv, relu, pool      # pool: (QuantMaxPool2d, k, s, p) or None
+        self.target = cconv if pool is None else pool[0]
+
+    def modules(self):
+        return (self.cconv, self.relu) + (() if self.pool is None else (self.pool[0],))
+
+    def frozen_quantizers(self, conv):
+        """are the quantizers of producer ``conv``, the pool and the consumer still frozen (qaft) symmetric 2..8-bit ones?"""
+        return (_qaft_conv(conv) and _qaft_conv(self.cconv)
+                and (self.pool is None or _qaft_quantizer(self.pool[0].activation_quantizer)))
+
+    def consumer(self):
+        c = self.cconv
+        pool_spec = None if self.pool is None else self.pool[0].activation_quantizer.act_spec()
+        return F_.Consumer(c, c.activation_quantizer.act_spec(), True, True, tuple(c.weight.shape), tuple(c.stride),
+                           tuple(c.padding), tuple(c.dilation), c.groups, True, pool=self.pool, post_spec=pool_spec)
+
+
+def _qaft_quantizer(q):
+    return _sym_quantizer(q) and q.qaft
+
+
+def _qaft_conv(conv):
+    """can ``conv`` produce or consume a QAFT hand-off?  A BN-fused conv (running statistics folded, IAO:903-935) with frozen
+    symmetric 2..8-bit quantizers"""
+    return (isinstance(conv, QuantBNFuseConv2d) and conv.qaft and _qaft_quantizer(conv.activation_quantizer)
+            and _qaft_quantizer(conv.weight_quantizer))
+
+
+def _train_pool_cover(m):
+    """(k, s, p) of a QuantMaxPool2d with a frozen symmetric quantizer that mnb_pk_plane_maxpool_requant_train runs"""
+    from .fused import _pool_cfg
+    return _pool_cfg(m) if type(m) is QuantMaxPool2d and _qaft_quantizer(m.activation_quantizer) else None
+
+
+def _train_pool_forward(pool, link, x):
+    """the QuantMaxPool2d of a QAFT hand-off: on the producer's plane when one came, as usual otherwise"""
+    handed = F_.handed_train(pool, x) if pool.training else None
+    if handed is None:
+        return type(pool).forward(pool, x)
+    _, k, s, p = link.pool
+    return F_.PlanePoolFn.apply(x, handed[0], handed[1], k, s, p, pool.activation_quantizer.act_spec(),
+                                link.cconv.activation_quantizer.act_spec(), link.cconv)
+
+
+def _link_training(model):
+    """QAFT hand-offs of NIN / NIN-GC-style graphs: a conv-bn-relu block (prepare(bn_fuse=True, qaft=True)) is linked to the
+    first conv of the next block across a QuantMaxPool2d when both convs and the pool have frozen symmetric 2..8-bit
+    quantizers, the next block does not shuffle its input (a shuffled epilogue stores one level at a time, which does not pay
+    on bf16 planes: _shuffled_link_pays), the consumer reads a plain plane (not group-padded) and the producer writes whole
+    8-channel units.  Only links across a pool are made: the epilogue that writes plane and mask costs more than the ReLU
+    and pack passes a pool-less link removes; measured on an H100, pool-less links made the step slower (DESIGN.md 4.21).  Links and the instance-level ``forward`` of the absorbed nn.ReLU and pool live in the
+    modules' ``__dict__``: types, repr and state_dict are unchanged.  The producer checks the shapes per call
+    (QuantConv2d._train_post); anything outside the cover, and every module in eval mode, runs as if un-linked."""
+    import functools
+    from . import pk as PK
+    model.__dict__[_TRAIN_LINKED] = True
+    for (conv, relu), pool, cfg, nxt, cconv, _ in FG.block_pairs(model, _conv_relu, _train_pool_cover):
+        if not (_qaft_conv(conv) and _qaft_conv(cconv)) or FG.block_shuffle(nxt) > 1:
+            continue
+        if pool is None or tuple(cconv.stride) != (1, 1):
+            continue
+        if (conv.out_channels // conv.groups) % 8 or PK.padded(cconv.in_channels, cconv.groups):
+            continue
+        link = _TrainLink(cconv, relu, None if pool is None else (pool,) + cfg)
+        conv.__dict__["_mnb_train_link"] = link
+        relu.__dict__["forward"] = functools.partial(FG.absorbed_forward, _no_check, relu, link.target)
+        if pool is not None:
+            pool.__dict__["forward"] = functools.partial(_train_pool_forward, pool, link)
+
+
 def _first_quant_conv(seq):
     kids = [k for k in seq.children() if not isinstance(k, nn.Identity)] if isinstance(seq, nn.Sequential) else []
     return kids[0] if kids and isinstance(kids[0], QuantConv2d) else None
@@ -865,7 +963,8 @@ def prepare(model, inplace=False, a_bits=8, w_bits=8, q_type=0, q_level=0, weigh
             bn_fuse_calib=False, quant_inference=False, pretrained_model=False, qaft=False, ptq=False,
             percentile=0.9999, fuse=False):
     """``fuse`` (extension, off by default): engine max-pool kernels and channel-shuffle folding
-    (micronet_b200.fused); parameters, state_dict keys and results are unchanged."""
+    (micronet_b200.fused), and the QAFT hand-offs of BN-fused NIN / NIN-GC blocks (_link_training, DESIGN.md 4.21);
+    parameters, state_dict keys and results are unchanged."""
     if not inplace:
         model = copy.deepcopy(model)
     add_quant_op(model, a_bits=a_bits, w_bits=w_bits, q_type=q_type, q_level=q_level,
@@ -875,4 +974,5 @@ def prepare(model, inplace=False, a_bits=8, w_bits=8, q_type=0, q_level=0, weigh
     if fuse:
         from .fused import fuse_blocks
         fuse_blocks(model)
+        _link_training(model)
     return model

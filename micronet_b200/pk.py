@@ -161,11 +161,21 @@ def post_struct(qp, plane, relu, split, bn=None, shuffle_groups=1):
     return post
 
 
+def consumer_bits(b, c, h, w, device):
+    """empty STE mask bits8 [b][c/8][h][w] of a conv that reads a [b, c, h, w] activation (c % 8 == 0)"""
+    return torch.empty((b, c // 8, h, w), dtype=torch.uint8, device=device)
+
+
 def conv_post(sh, a_pk, terms_a, w_img, terms_w, out, post_qp, post_plane, post_relu, post_split, n_scale=None, a_scale=None,
-              a_scale_const=1.0, bias=None, bn=None, shuffle_groups=1):
-    """forward conv whose epilogue also writes the consumer's operand plane (frozen inference graphs); out may be None"""
+              a_scale_const=1.0, bias=None, bn=None, shuffle_groups=1, post_bits=None):
+    """forward conv whose epilogue also writes the consumer's operand plane (frozen inference graphs) and, with
+    ``post_bits``, its STE mask (QAFT training hand-offs, mnb_pk_conv_post_train); out may be None"""
     lib = L.load()
     post = post_struct(post_qp, post_plane, post_relu, post_split, bn, shuffle_groups)
+    if post_bits is not None:
+        return lib.mnb_pk_conv_post_train(C.byref(sh), a_pk.data_ptr(), terms_a, w_img.data_ptr(), terms_w, L.ptr(n_scale),
+                                          L.ptr(a_scale), float(a_scale_const), L.ptr(bias), L.ptr(out), C.byref(post),
+                                          post_bits.data_ptr(), L.tc_err_flag(a_pk.device).data_ptr(), L.stream())
     return lib.mnb_pk_conv_post(C.byref(sh), a_pk.data_ptr(), terms_a, w_img.data_ptr(), terms_w, L.ptr(n_scale), L.ptr(a_scale),
                                 float(a_scale_const), L.ptr(bias), L.ptr(out), C.byref(post),
                                 L.tc_err_flag(a_pk.device).data_ptr(), L.stream())
@@ -266,6 +276,28 @@ def plane_maxpool_requant(plane, b, c, h, w, k, s, p, q_in, q_out, int8=False):
     L.check(L.load().mnb_pk_plane_maxpool_requant(plane.data_ptr(), b, c, h, w, k, s, p, 1 if int8 else 0, C.byref(q_in),
                                                   C.byref(q_out), out.data_ptr(), L.stream()), "pk_plane_maxpool_requant")
     return out
+
+
+def plane_maxpool_requant_train(plane, b, c, h, w, k, s, p, q_in, q_out):
+    """plane_maxpool_requant of a QAFT training step (mnb_pk_plane_maxpool_requant_train, bf16 planes) -> (the consumer's
+    plane, window indices u8 [b][c/8][oh][ow][8], the consumer's STE mask bits8 [b][c/8][oh][ow])"""
+    oh, ow = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    out = consumer_plane(b, c, oh, ow, plane.device)
+    arg = torch.empty((b, c // 8, oh, ow, 8), dtype=torch.uint8, device=plane.device)
+    bits = consumer_bits(b, c, oh, ow, plane.device)
+    L.check(L.load().mnb_pk_plane_maxpool_requant_train(plane.data_ptr(), b, c, h, w, k, s, p, C.byref(q_in), C.byref(q_out),
+                                                        out.data_ptr(), arg.data_ptr(), bits.data_ptr(), L.stream()),
+            "pk_plane_maxpool_requant_train")
+    return out, arg, bits
+
+
+def plane_maxpool_requant_bwd(g, arg, bits, b, c, h, w, k, s, p, q_in):
+    """backward of plane_maxpool_requant_train through the pool quantizer's STE and the producer's mask ``bits`` (written by
+    the producer's epilogue) -> the producer's fp32 gradient [b, c, h, w]"""
+    dx = torch.empty((b, c, h, w), dtype=torch.float32, device=g.device)
+    L.check(L.load().mnb_pk_plane_maxpool_requant_bwd(g.data_ptr(), arg.data_ptr(), bits.data_ptr(), b, c, h, w, k, s, p,
+                                                      C.byref(q_in), dx.data_ptr(), L.stream()), "pk_plane_maxpool_requant_bwd")
+    return dx
 
 
 def pack_weight_i8(sh, w_int):
