@@ -101,7 +101,7 @@ def main():
     for h in handles:
         h.remove()
 
-    terms_dy = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    terms_dy = L.PK_TERMS_BWD
     want = {}
     for rec in calls:
         for k, b in producer_bytes(rec, terms_dy).items():

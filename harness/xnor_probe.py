@@ -1,6 +1,6 @@
 """XNOR-popcount forward (csrc/mnb_xnor.cu) against the packed-operand tensor-core forward (csrc/mnb_pk.cu) on the wbwtab
 layers of NIN-GC at the bench batch: CUDA events around each kernel, inputs rotated over 4 buffers.  The table this prints
-is the evidence for functional.xnor_preferred (north_star: the XNOR kernel is "picked when ncu shows it beating the
+is the evidence for the choice in functional._xnor_forward (north_star: the XNOR kernel is "picked when ncu shows it beating the
 tensor-core path").
 
     python -m harness.xnor_probe [--batch 256] [--json out.json]

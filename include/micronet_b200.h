@@ -654,7 +654,7 @@ int mnb_pk_gc3_conv_codes(const mnb_conv_shape* s, const void* a_pk, int32_t ter
  * Bit-packed XNOR-popcount forward for wbwtab layers (mnb_xnor.cu): binary activations (WB:11-36, sign with 0 -> +1)
  * times binary / ternary weights (WB:40-75, 98-146) as sum = popc(N) - 2 popc(N & (A ^ S)) on 1-bit planes; the integer
  * sum is exact, y = fmaf(sum, alpha[k], bias[k]) equals mnb_pk_conv's result bit for bit.  Forward only (the gradients
- * of a QAT step multiply real-valued dy).  functional.py picks it per layer (functional.xnor_preferred).
+ * of a QAT step multiply real-valued dy).  functional.py picks it per layer (functional._xnor_forward).
  *   a_bits : u32 [B][G][ceil(C/g / 32)][H][W], bit j of word n = [x[b][g*C/g + 32 n + j][h][w] is not < 0]
  *   w_img  : mnb_xnor_wimage_bytes() bytes, built from the i16 levels {-1, 0, +1} [K][C/g][R][S] of mnb_wb_weight_fwd
  * Cover: square filter 1/3/5, equal strides / pads, dilation 1, C/g <= 128 (3x3), <= 64 (5x5), <= 256 (1x1); else

@@ -263,34 +263,17 @@ USE_TC = os.environ.get("MNB_DISABLE_TC", "0") != "1"
 # layer; "all" = every conv it supports; "off" = never
 PK_MODE = os.environ.get("MNB_PK", "auto")
 # exact bf16 pieces per fp32 operand on the pk path (3 = exact 24-bit split; 2 = 16 bits, ~4e-6 relative)
-PK_TERMS = int(os.environ.get("MNB_PK_TERMS", "3"))
+PK_TERMS = 3
 # pieces of the fp32 operands of the BACKWARD convolutions (dy, the statistics conv's dpre, fp32 weights / inputs as their
 # second operand).  Two pieces = 16 significand bits: gradient errors of ~3e-6 of the largest element (inside the 1e-5
 # contract, every gradient check of the suite passes with margin) for 2/3 resp. 1/2 of the tensor-core work; nothing that
 # decides an integer level depends on them.  The forward statistics conv keeps PK_TERMS (its mean / variance decide the
-# quantized weight levels).  MNB_PK_TERMS_BWD=3 restores the exact split.
-PK_TERMS_BWD = int(os.environ.get("MNB_PK_TERMS_BWD", "2"))
+# quantized weight levels).  3 would restore the exact split.
+PK_TERMS_BWD = 2
 # wbwtab layers between two fused BatchNorm + binarizer producers (fused.BatchNormBinarize2d) take the packed-operand family
 # with BOTH operands written by the producers: +-1 planes forward (mnb_bn_sign_fwd_packed), gradient pieces backward
 # (mnb_bn_sign_bwd_pack); 3x3 layers take it in any case.  MNB_PK_WBWTAB=0 keeps every wbwtab layer on the fused kernels.
 PK_WBWTAB = os.environ.get("MNB_PK_WBWTAB", "1") == "1"
-# weight gradient of narrow grouped 3x3 layers (16 / 32 channels per group) on mnb_pk_wgrad_taps, all taps of a CTA in
-# registers; MNB_PK_WG_TAPS=0 keeps them on mnb_pk_wgrad (to compare the two in one process)
-PK_WG_TAPS = os.environ.get("MNB_PK_WG_TAPS", "1") != "0"
-# forward and data gradient of the same layers on mnb_pk_gc3_conv / mnb_pk_gc3_conv_codes (whole images as M tiles, the
-# weights of a block of groups resident in shared memory); MNB_PK_GC3=0 keeps them on mnb_pk_conv / mnb_pk_conv_codes
-PK_GC3 = os.environ.get("MNB_PK_GC3", "1") != "0"
-# data and weight gradient of the 1x1 grouped layers in one pass over dy on mnb_pk_bwd1x1; MNB_PK_BWD1X1=0 keeps them on
-# mnb_pk_conv + mnb_pk_wgrad (to compare the two in one process)
-PK_BWD1X1 = os.environ.get("MNB_PK_BWD1X1", "1") != "0"
-
-# bit-packed XNOR-popcount forward for wbwtab inference (mnb_xnor.cu): "auto" = the layers where it is expected to beat the
-# tensor-core forward (functional.xnor_preferred), "all" = wherever it has cover, "off" = never
-XNOR_MODE = os.environ.get("MNB_XNOR", "auto")
-
-# fused BatchNorm + binarizer producers whose only reader takes the bf16 operand plane skip their fp32 output (fused.py
-# _mark_plane_only); MNB_PLANE_ONLY=0 makes them write it again (e.g. to look at intermediate activations with hooks)
-PLANE_ONLY = os.environ.get("MNB_PLANE_ONLY", "1") == "1"
 
 _scratch = {}
 

@@ -40,7 +40,6 @@ struct Params {
   const float* x; const float* w; const float* bias; float* y;
   const float* dy; float* partial;
   int* err;
-  int dbg;   // MNB_FCONV_DEBUG bit mask (timing experiments only): 1 skip im2col/dy conversion, 2 skip MMAs, 4 skip stores/drain adds, 8 skip x conversion
 };
 
 struct alignas(16) Shared {
@@ -182,9 +181,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
         tc::zero_acc(acc0); tc::zero_acc(acc1);
         tc::wg_fence();
         tc::fence_acc(acc0); tc::fence_acc(acc1);
-        for (int q = (p.dbg & 2) ? 6 : 0; q < 6; ++q) {
+        for (int q = 0; q < 6; ++q) {
           const uint64_t aq = a_desc0 + (uint64_t)(ab * a_buf16 + (uint32_t)kProdA[q] * a_term16);
           const uint64_t bq = b_desc0 + (uint64_t)((uint32_t)kProdB[q] * b_term16 + (uint32_t)n0);
+          // kept rolled: unrolled, ptxas puts a warpgroup.arrive in a divergent path and waits after every wgmma (C7520)
+#pragma unroll 1
           for (int ks = 0; ks < p.KP / 16; ++ks) {
             const uint64_t ad = aq + (uint64_t)((uint32_t)ks * a_step16), bd = bq + (uint64_t)((uint32_t)ks * b_step16);
             tc::Mma<32>::bf16<0, 0>(acc0, ad, bd, 1);
@@ -202,7 +203,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
         tc::frag_to_smem(acc0, stage, tc::kStageLd, 0);
         tc::frag_to_smem(acc1, stage, tc::kStageLd, 64);
         mma_bar_sync();
-        if (p.dbg & 4) continue;
         // bias as vector loads from shared memory up front so that the store loop is a pure FADD + STG stream (a
         // per-element bias load serialises against the stores)
         float bs[32];
@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fwd_kernel(const Params p) {
       const uint32_t ab = p.nbuf_a == 2 ? (t & 1u) : 0u, aph = p.nbuf_a == 2 ? ((t >> 1) & 1u) : (t & 1u);
       if (!tc::mbar_wait(&sh.a_empty[ab], aph ^ 1u, p.err, 504)) break;
       uint8_t* abuf = aop + (size_t)ab * p.a_buf_bytes;
-      for (int i = (p.dbg & 1) ? items : ct; i < items; i += FWD_NCONV) {
+      for (int i = ct; i < items; i += FWD_NCONV) {
         const int j = i >> 7, m = i & 127;
         const int base = (m / p.W) * p.PW + (m % p.W);
         int off[8];
@@ -317,7 +317,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
       for (int sub = 0; sub < nsub; ++sub, ++it) {
         const uint32_t ob = it & 1u, oph = (it >> 1) & 1u;
         tc::mbar_wait_soft(&sh.a_full[ob], oph, p.err, 511, &sh.abort);
-        for (int hf = (p.dbg & 2) ? halves : 0; hf < halves; ++hf) {
+        for (int hf = 0; hf < halves; ++hf) {
           for (int k0 = 0; k0 < p.KP; k0 += 32) {
             float acc0[16], acc1[16];
             tc::zero_acc(acc0); tc::zero_acc(acc1);
@@ -336,7 +336,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
             tc::wg_commit();
             tc::wg_wait<0>();
             tc::fence_acc(acc0); tc::fence_acc(acc1);
-            if (p.dbg & 4) continue;
 #pragma unroll
             for (int j = 0; j < 4; ++j)
 #pragma unroll
@@ -408,20 +407,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_kernel(const Params p) {
         uint8_t* abuf = aop + (size_t)ob * p.a_buf_bytes;
         uint8_t* bbuf = bop + (size_t)ob * b_buf_bytes;
         // dy: item = (channel n, 8-position chunk j): 32 contiguous bytes of global memory
-        if (!(p.dbg & 1)) {
 #pragma unroll
-          for (int k = 0; k < DMAX; ++k) {
-            const int i = ct + k * WG_NCONV;
-            if (i < d_items) {
-              const int n = i / (SUB / 8), j = i - n * (SUB / 8);
-              const float v[8] = {dcur[k][0].x, dcur[k][0].y, dcur[k][0].z, dcur[k][0].w,
-                                  dcur[k][1].x, dcur[k][1].y, dcur[k][1].z, dcur[k][1].w};
-              store_split8(v, abuf + ((size_t)j * p.NP + n) * 16, p.a_term_bytes);
-            }
+        for (int k = 0; k < DMAX; ++k) {
+          const int i = ct + k * WG_NCONV;
+          if (i < d_items) {
+            const int n = i / (SUB / 8), j = i - n * (SUB / 8);
+            const float v[8] = {dcur[k][0].x, dcur[k][0].y, dcur[k][0].z, dcur[k][0].w,
+                                dcur[k][1].x, dcur[k][1].y, dcur[k][1].z, dcur[k][1].w};
+            store_split8(v, abuf + ((size_t)j * p.NP + n) * 16, p.a_term_bytes);
           }
         }
         // Xcol^T: item = (kk, 8-position chunk j): 8 consecutive patch columns
-        for (int i = (p.dbg & 8) ? x_items : ct; i < x_items; i += WG_NCONV) {
+        for (int i = ct; i < x_items; i += WG_NCONV) {
           const int kk = i / (SUB / 8), j = i - kk * (SUB / 8);
           const int m = sub * SUB + j * 8;
           const float* src = patch + tab[kk] + (m / p.W) * p.PW + (m % p.W);
@@ -893,11 +890,6 @@ static int plan_wgrad_wg(const mnb_conv_shape* s, Params& p, int& smem_bytes) {
   return 0;
 }
 
-static int debug_mask() {
-  static const int m = [] { const char* e = getenv("MNB_FCONV_DEBUG"); return e ? atoi(e) : 0; }();
-  return m;
-}
-
 }  // namespace tcfp32
 
 extern "C" int mnb_fconv2d_plan(const mnb_conv_shape* s, int32_t wgrad, int32_t* out, int32_t n) {
@@ -917,7 +909,7 @@ extern "C" int mnb_fconv2d_fwd_tc(const mnb_conv_shape* s, const float* x, const
   Params p{};
   int smem_bytes = 0;
   if (int e = plan(s, false, p, smem_bytes)) return e;
-  p.x = x; p.w = w; p.bias = bias; p.y = y; p.err = err_flag; p.dbg = debug_mask();
+  p.x = x; p.w = w; p.bias = bias; p.y = y; p.err = err_flag;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t ce = cudaFuncSetAttribute(fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
@@ -965,7 +957,7 @@ extern "C" int mnb_fconv2d_wgrad_tc(const mnb_conv_shape* s, const float* dy, co
   Params p{};
   int smem_bytes = 0;
   if (int e = plan(s, true, p, smem_bytes)) return e;
-  p.x = x; p.dy = dy; p.partial = reinterpret_cast<float*>(scratch); p.err = err_flag; p.dbg = debug_mask();
+  p.x = x; p.dy = dy; p.partial = reinterpret_cast<float*>(scratch); p.err = err_flag;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t ce = cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);

@@ -47,7 +47,6 @@ struct Params {
   int npos_in, row_tiles, n_tiles, slab_groups, n_slabs;
   int quant_mode;   // 0: raw fp32 input (exact 3-term split); else MNB_ACT_DOREFA / MNB_ACT_IAO
   int dgrad;        // 1: weights transposed + flipped, per-input-channel pre-scale, STE epilogue
-  int dbg;          // MNB_TC_DEBUG (timing experiments only): 1 no converter fence, 2 no converter work, 4 no epilogue stores, 8 no MMAs
   int a_offset;
   int stage_bytes, op_term_bytes, op_buf_bytes, b_group_bytes, off_stage, off_op, off_b, off_stg;
   float a_scale_const;
@@ -238,7 +237,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
           const uint64_t a_chunk = a_desc0 + (uint64_t)((uint32_t)ob * a_buf);
           const uint64_t b_chunk_d = b_desc0 + (uint64_t)((uint32_t)gi * b_group + (uint32_t)ch * b_chunk);
           const long long tmma0 = p.prof ? clock64() : 0;
-          const int n_off = (p.dbg & 8) ? 0 : p.R * p.S * ksteps;
+          const int n_off = p.R * p.S * ksteps;
           tc::wg_fence();
           tc::fence_acc(acc);
           if (max_terms == 3 && need_low) {
@@ -269,7 +268,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
           tc::frag_cols_to_smem(acc, stage, tc::kStageLd64, 0, c0, 32);
           wg_bar_sync(wg);
           const int nb = gcol + c0 + 16 * ehalf;   // first slab column of this thread
-          if (c0 + 16 * ehalf >= NG || !valid || (p.dbg & 4)) continue;
+          if (c0 + 16 * ehalf >= NG || !valid) continue;
           float r[16];
 #pragma unroll
           for (int j = 0; j < 16; ++j) r[j] = stage[(16 * ehalf + j) * tc::kStageLd64 + (lt & 63)];
@@ -365,7 +364,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
           uint32_t any_low = 0;
 #pragma unroll
           for (int k = 0; k < KMAX; ++k) {
-            if ((ct & ~31) + k * NCONV >= total || (p.dbg & 2)) break;  // warp-uniform
+            if ((ct & ~31) + k * NCONV >= total) break;  // warp-uniform
             const int idx = ct + k * NCONV;
             const bool live = idx < total;
             const int so = soff[k];
@@ -460,7 +459,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const Params p) {
             any_low = __reduce_or_sync(0xffffffffu, any_low);
             if (lane == 0) sh.op_flags[ob][cw] = any_low;
           }
-          if (!(p.dbg & 1)) tc::fence_proxy_async_smem();   // every writer publishes its smem stores to the async proxy
+          tc::fence_proxy_async_smem();   // every writer publishes its smem stores to the async proxy
           __syncwarp();
           if (lane == 0) {                // one arrival per warp: 16 instead of 512 smem atomics per chunk
             tc::mbar_arrive(&sh.op_full[ob]);
@@ -625,10 +624,6 @@ static int launch(const Params& p, const void* in, int smem_bytes, cudaStream_t 
   const int grid = grid_size(p);
   Params pp = p;
   pp.prof = g_prof_buffer;
-  {
-    static const int dbg = [] { const char* e = getenv("MNB_TC_DEBUG"); return e ? atoi(e) : 0; }();
-    pp.dbg = dbg;
-  }
   {
     const int ks = p.CC / 16, c8_per_group = p.cin_g / 8;
     for (int e = 0; e < p.R * p.S * ks && e < 64; ++e) {

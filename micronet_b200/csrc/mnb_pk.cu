@@ -1115,7 +1115,6 @@ struct ConvParams {
   const uint8_t* w_img;
   // epilogue
   int B, THH, BW, OHr, OWr, OH, OW, omul, ny, ng, Nt, NOUT, C8O, smem_bytes, off_stg, mode;
-  int dbg;                  // MNB_PK_DEBUG (timing experiments only): 1 no epilogue stores, 2 no MMAs
   const float* n_scale;     // [NOUT] per-output-channel scale or NULL
   const float* a_scale;     // device scalar multiplied into n_scale, or NULL
   float a_scale_const;
@@ -1223,12 +1222,10 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           for (int cc = 0; cc < p.chunks; ++cc, ++sc) {
             const uint32_t slot = sc & (uint32_t)p.st_mask, ph = (sc >> p.st_log2) & 1u;
             if (!tc::mbar_wait(&sh.empty[slot], ph ^ 1u, p.err, 701)) goto done;
-            // MNB_PK_DEBUG bits 8 / 16 (timing experiments only): leave out the activation boxes / the weight block
-            const bool ld_a = !(p.dbg & 8), ld_b = !(p.dbg & 16);
-            tc::mbar_arrive_expect_tx(&sh.full[slot], (ld_a ? (uint32_t)(p.MT * p.TA * p.a_box_bytes) : 0u) + (ld_b ? blk : 0u));
+            tc::mbar_arrive_expect_tx(&sh.full[slot], (uint32_t)(p.MT * p.TA * p.a_box_bytes) + blk);
             uint8_t* sbase = smem + (size_t)slot * p.stage_bytes;
             const int c8 = kph * p.C8A + g * p.kg8 + cc * p.CC8;
-            for (int mt = 0; mt < (ld_a ? p.MT : 0); ++mt) {
+            for (int mt = 0; mt < p.MT; ++mt) {
               const uint32_t tile = mg * (uint32_t)p.MT + (uint32_t)mt;
               uint32_t ct, r2, rt, bt;
               d_ct.divmod(tile, r2, ct);
@@ -1238,7 +1235,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
               if (p.TA > 1) tc::tma_load_4d(sbase + (size_t)(mt * p.TA + 1) * p.a_bytes, &tmap1, &sh.full[slot], 2 * cw, chh, cb, c8);
               if (p.TA > 2) tc::tma_load_4d(sbase + (size_t)(mt * p.TA + 2) * p.a_bytes, &tmap2, &sh.full[slot], 2 * cw, chh, cb, c8);
             }
-            if (ld_b) tc::bulk_load_1d(sbase + p.b_off, bsrc + (size_t)cc * blk, blk, &sh.full[slot]);
+            tc::bulk_load_1d(sbase + p.b_off, bsrc + (size_t)cc * blk, blk, &sh.full[slot]);
           }
         }
       }
@@ -1312,26 +1309,24 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
           tc::wg_fence();
 #pragma unroll
           for (int mt = 0; mt < MAXMT; ++mt) tc::fence_acc(acc[mt]);
-          if (!(p.dbg & 2)) {
 #pragma unroll
-            for (int mt = 0; mt < MAXMT; ++mt) {
-              if (mt >= (int)p.m.MT) break;
-              const uint32_t a_base = a_lo0 + s16 + (uint32_t)mt * p.m.a_mt16, b_base = b_lo0 + s16;
-              // flat program: one word per MMA of this stage template (tap x piece pair x K-step) = A offset | B offset << 16,
-              // padded with 0xffffffff to groups of four
-              for (uint32_t e = 0; e < pc; ++e) {
-                const uint4 w4 = p.m.prog4[pb + e];
-                const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
+          for (int mt = 0; mt < MAXMT; ++mt) {
+            if (mt >= (int)p.m.MT) break;
+            const uint32_t a_base = a_lo0 + s16 + (uint32_t)mt * p.m.a_mt16, b_base = b_lo0 + s16;
+            // flat program: one word per MMA of this stage template (tap x piece pair x K-step) = A offset | B offset << 16,
+            // padded with 0xffffffff to groups of four
+            for (uint32_t e = 0; e < pc; ++e) {
+              const uint4 w4 = p.m.prog4[pb + e];
+              const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  if (w[k] == 0xffffffffu) continue;
-                  if constexpr (I8)   // s32 accumulators in the registers of acc (zero bits = 0 either way)
-                    tc::Mma<NT>::s8(reinterpret_cast<int32_t(&)[NR]>(acc[mt]), a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
-                                    b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
-                  else
-                    tc::Mma<NT>::template bf16<0, 0>(acc[mt], a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
-                                                      b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
-                }
+              for (int k = 0; k < 4; ++k) {
+                if (w[k] == 0xffffffffu) continue;
+                if constexpr (I8)   // s32 accumulators in the registers of acc (zero bits = 0 either way)
+                  tc::Mma<NT>::s8(reinterpret_cast<int32_t(&)[NR]>(acc[mt]), a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
+                                  b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
+                else
+                  tc::Mma<NT>::template bf16<0, 0>(acc[mt], a_hi | (uint64_t)(a_base + (w[k] & 0xffffu)),
+                                                    b_hi | (uint64_t)(b_base + (w[k] >> 16)), 1);
               }
             }
           }
@@ -1395,7 +1390,7 @@ pk_conv_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant_
             if (XPOST && !I8 && p.post_bits) qrow = p.post_bits + (int64_t)b * p.C8O * plane + (int64_t)oh * p.OW + ow;
           }
         }
-        if (!valid || n0 >= n_cnt || (p.dbg & 1)) return;
+        if (!valid || n0 >= n_cnt) return;
         if (!SEG && !I8 && p.codes) {   // exact integer sums (|r| <= 32767: checked on the host) as int16
           int16_t* cp = p.codes + orow + (int64_t)n0 * plane;
 #pragma unroll
@@ -3277,7 +3272,6 @@ static int pk_conv_impl(const mnb_conv_shape* s, int32_t mode, const void* a_pk,
     p.post_terms = terms_out ? post->terms_out : 0;
     p.post_bits = post_bits;
   }
-  { static const int dbg = [] { const char* e = getenv("MNB_PK_DEBUG"); return e ? atoi(e) : 0; }(); p.dbg = dbg; }
   CUtensorMap tm[3];
   const int C8tot = pl.nkph * pl.C8A;
   const int64_t plane_bytes = (int64_t)pl.B * C8tot * pl.HA * pl.WA * 16;

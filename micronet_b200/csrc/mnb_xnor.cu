@@ -2,7 +2,7 @@
 //
 // BASELINE.json north_star: "the wbwtab binary/ternary case additionally gets a bit-packed XNOR-popcount kernel picked
 // when ncu shows it beating the tensor-core path".  This file is that kernel; harness/xnor_probe.py times it against the
-// packed-operand tensor-core forward (mnb_pk.cu) layer by layer and functional.xnor_preferred picks per layer (DESIGN.md 4.12).
+// packed-operand tensor-core forward (mnb_pk.cu) layer by layer and functional._xnor_forward picks per layer (DESIGN.md 4.12).
 //
 // Reference math (WB:11-36, 55-75, 98-146, 181-195): y = bias + alpha[k] * sum_{c,r,s} a[c] * w[k][c][r][s] with
 // a = sign(x) in {-1, +1} (0 -> +1) and w in {-1, +1} (binary) or {-1, 0, +1} (ternary); out-of-image taps contribute 0.

@@ -316,19 +316,6 @@ def materialized(t):
     return plane.permute(0, 1, 4, 2, 3).reshape(b, c, h, w).float()
 
 
-def xnor_preferred(sh, has_plane):
-    """MNB_XNOR=auto: take the XNOR-popcount forward for this wbwtab inference layer?
-
-    * both convolution kernels are dominated by the fp32 output they write, and the popc pipe gives the bit kernel no
-      arithmetic edge over the tensor cores on +-1 operands;
-    * the operand it reads is 16 x smaller (1 bit vs one bf16 per activation), so a layer that has to pack its own input
-      saves most of its pack pass (harness/xnor_probe.py times both forms layer by layer; not yet measured on the H100).
-
-    Hence: XNOR when the layer packs its own operand (no producer-written plane came with x), the tensor-core forward when a
-    fused BatchNorm + binarizer already wrote the bf16 plane (the pack pass is free there)."""
-    return not has_plane
-
-
 def _pk_terms(spec, w_int, pm1=False):
     """(terms of the activation operand, terms of the weight operand) on the packed-operand path; ``pm1``: the raw input is
     known to hold only +-1 (output of a binarizer): one bf16 piece is exact"""
@@ -357,7 +344,7 @@ def _pk_forward(ctx, x, wq, bias, w_int, w_scale, spec, sh, y, prepacked=None, p
     if not PK.supported(sh, 0, ta, tw):
         return False
     # the backward of a layer stays in the family its forward ran in (saved operands are packed): check its cover now
-    Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    Tb = L.PK_TERMS_BWD
     if need_dx and not PK.supported(sh, 1, Tb, 1 if w_int is not None else Tb):
         return False
     if need_dw and not PK.wgrad_supported(sh, Tb, min(ta, Tb)):
@@ -411,7 +398,7 @@ def _pk_backward(ctx, dy):
     """data and weight gradients of a layer whose forward ran on the packed-operand path"""
     from . import pk as PK
     sh = ctx.sh
-    T = min(L.PK_TERMS, L.PK_TERMS_BWD)     # pieces of dy and of an fp32 second operand (see _lib.PK_TERMS_BWD)
+    T = L.PK_TERMS_BWD     # pieces of dy and of an fp32 second operand (see _lib.PK_TERMS_BWD)
     int_w = ctx.w_int is not None
     need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
     # dy is packed once for both gradients; the data gradient wants the per-channel weight scale folded in (it sits on
@@ -454,11 +441,17 @@ def _pk_backward(ctx, dy):
 
 def _xnor_forward(x, w_int, w_scale, bias, sh, y, groups):
     """wbwtab inference forward on +-1 activations: bit-packed XNOR-popcount kernel where it is expected to beat the
-    tensor-core forward (xnor_preferred).  Same integer sums, same fmaf epilogue: bit-identical to the packed-operand
-    path.  Only taken where no backward follows (training steps multiply real-valued gradients and want the bf16 operand
-    plane the forward already read), so it saves nothing."""
+    tensor-core forward.  Same integer sums, same fmaf epilogue: bit-identical to the packed-operand path.  Only taken
+    where no backward follows (training steps multiply real-valued gradients and want the bf16 operand plane the forward
+    already read), so it saves nothing."""
     from . import xnor as XN
-    if not (XN.supported(sh) and (L.XNOR_MODE == "all" or xnor_preferred(sh, getattr(x, "_mnb_pk_pm1", None) is not None))):
+    # Both convolution kernels are dominated by the fp32 output they write, and the popc pipe gives the bit kernel no
+    # arithmetic edge over the tensor cores on +-1 operands.  The operand it reads is 16 x smaller (1 bit vs one bf16 per
+    # activation), so a layer that has to pack its own input saves most of its pack pass (harness/xnor_probe.py times both
+    # forms layer by layer; not yet measured on the H100).  Hence XNOR only when no producer-written plane came with x;
+    # where a fused BatchNorm + binarizer already wrote the bf16 plane, the pack pass is free and the tensor-core forward
+    # runs.
+    if not XN.supported(sh) or getattr(x, "_mnb_pk_pm1", None) is not None:
         return False
     a_bits = XN.pack_act(materialized(x), groups)
     rc = _timed("fwd_xnor", sh, lambda: XN.conv(sh, a_bits, XN.pack_weight(sh, w_int), y, alpha=w_scale, bias=bias))
@@ -663,7 +656,7 @@ class QuantConv2dFn(Function):
         plane_only = getattr(x, "_mnb_plane_only", False)
         if plane_only and padded_in:
             x, plane_only = materialized(x), False
-        if (L.XNOR_MODE != "off" and spec is None and w_int is not None and pm1 and not pre_relu
+        if (spec is None and w_int is not None and pm1 and not pre_relu
                 and (no_grad or not any(ctx.needs_input_grad[:3])) and _xnor_forward(x, w_int, w_scale, bias, sh, y, groups)):
             family = "xnor"
         elif handed is not None:
@@ -817,7 +810,7 @@ class ConvTranspose2dFn(Function):
         sh = ctx.sh
         gy = gy.contiguous()
         gx = gw = gb = None
-        T = min(L.PK_TERMS, L.PK_TERMS_BWD)
+        T = L.PK_TERMS_BWD
         if ctx.needs_input_grad[0]:
             gx = torch.empty_like(x)
             if not _pk_plain(sh, 0, gy, w, gx, T):
@@ -925,7 +918,7 @@ def train_consumer_ok(consumer, out_shape):
     if not consumer.accepts(act):
         return False
     sh = _shape_struct(act, consumer.w_shape, consumer.stride, consumer.padding, consumer.dilation, consumer.groups)
-    Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    Tb = L.PK_TERMS_BWD
     return PK.supported(sh, 1, Tb, 1) and PK.wgrad_supported(sh, Tb, 1)
 
 

@@ -73,7 +73,7 @@ class BNSignFn(Function):
                 plane = torch.empty(x.numel() * 2, dtype=torch.uint8, device=x.device)
                 # plane_only (set by the rewrite pass when the ONLY reader is a conv of the packed-operand family): the fp32
                 # tensor is a shape-carrying placeholder, 4 of the 10 bytes per element this pass moved are never written
-                skip_y = bool(plane_only) and L.PLANE_ONLY
+                skip_y = bool(plane_only)
                 fn, xa = _xargs(lib, "mnb_bn_sign_fwd_packed", x, codes)
                 rc = fn(*xa, b, c, hw, mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(), beta.data_ptr(), shuffle_groups,
                         None if skip_y else y.data_ptr(), bits.data_ptr(), plane.data_ptr(), L.stream())
@@ -397,7 +397,7 @@ class EnginePmConv2d(nn.Conv2d):
         if (getattr(input, "_mnb_pm1", False) and L.PK_MODE != "off" and input.is_cuda and input.dtype == torch.float32
                 and input.dim() == 4 and self.padding_mode == "zeros" and not isinstance(self.padding, str)):
             sh = F_._shape_struct(input.shape, self.weight.shape, self.stride, self.padding, self.dilation, self.groups)
-            T, Tb = L.PK_TERMS, min(L.PK_TERMS, L.PK_TERMS_BWD)
+            T, Tb = L.PK_TERMS, L.PK_TERMS_BWD
             if (PK.supported(sh, 0, 1, T) and PK.supported(sh, 1, Tb, Tb) and PK.wgrad_supported(sh, Tb, 1)):
                 return F_.quant_conv2d(input, self.weight, self.bias, None, None, None, self.stride, self.padding,
                                        self.dilation, self.groups)

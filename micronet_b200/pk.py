@@ -11,8 +11,9 @@ shared memory, stride 2, 5x5 filters, 4x4 or 224x224 images ...) and every fused
     gc3_conv    forward / data gradient of the same layers with whole images as M tiles (same result as conv)
     bwd1x1      data gradient and weight gradient of a 1x1 layer in one pass over dy (same results as conv + wgrad)
 
-The layers of the engine go through run_conv / run_conv_codes / run_wgrad / run_bwd, which pick among those kernels
-(``PK_GC3``, ``PK_WG_TAPS``, ``PK_BWD1X1``); the single-kernel calls stay for tests and probes that compare the kernels directly.
+The layers of the engine go through run_conv / run_conv_codes / run_wgrad / run_bwd, which pick among those kernels by
+their plans alone: gc3_conv, wgrad_taps and bwd1x1 wherever their plans cover the shape.  The single-kernel calls serve
+every other shape, and tests and probes call them to compare the kernels directly.
 
 Reference math: F.conv2d of the fake-quantized tensors (WB:186, DF:113, IAO:498/843/947) and ATen's
 convolution_backward."""
@@ -420,9 +421,9 @@ def gc3_conv_codes(sh, a_pk, w_img, codes, dec, n_scale=None, a_scale=None, a_sc
 
 # ---- kernel choice of the engine's layers
 def run_conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, **epilogue):
-    """forward (mode 0) or data gradient (mode 1) with conv's arguments: on gc3_conv where its plan covers the shape and
-    PK_GC3 allows, on conv otherwise and for whatever gc3_conv refuses.  Returns the C status."""
-    if L.PK_GC3 and gc3_plan(sh, mode, terms_a, terms_w) is not None:
+    """forward (mode 0) or data gradient (mode 1) with conv's arguments: on gc3_conv where its plan covers the shape, on
+    conv otherwise and for whatever gc3_conv refuses.  Returns the C status."""
+    if gc3_plan(sh, mode, terms_a, terms_w) is not None:
         rc = gc3_conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, **epilogue)
         if rc != L.E_UNSUPPORTED:
             return rc
@@ -431,7 +432,7 @@ def run_conv(sh, mode, a_pk, terms_a, w_img, terms_w, out, **epilogue):
 
 def run_conv_codes(sh, a_pk, w_img, codes, dec, **epilogue):
     """conv_codes with the same choice as run_conv: gc3_conv_codes first where it applies.  Returns the C status."""
-    if L.PK_GC3 and gc3_plan(sh, 0, 1, 1) is not None:
+    if gc3_plan(sh, 0, 1, 1) is not None:
         rc = gc3_conv_codes(sh, a_pk, w_img, codes, dec, **epilogue)
         if rc != L.E_UNSUPPORTED:
             return rc
@@ -439,21 +440,21 @@ def run_conv_codes(sh, a_pk, w_img, codes, dec, **epilogue):
 
 
 def run_wgrad(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=None, kdiv=None):
-    """weight gradient with wgrad's arguments: on wgrad_taps where its plan covers the shape and PK_WG_TAPS allows, on
-    wgrad otherwise.  Returns the C status."""
-    fn = wgrad_taps if L.PK_WG_TAPS and wgrad_taps_plan(sh, terms_dy, terms_x) is not None else wgrad
+    """weight gradient with wgrad's arguments: on wgrad_taps where its plan covers the shape, on wgrad
+    otherwise.  Returns the C status."""
+    fn = wgrad_taps if wgrad_taps_plan(sh, terms_dy, terms_x) is not None else wgrad
     return fn(sh, dy_pk, terms_dy, x_pk, terms_x, dw, a_scale=a_scale, kdiv=kdiv)
 
 
 def bwd1x1_taken(sh, terms_dy, terms_x, terms_w):
     """does run_bwd take mnb_pk_bwd1x1 for this layer?"""
-    return L.PK_BWD1X1 and bwd1x1_plan(sh, terms_dy, terms_x, terms_w) is not None
+    return bwd1x1_plan(sh, terms_dy, terms_x, terms_w) is not None
 
 
 def run_bwd(sh, dy_pk, terms_dy, x_pk, terms_x, w_img, terms_w, dx, dw, bits8=None, gain=1.0, a_scale_const=1.0, a_scale=None,
             kdiv=None):
-    """data and weight gradient: on bwd1x1 where its plan covers the shape and PK_BWD1X1 allows, otherwise run_conv
-    (mode 1) followed by run_wgrad.  Returns the C status of the first call that fails, or 0."""
+    """data and weight gradient: on bwd1x1 where its plan covers the shape, otherwise run_conv (mode 1)
+    followed by run_wgrad.  Returns the C status of the first call that fails, or 0."""
     if bwd1x1_taken(sh, terms_dy, terms_x, terms_w):
         return bwd1x1(sh, dy_pk, terms_dy, x_pk, terms_x, w_img, terms_w, dx, dw, bits8=bits8, gain=gain,
                       a_scale_const=a_scale_const, a_scale=a_scale, kdiv=kdiv)

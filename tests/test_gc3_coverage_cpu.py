@@ -236,7 +236,7 @@ def _bench_launches():
     """(workload, layer, mode, shape, pieces) of every gc3 launch of a bench step at batch 256: the forward and the data
     gradient of the grouped 3x3 layers, at the piece counts the engine gives them"""
     from micronet_b200 import _lib as L, functional as F_
-    Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    Tb = L.PK_TERMS_BWD
     out = []
     for name, B, Cc, H, W, K, R, st, pad, G in PU.model_convs():
         if not name.startswith("gc") or R != 3:

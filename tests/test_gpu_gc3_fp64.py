@@ -292,10 +292,10 @@ def test_refused_launch_writes_nothing(ref, monkeypatch):
 
 
 @pytest.mark.parametrize("fuse", [True, False], ids=["fused", "unfused"])
-def test_dorefa_w4a4_step_runs_gc3_and_matches_the_other_kernels(fuse):
+def test_dorefa_w4a4_step_runs_gc3_and_matches_the_plain_kernels(fuse):
     """one QAT step of the bench DoReFa W4A4 NIN-GC model (fused producers, and un-fused): both grouped 3x3 layers run the
     gc3 forward (a_scale_const 1/15), the gc3 data gradient (the STE mask with the gain 0.1) and the taps weight gradient,
-    and the loss and every gradient are bit-identical to the step with MNB_PK_GC3 / MNB_PK_WG_TAPS off"""
+    and the loss and every gradient are bit-identical to the step with gc3_plan and wgrad_taps_plan forced to refuse"""
     from harness import train as H
     from micronet_b200 import _lib as L, pk as PK
     w = H.WORKLOADS["nin_gc_dorefa_w4a4"]
@@ -304,6 +304,7 @@ def test_dorefa_w4a4_step_runs_gc3_and_matches_the_other_kernels(fuse):
     x, t = H.synthetic_batch(8, w["hw"], seed=11, device=DEV)
     calls = []
     real = (PK.gc3_conv, PK.gc3_conv_codes, PK.wgrad_taps)
+    plans = (PK.gc3_plan, PK.wgrad_taps_plan)
 
     def spy_conv(sh, mode, *args, **kw):
         calls.append((sh.in_c, sh.groups, "fwd" if mode == 0 else "dgrad", kw.get("bits8") is not None,
@@ -319,11 +320,10 @@ def test_dorefa_w4a4_step_runs_gc3_and_matches_the_other_kernels(fuse):
         return real[2](sh, *args, **kw)
 
     res = {}
-    saved = (L.PK_GC3, L.PK_WG_TAPS)
     try:
         PK.gc3_conv, PK.gc3_conv_codes, PK.wgrad_taps = spy_conv, spy_codes, spy_taps
         for on in (False, True):
-            L.PK_GC3 = L.PK_WG_TAPS = on
+            PK.gc3_plan, PK.wgrad_taps_plan = plans if on else (lambda *a: None, lambda *a: None)
             n_calls = len(calls)
             m = copy.deepcopy(base).to(DEV).train()
             loss = torch.nn.functional.cross_entropy(m(x), t)
@@ -333,8 +333,8 @@ def test_dorefa_w4a4_step_runs_gc3_and_matches_the_other_kernels(fuse):
                 assert len(calls) == n_calls, calls[n_calls:]
             res[on] = (loss.detach(), {n: p.grad.detach().clone() for n, p in m.named_parameters() if p.grad is not None})
     finally:
-        L.PK_GC3, L.PK_WG_TAPS = saved
         PK.gc3_conv, PK.gc3_conv_codes, PK.wgrad_taps = real
+        PK.gc3_plan, PK.wgrad_taps_plan = plans
     L.tc_check()
     # (mask, a_scale_const, gain) of a data gradient: a max-pool sits between each grouped layer and the BatchNorm + ReLU +
     # quantizer in front of it, so even the fused model packs the layer's input in the conv and keeps the STE mask bits8 with

@@ -386,7 +386,7 @@ def _teacher_forced(om, em, x, t, wtol=TOL):
                 tol = wtol if flips == 0 else 5e-3
                 if bnfuse and k in ("gamma", "beta") and L.PK_TERMS_BWD < 3 and flips == 0:
                     # 2-piece (16 significand bits) gradient operands of the packed-operand backward: 2^-17 relative per
-                    # element of dy, see _lib.PK_TERMS_BWD (MNB_PK_TERMS_BWD=3 restores the exact split: <= 1e-5 then)
+                    # element of dy, see _lib.PK_TERMS_BWD (PK_TERMS_BWD = 3 restores the exact split: <= 1e-5 then)
                     tol = 2 * wtol
                 if dorefa and k == "weight":
                     am = torch.tanh(dict(o.named_parameters())[k].detach()).abs().flatten().argmax()

@@ -134,27 +134,26 @@ def test_synthetic(case, terms, mask):
     _check(case, terms, 7 + SYNTH.index((case, terms)), mask, levels=terms[2] == 1)
 
 
-def test_headline_model_step_fused_and_separate():
-    """one QAT step of the fused NIN-GC wbwtab W3/A2 model with MNB_PK_BWD1X1=0 and =1: the fused kernel runs for exactly
-    the five 1x1 grouped layers, and the loss and every gradient are bit-identical"""
+def test_headline_model_step_with_and_without_the_bwd1x1_plan():
+    """one QAT step of the fused NIN-GC wbwtab W3/A2 model with bwd1x1_plan forced to refuse every shape and as it is: the
+    fused kernel runs for exactly the five 1x1 grouped layers, and the loss and every gradient are bit-identical"""
     from harness import train as H
     from micronet_b200 import _lib as L, pk as PK
     w = H.WORKLOADS["nin_gc_wbwtab_w3a2"]
     base = H.prepare_engine(H.build_float_model(w["model"]), w["scheme"], **w["prepare"], **w["engine_extra"])
     x, t = H.synthetic_batch(16, w["hw"], seed=5, device=DEV)
     calls = []
-    real = PK.bwd1x1
+    real, real_plan = PK.bwd1x1, PK.bwd1x1_plan
 
     def spy(sh, *args, **kw):
         calls.append((sh.in_c, sh.out_c, sh.groups))
         return real(sh, *args, **kw)
 
     res = {}
-    saved = L.PK_BWD1X1
     try:
         PK.bwd1x1 = spy
         for on in (False, True):
-            L.PK_BWD1X1 = on
+            PK.bwd1x1_plan = real_plan if on else (lambda *a: None)   # bwd1x1 reads it too: only on the old leg
             n_calls = len(calls)
             m = copy.deepcopy(base).to(DEV).train()
             loss = torch.nn.functional.cross_entropy(m(x), t)
@@ -163,7 +162,7 @@ def test_headline_model_step_fused_and_separate():
             assert len(calls) - n_calls == (5 if on else 0)
             res[on] = (loss.detach(), {n: p.grad.detach().clone() for n, p in m.named_parameters() if p.grad is not None})
     finally:
-        L.PK_BWD1X1, PK.bwd1x1 = saved, real
+        PK.bwd1x1, PK.bwd1x1_plan = real, real_plan
     L.tc_check()
     assert sorted(calls) == sorted([(256, 256, 2)] * 2 + [(512, 512, 4)] * 2 + [(1024, 1024, 8)]), calls
     assert torch.equal(res[False][0], res[True][0])

@@ -107,16 +107,17 @@ def test_data_gradient(case, mask):
     _same(outs["again"], outs["old"], "data gradient (second run)")
 
 
-def test_headline_model_step_old_and_new_kernels():
-    """one QAT step of the fused NIN-GC wbwtab W3/A2 model with MNB_PK_GC3=0 and =1: the new kernels run for exactly the
-    forward and the data gradient of the two grouped 3x3 layers, and the loss and every gradient are bit-identical"""
+def test_headline_model_step_with_and_without_the_gc3_plan():
+    """one QAT step of the fused NIN-GC wbwtab W3/A2 model with gc3_plan forced to refuse every shape and as it is: the new
+    kernels run for exactly the forward and the data gradient of the two grouped 3x3 layers, and the loss and every gradient
+    are bit-identical"""
     from harness import train as H
     from micronet_b200 import _lib as L, pk as PK
     w = H.WORKLOADS["nin_gc_wbwtab_w3a2"]
     base = H.prepare_engine(H.build_float_model(w["model"]), w["scheme"], **w["prepare"], **w["engine_extra"])
     x, t = H.synthetic_batch(16, w["hw"], seed=5, device=DEV)
     calls = []
-    real = (PK.gc3_conv, PK.gc3_conv_codes)
+    real = (PK.gc3_conv, PK.gc3_conv_codes, PK.gc3_plan)
 
     def spy_conv(sh, mode, *args, **kw):
         calls.append((sh.in_c, sh.out_c, sh.groups, "fwd" if mode == 0 else "dgrad"))
@@ -127,11 +128,10 @@ def test_headline_model_step_old_and_new_kernels():
         return real[1](sh, *args, **kw)
 
     res = {}
-    saved = L.PK_GC3
     try:
         PK.gc3_conv, PK.gc3_conv_codes = spy_conv, spy_codes
         for on in (False, True):
-            L.PK_GC3 = on
+            PK.gc3_plan = real[2] if on else (lambda *a: None)
             n_calls = len(calls)
             m = copy.deepcopy(base).to(DEV).train()
             loss = torch.nn.functional.cross_entropy(m(x), t)
@@ -140,8 +140,7 @@ def test_headline_model_step_old_and_new_kernels():
             assert len(calls) - n_calls == (4 if on else 0)
             res[on] = (loss.detach(), {n: p.grad.detach().clone() for n, p in m.named_parameters() if p.grad is not None})
     finally:
-        L.PK_GC3 = saved
-        PK.gc3_conv, PK.gc3_conv_codes = real
+        PK.gc3_conv, PK.gc3_conv_codes, PK.gc3_plan = real
     L.tc_check()
     assert sorted(calls) == [(256, 512, 16, "dgrad"), (256, 512, 16, "fwd"), (512, 1024, 32, "dgrad"),
                              (512, 1024, 32, "fwd")], calls
@@ -151,16 +150,16 @@ def test_headline_model_step_old_and_new_kernels():
         assert torch.equal(res[False][1][n], res[True][1][n]), n
 
 
-def test_refused_launches_fall_back_to_mnb_pk_conv():
+def test_refused_gc3_launches_fall_back_to_mnb_pk_conv():
     """a shape the plan covers but whose launch mnb_pk_gc3_conv* refuses (MNB_E_UNSUPPORTED, e.g. an unaligned tensor) runs on
     mnb_pk_conv / mnb_pk_conv_codes instead: the step still takes the packed-operand path and gives the same loss and
-    gradients as with MNB_PK_GC3=0"""
+    gradients as with gc3_plan forced to refuse every shape"""
     from harness import train as H
     from micronet_b200 import _lib as L, pk as PK
     w = H.WORKLOADS["nin_gc_wbwtab_w3a2"]
     base = H.prepare_engine(H.build_float_model(w["model"]), w["scheme"], **w["prepare"], **w["engine_extra"])
     x, t = H.synthetic_batch(8, w["hw"], seed=9, device=DEV)
-    real = (PK.gc3_conv, PK.gc3_conv_codes, PK.conv, PK.conv_codes)
+    real = (PK.gc3_conv, PK.gc3_conv_codes, PK.conv, PK.conv_codes, PK.gc3_plan)
     refused, old_calls = [], []
 
     def refuse(sh, *args, **kw):
@@ -176,11 +175,10 @@ def test_refused_launches_fall_back_to_mnb_pk_conv():
         return real[3](sh, *args, **kw)
 
     res = {}
-    saved = L.PK_GC3
     try:
         PK.conv, PK.conv_codes = count_conv, count_codes
         for on in (False, True):
-            L.PK_GC3 = on
+            PK.gc3_plan = real[4] if on else (lambda *a: None)
             PK.gc3_conv, PK.gc3_conv_codes = (refuse, refuse) if on else real[:2]
             n_old = len(old_calls)
             m = copy.deepcopy(base).to(DEV).train()
@@ -190,8 +188,7 @@ def test_refused_launches_fall_back_to_mnb_pk_conv():
             res[on] = (loss.detach(), {n: p.grad.detach().clone() for n, p in m.named_parameters() if p.grad is not None},
                        sorted(old_calls[n_old:]))
     finally:
-        L.PK_GC3 = saved
-        PK.gc3_conv, PK.gc3_conv_codes, PK.conv, PK.conv_codes = real
+        PK.gc3_conv, PK.gc3_conv_codes, PK.conv, PK.conv_codes, PK.gc3_plan = real
     L.tc_check()
     assert sorted(set(refused)) == [(256, 16), (512, 32)] and len(refused) == 4, refused
     assert res[True][2] == res[False][2], "the refused launches did not all run on mnb_pk_conv"

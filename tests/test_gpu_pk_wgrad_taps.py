@@ -100,9 +100,9 @@ def test_taps_weight_gradient(case, terms, levels):
     assert torch.equal(new, old), f"differs from mnb_pk_wgrad by up to {(new - old).abs().max().item():.3e}"
 
 
-def test_headline_model_step_old_and_new_weight_gradient():
-    """one QAT step of the fused NIN-GC wbwtab W3/A2 model with MNB_PK_WG_TAPS=0 and =1: the new kernel runs for exactly the
-    two grouped 3x3 layers, and the loss and every gradient are bit-identical"""
+def test_headline_model_step_with_and_without_the_taps_plan():
+    """one QAT step of the fused NIN-GC wbwtab W3/A2 model with wgrad_taps_plan forced to refuse every shape and as it is: the
+    new kernel runs for exactly the two grouped 3x3 layers, and the loss and every gradient are bit-identical"""
     from harness import train as H
     from micronet_b200 import _lib as L, pk as PK
     from micronet_b200 import functional as F_
@@ -110,18 +110,17 @@ def test_headline_model_step_old_and_new_weight_gradient():
     base = H.prepare_engine(H.build_float_model(w["model"]), w["scheme"], **w["prepare"], **w["engine_extra"])
     x, t = H.synthetic_batch(16, w["hw"], seed=5, device=DEV)
     calls = []
-    real_taps = PK.wgrad_taps
+    real_taps, real_plan = PK.wgrad_taps, PK.wgrad_taps_plan
 
     def spy_taps(sh, *args, **kw):
         calls.append((sh.in_c, sh.out_c, sh.groups))
         return real_taps(sh, *args, **kw)
 
     res = {}
-    saved = L.PK_WG_TAPS
     try:
         PK.wgrad_taps = spy_taps
         for on in (False, True):
-            L.PK_WG_TAPS = on
+            PK.wgrad_taps_plan = real_plan if on else (lambda *a: None)   # wgrad_taps reads it too: only on the old leg
             n_calls = len(calls)
             m = copy.deepcopy(base).to(DEV).train()
             loss = torch.nn.functional.cross_entropy(m(x), t)
@@ -130,7 +129,7 @@ def test_headline_model_step_old_and_new_weight_gradient():
             assert len(calls) - n_calls == (2 if on else 0)
             res[on] = (loss.detach(), {n: p.grad.detach().clone() for n, p in m.named_parameters() if p.grad is not None})
     finally:
-        L.PK_WG_TAPS, PK.wgrad_taps = saved, real_taps
+        PK.wgrad_taps, PK.wgrad_taps_plan = real_taps, real_plan
     L.tc_check()
     assert sorted(calls) == [(256, 512, 16), (512, 1024, 32)], calls
     assert torch.equal(res[False][0], res[True][0])

@@ -84,9 +84,10 @@ def test_xnor_equals_the_tensor_core_forward_bit_for_bit(shape):
 
 
 @pytest.mark.parametrize("W", [2, 3], ids=["binary", "ternary"])
-def test_eval_module_on_the_xnor_path_matches_the_oracle(W):
-    """WB.QuantConv2d in eval mode (no autograd): the engine may take the XNOR forward; result vs the CPU oracle"""
-    from micronet_b200 import _lib as L, functional as F_, wbwtab
+def test_eval_module_takes_the_xnor_path_and_matches_the_oracle(W):
+    """WB.QuantConv2d in eval mode (no autograd) on a +-1 input without a producer-written plane: the engine takes the XNOR
+    forward; result vs the CPU oracle"""
+    from micronet_b200 import functional as F_, wbwtab
     from oracle import reference_port as O
     torch.manual_seed(3 + W)
     conv_e = wbwtab.QuantConv2d(64, 96, 3, padding=1, groups=2, W=W)
@@ -94,8 +95,6 @@ def test_eval_module_on_the_xnor_path_matches_the_oracle(W):
     conv_o.load_state_dict(conv_e.state_dict())
     x = torch.where(torch.randn(4, 64, 12, 12) < 0, -1.0, 1.0)
     conv_e.to(DEV).eval(); conv_o.eval()
-    saved = L.XNOR_MODE
-    L.XNOR_MODE = "all"
     try:
         F_.TIMER = F_.KernelTimer()
         with torch.no_grad():
@@ -104,7 +103,6 @@ def test_eval_module_on_the_xnor_path_matches_the_oracle(W):
             ye = conv_e(xe)
         kinds = {k for k, _, _, _ in F_.TIMER.records}
     finally:
-        L.XNOR_MODE = saved
         F_.TIMER = None
     with torch.no_grad():
         yo = conv_o(x)

@@ -439,7 +439,7 @@ def test_7x7_stride2_dgrad_is_refused_and_routed_to_the_generic_kernels():
     assert fake_launch("dgrad", sh, (2, 1)) == (rc, text)
     # QuantConv2dFn's forward asks _pk_forward first; it declines the layer before touching any tensor (the backward's data
     # gradient is outside the cover), and the forward takes the next family.  Integer weights, a DoReFa activation.
-    assert min(L.PK_TERMS, L.PK_TERMS_BWD) == 2
+    assert L.PK_TERMS_BWD == 2
     ctx = SimpleNamespace(needs_input_grad=(True, True, False))
     spec = SimpleNamespace(mode=L.ACT_DOREFA, q_type=0, bits=4)
     assert F._pk_forward(ctx, None, None, None, object(), None, spec, sh, None) is False

@@ -53,7 +53,7 @@ def test_packed_operand_plan_covers_the_bench_models(conv):
     name, B, Cc, H, W, K, R, st, pad, G = conv
     sh = L.ConvShape(B, Cc, H, W, K, R, R, st, st, pad, pad, 1, 1, G)
     names = "Nt ntiles MT CC chunks nstage smem acc TH TB BW n_mtiles n_items ny".split()
-    Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    Tb = L.PK_TERMS_BWD
     cases = [(0, 1, 1), (1, Tb, 1)]                                  # quantized forward / data gradient with integer weights
     if "res" in name:
         cases += [(0, L.PK_TERMS, L.PK_TERMS), (1, Tb, Tb)]         # the fp32 x fp32 statistics conv of QuantBNFuseConv2d

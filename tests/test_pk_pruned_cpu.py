@@ -39,7 +39,7 @@ def test_plans_cover_the_pruned_nin_gc(conv):
     sh = _sh(conv)
     name, B, Cc, H, W, K, R, st, pad, G = conv
     assert PK.padded_conv(sh) == (name != "L5"), name
-    Tb = min(L.PK_TERMS, L.PK_TERMS_BWD)
+    Tb = L.PK_TERMS_BWD
     # forward: levels x integer weights (DoReFa, symmetric IAO, wbwtab), two level pieces x integer weights (asymmetric
     # IAO), +-1 x fp32 pieces, fp32 x fp32; data gradient against integer / fp32 weights
     for mode, ta, tw in ((0, 1, 1), (0, 2, 1), (0, 1, 3), (0, 3, 3), (1, Tb, 1), (1, Tb, Tb)):
